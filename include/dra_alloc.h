@@ -372,6 +372,29 @@ int  dra_set_profiling(dra_ctx* ctx, int enabled);
 /* Instrumentation (env DRA_TIMELINE=1): 8 clock stamps per CTA of the last single-launch kernel; returns the
  * number of u64 words copied to host. */
 int  dra_debug_timeline(dra_ctx* ctx, unsigned long long* host, uint32_t n);
+/* Kernels enqueued by the last Allocate-family call on this context (DRA_K_* bits) and the hist tile it used (claims per
+ * tile of k_bucket_hist8 / k_bucket_hist; 0 when the call ran neither).  A CUDA-graph replay reports the chain of the call
+ * that was captured.  Returns DRA_OK. */
+int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_tile);
+#define DRA_K_FUSED_STAGED      0x00001u  /* single-launch kernel, claim array staged in shared memory */
+#define DRA_K_FUSED_STREAM      0x00002u  /* single-launch kernel, claims streamed from global memory */
+#define DRA_K_FUSED_DIRECT      0x00004u  /* single-launch kernel reading / writing the pinned host buffers (cooperative) */
+#define DRA_K_SERVE             0x00008u  /* the batch was answered by the resident kernel */
+#define DRA_K_SORTED_PREP       0x00010u  /* DRA_F_NODE_SORTED: k_sorted_prep instead of the counting sort */
+#define DRA_K_BUCKET_SMALL      0x00020u  /* the whole counting sort in one CTA */
+#define DRA_K_HIST8             0x00040u  /* CTA-wide histogram, 2048-claim tiles */
+#define DRA_K_HIST8_MULTI       0x00080u  /* CTA-wide histogram, tiles grown to a multiple of 2048 */
+#define DRA_K_HIST_WARP         0x00100u  /* one-warp histogram tiles (node ranges too wide for the CTA-wide form) */
+#define DRA_K_SCAN8             0x00200u  /* scan of the tile histograms: one warp per node */
+#define DRA_K_SCAN_ROWS         0x00400u  /* scan of the tile histograms: coalesced rows, look-back over CTAs */
+#define DRA_K_SCAN              0x00800u  /* scan of the one-warp histograms: one CTA */
+#define DRA_K_SCATTER           0x01000u
+#define DRA_K_PACK1             0x02000u  /* one warp per node, one node per CTA */
+#define DRA_K_PACK4             0x04000u  /* CTAs of four warps, each warp walking several nodes */
+#define DRA_K_COMPACT_FLAT1     0x08000u  /* sharded call: compaction in 256-claim tiles */
+#define DRA_K_COMPACT_FLAT8     0x10000u  /* sharded call: compaction in 2048-claim tiles */
+#define DRA_K_COMPACT_LOOKBACK  0x20000u  /* sharded call: compaction with a decoupled look-back (beyond 2M claims) */
+#define DRA_K_COMPACT_IN_KERNEL 0x40000u  /* sharded call: compaction inside the single-launch kernel */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

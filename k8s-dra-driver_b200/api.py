@@ -17,6 +17,12 @@ SO_PATH = os.path.join(_HERE, "libdra_alloc.so")
 OK, E_INVAL, E_CUDA, E_NCCL, E_NOMEM, E_STATE = 0, -1, -2, -3, -4, -5
 CFG_USE_GRAPH, CFG_NO_FUSED, CFG_NO_DIRECT, CFG_RESIDENT = 0x1, 0x2, 0x4, 0x8
 F_NODE_SORTED, F_FRESH_INVENTORY, F_EXHAUSTIVE = 0x1, 0x2, 0x4
+# DRA_K_*: the kernels an Allocate-family call enqueued (dra_debug_last_chain)
+KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x00004, "serve": 0x00008,
+           "sorted_prep": 0x00010, "bucket_small": 0x00020, "hist8": 0x00040, "hist8_multi": 0x00080,
+           "hist_warp": 0x00100, "scan8": 0x00200, "scan_rows": 0x00400, "scan": 0x00800, "scatter": 0x01000,
+           "pack1": 0x02000, "pack4": 0x04000, "compact_flat1": 0x08000, "compact_flat8": 0x10000,
+           "compact_lookback": 0x20000, "compact_in_kernel": 0x40000}
 
 
 class DraError(RuntimeError):
@@ -74,6 +80,7 @@ SYMBOLS = {
     "dra_launch_count": (_u64, [_vp]),
     "dra_set_profiling": (_i32, [_vp, _i32]),
     "dra_debug_timeline": (_i32, [_vp, _vp, _u32]),
+    "dra_debug_last_chain": (_i32, [_vp, C.POINTER(_u32), C.POINTER(_u32)]),
     "dra_debug_shard_times": (_i32, [_vp, _vp]),
     "dra_debug_serve_times": (_i32, [_vp, _vp]),
     "dra_debug_noop": (_i32, [_vp, _u32, _u32, _u32]),
@@ -389,6 +396,18 @@ class Context:
 
     def debug_noop(self, grid: int, block: int, smem: int) -> None:
         self._check(self._lib.dra_debug_noop(self._h, grid, block, smem))
+
+    def last_chain(self) -> set:
+        """Names (KERNELS keys) of the kernels the last Allocate-family call enqueued."""
+        k = _u32(0)
+        self._check(self._lib.dra_debug_last_chain(self._h, C.byref(k), None))
+        return {n for n, bit in KERNELS.items() if k.value & bit}
+
+    def last_hist_tile(self) -> int:
+        """Claims per histogram tile of the last Allocate-family call (0: it ran no histogram kernel)."""
+        t = _u32(0)
+        self._check(self._lib.dra_debug_last_chain(self._h, None, C.byref(t)))
+        return int(t.value)
 
     def debug_timeline(self, n_cta: int) -> np.ndarray:
         buf = np.zeros(n_cta * 8, dtype=np.uint64)

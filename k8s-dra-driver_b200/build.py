@@ -1,10 +1,12 @@
 """In-tree build of libdra_alloc.so for sm_90a (nvcc cross-compiles without a GPU)."""
 from __future__ import annotations
 
+import atexit
 import os
 import shutil
 import subprocess
 import sys
+import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -49,17 +51,24 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
 
 def build_cpp_tests(force: bool = False) -> str:
-    """tests/cpp/driver_test: the C++ host layer's own test program, linked against libdra_alloc.so."""
+    """tests/cpp/driver_test: the C++ host layer's own test program, linked against libdra_alloc.so.  Linked in the tree
+    when the tree is writable; a read-only tree whose program is missing or older than its source gets it linked into a
+    temporary directory instead (removed at exit), and that path is returned."""
     build()
     if (not force and os.path.exists(CPP_TEST_EXE)
             and os.path.getmtime(CPP_TEST_EXE) >= max(os.path.getmtime(CPP_TEST_SRC), os.path.getmtime(SO))):
         return CPP_TEST_EXE
-    cmd = ["g++", "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include"), CPP_TEST_SRC, "-o", CPP_TEST_EXE,
+    exe = CPP_TEST_EXE
+    if not os.access(os.path.dirname(CPP_TEST_EXE), os.W_OK):
+        tmp = tempfile.mkdtemp(prefix="dra_driver_test_")
+        atexit.register(shutil.rmtree, tmp, True)
+        exe = os.path.join(tmp, "driver_test")
+    cmd = ["g++", "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include"), CPP_TEST_SRC, "-o", exe,
            "-L", HERE, "-ldra_alloc", "-Wl,-rpath," + HERE]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("g++ failed:\n" + r.stdout + r.stderr)
-    return CPP_TEST_EXE
+    return exe
 
 
 if __name__ == "__main__":

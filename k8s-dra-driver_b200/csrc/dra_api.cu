@@ -102,6 +102,7 @@ struct dra_ctx {
     uint8_t* h_out = nullptr; size_t h_out_cap = 0;
 
     uint64_t launches = 0;
+    uint32_t chain = 0, chain_tile = 0;   // DRA_K_* bits and hist tile of the last Allocate-family call (dra_debug_last_chain)
     bool profiling = false;
     cudaEvent_t ev[8] = {};
     bool ev_ok = false;
@@ -140,7 +141,7 @@ struct dra_ctx {
                        bool operator==(const GraphKeyT& k) const { return c == k.c && o == k.o && d == k.d && n_claim == k.n_claim && n_out == k.n_out && flags == k.flags && epoch == k.epoch && c != nullptr; } };
     GraphKeyT graph_key{};
     cudaGraphExec_t graph_exec = nullptr;
-    uint32_t graph_launches = 0;
+    uint32_t graph_launches = 0, graph_chain = 0, graph_tile = 0;
     uint64_t state_epoch = 1;     // bumped by every call that reallocates or re-points device state
 
     // peer-memory all-gather (packets over NVLink, dra_device.cuh PktGather)
@@ -338,7 +339,7 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
         uint32_t blocks = std::max(1u, (n_claim + 255) / 256);
         k_sorted_prep<<<blocks, 256, 0, ctx->stream>>>(d_claims, n_claim, n_node, d_out_off, ctx->d_claim_off,
                                                        ctx->d_sorted, d_out, n_out, err);
-        ctx->launches += 1;
+        ctx->launches += 1; ctx->chain |= DRA_K_SORTED_PREP;
         prof.mark(); prof.skip_to(3);
     } else {
         const size_t nbp = ((size_t)n_node + 2) & ~(size_t)1;
@@ -357,7 +358,7 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
             pf.p[2] = ctx->d_tbl; pf.bytes[2] = 1024;
             k_bucket_small<<<1, 1024, small_smem, ctx->stream>>>(d_claims, n_claim, n_node, d_out_off, ctx->d_claim_off,
                                                                  ctx->d_sorted, d_out, n_out, err, pf, n_dev);
-            ctx->launches += 1;
+            ctx->launches += 1; ctx->chain |= DRA_K_BUCKET_SMALL;
             prof.mark(); prof.skip_to(3);
         } else {
             Tiling t = tiling(n_claim, n_node, ctx->n_sm);
@@ -371,6 +372,7 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
                 if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, ctx->stream)); }
                 if (t.T == H8_TILE) k_bucket_hist8<false><<<t.n_tiles, 256, smem, ctx->stream>>>(d_claims, n_claim, n_node, ctx->d_hist, ctx->d_rank, n_dev, t.T);
                 else k_bucket_hist8<true><<<t.n_tiles, 256, smem, ctx->stream>>>(d_claims, n_claim, n_node, ctx->d_hist, ctx->d_rank, n_dev, t.T);
+                ctx->chain |= t.T == H8_TILE ? DRA_K_HIST8 : DRA_K_HIST8_MULTI;
                 prof.mark();
                 // the scan: a warp per node with every load in flight at once (latency), or — big matrices — coalesced rows
                 static const bool no_rows = getenv("DRA_SCAN_BY_NODE") != nullptr;
@@ -378,9 +380,11 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
                     const uint32_t n_cta = (n_node + 1 + 31) / 32;
                     if (ctx->cap_scan_status < n_cta) return fail(ctx, DRA_E_STATE, "scan status words not allocated (ensure_batch)");
                     CU(launch_k(k_bucket_scan_rows, dim3(n_cta), dim3(256), 0, ctx->stream, pdl, ctx->d_hist, t.n_tiles, n_node, ctx->d_claim_off, ctx->d_ticket + 10, ctx->d_scan_status, err));
-                }
-                else
+                    ctx->chain |= DRA_K_SCAN_ROWS;
+                } else {
                     CU(launch_k(k_bucket_scan8, dim3((n_node + 1 + 7) / 8), dim3(256), 0, ctx->stream, pdl, ctx->d_hist, t.n_tiles, n_node, ctx->d_claim_off, ctx->d_ticket + 8));
+                    ctx->chain |= DRA_K_SCAN8;
+                }
                 prof.mark();
             } else {
                 if (n_dev) return fail(ctx, DRA_E_INVAL, "sharded call: node range too wide for the CTA-wide histogram");
@@ -393,13 +397,14 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
                 k_bucket_hist<<<t.n_tiles, 32, smem, ctx->stream>>>(d_claims, n_claim, n_node, t.T, ctx->d_hist, ctx->d_rank);
                 prof.mark();
                 CU(launch_k(k_bucket_scan, dim3(1), dim3(1024), 0, ctx->stream, pdl, ctx->d_hist, t.n_tiles, n_node, ctx->d_claim_off));
+                ctx->chain |= DRA_K_HIST_WARP | DRA_K_SCAN;
                 prof.mark();
             }
             uint32_t blocks = std::max(1u, (n_claim + 255) / 256);
             CU(launch_k(k_bucket_scatter, dim3(blocks), dim3(256), 0, ctx->stream, pdl, d_claims, n_claim, n_node, t.T, ctx->d_hist, ctx->d_rank,
                         ctx->d_claim_off, d_out_off, ctx->d_sorted, d_out, n_out, err, n_dev));
             prof.mark();
-            ctx->launches += 3;
+            ctx->launches += 3; ctx->chain |= DRA_K_SCATTER; ctx->chain_tile = t.T;
         }
     }
 
@@ -422,6 +427,7 @@ int launch_compaction(dra_ctx* ctx, const ShardArgs& sa, uint32_t sc_rows, bool 
     else if (sc_rows == 1) k_shard_compact_flat<1><<<sa.n_tiles, 256, 0, ctx->stream>>>(sa);
     else k_shard_compact_flat<8><<<sa.n_tiles, 256, 0, ctx->stream>>>(sa);
     ctx->launches += 1;
+    ctx->chain |= !sc_flat ? DRA_K_COMPACT_LOOKBACK : sc_rows == 1 ? DRA_K_COMPACT_FLAT1 : DRA_K_COMPACT_FLAT8;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "shard compaction launch: %s", cudaGetErrorString(e));
     return DRA_OK;
@@ -544,6 +550,8 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
             else CU(launch_k(k_fused<FUSED_NW, false, 1>, dim3(n_node + 1), dim3(FUSED_NW * 32), launch_smem, ctx->stream, dep, a));
         }
         ctx->launches += 1;
+        ctx->chain |= (stage && dio.h_claims && !cluster) ? DRA_K_FUSED_DIRECT : stage ? DRA_K_FUSED_STAGED : DRA_K_FUSED_STREAM;
+        if (a.sh_on) ctx->chain |= DRA_K_COMPACT_IN_KERNEL;
         prof.mark();
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "kernel launch: %s", cudaGetErrorString(e));
@@ -558,8 +566,10 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
     a.sorted = ctx->d_sorted;
     a.claim_off = ctx->d_claim_off;
     if (n_node) {
-        if (n_node <= (uint32_t)ctx->n_sm * 16u) CU(launch_k(k_pack<1>, dim3(n_node), dim3(32), pack_smem_bytes(1), ctx->stream, pdl, a));
-        else {
+        if (n_node <= (uint32_t)ctx->n_sm * 16u) {
+            CU(launch_k(k_pack<1>, dim3(n_node), dim3(32), pack_smem_bytes(1), ctx->stream, pdl, a));
+            ctx->chain |= DRA_K_PACK1;
+        } else {
             // more nodes than warps can be resident: CTAs of 4 warps, exactly as many as fit at once, each warp walking nodes
             if (ctx->pack4_occ < 0) {
                 int nb = 0;
@@ -567,6 +577,7 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
                 ctx->pack4_occ = std::max(1, nb);
             }
             CU(launch_k(k_pack<4>, dim3(std::min((n_node + 3) / 4, (uint32_t)(ctx->n_sm * ctx->pack4_occ))), dim3(128), pack_smem_bytes(4), ctx->stream, pdl, a));
+            ctx->chain |= DRA_K_PACK4;
         }
         ctx->launches += 1;
     }
@@ -723,7 +734,7 @@ int serve_call(dra_ctx* ctx, const void* src_c, uint32_t n_claim, const void* sr
                 if (spins > (1ull << 31)) return fail(ctx, DRA_E_CUDA, "resident kernel does not answer");
             }
         }
-        if (done) { ctx->serve_seq = seq; ctx->serve_batches++; return DRA_OK; }
+        if (done) { ctx->serve_seq = seq; ctx->serve_batches++; ctx->chain |= DRA_K_SERVE; return DRA_OK; }
         // the kernel left (idle time-out) before it saw this doorbell: start it again and ring once more
         CU(cudaStreamSynchronize(ctx->serve_stream));
         ctx->serve_on = false;
@@ -935,6 +946,7 @@ int dra_allocate_batch_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint3
                               dra_out_rec* d_out, uint32_t n_out, uint32_t flags) {
     if (!ctx || (n_claim && (!d_claims || !d_out))) return DRA_E_INVAL;
     QUIESCE();
+    ctx->chain = ctx->chain_tile = 0;
     CU(cudaSetDevice(ctx->device));
     int rc = ensure_batch(ctx, n_claim, n_out, false);
     if (rc) return rc;
@@ -945,6 +957,7 @@ int dra_allocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
                        dra_out_rec* out, uint32_t n_out, uint32_t flags) {
     if (!ctx || (n_claim && (!claims || !out))) return DRA_E_INVAL;
     if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    ctx->chain = ctx->chain_tile = 0;
     CU(cudaSetDevice(ctx->device));
     int rc = ensure_batch(ctx, n_claim, n_out, true);
     if (rc) return rc;
@@ -1045,6 +1058,7 @@ int dra_allocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
     if (want_graph && ctx->graph_exec && key == ctx->graph_key) {
         CU(cudaGraphLaunch(ctx->graph_exec, ctx->stream));
         ctx->launches += ctx->graph_launches;
+        ctx->chain = ctx->graph_chain; ctx->chain_tile = ctx->graph_tile;
     } else {
         const bool capture = want_graph && key == ctx->graph_key;      // second call of this shape: capture it
         if (want_graph && !capture) { ctx->graph_key = key; if (ctx->graph_exec) { cudaGraphExecDestroy(ctx->graph_exec); ctx->graph_exec = nullptr; } }
@@ -1065,6 +1079,7 @@ int dra_allocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
                 return rc != DRA_OK ? rc : fail(ctx, DRA_E_CUDA, "graph capture failed: %s", cudaGetErrorString(ce != cudaSuccess ? ce : ee));
             }
             ctx->graph_launches = (uint32_t)(ctx->launches - l0);
+            ctx->graph_chain = ctx->chain; ctx->graph_tile = ctx->chain_tile;
             cudaError_t ie = cudaGraphInstantiate(&ctx->graph_exec, g, 0);
             cudaGraphDestroy(g);
             if (ie != cudaSuccess) { ctx->graph_exec = nullptr; return fail(ctx, DRA_E_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ie)); }
@@ -1193,6 +1208,7 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
     for (uint32_t q = 0; q < n_pod; ++q)
         if (pod_off[q + 1] < pod_off[q]) return fail(ctx, DRA_E_INVAL, "pod_off not monotone at pod %u", q);
+    ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     CU(cudaSetDevice(ctx->device));
     int rc = ensure_batch(ctx, std::max(n_claim, n_pod), n_out, true);
@@ -1455,6 +1471,7 @@ int dra_allocate_batch_gather_device(dra_ctx* ctx, const dra_claim_rec* d_claims
     if (!ctx->comm && !ctx->peer_ready) return fail(ctx, DRA_E_STATE, "dra_comm_init has not been called");
     if (!d_out_all && !ctx->peer_ready) return fail(ctx, DRA_E_INVAL, "d_out_all may be NULL only with the peer all-gather set up");
     if (n_out > n_per_rank) return fail(ctx, DRA_E_INVAL, "n_out %u > n_per_rank %u", n_out, n_per_rank);
+    ctx->chain = ctx->chain_tile = 0;
     CU(cudaSetDevice(ctx->device));
     int rc = ensure_batch(ctx, n_claim, n_out, false);
     if (rc) return rc;
@@ -1525,6 +1542,7 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
     const bool gather = ctx->world > 1;
     if (gather && !(ctx->peer_ready && ctx->peer_form == 2)) return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
     if (gather && n_out > ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", n_out, ctx->peer_tab_len);
+    ctx->chain = ctx->chain_tile = 0;
     CU(cudaSetDevice(ctx->device));
     const uint32_t n_local_node = ctx->shard_hi - ctx->shard_lo;
     // Plan.  The single-launch kernel lays its shared memory out for a CAPACITY of claims; the real number is only known
@@ -1600,6 +1618,10 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
     }
     // 1. this rank's claims, compacted in input order, node indices local to the shard
     ctx->shard_epoch += 1;
+    // A tile takes a predecessor's status word for this call's when the word's 10-bit epoch matches and its state is set, so a
+    // word left 1,024 calls back would pass.  The call whose epoch wraps to 0 starts from cleared words — all of them, since a
+    // later call may have more tiles than this one — and no word older than that call can then alias.
+    if ((ctx->shard_epoch & 0x3FFu) == 0u) CU(cudaMemsetAsync(ctx->d_sc_status, 0, ctx->cap_sc_status * 8, ctx->stream));
     if (counted) g.expect = ctx->d_rank_slots + (ctx->shard_epoch & 1u) * PEER_MAX;
     ShardArgs sa; memset(&sa, 0, sizeof sa);
     if (counted) {
@@ -1722,6 +1744,7 @@ int dra_calibrate(dra_ctx* ctx, uint32_t* crossover_claims) {
     const uint32_t saved_flags = ctx->cfg_flags;
     const uint32_t saved_a = ctx->fused_max_one_wave, saved_b = ctx->fused_max_multi;
     const bool prof = ctx->profiling; ctx->profiling = false;
+    const uint32_t saved_chain = ctx->chain, saved_tile = ctx->chain_tile;   // (calibration runs are no Allocate call)
     uint32_t best = 0; bool lost = false;
     for (uint32_t n : sizes) {
         float t[2] = {1e30f, 1e30f};
@@ -1742,6 +1765,7 @@ int dra_calibrate(dra_ctx* ctx, uint32_t* crossover_claims) {
         if (t[0] <= t[1] && !lost) best = n; else lost = true;          // the first size at which the sort path wins ends the range
     }
     ctx->cfg_flags = saved_flags; ctx->profiling = prof;
+    ctx->chain = saved_chain; ctx->chain_tile = saved_tile;
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     cudaMemcpy(ctx->d_inv_live, d_save, (size_t)ctx->n_gpu * 16, cudaMemcpyDeviceToDevice);
     cudaFree(d_save);
@@ -1783,6 +1807,13 @@ void dra_host_free(void* p) {
 }
 
 uint64_t dra_launch_count(const dra_ctx* ctx) { return ctx ? ctx->launches : 0; }
+
+int dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_tile) {
+    if (!ctx) return DRA_E_INVAL;
+    if (kernels) *kernels = ctx->chain;
+    if (hist_tile) *hist_tile = ctx->chain_tile;
+    return DRA_OK;
+}
 
 namespace { __global__ void k_noop(int x) { extern __shared__ uint8_t sm[]; if (x == 12345) sm[0] = 1; } }
 

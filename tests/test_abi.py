@@ -80,13 +80,16 @@ def test_kernels_are_sm90a_and_use_tma(pkg):
 
 
 def test_flag_constants_match_header(pkg):
-    """DRA_CFG_* / DRA_F_* / error codes of the ctypes binding are the header's."""
+    """DRA_CFG_* / DRA_F_* / DRA_K_* / error codes of the ctypes binding are the header's."""
     text = open(HEADER).read()
     defs = {m.group(1): int(m.group(2), 0) for m in re.finditer(r"#define\s+(DRA_(?:CFG|F)_[A-Z_]+)\s+(0x[0-9a-fA-F]+)u", text)}
     A = pkg.api
     assert defs == {"DRA_CFG_USE_GRAPH": A.CFG_USE_GRAPH, "DRA_CFG_NO_FUSED": A.CFG_NO_FUSED,
                     "DRA_CFG_NO_DIRECT": A.CFG_NO_DIRECT, "DRA_CFG_RESIDENT": A.CFG_RESIDENT, "DRA_F_NODE_SORTED": A.F_NODE_SORTED,
                     "DRA_F_FRESH_INVENTORY": A.F_FRESH_INVENTORY, "DRA_F_EXHAUSTIVE": A.F_EXHAUSTIVE}
+    kern = {m.group(1): int(m.group(2), 0) for m in re.finditer(r"#define\s+DRA_K_([A-Z0-9_]+)\s+(0x[0-9a-fA-F]+)u", text)}
+    assert kern == {k.upper(): v for k, v in A.KERNELS.items()}
+    assert len(set(kern.values())) == len(kern) and all(v & (v - 1) == 0 for v in kern.values())   # one bit each
     errs = {m.group(1): int(m.group(2)) for m in re.finditer(r"#define\s+(DRA_E_[A-Z]+)\s+\((-\d+)\)", text)}
     assert errs == {"DRA_E_INVAL": A.E_INVAL, "DRA_E_CUDA": A.E_CUDA, "DRA_E_NCCL": A.E_NCCL, "DRA_E_NOMEM": A.E_NOMEM,
                     "DRA_E_STATE": A.E_STATE}

@@ -74,13 +74,18 @@ def test_cuda_matches_oracle_fuzz(pkg, ctx, oracle, seed):
     _assert_same(out, inv, ref_out, ref_inv, f"mixed seed {seed}")
 
 
-# ---- large batches: hist tiles that are multiples of 2048 (one wave of tiles), the row-wise scan of a big matrix ----
+# ---- large batches: hist tiles grown to multiples of 2048 (one wave of tiles); only 1M x 10k has enough counters
+# (n_tiles x (n_node + 1) > 524,288) for the row-wise scan — 350k x 6,000 gives 86 x 6,001 = 516,086 ----
+# The sort path is what every context takes at these sizes; the chain each shape takes holds from 86 to 170 SMs.
 @pytest.mark.parametrize("n_claim,n_node,kind", [(350_000, 6000, "mixed"), (700_000, 1200, "mixed"), (1_000_000, 10_000, "cfg2")])
 def test_large_batches_match_oracle(pkg, ctx, oracle, n_claim, n_node, kind):
     w = pkg.synth.mixed(n_claim, n_node, 77, invalid=True) if kind == "mixed" else pkg.synth.cfg2(n_claim, n_node)
     out, inv = _run(ctx, w)
     ref_out, ref_inv = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out)
     _assert_same(out, inv, ref_out, ref_inv, f"{kind} {n_claim} x {n_node}")
+    scan = "scan_rows" if n_node == 10_000 else "scan8"
+    pack = "pack1" if n_node == 1200 else "pack4"
+    assert ctx.last_chain() == {"hist8_multi", scan, "scatter", pack}, ctx.last_chain()
 
 
 def test_large_batch_through_a_replayed_graph(pkg, oracle):
@@ -97,6 +102,7 @@ def test_large_batch_through_a_replayed_graph(pkg, oracle):
             po.array[:] = 0
             g.allocate(pc.array, None, w.n_out, flags=pkg.api.F_FRESH_INVENTORY, out=po.array)
             assert po.array.tobytes() == ref.tobytes(), it
+            assert g.last_chain() == {"hist8_multi", "scan_rows", "scatter", "pack4"}, it   # (a replay reports the captured chain)
         pc.free(); po.free()
 
 
@@ -255,20 +261,25 @@ def test_unsuitable_matches_oracle(pkg, ctx, oracle):
 
 
 def test_launch_counter_counts_our_kernels(pkg, ctx):
+    """Each path's chain as the library reports it, and one counted launch per kernel of it."""
     w = pkg.synth.cfg2(1000, 10)
     ctx.set_table(w.table); ctx.set_inventory(w.gpus, w.node_off)
     before = ctx.launch_count()
     ctx.allocate(w.claims)
-    assert ctx.launch_count() - before == (2 if ctx.path == "bucket+pack" else 1)   # fused | bucket_small, pack
+    want = {"auto": {"fused_direct"}, "copy-engine": {"fused_staged"}, "bucket+pack": {"bucket_small", "pack1"}}[ctx.path]
+    assert ctx.last_chain() == want and ctx.last_hist_tile() == 0
+    assert ctx.launch_count() - before == len(want)
     ctx.set_inventory(w.gpus, w.node_off)
     before = ctx.launch_count()
     ctx.allocate(w.node_sorted().claims, flags=pkg.api.F_NODE_SORTED)
-    assert ctx.launch_count() - before == 2          # sorted_prep, pack
+    assert ctx.last_chain() == {"sorted_prep", "pack1"}
+    assert ctx.launch_count() - before == 2
     w = pkg.synth.cfg2(40_000, 300)
     ctx.set_inventory(w.gpus, w.node_off)
     before = ctx.launch_count()
     ctx.allocate(w.claims)
-    assert ctx.launch_count() - before == 4          # hist, scan, scatter, pack
+    assert ctx.last_chain() == {"hist8", "scan8", "scatter", "pack1"} and ctx.last_hist_tile() == 2048
+    assert ctx.launch_count() - before == 4
 
 
 # ---- selectors on the device (spec §10) -----------------------------------------------------------------

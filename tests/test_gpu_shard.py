@@ -169,6 +169,141 @@ def test_device_rendezvous_of_world_contexts(pkg):
         c.peer_rendezvous()                      # world 1: nothing to do
 
 
-# (A LARGE sharded batch — wave-sized hist tiles, row-wise scan, stand-alone gather — is checked on real ranks only:
-#  tests/multi_gpu_check.py, "1M claims x 10k nodes".  Two contexts on ONE device cannot run it: a rank's gather kernel holds
-#  every SM at the default shared-memory split while it waits for its peer, whose histogram CTAs need the SMs re-split.)
+# ---- the compaction on one device: world-1 contexts with sub-range shards (no peers, no gather) ---------------------------
+# A world-1 context serves [lo, hi) of the inventory and drops every other claim, so each compaction form is checked where
+# it matters: the kept claims' positions among dropped ones.  The shard writes the OutRecs of its kept claims only; those
+# slots, and the shard's slice of the inventory, must be the oracle's answer to the whole batch (nodes are independent).
+
+def _kept(w, lo, hi, stray):
+    node = w.claims["node"].astype(np.int64)
+    return np.where(node >= w.n_node, bool(stray), (node >= lo) & (node < hi))
+
+
+def _slots_of(pkg, w, keep):
+    """OutRec slots of the claims in `keep` (bool mask over the claims)."""
+    sl = pkg.records.claim_slots(w.claims, w.n_node).astype(np.int64)
+    start = (np.arange(w.n_claim) if w.out_off is None else w.out_off.astype(np.int64))[keep]
+    n = sl[keep]
+    first = np.repeat(np.cumsum(n) - n, n)
+    m = np.zeros(w.n_out, dtype=bool)
+    m[np.repeat(start, n) + np.arange(int(n.sum())) - first] = True
+    return m
+
+
+def _shard_call(pkg, c, w, d_claims, d_off, lo, hi, stray, ref, ref_inv, what):
+    """One sharded call on [lo, hi): kept slots and the shard's inventory slice against the oracle, the rest untouched."""
+    R = pkg.records
+    c.allocate_global_device(d_claims.data_ptr(), w.n_claim, None if d_off is None else d_off.data_ptr(), w.n_out,
+                             pkg.api.F_FRESH_INVENTORY)
+    got = c.gather_read(np.zeros(w.n_out, dtype=R.OUT_DTYPE))
+    keep = _kept(w, lo, hi, stray)
+    assert 0 < keep.sum() < w.n_claim, f"{what}: the shard must keep some claims and drop others"
+    m = _slots_of(pkg, w, keep)
+    if got[m].tobytes() != ref[m].tobytes():
+        bad = np.nonzero(got.view(np.uint64)[m] != ref.view(np.uint64)[m])[0]
+        raise AssertionError(f"{what}: {len(bad)} kept OutRecs differ, first at slot {np.nonzero(m)[0][bad[0]]}")
+    inv = c.get_inventory()
+    g0, g1 = int(w.node_off[lo]), int(w.node_off[hi])
+    assert inv[g0:g1].tobytes() == ref_inv[g0:g1].tobytes(), f"{what}: shard inventory differs"
+    return got, m, c.last_chain()
+
+
+@pytest.mark.parametrize("n_claim,compaction", [(262_144, "compact_flat1"), (262_145, "compact_flat8"),
+                                                (2_097_152, "compact_flat8"), (2_097_153, "compact_lookback")])
+def test_shard_compaction_forms_drop_claims(pkg, oracle, n_claim, compaction):
+    """256-claim tiles up to 262,144 claims, 2048-claim tiles up to 2,097,152, the look-back form beyond; strays kept."""
+    w = pkg.synth.mixed(n_claim, 2_000, 50, invalid=True)
+    ref, ref_inv = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out, threads=8)
+    with pkg.api.Context(device=0) as c:
+        c.set_table(w.table); c.set_inventory(w.gpus, w.node_off); c.set_shard(500, 1_300, take_stray=True)
+        d, o = _dev(w.claims), _dev(w.out_off)
+        _, _, chain = _shard_call(pkg, c, w, d, o, 500, 1_300, True, ref, ref_inv, f"{n_claim} claims")
+        assert compaction in chain, chain
+        outside = np.ones(w.n_gpu, dtype=bool); outside[int(w.node_off[500]):int(w.node_off[1_300])] = False
+        assert c.get_inventory()[outside].tobytes() == w.gpus[outside].tobytes(), "a GPU outside the shard changed"
+
+
+def test_three_shards_cover_the_inventory(pkg, oracle):
+    """Three sub-ranges whose union is the whole inventory, strays to the middle one: together they are the oracle's batch."""
+    R = pkg.records
+    w = pkg.synth.mixed(300_000, 1_500, 51, invalid=True)
+    ref, ref_inv = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out, threads=8)
+    merged = np.zeros(w.n_out, dtype=R.OUT_DTYPE)
+    covered = np.zeros(w.n_out, dtype=bool)
+    with pkg.api.Context(device=0) as c:
+        c.set_table(w.table); c.set_inventory(w.gpus, w.node_off)
+        d, o = _dev(w.claims), _dev(w.out_off)
+        for lo, hi, stray in ((0, 400, False), (400, 1_111, True), (1_111, 1_500, False)):
+            c.set_shard(lo, hi, take_stray=stray)
+            got, m, chain = _shard_call(pkg, c, w, d, o, lo, hi, stray, ref, ref_inv, f"shard [{lo}, {hi})")
+            assert "compact_flat8" in chain, chain
+            assert not (covered & m).any()
+            merged[m] = got[m]; covered |= m
+        assert covered.all() and merged.tobytes() == ref.tobytes()
+        assert c.get_inventory().tobytes() == ref_inv.tobytes()
+
+
+def test_plan_hint_takes_the_staged_kernel_on_a_narrow_shard(pkg, oracle):
+    """The first call of a batch size plans for the whole batch (sort path); the second plans from the first call's count
+    and, the shard being narrow, lays the staged single-launch kernel out for a few thousand claims."""
+    w = pkg.synth.mixed(262_145, 2_000, 52, invalid=True)
+    ref, ref_inv = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out, threads=8)
+    with pkg.api.Context(device=0) as c:
+        c.set_table(w.table); c.set_inventory(w.gpus, w.node_off); c.set_shard(960, 1_000, take_stray=False)
+        d, o = _dev(w.claims), _dev(w.out_off)
+        _, _, first = _shard_call(pkg, c, w, d, o, 960, 1_000, False, ref, ref_inv, "first call")
+        assert "compact_flat8" in first and not first & {"fused_staged", "fused_stream"}, first
+        for rep in range(2):
+            _, _, chain = _shard_call(pkg, c, w, d, o, 960, 1_000, False, ref, ref_inv, f"planned call {rep}")
+            assert chain == {"compact_flat8", "fused_staged"}, chain
+
+
+def test_shard_beyond_the_cta_wide_histogram_is_an_error(pkg, oracle):
+    """A shard of 12,799 local nodes past the single-launch kernel's limits needs the one-warp histogram, which the sharded
+    call does not support: DRA_E_INVAL with the inventory unchanged; one node fewer works."""
+    w = pkg.synth.mixed(10_000, 13_000, 53, invalid=True)
+    ref, ref_inv = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out)
+    with pkg.api.Context(device=0) as c:
+        c.set_table(w.table); c.set_inventory(w.gpus, w.node_off); c.set_shard(0, 12_799, take_stray=True)
+        d, o = _dev(w.claims), _dev(w.out_off)
+        with pytest.raises(pkg.api.DraError) as e:
+            c.allocate_global_device(d.data_ptr(), w.n_claim, o.data_ptr(), w.n_out, pkg.api.F_FRESH_INVENTORY)
+        assert e.value.code == pkg.api.E_INVAL
+        assert c.get_inventory().tobytes() == w.gpus.tobytes()
+        c.set_shard(0, 12_798, take_stray=True)
+        _, _, chain = _shard_call(pkg, c, w, d, o, 0, 12_798, True, ref, ref_inv, "12,798 local nodes")
+        assert {"compact_flat1", "hist8", "scan8"} <= chain, chain
+
+
+def test_shard_status_words_do_not_alias_after_1024_calls(pkg, oracle):
+    """A compaction tile accepts a predecessor's status word by its 10-bit epoch.  A large call, 1,023 one-tile calls, then a
+    large call of the same size on other claims: the last call's epoch equals the first's modulo 1,024, and its tiles must
+    not take the words the first call left as their own.  Without the clear at the epoch wrap this fails only when a tile
+    reads a predecessor before that predecessor has published in the last call, which is likely with hundreds of tiles in
+    flight but not certain; with it the test passes deterministically."""
+    n = 200_000                                                         # 782 tiles of 256 claims
+    x = pkg.synth.mixed(n, 400, 54, invalid=True)
+    y = pkg.synth.mixed(n, 400, 55, invalid=True)
+    y.claims["node"] = np.where(y.claims["node"] < 400, (y.claims["node"].astype(np.int64) ** 2) % 400, y.claims["node"]).astype(np.uint32)
+    y.out_off, y.n_out = pkg.records.out_offsets(y.claims, y.n_node)
+    y.gpus, y.node_off = x.gpus, x.node_off                            # same inventory, different per-tile counts
+    small = pkg.synth.mixed(200, 400, 56, invalid=True)
+    with pkg.api.Context(device=0) as c:
+        c.set_table(x.table); c.set_inventory(x.gpus, x.node_off); c.set_shard(0, 200, take_stray=True)
+        rx, rx_inv = oracle.allocate(x.gpus, x.node_off, x.table, x.claims, x.out_off, x.n_out, threads=8)
+        dx, ox = _dev(x.claims), _dev(x.out_off)
+        _shard_call(pkg, c, x, dx, ox, 0, 200, True, rx, rx_inv, "first large call")
+        ds, os_ = _dev(small.claims), _dev(small.out_off)
+        for _ in range(1_023):
+            c.allocate_global_device(ds.data_ptr(), small.n_claim, os_.data_ptr(), small.n_out, pkg.api.F_FRESH_INVENTORY)
+        c.sync()
+        ry, ry_inv = oracle.allocate(y.gpus, y.node_off, y.table, y.claims, y.out_off, y.n_out, threads=8)
+        dy, oy = _dev(y.claims), _dev(y.out_off)
+        _, _, chain = _shard_call(pkg, c, y, dy, oy, 0, 200, True, ry, ry_inv, "large call 1,024 epochs later")
+        assert "compact_flat1" in chain
+
+
+# (A LARGE sharded batch across ranks — stand-alone gather after wave-sized hist tiles and the row-wise scan — is checked on
+#  real ranks only: tests/multi_gpu_check.py, "1M claims x 10k nodes".  Two world contexts on ONE device cannot run it: a
+#  rank's gather kernel holds every SM at the default shared-memory split while it waits for its peer, whose histogram CTAs
+#  need the SMs re-split.  The compaction forms themselves are covered above on world-1 contexts, which have no gather.)
