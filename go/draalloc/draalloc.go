@@ -266,6 +266,43 @@ func (c *Context) AllocateBatchGlobal(pinnedClaims unsafe.Pointer, nClaim int, n
 	return nil
 }
 
+// SetShardPairs reserves room for the sharded UnsuitableNodes bit exchange: before ShardExport, the same on every context.
+// Unbuilt, like the rest of this file.
+func (c *Context) SetShardPairs(maxPairs uint32) error {
+	if rc := C.dra_set_shard_pairs(c.h, C.uint32_t(maxPairs)); rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
+// UnsuitableNodesGlobal: UnsuitableNodes on a sharded world (dra_unsuitable_batch_global_device).  The same pods and
+// candidates on every context, in dra_host_alloc'ed (pinned) memory; each context decides the pairs of its node range and
+// every context ends with the whole bitmap in pinnedBits (ceil(nPair/8) bytes).  candNodes == candOff == nil: dense form,
+// nPair = nPod * nNode.  Returns at once; Sync reports completion and errors found on the device.  Unbuilt, like the rest
+// of this file.
+func (c *Context) UnsuitableNodesGlobal(pinnedClaims unsafe.Pointer, nClaim int, pinnedPodOff unsafe.Pointer, nPod int,
+	pinnedCandNodes, pinnedCandOff unsafe.Pointer, nPair int, pinnedBits unsafe.Pointer, flags uint32) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_unsuitable_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
+		(*C.uint32_t)(pinnedPodOff), C.uint32_t(nPod), (*C.uint32_t)(pinnedCandNodes), (*C.uint32_t)(pinnedCandOff),
+		C.uint32_t(nPair), (*C.uint8_t)(pinnedBits), C.uint32_t(flags))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
+// Sync waits for the calls enqueued on the context and reports the errors they found on the device (dra_ctx_sync).
+func (c *Context) Sync() error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	if rc := C.dra_ctx_sync(c.h); rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
 func (c *Context) GatherRead(out []OutRec) error {
 	c.mu.Lock()
 	defer c.mu.Unlock()

@@ -323,7 +323,7 @@ int  dra_peer_rendezvous_device(dra_ctx* ctx);
  *   result: dra_gather_table / dra_gather_read (n_out records, input order, global GPU indices)
  * out_off must tile [0, n_out) (slots no claim owns keep their previous contents).  flags: DRA_F_FRESH_INVENTORY.
  * With world == 1 no export is needed (the table is local).  A rank's live inventory is authoritative for its own
- * node range only.  d_claims may also be a pinned host buffer (dra_host_alloc): the compaction kernel reads every claim
+ * node range only (UnsuitableNodes on such a world: dra_unsuitable_batch_global_device below).  d_claims may also be a pinned host buffer (dra_host_alloc): the compaction kernel reads every claim
  * exactly once, so it then ingests the batch over PCIe itself — no copy-engine transfer in front of the call. */
 int  dra_set_shard(dra_ctx* ctx, uint32_t node_lo, uint32_t node_hi, int take_stray);
 /* The whole partition: rank r serves nodes [bounds[r], bounds[r+1]) (bounds has world+1 entries, bounds[world] = n_node),
@@ -334,6 +334,27 @@ int  dra_set_shard_map(dra_ctx* ctx, const uint32_t* bounds, int stray_rank);
 int  dra_shard_export(dra_ctx* ctx, uint32_t n_out_max, uint32_t cap_per_rank, void* handle64);
 int  dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
                                       const uint32_t* d_out_off, uint32_t n_out, uint32_t flags);
+
+/* Sharded UnsuitableNodes.  After sharded Allocate calls a rank's inventory is stale outside its node range, so
+ * dra_unsuitable_batch on one rank cannot answer for the whole world; this call can.  Each rank evaluates only the pairs
+ * whose candidate node lies in its range, on its live inventory, and the ranks exchange their bits over peer memory.
+ *
+ * Room for the bit exchange in the buffer dra_shard_export maps.  World > 1: call before dra_shard_export (afterwards:
+ * DRA_E_STATE); every rank with the same max_pairs.  The export then also sizes the call's scratch for max_pairs (about
+ * 4 bytes per pair beyond the staging), so that no call reallocates while its peers wait.  World 1 needs no call (buffers
+ * grow on demand). */
+int  dra_set_shard_pairs(dra_ctx* ctx, uint32_t max_pairs);
+/* UnsuitableNodes over a sharded world (spec §8 / §12).  The SAME pods and candidates on every rank (device pointers, or
+ * dra_host_alloc'ed buffers).  A pair is decided by the rank whose node range holds its candidate node, against that rank's
+ * live inventory; a candidate that names no node of the inventory is unsuitable.  Every rank ends with the WHOLE bitmap in
+ * d_suitable_bits: exactly ceil(n_pair/8) bytes, bits past n_pair zero.  Dense form = cand_nodes == cand_off == NULL
+ * (pair = pod * n_node + node, n_pair = n_pod * n_node).  Enqueues on ctx's stream and returns; completion and
+ * device-detected errors (pod_off / cand_off not monotone or not spanning their arrays: DRA_E_INVAL, every bit zero) surface
+ * at dra_ctx_sync.  Every rank must make the same calls.  flags: 0 or DRA_F_EXHAUSTIVE. */
+int  dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                        const uint32_t* d_pod_off, uint32_t n_pod,
+                                        const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                        uint8_t* d_suitable_bits, uint32_t flags);
 
 /* ---- adjacent integer searches of the reference, batched (API completeness; SURVEY §8f-4) -------------- */
 

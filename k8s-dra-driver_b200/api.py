@@ -69,6 +69,8 @@ SYMBOLS = {
     "dra_set_shard_map": (_i32, [_vp, _vp, _i32]),
     "dra_shard_export": (_i32, [_vp, _u32, _u32, _vp]),
     "dra_allocate_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _u32]),
+    "dra_set_shard_pairs": (_i32, [_vp, _u32]),
+    "dra_unsuitable_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _u32]),
     "dra_mps_limits_batch": (_i32, [_vp, _vp, _u32, _vp, _vp]),
     "dra_imex_offsets_batch": (_i32, [_vp, _vp, _vp, _u32, C.c_int32, C.c_int32, _vp]),
     "dra_calibrate": (_i32, [_vp, C.POINTER(_u32)]),
@@ -365,6 +367,19 @@ class Context:
         """Sharded global batch: the SAME claim array on every rank (device pointer); enqueues, no synchronisation.
         The result table: gather_read()."""
         self._check(self._lib.dra_allocate_batch_global_device(self._h, _ptr(d_claims), n_claim, _ptr(d_out_off), n_out, flags))
+
+    def set_shard_pairs(self, max_pairs: int) -> None:
+        """Room for the sharded UnsuitableNodes bit exchange; world > 1: before shard_export, the same on every rank."""
+        self._check(self._lib.dra_set_shard_pairs(self._h, max_pairs))
+
+    def unsuitable_global_device(self, d_claims: int, n_claim: int, d_pod_off: int, n_pod: int, d_cand_nodes: int | None,
+                                 d_cand_off: int | None, n_pair: int, d_bits: int, flags: int = 0) -> None:
+        """Sharded UnsuitableNodes: the SAME pods and candidates on every rank (device pointers); every rank receives the
+        whole bitmap, ceil(n_pair / 8) bytes at d_bits.  d_cand_nodes / d_cand_off None = dense form (n_pair = n_pod *
+        n_node).  Enqueues, no synchronisation; errors found on the device surface at sync()."""
+        self._check(self._lib.dra_unsuitable_batch_global_device(self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod,
+                                                                 _ptr(d_cand_nodes), _ptr(d_cand_off), n_pair, _ptr(d_bits),
+                                                                 flags))
 
     def peer_import(self, handles) -> None:
         blob = b"".join(handles)

@@ -168,6 +168,12 @@ struct dra_ctx {
     uint32_t* h_sc_counts_dev = nullptr;
     uint2* d_gtable = nullptr; size_t cap_gtable = 0;   // result table when no peers are set up (world 1)
     uint32_t* d_ticket = nullptr;
+    // sharded UnsuitableNodes: bit exchange in the peer buffer ([staging x2: world slices of uns_stride words][flags])
+    uint32_t uns_max_pairs = 0;                 // dra_set_shard_pairs, reserved by the next peer_setup
+    uint32_t peer_uns_pairs = 0, uns_stride = 0, uns_seq = 0;
+    size_t off_ustage[2] = {0, 0}, off_uflags = 0;
+    uint32_t* d_ubits = nullptr; size_t cap_ubits = 0;   // this rank's words of the call
+    uint32_t* d_upair_pod = nullptr; size_t cap_upair_pod = 0;   // candidate form: pair -> pod (k_uns_prep)
     unsigned long long* d_timeline = nullptr; size_t tl_cap = 0; uint32_t tl_n = 0;
     const dra_out_rec* gather_table = nullptr;  // where the last gather's complete table lives (device)
     uint32_t gather_n_per = 0, gather_len = 0;   // gather_len != 0: a global table of that many records
@@ -587,6 +593,36 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
     return DRA_OK;
 }
 
+template <bool WIN>
+void launch_unsuitable_w(dra_ctx* ctx, const UnsArgs& a, uint32_t W, uint32_t grid) {
+    if (a.exhaustive) {
+        if (W == 8) k_unsuitable<8, 8, true, WIN><<<grid, 256, 0, ctx->stream>>>(a);
+        else if (W == 16) k_unsuitable<8, 16, true, WIN><<<grid, 256, 0, ctx->stream>>>(a);
+        else k_unsuitable<8, 32, true, WIN><<<grid, 256, 0, ctx->stream>>>(a);
+    } else {
+        if (W == 8) k_unsuitable<8, 8, false, WIN><<<grid, 256, 0, ctx->stream>>>(a);
+        else if (W == 16) k_unsuitable<8, 16, false, WIN><<<grid, 256, 0, ctx->stream>>>(a);
+        else k_unsuitable<8, 32, false, WIN><<<grid, 256, 0, ctx->stream>>>(a);
+    }
+}
+
+// k_unsuitable over n_walk pairs (win: the sharded call's node window, n_walk = a.n_walk; else n_walk = a.n_pair); lanes per
+// pair from the widest node: 8 lanes = 4 pairs per warp.  Enqueues only.
+int launch_unsuitable(dra_ctx* ctx, UnsArgs& a, bool win) {
+    const uint32_t W = ctx->max_width <= 8 ? 8u : (ctx->max_width <= 16 ? 16u : 32u);
+    const uint32_t per_cta = 8 * (32 / W);
+    const uint32_t n_walk = win ? a.n_walk : a.n_pair;
+    const uint32_t grid = std::max(1u, std::min((n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
+    if (a.exhaustive) {
+        a.work = ctx->d_ticket + 12;
+        CU(cudaMemsetAsync(a.work, 0, 4, ctx->stream));
+    }
+    if (win) launch_unsuitable_w<true>(ctx, a, W, grid);
+    else launch_unsuitable_w<false>(ctx, a, W, grid);
+    ctx->launches += 1;
+    return DRA_OK;
+}
+
 int collect_timings(dra_ctx* ctx, int n_marks) {
     if (!ctx->profiling) return DRA_OK;
     for (int i = 0; i < 5; ++i) ctx->timings[i] = 0.f;
@@ -601,13 +637,14 @@ int collect_timings(dra_ctx* ctx, int n_marks) {
 
 int check_err(dra_ctx* ctx) {
     uint32_t oor = ctx->h_err[ERR_OUT_RANGE], ns = ctx->h_err[ERR_NOT_SORTED], pt = ctx->h_err[ERR_PEER_TIMEOUT], sp = ctx->h_err[ERR_SHARD_PLAN];
-    const uint32_t dw = ctx->h_err[ERR_DEVICE_WAIT];
-    if (!oor && !ns && !pt && !sp && !dw) return DRA_OK;
+    const uint32_t dw = ctx->h_err[ERR_DEVICE_WAIT], bo = ctx->h_err[ERR_BAD_OFFSETS];
+    if (!oor && !ns && !pt && !sp && !dw && !bo) return DRA_OK;
     for (uint32_t i = 0; i < ERR_WORDS; ++i) ctx->h_err[i] = 0;
     cudaMemsetAsync(ctx->d_err, 0, ERR_WORDS * sizeof(uint32_t), ctx->stream);
     cudaStreamSynchronize(ctx->stream);
     if (sp) return fail(ctx, DRA_E_STATE, "sharded call: %u claims fell into this shard, more than the launch was laid out for; nothing was changed, call again", ctx->h_sc_counts ? ctx->h_sc_counts[0] : 0u);
     if (dw) return fail(ctx, DRA_E_CUDA, "a device-side wait inside one kernel (grid barrier / look-back over CTAs) timed out: CTAs were not scheduled together; state is undefined, reload the inventory");
+    if (bo) return fail(ctx, DRA_E_INVAL, "sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays; nothing was evaluated");
     if (pt) return fail(ctx, DRA_E_NCCL, "all-gather: a rank did not deliver its records in time (or aborted its batch)");
     if (ns) return fail(ctx, DRA_E_INVAL, "DRA_F_NODE_SORTED given but claims are not sorted by node; inventory unchanged");
     return fail(ctx, DRA_E_INVAL, "out_off/n_out: a claim's slots fall outside out[]; inventory state is undefined, reset it");
@@ -813,7 +850,7 @@ void dra_ctx_destroy(dra_ctx* c) {
     void* dev[] = {c->d_inv_live, c->d_inv_pristine, c->d_node_off, c->d_tbl, c->d_claims, c->d_sorted, c->d_out_off,
                    c->d_out, c->d_rank, c->d_hist, c->d_claim_off, c->d_pod_off, c->d_cand_off, c->d_cand_nodes,
                    c->d_pair_pod, c->d_bits, c->d_err, c->d_attrs, c->d_sels, c->d_podrec, c->d_cursor, c->d_cclaims, c->d_coff,
-                   c->d_sc_status, c->d_sc_counts, c->d_gtable, c->d_rank_slots, c->d_sc_times};
+                   c->d_sc_status, c->d_sc_counts, c->d_gtable, c->d_rank_slots, c->d_sc_times, c->d_ubits, c->d_upair_pod};
     for (void* p : dev) if (p) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
     if (c->h_sc_counts) cudaFreeHost((void*)c->h_sc_counts);
@@ -1168,23 +1205,8 @@ int dra_unsuitable_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
         a.dense = dense ? 1u : 0u;
         a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
         Prof prof(ctx);
-        // lanes per pair from the widest node: 8 lanes = 4 pairs per warp
-        const uint32_t W = ctx->max_width <= 8 ? 8u : (ctx->max_width <= 16 ? 16u : 32u);
-        const uint32_t per_cta = 8 * (32 / W);
-        const uint32_t grid = std::max(1u, std::min((n_pair + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
-        if (a.exhaustive) {
-            a.work = ctx->d_ticket + 12;
-            CU(cudaMemsetAsync(a.work, 0, 4, ctx->stream));
-            if (W == 8) k_unsuitable<8, 8, true><<<grid, 256, 0, ctx->stream>>>(a);
-            else if (W == 16) k_unsuitable<8, 16, true><<<grid, 256, 0, ctx->stream>>>(a);
-            else k_unsuitable<8, 32, true><<<grid, 256, 0, ctx->stream>>>(a);
-        } else {
-            if (W == 8) k_unsuitable<8, 8, false><<<grid, 256, 0, ctx->stream>>>(a);
-            else if (W == 16) k_unsuitable<8, 16, false><<<grid, 256, 0, ctx->stream>>>(a);
-            else k_unsuitable<8, 32, false><<<grid, 256, 0, ctx->stream>>>(a);
-        }
+        if ((rc = launch_unsuitable(ctx, a, false))) return rc;
         prof.mark();
-        ctx->launches += 1;
         if ((rc = grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, words * 4))) return rc;
         CU(cudaMemcpyAsync(ctx->h_out, ctx->d_bits, words * 4, cudaMemcpyDeviceToHost, ctx->stream));
     }
@@ -1321,7 +1343,8 @@ int dra_comm_init(dra_ctx* ctx, const void* id128, int rank, int world) {
 
 namespace {
 
-// (Re)allocates this rank's gather buffer:  [table x2][staging x2: world slices of cap packets][headers x2]
+// (Re)allocates this rank's gather buffer:  [table x2][staging x2: world slices of cap packets][headers x2][rendezvous flags]
+// and, after dra_set_shard_pairs(max_pairs > 0), [UnsuitableNodes staging x2: world slices of uns_stride words][their flags]
 int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, uint32_t cap) {
     if (ctx->world > (int)PEER_MAX) return fail(ctx, DRA_E_INVAL, "world %d > %u", ctx->world, PEER_MAX);
     CU(cudaSetDevice(ctx->device));
@@ -1338,6 +1361,18 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
     for (int p = 0; p < 2; ++p) ctx->off_stage[p] = take((size_t)ctx->world * cap * 16);
     for (int p = 0; p < 2; ++p) ctx->off_hdr[p] = take((size_t)ctx->world * 16);
     ctx->off_flags = take((size_t)PEER_MAX * 4); ctx->rendezvous_seq = 0;
+    ctx->peer_uns_pairs = ctx->uns_max_pairs;
+    ctx->uns_stride = (uint32_t)(((size_t)ctx->uns_max_pairs + 127) / 128 * 4);     // words, whole 16-byte units
+    if (ctx->uns_stride) {
+        for (int p = 0; p < 2; ++p) ctx->off_ustage[p] = take((size_t)ctx->world * ctx->uns_stride * 4);
+        ctx->off_uflags = take((size_t)PEER_MAX * 4);
+        // the call's own buffers at full size now: growing one inside the call would cudaFree the old one, which waits for
+        // the whole device — where a peer's merge may already be spinning for this rank's push (ranks sharing a device)
+        int rc;
+        if ((rc = grow(ctx, ctx->d_ubits, ctx->cap_ubits, ctx->uns_stride))) return rc;
+        if ((rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, ctx->uns_max_pairs))) return rc;
+    }
+    ctx->uns_seq = 0;
     ctx->peer_bytes = off;
     CU(cudaMalloc((void**)&ctx->peer_local, ctx->peer_bytes));
     CU(cudaMemset(ctx->peer_local, 0, ctx->peer_bytes));
@@ -1427,7 +1462,7 @@ int dra_peer_import_local(dra_ctx* ctx, dra_ctx* const* ctxs) {
     for (int r = 0; r < ctx->world; ++r) {
         dra_ctx* o = ctxs[r];
         if (!o || !o->peer_local || o->world != ctx->world || o->rank != r || o->peer_form != ctx->peer_form ||
-            o->peer_cap != ctx->peer_cap || o->peer_tab_len != ctx->peer_tab_len)
+            o->peer_cap != ctx->peer_cap || o->peer_tab_len != ctx->peer_tab_len || o->peer_uns_pairs != ctx->peer_uns_pairs)
             return fail(ctx, DRA_E_INVAL, "dra_peer_import_local: context %d is not set up like this one", r);
         if (o->device != ctx->device) {
             int ok = 0; CU(cudaDeviceCanAccessPeer(&ok, ctx->device, o->device));
@@ -1649,6 +1684,86 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
     if (rc) return rc;
     if (gather && !tail_done && (rc = launch_gather(ctx, g, ctx->d_cclaims, cap, ctx->d_sc_counts, ctx->d_coff, n_out, d_out_off != nullptr, n_local_node))) return rc;
     ctx->gather_table = (const dra_out_rec*)table; ctx->gather_n_per = n_out; ctx->gather_len = n_out;
+    return DRA_OK;
+}
+
+int dra_set_shard_pairs(dra_ctx* ctx, uint32_t max_pairs) {
+    if (!ctx) return DRA_E_INVAL;
+    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "dra_set_shard_pairs: call it before dra_shard_export");
+    if (max_pairs > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "max_pairs %u: too many (pod, node) pairs", max_pairs);
+    ctx->uns_max_pairs = max_pairs;
+    return DRA_OK;
+}
+
+// Sharded UnsuitableNodes: prep (offset checks, pair -> pod) -> k_unsuitable on this rank's node window -> push of this rank's
+// words to every peer -> wait + OR into the caller's bytes.  Enqueues only.
+int dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                       const uint32_t* d_pod_off, uint32_t n_pod,
+                                       const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                       uint8_t* d_suitable_bits, uint32_t flags) {
+    if (!ctx || !d_pod_off || (n_claim && !d_claims)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_unsuitable_batch_global_device: unknown flags 0x%x", flags);
+    if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    const bool dense = d_cand_nodes == nullptr && d_cand_off == nullptr;
+    if (!dense && (!d_cand_nodes || !d_cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
+    if (dense && (uint64_t)n_pod * ctx->n_node != n_pair)
+        return fail(ctx, DRA_E_INVAL, "dense form: n_pair %u != n_pod %u x n_node %u", n_pair, n_pod, ctx->n_node);
+    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    const bool gather = ctx->world > 1;
+    if (gather && !(ctx->peer_ready && ctx->peer_form == 2)) return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
+    if (gather && n_pair > ctx->peer_uns_pairs)
+        return fail(ctx, DRA_E_INVAL, "n_pair %u exceeds the max_pairs (%u) of dra_set_shard_pairs before dra_shard_export", n_pair, ctx->peer_uns_pairs);
+    if (n_pair && !d_suitable_bits) return DRA_E_INVAL;
+    if (!n_pair) return DRA_OK;                        // every rank sees the same n_pair: none of them exchanges anything
+    CU(cudaSetDevice(ctx->device));
+    int rc = upload_table(ctx);
+    if (rc) return rc;
+    const size_t n_words = ((size_t)n_pair + 31) / 32, n_words4 = ((size_t)n_pair + 127) / 128 * 4;
+    // world > 1: peer_setup sized both for max_pairs, so these never reallocate there (no cudaFree while peers wait)
+    if ((rc = grow(ctx, ctx->d_ubits, ctx->cap_ubits, n_words4))) return rc;
+    if (!dense && (rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, n_pair))) return rc;
+    const Err err = err_of(ctx);
+    CU(cudaMemsetAsync(ctx->d_ubits, 0, n_words4 * 4, ctx->stream));
+    k_uns_prep<<<std::max(1u, (n_pod + 7) / 8), 256, 0, ctx->stream>>>(d_pod_off, dense ? nullptr : d_cand_off, n_pod, n_claim, n_pair,
+                                                                       ctx->d_upair_pod, err);
+    ctx->launches += 1;
+    UnsArgs a; memset(&a, 0, sizeof a);
+    a.claims = (const uint4*)d_claims; a.pod_off = d_pod_off; a.n_pod = n_pod;
+    a.cand_nodes = d_cand_nodes; a.cand_off = d_cand_off; a.pair_pod = ctx->d_upair_pod; a.n_pair = n_pair;
+    a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.tbl = ctx->d_tbl; a.bits = ctx->d_ubits;
+    a.sel = sel_of(ctx);
+    a.dense = dense ? 1u : 0u;
+    a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
+    a.node_lo = ctx->shard_lo; a.n_win = ctx->shard_hi - ctx->shard_lo;
+    a.n_walk = dense ? n_pod * a.n_win : n_pair;           // (n_pod * n_win <= n_pod * n_node = n_pair)
+    a.gate = ctx->d_err + ERR_BAD_OFFSETS;
+    Prof prof(ctx);
+    if (a.n_walk && (rc = launch_unsuitable(ctx, a, true))) return rc;
+    prof.mark();
+    UnsExchange x; memset(&x, 0, sizeof x);
+    x.bits = ctx->d_ubits; x.out = d_suitable_bits;
+    x.n_words = (uint32_t)n_words; x.n_bytes = (uint32_t)(((size_t)n_pair + 7) / 8);
+    x.world = 1; x.rank = 0; x.spin_limit = ctx->peer_spin; x.err = err;
+    if (gather) {
+        const uint32_t seq = ++ctx->uns_seq, par = seq & 1u;
+        x.world = (uint32_t)ctx->world; x.rank = (uint32_t)ctx->rank; x.seq = seq; x.stride = ctx->uns_stride;
+        for (int r = 0; r < ctx->world; ++r) {
+            x.stage[r] = (uint32_t*)(ctx->peer_base[r] + ctx->off_ustage[par]) + (size_t)ctx->rank * ctx->uns_stride;
+            x.flag[r] = (uint32_t*)(ctx->peer_base[r] + ctx->off_uflags) + ctx->rank;
+        }
+        x.my_stage = (const uint32_t*)(ctx->peer_local + ctx->off_ustage[par]);
+        x.my_flags = (const uint32_t*)(ctx->peer_local + ctx->off_uflags);
+        const uint32_t n4 = (uint32_t)(n_words4 / 4);
+        k_uns_push<<<std::max(1u, std::min((n4 + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, ctx->stream>>>(x);
+        ctx->launches += 1;
+    }
+    const uint32_t merge_grid = std::max(1u, std::min((uint32_t)((n_words + 1023) / 1024), (uint32_t)std::max(1, ctx->n_sm / 4)));
+    k_uns_merge<<<merge_grid, 256, 0, ctx->stream>>>(x);
+    ctx->launches += 1;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded UnsuitableNodes launch: %s", cudaGetErrorString(e));
     return DRA_OK;
 }
 

@@ -32,6 +32,7 @@ constexpr uint32_t ERR_NOT_SORTED = 2u;
 constexpr uint32_t ERR_PEER_TIMEOUT = 3u;
 constexpr uint32_t ERR_DEVICE_WAIT = 5u;     // a wait inside ONE GPU gave up (grid barrier, look-back): cannot happen unless CTAs were not co-scheduled
 constexpr uint32_t ERR_SHARD_PLAN = 4u;      // sharded call: more claims fell into this shard than the launch was laid out for
+constexpr uint32_t ERR_BAD_OFFSETS = 6u;     // sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays
 constexpr uint32_t ERR_WORDS = 8u;
 constexpr uint32_t PEER_MAX = 16;         // ranks of one box
 
@@ -2662,6 +2663,10 @@ struct UnsArgs {
     uint32_t exhaustive; // spec §12: pod evaluation with the backtracking search
     uint32_t* work;      // EXH: next unclaimed pair (zeroed by the caller) — searches differ by orders of magnitude in length,
                          //      so the warps take their pairs from a counter instead of a fixed stride
+    // sharded call only (k_unsuitable<..., WIN = true>):
+    uint32_t node_lo, n_win;   // node window: only pairs whose node lies in [node_lo, node_lo + n_win) are evaluated
+    uint32_t n_walk;           // pairs the kernel walks: dense n_pod * n_win (mapped back to pod * n_node + node), else n_pair
+    const uint32_t* gate;      // *gate != 0: the inputs failed their device-side check, evaluate nothing
 };
 
 struct GlobalGet {
@@ -2672,10 +2677,13 @@ struct GlobalGet {
 // W lanes per (pod, candidate) pair: 32/W pairs share a warp (W = 8 for the usual <= 8 GPUs per node), each
 // group running its own claim loop with group-wide ballots.  dense = every pod against every node
 // (pair = pod * n_node + node): no candidate arrays at all.
-template <int WPC, int W, bool EXH>                    // EXH: spec §12 (own instantiation: the default kernel stays as lean as it was)
+// WIN: the node window and the gate of the sharded call (own instantiations: with the window the exhaustive kernel needs
+// 81 registers instead of 80, which costs dra_unsuitable_batch a third of its CTAs per SM).
+template <int WPC, int W, bool EXH, bool WIN>          // EXH: spec §12 (own instantiation: the default kernel stays as lean as it was)
 __global__ void __launch_bounds__(WPC * 32, 2)
 k_unsuitable(const UnsArgs a) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
+    if (WIN && a.gate && __ldcg(a.gate)) return;
     for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
     __syncthreads();
     constexpr uint32_t G = 32 / W;
@@ -2689,13 +2697,17 @@ k_unsuitable(const UnsArgs a) {
             if (lane == 0) nxt = atomicAdd(a.work, G);
             pw = __shfl_sync(FULLMASK, nxt, 0);
         }
-        if (pw >= a.n_pair) break;
-        const uint32_t pair = pw + grp;
-        if (pair >= a.n_pair) continue;                                  // whole group skips together
-        uint32_t pod, node;
-        if (a.dense) { pod = pair / a.n_node; node = pair - pod * a.n_node; }
+        const uint32_t n_walk = WIN ? a.n_walk : a.n_pair;
+        if (pw >= n_walk) break;
+        const uint32_t walk = pw + grp;
+        if (walk >= n_walk) continue;                                    // whole group skips together
+        uint32_t pod, node, pair = walk;
+        if (a.dense) {
+            if (WIN) { pod = walk / a.n_win; node = a.node_lo + (walk - pod * a.n_win); pair = pod * a.n_node + node; }
+            else { pod = pair / a.n_node; node = pair - pod * a.n_node; }
+        }
         else { pod = __ldg(&a.pair_pod[pair]); node = __ldg(&a.cand_nodes[pair]); }
-        if (node >= a.n_node || pod >= a.n_pod) continue;                 // unknown node: unsuitable
+        if ((WIN ? node - a.node_lo >= a.n_win : node >= a.n_node) || pod >= a.n_pod) continue;   // unknown node (or another rank's): unsuitable here
         const uint32_t c0 = __ldg(&a.pod_off[pod]);
         const uint32_t cnt = __ldg(&a.pod_off[pod + 1]) - c0;
         const uint32_t g0 = __ldg(&a.node_off[node]);
@@ -2716,6 +2728,91 @@ k_unsuitable(const UnsArgs a) {
         uint32_t k = 0;
         while (k < cnt && !sink.stop()) k += node_step(L, D, lane, g0, tbl_s, get, k, cnt, sink, true, a.sel, gmask, gbase);
         if (!sink.failed && gl == 0) atomicOr(&a.bits[pair >> 5], 1u << (pair & 31));
+    }
+}
+
+// ---- sharded UnsuitableNodes (dra_unsuitable_batch_global_device) ----------------------------------------------------
+// Warp per pod: checks that pod_off (and cand_off) are monotone and span their arrays — every rank gets the same arrays,
+// so every rank finds the same fault — and, in the candidate form, writes pair -> pod for the pod's candidates (the
+// warp's lanes stride the pod's range: one pod with many candidates costs coalesced stores, not a serial loop).
+// A fault sets ERR_BAD_OFFSETS, which gates k_unsuitable (UnsArgs::gate).
+__global__ void __launch_bounds__(256)
+k_uns_prep(const uint32_t* __restrict__ pod_off, const uint32_t* __restrict__ cand_off, uint32_t n_pod, uint32_t n_claim,
+           uint32_t n_pair, uint32_t* __restrict__ pair_pod, Err err) {
+    const uint32_t lane = threadIdx.x & 31, p = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (p == 0 && lane == 0) {
+        const bool span = __ldg(&pod_off[0]) == 0 && __ldg(&pod_off[n_pod]) == n_claim &&
+                          (!cand_off || (__ldg(&cand_off[0]) == 0 && __ldg(&cand_off[n_pod]) == n_pair));
+        if (!span) err.set(ERR_BAD_OFFSETS);
+    }
+    if (p >= n_pod) return;
+    bool bad = __ldg(&pod_off[p + 1]) < __ldg(&pod_off[p]);
+    if (cand_off) {
+        const uint32_t k0 = __ldg(&cand_off[p]), k1 = __ldg(&cand_off[p + 1]);
+        bad = bad || k1 < k0 || k1 > n_pair;
+        if (!bad) for (uint32_t k = k0 + lane; k < k1; k += 32) pair_pod[k] = p;
+    }
+    if (bad && lane == 0) err.set(ERR_BAD_OFFSETS);
+}
+
+// The bit exchange.  Latency matters little next to the evaluation (100 us to ms), so: plain copies, one fence, one flag.
+//   k_uns_push   this rank's words (its own pairs' bits, every other bit zero) into its slice of every peer's staging area
+//                (parity applied), then a system-scope fence per thread.  Nothing waits here.
+//   k_uns_merge  block 0 raises this rank's flag word at every peer to the call's sequence number (the push grid has
+//                completed, its stores are fenced); every block then waits — bounded, ERR_PEER_TIMEOUT, never a hang — until
+//                every peer's flag here has reached it, and ORs the world's slices into the caller's bytes.  A small grid of
+//                its own: ranks sharing one device must not find their evaluation's SMs held by a peer's waiting CTAs.
+// Staging is double-buffered by call parity: a rank is never two calls ahead, since its next merge waits for this rank's next
+// push.  With world 1 the merge only turns the words into ceil(n_pair/8) bytes.
+struct UnsExchange {
+    uint32_t* stage[PEER_MAX];    // stage[p]: THIS rank's slice inside peer p's staging area (parity applied)
+    uint32_t* flag[PEER_MAX];     // flag[p]: this rank's flag word at peer p
+    const uint32_t* my_stage;     // this rank's staging area (parity applied): sender s's slice at my_stage + s * stride
+    const uint32_t* my_flags;     // [PEER_MAX], indexed by sender
+    const uint32_t* bits;         // this rank's words
+    uint8_t* out;                 // ceil(n_pair / 8) bytes
+    uint32_t n_words, n_bytes, stride, world, rank, seq;
+    long long spin_limit;
+    Err err;
+};
+
+__global__ void __launch_bounds__(256)
+k_uns_push(const UnsExchange x) {
+    const uint32_t n4 = (x.n_words + 3) / 4;                          // slices and the local words are padded to 16 bytes
+    const uint4* src = reinterpret_cast<const uint4*>(x.bits);
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x) {
+        const uint4 v = __ldcg(&src[i]);
+        for (uint32_t p = 0; p < x.world; ++p)
+            if (p != x.rank) reinterpret_cast<uint4*>(x.stage[p])[i] = v;
+    }
+    __threadfence_system();
+}
+
+__global__ void __launch_bounds__(256)
+k_uns_merge(const UnsExchange x) {
+    const uint32_t tid = threadIdx.x;
+    if (blockIdx.x == 0 && tid < x.world && tid != x.rank) {
+        __threadfence_system();
+        asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(x.flag[tid]), "r"(x.seq) : "memory");
+    }
+    if (tid < x.world && tid != x.rank) {
+        const long long t0 = clock64();
+        uint32_t v;
+        do {
+            asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(x.my_flags + tid) : "memory");
+            if ((int32_t)(v - x.seq) >= 0) break;
+            if (clock64() - t0 > x.spin_limit) { x.err.set(ERR_PEER_TIMEOUT); break; }
+        } while (true);
+    }
+    __syncthreads();
+    const bool whole = (reinterpret_cast<uintptr_t>(x.out) & 3u) == 0;
+    for (uint32_t w = blockIdx.x * blockDim.x + tid; w < x.n_words; w += gridDim.x * blockDim.x) {
+        uint32_t v = __ldcg(&x.bits[w]);
+        for (uint32_t s = 0; s < x.world; ++s)
+            if (s != x.rank) v |= __ldcg(&x.my_stage[(size_t)s * x.stride + w]);
+        const uint32_t b0 = w * 4;
+        if (whole && b0 + 4 <= x.n_bytes) *reinterpret_cast<uint32_t*>(x.out + b0) = v;
+        else for (uint32_t b = 0; b < 4 && b0 + b < x.n_bytes; ++b) x.out[b0 + b] = (uint8_t)(v >> (8 * b));
     }
 }
 
