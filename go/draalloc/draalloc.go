@@ -293,6 +293,23 @@ func (c *Context) UnsuitableNodesGlobal(pinnedClaims unsafe.Pointer, nClaim int,
 	return nil
 }
 
+// AllocatePodsGlobal: pod-mode Allocate on a sharded world (dra_allocate_pods_batch_global_device), the step after
+// UnsuitableNodesGlobal with DRA_F_EXHAUSTIVE.  The same pods on every context, in dra_host_alloc'ed (pinned) memory
+// (pinnedOutOff may be nil); each context places the pods whose first claim names one of its nodes, and GatherRead gives
+// every context the whole table.  Returns at once; Sync reports completion and errors found on the device.  Unbuilt,
+// like the rest of this file.
+func (c *Context) AllocatePodsGlobal(pinnedClaims unsafe.Pointer, nClaim int, pinnedPodOff unsafe.Pointer, nPod int,
+	pinnedOutOff unsafe.Pointer, nOut int, flags uint32) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_allocate_pods_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
+		(*C.uint32_t)(pinnedPodOff), C.uint32_t(nPod), (*C.uint32_t)(pinnedOutOff), C.uint32_t(nOut), C.uint32_t(flags))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
 // Sync waits for the calls enqueued on the context and reports the errors they found on the device (dra_ctx_sync).
 func (c *Context) Sync() error {
 	c.mu.Lock()

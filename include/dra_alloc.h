@@ -323,7 +323,8 @@ int  dra_peer_rendezvous_device(dra_ctx* ctx);
  *   result: dra_gather_table / dra_gather_read (n_out records, input order, global GPU indices)
  * out_off must tile [0, n_out) (slots no claim owns keep their previous contents).  flags: DRA_F_FRESH_INVENTORY.
  * With world == 1 no export is needed (the table is local).  A rank's live inventory is authoritative for its own
- * node range only (UnsuitableNodes on such a world: dra_unsuitable_batch_global_device below).  d_claims may also be a pinned host buffer (dra_host_alloc): the compaction kernel reads every claim
+ * node range only (UnsuitableNodes and pods Allocate on such a world: dra_unsuitable_batch_global_device and
+ * dra_allocate_pods_batch_global_device below).  d_claims may also be a pinned host buffer (dra_host_alloc): the compaction kernel reads every claim
  * exactly once, so it then ingests the batch over PCIe itself — no copy-engine transfer in front of the call. */
 int  dra_set_shard(dra_ctx* ctx, uint32_t node_lo, uint32_t node_hi, int take_stray);
 /* The whole partition: rank r serves nodes [bounds[r], bounds[r+1]) (bounds has world+1 entries, bounds[world] = n_node),
@@ -355,6 +356,23 @@ int  dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cla
                                         const uint32_t* d_pod_off, uint32_t n_pod,
                                         const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
                                         uint8_t* d_suitable_bits, uint32_t flags);
+
+/* Pods Allocate over a sharded world (spec §12, "Sharded form"): the classic flow's second step after
+ * dra_unsuitable_batch_global_device(..., DRA_F_EXHAUSTIVE).  The SAME claims, pod_off, out_off, n_out and flags on every
+ * rank (device pointers, or dra_host_alloc'ed buffers).  A non-empty pod belongs to the rank whose node range holds the
+ * node of its FIRST claim (a node outside the inventory: the stray rank); the owner writes every slot of every claim of the
+ * pod (OK, POD, SEARCH_LIMIT or INVALID, validated and counted on global node indices) and applies the placements to its
+ * live inventory.  Every rank ends with the WHOLE table (dra_gather_table / dra_gather_read: n_out records, global slots,
+ * global GPU indices): byte for byte what dra_allocate_pods_batch answers on ONE inventory made of every rank's own nodes,
+ * and each rank's inventory over its own GPU range equals that call's; GPUs outside the range are not written.
+ * flags: DRA_F_EXHAUSTIVE, DRA_F_FRESH_INVENTORY (the pristine copy of the rank's own GPUs is read, the live one written).
+ * Prerequisites as for dra_allocate_batch_global_device, except that world > 1 needs dra_set_shard_map (a bare
+ * dra_set_shard: DRA_E_STATE).  Enqueues on ctx's stream and returns; n_pod == 0 enqueues nothing.  Completion and device-detected errors
+ * surface at dra_ctx_sync: pod_off not monotone or not spanning [0, n_claim], a slot range outside n_out, or a rank owning
+ * more slots than its packet room give DRA_E_INVAL on EVERY rank (they read the same arrays), with no inventory changed. */
+int  dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                           const uint32_t* d_pod_off, uint32_t n_pod,
+                                           const uint32_t* d_out_off, uint32_t n_out, uint32_t flags);
 
 /* ---- adjacent integer searches of the reference, batched (API completeness; SURVEY §8f-4) -------------- */
 
@@ -416,6 +434,8 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_COMPACT_FLAT8     0x10000u  /* sharded call: compaction in 2048-claim tiles */
 #define DRA_K_COMPACT_LOOKBACK  0x20000u  /* sharded call: compaction with a decoupled look-back (beyond 2M claims) */
 #define DRA_K_COMPACT_IN_KERNEL 0x40000u  /* sharded call: compaction inside the single-launch kernel */
+#define DRA_K_POD_SHARD         0x80000u  /* sharded pods Allocate: pod records + ownership, gate, k_pods on the node window */
+#define DRA_K_POD_GATHER        0x100000u /* sharded pods Allocate: all-gather of the owned pods' records (world > 1) */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

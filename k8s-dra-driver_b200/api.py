@@ -22,7 +22,7 @@ KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x0
            "sorted_prep": 0x00010, "bucket_small": 0x00020, "hist8": 0x00040, "hist8_multi": 0x00080,
            "hist_warp": 0x00100, "scan8": 0x00200, "scan_rows": 0x00400, "scan": 0x00800, "scatter": 0x01000,
            "pack1": 0x02000, "pack4": 0x04000, "compact_flat1": 0x08000, "compact_flat8": 0x10000,
-           "compact_lookback": 0x20000, "compact_in_kernel": 0x40000}
+           "compact_lookback": 0x20000, "compact_in_kernel": 0x40000, "pod_shard": 0x80000, "pod_gather": 0x100000}
 
 
 class DraError(RuntimeError):
@@ -71,6 +71,7 @@ SYMBOLS = {
     "dra_allocate_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _u32]),
     "dra_set_shard_pairs": (_i32, [_vp, _u32]),
     "dra_unsuitable_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _u32]),
+    "dra_allocate_pods_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _u32, _u32]),
     "dra_mps_limits_batch": (_i32, [_vp, _vp, _u32, _vp, _vp]),
     "dra_imex_offsets_batch": (_i32, [_vp, _vp, _vp, _u32, C.c_int32, C.c_int32, _vp]),
     "dra_calibrate": (_i32, [_vp, C.POINTER(_u32)]),
@@ -380,6 +381,14 @@ class Context:
         self._check(self._lib.dra_unsuitable_batch_global_device(self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod,
                                                                  _ptr(d_cand_nodes), _ptr(d_cand_off), n_pair, _ptr(d_bits),
                                                                  flags))
+
+    def allocate_pods_global_device(self, d_claims: int, n_claim: int, d_pod_off: int, n_pod: int, d_out_off: int | None,
+                                    n_out: int, flags: int = 0) -> None:
+        """Sharded pods Allocate (spec §12): the SAME pods on every rank (device pointers); a pod is placed by the rank that
+        owns its first claim's node, and every rank receives the whole table (gather_read()).  flags: F_EXHAUSTIVE,
+        F_FRESH_INVENTORY.  Enqueues, no synchronisation; errors found on the device surface at sync()."""
+        self._check(self._lib.dra_allocate_pods_batch_global_device(self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod,
+                                                                    _ptr(d_out_off), n_out, flags))
 
     def peer_import(self, handles) -> None:
         blob = b"".join(handles)

@@ -174,6 +174,12 @@ struct dra_ctx {
     size_t off_ustage[2] = {0, 0}, off_uflags = 0;
     uint32_t* d_ubits = nullptr; size_t cap_ubits = 0;   // this rank's words of the call
     uint32_t* d_upair_pod = nullptr; size_t cap_upair_pod = 0;   // candidate form: pair -> pod (k_uns_prep)
+    // sharded pods Allocate
+    uint32_t* d_spod = nullptr;                 // [SP_WORDS] call words (dra_device.cuh SPodArgs)
+    // Buffers a sharded call outgrew while peers on this device may be waiting for it: cudaFree would wait for the whole
+    // device, so they are freed at the next dra_ctx_sync instead (grow / grow_nc while defer_free is set).
+    bool defer_free = false;
+    std::vector<void*> retired;
     unsigned long long* d_timeline = nullptr; size_t tl_cap = 0; uint32_t tl_n = 0;
     const dra_out_rec* gather_table = nullptr;  // where the last gather's complete table lives (device)
     uint32_t gather_n_per = 0, gather_len = 0;   // gather_len != 0: a global table of that many records
@@ -200,7 +206,8 @@ template <class T>
 int grow(dra_ctx* ctx, T*& p, size_t& cap, size_t need, size_t slack = 16) {
     if (need <= cap && p) return DRA_OK;
     size_t ncap = std::max(need, cap + cap / 2) + slack;
-    if (p) CU(cudaFree(p));
+    if (p && ctx->defer_free) ctx->retired.push_back(p);
+    else if (p) CU(cudaFree(p));
     p = nullptr;
     CU(cudaMalloc((void**)&p, ncap * sizeof(T)));
     cap = ncap;
@@ -211,7 +218,8 @@ int grow(dra_ctx* ctx, T*& p, size_t& cap, size_t need, size_t slack = 16) {
 template <class T>
 int grow_nc(dra_ctx* ctx, T*& p, size_t have_cap, size_t new_cap) {   // companion buffer, cap tracked elsewhere
     if (p && new_cap <= have_cap) return DRA_OK;
-    if (p) CU(cudaFree(p));
+    if (p && ctx->defer_free) ctx->retired.push_back(p);
+    else if (p) CU(cudaFree(p));
     p = nullptr;
     CU(cudaMalloc((void**)&p, new_cap * sizeof(T)));
     ctx->state_epoch++;
@@ -637,14 +645,16 @@ int collect_timings(dra_ctx* ctx, int n_marks) {
 
 int check_err(dra_ctx* ctx) {
     uint32_t oor = ctx->h_err[ERR_OUT_RANGE], ns = ctx->h_err[ERR_NOT_SORTED], pt = ctx->h_err[ERR_PEER_TIMEOUT], sp = ctx->h_err[ERR_SHARD_PLAN];
-    const uint32_t dw = ctx->h_err[ERR_DEVICE_WAIT], bo = ctx->h_err[ERR_BAD_OFFSETS];
-    if (!oor && !ns && !pt && !sp && !dw && !bo) return DRA_OK;
+    const uint32_t dw = ctx->h_err[ERR_DEVICE_WAIT], bo = ctx->h_err[ERR_BAD_OFFSETS], bp = ctx->h_err[ERR_BAD_PODS];
+    if (!oor && !ns && !pt && !sp && !dw && !bo && !bp) return DRA_OK;
     for (uint32_t i = 0; i < ERR_WORDS; ++i) ctx->h_err[i] = 0;
     cudaMemsetAsync(ctx->d_err, 0, ERR_WORDS * sizeof(uint32_t), ctx->stream);
     cudaStreamSynchronize(ctx->stream);
     if (sp) return fail(ctx, DRA_E_STATE, "sharded call: %u claims fell into this shard, more than the launch was laid out for; nothing was changed, call again", ctx->h_sc_counts ? ctx->h_sc_counts[0] : 0u);
     if (dw) return fail(ctx, DRA_E_CUDA, "a device-side wait inside one kernel (grid barrier / look-back over CTAs) timed out: CTAs were not scheduled together; state is undefined, reload the inventory");
     if (bo) return fail(ctx, DRA_E_INVAL, "sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays; nothing was evaluated");
+    if (bp) return fail(ctx, DRA_E_INVAL, "sharded pods Allocate: pod_off not monotone or not spanning [0, n_claim], a pod's OutRec slots outside n_out, "
+                                          "or one rank's slots beyond the cap_per_rank of dra_shard_export; no inventory was changed");
     if (pt) return fail(ctx, DRA_E_NCCL, "all-gather: a rank did not deliver its records in time (or aborted its batch)");
     if (ns) return fail(ctx, DRA_E_INVAL, "DRA_F_NODE_SORTED given but claims are not sorted by node; inventory unchanged");
     return fail(ctx, DRA_E_INVAL, "out_off/n_out: a claim's slots fall outside out[]; inventory state is undefined, reset it");
@@ -850,8 +860,9 @@ void dra_ctx_destroy(dra_ctx* c) {
     void* dev[] = {c->d_inv_live, c->d_inv_pristine, c->d_node_off, c->d_tbl, c->d_claims, c->d_sorted, c->d_out_off,
                    c->d_out, c->d_rank, c->d_hist, c->d_claim_off, c->d_pod_off, c->d_cand_off, c->d_cand_nodes,
                    c->d_pair_pod, c->d_bits, c->d_err, c->d_attrs, c->d_sels, c->d_podrec, c->d_cursor, c->d_cclaims, c->d_coff,
-                   c->d_sc_status, c->d_sc_counts, c->d_gtable, c->d_rank_slots, c->d_sc_times, c->d_ubits, c->d_upair_pod};
+                   c->d_sc_status, c->d_sc_counts, c->d_gtable, c->d_rank_slots, c->d_sc_times, c->d_ubits, c->d_upair_pod, c->d_spod};
     for (void* p : dev) if (p) cudaFree(p);
+    for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
     if (c->h_sc_counts) cudaFreeHost((void*)c->h_sc_counts);
     if (c->h_in) cudaFreeHost(c->h_in);
@@ -975,6 +986,8 @@ int dra_ctx_sync(dra_ctx* ctx) {
     QUIESCE();
     CU(cudaSetDevice(ctx->device));
     CU(cudaStreamSynchronize(ctx->stream));
+    std::vector<void*> retired; retired.swap(ctx->retired);
+    for (void* p : retired) CU(cudaFree(p));
     collect_timings(ctx, 5);
     return check_err(ctx);
 }
@@ -1764,6 +1777,100 @@ int dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     ctx->launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded UnsuitableNodes launch: %s", cudaGetErrorString(e));
+    return DRA_OK;
+}
+
+// Sharded pods Allocate: pod records + ownership over every pod (k_spod_records) -> gate / FRESH copy (k_spod_gate) ->
+// stable counting sort of this rank's pods by window node -> k_pods on the window -> all-gather of the owned pods' records
+// (k_spod_gather).  Enqueues only.
+int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                          const uint32_t* d_pod_off, uint32_t n_pod,
+                                          const uint32_t* d_out_off, uint32_t n_out, uint32_t flags) {
+    if (!ctx || !d_pod_off || (n_claim && !d_claims)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~(DRA_F_EXHAUSTIVE | DRA_F_FRESH_INVENTORY))
+        return fail(ctx, DRA_E_INVAL, "dra_allocate_pods_batch_global_device: unknown flags 0x%x", flags);
+    if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (n_claim > (1u << 26) || n_out > (1u << 26) || n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
+    if (!d_out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    if (!n_pod && n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]: no pods for %u claims", n_claim);
+    const bool gather = ctx->world > 1;
+    if (gather && !ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the gather needs every rank's range)");
+    if (gather && !(ctx->peer_ready && ctx->peer_form == 2)) return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
+    if (gather && n_out > ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", n_out, ctx->peer_tab_len);
+    ctx->chain = ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
+    CU(cudaSetDevice(ctx->device));
+    // peers on this device may already wait for this rank: no buffer this call outgrows is freed before the next sync
+    struct DeferFree { dra_ctx* c; ~DeferFree() { c->defer_free = false; } } defer{ctx};
+    ctx->defer_free = gather;
+    int rc = upload_table(ctx);
+    if (rc) return rc;
+    const uint32_t n_win = ctx->shard_hi - ctx->shard_lo;
+    if ((rc = ensure_batch(ctx, n_pod, 1, false))) return rc;
+    const Tiling t = tiling(n_pod, n_win, ctx->n_sm);                 // the sort's tiles are laid out on the window
+    if ((rc = grow(ctx, ctx->d_hist, ctx->cap_hist, (size_t)t.n_tiles * (n_win + 1), 64))) return rc;
+    if (n_pod + 8 > ctx->cap_podrec) {
+        const size_t cap = (size_t)n_pod + n_pod / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_podrec, ctx->cap_podrec, cap))) return rc;
+        ctx->cap_podrec = cap;
+    }
+    if (!ctx->d_spod) CU(cudaMalloc((void**)&ctx->d_spod, SP_WORDS * 4));
+    uint2* table = nullptr; PktGather g; memset(&g, 0, sizeof g);
+    if (gather) {
+        ctx->peer_epoch += 1;
+        g = make_gather(ctx, ctx->peer_epoch, 0, 0, 0, nullptr);
+        g.expect = ctx->d_spod + SP_EXPECT;
+        table = g.table;
+    } else {
+        if ((size_t)n_out + 16 > ctx->cap_gtable) {
+            const size_t ncap = (size_t)n_out + n_out / 4 + 64;
+            if ((rc = grow_nc(ctx, ctx->d_gtable, 0, ncap))) return rc;
+            ctx->cap_gtable = ncap;
+        }
+        table = ctx->d_gtable;
+    }
+    const Err err = err_of(ctx);
+    SPodArgs sa; memset(&sa, 0, sizeof sa);
+    sa.claims = (const uint4*)d_claims; sa.pod_off = d_pod_off; sa.out_off = d_out_off;
+    sa.n_claim = n_claim; sa.n_pod = n_pod; sa.n_out = n_out; sa.n_node = ctx->n_node;
+    sa.node_lo = ctx->shard_lo; sa.node_hi = ctx->shard_hi; sa.take_stray = ctx->shard_stray;
+    sa.rank = (uint32_t)ctx->rank; sa.world = gather ? (uint32_t)ctx->world : 1u; sa.stray_rank = ctx->shard_stray_rank;
+    if (gather) for (int r = 0; r < ctx->world; ++r) sa.rank_hi[r] = ctx->shard_bounds[r + 1];
+    sa.table = table; sa.podrec = ctx->d_podrec; sa.w = ctx->d_spod; sa.err = err;
+    const bool fresh = (flags & DRA_F_FRESH_INVENTORY) != 0;
+    Prof prof(ctx);
+    CU(cudaMemsetAsync(ctx->d_spod, 0, (SP_BAD + 1) * 4, ctx->stream));
+    k_spod_records<<<(n_pod + 255) / 256, 256, 0, ctx->stream>>>(sa);
+    const uint32_t gate_grid = fresh ? std::max(1u, std::min((uint32_t)ctx->n_sm, (ctx->n_gpu + 255) / 256)) : 1u;
+    k_spod_gate<<<gate_grid, 256, 0, ctx->stream>>>(sa, gather ? ctx->peer_cap : 0u, fresh ? ctx->d_inv_pristine : nullptr,
+                                                    ctx->d_inv_live, ctx->d_node_off);
+    ctx->launches += 2; ctx->chain |= DRA_K_POD_SHARD;
+    const uint32_t* d_node_off = ctx->d_node_off + ctx->shard_lo;
+    if ((rc = launch_sort(ctx, ctx->d_podrec, n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, n_win, d_node_off,
+                          ctx->d_spod + SP_NDEV))) return rc;
+    if (n_win) {
+        PodArgs a; memset(&a, 0, sizeof a);
+        a.claims = (const uint4*)d_claims; a.out_off = d_out_off; a.out = table;
+        a.sorted = ctx->d_sorted; a.claim_off = ctx->d_claim_off;
+        a.inv_src = ctx->d_inv_live; a.inv_dst = ctx->d_inv_live; a.node_off = d_node_off; a.tbl = ctx->d_tbl;
+        a.n_node = n_win; a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.sel = sel_of(ctx); a.err = err;
+        static const bool no_pdl = getenv("DRA_NO_PDL") != nullptr;
+        const uint32_t grid = std::max(1u, std::min((n_win + 3) / 4, (uint32_t)ctx->n_sm * 8u));
+        CU(launch_k(k_pods<4>, dim3(grid), dim3(128), 0, ctx->stream, !no_pdl && !ctx->profiling, a));
+        ctx->launches += 1;
+    }
+    prof.mark();
+    if (gather) {
+        // a small grid: it waits for its peers, and ranks sharing one device must not find their sort / k_pods SMs held by it
+        const uint32_t blocks = std::max(1u, std::min((uint32_t)std::max(1, ctx->n_sm / 4), (std::max(n_pod, g.world * g.cap / 4u) + 255u) / 256u));
+        k_spod_gather<<<blocks, 256, 0, ctx->stream>>>(g, sa, ctx->peer_tab_len);
+        ctx->launches += 1; ctx->chain |= DRA_K_POD_GATHER;
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded pods Allocate launch: %s", cudaGetErrorString(e));
+    ctx->gather_table = (const dra_out_rec*)table; ctx->gather_n_per = n_out; ctx->gather_len = n_out;
     return DRA_OK;
 }
 

@@ -33,6 +33,7 @@ constexpr uint32_t ERR_PEER_TIMEOUT = 3u;
 constexpr uint32_t ERR_DEVICE_WAIT = 5u;     // a wait inside ONE GPU gave up (grid barrier, look-back): cannot happen unless CTAs were not co-scheduled
 constexpr uint32_t ERR_SHARD_PLAN = 4u;      // sharded call: more claims fell into this shard than the launch was laid out for
 constexpr uint32_t ERR_BAD_OFFSETS = 6u;     // sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays
+constexpr uint32_t ERR_BAD_PODS = 7u;        // sharded pods Allocate: bad pod_off, slots outside n_out, or a rank's slots beyond its packet room
 constexpr uint32_t ERR_WORDS = 8u;
 constexpr uint32_t PEER_MAX = 16;         // ranks of one box
 
@@ -2886,6 +2887,154 @@ k_pkt_gather(const PktGather g, const uint4* __restrict__ claims, uint32_t n_cla
     }
     pkt_finish_send(g);
     pkt_receive(g, T, NT, err);
+}
+
+// ====================================================================================================
+// sharded pods Allocate (dra_allocate_pods_batch_global_device): every rank reads the WHOLE pod array
+// ====================================================================================================
+// A non-empty pod belongs to the rank whose node range holds its FIRST claim's node (a node outside the inventory: the
+// stray rank).  Every rank validates every pod on GLOBAL node indices and counts every rank's slots (the gather's expected
+// counts); the owner writes the INVALID records of its malformed pods and keys its well-formed pods by their node inside
+// its window for the claim path's counting sort (any other pod gets no node, and the sort drops it — the sort is stable,
+// so a node's pods stay in input order).  k_pods then runs unchanged on the window.
+// Call words (SPodArgs::w), zeroed by the host before the call up to and including SP_BAD:
+constexpr uint32_t SP_BAD = PEER_MAX;             // a fault in the inputs (every rank finds the same one)
+constexpr uint32_t SP_EXPECT = 2 * PEER_MAX;      // [PEER_MAX] packets expected from each rank (its slots, at least 1)
+constexpr uint32_t SP_NDEV = 3 * PEER_MAX;        // pod records the sort takes: n_pod, or 0 when the call is gated
+constexpr uint32_t SP_GATED = 3 * PEER_MAX + 1;   // nothing is evaluated or sent
+constexpr uint32_t SP_WORDS = 4 * PEER_MAX;
+constexpr uint32_t SP_NONE = 0xFFFFFFFFu;
+struct SPodArgs {
+    const uint4* claims; const uint32_t* pod_off; const uint32_t* out_off;
+    uint32_t n_claim, n_pod, n_out, n_node;       // n_node: the whole inventory
+    uint32_t node_lo, node_hi, take_stray;        // this rank's window; take_stray: it owns pods naming no node
+    uint32_t rank, world, stray_rank;             // world > 1: counted with rank_hi (the shard map)
+    uint32_t rank_hi[PEER_MAX];                   // rank r serves nodes [rank_hi[r-1], rank_hi[r])
+    uint2* table;                                 // this rank's table, global slots
+    uint4* podrec;                                // [n_pod] {claims, window node or SP_NONE, first claim, owner rank or SP_NONE}
+    uint32_t* w;                                  // [SP_WORDS] call words
+    Err err;
+};
+
+// OutRec slots of one claim of a pod (spec §1/§3): `count` for a well-formed GPU claim naming a node of the inventory, else 1
+__device__ __forceinline__ uint32_t pod_claim_slots(const uint4 c, uint32_t n_node, bool have_off) {
+    const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
+    return (kind == DRA_KIND_GPU && c.y < n_node && !claim_invalid(kind, prof, count, have_off)) ? count : 1u;
+}
+
+// thread per pod, every pod: the checks of k_pod_records plus the device-side ones (pod_off monotone and spanning
+// [0, n_claim]) — those set SP_BAD instead of failing one pod, since every rank sees the same arrays
+__global__ void __launch_bounds__(256)
+k_spod_records(const SPodArgs a) {
+    __shared__ uint32_t rs_s[PEER_MAX];
+    const uint32_t tid = threadIdx.x, p = blockIdx.x * blockDim.x + tid;
+    if (tid < PEER_MAX) rs_s[tid] = 0;
+    __syncthreads();
+    if (p < a.n_pod) {
+        const uint32_t c0 = __ldg(&a.pod_off[p]), c1 = __ldg(&a.pod_off[p + 1]);
+        uint4 rec = make_uint4(c1 - c0, SP_NONE, c0, SP_NONE);
+        bool fault = p == 0 && (c0 != 0 || __ldg(&a.pod_off[a.n_pod]) != a.n_claim);
+        if (c1 < c0 || c1 > a.n_claim) fault = true;
+        else if (c1 > c0) {
+            const bool have_off = a.out_off != nullptr;
+            const uint32_t node = __ldg(&a.claims[c0]).y;
+            bool bad = c1 - c0 > DRA_MAX_POD || node >= a.n_node;
+            uint32_t total = 0;
+            for (uint32_t i = c0; i < c1; ++i) {
+                const uint4 c = __ldg(&a.claims[i]);
+                bad = bad || c.y != node;
+                const uint32_t slots = pod_claim_slots(c, a.n_node, have_off);
+                const uint32_t dst = have_off ? __ldg(&a.out_off[i]) : i;
+                fault = fault || dst > a.n_out || slots > a.n_out - dst;
+                total += slots;
+            }
+            const bool stray = node >= a.n_node;
+            const bool mine = stray ? a.take_stray != 0 : (node >= a.node_lo && node < a.node_hi);
+            if (!fault) {
+                if (a.world > 1) {
+                    uint32_t o = a.stray_rank;
+                    if (!stray) { o = 0; for (uint32_t q = 0; q + 1 < a.world; ++q) o += node >= a.rank_hi[q] ? 1u : 0u; }
+                    atomicAdd(&rs_s[o], total);
+                }
+                if (mine) {
+                    rec.w = a.rank;
+                    if (!bad) rec.y = node - a.node_lo;
+                    else for (uint32_t i = c0; i < c1; ++i) {
+                        const uint4 c = __ldg(&a.claims[i]);
+                        const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu;
+                        const uint32_t op = kind == DRA_KIND_GPU ? DRA_PROFILE_GPU : kind == DRA_KIND_SHARED ? DRA_PROFILE_SHARED : prof;
+                        const uint32_t slots = pod_claim_slots(c, a.n_node, have_off);
+                        const uint32_t dst = have_off ? __ldg(&a.out_off[i]) : i;
+                        for (uint32_t k = 0; k < slots; ++k) a.table[dst + k] = make_uint2(DRA_GPU_NONE, meta(0, 0, op, DRA_ST_INVALID));
+                    }
+                }
+            }
+        }
+        if (fault) { a.w[SP_BAD] = 1u; a.err.set(ERR_BAD_PODS); }
+        a.podrec[p] = rec;
+    }
+    __syncthreads();
+    if (a.world > 1 && tid < a.world && rs_s[tid]) atomicAdd(&a.w[tid], rs_s[tid]);
+}
+
+// After the records, before the sort: decides whether the call goes ahead (no fault, and every rank's packets fit the
+// staging slices: cap), publishes the sort's record count and the gather's expected counts, and — DRA_F_FRESH_INVENTORY
+// (inv_src = the pristine copy) — copies this rank's GPUs from the pristine copy to the live one, so that k_pods reads and
+// writes the live copy alone.  A gated call changes no inventory.  Every block decides alike; block 0 publishes.
+__global__ void __launch_bounds__(256)
+k_spod_gate(const SPodArgs a, uint32_t cap, const uint4* __restrict__ inv_src, uint4* __restrict__ inv_dst,
+            const uint32_t* __restrict__ node_off) {
+    const uint32_t tid = threadIdx.x;
+    const bool over = a.world > 1 && tid < a.world && __ldcg(&a.w[tid]) > cap;
+    const bool gated = __syncthreads_or(over || __ldcg(&a.w[SP_BAD]) != 0) != 0;
+    if (blockIdx.x == 0) {
+        if (tid < PEER_MAX) a.w[SP_EXPECT + tid] = gated ? 1u : max(__ldcg(&a.w[tid]), 1u);
+        if (tid == 0) { a.w[SP_NDEV] = gated ? 0u : a.n_pod; a.w[SP_GATED] = gated ? 1u : 0u; }
+        if (over) a.err.set(ERR_BAD_PODS);
+    }
+    if (gated || !inv_src) return;
+    const uint32_t g1 = __ldg(&node_off[a.node_hi]);
+    for (uint32_t i = __ldg(&node_off[a.node_lo]) + blockIdx.x * blockDim.x + tid; i < g1; i += gridDim.x * blockDim.x)
+        inv_dst[i] = __ldg(&inv_src[i]);
+}
+
+// The all-gather of the owned pods' records, with the packets of k_pkt_gather (global slots, expected counts known from
+// k_spod_records, so no header).  Thread per pod; a pod's slots need not be contiguous, the slot rides in the packet.
+// A rank with nothing to send — it owns no slot, or the call is gated — sends one packet addressed to the table's padding
+// slot pad_slot instead (k_spod_gate expects it): each call is then a real exchange with every peer, so no rank gets two
+// calls ahead of a peer still reading the staging slices of the same parity.
+__global__ void __launch_bounds__(256)
+k_spod_gather(const PktGather g, const SPodArgs a, uint32_t pad_slot) {
+    const uint32_t T = blockIdx.x * blockDim.x + threadIdx.x, NT = gridDim.x * blockDim.x, lane = threadIdx.x & 31;
+    if (blockIdx.x == 0 && threadIdx.x == 32) g.cursor[g.parity ^ 1u] = 0;
+    const bool gated = __ldcg(&a.w[SP_GATED]) != 0;
+    if (T == 0 && (gated || __ldcg(&a.w[g.rank]) == 0)) pkt_send(g, atomicAdd(&g.cursor[g.parity], 1u), make_uint2(0u, 0u), pad_slot);
+    const uint32_t n_pod = gated ? 0u : a.n_pod;
+    const bool have_off = a.out_off != nullptr;
+    for (uint32_t p0 = blockIdx.x * blockDim.x; p0 < n_pod; p0 += NT) {
+        const uint32_t p = p0 + threadIdx.x;
+        uint4 rec = make_uint4(0u, SP_NONE, 0u, SP_NONE);
+        if (p < n_pod) rec = __ldcg(&a.podrec[p]);
+        const bool mine = rec.w == g.rank;
+        uint32_t sl = 0;
+        if (mine) for (uint32_t i = rec.z; i < rec.z + rec.x; ++i) sl += pod_claim_slots(__ldg(&a.claims[i]), a.n_node, have_off);
+        // one reservation per warp
+        uint32_t incl = sl;
+        #pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(FULLMASK, incl, d); if (lane >= (uint32_t)d) incl += y; }
+        const uint32_t tot = __shfl_sync(FULLMASK, incl, 31);
+        uint32_t base = 0;
+        if (lane == 0 && tot) base = atomicAdd(&g.cursor[g.parity], tot);
+        uint32_t pos = __shfl_sync(FULLMASK, base, 0) + incl - sl;
+        if (!mine) continue;
+        for (uint32_t i = rec.z; i < rec.z + rec.x; ++i) {
+            const uint32_t s = pod_claim_slots(__ldg(&a.claims[i]), a.n_node, have_off);
+            const uint32_t dst = have_off ? __ldg(&a.out_off[i]) : i;
+            for (uint32_t k = 0; k < s; ++k, ++pos)
+                if (pos < g.cap) pkt_send(g, pos, __ldcg(&g.table[dst + k]), dst + k);
+        }
+    }
+    pkt_receive(g, T, NT, a.err);
 }
 
 // ====================================================================================================
