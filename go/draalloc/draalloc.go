@@ -310,6 +310,21 @@ func (c *Context) AllocatePodsGlobal(pinnedClaims unsafe.Pointer, nClaim int, pi
 	return nil
 }
 
+// ShardSyncInventory makes every context's live inventory the world's state (dra_shard_sync_inventory_device): each GPU's
+// record as the context owning its node holds it.  Afterwards dra_get_inventory on any context returns the whole world,
+// and SetShardMap may move node ranges without losing allocations.  Every context must make the call; needs SetShardMap
+// and ShardExport after SetInventory, then PeerImportLocal.  One process: call it on EVERY context before SetShardMap or
+// dra_get_inventory on any, since both wait for the context's stream.  Returns at once; Sync reports completion and errors found
+// on the device.  Unbuilt, like the rest of this file.
+func (c *Context) ShardSyncInventory() error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	if rc := C.dra_shard_sync_inventory_device(c.h); rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
 // Sync waits for the calls enqueued on the context and reports the errors they found on the device (dra_ctx_sync).
 func (c *Context) Sync() error {
 	c.mu.Lock()

@@ -288,7 +288,9 @@ int  dra_gather_read(dra_ctx* ctx, dra_out_rec* out_all, uint32_t n_rec);
  *   dra_peer_export(ctx, n_per_rank, handle)   allocates this rank's gather buffer, returns its 64-byte
  *                                              cudaIpcMemHandle_t;  the host runtime all-gathers the handles;
  *   dra_peer_import(ctx, handles)              world * 64 bytes, in rank order.
- * Requires all ranks on one node with P2P access; on failure the NCCL path stays in use.
+ * Requires all ranks on one node with P2P access; on failure the NCCL path stays in use.  Every rank must export alike (the
+ * same sizes, dra_set_shard_pairs and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
+ * own layout, so dra_peer_import / dra_peer_import_local refuse a peer set up differently with DRA_E_INVAL.
  * dra_peer_export(ctx, 0, NULL) switches the peer path off again. */
 int  dra_peer_export(dra_ctx* ctx, uint32_t n_per_rank, void* handle64);
 int  dra_peer_import(dra_ctx* ctx, const void* handles);
@@ -324,7 +326,7 @@ int  dra_peer_rendezvous_device(dra_ctx* ctx);
  * out_off must tile [0, n_out) (slots no claim owns keep their previous contents).  flags: DRA_F_FRESH_INVENTORY.
  * With world == 1 no export is needed (the table is local).  A rank's live inventory is authoritative for its own
  * node range only (UnsuitableNodes and pods Allocate on such a world: dra_unsuitable_batch_global_device and
- * dra_allocate_pods_batch_global_device below).  d_claims may also be a pinned host buffer (dra_host_alloc): the compaction kernel reads every claim
+ * dra_allocate_pods_batch_global_device below; the whole world's state on every rank: dra_shard_sync_inventory_device).  d_claims may also be a pinned host buffer (dra_host_alloc): the compaction kernel reads every claim
  * exactly once, so it then ingests the batch over PCIe itself — no copy-engine transfer in front of the call. */
 int  dra_set_shard(dra_ctx* ctx, uint32_t node_lo, uint32_t node_hi, int take_stray);
 /* The whole partition: rank r serves nodes [bounds[r], bounds[r+1]) (bounds has world+1 entries, bounds[world] = n_node),
@@ -373,6 +375,20 @@ int  dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cla
 int  dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
                                            const uint32_t* d_pod_off, uint32_t n_pod,
                                            const uint32_t* d_out_off, uint32_t n_out, uint32_t flags);
+
+/* Every rank's live inventory becomes the world's state: for each GPU, the record its owning rank holds (the rank whose
+ * node range contains the GPU's node, per the current dra_set_shard_map).  Own range untouched, pristine copy untouched.
+ * Afterwards dra_get_inventory on any rank returns the whole world, and dra_set_shard_map may move node ranges between
+ * ranks without losing allocations.  Every rank must make the call; enqueues on ctx's stream and returns; completion and
+ * device-detected errors surface at dra_ctx_sync (a peer that never arrives within DRA_PEER_TIMEOUT_MS: DRA_E_NCCL, and
+ * no record was copied).  world == 1: DRA_OK, nothing enqueued.
+ * Prerequisites, each DRA_E_STATE with nothing enqueued: world > 1 needs dra_set_shard_map (a bare dra_set_shard is
+ * refused); dra_shard_export, then dra_peer_import or dra_peer_import_local; the inventory loaded BEFORE the export (which
+ * reserves n_gpu x 16 bytes of staging per call parity) and not grown since.
+ * One process driving several ranks: dra_set_shard_map and dra_get_inventory synchronise the context's stream, so enqueue
+ * the sync on EVERY rank before calling either on any rank; otherwise that rank's stream waits for peers whose call the
+ * blocked thread has not made yet, and the sync times out. */
+int dra_shard_sync_inventory_device(dra_ctx* ctx);
 
 /* ---- adjacent integer searches of the reference, batched (API completeness; SURVEY §8f-4) -------------- */
 

@@ -72,6 +72,7 @@ SYMBOLS = {
     "dra_set_shard_pairs": (_i32, [_vp, _u32]),
     "dra_unsuitable_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _u32]),
     "dra_allocate_pods_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _u32, _u32]),
+    "dra_shard_sync_inventory_device": (_i32, [_vp]),
     "dra_mps_limits_batch": (_i32, [_vp, _vp, _u32, _vp, _vp]),
     "dra_imex_offsets_batch": (_i32, [_vp, _vp, _vp, _u32, C.c_int32, C.c_int32, _vp]),
     "dra_calibrate": (_i32, [_vp, C.POINTER(_u32)]),
@@ -389,6 +390,13 @@ class Context:
         F_FRESH_INVENTORY.  Enqueues, no synchronisation; errors found on the device surface at sync()."""
         self._check(self._lib.dra_allocate_pods_batch_global_device(self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod,
                                                                     _ptr(d_out_off), n_out, flags))
+
+    def shard_sync_inventory_device(self) -> None:
+        """Every rank's live inventory becomes the world's state (each GPU as its owning rank holds it), so get_inventory()
+        returns the whole world and set_shard_map() may move ranges without losing allocations.  Every rank must call it;
+        one process: enqueue it on every rank before get_inventory() / set_shard_map() on any.  Enqueues, no
+        synchronisation; errors found on the device surface at sync()."""
+        self._check(self._lib.dra_shard_sync_inventory_device(self._h))
 
     def peer_import(self, handles) -> None:
         blob = b"".join(handles)

@@ -176,6 +176,10 @@ struct dra_ctx {
     uint32_t* d_upair_pod = nullptr; size_t cap_upair_pod = 0;   // candidate form: pair -> pod (k_uns_prep)
     // sharded pods Allocate
     uint32_t* d_spod = nullptr;                 // [SP_WORDS] call words (dra_device.cuh SPodArgs)
+    // inventory sync: records in the peer buffer ([staging x2: peer_inv_gpus records][flags[PEER_MAX], elect[2]])
+    uint32_t peer_inv_gpus = 0, isync_seq = 0;  // peer_inv_gpus: n_gpu when the export ran (0: no inventory then)
+    size_t off_istage[2] = {0, 0}, off_iflags = 0;
+    std::vector<uint32_t> h_node_off;           // host copy of the inventory's node_off: each rank's GPU range
     // Buffers a sharded call outgrew while peers on this device may be waiting for it: cudaFree would wait for the whole
     // device, so they are freed at the next dra_ctx_sync instead (grow / grow_nc while defer_free is set).
     bool defer_free = false;
@@ -920,6 +924,7 @@ int dra_set_inventory(dra_ctx* ctx, const dra_gpu_rec* gpus, uint32_t n_gpu, con
     if (n_gpu) CU(cudaMemcpy(ctx->d_inv_pristine, gpus, (size_t)n_gpu * 16, cudaMemcpyHostToDevice));
     if (n_gpu) CU(cudaMemcpy(ctx->d_inv_live, gpus, (size_t)n_gpu * 16, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(ctx->d_node_off, node_off, ((size_t)n_node + 1) * 4, cudaMemcpyHostToDevice));
+    ctx->h_node_off.assign(node_off, node_off + n_node + 1);
     ctx->n_gpu = n_gpu; ctx->n_node = n_node;
     ctx->state_epoch++;
     ctx->max_width = 0;
@@ -1356,8 +1361,22 @@ int dra_comm_init(dra_ctx* ctx, const void* id128, int rank, int world) {
 
 namespace {
 
-// (Re)allocates this rank's gather buffer:  [table x2][staging x2: world slices of cap packets][headers x2][rendezvous flags]
+// What a peer buffer's layout depends on.  Every rank computes its peers' offsets from its OWN layout, so an import requires
+// every rank to be set up alike; the export writes this at offset 0 of the buffer for importers in other processes to read.
+struct PeerLayout {
+    uint32_t world, rank, form, cap, tab_len, uns_pairs, inv_gpus, rsvd;
+    bool operator==(const PeerLayout& o) const { return memcmp(this, &o, sizeof o) == 0; }
+};
+PeerLayout layout_of(const dra_ctx* c, int rank) {
+    PeerLayout l; memset(&l, 0, sizeof l);
+    l.world = (uint32_t)c->world; l.rank = (uint32_t)rank; l.form = c->peer_form; l.cap = c->peer_cap; l.tab_len = c->peer_tab_len;
+    l.uns_pairs = c->peer_uns_pairs; l.inv_gpus = c->peer_inv_gpus;
+    return l;
+}
+
+// (Re)allocates this rank's gather buffer:  [layout][table x2][staging x2: world slices of cap packets][headers x2][rendezvous flags]
 // and, after dra_set_shard_pairs(max_pairs > 0), [UnsuitableNodes staging x2: world slices of uns_stride words][their flags]
+// and, for dra_shard_export with an inventory loaded, [inventory staging x2: n_gpu records][their flags + election words]
 int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, uint32_t cap) {
     if (ctx->world > (int)PEER_MAX) return fail(ctx, DRA_E_INVAL, "world %d > %u", ctx->world, PEER_MAX);
     CU(cudaSetDevice(ctx->device));
@@ -1370,6 +1389,7 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
     if (ctx->peer_local) { CU(cudaFree(ctx->peer_local)); ctx->peer_local = nullptr; }
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
+    take(sizeof(PeerLayout));                                                      // offset 0, whatever the sizes
     for (int p = 0; p < 2; ++p) ctx->off_table[p] = take((size_t)tab_len * 8 + 16);
     for (int p = 0; p < 2; ++p) ctx->off_stage[p] = take((size_t)ctx->world * cap * 16);
     for (int p = 0; p < 2; ++p) ctx->off_hdr[p] = take((size_t)ctx->world * 16);
@@ -1386,12 +1406,21 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
         if ((rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, ctx->uns_max_pairs))) return rc;
     }
     ctx->uns_seq = 0;
+    // the inventory sync's staging, sized for the inventory loaded now (sharded form only)
+    ctx->peer_inv_gpus = form == 2 && ctx->d_inv_live ? ctx->n_gpu : 0u;
+    if (ctx->peer_inv_gpus) {
+        for (int p = 0; p < 2; ++p) ctx->off_istage[p] = take((size_t)ctx->peer_inv_gpus * 16);
+        ctx->off_iflags = take((size_t)(PEER_MAX + 2) * 4);
+    }
+    ctx->isync_seq = 0;
     ctx->peer_bytes = off;
     CU(cudaMalloc((void**)&ctx->peer_local, ctx->peer_bytes));
     CU(cudaMemset(ctx->peer_local, 0, ctx->peer_bytes));
     if (!ctx->d_cursor) CU(cudaMalloc((void**)&ctx->d_cursor, 64));
     CU(cudaMemset(ctx->d_cursor, 0, 64));
     ctx->peer_form = form; ctx->peer_n_per = n_per; ctx->peer_tab_len = tab_len; ctx->peer_cap = cap; ctx->peer_epoch = 0;
+    const PeerLayout mine = layout_of(ctx, ctx->rank);
+    CU(cudaMemcpy(ctx->peer_local, &mine, sizeof mine, cudaMemcpyHostToDevice));
     if (const char* e = getenv("DRA_PEER_TIMEOUT_MS")) ctx->peer_spin = std::max(1ll, atoll(e)) * 1900000ll;
     ctx->gather_table = nullptr;
     ctx->state_epoch++;
@@ -1463,6 +1492,10 @@ int dra_peer_import(dra_ctx* ctx, const void* handles) {
         cudaError_t e = cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess);
         if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(ctx, DRA_E_CUDA, "cudaIpcOpenMemHandle(rank %d): %s", r, cudaGetErrorString(e)); }
         ctx->peer_base[r] = (uint8_t*)p; ctx->peer_ipc[r] = true;
+        // a peer laid out differently would take this rank's stores at offsets past its regions: refuse it here
+        PeerLayout theirs;
+        CU(cudaMemcpy(&theirs, p, sizeof theirs, cudaMemcpyDeviceToHost));
+        if (!(theirs == layout_of(ctx, r))) return fail(ctx, DRA_E_INVAL, "dra_peer_import: rank %d is not set up like this one", r);
     }
     ctx->peer_ready = true;
     return DRA_OK;
@@ -1474,8 +1507,7 @@ int dra_peer_import_local(dra_ctx* ctx, dra_ctx* const* ctxs) {
     CU(cudaSetDevice(ctx->device));
     for (int r = 0; r < ctx->world; ++r) {
         dra_ctx* o = ctxs[r];
-        if (!o || !o->peer_local || o->world != ctx->world || o->rank != r || o->peer_form != ctx->peer_form ||
-            o->peer_cap != ctx->peer_cap || o->peer_tab_len != ctx->peer_tab_len || o->peer_uns_pairs != ctx->peer_uns_pairs)
+        if (!o || !o->peer_local || o->rank != r || !(layout_of(o, r) == layout_of(ctx, r)))
             return fail(ctx, DRA_E_INVAL, "dra_peer_import_local: context %d is not set up like this one", r);
         if (o->device != ctx->device) {
             int ok = 0; CU(cudaDeviceCanAccessPeer(&ok, ctx->device, o->device));
@@ -1871,6 +1903,41 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded pods Allocate launch: %s", cudaGetErrorString(e));
     ctx->gather_table = (const dra_out_rec*)table; ctx->gather_n_per = n_out; ctx->gather_len = n_out;
+    return DRA_OK;
+}
+
+// Inventory sync: this rank's GPU range into every peer's staging (k_isync_push) -> flags, wait, and the copy of every other
+// rank's range into the live copy (k_isync_copy).  Enqueues only.
+int dra_shard_sync_inventory_device(dra_ctx* ctx) {
+    if (!ctx) return DRA_E_INVAL;
+    QUIESCE();
+    if (ctx->world <= 1) return DRA_OK;
+    if (!ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the sync needs every rank's range)");
+    if (!(ctx->peer_ready && ctx->peer_form == 2)) return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
+    if (!ctx->peer_inv_gpus) return fail(ctx, DRA_E_STATE, "the inventory was not loaded before dra_shard_export: the export reserved no staging for it");
+    if (ctx->n_gpu > ctx->peer_inv_gpus)
+        return fail(ctx, DRA_E_STATE, "the inventory grew to %u GPUs after dra_shard_export reserved staging for %u", ctx->n_gpu, ctx->peer_inv_gpus);
+    if (ctx->shard_bounds[ctx->world] != ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard map does not span the inventory's %u nodes", ctx->n_node);
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t seq = ++ctx->isync_seq, par = seq & 1u;
+    InvSync x; memset(&x, 0, sizeof x);
+    for (int r = 0; r < ctx->world; ++r) {
+        x.stage[r] = (uint4*)(ctx->peer_base[r] + ctx->off_istage[par]);
+        x.flag[r] = (uint32_t*)(ctx->peer_base[r] + ctx->off_iflags) + ctx->rank;
+    }
+    x.my_stage = (const uint4*)(ctx->peer_local + ctx->off_istage[par]);
+    x.my_flags = (const uint32_t*)(ctx->peer_local + ctx->off_iflags);
+    x.elect = (uint32_t*)(ctx->peer_local + ctx->off_iflags) + PEER_MAX;
+    x.inv = ctx->d_inv_live; x.n_gpu = ctx->n_gpu;
+    x.own_lo = ctx->h_node_off[ctx->shard_bounds[ctx->rank]]; x.own_hi = ctx->h_node_off[ctx->shard_bounds[ctx->rank + 1]];
+    x.world = (uint32_t)ctx->world; x.rank = (uint32_t)ctx->rank; x.seq = seq; x.spin_limit = ctx->peer_spin; x.err = err_of(ctx);
+    const uint32_t n_own = x.own_hi - x.own_lo;
+    k_isync_push<<<std::max(1u, std::min((n_own + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, ctx->stream>>>(x);
+    // a small grid: it waits for its peers, and ranks sharing one device must not find their push's SMs held by it
+    k_isync_copy<<<std::max(1u, std::min((ctx->n_gpu + 255) / 256, (uint32_t)std::max(1, ctx->n_sm / 4))), 256, 0, ctx->stream>>>(x);
+    ctx->launches += 2;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "inventory sync launch: %s", cudaGetErrorString(e));
     return DRA_OK;
 }
 

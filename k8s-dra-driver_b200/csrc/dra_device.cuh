@@ -2817,6 +2817,77 @@ k_uns_merge(const UnsExchange x) {
     }
 }
 
+// The inventory sync (dra_shard_sync_inventory_device): every rank's GPU records of its own range to every peer, so that
+// every live copy becomes the world's state.  The same exchange as UnsuitableNodes': plain copies, one fence, one flag.
+// Owned ranges are disjoint, so every rank writes its records at their GLOBAL indices into one staging area per peer.
+//   k_isync_push  this rank's GPUs [own_lo, own_hi) of the live copy into every peer's staging (parity applied), 16-byte
+//                 stores, then a system-scope fence per thread.  Nothing waits here.
+//   k_isync_copy  a grid of at most SMs / 4 CTAs.  The first CTA to arrive (one atomicMax on `elect`) raises this rank's flag at
+//                 every peer to the call's sequence number, waits for every peer's flag here (bounded: ERR_PEER_TIMEOUT,
+//                 never a hang) and publishes ONE verdict for the call in `verdict`; the other CTAs wait for that verdict
+//                 (locally) and all of them copy GPUs outside [own_lo, own_hi) from staging into the live copy only when
+//                 every peer arrived.  One verdict makes it all or nothing: a timed-out call leaves the live copy as it was.
+//                 The elected CTA started before any CTA waiting for it, so those wait at most twice the spin limit.
+// Staging is double-buffered by call parity: a rank is never two calls ahead, since its next copy kernel waits for this
+// rank's next flag, which this rank raises only after its copy of the call before.
+struct InvSync {
+    uint4* stage[PEER_MAX];       // stage[p]: peer p's staging area (parity applied), indexed by global GPU
+    uint32_t* flag[PEER_MAX];     // flag[p]: this rank's flag word at peer p
+    const uint4* my_stage;        // this rank's staging area (parity applied)
+    const uint32_t* my_flags;     // [PEER_MAX], indexed by sender
+    uint4* inv;                   // the live copy
+    uint32_t* elect;              // [0] the last call whose CTA was elected, [1] that call's verdict: seq << 1 | all arrived
+    uint32_t n_gpu, own_lo, own_hi, world, rank, seq;
+    long long spin_limit;
+    Err err;
+};
+
+__global__ void __launch_bounds__(256)
+k_isync_push(const InvSync x) {
+    for (uint32_t i = x.own_lo + blockIdx.x * blockDim.x + threadIdx.x; i < x.own_hi; i += gridDim.x * blockDim.x) {
+        const uint4 v = x.inv[i];
+        for (uint32_t p = 0; p < x.world; ++p)
+            if (p != x.rank) x.stage[p][i] = v;
+    }
+    __threadfence_system();
+}
+
+__global__ void __launch_bounds__(256)
+k_isync_copy(const InvSync x) {
+    __shared__ uint32_t s_lead, s_ok;
+    const uint32_t tid = threadIdx.x;
+    if (tid == 0) { s_lead = atomicMax(&x.elect[0], x.seq) < x.seq; s_ok = 1u; }
+    __syncthreads();
+    const long long t0 = clock64();
+    if (s_lead) {
+        if (tid < x.world && tid != x.rank) {
+            __threadfence_system();
+            asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(x.flag[tid]), "r"(x.seq) : "memory");
+            uint32_t v;
+            do {
+                asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(x.my_flags + tid) : "memory");
+                if ((int32_t)(v - x.seq) >= 0) break;
+                if (clock64() - t0 > x.spin_limit) { x.err.set(ERR_PEER_TIMEOUT); s_ok = 0u; break; }
+            } while (true);
+        }
+        __syncthreads();
+        if (tid == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(x.elect + 1), "r"(x.seq << 1 | s_ok) : "memory");
+    } else {
+        if (tid == 0) {
+            uint32_t v;
+            do {
+                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(x.elect + 1) : "memory");
+                if ((v >> 1) == (x.seq & 0x7FFFFFFFu)) { s_ok = v & 1u; break; }
+                if (clock64() - t0 > 2 * x.spin_limit) { x.err.set(ERR_PEER_TIMEOUT); s_ok = 0u; break; }
+            } while (true);
+        }
+        __syncthreads();
+    }
+    if (!s_ok) return;
+    for (uint32_t i = blockIdx.x * blockDim.x + tid; i < x.n_gpu; i += gridDim.x * blockDim.x)
+        if (i < x.own_lo || i >= x.own_hi) x.inv[i] = __ldcg(&x.my_stage[i]);
+}
+
 // ====================================================================================================
 // Deallocate: thread per claim, atomics on the GpuRec words (updates commute, spec §9)
 // ====================================================================================================
