@@ -310,6 +310,24 @@ func (c *Context) AllocatePodsGlobal(pinnedClaims unsafe.Pointer, nClaim int, pi
 	return nil
 }
 
+// DeallocateGlobal: Deallocate on a sharded world (dra_deallocate_batch_global_device), the step after AllocatePodsGlobal.
+// The same claims, out_off and OutRecs on every context, in dra_host_alloc'ed (pinned) memory (pinnedOutOff may be nil);
+// each context applies the OK records whose GPU lies in its own range and writes no other GPU.  Needs SetShardMap (or
+// SetShard) after SetInventory, and no export, import or peer.  A slot range outside nOut fails the call at Sync on every
+// context with no inventory changed.  Returns at once; Sync reports completion and errors found on the device.  Unbuilt,
+// like the rest of this file.
+func (c *Context) DeallocateGlobal(pinnedClaims unsafe.Pointer, nClaim int, pinnedOutOff unsafe.Pointer, pinnedOut unsafe.Pointer,
+	nOut int) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_deallocate_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
+		(*C.uint32_t)(pinnedOutOff), (*C.dra_out_rec)(pinnedOut), C.uint32_t(nOut))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
 // ShardSyncInventory makes every context's live inventory the world's state (dra_shard_sync_inventory_device): each GPU's
 // record as the context owning its node holds it.  Afterwards dra_get_inventory on any context returns the whole world,
 // and SetShardMap may move node ranges without losing allocations.  Every context must make the call; needs SetShardMap

@@ -326,7 +326,8 @@ int  dra_peer_rendezvous_device(dra_ctx* ctx);
  * out_off must tile [0, n_out) (slots no claim owns keep their previous contents).  flags: DRA_F_FRESH_INVENTORY.
  * With world == 1 no export is needed (the table is local).  A rank's live inventory is authoritative for its own
  * node range only (UnsuitableNodes and pods Allocate on such a world: dra_unsuitable_batch_global_device and
- * dra_allocate_pods_batch_global_device below; the whole world's state on every rank: dra_shard_sync_inventory_device).  d_claims may also be a pinned host buffer (dra_host_alloc): the compaction kernel reads every claim
+ * dra_allocate_pods_batch_global_device below; the whole world's state on every rank: dra_shard_sync_inventory_device;
+ * Deallocate: dra_deallocate_batch_global_device).  d_claims may also be a pinned host buffer (dra_host_alloc): the compaction kernel reads every claim
  * exactly once, so it then ingests the batch over PCIe itself — no copy-engine transfer in front of the call. */
 int  dra_set_shard(dra_ctx* ctx, uint32_t node_lo, uint32_t node_hi, int take_stray);
 /* The whole partition: rank r serves nodes [bounds[r], bounds[r+1]) (bounds has world+1 entries, bounds[world] = n_node),
@@ -389,6 +390,25 @@ int  dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_
  * the sync on EVERY rank before calling either on any rank; otherwise that rank's stream waits for peers whose call the
  * blocked thread has not made yet, and the sync times out. */
 int dra_shard_sync_inventory_device(dra_ctx* ctx);
+
+/* Deallocate over a sharded world (spec §9, "Sharded form"): the classic flow's last step.  The SAME claims, out_off and
+ * OutRecs on every rank (device pointers, or dra_host_alloc'ed buffers; d_out may be the table dra_gather_table returns).
+ * slots(c) is counted as by dra_deallocate_batch, on the whole inventory's node indices.  A rank applies only the OK slots
+ * whose gpu lies in its own GPU range [node_off[node_lo], node_off[node_hi]) of dra_set_shard / dra_set_shard_map, and
+ * writes no other GPU record (the pristine copy neither).  When every rank makes the call, every rank's own range ends as
+ * dra_deallocate_batch would leave the world's state; dra_shard_sync_inventory_device then gives every rank that state.
+ * Do NOT run dra_deallocate_batch on every rank with gathered records instead: it writes every GPU the records name, and a
+ * SHARED slot on another rank's GPU wraps that copy's share count.
+ * All or nothing: every claim's slot range [base, base + slots) is checked on the device before any record is applied; one
+ * outside [0, n_out) gives DRA_E_INVAL at dra_ctx_sync on every rank, with no inventory word changed.
+ * No exchange: no dra_shard_export or peer import is needed, the call waits for no peer, and it allocates nothing.  World 1
+ * with dra_set_shard(0, n_node, 1) makes it a device-side, all-or-nothing dra_deallocate_batch of the whole inventory.
+ * Prerequisites, each DRA_E_STATE with nothing enqueued: dra_set_inventory, and a shard (dra_set_shard or
+ * dra_set_shard_map).  DRA_E_INVAL with nothing enqueued: NULL d_claims or d_out with n_claim > 0, n_out < n_claim
+ * without out_off, n_claim or n_out above 2^26.  n_claim == 0: DRA_OK, nothing enqueued.  Otherwise two kernels are
+ * enqueued on ctx's stream and the call returns; completion surfaces at dra_ctx_sync. */
+int dra_deallocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                       const uint32_t* d_out_off, const dra_out_rec* d_out, uint32_t n_out);
 
 /* ---- adjacent integer searches of the reference, batched (API completeness; SURVEY §8f-4) -------------- */
 

@@ -73,6 +73,7 @@ SYMBOLS = {
     "dra_unsuitable_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _u32]),
     "dra_allocate_pods_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _u32, _u32]),
     "dra_shard_sync_inventory_device": (_i32, [_vp]),
+    "dra_deallocate_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_mps_limits_batch": (_i32, [_vp, _vp, _u32, _vp, _vp]),
     "dra_imex_offsets_batch": (_i32, [_vp, _vp, _vp, _u32, C.c_int32, C.c_int32, _vp]),
     "dra_calibrate": (_i32, [_vp, C.POINTER(_u32)]),
@@ -397,6 +398,14 @@ class Context:
         one process: enqueue it on every rank before get_inventory() / set_shard_map() on any.  Enqueues, no
         synchronisation; errors found on the device surface at sync()."""
         self._check(self._lib.dra_shard_sync_inventory_device(self._h))
+
+    def deallocate_global_device(self, d_claims: int, n_claim: int, d_out_off: int | None, d_out: int, n_out: int) -> None:
+        """Sharded Deallocate (spec §9): the SAME claims, out_off and OutRecs on every rank (device pointers or PinnedBuffer
+        addresses; d_out may be the gathered table).  This rank applies the OK records on its own GPU range and writes no
+        other GPU.  A slot range outside n_out fails the call at sync() with no inventory changed.  Needs no export or
+        import and waits for no peer.  Enqueues, no synchronisation."""
+        self._check(self._lib.dra_deallocate_batch_global_device(self._h, _ptr(d_claims), n_claim, _ptr(d_out_off), _ptr(d_out),
+                                                                 n_out))
 
     def peer_import(self, handles) -> None:
         blob = b"".join(handles)

@@ -650,7 +650,8 @@ int collect_timings(dra_ctx* ctx, int n_marks) {
 int check_err(dra_ctx* ctx) {
     uint32_t oor = ctx->h_err[ERR_OUT_RANGE], ns = ctx->h_err[ERR_NOT_SORTED], pt = ctx->h_err[ERR_PEER_TIMEOUT], sp = ctx->h_err[ERR_SHARD_PLAN];
     const uint32_t dw = ctx->h_err[ERR_DEVICE_WAIT], bo = ctx->h_err[ERR_BAD_OFFSETS], bp = ctx->h_err[ERR_BAD_PODS];
-    if (!oor && !ns && !pt && !sp && !dw && !bo && !bp) return DRA_OK;
+    const uint32_t bd = ctx->h_err[ERR_BAD_DEALLOC];
+    if (!oor && !ns && !pt && !sp && !dw && !bo && !bp && !bd) return DRA_OK;
     for (uint32_t i = 0; i < ERR_WORDS; ++i) ctx->h_err[i] = 0;
     cudaMemsetAsync(ctx->d_err, 0, ERR_WORDS * sizeof(uint32_t), ctx->stream);
     cudaStreamSynchronize(ctx->stream);
@@ -659,6 +660,7 @@ int check_err(dra_ctx* ctx) {
     if (bo) return fail(ctx, DRA_E_INVAL, "sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays; nothing was evaluated");
     if (bp) return fail(ctx, DRA_E_INVAL, "sharded pods Allocate: pod_off not monotone or not spanning [0, n_claim], a pod's OutRec slots outside n_out, "
                                           "or one rank's slots beyond the cap_per_rank of dra_shard_export; no inventory was changed");
+    if (bd) return fail(ctx, DRA_E_INVAL, "sharded Deallocate: out_off/n_out: a claim's slots fall outside out[]; no record was applied, inventory unchanged");
     if (pt) return fail(ctx, DRA_E_NCCL, "all-gather: a rank did not deliver its records in time (or aborted its batch)");
     if (ns) return fail(ctx, DRA_E_INVAL, "DRA_F_NODE_SORTED given but claims are not sorted by node; inventory unchanged");
     return fail(ctx, DRA_E_INVAL, "out_off/n_out: a claim's slots fall outside out[]; inventory state is undefined, reset it");
@@ -1321,7 +1323,8 @@ int dra_deallocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     if (ob) CU(cudaMemcpyAsync(ctx->d_out_off, ctx->h_in + cb, ob, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemcpyAsync(ctx->d_out, ctx->h_in + cb + ob, rb, cudaMemcpyHostToDevice, ctx->stream));
     k_dealloc<<<(n_claim + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_claims, n_claim, out_off ? ctx->d_out_off : nullptr,
-                                                             ctx->d_out, n_out, (uint32_t*)ctx->d_inv_live, ctx->n_gpu, ctx->n_node, err_of(ctx));
+                                                             ctx->d_out, n_out, (uint32_t*)ctx->d_inv_live, 0u, ctx->n_gpu, ctx->n_node,
+                                                             nullptr, err_of(ctx));
     ctx->launches += 1;
     CU(cudaStreamSynchronize(ctx->stream));
     cudaError_t e = cudaGetLastError();
@@ -1938,6 +1941,34 @@ int dra_shard_sync_inventory_device(dra_ctx* ctx) {
     ctx->launches += 2;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "inventory sync launch: %s", cudaGetErrorString(e));
+    return DRA_OK;
+}
+
+// Sharded Deallocate: the slot-range check over every claim (k_dealloc_check) -> the gated apply on this rank's GPU range
+// (k_dealloc, a programmatic dependent of the check).  Spec §9 updates commute and touch only the GPU a record names, so no
+// rank exchanges anything and none waits for a peer.  Enqueues only; allocates nothing.
+int dra_deallocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                       const uint32_t* d_out_off, const dra_out_rec* d_out, uint32_t n_out) {
+    if (!ctx || (n_claim && (!d_claims || !d_out))) return DRA_E_INVAL;
+    QUIESCE();
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
+    if (ctx->shard_hi > ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard [%u, %u) lies outside the inventory's %u nodes", ctx->shard_lo, ctx->shard_hi, ctx->n_node);
+    if (n_claim > (1u << 26) || n_out > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
+    if (!d_out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    if (!n_claim) return DRA_OK;
+    CU(cudaSetDevice(ctx->device));
+    const Err err = err_of(ctx);
+    const uint32_t gpu_lo = ctx->h_node_off[ctx->shard_lo], gpu_hi = ctx->h_node_off[ctx->shard_hi];
+    k_dealloc_check<<<std::max(1u, std::min((n_claim + 255) / 256, (uint32_t)ctx->n_sm * 4u)), 256, 0, ctx->stream>>>(
+        (const uint4*)d_claims, n_claim, d_out_off, n_out, ctx->n_node, err);
+    static const bool no_pdl = getenv("DRA_NO_PDL") != nullptr;
+    CU(launch_k(k_dealloc, dim3((n_claim + 255) / 256), dim3(256), 0, ctx->stream, !no_pdl && !ctx->profiling,
+                (const uint4*)d_claims, n_claim, d_out_off, (const uint2*)d_out, n_out, (uint32_t*)ctx->d_inv_live, gpu_lo, gpu_hi,
+                ctx->n_node, (const uint32_t*)(ctx->d_err + ERR_BAD_DEALLOC), err));
+    ctx->launches += 2;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded Deallocate launch: %s", cudaGetErrorString(e));
     return DRA_OK;
 }
 

@@ -10,7 +10,7 @@
 //                    claim is tested on all GPUs at once, __ballot_sync + __ffs pick lowest GPU / lowest
 //                    start (first-fit), the winner lane updates its register-resident occupancy mask.
 //   k_unsuitable     one warp per (pod, candidate node) pair, same step function on a snapshot
-//   k_dealloc        inverse updates with atomics
+//   k_dealloc        inverse updates with atomics (sharded: behind k_dealloc_check, on the rank's GPU range only)
 //
 // What this replaces in the reference: the per-node search behind Allocate()/UnsuitableNodes() that
 // north_star names (absent from the snapshot, SURVEY F1), over the device model of
@@ -34,7 +34,8 @@ constexpr uint32_t ERR_DEVICE_WAIT = 5u;     // a wait inside ONE GPU gave up (g
 constexpr uint32_t ERR_SHARD_PLAN = 4u;      // sharded call: more claims fell into this shard than the launch was laid out for
 constexpr uint32_t ERR_BAD_OFFSETS = 6u;     // sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays
 constexpr uint32_t ERR_BAD_PODS = 7u;        // sharded pods Allocate: bad pod_off, slots outside n_out, or a rank's slots beyond its packet room
-constexpr uint32_t ERR_WORDS = 8u;
+constexpr uint32_t ERR_BAD_DEALLOC = 8u;     // sharded Deallocate: a claim's slots outside n_out (nothing applied)
+constexpr uint32_t ERR_WORDS = 9u;
 constexpr uint32_t PEER_MAX = 16;         // ranks of one box
 
 // Error flags: `dev` (device memory) gates later kernels of the same batch, `host` (mapped pinned
@@ -2891,23 +2892,50 @@ k_isync_copy(const InvSync x) {
 // ====================================================================================================
 // Deallocate: thread per claim, atomics on the GpuRec words (updates commute, spec §9)
 // ====================================================================================================
+// slots(c) exactly as Allocate counted them (spec §9): an INVALID claim — here: one naming no node — has one
+__device__ __forceinline__ uint32_t dealloc_slots(const uint4 c, uint32_t n_node, bool have_off) {
+    const uint32_t kind = c.x & 0xFFu, count = c.x >> 16;
+    return (kind == DRA_KIND_GPU && c.y < n_node && count >= 1 && count <= DRA_MAX_COUNT && (have_off || count == 1)) ? count : 1u;
+}
+
+// The sharded Deallocate's all-or-nothing check (dra_deallocate_batch_global_device), grid-stride over every claim: a slot
+// range [base, base + slots) outside [0, n_out) sets ERR_BAD_DEALLOC, which gates k_dealloc.  Every rank reads the same
+// arrays, so every rank finds the same fault.
+__global__ void __launch_bounds__(256)
+k_dealloc_check(const uint4* __restrict__ claims, uint32_t n_claim, const uint32_t* __restrict__ out_off, uint32_t n_out,
+                uint32_t n_node, Err err) {
+    pdl_trigger();                                          // k_dealloc may be scheduled now; it waits for this grid
+    const bool have_off = out_off != nullptr;
+    bool bad = false;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_claim; i += gridDim.x * blockDim.x) {
+        const uint32_t base = have_off ? __ldg(&out_off[i]) : i, slots = dealloc_slots(__ldg(&claims[i]), n_node, have_off);
+        bad = bad || base > n_out || slots > n_out - base;
+    }
+    if (bad) err.set(ERR_BAD_DEALLOC);
+}
+
+// GPUs outside [gpu_lo, gpu_hi) are not written (dra_deallocate_batch: [0, n_gpu)).  gate: when set (the sharded call,
+// launched as a programmatic dependent of k_dealloc_check), a non-zero word means the check found a bad slot range and
+// nothing is applied; without it a bad range stops the thread with ERR_OUT_RANGE after others may have applied theirs.
 __global__ void __launch_bounds__(256)
 k_dealloc(const uint4* __restrict__ claims, uint32_t n_claim, const uint32_t* __restrict__ out_off,
-          const uint2* __restrict__ out, uint32_t n_out, uint32_t* __restrict__ inv, uint32_t n_gpu,
-          uint32_t n_node, Err err) {
+          const uint2* __restrict__ out, uint32_t n_out, uint32_t* __restrict__ inv, uint32_t gpu_lo, uint32_t gpu_hi,
+          uint32_t n_node, const uint32_t* gate, Err err) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_claim) return;
     const uint4 c = __ldg(&claims[i]);
-    const uint32_t kind = c.x & 0xFFu, count = c.x >> 16;
+    const uint32_t kind = c.x & 0xFFu;
     const bool have_off = out_off != nullptr;
     const uint32_t base = have_off ? __ldg(&out_off[i]) : i;
-    // slots(c) exactly as Allocate counted them (spec §9): an INVALID claim — here: one naming no node — has one
-    const uint32_t slots = (kind == DRA_KIND_GPU && c.y < n_node && count >= 1 && count <= DRA_MAX_COUNT &&
-                            (have_off || count == 1)) ? count : 1u;
+    const uint32_t slots = dealloc_slots(c, n_node, have_off);
+    if (gate) {
+        pdl_wait();                                         // the check's grid has completed and its gate word is visible
+        if (*(volatile const uint32_t*)gate) return;
+    }
     if (base > n_out || slots > n_out - base) { err.set(ERR_OUT_RANGE); return; }
     for (uint32_t s = 0; s < slots; ++s) {
         const uint2 o = __ldg(&out[base + s]);
-        if ((o.y >> 24) != DRA_ST_OK || o.x >= n_gpu) continue;
+        if ((o.y >> 24) != DRA_ST_OK || o.x < gpu_lo || o.x >= gpu_hi) continue;
         uint32_t* w = inv + (size_t)o.x * 4;
         if (kind == DRA_KIND_GPU) atomicAnd(&w[0], ~((uint32_t)DRA_GPU_FULL_ALLOCATED << 16));
         else if (kind == DRA_KIND_MIG) {
