@@ -63,6 +63,13 @@ std::mutex g_nccl_mu;
 
 }  // namespace
 
+// A peer exchange's region of the peer buffer (dra_device.cuh PeerExchange): [staging x2 by call parity][flag words].
+// slice: the bytes of one sender's slice of the staging (0: every sender writes at global indices, as the sync does).
+struct PeerRegion {
+    size_t stage[2] = {0, 0}, flags = 0, slice = 0;
+    uint32_t seq = 0;             // the exchange's last call
+};
+
 struct dra_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -148,8 +155,8 @@ struct dra_ctx {
     bool peer_ready = false;
     uint32_t peer_form = 0;                     // 1: per-rank slices [world][n_per]   2: global slots [tab_len]
     uint32_t peer_n_per = 0, peer_tab_len = 0, peer_cap = 0, peer_epoch = 0;
-    size_t peer_bytes = 0, off_table[2] = {0, 0}, off_stage[2] = {0, 0}, off_hdr[2] = {0, 0}, off_flags = 0;
-    uint32_t rendezvous_seq = 0;
+    size_t peer_bytes = 0, off_table[2] = {0, 0}, off_stage[2] = {0, 0}, off_hdr[2] = {0, 0};
+    PeerRegion rendezvous_x, uns_x, isync_x;    // the peer exchanges: rendezvous (flags alone), UnsuitableNodes, inventory sync
     uint8_t* peer_local = nullptr;              // this rank's buffer (cudaMalloc, exported by IPC handle)
     uint8_t* peer_base[PEER_MAX] = {};          // every rank's buffer as mapped here
     bool peer_ipc[PEER_MAX] = {};               // mapped with cudaIpcOpenMemHandle (else: same process)
@@ -170,15 +177,13 @@ struct dra_ctx {
     uint32_t* d_ticket = nullptr;
     // sharded UnsuitableNodes: bit exchange in the peer buffer ([staging x2: world slices of uns_stride words][flags])
     uint32_t uns_max_pairs = 0;                 // dra_set_shard_pairs, reserved by the next peer_setup
-    uint32_t peer_uns_pairs = 0, uns_stride = 0, uns_seq = 0;
-    size_t off_ustage[2] = {0, 0}, off_uflags = 0;
+    uint32_t peer_uns_pairs = 0, uns_stride = 0;
     uint32_t* d_ubits = nullptr; size_t cap_ubits = 0;   // this rank's words of the call
     uint32_t* d_upair_pod = nullptr; size_t cap_upair_pod = 0;   // candidate form: pair -> pod (k_uns_prep)
     // sharded pods Allocate
     uint32_t* d_spod = nullptr;                 // [SP_WORDS] call words (dra_device.cuh SPodArgs)
     // inventory sync: records in the peer buffer ([staging x2: peer_inv_gpus records][flags[PEER_MAX], elect[2]])
-    uint32_t peer_inv_gpus = 0, isync_seq = 0;  // peer_inv_gpus: n_gpu when the export ran (0: no inventory then)
-    size_t off_istage[2] = {0, 0}, off_iflags = 0;
+    uint32_t peer_inv_gpus = 0;                 // n_gpu when the export ran (0: no inventory then)
     std::vector<uint32_t> h_node_off;           // host copy of the inventory's node_off: each rank's GPU range
     // Buffers a sharded call outgrew while peers on this device may be waiting for it: cudaFree would wait for the whole
     // device, so they are freed at the next dra_ctx_sync instead (grow / grow_nc while defer_free is set).
@@ -1392,30 +1397,28 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
     if (ctx->peer_local) { CU(cudaFree(ctx->peer_local)); ctx->peer_local = nullptr; }
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) & ~(size_t)255; return o; };
+    auto reserve = [&](PeerRegion& rg, size_t stage_bytes, size_t slice, size_t flag_bytes) {   // stage_bytes 0: no staging
+        if (stage_bytes) for (int p = 0; p < 2; ++p) rg.stage[p] = take(stage_bytes);
+        rg.flags = take(flag_bytes); rg.slice = slice; rg.seq = 0;
+    };
     take(sizeof(PeerLayout));                                                      // offset 0, whatever the sizes
     for (int p = 0; p < 2; ++p) ctx->off_table[p] = take((size_t)tab_len * 8 + 16);
     for (int p = 0; p < 2; ++p) ctx->off_stage[p] = take((size_t)ctx->world * cap * 16);
     for (int p = 0; p < 2; ++p) ctx->off_hdr[p] = take((size_t)ctx->world * 16);
-    ctx->off_flags = take((size_t)PEER_MAX * 4); ctx->rendezvous_seq = 0;
+    reserve(ctx->rendezvous_x, 0, 0, (size_t)PEER_MAX * 4);
     ctx->peer_uns_pairs = ctx->uns_max_pairs;
     ctx->uns_stride = (uint32_t)(((size_t)ctx->uns_max_pairs + 127) / 128 * 4);     // words, whole 16-byte units
     if (ctx->uns_stride) {
-        for (int p = 0; p < 2; ++p) ctx->off_ustage[p] = take((size_t)ctx->world * ctx->uns_stride * 4);
-        ctx->off_uflags = take((size_t)PEER_MAX * 4);
+        reserve(ctx->uns_x, (size_t)ctx->world * ctx->uns_stride * 4, (size_t)ctx->uns_stride * 4, (size_t)PEER_MAX * 4);
         // the call's own buffers at full size now: growing one inside the call would cudaFree the old one, which waits for
         // the whole device — where a peer's merge may already be spinning for this rank's push (ranks sharing a device)
         int rc;
         if ((rc = grow(ctx, ctx->d_ubits, ctx->cap_ubits, ctx->uns_stride))) return rc;
         if ((rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, ctx->uns_max_pairs))) return rc;
     }
-    ctx->uns_seq = 0;
-    // the inventory sync's staging, sized for the inventory loaded now (sharded form only)
+    // the inventory sync's staging, sized for the inventory loaded now (sharded form only); its flags, then `elect` [2]
     ctx->peer_inv_gpus = form == 2 && ctx->d_inv_live ? ctx->n_gpu : 0u;
-    if (ctx->peer_inv_gpus) {
-        for (int p = 0; p < 2; ++p) ctx->off_istage[p] = take((size_t)ctx->peer_inv_gpus * 16);
-        ctx->off_iflags = take((size_t)(PEER_MAX + 2) * 4);
-    }
-    ctx->isync_seq = 0;
+    if (ctx->peer_inv_gpus) reserve(ctx->isync_x, (size_t)ctx->peer_inv_gpus * 16, 0, (size_t)(PEER_MAX + 2) * 4);
     ctx->peer_bytes = off;
     CU(cudaMalloc((void**)&ctx->peer_local, ctx->peer_bytes));
     CU(cudaMemset(ctx->peer_local, 0, ctx->peer_bytes));
@@ -1444,6 +1447,47 @@ PktGather make_gather(dra_ctx* ctx, uint32_t epoch, uint32_t slot_base, uint32_t
     g.world = ctx->world; g.rank = ctx->rank; g.cap = ctx->peer_cap; g.epoch = epoch; g.parity = par;
     g.slot_base = slot_base; g.n_per = n_per; g.count = count; g.count_dev = count_dev; g.spin_limit = ctx->peer_spin;
     return g;
+}
+
+// The next call of the exchange whose region is rg
+PeerExchange bind_exchange(dra_ctx* ctx, PeerRegion& rg) {
+    PeerExchange x; memset(&x, 0, sizeof x);
+    x.world = (uint32_t)ctx->world; x.rank = (uint32_t)ctx->rank; x.seq = ++rg.seq; x.spin_limit = ctx->peer_spin; x.err = err_of(ctx);
+    const size_t stage = rg.stage[x.seq & 1u];
+    for (int r = 0; r < ctx->world; ++r) {
+        x.stage[r] = (uint4*)(ctx->peer_base[r] + stage + (size_t)ctx->rank * rg.slice);
+        x.flag[r] = (uint32_t*)(ctx->peer_base[r] + rg.flags) + ctx->rank;
+    }
+    x.my_stage = (const uint4*)(ctx->peer_local + stage);
+    x.my_flags = (const uint32_t*)(ctx->peer_local + rg.flags);
+    return x;
+}
+
+// The result table of a global Allocate call: at world > 1 the table of g, a gather of a new epoch, else this context's own
+int result_table(dra_ctx* ctx, uint32_t n_out, const uint32_t* count_dev, PktGather& g, uint2*& table) {
+    if (ctx->world > 1) {
+        ctx->peer_epoch += 1;
+        g = make_gather(ctx, ctx->peer_epoch, 0, 0, 0, count_dev);
+    } else if ((size_t)n_out + 16 > ctx->cap_gtable) {
+        const size_t ncap = (size_t)n_out + n_out / 4 + 64;
+        if (int rc = grow_nc(ctx, ctx->d_gtable, 0, ncap)) return rc;
+        ctx->cap_gtable = ncap;
+    }
+    table = ctx->world > 1 ? g.table : ctx->d_gtable;
+    return DRA_OK;
+}
+
+// A sharded call at world > 1 needs the sharded form of the peer buffer, exported and imported
+int need_peers(dra_ctx* ctx) {
+    if (ctx->world <= 1 || (ctx->peer_ready && ctx->peer_form == 2)) return DRA_OK;
+    return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
+}
+
+// A sharded call's claims and OutRec slots: at most 2^26 of each, and without out_off one slot per claim at least
+int check_slots(dra_ctx* ctx, uint32_t n_claim, uint32_t n_out, bool have_off) {
+    if (n_claim > (1u << 26) || n_out > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
+    if (!have_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    return DRA_OK;
 }
 
 int launch_gather(dra_ctx* ctx, const PktGather& g, const uint4* d_claims, uint32_t n_claim, const uint32_t* n_dev,
@@ -1531,11 +1575,7 @@ int dra_peer_rendezvous_device(dra_ctx* ctx) {
     if (ctx->world <= 1) return DRA_OK;
     if (!ctx->peer_ready) return fail(ctx, DRA_E_STATE, "dra_peer_import has not been called");
     CU(cudaSetDevice(ctx->device));
-    RendezvousArgs a; memset(&a, 0, sizeof a);
-    for (int r = 0; r < ctx->world; ++r) a.peer_flags[r] = (uint32_t*)(ctx->peer_base[r] + ctx->off_flags);
-    a.my_flags = (const uint32_t*)(ctx->peer_local + ctx->off_flags);
-    a.world = (uint32_t)ctx->world; a.rank = (uint32_t)ctx->rank; a.seq = ++ctx->rendezvous_seq; a.spin_limit = ctx->peer_spin; a.err = err_of(ctx);
-    k_rendezvous<<<1, 32, 0, ctx->stream>>>(a);              // (not counted in dra_launch_count: it is no part of a batch)
+    k_rendezvous<<<1, 32, 0, ctx->stream>>>(bind_exchange(ctx, ctx->rendezvous_x));   // (not counted in dra_launch_count: it is no part of a batch)
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "k_rendezvous: %s", cudaGetErrorString(e));
     return DRA_OK;
@@ -1620,10 +1660,9 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
     QUIESCE();
     if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
     if (flags & ~DRA_F_FRESH_INVENTORY) return fail(ctx, DRA_E_INVAL, "dra_allocate_batch_global_device: unsupported flags 0x%x", flags);
-    if (n_claim > (1u << 26) || n_out > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
-    if (!d_out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    if (int rc = check_slots(ctx, n_claim, n_out, d_out_off != nullptr)) return rc;
     const bool gather = ctx->world > 1;
-    if (gather && !(ctx->peer_ready && ctx->peer_form == 2)) return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
+    if (int rc = need_peers(ctx)) return rc;
     if (gather && n_out > ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", n_out, ctx->peer_tab_len);
     ctx->chain = ctx->chain_tile = 0;
     CU(cudaSetDevice(ctx->device));
@@ -1685,20 +1724,8 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
     if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, ctx->stream)); }
     if (!ctx->d_rank_slots) { CU(cudaMalloc((void**)&ctx->d_rank_slots, 2 * PEER_MAX * 4)); CU(cudaMemsetAsync(ctx->d_rank_slots, 0, 2 * PEER_MAX * 4, ctx->stream)); }
     const bool counted = gather && ctx->shard_map_on;          // every rank counts every rank's slots: the gather needs no header
-    // result table
     uint2* table = nullptr; PktGather g; memset(&g, 0, sizeof g);
-    if (gather) {
-        ctx->peer_epoch += 1;
-        g = make_gather(ctx, ctx->peer_epoch, 0, 0, 0, ctx->d_sc_counts + 1);
-        table = g.table;
-    } else {
-        if ((size_t)n_out + 16 > ctx->cap_gtable) {
-            const size_t ncap = (size_t)n_out + n_out / 4 + 64;
-            if ((rc = grow_nc(ctx, ctx->d_gtable, 0, ncap))) return rc;
-            ctx->cap_gtable = ncap;
-        }
-        table = ctx->d_gtable;
-    }
+    if ((rc = result_table(ctx, n_out, ctx->d_sc_counts + 1, g, table))) return rc;
     // 1. this rank's claims, compacted in input order, node indices local to the shard
     ctx->shard_epoch += 1;
     // A tile takes a predecessor's status word for this call's when the word's 10-bit epoch matches and its state is set, so a
@@ -1760,7 +1787,7 @@ int dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
         return fail(ctx, DRA_E_INVAL, "dense form: n_pair %u != n_pod %u x n_node %u", n_pair, n_pod, ctx->n_node);
     if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
     const bool gather = ctx->world > 1;
-    if (gather && !(ctx->peer_ready && ctx->peer_form == 2)) return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
+    if (int rc = need_peers(ctx)) return rc;
     if (gather && n_pair > ctx->peer_uns_pairs)
         return fail(ctx, DRA_E_INVAL, "n_pair %u exceeds the max_pairs (%u) of dra_set_shard_pairs before dra_shard_export", n_pair, ctx->peer_uns_pairs);
     if (n_pair && !d_suitable_bits) return DRA_E_INVAL;
@@ -1790,25 +1817,17 @@ int dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     Prof prof(ctx);
     if (a.n_walk && (rc = launch_unsuitable(ctx, a, true))) return rc;
     prof.mark();
-    UnsExchange x; memset(&x, 0, sizeof x);
-    x.bits = ctx->d_ubits; x.out = d_suitable_bits;
-    x.n_words = (uint32_t)n_words; x.n_bytes = (uint32_t)(((size_t)n_pair + 7) / 8);
-    x.world = 1; x.rank = 0; x.spin_limit = ctx->peer_spin; x.err = err;
+    UnsMerge m; memset(&m, 0, sizeof m);
+    m.bits = ctx->d_ubits; m.out = d_suitable_bits;
+    m.n_words = (uint32_t)n_words; m.n_bytes = (uint32_t)(((size_t)n_pair + 7) / 8); m.stride = ctx->uns_stride;
+    const PeerExchange x = gather ? bind_exchange(ctx, ctx->uns_x) : PeerExchange{};   // world 1: no peers
     if (gather) {
-        const uint32_t seq = ++ctx->uns_seq, par = seq & 1u;
-        x.world = (uint32_t)ctx->world; x.rank = (uint32_t)ctx->rank; x.seq = seq; x.stride = ctx->uns_stride;
-        for (int r = 0; r < ctx->world; ++r) {
-            x.stage[r] = (uint32_t*)(ctx->peer_base[r] + ctx->off_ustage[par]) + (size_t)ctx->rank * ctx->uns_stride;
-            x.flag[r] = (uint32_t*)(ctx->peer_base[r] + ctx->off_uflags) + ctx->rank;
-        }
-        x.my_stage = (const uint32_t*)(ctx->peer_local + ctx->off_ustage[par]);
-        x.my_flags = (const uint32_t*)(ctx->peer_local + ctx->off_uflags);
         const uint32_t n4 = (uint32_t)(n_words4 / 4);
-        k_uns_push<<<std::max(1u, std::min((n4 + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, ctx->stream>>>(x);
+        k_peer_push<<<std::max(1u, std::min((n4 + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, ctx->stream>>>(x, (const uint4*)ctx->d_ubits, 0u, n4);
         ctx->launches += 1;
     }
     const uint32_t merge_grid = std::max(1u, std::min((uint32_t)((n_words + 1023) / 1024), (uint32_t)std::max(1, ctx->n_sm / 4)));
-    k_uns_merge<<<merge_grid, 256, 0, ctx->stream>>>(x);
+    k_uns_merge<<<merge_grid, 256, 0, ctx->stream>>>(x, m);
     ctx->launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded UnsuitableNodes launch: %s", cudaGetErrorString(e));
@@ -1827,12 +1846,12 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
         return fail(ctx, DRA_E_INVAL, "dra_allocate_pods_batch_global_device: unknown flags 0x%x", flags);
     if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
-    if (n_claim > (1u << 26) || n_out > (1u << 26) || n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
-    if (!d_out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    if (n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
+    if (int rc = check_slots(ctx, n_claim, n_out, d_out_off != nullptr)) return rc;
     if (!n_pod && n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]: no pods for %u claims", n_claim);
     const bool gather = ctx->world > 1;
     if (gather && !ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the gather needs every rank's range)");
-    if (gather && !(ctx->peer_ready && ctx->peer_form == 2)) return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
+    if (int rc = need_peers(ctx)) return rc;
     if (gather && n_out > ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", n_out, ctx->peer_tab_len);
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
@@ -1853,19 +1872,8 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     }
     if (!ctx->d_spod) CU(cudaMalloc((void**)&ctx->d_spod, SP_WORDS * 4));
     uint2* table = nullptr; PktGather g; memset(&g, 0, sizeof g);
-    if (gather) {
-        ctx->peer_epoch += 1;
-        g = make_gather(ctx, ctx->peer_epoch, 0, 0, 0, nullptr);
-        g.expect = ctx->d_spod + SP_EXPECT;
-        table = g.table;
-    } else {
-        if ((size_t)n_out + 16 > ctx->cap_gtable) {
-            const size_t ncap = (size_t)n_out + n_out / 4 + 64;
-            if ((rc = grow_nc(ctx, ctx->d_gtable, 0, ncap))) return rc;
-            ctx->cap_gtable = ncap;
-        }
-        table = ctx->d_gtable;
-    }
+    if ((rc = result_table(ctx, n_out, nullptr, g, table))) return rc;
+    if (gather) g.expect = ctx->d_spod + SP_EXPECT;
     const Err err = err_of(ctx);
     SPodArgs sa; memset(&sa, 0, sizeof sa);
     sa.claims = (const uint4*)d_claims; sa.pod_off = d_pod_off; sa.out_off = d_out_off;
@@ -1909,35 +1917,27 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     return DRA_OK;
 }
 
-// Inventory sync: this rank's GPU range into every peer's staging (k_isync_push) -> flags, wait, and the copy of every other
+// Inventory sync: this rank's GPU range into every peer's staging (k_peer_push) -> flags, wait, and the copy of every other
 // rank's range into the live copy (k_isync_copy).  Enqueues only.
 int dra_shard_sync_inventory_device(dra_ctx* ctx) {
     if (!ctx) return DRA_E_INVAL;
     QUIESCE();
     if (ctx->world <= 1) return DRA_OK;
     if (!ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the sync needs every rank's range)");
-    if (!(ctx->peer_ready && ctx->peer_form == 2)) return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
+    if (int rc = need_peers(ctx)) return rc;
     if (!ctx->peer_inv_gpus) return fail(ctx, DRA_E_STATE, "the inventory was not loaded before dra_shard_export: the export reserved no staging for it");
     if (ctx->n_gpu > ctx->peer_inv_gpus)
         return fail(ctx, DRA_E_STATE, "the inventory grew to %u GPUs after dra_shard_export reserved staging for %u", ctx->n_gpu, ctx->peer_inv_gpus);
     if (ctx->shard_bounds[ctx->world] != ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard map does not span the inventory's %u nodes", ctx->n_node);
     CU(cudaSetDevice(ctx->device));
-    const uint32_t seq = ++ctx->isync_seq, par = seq & 1u;
-    InvSync x; memset(&x, 0, sizeof x);
-    for (int r = 0; r < ctx->world; ++r) {
-        x.stage[r] = (uint4*)(ctx->peer_base[r] + ctx->off_istage[par]);
-        x.flag[r] = (uint32_t*)(ctx->peer_base[r] + ctx->off_iflags) + ctx->rank;
-    }
-    x.my_stage = (const uint4*)(ctx->peer_local + ctx->off_istage[par]);
-    x.my_flags = (const uint32_t*)(ctx->peer_local + ctx->off_iflags);
-    x.elect = (uint32_t*)(ctx->peer_local + ctx->off_iflags) + PEER_MAX;
-    x.inv = ctx->d_inv_live; x.n_gpu = ctx->n_gpu;
-    x.own_lo = ctx->h_node_off[ctx->shard_bounds[ctx->rank]]; x.own_hi = ctx->h_node_off[ctx->shard_bounds[ctx->rank + 1]];
-    x.world = (uint32_t)ctx->world; x.rank = (uint32_t)ctx->rank; x.seq = seq; x.spin_limit = ctx->peer_spin; x.err = err_of(ctx);
-    const uint32_t n_own = x.own_hi - x.own_lo;
-    k_isync_push<<<std::max(1u, std::min((n_own + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, ctx->stream>>>(x);
+    const PeerExchange x = bind_exchange(ctx, ctx->isync_x);
+    InvSync s; memset(&s, 0, sizeof s);
+    s.inv = ctx->d_inv_live; s.n_gpu = ctx->n_gpu;
+    s.elect = (uint32_t*)(ctx->peer_local + ctx->isync_x.flags) + PEER_MAX;
+    s.own_lo = ctx->h_node_off[ctx->shard_bounds[ctx->rank]]; s.own_hi = ctx->h_node_off[ctx->shard_bounds[ctx->rank + 1]];
+    k_peer_push<<<std::max(1u, std::min((s.own_hi - s.own_lo + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, ctx->stream>>>(x, s.inv, s.own_lo, s.own_hi);
     // a small grid: it waits for its peers, and ranks sharing one device must not find their push's SMs held by it
-    k_isync_copy<<<std::max(1u, std::min((ctx->n_gpu + 255) / 256, (uint32_t)std::max(1, ctx->n_sm / 4))), 256, 0, ctx->stream>>>(x);
+    k_isync_copy<<<std::max(1u, std::min((ctx->n_gpu + 255) / 256, (uint32_t)std::max(1, ctx->n_sm / 4))), 256, 0, ctx->stream>>>(x, s);
     ctx->launches += 2;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "inventory sync launch: %s", cudaGetErrorString(e));
@@ -1954,8 +1954,7 @@ int dra_deallocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
     if (ctx->shard_hi > ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard [%u, %u) lies outside the inventory's %u nodes", ctx->shard_lo, ctx->shard_hi, ctx->n_node);
-    if (n_claim > (1u << 26) || n_out > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
-    if (!d_out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    if (int rc = check_slots(ctx, n_claim, n_out, d_out_off != nullptr)) return rc;
     if (!n_claim) return DRA_OK;
     CU(cudaSetDevice(ctx->device));
     const Err err = err_of(ctx);

@@ -1222,23 +1222,58 @@ k_shard_compact_flat(const ShardArgs a) {
     shard_tile_flat<ROWS>(a, blockIdx.x);
 }
 
-// Cross-rank rendezvous on the device (dra_peer_rendezvous_device): lane r stores this call's sequence number into peer
-// r's flag word for this rank, then every lane waits until its own peer's word for THIS rank has reached it.  Monotonic
-// sequence numbers: nothing is ever reset.  Orders nothing but time — it lines the ranks' streams up (a benchmark uses it
-// after its untimed L2 flush so that a rank's timed step does not absorb its peers' flush-duration skew).
-struct RendezvousArgs { uint32_t* peer_flags[PEER_MAX]; const uint32_t* my_flags; uint32_t world, rank, seq; long long spin_limit; Err err; };
-__global__ void __launch_bounds__(32)
-k_rendezvous(const RendezvousArgs a) {
-    const uint32_t lane = threadIdx.x;
-    if (lane >= a.world) return;
-    asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(a.peer_flags[lane] + a.rank), "r"(a.seq) : "memory");
-    const long long t0 = clock64();
+// The flag-and-staging exchange of the sharded calls whose latency matters little (the rendezvous, UnsuitableNodes' bit
+// exchange, the inventory sync): plain 16-byte stores into every peer's staging (k_peer_push), a system-scope fence, one
+// flag per peer raised to the call's sequence number (peer_raise), and a bounded wait for every peer's flag here
+// (peer_wait: ERR_PEER_TIMEOUT after spin_limit cycles, never a hang).  Monotonic sequence numbers: nothing is ever reset.
+// Each exchange has its own region of the peer buffer; staging is double-buffered by call parity.
+struct PeerExchange {
+    uint4* stage[PEER_MAX];       // stage[p]: this rank's destination inside peer p's staging area (parity and slice applied)
+    uint32_t* flag[PEER_MAX];     // flag[p]: this rank's flag word at peer p
+    const uint4* my_stage;        // this rank's staging area (parity applied)
+    const uint32_t* my_flags;     // [PEER_MAX], indexed by sender
+    uint32_t world, rank, seq;
+    long long spin_limit;         // clock cycles before a missing peer becomes ERR_PEER_TIMEOUT (never a hang)
+    Err err;
+};
+
+// thread tid raises this rank's flag at peer tid, after a system-scope fence: the staged stores before it are seen first
+__device__ __forceinline__ void peer_raise(const PeerExchange& x, uint32_t tid) {
+    if (tid >= x.world || tid == x.rank) return;
+    __threadfence_system();
+    asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(x.flag[tid]), "r"(x.seq) : "memory");
+}
+// thread tid waits until peer tid's flag here has reached the call's sequence number; false (ERR_PEER_TIMEOUT set) once
+// spin_limit cycles have passed since t0
+__device__ __forceinline__ bool peer_wait(const PeerExchange& x, uint32_t tid, long long t0) {
+    if (tid >= x.world || tid == x.rank) return true;
     uint32_t v;
     do {
-        asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(a.my_flags + lane) : "memory");
-        if ((int32_t)(v - a.seq) >= 0) break;
-        if (clock64() - t0 > a.spin_limit) { a.err.set(ERR_PEER_TIMEOUT); break; }
-    } while (true);
+        asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(x.my_flags + tid) : "memory");
+        if ((int32_t)(v - x.seq) >= 0) return true;
+    } while (clock64() - t0 <= x.spin_limit);
+    x.err.set(ERR_PEER_TIMEOUT);
+    return false;
+}
+
+// src[lo, hi) into stage[p] at the same indices for every peer p, then a system-scope fence per thread.  Nothing waits here.
+__global__ void __launch_bounds__(256)
+k_peer_push(const PeerExchange x, const uint4* __restrict__ src, uint32_t lo, uint32_t hi) {
+    for (uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += gridDim.x * blockDim.x) {
+        const uint4 v = __ldcg(&src[i]);
+        for (uint32_t p = 0; p < x.world; ++p)
+            if (p != x.rank) x.stage[p][i] = v;
+    }
+    __threadfence_system();
+}
+
+// Cross-rank rendezvous on the device (dra_peer_rendezvous_device): the exchange's flags alone, nothing staged.  Orders
+// nothing but time — it lines the ranks' streams up (a benchmark uses it after its untimed L2 flush so that a rank's timed
+// step does not absorb its peers' flush-duration skew).
+__global__ void __launch_bounds__(32)
+k_rendezvous(const PeerExchange x) {
+    peer_raise(x, threadIdx.x);
+    peer_wait(x, threadIdx.x, clock64());
 }
 
 // ====================================================================================================
@@ -2757,127 +2792,76 @@ k_uns_prep(const uint32_t* __restrict__ pod_off, const uint32_t* __restrict__ ca
     if (bad && lane == 0) err.set(ERR_BAD_OFFSETS);
 }
 
-// The bit exchange.  Latency matters little next to the evaluation (100 us to ms), so: plain copies, one fence, one flag.
-//   k_uns_push   this rank's words (its own pairs' bits, every other bit zero) into its slice of every peer's staging area
-//                (parity applied), then a system-scope fence per thread.  Nothing waits here.
-//   k_uns_merge  block 0 raises this rank's flag word at every peer to the call's sequence number (the push grid has
-//                completed, its stores are fenced); every block then waits — bounded, ERR_PEER_TIMEOUT, never a hang — until
-//                every peer's flag here has reached it, and ORs the world's slices into the caller's bytes.  A small grid of
-//                its own: ranks sharing one device must not find their evaluation's SMs held by a peer's waiting CTAs.
-// Staging is double-buffered by call parity: a rank is never two calls ahead, since its next merge waits for this rank's next
-// push.  With world 1 the merge only turns the words into ceil(n_pair/8) bytes.
-struct UnsExchange {
-    uint32_t* stage[PEER_MAX];    // stage[p]: THIS rank's slice inside peer p's staging area (parity applied)
-    uint32_t* flag[PEER_MAX];     // flag[p]: this rank's flag word at peer p
-    const uint32_t* my_stage;     // this rank's staging area (parity applied): sender s's slice at my_stage + s * stride
-    const uint32_t* my_flags;     // [PEER_MAX], indexed by sender
+// The bit exchange: the peer exchange (PeerExchange) with one slice per sender.  Latency matters little next to the
+// evaluation (100 us to ms).  k_peer_push sends this rank's words (its own pairs' bits, every other bit zero; slices and
+// the local words are padded to 16 bytes), then
+//   k_uns_merge  block 0 raises this rank's flags (the push grid has completed, its stores are fenced); every block waits
+//                for every peer's flag and ORs the world's slices into the caller's bytes, whatever the wait returned.  A
+//                small grid of its own: ranks sharing one device must not find their evaluation's SMs held by a peer's
+//                waiting CTAs.
+// A rank is never two calls ahead, since its next merge waits for this rank's next push.  With world 1 (an all-zero
+// PeerExchange: no peers) the merge only turns the words into ceil(n_pair/8) bytes.
+struct UnsMerge {
     const uint32_t* bits;         // this rank's words
     uint8_t* out;                 // ceil(n_pair / 8) bytes
-    uint32_t n_words, n_bytes, stride, world, rank, seq;
-    long long spin_limit;
-    Err err;
+    uint32_t n_words, n_bytes;
+    uint32_t stride;              // words of one sender's slice: sender s's at PeerExchange::my_stage + s * stride words
 };
 
 __global__ void __launch_bounds__(256)
-k_uns_push(const UnsExchange x) {
-    const uint32_t n4 = (x.n_words + 3) / 4;                          // slices and the local words are padded to 16 bytes
-    const uint4* src = reinterpret_cast<const uint4*>(x.bits);
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x) {
-        const uint4 v = __ldcg(&src[i]);
-        for (uint32_t p = 0; p < x.world; ++p)
-            if (p != x.rank) reinterpret_cast<uint4*>(x.stage[p])[i] = v;
-    }
-    __threadfence_system();
-}
-
-__global__ void __launch_bounds__(256)
-k_uns_merge(const UnsExchange x) {
+k_uns_merge(const PeerExchange x, const UnsMerge m) {
     const uint32_t tid = threadIdx.x;
-    if (blockIdx.x == 0 && tid < x.world && tid != x.rank) {
-        __threadfence_system();
-        asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(x.flag[tid]), "r"(x.seq) : "memory");
-    }
-    if (tid < x.world && tid != x.rank) {
-        const long long t0 = clock64();
-        uint32_t v;
-        do {
-            asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(x.my_flags + tid) : "memory");
-            if ((int32_t)(v - x.seq) >= 0) break;
-            if (clock64() - t0 > x.spin_limit) { x.err.set(ERR_PEER_TIMEOUT); break; }
-        } while (true);
-    }
+    if (blockIdx.x == 0) peer_raise(x, tid);
+    peer_wait(x, tid, clock64());
     __syncthreads();
-    const bool whole = (reinterpret_cast<uintptr_t>(x.out) & 3u) == 0;
-    for (uint32_t w = blockIdx.x * blockDim.x + tid; w < x.n_words; w += gridDim.x * blockDim.x) {
-        uint32_t v = __ldcg(&x.bits[w]);
-        for (uint32_t s = 0; s < x.world; ++s)
-            if (s != x.rank) v |= __ldcg(&x.my_stage[(size_t)s * x.stride + w]);
+    const uint32_t* my_stage = reinterpret_cast<const uint32_t*>(x.my_stage);
+    const uint32_t world = x.world, rank = x.rank;           // (read from the parameters once: 32 registers, not 34)
+    const bool whole = (reinterpret_cast<uintptr_t>(m.out) & 3u) == 0;
+    for (uint32_t w = blockIdx.x * blockDim.x + tid; w < m.n_words; w += gridDim.x * blockDim.x) {
+        uint32_t v = __ldcg(&m.bits[w]);
+        for (uint32_t s = 0; s < world; ++s)
+            if (s != rank) v |= __ldcg(&my_stage[(size_t)s * m.stride + w]);
         const uint32_t b0 = w * 4;
-        if (whole && b0 + 4 <= x.n_bytes) *reinterpret_cast<uint32_t*>(x.out + b0) = v;
-        else for (uint32_t b = 0; b < 4 && b0 + b < x.n_bytes; ++b) x.out[b0 + b] = (uint8_t)(v >> (8 * b));
+        if (whole && b0 + 4 <= m.n_bytes) *reinterpret_cast<uint32_t*>(m.out + b0) = v;
+        else for (uint32_t b = 0; b < 4 && b0 + b < m.n_bytes; ++b) m.out[b0 + b] = (uint8_t)(v >> (8 * b));
     }
 }
 
 // The inventory sync (dra_shard_sync_inventory_device): every rank's GPU records of its own range to every peer, so that
-// every live copy becomes the world's state.  The same exchange as UnsuitableNodes': plain copies, one fence, one flag.
-// Owned ranges are disjoint, so every rank writes its records at their GLOBAL indices into one staging area per peer.
-//   k_isync_push  this rank's GPUs [own_lo, own_hi) of the live copy into every peer's staging (parity applied), 16-byte
-//                 stores, then a system-scope fence per thread.  Nothing waits here.
-//   k_isync_copy  a grid of at most SMs / 4 CTAs.  The first CTA to arrive (one atomicMax on `elect`) raises this rank's flag at
-//                 every peer to the call's sequence number, waits for every peer's flag here (bounded: ERR_PEER_TIMEOUT,
-//                 never a hang) and publishes ONE verdict for the call in `verdict`; the other CTAs wait for that verdict
-//                 (locally) and all of them copy GPUs outside [own_lo, own_hi) from staging into the live copy only when
-//                 every peer arrived.  One verdict makes it all or nothing: a timed-out call leaves the live copy as it was.
-//                 The elected CTA started before any CTA waiting for it, so those wait at most twice the spin limit.
-// Staging is double-buffered by call parity: a rank is never two calls ahead, since its next copy kernel waits for this
-// rank's next flag, which this rank raises only after its copy of the call before.
+// every live copy becomes the world's state, over the peer exchange (PeerExchange).  Owned ranges are disjoint, so every
+// rank writes its records at their GLOBAL indices into one staging area per peer: k_peer_push sends this rank's GPUs
+// [own_lo, own_hi) of the live copy, then
+//   k_isync_copy  a grid of at most SMs / 4 CTAs.  The first CTA to arrive (one atomicMax on `elect`) raises this rank's
+//                 flags, waits for every peer's flag and publishes ONE verdict for the call in `elect`; the other CTAs wait
+//                 for that verdict (locally) and all of them copy GPUs outside [own_lo, own_hi) from staging into the live
+//                 copy only when every peer arrived.  One verdict makes it all or nothing: a timed-out call leaves the live
+//                 copy as it was.  The elected CTA started before any CTA waiting for it, so those wait at most twice the
+//                 spin limit.
+// A rank is never two calls ahead, since its next copy kernel waits for this rank's next flag, which this rank raises only
+// after its copy of the call before.
 struct InvSync {
-    uint4* stage[PEER_MAX];       // stage[p]: peer p's staging area (parity applied), indexed by global GPU
-    uint32_t* flag[PEER_MAX];     // flag[p]: this rank's flag word at peer p
-    const uint4* my_stage;        // this rank's staging area (parity applied)
-    const uint32_t* my_flags;     // [PEER_MAX], indexed by sender
     uint4* inv;                   // the live copy
     uint32_t* elect;              // [0] the last call whose CTA was elected, [1] that call's verdict: seq << 1 | all arrived
-    uint32_t n_gpu, own_lo, own_hi, world, rank, seq;
-    long long spin_limit;
-    Err err;
+    uint32_t n_gpu, own_lo, own_hi;
 };
 
 __global__ void __launch_bounds__(256)
-k_isync_push(const InvSync x) {
-    for (uint32_t i = x.own_lo + blockIdx.x * blockDim.x + threadIdx.x; i < x.own_hi; i += gridDim.x * blockDim.x) {
-        const uint4 v = x.inv[i];
-        for (uint32_t p = 0; p < x.world; ++p)
-            if (p != x.rank) x.stage[p][i] = v;
-    }
-    __threadfence_system();
-}
-
-__global__ void __launch_bounds__(256)
-k_isync_copy(const InvSync x) {
+k_isync_copy(const PeerExchange x, const InvSync s) {
     __shared__ uint32_t s_lead, s_ok;
     const uint32_t tid = threadIdx.x;
-    if (tid == 0) { s_lead = atomicMax(&x.elect[0], x.seq) < x.seq; s_ok = 1u; }
+    if (tid == 0) { s_lead = atomicMax(&s.elect[0], x.seq) < x.seq; s_ok = 1u; }
     __syncthreads();
     const long long t0 = clock64();
     if (s_lead) {
-        if (tid < x.world && tid != x.rank) {
-            __threadfence_system();
-            asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(x.flag[tid]), "r"(x.seq) : "memory");
-            uint32_t v;
-            do {
-                asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(x.my_flags + tid) : "memory");
-                if ((int32_t)(v - x.seq) >= 0) break;
-                if (clock64() - t0 > x.spin_limit) { x.err.set(ERR_PEER_TIMEOUT); s_ok = 0u; break; }
-            } while (true);
-        }
+        peer_raise(x, tid);
+        if (!peer_wait(x, tid, t0)) s_ok = 0u;
         __syncthreads();
-        if (tid == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(x.elect + 1), "r"(x.seq << 1 | s_ok) : "memory");
+        if (tid == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(s.elect + 1), "r"(x.seq << 1 | s_ok) : "memory");
     } else {
         if (tid == 0) {
             uint32_t v;
             do {
-                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(x.elect + 1) : "memory");
+                asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(s.elect + 1) : "memory");
                 if ((v >> 1) == (x.seq & 0x7FFFFFFFu)) { s_ok = v & 1u; break; }
                 if (clock64() - t0 > 2 * x.spin_limit) { x.err.set(ERR_PEER_TIMEOUT); s_ok = 0u; break; }
             } while (true);
@@ -2885,8 +2869,8 @@ k_isync_copy(const InvSync x) {
         __syncthreads();
     }
     if (!s_ok) return;
-    for (uint32_t i = blockIdx.x * blockDim.x + tid; i < x.n_gpu; i += gridDim.x * blockDim.x)
-        if (i < x.own_lo || i >= x.own_hi) x.inv[i] = __ldcg(&x.my_stage[i]);
+    for (uint32_t i = blockIdx.x * blockDim.x + tid; i < s.n_gpu; i += gridDim.x * blockDim.x)
+        if (i < s.own_lo || i >= s.own_hi) s.inv[i] = __ldcg(&x.my_stage[i]);
 }
 
 // ====================================================================================================
@@ -2954,12 +2938,25 @@ k_dealloc(const uint4* __restrict__ claims, uint32_t n_claim, const uint32_t* __
 // ====================================================================================================
 // the all-gather as its own kernel (sort path: the pack kernel has no tail), same packets as k_fused's tail
 // ====================================================================================================
+// Warp-collective: one reservation per warp of the lanes' n packets, contiguous in this rank's slice, so that they leave
+// as 128-byte lines on the wire.  Returns the lane's first position.
+__device__ __forceinline__ uint32_t pkt_warp_reserve(const PktGather& g, uint32_t n) {
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t incl = n;
+    #pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(FULLMASK, incl, d); if (lane >= (uint32_t)d) incl += y; }
+    const uint32_t tot = __shfl_sync(FULLMASK, incl, 31);
+    uint32_t base = 0;
+    if (lane == 0 && tot) base = atomicAdd(&g.cursor[g.parity], tot);
+    return __shfl_sync(FULLMASK, base, 0) + incl - n;
+}
+
 // claims[0..n) are THIS rank's claims (input order or sorted, any order), out_off their first local slot (NULL: slot i);
 // their OutRecs already sit in the local table at slot_base + slot.  Thread per claim: send; then everybody receives.
 __global__ void __launch_bounds__(256)
 k_pkt_gather(const PktGather g, const uint4* __restrict__ claims, uint32_t n_claim, const uint32_t* __restrict__ n_dev,
              const uint32_t* __restrict__ out_off, uint32_t n_out, uint32_t have_off, uint32_t n_node, Err err) {
-    const uint32_t T = blockIdx.x * blockDim.x + threadIdx.x, NT = gridDim.x * blockDim.x, lane = threadIdx.x & 31;
+    const uint32_t T = blockIdx.x * blockDim.x + threadIdx.x, NT = gridDim.x * blockDim.x;
     if (n_dev) n_claim = min(n_claim, __ldcg(n_dev));
     if (blockIdx.x == 0 && threadIdx.x == 32) g.cursor[g.parity ^ 1u] = 0;
     const uint2* local = g.table + g.slot_base;
@@ -2973,14 +2970,7 @@ k_pkt_gather(const PktGather g, const uint4* __restrict__ claims, uint32_t n_cla
             sl = (kind == DRA_KIND_GPU && c.y < n_node && !claim_invalid(kind, 0, count, have_off != 0)) ? count : 1u;
             if (dst > n_out || sl > n_out - dst) sl = 0;
         }
-        // one reservation per warp: contiguous packets, 128-byte lines on the wire
-        uint32_t incl = sl;
-        #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(FULLMASK, incl, d); if (lane >= (uint32_t)d) incl += y; }
-        const uint32_t tot = __shfl_sync(FULLMASK, incl, 31);
-        uint32_t base = 0;
-        if (lane == 0 && tot) base = atomicAdd(&g.cursor[g.parity], tot);
-        base = __shfl_sync(FULLMASK, base, 0) + incl - sl;
+        const uint32_t base = pkt_warp_reserve(g, sl);
         for (uint32_t s_ = 0; s_ < sl; ++s_)
             if (base + s_ < g.cap) pkt_send(g, base + s_, __ldcg(local + dst + s_), g.slot_base + dst + s_);
     }
@@ -3104,7 +3094,7 @@ k_spod_gate(const SPodArgs a, uint32_t cap, const uint4* __restrict__ inv_src, u
 // calls ahead of a peer still reading the staging slices of the same parity.
 __global__ void __launch_bounds__(256)
 k_spod_gather(const PktGather g, const SPodArgs a, uint32_t pad_slot) {
-    const uint32_t T = blockIdx.x * blockDim.x + threadIdx.x, NT = gridDim.x * blockDim.x, lane = threadIdx.x & 31;
+    const uint32_t T = blockIdx.x * blockDim.x + threadIdx.x, NT = gridDim.x * blockDim.x;
     if (blockIdx.x == 0 && threadIdx.x == 32) g.cursor[g.parity ^ 1u] = 0;
     const bool gated = __ldcg(&a.w[SP_GATED]) != 0;
     if (T == 0 && (gated || __ldcg(&a.w[g.rank]) == 0)) pkt_send(g, atomicAdd(&g.cursor[g.parity], 1u), make_uint2(0u, 0u), pad_slot);
@@ -3117,14 +3107,7 @@ k_spod_gather(const PktGather g, const SPodArgs a, uint32_t pad_slot) {
         const bool mine = rec.w == g.rank;
         uint32_t sl = 0;
         if (mine) for (uint32_t i = rec.z; i < rec.z + rec.x; ++i) sl += pod_claim_slots(__ldg(&a.claims[i]), a.n_node, have_off);
-        // one reservation per warp
-        uint32_t incl = sl;
-        #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(FULLMASK, incl, d); if (lane >= (uint32_t)d) incl += y; }
-        const uint32_t tot = __shfl_sync(FULLMASK, incl, 31);
-        uint32_t base = 0;
-        if (lane == 0 && tot) base = atomicAdd(&g.cursor[g.parity], tot);
-        uint32_t pos = __shfl_sync(FULLMASK, base, 0) + incl - sl;
+        uint32_t pos = pkt_warp_reserve(g, sl);
         if (!mine) continue;
         for (uint32_t i = rec.z; i < rec.z + rec.x; ++i) {
             const uint32_t s = pod_claim_slots(__ldg(&a.claims[i]), a.n_node, have_off);
