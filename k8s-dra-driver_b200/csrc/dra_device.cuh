@@ -2044,6 +2044,9 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
     if (has_node) { g0 = __ldg(&a.node_off[node]); g1 = __ldg(&a.node_off[node + 1]); }
     // barrier init spread over the threads (one mbarrier.init each), then one fence + sync
     if (again) {                                   // resident mode: the previous batch's barriers are dead objects now
+        // warp 0 wrote this node's GpuRecs with generic stores in the previous batch; the bulk copy below reads them
+        // through the async proxy
+        asm volatile("fence.proxy.async;" ::: "memory");
         __syncthreads();
         if (threadIdx.x == 0) { mbar_inval_a(tbar); mbar_inval_a(ibar); }
         if (STAGE && threadIdx.x < NW * FU_MAXPIECE) mbar_inval_a(sbar + threadIdx.x * 8);
