@@ -261,6 +261,27 @@ int  dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t
                              const uint32_t* pod_off, uint32_t n_pod,
                              const uint32_t* out_off, dra_out_rec* out, uint32_t n_out, uint32_t flags);
 
+/* Choose the node and Allocate() in one call (spec §13): the batched form of the classic controller's "pending"
+ * allocations — when it evaluated a pod for UnsuitableNodes it folded in the tentative assignments of the pods before
+ * it (SURVEY App. A), so that two pods needing the last free slot of a node were not both sent there.  Pods are taken
+ * in input order; pod p tries its candidates cand_nodes[cand_off[p] .. cand_off[p+1]) in list order, each evaluated
+ * as in dra_allocate_pods_batch (spec §12, with DRA_F_EXHAUSTIVE the backtracking search) on that node's CURRENT state,
+ * with every claim's node taken to be the candidate; the first candidate where the pod fits takes it.
+ *   cand_nodes == cand_off == NULL   dense form: every pod against every node of the inventory, ascending
+ *   pod_node[n_pod]                  the node each pod was placed on, 0xFFFFFFFF when none
+ * A claim's own node field is ignored and never written.  A candidate naming no node of the inventory is skipped.  A
+ * pod placed nowhere takes nothing: its slots carry DRA_ST_POD, or DRA_ST_SEARCH_LIMIT when any of its evaluations ran
+ * out of budget (DRA_ST_INVALID for claims invalid by §3/§10); a pod of more than DRA_MAX_POD claims is INVALID; an
+ * empty pod is skipped.  Slots are counted as if each claim named a node of the inventory.  With one candidate per pod,
+ * the node its claims name, the result is byte for byte dra_allocate_pods_batch's.  pod_off / cand_off not monotone or
+ * not spanning, a slot outside n_out, or unknown flags: DRA_E_INVAL, nothing changed.  Host buffers; flags:
+ * DRA_F_EXHAUSTIVE, DRA_F_FRESH_INVENTORY. */
+int  dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
+                          const uint32_t* pod_off, uint32_t n_pod,
+                          const uint32_t* cand_nodes, const uint32_t* cand_off,
+                          const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
+                          uint32_t* pod_node, uint32_t flags);
+
 /* Deallocate(): stands in for controller.Driver.Deallocate(ctx, claim).  Inverse update from the
  * claims and the OutRecs dra_allocate_batch produced for them (same out_off convention). */
 int  dra_deallocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
@@ -472,6 +493,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_COMPACT_IN_KERNEL 0x40000u  /* sharded call: compaction inside the single-launch kernel */
 #define DRA_K_POD_SHARD         0x80000u  /* sharded pods Allocate: pod records + ownership, gate, k_pods on the node window */
 #define DRA_K_POD_GATHER        0x100000u /* sharded pods Allocate: all-gather of the owned pods' records (world > 1) */
+#define DRA_K_PLACE             0x200000u /* place pods: pod states + pair records, persistent walk of the nodes' visit lists */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

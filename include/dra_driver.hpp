@@ -110,6 +110,12 @@ public:
     struct PodRequest { std::vector<ClaimAllocation*> Claims; std::string SelectedNode; std::vector<std::string> PotentialNodes; };
     void AllocateBatch(const std::vector<PodRequest>& pods);
     void UnsuitableNodesBatch(const std::vector<PodRequest>& pods);
+    // choose the node and allocate in one call (spec §13, dra_place_pods_batch): pods in order, each on the first of its
+    // PotentialNodes where all its claims fit, given what the pods before it took — the classic controller's pending
+    // allocations.  SelectedNode is not read; each claim gets AllocatedNode and Allocation, or Error when the pod fits
+    // on none of its nodes.  Each pod is atomic (spec §12), its MIG claims by the backtracking search when
+    // SetExhaustive(true).  Placed claims can be given back with Deallocate.
+    void PlaceBatch(const std::vector<PodRequest>& pods);
 
     // live occupancy of one GPU (memory-slice mask), for inspection
     uint16_t BusyMask(const std::string& node, uint32_t gpuIndex);

@@ -22,7 +22,7 @@ KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x0
            "sorted_prep": 0x00010, "bucket_small": 0x00020, "hist8": 0x00040, "hist8_multi": 0x00080,
            "hist_warp": 0x00100, "scan8": 0x00200, "scan_rows": 0x00400, "scan": 0x00800, "scatter": 0x01000,
            "pack1": 0x02000, "pack4": 0x04000, "compact_flat1": 0x08000, "compact_flat8": 0x10000,
-           "compact_lookback": 0x20000, "compact_in_kernel": 0x40000, "pod_shard": 0x80000, "pod_gather": 0x100000}
+           "compact_lookback": 0x20000, "compact_in_kernel": 0x40000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000}
 
 
 class DraError(RuntimeError):
@@ -54,6 +54,7 @@ SYMBOLS = {
     "dra_ctx_sync": (_i32, [_vp]),
     "dra_unsuitable_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _u32]),
     "dra_allocate_pods_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _u32]),
+    "dra_place_pods_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u32]),
     "dra_deallocate_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_comm_unique_id": (_i32, [_vp]),
     "dra_comm_init": (_i32, [_vp, _vp, _i32, _i32]),
@@ -274,6 +275,31 @@ class Context:
         self._check(self._lib.dra_allocate_pods_batch(self._h, _ptr(c), len(c), _ptr(po), len(po) - 1, _ptr(oo), _ptr(out),
                                                       n_out, flags))
         return out
+
+    def place_pods(self, claims, pod_off, cand_nodes=None, cand_off=None, out_off=None, n_out=None, flags: int = 0):
+        """Choose the node and allocate (spec §13): pods in input order, each on its first candidate where it fits given
+        what the pods before it took.  cand_nodes/cand_off None = every node, ascending.  The claims' node fields are
+        ignored.  Returns (out, pod_node); pod_node[p] = 0xFFFFFFFF when the pod was placed nowhere.
+        flags: F_EXHAUSTIVE, F_FRESH_INVENTORY."""
+        c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
+        po = np.ascontiguousarray(pod_off, dtype=np.uint32)
+        oo = None if out_off is None else np.ascontiguousarray(out_off, dtype=np.uint32)
+        if n_out is None:
+            placed = c.copy()
+            placed["node"] = 0                         # slots as if every claim named a node of the inventory
+            n_out = len(c) if oo is None else int(R.claim_slots(placed, 1).sum())
+        cn = co = None
+        if cand_nodes is not None or cand_off is not None:
+            co = np.ascontiguousarray(cand_off, dtype=np.uint32)
+            cn = np.ascontiguousarray(cand_nodes if cand_nodes is not None else [], dtype=np.uint32)
+            if len(cn) == 0:
+                cn = np.zeros(1, np.uint32)            # NULL would mean the dense form
+        n_pod = len(po) - 1
+        out = np.zeros(n_out, dtype=R.OUT_DTYPE)
+        pod_node = np.zeros(max(n_pod, 1), dtype=np.uint32)
+        self._check(self._lib.dra_place_pods_batch(self._h, _ptr(c), len(c), _ptr(po), n_pod, _ptr(cn), _ptr(co), _ptr(oo),
+                                                   _ptr(out), n_out, _ptr(pod_node), flags))
+        return out, pod_node[:n_pod]
 
     def unsuitable(self, claims, pod_off, cand_nodes=None, cand_off=None, flags: int = 0) -> np.ndarray:
         """cand_nodes/cand_off None = dense form: every pod against every node (bit k = pod * n_node + node).

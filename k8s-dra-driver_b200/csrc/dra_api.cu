@@ -97,7 +97,10 @@ struct dra_ctx {
     uint32_t* d_hist = nullptr;
     uint32_t* d_claim_off = nullptr;
     uint32_t *d_pod_off = nullptr, *d_cand_off = nullptr, *d_cand_nodes = nullptr, *d_pair_pod = nullptr, *d_bits = nullptr;
-    uint4* d_podrec = nullptr; size_t cap_podrec = 0;     // pod mode (spec §12)
+    uint4* d_podrec = nullptr; size_t cap_podrec = 0;     // pod mode (spec §12); place pods (§13): the pair records
+    uint32_t *d_place_state = nullptr, *d_place_node = nullptr; size_t cap_place_pods = 0;   // place pods: per pod
+    uint32_t* d_place_cursor = nullptr; size_t cap_place_cursor = 0;                          // place pods: per node (+ 1)
+    int place_occ = -1;                   // resident CTAs of k_pods_place<4> per SM (occupancy query, once)
 
     // error flags
     uint32_t* d_err = nullptr;            // device memory
@@ -871,7 +874,8 @@ void dra_ctx_destroy(dra_ctx* c) {
     void* dev[] = {c->d_inv_live, c->d_inv_pristine, c->d_node_off, c->d_tbl, c->d_claims, c->d_sorted, c->d_out_off,
                    c->d_out, c->d_rank, c->d_hist, c->d_claim_off, c->d_pod_off, c->d_cand_off, c->d_cand_nodes,
                    c->d_pair_pod, c->d_bits, c->d_err, c->d_attrs, c->d_sels, c->d_podrec, c->d_cursor, c->d_cclaims, c->d_coff,
-                   c->d_sc_status, c->d_sc_counts, c->d_gtable, c->d_rank_slots, c->d_sc_times, c->d_ubits, c->d_upair_pod, c->d_spod};
+                   c->d_sc_status, c->d_sc_counts, c->d_gtable, c->d_rank_slots, c->d_sc_times, c->d_ubits, c->d_upair_pod, c->d_spod,
+                   c->d_place_state, c->d_place_node, c->d_place_cursor};
     for (void* p : dev) if (p) cudaFree(p);
     for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
@@ -1307,6 +1311,134 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "pod kernels: %s", cudaGetErrorString(e));
     if ((rc = check_err(ctx))) return rc;
     if (rb) memcpy(out, ctx->h_out, rb);
+    return DRA_OK;
+}
+
+// Place pods (spec §13): pod records -> (candidate form) the pair records stably sorted by node with the claim path's
+// bucketing kernels -> one persistent cooperative launch in which each warp walks its nodes' visit lists.  Everything is
+// validated here, before anything is enqueued: a rejected call changes nothing.
+int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, uint32_t n_pod,
+                         const uint32_t* cand_nodes, const uint32_t* cand_off, const uint32_t* out_off, dra_out_rec* out,
+                         uint32_t n_out, uint32_t* pod_node, uint32_t flags) {
+    if (!ctx || !pod_off || (n_claim && (!claims || !out)) || (n_pod && !pod_node)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~(DRA_F_EXHAUSTIVE | DRA_F_FRESH_INVENTORY)) return fail(ctx, DRA_E_INVAL, "dra_place_pods_batch: unknown flags 0x%x", flags);
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (pod_off[0] != 0 || pod_off[n_pod] != n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]");
+    for (uint32_t q = 0; q < n_pod; ++q)
+        if (pod_off[q + 1] < pod_off[q]) return fail(ctx, DRA_E_INVAL, "pod_off not monotone at pod %u", q);
+    const bool dense = cand_nodes == nullptr && cand_off == nullptr;      // every pod against every node, ascending
+    if (!dense && !cand_off) return fail(ctx, DRA_E_INVAL, "cand_nodes without cand_off");
+    if (!dense && cand_off[0] != 0) return fail(ctx, DRA_E_INVAL, "cand_off[0] must be 0");
+    for (uint32_t q = 0; !dense && q < n_pod; ++q) {
+        if (cand_off[q + 1] < cand_off[q]) return fail(ctx, DRA_E_INVAL, "cand_off not monotone at pod %u", q);
+        if (cand_off[q + 1] - cand_off[q] > PL_POS) return fail(ctx, DRA_E_INVAL, "pod %u has more than %u candidates", q, PL_POS);
+    }
+    const uint32_t n_pair = dense ? 0u : cand_off[n_pod];
+    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    if (n_pair && !cand_nodes) return fail(ctx, DRA_E_INVAL, "cand_off lists candidates but cand_nodes is NULL");
+    if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
+    if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    for (uint32_t i = 0; i < n_claim; ++i) {                              // slots as if the claim named a node of the inventory
+        const dra_claim_rec& c = claims[i];
+        const bool gpu = c.kind == DRA_KIND_GPU && c.count >= 1 && c.count <= DRA_MAX_COUNT && (out_off || c.count == 1);
+        const uint32_t slots = gpu ? c.count : 1u, dst = out_off ? out_off[i] : i;
+        if (dst > n_out || slots > n_out - dst) return fail(ctx, DRA_E_INVAL, "claim %u: slots [%u, %u) outside n_out %u", i, dst, dst + slots, n_out);
+    }
+    ctx->chain = ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;
+    if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "dra_place_pods_batch needs cooperative launches, which this device does not offer");
+    CU(cudaSetDevice(ctx->device));
+    int rc = ensure_batch(ctx, std::max(std::max(n_claim, n_pod), n_pair), n_out, true);
+    if (rc) return rc;
+    if ((rc = upload_table(ctx))) return rc;
+    if (n_pod + 8 > ctx->cap_pods) {
+        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_pod_off, 0, cap))) return rc;
+        if ((rc = grow_nc(ctx, ctx->d_cand_off, 0, cap))) return rc;
+        ctx->cap_pods = cap;
+    }
+    if ((size_t)n_pair + 64 > ctx->cap_pairs) {
+        size_t cap = (size_t)n_pair + n_pair / 2 + 128;
+        if ((rc = grow_nc(ctx, ctx->d_cand_nodes, 0, cap))) return rc;
+        if ((rc = grow_nc(ctx, ctx->d_pair_pod, 0, cap))) return rc;
+        ctx->cap_pairs = cap;
+    }
+    if ((size_t)n_pair + 8 > ctx->cap_podrec) {
+        size_t cap = (size_t)n_pair + n_pair / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_podrec, 0, cap))) return rc;
+        ctx->cap_podrec = cap;
+    }
+    if ((size_t)n_pod + 8 > ctx->cap_place_pods) {
+        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_place_state, 0, cap))) return rc;
+        if ((rc = grow_nc(ctx, ctx->d_place_node, 0, cap))) return rc;
+        ctx->cap_place_pods = cap;
+    }
+    if ((size_t)ctx->n_node + 8 > ctx->cap_place_cursor) {
+        size_t cap = (size_t)ctx->n_node + ctx->n_node / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_place_cursor, 0, cap))) return rc;
+        ctx->cap_place_cursor = cap;
+    }
+    // staging: claims | pod_off | out_off | cand_off | cand_nodes
+    const size_t cb = (size_t)n_claim * 16, pb = ((size_t)n_pod + 1) * 4, ob = out_off ? (size_t)n_claim * 4 : 0;
+    const size_t kb = dense ? 0 : ((size_t)n_pod + 1) * 4, nb = (size_t)n_pair * 4, rb = (size_t)n_out * 8, qb = (size_t)n_pod * 4;
+    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + ob + kb + nb + 16))) return rc;
+    if ((rc = grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, rb + qb + 16))) return rc;
+    uint8_t* h = ctx->h_in;
+    if (cb) memcpy(h, claims, cb);
+    memcpy(h + cb, pod_off, pb);
+    if (ob) memcpy(h + cb + pb, out_off, ob);
+    if (kb) memcpy(h + cb + pb + ob, cand_off, kb);
+    if (nb) memcpy(h + cb + pb + ob + kb, cand_nodes, nb);
+    if (cb) CU(cudaMemcpyAsync(ctx->d_claims, h, cb, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->d_pod_off, h + cb, pb, cudaMemcpyHostToDevice, ctx->stream));
+    if (ob) CU(cudaMemcpyAsync(ctx->d_out_off, h + cb + pb, ob, cudaMemcpyHostToDevice, ctx->stream));
+    if (kb) CU(cudaMemcpyAsync(ctx->d_cand_off, h + cb + pb + ob, kb, cudaMemcpyHostToDevice, ctx->stream));
+    if (nb) CU(cudaMemcpyAsync(ctx->d_cand_nodes, h + cb + pb + ob + kb, nb, cudaMemcpyHostToDevice, ctx->stream));
+    if (rb) CU(cudaMemsetAsync(ctx->d_out, 0, rb, ctx->stream));
+    CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)ctx->n_node + 1) * 4, ctx->stream));
+    Prof prof(ctx);
+    PlaceArgs a; memset(&a, 0, sizeof a);
+    a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.n_pod = n_pod;
+    a.cand_nodes = dense ? nullptr : ctx->d_cand_nodes; a.cand_off = dense ? nullptr : ctx->d_cand_off;
+    a.out_off = out_off ? ctx->d_out_off : nullptr; a.out = ctx->d_out;
+    a.state = ctx->d_place_state; a.pod_node = ctx->d_place_node; a.pairs = ctx->d_podrec;
+    a.sorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.cursor = ctx->d_place_cursor;
+    a.inv_src = (flags & DRA_F_FRESH_INVENTORY) ? ctx->d_inv_pristine : ctx->d_inv_live; a.inv_dst = ctx->d_inv_live;
+    a.node_off = ctx->d_node_off; a.tbl = ctx->d_tbl;
+    a.n_node = ctx->n_node; a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.sel = sel_of(ctx); a.err = err_of(ctx);
+    k_pods_place_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, ctx->stream>>>(a);
+    ctx->launches += 1;
+    if (!dense && n_pair &&
+        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, a.inv_src, false, ctx->n_node, ctx->d_node_off)))
+        return rc;
+    if (ctx->n_node) {
+        if (ctx->place_occ < 0) {
+            int occ = 0;
+            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_place<4>, 128, 0));
+            ctx->place_occ = occ;
+        }
+        if (ctx->place_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_place: no CTA can be resident");
+        const uint32_t grid = std::max(1u, std::min((ctx->n_node + 3) / 4, (uint32_t)(ctx->place_occ * ctx->n_sm)));
+        cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
+        lc.gridDim = dim3(grid); lc.blockDim = dim3(128); lc.dynamicSmemBytes = 0; lc.stream = ctx->stream;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
+        lc.attrs = at; lc.numAttrs = 1;
+        CU(cudaLaunchKernelEx(&lc, k_pods_place<4>, a));
+        ctx->launches += 1;
+    }
+    ctx->chain |= DRA_K_PLACE;
+    prof.mark();
+    if (rb) CU(cudaMemcpyAsync(ctx->h_out, ctx->d_out, rb, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->h_out + rb, ctx->d_place_node, qb, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "place kernels: %s", cudaGetErrorString(e));
+    if ((rc = check_err(ctx))) return rc;
+    if (rb) memcpy(out, ctx->h_out, rb);
+    memcpy(pod_node, ctx->h_out + rb, qb);
     return DRA_OK;
 }
 

@@ -10,6 +10,7 @@
 //                    claim is tested on all GPUs at once, __ballot_sync + __ffs pick lowest GPU / lowest
 //                    start (first-fit), the winner lane updates its register-resident occupancy mask.
 //   k_unsuitable     one warp per (pod, candidate node) pair, same step function on a snapshot
+//   k_pods_place     place pods (spec §13): persistent, a warp walks each of its nodes' visit lists with a cursor
 //   k_dealloc        inverse updates with atomics (sharded: behind k_dealloc_check, on the rank's GPU range only)
 //
 // What this replaces in the reference: the per-node search behind Allocate()/UnsuitableNodes() that
@@ -2685,6 +2686,186 @@ k_pods(const PodArgs a) {
             __syncwarp();
         }
         if (lane < ng && (p1 > p0 || a.inv_src != a.inv_dst)) a.inv_dst[g0 + lane] = L.store(rec);
+    }
+}
+
+// ====================================================================================================
+// place pods (spec §13): pods in input order, each on the first candidate node where it fits on that node's current
+// state — the classic controller's pending allocations (SURVEY App. A), applied to a whole batch in one pass
+// ====================================================================================================
+// Every node keeps a LIST of the visits the sequential rule can make to it, in the order it makes them (candidate form:
+// the {pod, node, position} pair records, stably sorted by node; dense form: implicitly every pod at position = node),
+// and a CURSOR into it.  Every pod keeps a state word: the position in its candidate list it has reached, a done bit and
+// a "search budget ran out somewhere" bit.  One warp owns a node for the whole launch (one lane per GPU, as in k_pods);
+// at entry (q, k) of its list it skips q when q is done or already past position k, evaluates q when q is AT k, and
+// otherwise waits: q may still come here.  Exact: a node evaluates q only after every pod before q that lists the node
+// has passed its cursor.  Progress: the lowest unfinished pod heads its current node's list (everything before it there
+// belongs to finished pods or to its own earlier positions), so with every CTA resident the loop always advances.
+constexpr uint32_t PL_DONE = 0x80000000u, PL_LIMIT = 0x40000000u, PL_POS = 0x3FFFFFFFu;
+
+struct PlaceArgs {
+    const uint4* claims; const uint32_t* pod_off; uint32_t n_pod;
+    const uint32_t* cand_nodes; const uint32_t* cand_off;   // nullptr: dense form
+    const uint32_t* out_off; uint2* out;
+    uint32_t* state; uint32_t* pod_node;
+    uint4* pairs;                 // candidate form: {pod, node (0xFFFFFFFF: never visited), position, 0} per candidate
+    const uint4* sorted;          // the pairs stably sorted by node (the bucketing kernels), node n's at list_off[n] ..
+    const uint32_t* list_off;
+    uint32_t* cursor;             // [n_node] per node: entries of its list already passed; [n_node]: evaluations so far
+    const uint4* inv_src; uint4* inv_dst; const uint32_t* node_off; const uint32_t* tbl;
+    uint32_t n_node, exhaustive; SelCtx sel; Err err;
+};
+
+__device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
+    uint32_t v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
+}
+__device__ __forceinline__ void st_release_u32(uint32_t* p, uint32_t v) {
+    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// The final records of a pod placed nowhere (warp-wide): INVALID for the claims invalid by §3/§10 (every claim when the
+// pod has more than 32), `st` for the others; slots counted as if each claim named a node of the inventory.
+__device__ __forceinline__ void place_fail(const PlaceArgs& a, uint32_t c0, uint32_t cnt, uint32_t st, uint32_t lane) {
+    const bool have_off = a.out_off != nullptr;
+    for (uint32_t i = lane; i < cnt; i += 32) {
+        const uint4 c = __ldg(&a.claims[c0 + i]);
+        const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
+        const bool shape = claim_invalid(kind, prof, count, have_off);
+        const bool inv = cnt > DRA_MAX_POD || shape || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
+        const uint32_t op = kind == DRA_KIND_GPU ? DRA_PROFILE_GPU : kind == DRA_KIND_SHARED ? DRA_PROFILE_SHARED : prof;
+        const uint32_t slots = (kind == DRA_KIND_GPU && !shape) ? count : 1u;
+        const uint32_t dst = have_off ? __ldg(&a.out_off[c0 + i]) : c0 + i;
+        for (uint32_t k = 0; k < slots; ++k) a.out[dst + k] = make_uint2(DRA_GPU_NONE, meta(0, 0, op, inv ? (uint32_t)DRA_ST_INVALID : st));
+    }
+}
+
+// Warp per pod: the pod's state word (first usable position, or done), pod_node = NONE, the records of the pods that
+// will never be evaluated (more than 32 claims, or no candidate naming a node of the inventory) and, candidate form, the
+// pair records.  Pairs of pods that are never evaluated, and pairs naming no node, carry node NONE: the sort drops them.
+__global__ void __launch_bounds__(256)
+k_pods_place_prep(const PlaceArgs a) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (p >= a.n_pod) return;
+    const uint32_t c0 = __ldg(&a.pod_off[p]), cnt = __ldg(&a.pod_off[p + 1]) - c0;
+    const bool live = cnt != 0 && cnt <= DRA_MAX_POD;
+    uint32_t first = PL_DONE;
+    if (!a.cand_off) {
+        if (a.n_node) first = 0;
+    } else {
+        const uint32_t k0 = __ldg(&a.cand_off[p]), nk = __ldg(&a.cand_off[p + 1]) - k0;
+        for (uint32_t j0 = 0; j0 < nk; j0 += 32) {
+            const uint32_t j = j0 + lane;
+            const uint32_t n = j < nk ? __ldg(&a.cand_nodes[k0 + j]) : 0xFFFFFFFFu;
+            const bool usable = n < a.n_node;
+            if (j < nk) a.pairs[k0 + j] = make_uint4(p, live && usable ? n : 0xFFFFFFFFu, j, 0);
+            const uint32_t b = __ballot_sync(FULLMASK, usable);
+            if (b && first == PL_DONE) first = j0 + (uint32_t)__ffs(b) - 1u;
+        }
+    }
+    if (lane == 0) {
+        a.pod_node[p] = DRA_GPU_NONE;
+        a.state[p] = live ? first : PL_DONE;
+    }
+    if (cnt != 0 && (!live || first == PL_DONE)) place_fail(a, c0, cnt, live ? (uint32_t)DRA_ST_POD : (uint32_t)DRA_ST_INVALID, lane);
+}
+
+// Persistent: every CTA resident (cooperative launch); warp w owns nodes w, w + warps, ... and cycles over them.
+template <int WPC>
+__global__ void __launch_bounds__(WPC * 32)
+k_pods_place(const PlaceArgs a) {
+    __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
+    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
+    __syncthreads();
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t w0 = blockIdx.x * WPC + (threadIdx.x >> 5), n_warp = gridDim.x * WPC;
+    const bool dense = a.cand_off == nullptr, have_off = a.out_off != nullptr;
+    if (a.inv_src != a.inv_dst)                              // DRA_F_FRESH_INVENTORY: the owner copies its nodes first
+        for (uint32_t node = w0; node < a.n_node; node += n_warp) {
+            const uint32_t g0 = __ldg(&a.node_off[node]), ng = __ldg(&a.node_off[node + 1]) - g0;
+            if (lane < ng) a.inv_dst[g0 + lane] = __ldg(&a.inv_src[g0 + lane]);
+        }
+    uint32_t seen = 0;
+    long long t0 = clock64();
+    while (true) {
+        bool left = false, moved = false;
+        for (uint32_t node = w0; node < a.n_node; node += n_warp) {
+            const uint32_t l0 = dense ? 0u : __ldcg(&a.list_off[node]), l1 = dense ? a.n_pod : __ldcg(&a.list_off[node + 1]);
+            const uint32_t cur0 = l0 + __ldcg(&a.cursor[node]);
+            uint32_t cur = cur0;
+            if (cur >= l1) continue;
+            const uint32_t g0 = __ldg(&a.node_off[node]), ng = __ldg(&a.node_off[node + 1]) - g0;
+            Lane L;
+            bool loaded = false, dirty = false;
+            while (cur < l1) {
+                // 32 entries at once: the first one that is not to be skipped
+                const uint32_t e = cur + lane;
+                uint32_t q = 0, k = 0, s = PL_DONE;
+                if (e < l1) {
+                    if (dense) { q = e; k = node; }
+                    else { const uint4 r = __ldcg(&a.sorted[e]); q = r.x; k = r.z; }
+                    s = ld_acquire_u32(&a.state[q]);
+                }
+                const bool skip = (s & PL_DONE) || (s & PL_POS) > k;
+                const uint32_t act = __ballot_sync(FULLMASK, !skip);
+                if (!act) { cur = min(cur + 32u, l1); continue; }
+                const uint32_t f = (uint32_t)__ffs(act) - 1u;
+                cur += f;
+                const uint32_t qf = __shfl_sync(FULLMASK, q, f), kf = __shfl_sync(FULLMASK, k, f), sf = __shfl_sync(FULLMASK, s, f);
+                if ((sf & PL_POS) < kf) break;                   // q may still come here: this node waits
+                (void)ld_acquire_u32(&a.state[qf]);              // every lane: ordered after the previous owner's records
+                if (!loaded) {
+                    L.load(lane < ng ? a.inv_dst[g0 + lane] : make_uint4(0, 0, 0, 0), lane < ng);
+                    loaded = true;
+                }
+                uint32_t st;
+                {
+                    const uint32_t c0 = __ldg(&a.pod_off[qf]), cnt = __ldg(&a.pod_off[qf + 1]) - c0;
+                    const PodGet get{a.claims + c0, have_off ? a.out_off + c0 : nullptr, c0};
+                    Lane Lt = L;
+                    st = pod_eval<32>(Lt, lane, FULLMASK, 0, g0, tbl_s, get, cnt, a.sel, a.exhaustive != 0, have_off, a.out);
+                    if (st == 0) L = Lt;
+                }
+                uint32_t next = PL_DONE;
+                const uint32_t lim = (sf & PL_LIMIT) | (st == DRA_ST_SEARCH_LIMIT ? PL_LIMIT : 0u);
+                if (st == 0) {
+                    dirty = true;
+                    if (lane == 0) a.pod_node[qf] = node;
+                } else {
+                    // the pod's next candidate that names a node of the inventory
+                    if (dense) { if (kf + 1u < a.n_node) next = (kf + 1u) | lim; }
+                    else {
+                        const uint32_t k0 = __ldg(&a.cand_off[qf]), nk = __ldg(&a.cand_off[qf + 1]) - k0;
+                        for (uint32_t j0 = kf + 1u; j0 < nk; j0 += 32) {
+                            const uint32_t j = j0 + lane;
+                            const bool usable = j < nk && __ldg(&a.cand_nodes[k0 + j]) < a.n_node;
+                            const uint32_t b = __ballot_sync(FULLMASK, usable);
+                            if (b) { next = (j0 + (uint32_t)__ffs(b) - 1u) | lim; break; }
+                        }
+                    }
+                    if (next == PL_DONE) {
+                        const uint32_t c0 = __ldg(&a.pod_off[qf]), cnt = __ldg(&a.pod_off[qf + 1]) - c0;
+                        place_fail(a, c0, cnt, lim ? (uint32_t)DRA_ST_SEARCH_LIMIT : (uint32_t)DRA_ST_POD, lane);
+                    }
+                }
+                __threadfence();
+                __syncwarp();
+                if (lane == 0) { st_release_u32(&a.state[qf], next); atomicAdd(&a.cursor[a.n_node], 1u); }
+                moved = true;
+                ++cur;
+            }
+            if (dirty && lane < ng) a.inv_dst[g0 + lane] = L.store(a.inv_dst[g0 + lane]);    // (only this warp writes the node)
+            if (cur != cur0) { moved = true; a.cursor[node] = cur - l0; }     // (every lane: the next visit reads it on every lane)
+            if (cur < l1) left = true;
+        }
+        if (!left) break;
+        if (moved) { t0 = clock64(); continue; }
+        // nothing moved on this warp's nodes: back off, and give up when no pod was evaluated anywhere for a long time
+        // (cannot happen with every CTA resident)
+        __nanosleep(256);
+        const uint32_t pr = __shfl_sync(FULLMASK, ld_acquire_u32(&a.cursor[a.n_node]), 0);
+        if (pr != seen) { seen = pr; t0 = clock64(); }
+        else if (clock64() - t0 > 4000000000ll) { if (lane == 0) a.err.set(ERR_DEVICE_WAIT); break; }
     }
 }
 

@@ -265,6 +265,54 @@ void Driver::UnsuitableNodesBatch(const std::vector<PodRequest>& pods) {
     }
 }
 
+void Driver::PlaceBatch(const std::vector<PodRequest>& pods) {
+    Lowered lo;
+    std::vector<uint32_t> podOff(1, 0), candOff(1, 0), cand;
+    std::vector<size_t> podOf;                                  // lowered pod -> index in pods
+    for (size_t pi = 0; pi < pods.size(); ++pi) {
+        const auto& pod = pods[pi];
+        // profile names resolve against the first known candidate's model, as in UnsuitableNodesBatch; a pod whose
+        // claims cannot be lowered is not placed (each claim's Error says why)
+        uint32_t model = 0;
+        for (const auto& nn : pod.PotentialNodes) { const uint32_t n = nodeIndex(nn); if (n != 0xFFFFFFFFu) { model = nodeModel_[n]; break; } }
+        std::map<std::string, uint32_t> groups;
+        bool ok = true;
+        const size_t mark = lo.recs.size();
+        const uint32_t markOut = lo.nOut;
+        for (ClaimAllocation* ca : groupAdjacent(pod.Claims)) {
+            uint32_t g = 0;
+            if (ca->IsMig && !ca->Mig.GpuClaimName.empty()) {
+                auto it = groups.find(ca->Mig.GpuClaimName);
+                g = it == groups.end() ? (groups[ca->Mig.GpuClaimName] = nextGroup_++) : it->second;
+                if (nextGroup_ == 0) nextGroup_ = 1;
+            }
+            ca->AllocatedNode.clear();
+            ok = lower(*ca, 0, g, lo, model) && ok;             // node: ignored by the call, set from its answer below
+        }
+        if (!ok) {
+            lo.recs.resize(mark); lo.outOff.resize(mark); lo.owner.resize(mark); lo.nOut = markOut;
+            continue;
+        }
+        podOff.push_back((uint32_t)lo.recs.size());
+        for (const auto& nn : pod.PotentialNodes) cand.push_back(nodeIndex(nn));
+        candOff.push_back((uint32_t)cand.size());
+        podOf.push_back(pi);
+    }
+    if (podOf.empty()) return;
+    std::vector<dra_out_rec> out(lo.nOut);
+    std::vector<uint32_t> podNode(podOf.size());
+    check(dra_place_pods_batch(ctx_, lo.recs.data(), (uint32_t)lo.recs.size(), podOff.data(), (uint32_t)podOf.size(),
+                               cand.data(), candOff.data(), lo.outOff.data(), out.data(), lo.nOut, podNode.data(),
+                               exhaustive_ ? DRA_F_EXHAUSTIVE : 0u), "dra_place_pods_batch");
+    for (size_t q = 0; q < podOf.size(); ++q)                   // the records name the chosen node: lift and Deallocate need it
+        for (uint32_t i = podOff[q]; i < podOff[q + 1]; ++i) lo.recs[i].node = podNode[q] == DRA_GPU_NONE ? 0u : podNode[q];
+    lift(lo, out, true);
+    for (size_t q = 0; q < podOf.size(); ++q)
+        if (podNode[q] == DRA_GPU_NONE)
+            for (ClaimAllocation* ca : pods[podOf[q]].Claims)
+                if (ca->Error == status_text(DRA_ST_POD)) ca->Error = "the pod's claims fit together on none of its potential nodes";
+}
+
 void Driver::UnsuitableNodes(const std::vector<ClaimAllocation*>& claims, const std::vector<std::string>& potentialNodes) {
     PodRequest p; p.Claims = claims; p.PotentialNodes = potentialNodes;
     UnsuitableNodesBatch({p});
