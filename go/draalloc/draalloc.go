@@ -196,6 +196,47 @@ func (c *Context) AllocatePodsBatch(claims []ClaimRec, podOff, outOff []uint32, 
 	return out, nil
 }
 
+// PlacePodsBatch chooses the node and allocates in one call (dra_place_pods_batch, spec §13): pods in input order, each on
+// the first of its candidates cands[candOff[p]:candOff[p+1]] where all its claims fit given what the pods before it took.
+// cands == candOff == nil: every node, ascending.  The claims' node fields are ignored.  Returns the OutRecs and, per pod,
+// the node it was placed on (0xFFFFFFFF: none).  nOut counts slots as if every claim named a node.  Unbuilt, like the rest
+// of this file.
+func (c *Context) PlacePodsBatch(claims []ClaimRec, podOff []uint32, cands, candOff []uint32, outOff []uint32, nOut int,
+	flags uint32) ([]OutRec, []uint32, error) {
+	out := make([]OutRec, nOut)
+	podNode := make([]uint32, len(podOff)-1)
+	if len(podNode) == 0 {
+		return out, podNode, nil
+	}
+	var cp *C.dra_claim_rec
+	var oo, cn, co *C.uint32_t
+	if len(claims) > 0 {
+		cp = (*C.dra_claim_rec)(unsafe.Pointer(&claims[0]))
+	}
+	if outOff != nil {
+		oo = (*C.uint32_t)(unsafe.Pointer(&outOff[0]))
+	}
+	if candOff != nil {
+		co = (*C.uint32_t)(unsafe.Pointer(&candOff[0]))
+		if len(cands) == 0 {
+			cands = []uint32{0} // an empty list still needs an address (nil means the dense form)
+		}
+		cn = (*C.uint32_t)(unsafe.Pointer(&cands[0]))
+	}
+	var op *C.dra_out_rec
+	if nOut > 0 {
+		op = (*C.dra_out_rec)(unsafe.Pointer(&out[0]))
+	}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_place_pods_batch(c.h, cp, C.uint32_t(len(claims)), (*C.uint32_t)(unsafe.Pointer(&podOff[0])),
+		C.uint32_t(len(podNode)), cn, co, oo, op, C.uint32_t(nOut), (*C.uint32_t)(unsafe.Pointer(&podNode[0])), C.uint32_t(flags))
+	if rc != 0 {
+		return nil, nil, lastError(c.h)
+	}
+	return out, podNode, nil
+}
+
 func (c *Context) DeallocateBatch(claims []ClaimRec, outOff []uint32, out []OutRec) error {
 	if len(claims) == 0 {
 		return nil
@@ -304,6 +345,34 @@ func (c *Context) AllocatePodsGlobal(pinnedClaims unsafe.Pointer, nClaim int, pi
 	defer c.mu.Unlock()
 	rc := C.dra_allocate_pods_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
 		(*C.uint32_t)(pinnedPodOff), C.uint32_t(nPod), (*C.uint32_t)(pinnedOutOff), C.uint32_t(nOut), C.uint32_t(flags))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
+// SetShardPlace reserves room for the sharded place-pods call's replicated pod states (8 bytes per pod): before
+// ShardExport, the same on every context.  Unbuilt, like the rest of this file.
+func (c *Context) SetShardPlace(maxPods uint32) error {
+	if rc := C.dra_set_shard_place(c.h, C.uint32_t(maxPods)); rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
+// PlacePodsGlobal: place pods (spec §13) on a sharded world (dra_place_pods_batch_global_device).  The same pods and
+// candidates on every context, in dra_host_alloc'ed (pinned) memory (pinnedCandNodes == pinnedCandOff == nil and nPair == 0:
+// dense form; pinnedOutOff may be nil); each context evaluates the visits to its own nodes, and every context ends with the
+// whole table (GatherRead) and the whole pinnedPodNode (nPod uint32).  Returns at once; Sync reports completion and errors
+// found on the device.  Unbuilt, like the rest of this file.
+func (c *Context) PlacePodsGlobal(pinnedClaims unsafe.Pointer, nClaim int, pinnedPodOff unsafe.Pointer, nPod int,
+	pinnedCandNodes, pinnedCandOff unsafe.Pointer, nPair int, pinnedOutOff unsafe.Pointer, nOut int, pinnedPodNode unsafe.Pointer,
+	flags uint32) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_place_pods_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
+		(*C.uint32_t)(pinnedPodOff), C.uint32_t(nPod), (*C.uint32_t)(pinnedCandNodes), (*C.uint32_t)(pinnedCandOff),
+		C.uint32_t(nPair), (*C.uint32_t)(pinnedOutOff), C.uint32_t(nOut), (*C.uint32_t)(pinnedPodNode), C.uint32_t(flags))
 	if rc != 0 {
 		return lastError(c.h)
 	}

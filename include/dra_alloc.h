@@ -310,7 +310,7 @@ int  dra_gather_read(dra_ctx* ctx, dra_out_rec* out_all, uint32_t n_rec);
  *                                              cudaIpcMemHandle_t;  the host runtime all-gathers the handles;
  *   dra_peer_import(ctx, handles)              world * 64 bytes, in rank order.
  * Requires all ranks on one node with P2P access; on failure the NCCL path stays in use.  Every rank must export alike (the
- * same sizes, dra_set_shard_pairs and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
+ * same sizes, dra_set_shard_pairs, dra_set_shard_place and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
  * own layout, so dra_peer_import / dra_peer_import_local refuse a peer set up differently with DRA_E_INVAL.
  * dra_peer_export(ctx, 0, NULL) switches the peer path off again. */
 int  dra_peer_export(dra_ctx* ctx, uint32_t n_per_rank, void* handle64);
@@ -397,6 +397,31 @@ int  dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cla
 int  dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
                                            const uint32_t* d_pod_off, uint32_t n_pod,
                                            const uint32_t* d_out_off, uint32_t n_out, uint32_t flags);
+
+/* Room for the sharded place-pods call's replicated pod states (8 bytes per pod, plus 64) in the buffer dra_shard_export
+ * maps.  World > 1: call before dra_shard_export (afterwards: DRA_E_STATE), every rank with the same max_pods; the peer
+ * import refuses a peer set up differently.  Load the inventory first: the export then also sizes the call's sort for it,
+ * so that no call frees a buffer (which waits for the whole device) while a peer's walk waits for it.  World 1 needs no
+ * call. */
+int  dra_set_shard_place(dra_ctx* ctx, uint32_t max_pods);
+/* Place pods over a sharded world (spec §13, "Sharded form"): dra_place_pods_batch applied to the world's state.  The SAME
+ * claims, pod_off, candidates (cand_nodes == cand_off == NULL and n_pair == 0: the dense form), out_off, n_out and flags on
+ * every rank (device pointers, or dra_host_alloc'ed buffers).  Each rank evaluates the visits to its own nodes, on its live
+ * inventory, and the ranks hand pods to each other through replicated state words.  Every rank ends with the WHOLE table
+ * (dra_gather_table / dra_gather_read) and the whole d_pod_node[n_pod]: byte for byte what dra_place_pods_batch answers on
+ * ONE inventory made of every rank's own nodes; each rank's own GPU range ends as that call leaves it, and no rank writes
+ * a GPU record outside its range, live or pristine.  flags: DRA_F_EXHAUSTIVE, DRA_F_FRESH_INVENTORY (each rank starts its
+ * own range from the pristine copy).  Prerequisites as for dra_allocate_pods_batch_global_device, plus n_pod <= the
+ * max_pods of dra_set_shard_place at world > 1 (else DRA_E_STATE); world 1 (dra_set_shard(ctx, 0, n_node, 1)) needs no
+ * export and answers exactly as dra_place_pods_batch.  Enqueues on ctx's stream and returns; n_pod == 0 enqueues nothing.
+ * Completion and device-detected errors surface at dra_ctx_sync: pod_off / cand_off not monotone or not spanning their
+ * arrays, more than 2^30 - 1 candidates for a pod, a slot range outside n_out, or a rank that could finalise more slots
+ * than its packet room give DRA_E_INVAL on EVERY rank with no inventory changed; a peer that stops making progress gives
+ * DRA_E_NCCL once nothing moved anywhere in the world for DRA_PEER_TIMEOUT_MS. */
+int  dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                        const uint32_t* d_pod_off, uint32_t n_pod,
+                                        const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                        const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node, uint32_t flags);
 
 /* Every rank's live inventory becomes the world's state: for each GPU, the record its owning rank holds (the rank whose
  * node range contains the GPU's node, per the current dra_set_shard_map).  Own range untouched, pristine copy untouched.
@@ -494,6 +519,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_POD_SHARD         0x80000u  /* sharded pods Allocate: pod records + ownership, gate, k_pods on the node window */
 #define DRA_K_POD_GATHER        0x100000u /* sharded pods Allocate: all-gather of the owned pods' records (world > 1) */
 #define DRA_K_PLACE             0x200000u /* place pods: pod states + pair records, persistent walk of the nodes' visit lists */
+#define DRA_K_PLACE_SHARD       0x400000u /* sharded place pods: prep, gate, walk of the node window, finalisers (+ all-gather) */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

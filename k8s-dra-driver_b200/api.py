@@ -22,7 +22,8 @@ KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x0
            "sorted_prep": 0x00010, "bucket_small": 0x00020, "hist8": 0x00040, "hist8_multi": 0x00080,
            "hist_warp": 0x00100, "scan8": 0x00200, "scan_rows": 0x00400, "scan": 0x00800, "scatter": 0x01000,
            "pack1": 0x02000, "pack4": 0x04000, "compact_flat1": 0x08000, "compact_flat8": 0x10000,
-           "compact_lookback": 0x20000, "compact_in_kernel": 0x40000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000}
+           "compact_lookback": 0x20000, "compact_in_kernel": 0x40000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000,
+           "place_shard": 0x400000}
 
 
 class DraError(RuntimeError):
@@ -73,6 +74,8 @@ SYMBOLS = {
     "dra_set_shard_pairs": (_i32, [_vp, _u32]),
     "dra_unsuitable_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _u32]),
     "dra_allocate_pods_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _u32, _u32]),
+    "dra_set_shard_place": (_i32, [_vp, _u32]),
+    "dra_place_pods_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _u32, _vp, _u32]),
     "dra_shard_sync_inventory_device": (_i32, [_vp]),
     "dra_deallocate_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_mps_limits_batch": (_i32, [_vp, _vp, _u32, _vp, _vp]),
@@ -417,6 +420,22 @@ class Context:
         F_FRESH_INVENTORY.  Enqueues, no synchronisation; errors found on the device surface at sync()."""
         self._check(self._lib.dra_allocate_pods_batch_global_device(self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod,
                                                                     _ptr(d_out_off), n_out, flags))
+
+    def set_shard_place(self, max_pods: int) -> None:
+        """Room for the sharded place-pods call's replicated pod states; world > 1: before shard_export, the same on every
+        rank."""
+        self._check(self._lib.dra_set_shard_place(self._h, max_pods))
+
+    def place_pods_global_device(self, d_claims: int, n_claim: int, d_pod_off: int, n_pod: int, d_cand_nodes: int | None,
+                                 d_cand_off: int | None, n_pair: int, d_out_off: int | None, n_out: int, d_pod_node: int,
+                                 flags: int = 0) -> None:
+        """Sharded place pods (spec §13): the SAME pods and candidates on every rank (device pointers); d_cand_nodes /
+        d_cand_off None and n_pair 0 = dense form.  Each rank evaluates the visits to its own nodes; every rank receives the
+        whole table (gather_read()) and the whole pod_node array, n_pod uint32 at d_pod_node.  flags: F_EXHAUSTIVE,
+        F_FRESH_INVENTORY.  Enqueues, no synchronisation; errors found on the device surface at sync()."""
+        self._check(self._lib.dra_place_pods_batch_global_device(self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod,
+                                                                 _ptr(d_cand_nodes), _ptr(d_cand_off), n_pair, _ptr(d_out_off),
+                                                                 n_out, _ptr(d_pod_node), flags))
 
     def shard_sync_inventory_device(self) -> None:
         """Every rank's live inventory becomes the world's state (each GPU as its owning rank holds it), so get_inventory()

@@ -185,6 +185,15 @@ struct dra_ctx {
     uint32_t* d_upair_pod = nullptr; size_t cap_upair_pod = 0;   // candidate form: pair -> pod (k_uns_prep)
     // sharded pods Allocate
     uint32_t* d_spod = nullptr;                 // [SP_WORDS] call words (dra_device.cuh SPodArgs)
+    // sharded place pods: a region [progress counter, 64 bytes][state words: u64 per pod] (dra_device.cuh PlaceShard) in
+    // the peer buffer at world > 1, in d_splace_local at world 1
+    uint32_t place_max_pods = 0;                // dra_set_shard_place, reserved by the next peer_setup
+    uint32_t peer_place_pods = 0; size_t off_splace = 0;
+    uint8_t* d_splace_local = nullptr; size_t cap_splace_local = 0;    // pods
+    uint32_t splace_seq = 0;                    // the last call's sequence number (peer_setup starts over: fresh words)
+    uint4* d_splace_rec = nullptr; size_t cap_splace_rec = 0;          // [n_pod] finaliser records for k_spod_gather
+    int splace_occ = -1;                        // resident CTAs of k_pods_place<4, true> per SM (occupancy query, once)
+    int peers_on_device = 1;                    // ranks whose contexts share this device (dra_peer_import_local)
     // inventory sync: records in the peer buffer ([staging x2: peer_inv_gpus records][flags[PEER_MAX], elect[2]])
     uint32_t peer_inv_gpus = 0;                 // n_gpu when the export ran (0: no inventory then)
     std::vector<uint32_t> h_node_off;           // host copy of the inventory's node_off: each rank's GPU range
@@ -666,6 +675,10 @@ int check_err(dra_ctx* ctx) {
     if (sp) return fail(ctx, DRA_E_STATE, "sharded call: %u claims fell into this shard, more than the launch was laid out for; nothing was changed, call again", ctx->h_sc_counts ? ctx->h_sc_counts[0] : 0u);
     if (dw) return fail(ctx, DRA_E_CUDA, "a device-side wait inside one kernel (grid barrier / look-back over CTAs) timed out: CTAs were not scheduled together; state is undefined, reload the inventory");
     if (bo) return fail(ctx, DRA_E_INVAL, "sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays; nothing was evaluated");
+    if (bp && (ctx->chain & DRA_K_PLACE_SHARD))
+        return fail(ctx, DRA_E_INVAL, "sharded place pods: pod_off / cand_off not monotone or not spanning their arrays, more than %u candidates for a pod, "
+                                      "a pod's OutRec slots outside n_out, or one rank's slots beyond the cap_per_rank of dra_shard_export; "
+                                      "no inventory was changed", PL_POS);
     if (bp) return fail(ctx, DRA_E_INVAL, "sharded pods Allocate: pod_off not monotone or not spanning [0, n_claim], a pod's OutRec slots outside n_out, "
                                           "or one rank's slots beyond the cap_per_rank of dra_shard_export; no inventory was changed");
     if (bd) return fail(ctx, DRA_E_INVAL, "sharded Deallocate: out_off/n_out: a claim's slots fall outside out[]; no record was applied, inventory unchanged");
@@ -875,7 +888,7 @@ void dra_ctx_destroy(dra_ctx* c) {
                    c->d_out, c->d_rank, c->d_hist, c->d_claim_off, c->d_pod_off, c->d_cand_off, c->d_cand_nodes,
                    c->d_pair_pod, c->d_bits, c->d_err, c->d_attrs, c->d_sels, c->d_podrec, c->d_cursor, c->d_cclaims, c->d_coff,
                    c->d_sc_status, c->d_sc_counts, c->d_gtable, c->d_rank_slots, c->d_sc_times, c->d_ubits, c->d_upair_pod, c->d_spod,
-                   c->d_place_state, c->d_place_node, c->d_place_cursor};
+                   c->d_place_state, c->d_place_node, c->d_place_cursor, c->d_splace_local, c->d_splace_rec};
     for (void* p : dev) if (p) cudaFree(p);
     for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
@@ -1426,7 +1439,7 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
         lc.attrs = at; lc.numAttrs = 1;
-        CU(cudaLaunchKernelEx(&lc, k_pods_place<4>, a));
+        CU(cudaLaunchKernelEx(&lc, k_pods_place<4>, a, PlaceShard{}));
         ctx->launches += 1;
     }
     ctx->chain |= DRA_K_PLACE;
@@ -1504,19 +1517,39 @@ namespace {
 // What a peer buffer's layout depends on.  Every rank computes its peers' offsets from its OWN layout, so an import requires
 // every rank to be set up alike; the export writes this at offset 0 of the buffer for importers in other processes to read.
 struct PeerLayout {
-    uint32_t world, rank, form, cap, tab_len, uns_pairs, inv_gpus, rsvd;
+    uint32_t world, rank, form, cap, tab_len, uns_pairs, inv_gpus, rsvd;      // rsvd: dra_set_shard_place's max_pods
     bool operator==(const PeerLayout& o) const { return memcmp(this, &o, sizeof o) == 0; }
 };
 PeerLayout layout_of(const dra_ctx* c, int rank) {
     PeerLayout l; memset(&l, 0, sizeof l);
     l.world = (uint32_t)c->world; l.rank = (uint32_t)rank; l.form = c->peer_form; l.cap = c->peer_cap; l.tab_len = c->peer_tab_len;
-    l.uns_pairs = c->peer_uns_pairs; l.inv_gpus = c->peer_inv_gpus;
+    l.uns_pairs = c->peer_uns_pairs; l.inv_gpus = c->peer_inv_gpus; l.rsvd = c->peer_place_pods;
     return l;
+}
+
+// Loads every kernel of the sharded place-pods chain now.  With lazy module loading (CUDA's default) the first launch of a
+// kernel loads it, and the load waits for the kernels running on the device.  A rank's walk waits for its peers' walks, so
+// a host thread that enqueues the ranks of one process one after the other would stall at rank 0's first launch after
+// the walk until the walk gives up.  Called while no call of the world is in flight.
+int preload_place_shard(dra_ctx* ctx) {
+    const void* ks[] = {(const void*)k_splace_prep, (const void*)k_spod_gate, (const void*)k_pods_place<4, true>,
+                        (const void*)k_splace_final, (const void*)k_spod_gather<true>, (const void*)k_bucket_small,
+                        (const void*)k_bucket_hist8<false>, (const void*)k_bucket_hist8<true>, (const void*)k_bucket_scan_rows,
+                        (const void*)k_bucket_scan8, (const void*)k_bucket_hist, (const void*)k_bucket_scan,
+                        (const void*)k_bucket_scatter};
+    for (const void* k : ks) { cudaFuncAttributes fa; CU(cudaFuncGetAttributes(&fa, k)); }
+    // An SM holds CTAs of one L1/shared split at a time.  With ranks on one device, a rank's walk (and its waiting gather)
+    // may sit on every SM while a peer's counting sort still has to run, and the sort's CTA-wide histogram wants most of
+    // the shared memory: the kernels that wait take the all-shared split too, so the sort's CTAs fit beside them.
+    const void* waiting[] = {(const void*)k_pods_place<4, true>, (const void*)k_spod_gather<true>};
+    for (const void* k : waiting) CU(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    return DRA_OK;
 }
 
 // (Re)allocates this rank's gather buffer:  [layout][table x2][staging x2: world slices of cap packets][headers x2][rendezvous flags]
 // and, after dra_set_shard_pairs(max_pairs > 0), [UnsuitableNodes staging x2: world slices of uns_stride words][their flags]
 // and, for dra_shard_export with an inventory loaded, [inventory staging x2: n_gpu records][their flags + election words]
+// and, after dra_set_shard_place(max_pods > 0), [place pods: progress counter, 64 bytes][max_pods state words of 8 bytes]
 int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, uint32_t cap) {
     if (ctx->world > (int)PEER_MAX) return fail(ctx, DRA_E_INVAL, "world %d > %u", ctx->world, PEER_MAX);
     CU(cudaSetDevice(ctx->device));
@@ -1551,6 +1584,17 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
     // the inventory sync's staging, sized for the inventory loaded now (sharded form only); its flags, then `elect` [2]
     ctx->peer_inv_gpus = form == 2 && ctx->d_inv_live ? ctx->n_gpu : 0u;
     if (ctx->peer_inv_gpus) reserve(ctx->isync_x, (size_t)ctx->peer_inv_gpus * 16, 0, (size_t)(PEER_MAX + 2) * 4);
+    // sharded place pods, after dra_set_shard_place: the replicated state words (zeroed below, so the sequence starts over)
+    ctx->peer_place_pods = ctx->place_max_pods;
+    if (ctx->peer_place_pods) {
+        ctx->off_splace = take(64 + (size_t)ctx->peer_place_pods * 8);
+        if (int rc = preload_place_shard(ctx)) return rc;
+        // the sort's scan-status words for the loaded inventory now: ensure_batch grows them with a cudaFree, which waits
+        // for the whole device — where, inside a call, a peer's walk may be waiting for this rank
+        if (ctx->d_inv_live) { if (int rc = ensure_batch(ctx, 1, 1, false)) return rc; }
+    }
+    ctx->splace_seq = 0;
+    if (ctx->d_splace_local) CU(cudaMemset(ctx->d_splace_local, 0, 64 + ctx->cap_splace_local * 8));
     ctx->peer_bytes = off;
     CU(cudaMalloc((void**)&ctx->peer_local, ctx->peer_bytes));
     CU(cudaMemset(ctx->peer_local, 0, ctx->peer_bytes));
@@ -1676,6 +1720,7 @@ int dra_peer_import(dra_ctx* ctx, const void* handles) {
         CU(cudaMemcpy(&theirs, p, sizeof theirs, cudaMemcpyDeviceToHost));
         if (!(theirs == layout_of(ctx, r))) return fail(ctx, DRA_E_INVAL, "dra_peer_import: rank %d is not set up like this one", r);
     }
+    ctx->peers_on_device = 1;
     ctx->peer_ready = true;
     return DRA_OK;
 }
@@ -1697,6 +1742,8 @@ int dra_peer_import_local(dra_ctx* ctx, dra_ctx* const* ctxs) {
         }
         ctx->peer_base[r] = o->peer_local; ctx->peer_ipc[r] = false;
     }
+    ctx->peers_on_device = 0;
+    for (int r = 0; r < ctx->world; ++r) ctx->peers_on_device += ctxs[r]->device == ctx->device ? 1 : 0;
     ctx->peer_ready = true;
     return DRA_OK;
 }
@@ -2040,11 +2087,162 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     if (gather) {
         // a small grid: it waits for its peers, and ranks sharing one device must not find their sort / k_pods SMs held by it
         const uint32_t blocks = std::max(1u, std::min((uint32_t)std::max(1, ctx->n_sm / 4), (std::max(n_pod, g.world * g.cap / 4u) + 255u) / 256u));
-        k_spod_gather<<<blocks, 256, 0, ctx->stream>>>(g, sa, ctx->peer_tab_len);
+        k_spod_gather<false><<<blocks, 256, 0, ctx->stream>>>(g, sa, ctx->peer_tab_len);
         ctx->launches += 1; ctx->chain |= DRA_K_POD_GATHER;
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded pods Allocate launch: %s", cudaGetErrorString(e));
+    ctx->gather_table = (const dra_out_rec*)table; ctx->gather_n_per = n_out; ctx->gather_len = n_out;
+    return DRA_OK;
+}
+
+int dra_set_shard_place(dra_ctx* ctx, uint32_t max_pods) {
+    if (!ctx) return DRA_E_INVAL;
+    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "dra_set_shard_place: call it before dra_shard_export");
+    if (max_pods > (1u << 26)) return fail(ctx, DRA_E_INVAL, "max_pods %u exceeds 2^26", max_pods);
+    ctx->place_max_pods = max_pods;
+    return DRA_OK;
+}
+
+// Sharded place pods: checks, initial state words, pair records and every rank's slot bound (k_splace_prep) -> gate / FRESH
+// copy (k_spod_gate) -> stable counting sort of the pairs by window node -> the persistent walk of the window's visit lists,
+// every state word published to every rank (k_pods_place<4, true>) -> pod_node and the finalisers' slots (k_splace_final) ->
+// expected counts (k_spod_gate) -> all-gather of the finalised pods' records (k_spod_gather<true>).  Enqueues only.
+int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                       const uint32_t* d_pod_off, uint32_t n_pod,
+                                       const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                       const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node, uint32_t flags) {
+    if (!ctx || !d_pod_off || (n_claim && !d_claims) || (n_pod && !d_pod_node)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~(DRA_F_EXHAUSTIVE | DRA_F_FRESH_INVENTORY))
+        return fail(ctx, DRA_E_INVAL, "dra_place_pods_batch_global_device: unknown flags 0x%x", flags);
+    if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
+    if (int rc = check_slots(ctx, n_claim, n_out, d_out_off != nullptr)) return rc;
+    if (!n_pod && n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]: no pods for %u claims", n_claim);
+    const bool dense = d_cand_nodes == nullptr && d_cand_off == nullptr;
+    if (!dense && (!d_cand_nodes || !d_cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
+    if (dense && n_pair) return fail(ctx, DRA_E_INVAL, "dense form: n_pair must be 0");
+    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
+    const bool gather = ctx->world > 1;
+    if (gather && !ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the walk and the gather need every rank's range)");
+    if (int rc = need_peers(ctx)) return rc;
+    if (gather && n_out > ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", n_out, ctx->peer_tab_len);
+    if (gather && n_pod > ctx->peer_place_pods)
+        return fail(ctx, DRA_E_STATE, "n_pod %u exceeds the max_pods (%u) of dra_set_shard_place before dra_shard_export", n_pod, ctx->peer_place_pods);
+    ctx->chain = ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
+    CU(cudaSetDevice(ctx->device));
+    // peers on this device may already wait for this rank: no buffer this call outgrows is freed before the next sync
+    struct DeferFree { dra_ctx* c; ~DeferFree() { c->defer_free = false; } } defer{ctx};
+    ctx->defer_free = gather;
+    int rc = upload_table(ctx);
+    if (rc) return rc;
+    const uint32_t n_win = ctx->shard_hi - ctx->shard_lo;
+    if ((rc = ensure_batch(ctx, std::max(n_pod, n_pair), 1, false))) return rc;
+    const Tiling t = tiling(n_pair, n_win, ctx->n_sm);                // the sort's tiles are laid out on the window
+    if ((rc = grow(ctx, ctx->d_hist, ctx->cap_hist, (size_t)t.n_tiles * (n_win + 1), 64))) return rc;
+    if ((size_t)n_pair + 8 > ctx->cap_podrec) {
+        const size_t cap = (size_t)n_pair + n_pair / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_podrec, ctx->cap_podrec, cap))) return rc;
+        ctx->cap_podrec = cap;
+    }
+    if ((rc = grow(ctx, ctx->d_splace_rec, ctx->cap_splace_rec, n_pod))) return rc;
+    if ((size_t)n_win + 8 > ctx->cap_place_cursor) {
+        const size_t cap = (size_t)n_win + n_win / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_place_cursor, ctx->cap_place_cursor, cap))) return rc;
+        ctx->cap_place_cursor = cap;
+    }
+    if (!gather && n_pod > ctx->cap_splace_local) {          // world 1: the state words in plain device memory, zeroed
+        const size_t cap = (size_t)n_pod + n_pod / 2 + 64;
+        if (ctx->d_splace_local) CU(cudaFree(ctx->d_splace_local));
+        ctx->d_splace_local = nullptr;
+        CU(cudaMalloc((void**)&ctx->d_splace_local, 64 + cap * 8));
+        CU(cudaMemsetAsync(ctx->d_splace_local, 0, 64 + cap * 8, ctx->stream));
+        ctx->cap_splace_local = cap;
+    }
+    if (!ctx->d_spod) CU(cudaMalloc((void**)&ctx->d_spod, SP_WORDS * 4));
+    uint2* table = nullptr; PktGather g; memset(&g, 0, sizeof g);
+    if ((rc = result_table(ctx, n_out, nullptr, g, table))) return rc;
+    if (gather) g.expect = ctx->d_spod + SP_EXPECT;
+    const Err err = err_of(ctx);
+    const bool fresh = (flags & DRA_F_FRESH_INVENTORY) != 0;
+    const uint32_t* d_node_off = ctx->d_node_off + ctx->shard_lo;
+
+    PlaceShard sh; memset(&sh, 0, sizeof sh);
+    for (int r = 0; r < (gather ? ctx->world : 1); ++r) {
+        uint8_t* base = gather ? ctx->peer_base[r] + ctx->off_splace : ctx->d_splace_local;
+        sh.prog[r] = (uint32_t*)base; sh.rep[r] = (unsigned long long*)(base + 64);
+    }
+    sh.gated = ctx->d_spod + SP_GATED; sh.w = ctx->d_spod; sh.podrec = ctx->d_splace_rec;
+    sh.world = gather ? (uint32_t)ctx->world : 1u; sh.rank = gather ? (uint32_t)ctx->rank : 0u; sh.seq = ++ctx->splace_seq;
+    sh.node_lo = ctx->shard_lo; sh.n_win = n_win;
+    sh.n_claim = n_claim; sh.n_pair = n_pair; sh.n_out = n_out;
+    for (uint32_t r = 0; r < sh.world; ++r) sh.rank_hi[r] = gather ? ctx->shard_bounds[r + 1] : ctx->n_node;
+    sh.spin_limit = ctx->peer_spin;
+    PlaceArgs a; memset(&a, 0, sizeof a);
+    a.claims = (const uint4*)d_claims; a.pod_off = d_pod_off; a.n_pod = n_pod;
+    a.cand_nodes = dense ? nullptr : d_cand_nodes; a.cand_off = dense ? nullptr : d_cand_off;
+    a.out_off = d_out_off; a.out = table; a.pod_node = d_pod_node; a.pairs = ctx->d_podrec;
+    a.sorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.cursor = ctx->d_place_cursor;
+    a.inv_src = ctx->d_inv_live; a.inv_dst = ctx->d_inv_live; a.node_off = d_node_off; a.tbl = ctx->d_tbl;
+    a.n_node = ctx->n_node; a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.sel = sel_of(ctx); a.err = err;
+    // the gate's SPodArgs: its record count is the sort's (the pairs), its world the one the bounds were counted for
+    SPodArgs sa; memset(&sa, 0, sizeof sa);
+    sa.claims = (const uint4*)d_claims; sa.pod_off = d_pod_off; sa.out_off = d_out_off;
+    sa.n_claim = n_claim; sa.n_pod = n_pod; sa.n_out = n_out; sa.n_node = ctx->n_node;
+    sa.node_lo = ctx->shard_lo; sa.node_hi = ctx->shard_hi; sa.rank = sh.rank; sa.world = sh.world;
+    sa.table = table; sa.podrec = ctx->d_splace_rec; sa.w = ctx->d_spod; sa.err = err;
+    SPodArgs sa_sort = sa; sa_sort.n_pod = dense ? 0u : n_pair;
+
+    Prof prof(ctx);
+    CU(cudaMemsetAsync(ctx->d_spod, 0, (SP_BAD + 1) * 4, ctx->stream));
+    if (n_out) CU(cudaMemsetAsync(table, 0, (size_t)n_out * 8, ctx->stream));
+    CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)n_win + 1) * 4, ctx->stream));
+    k_splace_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, ctx->stream>>>(a, sh);
+    const uint32_t gate_grid = fresh ? std::max(1u, std::min((uint32_t)ctx->n_sm, (ctx->n_gpu + 255) / 256)) : 1u;
+    k_spod_gate<<<gate_grid, 256, 0, ctx->stream>>>(sa_sort, gather ? ctx->peer_cap : 0u, fresh ? ctx->d_inv_pristine : nullptr,
+                                                    ctx->d_inv_live, ctx->d_node_off);
+    ctx->launches += 2;
+    if (!dense && n_pair && n_win &&
+        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, n_win, d_node_off,
+                          ctx->d_spod + SP_NDEV)))
+        return rc;
+    // The gate has read the bounds: k_splace_final counts the slots each rank really finalises in the same words.  (Zeroed
+    // before the walk: after it, this thread launches only kernels preload_place_shard loaded, since anything it waits for
+    // there would hold back the peers' calls that the walk waits for.)
+    CU(cudaMemsetAsync(ctx->d_spod, 0, PEER_MAX * 4, ctx->stream));
+    {
+        // Every CTA resident.  Ranks sharing this device run their walks side by side, so each takes its share of the
+        // residency, less one CTA per SM left for a peer's waiting gather kernel.  Not a cooperative launch: cooperative
+        // grids do not run beside each other, and a rank's walk waits for its peers' walks.
+        if (ctx->splace_occ < 0) {
+            int occ = 0;
+            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_place<4, true>, 128, 0));
+            ctx->splace_occ = occ;
+        }
+        if (ctx->splace_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_place<4, true>: no CTA can be resident");
+        const int k = gather ? std::max(1, ctx->peers_on_device) : 1;
+        const int per_sm = k > 1 ? std::max(1, ctx->splace_occ - 1) : ctx->splace_occ;
+        const uint32_t share = (uint32_t)std::max(1, per_sm * ctx->n_sm / k);
+        const uint32_t grid = std::max(1u, std::min((n_win + 3) / 4, share));
+        k_pods_place<4, true><<<grid, 128, 0, ctx->stream>>>(a, sh);
+        ctx->launches += 1;
+    }
+    k_splace_final<<<(n_pod + 255) / 256, 256, 0, ctx->stream>>>(a, sh);
+    ctx->launches += 1; ctx->chain |= DRA_K_PLACE_SHARD;
+    prof.mark();
+    if (gather) {
+        k_spod_gate<<<1, 256, 0, ctx->stream>>>(sa, ctx->peer_cap, nullptr, ctx->d_inv_live, ctx->d_node_off);
+        // a small grid: it waits for its peers, and ranks sharing one device must not find their walk's SMs held by it
+        const uint32_t blocks = std::max(1u, std::min((uint32_t)std::max(1, ctx->n_sm / 4), (std::max(n_pod, g.world * g.cap / 4u) + 255u) / 256u));
+        k_spod_gather<true><<<blocks, 256, 0, ctx->stream>>>(g, sa, ctx->peer_tab_len);
+        ctx->launches += 2;
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded place pods launch: %s", cudaGetErrorString(e));
     ctx->gather_table = (const dra_out_rec*)table; ctx->gather_n_per = n_out; ctx->gather_len = n_out;
     return DRA_OK;
 }

@@ -10,7 +10,8 @@
 //                    claim is tested on all GPUs at once, __ballot_sync + __ffs pick lowest GPU / lowest
 //                    start (first-fit), the winner lane updates its register-resident occupancy mask.
 //   k_unsuitable     one warp per (pod, candidate node) pair, same step function on a snapshot
-//   k_pods_place     place pods (spec §13): persistent, a warp walks each of its nodes' visit lists with a cursor
+//   k_pods_place     place pods (spec §13): persistent, a warp walks each of its nodes' visit lists with a cursor;
+//                    sharded (<4, true>): the rank's node window, pod states replicated on every rank (k_splace_*)
 //   k_dealloc        inverse updates with atomics (sharded: behind k_dealloc_check, on the rank's GPU range only)
 //
 // What this replaces in the reference: the per-node search behind Allocate()/UnsuitableNodes() that
@@ -2716,11 +2717,49 @@ struct PlaceArgs {
     uint32_t n_node, exhaustive; SelCtx sel; Err err;
 };
 
+// Sharded form (dra_place_pods_batch_global_device): each rank walks the visit lists of its own node window, and every
+// rank holds a REPLICA of every pod's state word.  A word is 64 bits, {call sequence : state}, and every publication is an
+// atomic max into every rank's replica.  Within a call a pod's state only grows (positions rise, the limit bit is sticky,
+// DONE is highest), and a word of an earlier call loses to any word of the current one, so a late or reordered delivery
+// never moves a word back and nothing is ever reset.  The final word is DONE plus the global node the pod was placed on,
+// or PL_NOWHERE.
+constexpr uint32_t PL_NOWHERE = 0xFFFFFFFFu;
+struct PlaceShard {
+    unsigned long long* rep[PEER_MAX];   // rep[r]: rank r's replica of the state words (rep[rank]: this rank's own)
+    uint32_t* prog[PEER_MAX];            // prog[r]: rank r's progress counter, +1 per publication anywhere, never reset
+    const uint32_t* gated;               // the call words' SP_GATED: nothing is evaluated
+    uint32_t* w;                         // the call words (SP_*): [r] slots rank r may finalise / finalises, SP_BAD
+    uint4* podrec;                       // [n_pod] {claims, -, first claim, finalising rank or SP_NONE} for k_spod_gather
+    uint32_t world, rank, seq;           // seq: this call's sequence number, the same on every rank
+    uint32_t node_lo, n_win;             // this rank's node window [node_lo, node_lo + n_win)
+    uint32_t n_claim, n_pair, n_out;     // what the device-side checks hold the arrays to
+    uint32_t rank_hi[PEER_MAX];          // rank r serves nodes [rank_hi[r-1], rank_hi[r])
+    long long spin_limit;                // cycles without a publication anywhere before ERR_PEER_TIMEOUT
+};
+
 __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
     uint32_t v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
 }
 __device__ __forceinline__ void st_release_u32(uint32_t* p, uint32_t v) {
     asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long ld_acquire_sys_u64(const unsigned long long* p) {
+    unsigned long long v; asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory"); return v;
+}
+__device__ __forceinline__ uint32_t ld_acquire_sys_u32(const uint32_t* p) {
+    uint32_t v; asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
+}
+__device__ __forceinline__ void red_max_release_sys_u64(unsigned long long* p, unsigned long long v) {
+    asm volatile("red.release.sys.global.max.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ void red_add_sys_u32(uint32_t* p, uint32_t v) {
+    asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+// the rank whose node range holds global node n
+__device__ __forceinline__ uint32_t place_owner(const PlaceShard& s, uint32_t n) {
+    uint32_t o = 0;
+    for (uint32_t q = 0; q + 1 < s.world; ++q) o += n >= s.rank_hi[q] ? 1u : 0u;
+    return o;
 }
 
 // The final records of a pod placed nowhere (warp-wide): INVALID for the claims invalid by §3/§10 (every claim when the
@@ -2771,25 +2810,33 @@ k_pods_place_prep(const PlaceArgs a) {
 }
 
 // Persistent: every CTA resident (cooperative launch); warp w owns nodes w, w + warps, ... and cycles over them.
-template <int WPC>
+// SHARD: the nodes are this rank's window (a.node_off, list_off and cursor are the window's; a.n_node is still the whole
+// inventory, for the next usable candidate), states come from this rank's replica and go to every rank's, and warp 0
+// stays until every pod's word here is DONE: a rank's own lists can end while pods still move on other ranks.  Launched
+// without the cooperative attribute (cooperative grids do not run beside each other), sized to the rank's share of the
+// residency.
+template <int WPC, bool SHARD = false>
 __global__ void __launch_bounds__(WPC * 32)
-k_pods_place(const PlaceArgs a) {
+k_pods_place(const PlaceArgs a, const PlaceShard sh) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
+    if constexpr (SHARD) { if (__ldcg(sh.gated)) return; }
     for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
     __syncthreads();
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t w0 = blockIdx.x * WPC + (threadIdx.x >> 5), n_warp = gridDim.x * WPC;
     const bool dense = a.cand_off == nullptr, have_off = a.out_off != nullptr;
+    const uint32_t n_walk = SHARD ? sh.n_win : a.n_node, node_base = SHARD ? sh.node_lo : 0u;
     if (a.inv_src != a.inv_dst)                              // DRA_F_FRESH_INVENTORY: the owner copies its nodes first
-        for (uint32_t node = w0; node < a.n_node; node += n_warp) {
+        for (uint32_t node = w0; node < n_walk; node += n_warp) {
             const uint32_t g0 = __ldg(&a.node_off[node]), ng = __ldg(&a.node_off[node + 1]) - g0;
             if (lane < ng) a.inv_dst[g0 + lane] = __ldg(&a.inv_src[g0 + lane]);
         }
     uint32_t seen = 0;
+    bool dead = false;
     long long t0 = clock64();
     while (true) {
         bool left = false, moved = false;
-        for (uint32_t node = w0; node < a.n_node; node += n_warp) {
+        for (uint32_t node = w0; node < n_walk; node += n_warp) {
             const uint32_t l0 = dense ? 0u : __ldcg(&a.list_off[node]), l1 = dense ? a.n_pod : __ldcg(&a.list_off[node + 1]);
             const uint32_t cur0 = l0 + __ldcg(&a.cursor[node]);
             uint32_t cur = cur0;
@@ -2802,9 +2849,10 @@ k_pods_place(const PlaceArgs a) {
                 const uint32_t e = cur + lane;
                 uint32_t q = 0, k = 0, s = PL_DONE;
                 if (e < l1) {
-                    if (dense) { q = e; k = node; }
+                    if (dense) { q = e; k = node + node_base; }
                     else { const uint4 r = __ldcg(&a.sorted[e]); q = r.x; k = r.z; }
-                    s = ld_acquire_u32(&a.state[q]);
+                    if constexpr (SHARD) s = (uint32_t)ld_acquire_sys_u64(&sh.rep[sh.rank][q]);
+                    else s = ld_acquire_u32(&a.state[q]);
                 }
                 const bool skip = (s & PL_DONE) || (s & PL_POS) > k;
                 const uint32_t act = __ballot_sync(FULLMASK, !skip);
@@ -2813,7 +2861,8 @@ k_pods_place(const PlaceArgs a) {
                 cur += f;
                 const uint32_t qf = __shfl_sync(FULLMASK, q, f), kf = __shfl_sync(FULLMASK, k, f), sf = __shfl_sync(FULLMASK, s, f);
                 if ((sf & PL_POS) < kf) break;                   // q may still come here: this node waits
-                (void)ld_acquire_u32(&a.state[qf]);              // every lane: ordered after the previous owner's records
+                if constexpr (SHARD) (void)ld_acquire_sys_u64(&sh.rep[sh.rank][qf]);
+                else (void)ld_acquire_u32(&a.state[qf]);         // every lane: ordered after the previous owner's records
                 if (!loaded) {
                     L.load(lane < ng ? a.inv_dst[g0 + lane] : make_uint4(0, 0, 0, 0), lane < ng);
                     loaded = true;
@@ -2830,7 +2879,7 @@ k_pods_place(const PlaceArgs a) {
                 const uint32_t lim = (sf & PL_LIMIT) | (st == DRA_ST_SEARCH_LIMIT ? PL_LIMIT : 0u);
                 if (st == 0) {
                     dirty = true;
-                    if (lane == 0) a.pod_node[qf] = node;
+                    if (!SHARD && lane == 0) a.pod_node[qf] = node;
                 } else {
                     // the pod's next candidate that names a node of the inventory
                     if (dense) { if (kf + 1u < a.n_node) next = (kf + 1u) | lim; }
@@ -2848,9 +2897,19 @@ k_pods_place(const PlaceArgs a) {
                         place_fail(a, c0, cnt, lim ? (uint32_t)DRA_ST_SEARCH_LIMIT : (uint32_t)DRA_ST_POD, lane);
                     }
                 }
-                __threadfence();
-                __syncwarp();
-                if (lane == 0) { st_release_u32(&a.state[qf], next); atomicAdd(&a.cursor[a.n_node], 1u); }
+                if constexpr (SHARD) {
+                    __threadfence_system();
+                    __syncwarp();
+                    if (lane == 0) {
+                        const uint32_t wd = st == 0 ? (PL_DONE | (node + node_base)) : next == PL_DONE ? PL_NOWHERE : next;
+                        const unsigned long long v = ((unsigned long long)sh.seq << 32) | wd;
+                        for (uint32_t r = 0; r < sh.world; ++r) { red_max_release_sys_u64(sh.rep[r] + qf, v); red_add_sys_u32(sh.prog[r], 1u); }
+                    }
+                } else {
+                    __threadfence();
+                    __syncwarp();
+                    if (lane == 0) { st_release_u32(&a.state[qf], next); atomicAdd(&a.cursor[a.n_node], 1u); }
+                }
                 moved = true;
                 ++cur;
             }
@@ -2861,11 +2920,32 @@ k_pods_place(const PlaceArgs a) {
         if (!left) break;
         if (moved) { t0 = clock64(); continue; }
         // nothing moved on this warp's nodes: back off, and give up when no pod was evaluated anywhere for a long time
-        // (cannot happen with every CTA resident)
+        // (cannot happen with every CTA resident; sharded: unless a peer stopped)
         __nanosleep(256);
-        const uint32_t pr = __shfl_sync(FULLMASK, ld_acquire_u32(&a.cursor[a.n_node]), 0);
+        const uint32_t pr = __shfl_sync(FULLMASK, SHARD ? ld_acquire_sys_u32(sh.prog[sh.rank]) : ld_acquire_u32(&a.cursor[a.n_node]), 0);
         if (pr != seen) { seen = pr; t0 = clock64(); }
-        else if (clock64() - t0 > 4000000000ll) { if (lane == 0) a.err.set(ERR_DEVICE_WAIT); break; }
+        else if (clock64() - t0 > (SHARD ? sh.spin_limit : 4000000000ll)) {
+            if (lane == 0) a.err.set(SHARD ? ERR_PEER_TIMEOUT : ERR_DEVICE_WAIT);
+            dead = true;
+            break;
+        }
+    }
+    if constexpr (SHARD) {
+        if (w0 != 0 || dead) return;
+        // every pod's word here DONE: then every evaluation of the call is over on every rank
+        t0 = clock64();
+        for (uint32_t p0 = 0; p0 < a.n_pod; ) {
+            bool done = true;
+            if (p0 + lane < a.n_pod) {
+                const unsigned long long v = ld_acquire_sys_u64(&sh.rep[sh.rank][p0 + lane]);
+                done = (uint32_t)(v >> 32) == sh.seq && ((uint32_t)v & PL_DONE);
+            }
+            if (__all_sync(FULLMASK, done)) { p0 += 32; continue; }
+            __nanosleep(256);
+            const uint32_t pr = __shfl_sync(FULLMASK, ld_acquire_sys_u32(sh.prog[sh.rank]), 0);
+            if (pr != seen) { seen = pr; t0 = clock64(); }
+            else if (clock64() - t0 > sh.spin_limit) { if (lane == 0) a.err.set(ERR_PEER_TIMEOUT); break; }
+        }
     }
 }
 
@@ -3194,6 +3274,11 @@ __device__ __forceinline__ uint32_t pod_claim_slots(const uint4 c, uint32_t n_no
     const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
     return (kind == DRA_KIND_GPU && c.y < n_node && !claim_invalid(kind, prof, count, have_off)) ? count : 1u;
 }
+// ... and as place pods counts them (spec §13): as if the claim named a node of the inventory, whatever its node field
+__device__ __forceinline__ uint32_t place_claim_slots(const uint4 c, bool have_off) {
+    const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
+    return (kind == DRA_KIND_GPU && !claim_invalid(kind, prof, count, have_off)) ? count : 1u;
+}
 
 // thread per pod, every pod: the checks of k_pod_records plus the device-side ones (pod_off monotone and spanning
 // [0, n_claim]) — those set SP_BAD instead of failing one pod, since every rank sees the same arrays
@@ -3276,6 +3361,8 @@ k_spod_gate(const SPodArgs a, uint32_t cap, const uint4* __restrict__ inv_src, u
 // A rank with nothing to send — it owns no slot, or the call is gated — sends one packet addressed to the table's padding
 // slot pad_slot instead (k_spod_gate expects it): each call is then a real exchange with every peer, so no rank gets two
 // calls ahead of a peer still reading the staging slices of the same parity.
+// ANY_NODE (sharded place pods): a claim's node field is ignored, slots are counted as if it named a node (spec §13).
+template <bool ANY_NODE = false>
 __global__ void __launch_bounds__(256)
 k_spod_gather(const PktGather g, const SPodArgs a, uint32_t pad_slot) {
     const uint32_t T = blockIdx.x * blockDim.x + threadIdx.x, NT = gridDim.x * blockDim.x;
@@ -3289,18 +3376,126 @@ k_spod_gather(const PktGather g, const SPodArgs a, uint32_t pad_slot) {
         uint4 rec = make_uint4(0u, SP_NONE, 0u, SP_NONE);
         if (p < n_pod) rec = __ldcg(&a.podrec[p]);
         const bool mine = rec.w == g.rank;
+        auto slots = [&](uint32_t i) {
+            const uint4 c = __ldg(&a.claims[i]);
+            return ANY_NODE ? place_claim_slots(c, have_off) : pod_claim_slots(c, a.n_node, have_off);
+        };
         uint32_t sl = 0;
-        if (mine) for (uint32_t i = rec.z; i < rec.z + rec.x; ++i) sl += pod_claim_slots(__ldg(&a.claims[i]), a.n_node, have_off);
+        if (mine) for (uint32_t i = rec.z; i < rec.z + rec.x; ++i) sl += slots(i);
         uint32_t pos = pkt_warp_reserve(g, sl);
         if (!mine) continue;
         for (uint32_t i = rec.z; i < rec.z + rec.x; ++i) {
-            const uint32_t s = pod_claim_slots(__ldg(&a.claims[i]), a.n_node, have_off);
+            const uint32_t s = slots(i);
             const uint32_t dst = have_off ? __ldg(&a.out_off[i]) : i;
             for (uint32_t k = 0; k < s; ++k, ++pos)
                 if (pos < g.cap) pkt_send(g, pos, __ldcg(&g.table[dst + k]), dst + k);
         }
     }
     pkt_receive(g, T, NT, a.err);
+}
+
+// ====================================================================================================
+// sharded place pods (dra_place_pods_batch_global_device): every rank reads the WHOLE pod and candidate arrays
+// ====================================================================================================
+// k_splace_prep -> k_spod_gate -> counting sort of the pairs on the window -> k_pods_place<4, true> -> k_splace_final ->
+// k_spod_gate (expected counts) -> k_spod_gather<true>.  The call words are SPodArgs' (zeroed by the host up to SP_BAD).
+
+// Warp per pod, every pod: the device-side checks (pod_off and cand_off monotone and spanning their arrays, at most PL_POS
+// candidates, slots inside n_out — a fault sets SP_BAD and the pod writes nothing); the pod's initial state word, maxed into
+// this rank's replica (a peer may already have moved it further in this call); the pair records keyed by WINDOW node (a
+// candidate on another rank's node, or naming no node, gets none and the sort drops it); the final records of the pods that
+// are never evaluated, which every rank writes alike into its own table; and, world > 1, the slots of every pod that has a
+// usable candidate in rank r's range added to w[r] — an upper bound of what r can finalise, checked against the packet room
+// by k_spod_gate before anything is placed.
+__global__ void __launch_bounds__(256)
+k_splace_prep(const PlaceArgs a, const PlaceShard sh) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (p >= a.n_pod) return;
+    const bool dense = a.cand_off == nullptr, have_off = a.out_off != nullptr;
+    const uint32_t c0 = __ldg(&a.pod_off[p]), c1 = __ldg(&a.pod_off[p + 1]);
+    bool fault = c1 < c0 || c1 > sh.n_claim || (p == 0 && (c0 != 0 || __ldg(&a.pod_off[a.n_pod]) != sh.n_claim));
+    uint32_t k0 = 0, nk = 0;
+    if (!dense) {
+        const uint32_t k1 = __ldg(&a.cand_off[p + 1]);
+        k0 = __ldg(&a.cand_off[p]);
+        fault = fault || k1 < k0 || k1 > sh.n_pair || k1 - k0 > PL_POS || (p == 0 && (k0 != 0 || __ldg(&a.cand_off[a.n_pod]) != sh.n_pair));
+        nk = k1 - k0;
+    }
+    uint32_t total = 0;
+    if (!fault)
+        for (uint32_t i = c0 + lane; i < c1; i += 32) {
+            const uint32_t slots = place_claim_slots(__ldg(&a.claims[i]), have_off), dst = have_off ? __ldg(&a.out_off[i]) : i;
+            fault = fault || dst > sh.n_out || slots > sh.n_out - dst;
+            total += slots;
+        }
+    if (__any_sync(FULLMASK, fault)) {
+        if (lane == 0) { sh.w[SP_BAD] = 1u; a.err.set(ERR_BAD_PODS); }
+        return;
+    }
+    total = __reduce_add_sync(FULLMASK, total);
+    const uint32_t cnt = c1 - c0;
+    const bool live = cnt != 0 && cnt <= DRA_MAX_POD;
+    uint32_t first = PL_DONE, owners = 0;
+    if (dense) {
+        if (a.n_node) first = 0;
+        if (lane < sh.world && (lane ? sh.rank_hi[lane - 1] : 0u) < sh.rank_hi[lane]) owners = 1u << lane;
+    } else {
+        for (uint32_t j0 = 0; j0 < nk; j0 += 32) {
+            const uint32_t j = j0 + lane;
+            const uint32_t n = j < nk ? __ldg(&a.cand_nodes[k0 + j]) : 0xFFFFFFFFu;
+            const bool usable = n < a.n_node;
+            if (j < nk) a.pairs[k0 + j] = make_uint4(p, live && usable && n - sh.node_lo < sh.n_win ? n - sh.node_lo : 0xFFFFFFFFu, j, 0);
+            const uint32_t b = __ballot_sync(FULLMASK, usable);
+            if (b && first == PL_DONE) first = j0 + (uint32_t)__ffs(b) - 1u;
+            if (usable) owners |= 1u << place_owner(sh, n);
+        }
+    }
+    owners = __reduce_or_sync(FULLMASK, owners);
+    const bool walks = live && first != PL_DONE;
+    if (lane == 0) atomicMax(&sh.rep[sh.rank][p], ((unsigned long long)sh.seq << 32) | (walks ? first : PL_NOWHERE));
+    if (cnt != 0 && !walks) place_fail(a, c0, cnt, live ? (uint32_t)DRA_ST_POD : (uint32_t)DRA_ST_INVALID, lane);
+    if (walks && sh.world > 1 && lane < sh.world && ((owners >> lane) & 1u)) atomicAdd(&sh.w[lane], total);
+}
+
+// Thread per pod, after the walk (every word here is DONE): pod_node from the final word, and the pod's FINALISER — the
+// rank that wrote its final records: the owner of the node it was placed on; placed nowhere, the owner of its last usable
+// candidate (its last evaluation); never evaluated, none (every rank wrote those).  podrec and, world > 1, every
+// finaliser's slots in w[r] (zeroed by the host after the first gate): the packets k_spod_gather sends and expects.
+__global__ void __launch_bounds__(256)
+k_splace_final(const PlaceArgs a, const PlaceShard sh) {
+    __shared__ uint32_t rs_s[PEER_MAX];
+    const uint32_t tid = threadIdx.x, p = blockIdx.x * blockDim.x + tid;
+    if (tid < PEER_MAX) rs_s[tid] = 0;
+    __syncthreads();
+    if (p < a.n_pod) {
+        const bool gated = __ldcg(sh.gated) != 0;
+        uint32_t node = DRA_GPU_NONE, fin = SP_NONE, c0 = 0, cnt = 0;
+        if (!gated) {
+            c0 = __ldg(&a.pod_off[p]); cnt = __ldg(&a.pod_off[p + 1]) - c0;
+            const unsigned long long v = __ldcg(&sh.rep[sh.rank][p]);
+            const uint32_t wd = (uint32_t)v;
+            const bool final_ = (uint32_t)(v >> 32) == sh.seq && (wd & PL_DONE);    // (not after ERR_PEER_TIMEOUT)
+            if (final_ && (wd & ~PL_DONE) < a.n_node) { node = wd & ~PL_DONE; fin = place_owner(sh, node); }
+            else if (final_ && cnt != 0 && cnt <= DRA_MAX_POD) {
+                if (!a.cand_off) { if (a.n_node) fin = place_owner(sh, a.n_node - 1); }
+                else
+                    for (uint32_t j = __ldg(&a.cand_off[p + 1]), k0 = __ldg(&a.cand_off[p]); j > k0; --j) {
+                        const uint32_t n = __ldg(&a.cand_nodes[j - 1]);
+                        if (n < a.n_node) { fin = place_owner(sh, n); break; }
+                    }
+            }
+            if (fin != SP_NONE && sh.world > 1) {
+                uint32_t total = 0;
+                for (uint32_t i = c0; i < c0 + cnt; ++i) total += place_claim_slots(__ldg(&a.claims[i]), a.out_off != nullptr);
+                atomicAdd(&rs_s[fin], total);
+            }
+        }
+        a.pod_node[p] = node;
+        sh.podrec[p] = make_uint4(cnt, SP_NONE, c0, fin);
+    }
+    __syncthreads();
+    if (sh.world > 1 && tid < sh.world && rs_s[tid]) atomicAdd(&sh.w[tid], rs_s[tid]);
 }
 
 // ====================================================================================================
