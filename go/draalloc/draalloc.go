@@ -237,6 +237,99 @@ func (c *Context) PlacePodsBatch(claims []ClaimRec, podOff []uint32, cands, cand
 	return out, podNode, nil
 }
 
+// Running pods for PreemptBatch: the arrays DeallocateBatch takes for their allocations (outOff nil: slot i), split into
+// pods by PodOff, one priority per pod.  Pod index order is start order, earliest first.
+type RunningPods struct {
+	Claims []ClaimRec
+	PodOff []uint32
+	Prio   []int32
+	OutOff []uint32
+	Out    []OutRec
+}
+
+// Preemption answer (spec §14).  Per pair: Status (DRA_PRE_*) and, for EVICT, the victim count.  Per pod: the node to
+// evict on (0xFFFFFFFF: none), its status, the full victim count and the first maxVictims victims as running-pod indices
+// (row p at Victims[p*maxVictims:], padded with 0xFFFFFFFF).
+type Preemption struct {
+	PairStatus  []uint8
+	PairVictims []uint32
+	PodNode     []uint32
+	PodStatus   []uint8
+	NVictims    []uint32
+	Victims     []uint32
+}
+
+// PreemptBatch answers kube-scheduler's PostFilter for pods whose GPU claims fit nowhere (dra_preempt_batch, spec §14):
+// per candidate node the lower-priority running pods to evict, and per pod the node to evict them on.  Pure: the
+// inventory is not written.  cands == candOff == nil: every node, ascending (nNode: the inventory's node count, which
+// sizes the per-pair outputs of that form).  Unbuilt, like the rest of this file.
+func (c *Context) PreemptBatch(claims []ClaimRec, podOff []uint32, prio []int32, cands, candOff []uint32, nNode int,
+	run RunningPods, maxVictims int, flags uint32) (*Preemption, error) {
+	nPod := len(podOff) - 1
+	if nPod <= 0 || len(run.PodOff) == 0 {
+		return &Preemption{}, nil
+	}
+	nPair := nPod * nNode
+	var cn, co *C.uint32_t
+	if candOff != nil {
+		nPair = int(candOff[nPod])
+		co = (*C.uint32_t)(unsafe.Pointer(&candOff[0]))
+		if len(cands) == 0 {
+			cands = []uint32{0} // an empty list still needs an address (nil means the dense form)
+		}
+		cn = (*C.uint32_t)(unsafe.Pointer(&cands[0]))
+	}
+	r := &Preemption{make([]uint8, nPair+1), make([]uint32, nPair+1), make([]uint32, nPod), make([]uint8, nPod),
+		make([]uint32, nPod), make([]uint32, nPod*maxVictims+1)}
+	var cp, rcp *C.dra_claim_rec
+	if len(claims) > 0 {
+		cp = (*C.dra_claim_rec)(unsafe.Pointer(&claims[0]))
+	}
+	if len(run.Claims) > 0 {
+		rcp = (*C.dra_claim_rec)(unsafe.Pointer(&run.Claims[0]))
+	}
+	var rp *C.int32_t
+	if len(run.Prio) > 0 {
+		rp = (*C.int32_t)(unsafe.Pointer(&run.Prio[0]))
+	}
+	var roo *C.uint32_t
+	if run.OutOff != nil {
+		roo = (*C.uint32_t)(unsafe.Pointer(&run.OutOff[0]))
+	}
+	var rop *C.dra_out_rec
+	if len(run.Out) > 0 {
+		rop = (*C.dra_out_rec)(unsafe.Pointer(&run.Out[0]))
+	}
+	// the struct handed to C holds Go pointers: cgo accepts that only for pinned memory
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, q := range []unsafe.Pointer{unsafe.Pointer(rcp), unsafe.Pointer(&run.PodOff[0]), unsafe.Pointer(rp),
+		unsafe.Pointer(roo), unsafe.Pointer(rop)} {
+		if q != nil {
+			pin.Pin(q)
+		}
+	}
+	cr := C.dra_running_pods{claims: rcp, n_claim: C.uint32_t(len(run.Claims)),
+		pod_off: (*C.uint32_t)(unsafe.Pointer(&run.PodOff[0])), n_pod: C.uint32_t(len(run.PodOff) - 1), prio: rp,
+		out_off: roo, out: rop, n_out: C.uint32_t(len(run.Out))}
+	var vp *C.uint32_t
+	if maxVictims > 0 {
+		vp = (*C.uint32_t)(unsafe.Pointer(&r.Victims[0]))
+	}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_preempt_batch(c.h, cp, C.uint32_t(len(claims)), (*C.uint32_t)(unsafe.Pointer(&podOff[0])),
+		(*C.int32_t)(unsafe.Pointer(&prio[0])), C.uint32_t(nPod), cn, co, &cr,
+		(*C.uint8_t)(unsafe.Pointer(&r.PairStatus[0])), (*C.uint32_t)(unsafe.Pointer(&r.PairVictims[0])),
+		(*C.uint32_t)(unsafe.Pointer(&r.PodNode[0])), (*C.uint8_t)(unsafe.Pointer(&r.PodStatus[0])),
+		(*C.uint32_t)(unsafe.Pointer(&r.NVictims[0])), vp, C.uint32_t(maxVictims), C.uint32_t(flags))
+	if rc != 0 {
+		return nil, lastError(c.h)
+	}
+	r.PairStatus, r.PairVictims, r.Victims = r.PairStatus[:nPair], r.PairVictims[:nPair], r.Victims[:nPod*maxVictims]
+	return r, nil
+}
+
 func (c *Context) DeallocateBatch(claims []ClaimRec, outOff []uint32, out []OutRec) error {
 	if len(claims) == 0 {
 		return nil

@@ -282,6 +282,44 @@ int  dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
                           const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
                           uint32_t* pod_node, uint32_t flags);
 
+/* Preemption (spec §14): for pods that fit nowhere, which lower-priority running pods to evict on each candidate node,
+ * and which node to evict them on — kube-scheduler's DefaultPreemption (SelectVictimsOnNode, pickOneNodeForPreemption)
+ * without PodDisruptionBudgets.  Pure: nothing is written to the inventory. */
+#define DRA_PRE_FITS         0u   /* the pod fits on the node as it is: no victims */
+#define DRA_PRE_EVICT        1u   /* the pod fits once the victims are gone */
+#define DRA_PRE_NO           2u   /* it does not fit even with every lower-priority pod gone (or: no such node) */
+#define DRA_PRE_SEARCH_LIMIT 3u   /* an evaluation ran out of DRA_EXH_BUDGET */
+#define DRA_PRE_INVALID      4u   /* more than DRA_MAX_POD claims, or a claim invalid by §3/§10 */
+
+/* The running pods: the allocations the live inventory holds, as dra_deallocate_batch takes them (claims, out_off or
+ * NULL, out[n_out]), split into pods by pod_off[n_pod+1].  Pod index order is start order, earliest first. */
+typedef struct dra_running_pods {
+    const dra_claim_rec* claims; uint32_t n_claim;
+    const uint32_t* pod_off;     uint32_t n_pod;     /* n_pod + 1 entries */
+    const int32_t*  prio;                             /* n_pod */
+    const uint32_t* out_off;                          /* NULL: slot i, as dra_deallocate_batch */
+    const dra_out_rec* out;      uint32_t n_out;
+} dra_running_pods;
+
+/* Pending pods as in dra_place_pods_batch (claims, pod_off, candidates or the dense form; each claim's node field is
+ * ignored), with priority prio[p].  Per pair (n_pair = cand_off[n_pod], dense n_pod * n_node), each may be NULL:
+ *   pair_status[k]   DRA_PRE_*          pair_victims[k]  victims of an EVICT pair, else 0
+ * Per pod:
+ *   pod_node[p]      the node chosen (FITS or EVICT), else 0xFFFFFFFF      pod_status[p]  DRA_PRE_*
+ *   n_victims[p]     the chosen pair's victim count (always the full count)
+ *   victims[p * max_victims + k]  its first min(n_victims[p], max_victims) victims as running-pod indices, in eviction
+ *                    order (priority descending, then index); the rest of the row 0xFFFFFFFF.
+ * DRA_E_INVAL with nothing written: unknown flags, pod_off / cand_off / running->pod_off not monotone or not spanning,
+ * dense n_pod * n_node >= 2^32, a running slot range outside running->n_out, a running pod whose OK slots name a GPU
+ * index >= n_gpu or GPUs of two nodes, max_victims > 0 without victims.  Host buffers; flags: 0 or DRA_F_EXHAUSTIVE. */
+int  dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
+                       const uint32_t* pod_off, const int32_t* prio, uint32_t n_pod,
+                       const uint32_t* cand_nodes, const uint32_t* cand_off,
+                       const dra_running_pods* running,
+                       uint8_t* pair_status, uint32_t* pair_victims,
+                       uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
+                       uint32_t* victims, uint32_t max_victims, uint32_t flags);
+
 /* Deallocate(): stands in for controller.Driver.Deallocate(ctx, claim).  Inverse update from the
  * claims and the OutRecs dra_allocate_batch produced for them (same out_off convention). */
 int  dra_deallocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
@@ -520,6 +558,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_POD_GATHER        0x100000u /* sharded pods Allocate: all-gather of the owned pods' records (world > 1) */
 #define DRA_K_PLACE             0x200000u /* place pods: pod states + pair records, persistent walk of the nodes' visit lists */
 #define DRA_K_PLACE_SHARD       0x400000u /* sharded place pods: prep, gate, walk of the node window, finalisers (+ all-gather) */
+#define DRA_K_PREEMPT           0x800000u /* preemption: running-pod prep, victim lists, pairs, choice, victim rows */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

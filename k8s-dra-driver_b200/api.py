@@ -17,13 +17,14 @@ SO_PATH = os.path.join(_HERE, "libdra_alloc.so")
 OK, E_INVAL, E_CUDA, E_NCCL, E_NOMEM, E_STATE = 0, -1, -2, -3, -4, -5
 CFG_USE_GRAPH, CFG_NO_FUSED, CFG_NO_DIRECT, CFG_RESIDENT = 0x1, 0x2, 0x4, 0x8
 F_NODE_SORTED, F_FRESH_INVENTORY, F_EXHAUSTIVE = 0x1, 0x2, 0x4
+PRE_FITS, PRE_EVICT, PRE_NO, PRE_SEARCH_LIMIT, PRE_INVALID = 0, 1, 2, 3, 4     # dra_preempt_batch statuses (spec §14)
 # DRA_K_*: the kernels an Allocate-family call enqueued (dra_debug_last_chain)
 KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x00004, "serve": 0x00008,
            "sorted_prep": 0x00010, "bucket_small": 0x00020, "hist8": 0x00040, "hist8_multi": 0x00080,
            "hist_warp": 0x00100, "scan8": 0x00200, "scan_rows": 0x00400, "scan": 0x00800, "scatter": 0x01000,
            "pack1": 0x02000, "pack4": 0x04000, "compact_flat1": 0x08000, "compact_flat8": 0x10000,
            "compact_lookback": 0x20000, "compact_in_kernel": 0x40000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000,
-           "place_shard": 0x400000}
+           "place_shard": 0x400000, "preempt": 0x800000}
 
 
 class DraError(RuntimeError):
@@ -35,6 +36,12 @@ class DraError(RuntimeError):
 class _Cfg(C.Structure):
     _fields_ = [("abi_version", C.c_uint32), ("device", C.c_int32), ("stream", C.c_void_p),
                 ("max_claims", C.c_uint32), ("flags", C.c_uint32)]
+
+
+class RunningPods(C.Structure):
+    """dra_running_pods: the running pods of dra_preempt_batch (spec §14)."""
+    _fields_ = [("claims", C.c_void_p), ("n_claim", C.c_uint32), ("pod_off", C.c_void_p), ("n_pod", C.c_uint32),
+                ("prio", C.c_void_p), ("out_off", C.c_void_p), ("out", C.c_void_p), ("n_out", C.c_uint32)]
 
 
 # every symbol include/dra_alloc.h declares: name -> (restype, argtypes)
@@ -57,6 +64,7 @@ SYMBOLS = {
     "dra_allocate_pods_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _u32]),
     "dra_place_pods_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u32]),
     "dra_deallocate_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
+    "dra_preempt_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32]),
     "dra_comm_unique_id": (_i32, [_vp]),
     "dra_comm_init": (_i32, [_vp, _vp, _i32, _i32]),
     "dra_allocate_batch_gather_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _u32, _u32]),
@@ -321,6 +329,44 @@ class Context:
         self._check(self._lib.dra_unsuitable_batch(self._h, _ptr(c), len(c), _ptr(po), len(po) - 1,
                                                    _ptr(cn), _ptr(co), _ptr(bits), flags))
         return bits[: (n_pair + 7) // 8]
+
+    def preempt(self, claims, pod_off, prio, run_claims, run_pod_off, run_prio, run_out, run_out_off=None,
+                cand_nodes=None, cand_off=None, max_victims: int = 8, flags: int = 0):
+        """Preemption (spec §14): for each pending pod, the lower-priority running pods to evict on each candidate node and
+        the node to evict them on.  The running pods are the arrays dra_deallocate_batch takes (run_claims, run_out,
+        run_out_off) split by run_pod_off, index order = start order.  cand_nodes/cand_off None = every node, ascending.
+        Returns (pair_status, pair_victims, pod_node, pod_status, n_victims, victims); victims is [n_pod, max_victims]
+        with 0xFFFFFFFF past the end of a row, n_victims the full count."""
+        c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
+        po = np.ascontiguousarray(pod_off, dtype=np.uint32)
+        pr = np.ascontiguousarray(prio, dtype=np.int32)
+        n_pod = len(po) - 1
+        rc_ = np.ascontiguousarray(run_claims, dtype=R.CLAIM_DTYPE)
+        rpo = np.ascontiguousarray(run_pod_off, dtype=np.uint32)
+        rpr = np.ascontiguousarray(run_prio, dtype=np.int32)
+        ro = np.ascontiguousarray(run_out, dtype=R.OUT_DTYPE)
+        roo = None if run_out_off is None else np.ascontiguousarray(run_out_off, dtype=np.uint32)
+        cn = co = None
+        if cand_nodes is not None or cand_off is not None:
+            co = np.ascontiguousarray(cand_off, dtype=np.uint32)
+            cn = np.ascontiguousarray(cand_nodes if cand_nodes is not None else [], dtype=np.uint32)
+            if len(cn) == 0:
+                cn = np.zeros(1, np.uint32)            # NULL would mean the dense form
+        n_pair = n_pod * self.n_node if co is None else int(co[-1])
+        run = RunningPods(rc_.ctypes.data, len(rc_), rpo.ctypes.data, len(rpo) - 1, rpr.ctypes.data,
+                          None if roo is None else roo.ctypes.data, ro.ctypes.data, len(ro))
+        pair_status = np.zeros(max(n_pair, 1), dtype=np.uint8)
+        pair_victims = np.zeros(max(n_pair, 1), dtype=np.uint32)
+        pod_node = np.zeros(max(n_pod, 1), dtype=np.uint32)
+        pod_status = np.zeros(max(n_pod, 1), dtype=np.uint8)
+        n_victims = np.zeros(max(n_pod, 1), dtype=np.uint32)
+        victims = np.zeros(max(n_pod * max_victims, 1), dtype=np.uint32)
+        self._check(self._lib.dra_preempt_batch(self._h, _ptr(c), len(c), _ptr(po), _ptr(pr), n_pod, _ptr(cn), _ptr(co),
+                                                C.byref(run), _ptr(pair_status), _ptr(pair_victims), _ptr(pod_node),
+                                                _ptr(pod_status), _ptr(n_victims), _ptr(victims) if max_victims else None,
+                                                max_victims, flags))
+        return (pair_status[:n_pair], pair_victims[:n_pair], pod_node[:n_pod], pod_status[:n_pod], n_victims[:n_pod],
+                victims[:n_pod * max_victims].reshape(n_pod, max_victims))
 
     def deallocate(self, claims, out, out_off=None):
         c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)

@@ -101,6 +101,15 @@ struct dra_ctx {
     uint32_t *d_place_state = nullptr, *d_place_node = nullptr; size_t cap_place_pods = 0;   // place pods: per pod
     uint32_t* d_place_cursor = nullptr; size_t cap_place_cursor = 0;                          // place pods: per node (+ 1)
     int place_occ = -1;                   // resident CTAs of k_pods_place<4> per SM (occupancy query, once)
+    // preemption (spec §14): per pending pod, per pair, the running pods and the victim rows
+    uint32_t *d_pre_prio = nullptr, *d_pre_node = nullptr, *d_pre_nvic = nullptr, *d_pre_choice = nullptr; uint8_t* d_pre_pst = nullptr;
+    size_t cap_pre_pods = 0;
+    uint4* d_pre_psum = nullptr; unsigned long long* d_pre_psum64 = nullptr; uint8_t* d_pre_pairst = nullptr;
+    uint32_t* d_pre_pairvic = nullptr; size_t cap_pre_pairs = 0;
+    uint4* d_pre_rclaims = nullptr; uint32_t* d_pre_routoff = nullptr; size_t cap_pre_rclaims = 0;
+    uint32_t *d_pre_rpodoff = nullptr, *d_pre_rprio = nullptr; uint4 *d_pre_rrec = nullptr, *d_pre_vlist = nullptr; size_t cap_pre_rpods = 0;
+    uint2* d_pre_rout = nullptr; size_t cap_pre_rout = 0;
+    uint32_t* d_pre_vic = nullptr; size_t cap_pre_vic = 0;
 
     // error flags
     uint32_t* d_err = nullptr;            // device memory
@@ -245,6 +254,11 @@ int grow_nc(dra_ctx* ctx, T*& p, size_t have_cap, size_t new_cap) {   // compani
     CU(cudaMalloc((void**)&p, new_cap * sizeof(T)));
     ctx->state_epoch++;
     return DRA_OK;
+}
+
+template <class T>
+int grow_pre(dra_ctx* ctx, T*& p, size_t need) {            // a buffer of the preemption call, capacity tracked by the caller
+    return grow_nc(ctx, p, 0, need + need / 2 + 64);
 }
 
 int grow_pinned(dra_ctx* ctx, uint8_t*& p, size_t& cap, size_t need) {
@@ -674,6 +688,9 @@ int check_err(dra_ctx* ctx) {
     cudaStreamSynchronize(ctx->stream);
     if (sp) return fail(ctx, DRA_E_STATE, "sharded call: %u claims fell into this shard, more than the launch was laid out for; nothing was changed, call again", ctx->h_sc_counts ? ctx->h_sc_counts[0] : 0u);
     if (dw) return fail(ctx, DRA_E_CUDA, "a device-side wait inside one kernel (grid barrier / look-back over CTAs) timed out: CTAs were not scheduled together; state is undefined, reload the inventory");
+    if (bo && (ctx->chain & DRA_K_PREEMPT))
+        return fail(ctx, DRA_E_INVAL, "dra_preempt_batch: running pods: pod_off not monotone or not spanning the claims, a slot range outside "
+                                      "n_out, or OK slots naming a GPU index >= n_gpu or GPUs of two nodes; nothing was written");
     if (bo) return fail(ctx, DRA_E_INVAL, "sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays; nothing was evaluated");
     if (bp && (ctx->chain & DRA_K_PLACE_SHARD))
         return fail(ctx, DRA_E_INVAL, "sharded place pods: pod_off / cand_off not monotone or not spanning their arrays, more than %u candidates for a pod, "
@@ -888,7 +905,10 @@ void dra_ctx_destroy(dra_ctx* c) {
                    c->d_out, c->d_rank, c->d_hist, c->d_claim_off, c->d_pod_off, c->d_cand_off, c->d_cand_nodes,
                    c->d_pair_pod, c->d_bits, c->d_err, c->d_attrs, c->d_sels, c->d_podrec, c->d_cursor, c->d_cclaims, c->d_coff,
                    c->d_sc_status, c->d_sc_counts, c->d_gtable, c->d_rank_slots, c->d_sc_times, c->d_ubits, c->d_upair_pod, c->d_spod,
-                   c->d_place_state, c->d_place_node, c->d_place_cursor, c->d_splace_local, c->d_splace_rec};
+                   c->d_place_state, c->d_place_node, c->d_place_cursor, c->d_splace_local, c->d_splace_rec,
+                   c->d_pre_prio, c->d_pre_node, c->d_pre_nvic, c->d_pre_choice, c->d_pre_pst, c->d_pre_psum, c->d_pre_psum64,
+                   c->d_pre_pairst, c->d_pre_pairvic, c->d_pre_rclaims, c->d_pre_routoff, c->d_pre_rpodoff, c->d_pre_rprio,
+                   c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic};
     for (void* p : dev) if (p) cudaFree(p);
     for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
@@ -1452,6 +1472,202 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     if ((rc = check_err(ctx))) return rc;
     if (rb) memcpy(out, ctx->h_out, rb);
     memcpy(pod_node, ctx->h_out + rb, qb);
+    return DRA_OK;
+}
+
+// Preemption (spec §14): the pending-pod arrays are checked here; the running pods on the device (k_pre_running), whose
+// fault gates every later kernel.  Inputs are staged in, the kernels launched, the outputs copied back after ONE
+// synchronise, and the caller's buffers are written only when no fault was found.
+int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, const int32_t* prio,
+                      uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, const dra_running_pods* running,
+                      uint8_t* pair_status, uint32_t* pair_victims, uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
+                      uint32_t* victims, uint32_t max_victims, uint32_t flags) {
+    if (!ctx || !pod_off || !running || !running->pod_off || (n_claim && !claims) || (n_pod && (!prio || !pod_node || !pod_status || !n_victims)))
+        return DRA_E_INVAL;
+    const dra_running_pods& R = *running;
+    if ((R.n_claim && !R.claims) || (R.n_pod && !R.prio) || (R.n_out && !R.out)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_preempt_batch: unknown flags 0x%x", flags);
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (max_victims && !victims) return fail(ctx, DRA_E_INVAL, "max_victims %u without a victims buffer", max_victims);
+    if (pod_off[0] != 0 || pod_off[n_pod] != n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]");
+    for (uint32_t q = 0; q < n_pod; ++q)
+        if (pod_off[q + 1] < pod_off[q]) return fail(ctx, DRA_E_INVAL, "pod_off not monotone at pod %u", q);
+    const bool dense = cand_nodes == nullptr && cand_off == nullptr;
+    if (!dense && !cand_off) return fail(ctx, DRA_E_INVAL, "cand_nodes without cand_off");
+    if (!dense && cand_off[0] != 0) return fail(ctx, DRA_E_INVAL, "cand_off[0] must be 0");
+    for (uint32_t q = 0; !dense && q < n_pod; ++q)
+        if (cand_off[q + 1] < cand_off[q]) return fail(ctx, DRA_E_INVAL, "cand_off not monotone at pod %u", q);
+    const uint64_t n_pair64 = dense ? (uint64_t)n_pod * ctx->n_node : cand_off[n_pod];
+    if (dense && n_pair64 >= (1ull << 32)) return fail(ctx, DRA_E_INVAL, "dense form: n_pod * n_node must stay below 2^32");
+    const uint32_t n_pair = (uint32_t)n_pair64;
+    if (n_pair && !dense && !cand_nodes) return fail(ctx, DRA_E_INVAL, "cand_off lists candidates but cand_nodes is NULL");
+    ctx->chain = DRA_K_PREEMPT; ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;
+    CU(cudaSetDevice(ctx->device));
+    int rc = ensure_batch(ctx, std::max(n_claim, R.n_pod), 1, true);
+    if (rc) return rc;
+    if ((rc = upload_table(ctx))) return rc;
+    if (n_pod + 8 > ctx->cap_pods) {
+        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_pod_off, 0, cap))) return rc;
+        if ((rc = grow_nc(ctx, ctx->d_cand_off, 0, cap))) return rc;
+        ctx->cap_pods = cap;
+    }
+    if (!dense && (size_t)n_pair + 64 > ctx->cap_pairs) {
+        size_t cap = (size_t)n_pair + n_pair / 2 + 128;
+        if ((rc = grow_nc(ctx, ctx->d_cand_nodes, 0, cap))) return rc;
+        if ((rc = grow_nc(ctx, ctx->d_pair_pod, 0, cap))) return rc;
+        ctx->cap_pairs = cap;
+    }
+    if ((size_t)n_pod + 8 > ctx->cap_pre_pods) {
+        const size_t need = (size_t)n_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_prio, need)) || (rc = grow_pre(ctx, ctx->d_pre_node, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_nvic, need)) || (rc = grow_pre(ctx, ctx->d_pre_choice, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_pst, need))) return rc;
+        ctx->cap_pre_pods = need + need / 2 + 64;
+    }
+    if ((size_t)n_pair + 8 > ctx->cap_pre_pairs) {
+        const size_t need = (size_t)n_pair + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_psum, need)) || (rc = grow_pre(ctx, ctx->d_pre_psum64, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_pairst, need)) || (rc = grow_pre(ctx, ctx->d_pre_pairvic, need))) return rc;
+        ctx->cap_pre_pairs = need + need / 2 + 64;
+    }
+    if ((size_t)R.n_claim + 8 > ctx->cap_pre_rclaims) {
+        const size_t need = (size_t)R.n_claim + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rclaims, need)) || (rc = grow_pre(ctx, ctx->d_pre_routoff, need))) return rc;
+        ctx->cap_pre_rclaims = need + need / 2 + 64;
+    }
+    if ((size_t)R.n_pod + 8 > ctx->cap_pre_rpods) {
+        const size_t need = (size_t)R.n_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rpodoff, need)) || (rc = grow_pre(ctx, ctx->d_pre_rprio, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_rrec, need)) || (rc = grow_pre(ctx, ctx->d_pre_vlist, need))) return rc;
+        ctx->cap_pre_rpods = need + need / 2 + 64;
+    }
+    if ((size_t)R.n_out + 8 > ctx->cap_pre_rout) {
+        const size_t need = (size_t)R.n_out + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rout, need))) return rc;
+        ctx->cap_pre_rout = need + need / 2 + 64;
+    }
+    const size_t vb = (size_t)n_pod * max_victims * 4;
+    if (vb / 4 + 8 > ctx->cap_pre_vic) {
+        const size_t need = vb / 4 + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_vic, need))) return rc;
+        ctx->cap_pre_vic = need + need / 2 + 64;
+    }
+    // staging: claims | pod_off | prio | cand_off | cand_nodes | pair -> pod | running claims | pod_off | prio | out_off | out
+    auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    const size_t cb = al((size_t)n_claim * 16), pb = al(((size_t)n_pod + 1) * 4), prb = al((size_t)n_pod * 4);
+    const size_t kb = dense ? 0 : al(((size_t)n_pod + 1) * 4), nb = dense ? 0 : al((size_t)n_pair * 4);
+    const size_t rcb = al((size_t)R.n_claim * 16), rpb = al(((size_t)R.n_pod + 1) * 4), rprb = al((size_t)R.n_pod * 4);
+    const size_t rob = R.out_off ? al((size_t)R.n_claim * 4) : 0, routb = al((size_t)R.n_out * 8);
+    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + prb + kb + 2 * nb + rcb + rpb + rprb + rob + routb + 16))) return rc;
+    uint8_t* h = ctx->h_in;
+    auto put = [&](const void* src, size_t bytes, size_t room) { uint8_t* d = h; if (bytes) memcpy(d, src, bytes); h += room; return d; };
+    uint8_t* h_c = put(claims, (size_t)n_claim * 16, cb);
+    uint8_t* h_po = put(pod_off, ((size_t)n_pod + 1) * 4, pb);
+    uint8_t* h_pr = put(prio, (size_t)n_pod * 4, prb);
+    uint8_t* h_co = dense ? nullptr : put(cand_off, ((size_t)n_pod + 1) * 4, kb);
+    uint8_t* h_cn = dense ? nullptr : put(cand_nodes, (size_t)n_pair * 4, nb);
+    uint8_t* h_pp = dense ? nullptr : put(nullptr, 0, nb);
+    for (uint32_t q = 0; !dense && q < n_pod; ++q)
+        for (uint32_t k = cand_off[q]; k < cand_off[q + 1]; ++k) ((uint32_t*)h_pp)[k] = q;
+    uint8_t* h_rc = put(R.claims, (size_t)R.n_claim * 16, rcb);
+    uint8_t* h_rpo = put(R.pod_off, ((size_t)R.n_pod + 1) * 4, rpb);
+    uint8_t* h_rpr = put(R.prio, (size_t)R.n_pod * 4, rprb);
+    uint8_t* h_roo = R.out_off ? put(R.out_off, (size_t)R.n_claim * 4, rob) : nullptr;
+    uint8_t* h_ro = put(R.out, (size_t)R.n_out * 8, routb);
+    cudaStream_t st = ctx->stream;
+    if (n_claim) CU(cudaMemcpyAsync(ctx->d_claims, h_c, (size_t)n_claim * 16, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pod_off, h_po, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pre_prio, h_pr, (size_t)n_pod * 4, cudaMemcpyHostToDevice, st));
+    if (!dense) {
+        CU(cudaMemcpyAsync(ctx->d_cand_off, h_co, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
+        if (n_pair) {
+            CU(cudaMemcpyAsync(ctx->d_cand_nodes, h_cn, (size_t)n_pair * 4, cudaMemcpyHostToDevice, st));
+            CU(cudaMemcpyAsync(ctx->d_pair_pod, h_pp, (size_t)n_pair * 4, cudaMemcpyHostToDevice, st));
+        }
+    }
+    if (R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_rclaims, h_rc, (size_t)R.n_claim * 16, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pre_rpodoff, h_rpo, ((size_t)R.n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (R.n_pod) CU(cudaMemcpyAsync(ctx->d_pre_rprio, h_rpr, (size_t)R.n_pod * 4, cudaMemcpyHostToDevice, st));
+    if (h_roo && R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_routoff, h_roo, (size_t)R.n_claim * 4, cudaMemcpyHostToDevice, st));
+    if (R.n_out) CU(cudaMemcpyAsync(ctx->d_pre_rout, h_ro, (size_t)R.n_out * 8, cudaMemcpyHostToDevice, st));
+
+    PreArgs a; memset(&a, 0, sizeof a);
+    a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.prio = (const int32_t*)ctx->d_pre_prio; a.n_pod = n_pod;
+    a.cand_nodes = dense ? nullptr : ctx->d_cand_nodes; a.cand_off = dense ? nullptr : ctx->d_cand_off;
+    a.pair_pod = dense ? nullptr : ctx->d_pair_pod; a.n_pair = n_pair;
+    a.rclaims = ctx->d_pre_rclaims; a.rn_claim = R.n_claim; a.rpod_off = ctx->d_pre_rpodoff; a.rprio = (const int32_t*)ctx->d_pre_rprio;
+    a.rn_pod = R.n_pod; a.rout_off = R.out_off ? ctx->d_pre_routoff : nullptr; a.rout = ctx->d_pre_rout; a.rn_out = R.n_out;
+    a.rrec = ctx->d_pre_rrec; a.rsorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.vlist = ctx->d_pre_vlist;
+    a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.n_gpu = ctx->n_gpu; a.tbl = ctx->d_tbl;
+    a.sel = sel_of(ctx); a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
+    a.psum = ctx->d_pre_psum; a.psum64 = ctx->d_pre_psum64;
+    a.pair_status = pair_status ? ctx->d_pre_pairst : nullptr; a.pair_victims = pair_victims ? ctx->d_pre_pairvic : nullptr;
+    a.pod_node = ctx->d_pre_node; a.pod_status = ctx->d_pre_pst; a.n_victims = ctx->d_pre_nvic; a.choice = ctx->d_pre_choice;
+    a.victims = ctx->d_pre_vic; a.max_victims = max_victims;
+    a.gate = ctx->d_err + ERR_BAD_OFFSETS; a.err = err_of(ctx);
+    if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, st)); }
+    a.work = ctx->d_ticket + 13;
+    CU(cudaMemsetAsync(a.work, 0, 4, st));
+    Prof prof(ctx);
+    k_pre_running<<<std::max(1u, (R.n_pod + 255) / 256), 256, 0, st>>>(a);
+    ctx->launches += 1;
+    if (R.n_pod) {
+        if ((rc = launch_sort(ctx, ctx->d_pre_rrec, R.n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, ctx->n_node, ctx->d_node_off)))
+            return rc;
+    } else {
+        CU(cudaMemsetAsync(ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, st));
+    }
+    const uint32_t W = ctx->max_width <= 8 ? 8u : (ctx->max_width <= 16 ? 16u : 32u);
+    if (ctx->n_node) {
+        k_pre_vsort<<<std::min(ctx->n_node, (uint32_t)ctx->n_sm * 8u), 256, 0, st>>>(a);
+        ctx->launches += 1;
+    }
+    if (n_pair) {
+        const uint32_t per_cta = 8 * (32 / W);
+        const uint32_t grid = std::max(1u, std::min((n_pair + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
+        if (W == 8) k_pods_preempt<8, 8><<<grid, 256, 0, st>>>(a);
+        else if (W == 16) k_pods_preempt<8, 16><<<grid, 256, 0, st>>>(a);
+        else k_pods_preempt<8, 32><<<grid, 256, 0, st>>>(a);
+        ctx->launches += 1;
+    }
+    k_pre_choose<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a);
+    ctx->launches += 1;
+    if (max_victims) {
+        CU(cudaMemsetAsync(ctx->d_pre_vic, 0xFF, vb, st));
+        const uint32_t per_cta = 8 * (32 / W);
+        const uint32_t grid = std::max(1u, std::min((n_pod + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
+        if (W == 8) k_pods_preempt_victims<8, 8><<<grid, 256, 0, st>>>(a);
+        else if (W == 16) k_pods_preempt_victims<8, 16><<<grid, 256, 0, st>>>(a);
+        else k_pods_preempt_victims<8, 32><<<grid, 256, 0, st>>>(a);
+        ctx->launches += 1;
+    }
+    prof.mark();
+    // outputs: pair_status | pair_victims | pod_node | pod_status | n_victims | victims
+    const size_t osb = pair_status ? al(n_pair) : 0, ovb = pair_victims ? al((size_t)n_pair * 4) : 0;
+    const size_t onb = al((size_t)n_pod * 4), opb = al(n_pod), ocb = al((size_t)n_pod * 4);
+    if ((rc = grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, osb + ovb + onb + opb + ocb + vb + 16))) return rc;
+    uint8_t* o = ctx->h_out;
+    if (osb && n_pair) CU(cudaMemcpyAsync(o, ctx->d_pre_pairst, n_pair, cudaMemcpyDeviceToHost, st));
+    if (ovb && n_pair) CU(cudaMemcpyAsync(o + osb, ctx->d_pre_pairvic, (size_t)n_pair * 4, cudaMemcpyDeviceToHost, st));
+    uint8_t* o2 = o + osb + ovb;
+    CU(cudaMemcpyAsync(o2, ctx->d_pre_node, (size_t)n_pod * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(o2 + onb, ctx->d_pre_pst, n_pod, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(o2 + onb + opb, ctx->d_pre_nvic, (size_t)n_pod * 4, cudaMemcpyDeviceToHost, st));
+    if (vb) CU(cudaMemcpyAsync(o2 + onb + opb + ocb, ctx->d_pre_vic, vb, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "preemption kernels: %s", cudaGetErrorString(e));
+    collect_timings(ctx, 1);
+    if ((rc = check_err(ctx))) return rc;
+    if (pair_status && n_pair) memcpy(pair_status, o, n_pair);
+    if (pair_victims && n_pair) memcpy(pair_victims, o + osb, (size_t)n_pair * 4);
+    memcpy(pod_node, o2, (size_t)n_pod * 4);
+    memcpy(pod_status, o2 + onb, n_pod);
+    memcpy(n_victims, o2 + onb + opb, (size_t)n_pod * 4);
+    if (vb) memcpy(victims, o2 + onb + opb + ocb, vb);
     return DRA_OK;
 }
 

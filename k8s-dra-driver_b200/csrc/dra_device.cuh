@@ -12,6 +12,7 @@
 //   k_unsuitable     one warp per (pod, candidate node) pair, same step function on a snapshot
 //   k_pods_place     place pods (spec §13): persistent, a warp walks each of its nodes' visit lists with a cursor;
 //                    sharded (<4, true>): the rank's node window, pod states replicated on every rank (k_splace_*)
+//   k_pods_preempt   preemption (spec §14): per (pod, candidate) pair, W lanes, the victims by remove-all-then-reprieve
 //   k_dealloc        inverse updates with atomics (sharded: behind k_dealloc_check, on the rank's GPU range only)
 //
 // What this replaces in the reference: the per-node search behind Allocate()/UnsuitableNodes() that
@@ -3529,6 +3530,290 @@ k_imex_offsets(const int* __restrict__ used, const uint32_t* __restrict__ dom_of
         if (freeb) found = base + ((int)__ffs(freeb) - 1) * step;
     }
     if (lane == 0) out[dom] = found;
+}
+
+// ====================================================================================================
+// Preemption (spec §14): per (pending pod, candidate node) pair, which lower-priority running pods to evict — remove every
+// one of them, then reprieve them from the most important down (kube-scheduler's SelectVictimsOnNode) — and per pod the
+// node to evict them on (pickOneNodeForPreemption).  Pure: the inventory is read, never written.
+//   k_pre_running   thread per running pod: checks its offsets and slots, finds its node, writes its record
+//   (bucketing)     the records grouped by node with the stable counting sort of the claim path
+//   k_pre_vsort     CTA per node: the node's list by priority descending, index ascending (rank by counting)
+//   k_pods_preempt  W lanes per pair, one per GPU of the node: dry pod_eval, remove V, pod_eval, the reprieve loop
+//   k_pre_choose    warp per pod: the pod's pairs reduced in list order
+//   k_pods_preempt_victims  W lanes per pod: the reprieve of the chosen pair again, this time writing the victims
+// ====================================================================================================
+struct PreArgs {
+    const uint4* claims; const uint32_t* pod_off; const int32_t* prio; uint32_t n_pod;
+    const uint32_t* cand_nodes; const uint32_t* cand_off; const uint32_t* pair_pod;   // cand_off == nullptr: dense form
+    uint32_t n_pair;
+    const uint4* rclaims; uint32_t rn_claim; const uint32_t* rpod_off; const int32_t* rprio; uint32_t rn_pod;
+    const uint32_t* rout_off; const uint2* rout; uint32_t rn_out;
+    uint4* rrec;                  // [rn_pod] {claims, node or NONE, first claim, prio}: what the bucketing kernels sort
+    const uint4* rsorted;         // rrec grouped by node (stable; .y replaced by the running-pod index), node n's at list_off[n]
+    const uint32_t* list_off;
+    uint4* vlist;                 // each node's list by priority descending, then index: {claims, index, first claim, prio}
+    const uint4* inv; const uint32_t* node_off; uint32_t n_node, n_gpu; const uint32_t* tbl; SelCtx sel;
+    uint32_t exhaustive;
+    uint4* psum;                  // [n_pair] {status, victims, highest victim priority, running index of the first victim}
+    unsigned long long* psum64;   // [n_pair] sum over the victims of (priority + 2^31)
+    uint8_t* pair_status; uint32_t* pair_victims;                   // caller's per-pair outputs (may be nullptr)
+    uint32_t* pod_node; uint8_t* pod_status; uint32_t* n_victims; uint32_t* choice;
+    uint32_t* victims; uint32_t max_victims;
+    uint32_t* work;               // next unclaimed pair (zeroed by the host)
+    const uint32_t* gate;         // non-zero: the running pods failed their check, nothing is evaluated
+    Err err;
+};
+
+// Thread per running pod.  Its node is the node of the GPUs its OK slots name (slots counted as §9 counts them); a pod
+// without an OK slot is on no node.  Offsets not monotone or not spanning, a slot range outside rn_out, a GPU index
+// >= n_gpu or GPUs of two nodes set ERR_BAD_OFFSETS, which gates every kernel after the sort.
+__global__ void __launch_bounds__(256)
+k_pre_running(const PreArgs a) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r == 0 && (__ldg(&a.rpod_off[0]) != 0 || __ldg(&a.rpod_off[a.rn_pod]) != a.rn_claim)) a.err.set(ERR_BAD_OFFSETS);
+    if (r >= a.rn_pod) return;
+    const uint32_t c0 = __ldg(&a.rpod_off[r]), c1 = __ldg(&a.rpod_off[r + 1]);
+    const bool have_off = a.rout_off != nullptr;
+    uint32_t node = DRA_GPU_NONE;
+    bool bad = c1 < c0 || c1 > a.rn_claim;
+    for (uint32_t i = c0; !bad && i < c1; ++i) {
+        const uint4 c = __ldg(&a.rclaims[i]);
+        const uint32_t base = have_off ? __ldg(&a.rout_off[i]) : i, slots = dealloc_slots(c, a.n_node, have_off);
+        if (base > a.rn_out || slots > a.rn_out - base) { bad = true; break; }
+        for (uint32_t k = 0; k < slots; ++k) {
+            const uint2 o = __ldg(&a.rout[base + k]);
+            if ((o.y >> 24) != DRA_ST_OK) continue;
+            if (o.x >= a.n_gpu) { bad = true; break; }
+            const uint32_t n = __ldg(&a.inv[o.x]).z;
+            if (node == DRA_GPU_NONE) node = n;
+            else if (node != n) { bad = true; break; }
+        }
+    }
+    if (bad) { a.err.set(ERR_BAD_OFFSETS); node = DRA_GPU_NONE; }
+    a.rrec[r] = make_uint4(bad ? 0u : c1 - c0, node, c0, (uint32_t)__ldg(&a.rprio[r]));
+}
+
+// CTA per node: the node's running pods (index order after the stable bucketing) ranked by (priority descending, index
+// ascending), a total order, so each pod's rank is the number of pods before it.  Quadratic in the pods of one node.
+__global__ void __launch_bounds__(256)
+k_pre_vsort(const PreArgs a) {
+    if (__ldcg(a.gate)) return;
+    for (uint32_t n = blockIdx.x; n < a.n_node; n += gridDim.x) {
+        const uint32_t l0 = __ldcg(&a.list_off[n]), l1 = __ldcg(&a.list_off[n + 1]);
+        for (uint32_t e = l0 + threadIdx.x; e < l1; e += blockDim.x) {
+            const uint4 me = __ldcg(&a.rsorted[e]);
+            uint32_t rank = 0;
+            for (uint32_t f = l0; f < l1; ++f) {
+                const uint4 o = __ldcg(&a.rsorted[f]);
+                rank += ((int32_t)o.w > (int32_t)me.w || ((int32_t)o.w == (int32_t)me.w && o.y < me.y)) ? 1u : 0u;
+            }
+            a.vlist[l0 + rank] = me;
+        }
+    }
+}
+
+// Running pod v = {claims, -, first claim, -} applied to this lane's GPU (global index gidx, NONE for a lane without one):
+// add = the Allocate updates, else their §9 inverse, in the records' u16 / u32 arithmetic.
+__device__ __forceinline__ void pre_apply(Lane& L, const PreArgs& a, const uint4 v, const uint32_t gidx, const bool add) {
+    const bool have_off = a.rout_off != nullptr;
+    for (uint32_t i = v.z; i < v.z + v.x; ++i) {
+        const uint4 c = __ldg(&a.rclaims[i]);
+        const uint32_t kind = c.x & 0xFFu;
+        const uint32_t base = have_off ? __ldg(&a.rout_off[i]) : i, slots = dealloc_slots(c, a.n_node, have_off);
+        for (uint32_t k = 0; k < slots; ++k) {
+            const uint2 o = __ldg(&a.rout[base + k]);
+            if ((o.y >> 24) != DRA_ST_OK || o.x != gidx) continue;
+            if (kind == DRA_KIND_GPU) {
+                L.flags = add ? (L.flags | DRA_GPU_FULL_ALLOCATED) : (L.flags & ~(uint32_t)DRA_GPU_FULL_ALLOCATED);
+            } else if (kind == DRA_KIND_MIG) {
+                const uint32_t start = o.y & 0xFFu, size = (o.y >> 8) & 0xFFu;
+                const uint32_t m = start >= 16u ? 0u : (((size >= 16u ? 0xFFFFu : (1u << size) - 1u) << start) & 0xFFFFu);
+                L.busy = add ? (L.busy | m) : (L.busy & ~m);
+            } else if (kind == DRA_KIND_SHARED) {
+                L.mem = add ? L.mem - c.z : L.mem + c.z;
+                L.share = (add ? L.share + 1u : L.share - 1u) & 0xFFFFu;
+            }
+        }
+    }
+}
+
+struct PreSum { uint32_t st, count, hi, hi_idx; unsigned long long sum; };
+
+// Pair (pod, node) on the W lanes gbase.. of the warp.  skip_first: the pair is known to be EVICT (k_pods_preempt_victims), so the
+// evaluation on the node as it is and the validity check are left out.  row: where the victims go (lane gbase writes).
+template <int W>
+__device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __restrict__ tbl_s, const uint32_t pod,
+                                           const uint32_t node, const uint32_t lane, const uint32_t gmask, const uint32_t gbase,
+                                           const bool skip_first, uint32_t* row) {
+    PreSum s{DRA_PRE_NO, 0u, 0x80000000u, 0xFFFFFFFFu, 0ull};
+    if (node >= a.n_node) return s;
+    const uint32_t c0 = __ldg(&a.pod_off[pod]), cnt = __ldg(&a.pod_off[pod + 1]) - c0;
+    if (cnt > DRA_MAX_POD) { s.st = DRA_PRE_INVALID; return s; }
+    const uint32_t gl = lane - gbase;
+    const uint32_t g0 = __ldg(&a.node_off[node]), ng = __ldg(&a.node_off[node + 1]) - g0;
+    if (ng > W) return s;                                             // cannot happen: W is chosen from the inventory
+    const uint32_t gidx = gl < ng ? g0 + gl : DRA_GPU_NONE;
+    Lane L; L.load(gl < ng ? __ldg(&a.inv[g0 + gl]) : make_uint4(0, 0, 0, 0), gl < ng);
+    const PodGet get{a.claims + c0, nullptr, 0};
+    const bool exh = a.exhaustive != 0;
+    uint32_t st1 = DRA_ST_POD;
+    Lane Lt;                                                          // ONE copy handed to every pod_eval: one stack slot
+    if (!skip_first) {
+        Lt = L;
+        st1 = pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr);
+        if (st1 == 0) { s.st = DRA_PRE_FITS; return s; }
+        bool inv = false;
+        for (uint32_t i = gl; i < cnt; i += W) {
+            const uint4 c = get(i);
+            const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
+            inv = inv || claim_invalid(kind, prof, count, true) || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
+        }
+        if (__ballot_sync(gmask, inv) & gmask) { s.st = DRA_PRE_INVALID; return s; }
+    }
+    // V: the tail of the node's list below the pod's priority (the list is by priority descending)
+    const int32_t P = __ldg(&a.prio[pod]);
+    uint32_t v0 = __ldcg(&a.list_off[node]), hi = __ldcg(&a.list_off[node + 1]);
+    const uint32_t v1 = hi;
+    while (v0 < hi) {
+        const uint32_t mid = (v0 + hi) >> 1;
+        if ((int32_t)__ldcg(&a.vlist[mid]).w >= P) v0 = mid + 1; else hi = mid;
+    }
+    if (v0 == v1) { s.st = st1 == DRA_ST_SEARCH_LIMIT ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO; return s; }   // S' = S
+    for (uint32_t v = v0; v < v1; ++v) pre_apply(L, a, __ldcg(&a.vlist[v]), gidx, false);
+    {
+        Lt = L;
+        const uint32_t st = pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr);
+        if (st != 0) { s.st = st == DRA_ST_SEARCH_LIMIT ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO; return s; }
+    }
+    s.st = DRA_PRE_EVICT;
+    for (uint32_t v = v0; v < v1; ++v) {                            // the reprieve, most important first
+        const uint4 r = __ldcg(&a.vlist[v]);
+        Lane Lk = L;
+        pre_apply(Lk, a, r, gidx, true);
+        Lt = Lk;
+        if (pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr) == 0) { L = Lk; continue; }
+        if (s.count == 0) { s.hi = r.w; s.hi_idx = r.y; }            // V order: the first victim has the highest priority
+        s.sum += (unsigned long long)((long long)(int32_t)r.w + 2147483648ll);
+        if (row && s.count < a.max_victims && lane == gbase) row[s.count] = r.y;
+        ++s.count;
+    }
+    return s;
+}
+
+// W lanes per (pod, candidate) pair, 32/W pairs per warp, in k_unsuitable's layout; pairs are taken from a counter, since
+// a pair costs from one evaluation to |V| + 2 of them.
+template <int WPC, int W>
+__global__ void __launch_bounds__(WPC * 32, 2)
+k_pods_preempt(const PreArgs a) {
+    __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
+    if (__ldcg(a.gate)) return;
+    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
+    __syncthreads();
+    constexpr uint32_t G = 32 / W;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t grp = lane / W, gbase = grp * W;
+    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
+    while (true) {
+        uint32_t nxt = 0;
+        if (lane == 0) nxt = atomicAdd(a.work, G);
+        const uint32_t pw = __shfl_sync(FULLMASK, nxt, 0);
+        if (pw >= a.n_pair) break;
+        const uint32_t pair = pw + grp;
+        if (pair >= a.n_pair) continue;                                  // whole group skips together
+        uint32_t pod, node;
+        if (!a.cand_off) { pod = pair / a.n_node; node = pair - pod * a.n_node; }
+        else { pod = __ldg(&a.pair_pod[pair]); node = __ldg(&a.cand_nodes[pair]); }
+        const PreSum s = pre_pair<W>(a, tbl_s, pod, node, lane, gmask, gbase, false, nullptr);
+        if (lane == gbase) {
+            a.psum[pair] = make_uint4(s.st, s.count, s.hi, s.hi_idx);
+            a.psum64[pair] = s.sum;
+            if (a.pair_status) a.pair_status[pair] = (uint8_t)s.st;
+            if (a.pair_victims) a.pair_victims[pair] = s.st == DRA_PRE_EVICT ? s.count : 0u;
+        }
+    }
+}
+
+// is EVICT pair x (summary xs, sum x64) preferred to y?  Equal summaries: neither (list position decides)
+__device__ __forceinline__ bool pre_better(const uint4 xs, const unsigned long long x64, const uint4 ys, const unsigned long long y64) {
+    if (xs.z != ys.z) return (int32_t)xs.z < (int32_t)ys.z;             // lowest highest victim priority
+    if (x64 != y64) return x64 < y64;                                    // lowest sum of priorities
+    if (xs.y != ys.y) return xs.y < ys.y;                                // fewest victims
+    return xs.w > ys.w;                                                  // latest "start" among the highest-priority victims
+}
+
+// Warp per pod: FITS at the first such candidate, else the preferred EVICT pair, else INVALID / SEARCH_LIMIT / NO.
+__global__ void __launch_bounds__(256)
+k_pre_choose(const PreArgs a) {
+    if (__ldcg(a.gate)) return;
+    const uint32_t lane = threadIdx.x & 31, p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (p >= a.n_pod) return;
+    const bool dense = a.cand_off == nullptr;
+    const uint32_t k0 = dense ? p * a.n_node : __ldg(&a.cand_off[p]), k1 = dense ? k0 + a.n_node : __ldg(&a.cand_off[p + 1]);
+    uint32_t fit = DRA_GPU_NONE, best = DRA_GPU_NONE;
+    uint4 bs = make_uint4(0, 0, 0, 0); unsigned long long b64 = 0;
+    bool lim = false;
+    for (uint32_t k = k0 + lane; k < k1; k += 32) {                      // each lane in list order: ties keep the earlier
+        const uint4 s = __ldcg(&a.psum[k]);
+        if (s.x == DRA_PRE_FITS) fit = min(fit, k);
+        else if (s.x == DRA_PRE_SEARCH_LIMIT) lim = true;
+        else if (s.x == DRA_PRE_EVICT) {
+            const unsigned long long v = __ldcg(&a.psum64[k]);
+            if (best == DRA_GPU_NONE || pre_better(s, v, bs, b64)) { best = k; bs = s; b64 = v; }
+        }
+    }
+    fit = __reduce_min_sync(FULLMASK, fit);
+    lim = __any_sync(FULLMASK, lim);
+    for (uint32_t d = 16; d; d >>= 1) {
+        const uint32_t ob = __shfl_xor_sync(FULLMASK, best, d);
+        uint4 os;
+        os.x = __shfl_xor_sync(FULLMASK, bs.x, d); os.y = __shfl_xor_sync(FULLMASK, bs.y, d);
+        os.z = __shfl_xor_sync(FULLMASK, bs.z, d); os.w = __shfl_xor_sync(FULLMASK, bs.w, d);
+        const unsigned long long o64 = __shfl_xor_sync(FULLMASK, b64, d);
+        const bool take = ob != DRA_GPU_NONE &&
+                          (best == DRA_GPU_NONE || pre_better(os, o64, bs, b64) || (!pre_better(bs, b64, os, o64) && ob < best));
+        if (take) { best = ob; bs = os; b64 = o64; }
+    }
+    const uint32_t c0 = __ldg(&a.pod_off[p]), cnt = __ldg(&a.pod_off[p + 1]) - c0;
+    bool inv = cnt > DRA_MAX_POD;
+    for (uint32_t i = lane; i < cnt && !inv; i += 32) {
+        const uint4 c = __ldg(&a.claims[c0 + i]);
+        const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
+        inv = claim_invalid(kind, prof, count, true) || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
+    }
+    inv = __any_sync(FULLMASK, inv);
+    if (lane != 0) return;
+    uint32_t st, k = DRA_GPU_NONE;
+    if (fit != DRA_GPU_NONE) { st = DRA_PRE_FITS; k = fit; }
+    else if (best != DRA_GPU_NONE) { st = DRA_PRE_EVICT; k = best; }
+    else st = inv ? DRA_PRE_INVALID : lim ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO;
+    a.pod_status[p] = (uint8_t)st;
+    a.pod_node[p] = k == DRA_GPU_NONE ? DRA_GPU_NONE : dense ? k - k0 : __ldg(&a.cand_nodes[k]);
+    a.n_victims[p] = st == DRA_PRE_EVICT ? bs.y : 0u;
+    a.choice[p] = st == DRA_PRE_EVICT ? k : DRA_GPU_NONE;
+}
+
+// W lanes per pod whose choice is an EVICT pair: its reprieve once more, writing the victims into the pod's row (the rows
+// are filled with 0xFFFFFFFF by the host first).  Deterministic, so the victims are the ones k_pods_preempt counted.
+template <int WPC, int W>
+__global__ void __launch_bounds__(WPC * 32, 2)
+k_pods_preempt_victims(const PreArgs a) {
+    __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
+    if (__ldcg(a.gate)) return;
+    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
+    __syncthreads();
+    constexpr uint32_t G = 32 / W;
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t grp = lane / W, gbase = grp * W;
+    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
+    for (uint32_t pw = (blockIdx.x * WPC + wid) * G; pw < a.n_pod; pw += gridDim.x * WPC * G) {
+        const uint32_t p = pw + grp;
+        if (p >= a.n_pod) continue;
+        const uint32_t k = __ldcg(&a.choice[p]);
+        if (k == DRA_GPU_NONE) continue;
+        const uint32_t node = a.cand_off ? __ldg(&a.cand_nodes[k]) : k - p * a.n_node;
+        (void)pre_pair<W>(a, tbl_s, p, node, lane, gmask, gbase, true, a.victims + (size_t)p * a.max_victims);
+    }
 }
 
 }  // namespace dra

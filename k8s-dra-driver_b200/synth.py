@@ -312,3 +312,118 @@ def pods(n_pod: int = 20_000, n_node: int = 64, seed: int = 0, gpus_per_node: in
     c["group"] = np.repeat(np.where(grp, np.arange(1, n_pod + 1, dtype=np.uint32), 0).astype(np.uint32), sizes)
     w = Workload(f"pods{seed}", g, off, R.default_table(), c).finish()
     return w, pod_off
+
+
+@dataclass
+class PreemptWorld:
+    """A consistent inventory with the running pods that occupy it, and pending pods for spec §14 (preemption)."""
+    gpus: np.ndarray          # GPU_DTYPE: the inventory WITH the running pods' allocations applied
+    empty: np.ndarray         # GPU_DTYPE: the same inventory with nothing allocated
+    node_off: np.ndarray
+    table: np.ndarray
+    run_claims: np.ndarray    # CLAIM_DTYPE, one OutRec slot each (run_out_off None)
+    run_pod_off: np.ndarray
+    run_prio: np.ndarray      # int32
+    run_out: np.ndarray       # OUT_DTYPE
+    claims: np.ndarray        # pending pods' claims (node fields 0: the call ignores them)
+    pod_off: np.ndarray
+    prio: np.ndarray          # int32
+
+
+def preempt(n_node: int = 16, gpus_per_node: int = 8, n_pending: int = 64, seed: int = 0, fill: int = 90,
+            mig_nodes: int = 3, prio_lo: int = -100, prio_hi: int = 1000, pending_prio: int | None = None,
+            shared_per_gpu: int = 6, shapes=("3g", "7g", "2x3g", "gpu2"),
+            tiles=(R.GI_1_SLICE, R.GI_1_SLICE, R.GI_2_SLICE, R.GI_2_SLICE, R.GI_3_SLICE)) -> PreemptWorld:
+    """Preemption workload (spec §14), built directly — no allocator runs.  Of every 4 nodes, `mig_nodes` are MIG nodes
+    whose GPUs are tiled first-fit with running pods of the `tiles` profiles (1g, 2g, 3g) until `fill` % of the 8 slices are taken (the
+    fragmented regime of cfg5); the other nodes' GPUs each carry a full-GPU pod, up to `shared_per_gpu` SHARED pods (time
+    slicing or an MPS memory limit), or nothing.  Running pods take 1 or 2 claims, with seeded priorities in
+    [prio_lo, prio_hi); pending pods are 3g, 7g, 2x3g (one co-location group) or N-GPU ("gpuN") pods at `pending_prio` (default:
+    seeded in [prio_hi / 2, prio_hi + 100))."""
+    g, off = R.make_inventory([gpus_per_node] * n_node, mig=True)
+    r = splitmix64(BASE_SEED + 1400 + seed, 64 * len(g) * max(shared_per_gpu, 8) + 8 * n_pending + 64)
+    pos = [0]
+
+    def nxt(m):
+        v = int(r[pos[0]] % np.uint64(m))
+        pos[0] += 1
+        return v
+
+    mig_node = np.array([nxt(4) < mig_nodes for _ in range(n_node)])
+    g["flags"] = np.repeat(np.where(mig_node, R.GPU_MIG_ENABLED, 0), gpus_per_node).astype(np.uint8)
+    empty = g.copy()
+    rc, ro, pods, rprio = [], [], [], []
+    size_of = {R.GI_1_SLICE: (1, range(0, 7)), R.GI_2_SLICE: (2, (0, 2, 4)), R.GI_3_SLICE: (4, (0, 4))}
+
+    def claim(kind, prof, node, mem=0):
+        c = np.zeros(1, dtype=R.CLAIM_DTYPE)[0]
+        c["kind"], c["profile"], c["count"], c["node"], c["mem_limit_mib"] = kind, prof, 1, node, mem
+        return c
+
+    def out(gpu, start, size, prof):
+        o = np.zeros(1, dtype=R.OUT_DTYPE)[0]
+        o["gpu"], o["start"], o["size"], o["profile"], o["status"] = gpu, start, size, prof, R.ST_OK
+        return o
+
+    pending = []                # claims of the running pod being built: (claim, out)
+    for n in range(n_node):
+        for gi in range(off[n], off[n + 1]):
+            if mig_node[n]:
+                tries = 0
+                while bin(int(g["busy"][gi])).count("1") * 100 < fill * 8 and tries < 24:
+                    tries += 1
+                    prof = tiles[nxt(len(tiles))]
+                    size, starts = size_of[prof]
+                    for s in starts:
+                        m = ((1 << size) - 1) << s
+                        if not (int(g["busy"][gi]) & m):
+                            g["busy"][gi] |= m
+                            pending.append((claim(R.KIND_MIG, prof, n), out(gi, s, size, prof)))
+                            break
+                    if pending and (nxt(4) != 0 or len(pending) == 2):
+                        pods.append(pending); pending = []
+            else:
+                k = nxt(8)
+                if k < 2:
+                    g["flags"][gi] |= R.GPU_FULL_ALLOCATED
+                    pods.append([(claim(R.KIND_GPU, R.PROFILE_GPU, n), out(gi, 0, 0, R.PROFILE_GPU))])
+                elif k < 7:
+                    for _ in range(1 + nxt(max(shared_per_gpu, 1))):
+                        mem = (0, 0, 1024, 2048, 4096)[nxt(5)]
+                        if g["mem_free_mib"][gi] < mem:
+                            continue
+                        g["mem_free_mib"][gi] -= mem
+                        g["share_cnt"][gi] += 1
+                        c = claim(R.KIND_SHARED, 0, n, mem)
+                        c["profile"] = 0
+                        pods.append([(c, out(gi, 0, 0, R.PROFILE_SHARED))])
+            if pending:
+                pods.append(pending); pending = []
+    run_pod_off = np.zeros(len(pods) + 1, dtype=np.uint32)
+    run_pod_off[1:] = np.cumsum([len(p) for p in pods])
+    run_claims = np.array([c for p in pods for c, _ in p], dtype=R.CLAIM_DTYPE)
+    run_out = np.array([o for p in pods for _, o in p], dtype=R.OUT_DTYPE)
+    span = max(prio_hi - prio_lo, 1)
+    run_prio = np.array([prio_lo + nxt(span) for _ in pods], dtype=np.int32)
+    cl, pod_off, prio = [], [0], []
+    for q in range(n_pending):
+        shape = shapes[nxt(len(shapes))]
+        if shape == "3g":
+            cl.append(claim(R.KIND_MIG, R.GI_3_SLICE, 0))
+        elif shape == "7g":
+            cl.append(claim(R.KIND_MIG, R.GI_7_SLICE, 0))
+        elif shape == "2x3g":
+            for _ in range(2):
+                c = claim(R.KIND_MIG, R.GI_3_SLICE, 0)
+                c["group"] = q + 1
+                cl.append(c)
+        else:                                          # "gpu<N>": one claim of N full GPUs
+            c = claim(R.KIND_GPU, 0, 0)
+            c["count"] = int(shape[3:])
+            cl.append(c)
+        pod_off.append(len(cl))
+        prio.append(pending_prio if pending_prio is not None else prio_hi // 2 + nxt(prio_hi // 2 + 100))
+    return PreemptWorld(g, empty, off, R.default_table(), run_claims if len(run_claims) else np.zeros(0, R.CLAIM_DTYPE),
+                        run_pod_off, run_prio, run_out if len(run_out) else np.zeros(0, R.OUT_DTYPE),
+                        np.array(cl, dtype=R.CLAIM_DTYPE), np.array(pod_off, dtype=np.uint32),
+                        np.array(prio, dtype=np.int32))
