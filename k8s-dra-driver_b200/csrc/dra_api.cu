@@ -129,7 +129,7 @@ struct dra_ctx {
     uint32_t ev_mask = 0;
     // dynamic shared-memory limits are raised ONCE per device to the opt-in maximum (raise_smem_limits): the attribute is
     // per function, not per context — a lazily "grown" per-context value would LOWER it under another context's feet
-    int hist8_smem_set = 1 << 30, hist_smem_set = 1 << 30, small_smem_set = 1 << 30, fused_smem_set = 1 << 30, fused_smem_set_stage = 1 << 30, fused_smem_set_cl = 1 << 30;
+    int hist8_smem_set = 1 << 30, hist_smem_set = 1 << 30, small_smem_set = 1 << 30, fused_smem_set = 1 << 30, fused_smem_set_stage = 1 << 30;
     uint64_t fused_max_work = 3000000ull;   // n_node * n_claim up to which the single-launch kernel is used
     uint32_t fused_max_one_wave = 14000u, fused_max_multi = 7500u;   // claims up to which it beats the sort path (profiles/path_crossover.py,
                                                                      // fused_plan); dra_calibrate re-measures them on the device at hand
@@ -526,8 +526,8 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
             launch_smem = fused_smem + 32 + (size_t)q_cap * 16;
             if (ctx->tail_cap_smem != (int)launch_smem || ctx->tail_cap_stage != (int)stage) {
                 int nb = 0;
-                if (stage) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, true, 1>, FUSED_NW * 32, launch_smem));
-                else CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, false, 1>, FUSED_NW * 32, launch_smem));
+                if (stage) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, true>, FUSED_NW * 32, launch_smem));
+                else CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, false>, FUSED_NW * 32, launch_smem));
                 ctx->tail_cap_smem = (int)launch_smem; ctx->tail_cap_stage = (int)stage; ctx->tail_cap_cta = nb * ctx->n_sm;
             }
             const bool resident = (int)(n_node + 1) <= ctx->tail_cap_cta;
@@ -547,11 +547,6 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
         if (want_in && !a.sh_on && (rc = launch_compaction(ctx, *view->sa, view->sc_rows, view->sc_flat))) return rc;
         if (tail_ok) { a.peer = *tail; a.q_cap = q_cap; if (tail_done) *tail_done = true; }
         else if (!a.sh_on) launch_smem = fused_smem;
-        // clusters of 8 CTAs + TMA multicast: the cluster launch and synchronisation cost more than the L2 traffic they save;
-        // kept as an opt-in experiment (DRA_CLUSTER=1)
-        constexpr int CLS = 8;
-        static const bool want_cluster = getenv("DRA_CLUSTER") != nullptr;
-        const bool cluster = stage && want_cluster && n_node + 1 >= (uint32_t)CLS && !tail_ok;
         a.claims = d_claims; a.out_off = d_out_off; a.n_claim = n_claim;
         if (getenv("DRA_TIMELINE")) {           // instrumentation only: per-CTA clock stamps of the last fused launch
             if (ctx->tl_cap < (size_t)(2 * n_node + 24) * 8) {
@@ -563,17 +558,8 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
             a.timeline = ctx->d_timeline; ctx->tl_n = (2 * n_node + 6) * 8;
         }
         prof.skip_to(3);
-        // grid = one CTA per node + one CTA for the claims that name no node (+ padding to whole clusters)
-        if (cluster) {
-            cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
-            lc.gridDim = dim3(((n_node + 1 + CLS - 1) / CLS) * CLS); lc.blockDim = dim3(FUSED_NW * 32);
-            lc.dynamicSmemBytes = fused_smem; lc.stream = ctx->stream;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = CLS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-            lc.attrs = at; lc.numAttrs = 1;
-            CU(cudaLaunchKernelEx(&lc, k_fused<FUSED_NW, true, CLS>, a));
-        }
-        else if (stage && dio.h_claims) {
+        // grid = one CTA per node + one CTA for the claims that name no node
+        if (stage && dio.h_claims) {
             // direct host I/O: two grid barriers inside, so every CTA must be resident — cooperative launch
             a.dio = dio;
             cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
@@ -581,7 +567,7 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
             cudaLaunchAttribute at[1];
             at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
             lc.attrs = at; lc.numAttrs = 1;
-            CU(cudaLaunchKernelEx(&lc, k_fused<FUSED_NW, true, 1>, a));
+            CU(cudaLaunchKernelEx(&lc, k_fused<FUSED_NW, true>, a));
         }
         else {
             static const bool no_pdl_fused = getenv("DRA_NO_PDL") != nullptr;
@@ -592,14 +578,14 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
                 cudaLaunchAttribute at[1];
                 at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
                 lc.attrs = at; lc.numAttrs = 1;
-                if (stage) CU(cudaLaunchKernelEx(&lc, k_fused<FUSED_NW, true, 1>, a));
-                else CU(cudaLaunchKernelEx(&lc, k_fused<FUSED_NW, false, 1>, a));
+                if (stage) CU(cudaLaunchKernelEx(&lc, k_fused<FUSED_NW, true>, a));
+                else CU(cudaLaunchKernelEx(&lc, k_fused<FUSED_NW, false>, a));
             }
-            else if (stage) CU(launch_k(k_fused<FUSED_NW, true, 1>, dim3(n_node + 1), dim3(FUSED_NW * 32), launch_smem, ctx->stream, dep, a));
-            else CU(launch_k(k_fused<FUSED_NW, false, 1>, dim3(n_node + 1), dim3(FUSED_NW * 32), launch_smem, ctx->stream, dep, a));
+            else if (stage) CU(launch_k(k_fused<FUSED_NW, true>, dim3(n_node + 1), dim3(FUSED_NW * 32), launch_smem, ctx->stream, dep, a));
+            else CU(launch_k(k_fused<FUSED_NW, false>, dim3(n_node + 1), dim3(FUSED_NW * 32), launch_smem, ctx->stream, dep, a));
         }
         ctx->launches += 1;
-        ctx->chain |= (stage && dio.h_claims && !cluster) ? DRA_K_FUSED_DIRECT : stage ? DRA_K_FUSED_STAGED : DRA_K_FUSED_STREAM;
+        ctx->chain |= (stage && dio.h_claims) ? DRA_K_FUSED_DIRECT : stage ? DRA_K_FUSED_STAGED : DRA_K_FUSED_STREAM;
         if (a.sh_on) ctx->chain |= DRA_K_COMPACT_IN_KERNEL;
         prof.mark();
         cudaError_t e = cudaGetLastError();
@@ -717,9 +703,8 @@ int raise_one(dra_ctx* ctx, K k, int optin) {
 }
 int raise_smem_limits(dra_ctx* ctx, int optin) {
     int rc;
-    if ((rc = raise_one(ctx, k_fused<FUSED_NW, true, 1>, optin))) return rc;
-    if ((rc = raise_one(ctx, k_fused<FUSED_NW, false, 1>, optin))) return rc;
-    if ((rc = raise_one(ctx, k_fused<FUSED_NW, true, 8>, optin))) return rc;
+    if ((rc = raise_one(ctx, k_fused<FUSED_NW, true>, optin))) return rc;
+    if ((rc = raise_one(ctx, k_fused<FUSED_NW, false>, optin))) return rc;
     if ((rc = raise_one(ctx, k_bucket_small, optin))) return rc;
     if ((rc = raise_one(ctx, k_bucket_hist8<false>, optin))) return rc;
     if ((rc = raise_one(ctx, k_bucket_hist8<true>, optin))) return rc;
@@ -1107,7 +1092,7 @@ int dra_allocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
     // and all its CTAs can be resident at once, the kernel itself reads the claims from the (pinned, device-mapped)
     // host buffer and writes the OutRecs back there — no copy-engine transfers, no graph, one cooperative launch.
     {
-        static const bool no_direct = getenv("DRA_NO_DIRECT") != nullptr || getenv("DRA_CLUSTER") != nullptr;   // (the cluster experiment has no ingest)
+        static const bool no_direct = getenv("DRA_NO_DIRECT") != nullptr;
         const FusedPlan plan = fused_plan(ctx, n_claim, flags, ctx->n_node);
         bool ok = !no_direct && !(ctx->cfg_flags & DRA_CFG_NO_DIRECT) && ctx->coop_ok && plan.fused && plan.stage && n_claim && rb &&
                   !ctx->profiling && ((uintptr_t)src_c & 15) == 0 && ((uintptr_t)dst_o & 15) == 0 &&
@@ -1115,11 +1100,11 @@ int dra_allocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
         if (ok && ctx->dio_cap_smem != (int)plan.smem) {
             // co-resident capacity at this shared-memory size (the attribute must be raised before the query)
             if (plan.smem > 48 * 1024 && ctx->fused_smem_set_stage < (int)plan.smem) {
-                CU(cudaFuncSetAttribute(k_fused<FUSED_NW, true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
+                CU(cudaFuncSetAttribute(k_fused<FUSED_NW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
                 ctx->fused_smem_set_stage = (int)plan.smem;
             }
             int nb = 0;
-            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, true, 1>, FUSED_NW * 32, plan.smem));
+            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, true>, FUSED_NW * 32, plan.smem));
             ctx->dio_cap_smem = (int)plan.smem; ctx->dio_cap_cta = nb * ctx->n_sm;
         }
         ok = ok && (int)(ctx->n_node + 1) <= ctx->dio_cap_cta;

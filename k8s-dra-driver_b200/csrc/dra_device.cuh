@@ -1971,16 +1971,6 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 #define DRA_TSTAMP(k) do { if (a.timeline && threadIdx.x == 0) a.timeline[(a.n_node + 4) * 8 + blockIdx.x * 8 + (k)] = globaltimer_ns(); } while (0)
 #define DRA_STAMP(k) do { if (a.timeline && threadIdx.x == 0) a.timeline[blockIdx.x * 8 + (k)] = (k) == 0 ? globaltimer_ns() : (unsigned long long)clock64(); } while (0)
 
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-// 1-D TMA bulk copy global -> the same shared-memory offset of every CTA of the cluster named in `mask`; each
-// destination CTA's mbarrier (same offset) receives the complete_tx.  One L2 read feeds all of them.
-__device__ __forceinline__ void tma_load_multicast(uint32_t sdst, const void* gsrc, uint32_t bytes, uint32_t bar, uint16_t mask) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
-                 ::"r"(sdst), "l"(gsrc), "r"(bytes), "r"(bar), "h"(mask) : "memory");
-}
-
 // Grid-wide barrier for a cooperative launch (all CTAs resident).  Sense-free: the last arriver resets the count
 // and bumps the generation the others spin on, so the two words are reusable across barriers and launches.
 // bar.sync orders the CTA's earlier stores before thread 0's fence (fences are cumulative); a bounded spin turns a
@@ -2008,8 +1998,6 @@ __device__ __forceinline__ void grid_barrier(uint32_t* gbar, uint32_t n_cta, con
     __syncthreads();
 }
 
-// CL = thread-block cluster size (1 or 8).  With CL = 8 the staged claim array is fetched from L2 ONCE per
-// cluster: CTA r of the cluster loads pieces r, r+8, ... and TMA-multicasts each into all 8 CTAs.
 // The body of the single-launch kernel: one batch.  k_fused runs it once; k_serve (resident mode) runs it once per doorbell
 // (`again`: the shared-memory barriers of the previous batch are invalidated first).
 // What differs from batch to batch (resident mode keeps everything else in the kernel's parameter space)
@@ -2020,14 +2008,13 @@ struct Batch {
     const uint4* h_claims; const uint32_t* h_out_off; uint2* h_out;
 };
 
-template <int NW, bool STAGE, int CL>
+template <int NW, bool STAGE>
 __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uint8_t* dyn_smem, const bool again) {
-    static_assert(CL == 1 || STAGE, "clusters only make sense with the staged claim array");
     DRA_STAMP(0); DRA_STAMP(1); DRA_TSTAMP(0);
     const uint32_t sbase = smem_base(dyn_smem);
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const uint32_t node = blockIdx.x;
-    const bool has_node = node < a.n_node;       // CTA n_node handles claims that name no node; later CTAs pad the cluster
+    const bool has_node = node < a.n_node;       // CTA n_node handles claims that name no node
     const uint32_t tbar = sbase + FU_TBAR, ibar = sbase + FU_IBAR;
     const uint32_t list_addr = sbase + FU_LIST + (STAGE ? (uint32_t)NW * FU_MAXPIECE * 8u : 0u);
     const uint32_t stage_addr = STAGE ? ((list_addr + (uint32_t)fused_list_bytes(b.n_claim, NW, STAGE) + 15u) & ~15u) : 0u;
@@ -2083,7 +2070,7 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
         return;
     }
 
-    if (STAGE && CL == 1 && b.h_claims) {
+    if (STAGE && b.h_claims) {
         // direct ingest: one 16-byte load from the caller's pinned buffer per thread (a single PCIe round trip for
         // the whole grid), stored to the device copy that everybody's bulk copies below read from L2.
         // (Per-piece ready flags instead of the grid barrier were tried: slower to the first bulk copy — every
@@ -2098,20 +2085,18 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
         DRA_DSTAMP(2);
     }
     if (STAGE) {
-        if (CL > 1) { cluster_arrive(); cluster_wait(); }      // barriers initialised in every CTA of the cluster before any multicast
-        // every warp arms (and, for the pieces this CTA is responsible for, issues) its share of the pieces:
-        // TMA issues from one warp serialise (~100 cycles each), so they are spread over the 8 warps' lane 0
-        const uint32_t npt = (n_claim + FU_PIECE - 1) / FU_PIECE;
-        const uint32_t crank = CL > 1 ? cluster_ctarank() : 0u;
+        // every warp arms and issues the pieces of its own part of the filter, in order: TMA issues from one warp
+        // serialise, so they are spread over the 8 warps' lane 0, and the copies land about in issue order — each
+        // warp's first piece is among the first to arrive.  (Dealt round-robin over the warps, the pieces land in array
+        // order: the last warp's part lands last and the CTA waits ~3,400 cycles for it on cfg2, profiles/timeline.py.)
+        const uint32_t part = fused_chunk(n_claim, NW, true);
+        const uint32_t g_end = (min(n_claim, (wid + 1) * part) + FU_PIECE - 1) / FU_PIECE;
         if (lane == 0)
-            for (uint32_t g = wid; g < npt; g += NW) {
+            for (uint32_t g = wid * part / FU_PIECE; g < g_end; ++g) {
                 const uint32_t c0 = g * FU_PIECE, bytes = min(FU_PIECE, n_claim - c0) * 16u;
                 asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sbar + g * 8), "r"(bytes) : "memory");
-                if (g % CL == crank) {
-                    if (CL > 1) tma_load_multicast(stage_addr + (c0 << 4), a.claims + c0, bytes, sbar + g * 8, (uint16_t)((1u << CL) - 1u));
-                    else asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                      ::"r"(stage_addr + (c0 << 4)), "l"(a.claims + c0), "r"(bytes), "r"(sbar + g * 8) : "memory");
-                }
+                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                             ::"r"(stage_addr + (c0 << 4)), "l"(a.claims + c0), "r"(bytes), "r"(sbar + g * 8) : "memory");
             }
     }
     DRA_STAMP(2);
@@ -2211,7 +2196,6 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
         for (int i = 0; i < NW; ++i) tot += lds32(sbase + FU_CNT + 64 + (i << 2));
         use_q = tot != 0 && tot <= a.q_cap;
     }
-    if (CL > 1) cluster_arrive();                  // this CTA has received every piece; matched by the wait at the end
     DRA_STAMP(4);
 
     IdxGet<NW> get;
@@ -2290,8 +2274,7 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
             if (base + e < pg.cap) pkt_send(pg, base + e, make_uint2(v.x, v.y), pg.slot_base + v.z);
         }
     }
-    if (CL > 1) cluster_wait();                    // nobody leaves while a cluster peer may still be receiving multicasts
-    if (STAGE && CL == 1 && b.h_claims) {
+    if (STAGE && b.h_claims) {
         // direct egress: when every CTA's OutRecs are in the device buffer, the grid writes them to the caller's
         // pinned buffer as coalesced 16-byte stores (a scattered 8-byte store per record is what makes plain
         // zero-copy output slow: profiles/e2e_parts.py)
@@ -2346,12 +2329,12 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
     DRA_TSTAMP(4);
 }
 
-template <int NW, bool STAGE, int CL>
+template <int NW, bool STAGE>
 __global__ void __launch_bounds__(NW * 32, 1)
 k_fused(const PackArgs a) {
     extern __shared__ __align__(16) uint8_t dyn_smem[];
     const Batch b{a.n_claim, a.n_out, a.have_off, 0u, a.inv_src, a.out_off, a.dio.h_claims, a.dio.h_out_off, a.dio.h_out};
-    fused_body<NW, STAGE, CL>(a, b, dyn_smem, false);
+    fused_body<NW, STAGE>(a, b, dyn_smem, false);
 }
 
 // ---- resident mode: the kernel stays up and takes batches by DOORBELL ------------------------------------------------
@@ -2429,7 +2412,7 @@ k_serve(const ServeArgs s) {
         b.h_out = reinterpret_cast<uint2*>(((unsigned long long)cmd_s[9] << 32) | cmd_s[8]);
         b.out_off = b.h_out_off ? a.dio.d_out_off : nullptr;
         b.have_off = b.h_out_off != nullptr;
-        if (n_claim <= s.cap_claims) fused_body<NW, true, 1>(a, b, dyn_smem, again);
+        if (n_claim <= s.cap_claims) fused_body<NW, true>(a, b, dyn_smem, again);
         else if (blockIdx.x == 0 && threadIdx.x == 0) a.err.set(ERR_SHARD_PLAN);          // (the host never sends such a batch)
         // completion: every CTA fences its stores to the host's buffers and takes a ticket; the last one tells the host
         // (one word).  Nobody waits here: the next doorbell cannot ring before the host has seen this word.
