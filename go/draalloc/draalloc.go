@@ -472,6 +472,59 @@ func (c *Context) PlacePodsGlobal(pinnedClaims unsafe.Pointer, nClaim int, pinne
 	return nil
 }
 
+// SetShardPreempt reserves room for the sharded preemption call's per-pod partials and pair results: before ShardExport,
+// the same on every context.  Unbuilt, like the rest of this file.
+func (c *Context) SetShardPreempt(maxPods, maxPairs, maxVictims uint32) error {
+	if rc := C.dra_set_shard_preempt(c.h, C.uint32_t(maxPods), C.uint32_t(maxPairs), C.uint32_t(maxVictims)); rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
+// PinnedRunningPods: the running pods of PreemptBatchGlobalDevice, every array in dra_host_alloc'ed (pinned) or device
+// memory (OutOff may be nil: slot i).
+type PinnedRunningPods struct {
+	Claims unsafe.Pointer
+	NClaim int
+	PodOff unsafe.Pointer
+	NPod   int
+	Prio   unsafe.Pointer
+	OutOff unsafe.Pointer
+	Out    unsafe.Pointer
+	NOut   int
+}
+
+// PreemptBatchGlobalDevice: preemption (spec §14) on a sharded world (dra_preempt_batch_global_device).  The same pending
+// pods, candidates (pinnedCandNodes == pinnedCandOff == nil: dense form, nPair = nPod * nNode), running pods, maxVictims
+// and flags on every context, every array in dra_host_alloc'ed (pinned) memory; each context judges the pairs of its own
+// nodes, and every context ends with the whole outputs (the pair outputs may be nil).  Returns at once; Sync reports
+// completion and errors found on the device.  Unbuilt, like the rest of this file.
+func (c *Context) PreemptBatchGlobalDevice(pinnedClaims unsafe.Pointer, nClaim int, pinnedPodOff, pinnedPrio unsafe.Pointer,
+	nPod int, pinnedCandNodes, pinnedCandOff unsafe.Pointer, nPair int, run PinnedRunningPods,
+	pinnedPairStatus, pinnedPairVictims, pinnedPodNode, pinnedPodStatus, pinnedNVictims, pinnedVictims unsafe.Pointer,
+	maxVictims int, flags uint32) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var r C.dra_running_pods
+	r.claims = (*C.dra_claim_rec)(run.Claims)
+	r.n_claim = C.uint32_t(run.NClaim)
+	r.pod_off = (*C.uint32_t)(run.PodOff)
+	r.n_pod = C.uint32_t(run.NPod)
+	r.prio = (*C.int32_t)(run.Prio)
+	r.out_off = (*C.uint32_t)(run.OutOff)
+	r.out = (*C.dra_out_rec)(run.Out)
+	r.n_out = C.uint32_t(run.NOut)
+	rc := C.dra_preempt_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
+		(*C.uint32_t)(pinnedPodOff), (*C.int32_t)(pinnedPrio), C.uint32_t(nPod), (*C.uint32_t)(pinnedCandNodes),
+		(*C.uint32_t)(pinnedCandOff), C.uint32_t(nPair), &r, (*C.uint8_t)(pinnedPairStatus), (*C.uint32_t)(pinnedPairVictims),
+		(*C.uint32_t)(pinnedPodNode), (*C.uint8_t)(pinnedPodStatus), (*C.uint32_t)(pinnedNVictims), (*C.uint32_t)(pinnedVictims),
+		C.uint32_t(maxVictims), C.uint32_t(flags))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
 // DeallocateGlobal: Deallocate on a sharded world (dra_deallocate_batch_global_device), the step after AllocatePodsGlobal.
 // The same claims, out_off and OutRecs on every context, in dra_host_alloc'ed (pinned) memory (pinnedOutOff may be nil);
 // each context applies the OK records whose GPU lies in its own range and writes no other GPU.  Needs SetShardMap (or

@@ -348,7 +348,7 @@ int  dra_gather_read(dra_ctx* ctx, dra_out_rec* out_all, uint32_t n_rec);
  *                                              cudaIpcMemHandle_t;  the host runtime all-gathers the handles;
  *   dra_peer_import(ctx, handles)              world * 64 bytes, in rank order.
  * Requires all ranks on one node with P2P access; on failure the NCCL path stays in use.  Every rank must export alike (the
- * same sizes, dra_set_shard_pairs, dra_set_shard_place and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
+ * same sizes, dra_set_shard_pairs, dra_set_shard_place, dra_set_shard_preempt and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
  * own layout, so dra_peer_import / dra_peer_import_local refuse a peer set up differently with DRA_E_INVAL.
  * dra_peer_export(ctx, 0, NULL) switches the peer path off again. */
 int  dra_peer_export(dra_ctx* ctx, uint32_t n_per_rank, void* handle64);
@@ -461,6 +461,35 @@ int  dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cla
                                         const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
                                         const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node, uint32_t flags);
 
+/* Room for the sharded preemption call in the buffer dra_shard_export maps: each rank's per-pod partials (32 bytes plus a
+ * row of max_victims words, padded to 16 bytes) and its pairs' results (8 bytes a pair), one slice per rank and call parity.
+ * World > 1: call before dra_shard_export (afterwards: DRA_E_STATE), every rank with the same sizes; the peer import refuses
+ * a peer set up differently.  Load the inventory first: the export then also sizes the call's sort for it and its scratch
+ * for max_pairs, so that no call frees a buffer (which waits for the whole device) while a peer waits for it.  World 1
+ * needs no call. */
+int  dra_set_shard_preempt(dra_ctx* ctx, uint32_t max_pods, uint32_t max_pairs, uint32_t max_victims);
+/* Preemption over a sharded world (spec §14, "Sharded form"): dra_preempt_batch answered on the world's state.  The SAME
+ * pending pods (claims, pod_off, prio), candidates (cand_nodes == cand_off == NULL: the dense form, n_pair = n_pod * n_node),
+ * running pods, max_victims and flags on every rank (device pointers, or dra_host_alloc'ed buffers; `running` itself is a
+ * host struct whose pointers are device-visible).  A pair is judged by the rank whose node range holds its candidate node,
+ * against that rank's live inventory; a candidate naming no node of the inventory is DRA_PRE_NO.  Every rank ends with the
+ * WHOLE outputs, laid out as dra_preempt_batch's, byte for byte what that call answers on ONE inventory made of every
+ * rank's own nodes; d_pair_status / d_pair_victims may be NULL.  Nothing is written to any inventory, live or pristine.
+ * world > 1 needs dra_set_shard_map (a bare dra_set_shard: DRA_E_STATE), dra_shard_export after dra_set_shard_preempt, and
+ * dra_peer_import / dra_peer_import_local (else DRA_E_STATE); n_pod, n_pair and max_victims above its sizes: DRA_E_INVAL.
+ * World 1 needs none of it and judges every node.  Host-side argument errors return before anything is enqueued.  Enqueues
+ * on ctx's stream and returns; n_pod == 0 enqueues nothing.  Completion and device-detected errors surface at
+ * dra_ctx_sync: pod_off / cand_off not monotone or not spanning their arrays, or the running pods' faults of
+ * dra_preempt_batch give DRA_E_INVAL on EVERY rank with none of the outputs written; a peer that does not arrive within
+ * DRA_PEER_TIMEOUT_MS gives DRA_E_NCCL.  flags: 0 or DRA_F_EXHAUSTIVE. */
+int  dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                     const uint32_t* d_pod_off, const int32_t* d_prio, uint32_t n_pod,
+                                     const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                     const dra_running_pods* running,
+                                     uint8_t* d_pair_status, uint32_t* d_pair_victims,
+                                     uint32_t* d_pod_node, uint8_t* d_pod_status, uint32_t* d_n_victims,
+                                     uint32_t* d_victims, uint32_t max_victims, uint32_t flags);
+
 /* Every rank's live inventory becomes the world's state: for each GPU, the record its owning rank holds (the rank whose
  * node range contains the GPU's node, per the current dra_set_shard_map).  Own range untouched, pristine copy untouched.
  * Afterwards dra_get_inventory on any rank returns the whole world, and dra_set_shard_map may move node ranges between
@@ -559,6 +588,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_PLACE             0x200000u /* place pods: pod states + pair records, persistent walk of the nodes' visit lists */
 #define DRA_K_PLACE_SHARD       0x400000u /* sharded place pods: prep, gate, walk of the node window, finalisers (+ all-gather) */
 #define DRA_K_PREEMPT           0x800000u /* preemption: running-pod prep, victim lists, pairs, choice, victim rows */
+#define DRA_K_PREEMPT_SHARD    0x1000000u /* sharded preemption: prep, victim lists, the window's pairs, partials, merge */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

@@ -201,6 +201,11 @@ struct dra_ctx {
     uint8_t* d_splace_local = nullptr; size_t cap_splace_local = 0;    // pods
     uint32_t splace_seq = 0;                    // the last call's sequence number (peer_setup starts over: fresh words)
     uint4* d_splace_rec = nullptr; size_t cap_splace_rec = 0;          // [n_pod] finaliser records for k_spod_gather
+    // sharded preemption: a region [partials x2: world slices][flags] (dra_device.cuh PreShard) in the peer buffer
+    uint32_t pre_max_pods = 0, pre_max_pairs = 0, pre_max_victims = 0;   // dra_set_shard_preempt, reserved by the next peer_setup
+    uint32_t peer_pre_pods = 0, peer_pre_pairs = 0, peer_pre_victims = 0;
+    PeerRegion pre_x;
+    uint4* d_spre_part = nullptr; size_t cap_spre_part = 0;           // this rank's partials and pair results (uint4 units)
     int splace_occ = -1;                        // resident CTAs of k_pods_place<4, true> per SM (occupancy query, once)
     int peers_on_device = 1;                    // ranks whose contexts share this device (dra_peer_import_local)
     // inventory sync: records in the peer buffer ([staging x2: peer_inv_gpus records][flags[PEER_MAX], elect[2]])
@@ -677,6 +682,10 @@ int check_err(dra_ctx* ctx) {
     if (bo && (ctx->chain & DRA_K_PREEMPT))
         return fail(ctx, DRA_E_INVAL, "dra_preempt_batch: running pods: pod_off not monotone or not spanning the claims, a slot range outside "
                                       "n_out, or OK slots naming a GPU index >= n_gpu or GPUs of two nodes; nothing was written");
+    if (bo && (ctx->chain & DRA_K_PREEMPT_SHARD))
+        return fail(ctx, DRA_E_INVAL, "sharded preemption: pod_off / cand_off not monotone or not spanning their arrays, or running pods: pod_off "
+                                      "not monotone or not spanning the claims, a slot range outside n_out, or OK slots naming a GPU index "
+                                      ">= n_gpu or GPUs of two nodes (on this rank or a peer); nothing was written");
     if (bo) return fail(ctx, DRA_E_INVAL, "sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays; nothing was evaluated");
     if (bp && (ctx->chain & DRA_K_PLACE_SHARD))
         return fail(ctx, DRA_E_INVAL, "sharded place pods: pod_off / cand_off not monotone or not spanning their arrays, more than %u candidates for a pod, "
@@ -893,7 +902,7 @@ void dra_ctx_destroy(dra_ctx* c) {
                    c->d_place_state, c->d_place_node, c->d_place_cursor, c->d_splace_local, c->d_splace_rec,
                    c->d_pre_prio, c->d_pre_node, c->d_pre_nvic, c->d_pre_choice, c->d_pre_pst, c->d_pre_psum, c->d_pre_psum64,
                    c->d_pre_pairst, c->d_pre_pairvic, c->d_pre_rclaims, c->d_pre_routoff, c->d_pre_rpodoff, c->d_pre_rprio,
-                   c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic};
+                   c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic, c->d_spre_part};
     for (void* p : dev) if (p) cudaFree(p);
     for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
@@ -1719,12 +1728,14 @@ namespace {
 // every rank to be set up alike; the export writes this at offset 0 of the buffer for importers in other processes to read.
 struct PeerLayout {
     uint32_t world, rank, form, cap, tab_len, uns_pairs, inv_gpus, rsvd;      // rsvd: dra_set_shard_place's max_pods
+    uint32_t pre_pods, pre_pairs, pre_victims, pad;                           // dra_set_shard_preempt's sizes
     bool operator==(const PeerLayout& o) const { return memcmp(this, &o, sizeof o) == 0; }
 };
 PeerLayout layout_of(const dra_ctx* c, int rank) {
     PeerLayout l; memset(&l, 0, sizeof l);
     l.world = (uint32_t)c->world; l.rank = (uint32_t)rank; l.form = c->peer_form; l.cap = c->peer_cap; l.tab_len = c->peer_tab_len;
     l.uns_pairs = c->peer_uns_pairs; l.inv_gpus = c->peer_inv_gpus; l.rsvd = c->peer_place_pods;
+    l.pre_pods = c->peer_pre_pods; l.pre_pairs = c->peer_pre_pairs; l.pre_victims = c->peer_pre_victims;
     return l;
 }
 
@@ -1747,10 +1758,51 @@ int preload_place_shard(dra_ctx* ctx) {
     return DRA_OK;
 }
 
+// The same for the sharded preemption chain, whose merge waits for its peers: it also takes the all-shared split.
+int preload_preempt_shard(dra_ctx* ctx) {
+    const void* ks[] = {(const void*)k_uns_prep, (const void*)k_pre_running, (const void*)k_pre_vsort,
+                        (const void*)k_pods_preempt_win<8, 8>, (const void*)k_pods_preempt_win<8, 16>, (const void*)k_pods_preempt_win<8, 32>,
+                        (const void*)k_spre_reduce, (const void*)k_pods_preempt_victims_win<8, 8>, (const void*)k_pods_preempt_victims_win<8, 16>,
+                        (const void*)k_pods_preempt_victims_win<8, 32>, (const void*)k_peer_push, (const void*)k_spre_merge,
+                        (const void*)k_bucket_small, (const void*)k_bucket_hist8<false>, (const void*)k_bucket_hist8<true>,
+                        (const void*)k_bucket_scan_rows, (const void*)k_bucket_scan8, (const void*)k_bucket_hist,
+                        (const void*)k_bucket_scan, (const void*)k_bucket_scatter};
+    for (const void* k : ks) { cudaFuncAttributes fa; CU(cudaFuncGetAttributes(&fa, k)); }
+    CU(cudaFuncSetAttribute((const void*)k_spre_merge, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    return DRA_OK;
+}
+
+// uint4 units of one rank's preemption partials (dra_device.cuh PreShard): the header, n_pod partials of 2 + ceil(max_victims
+// / 4) units, then n_pair {status, victims} pairs
+size_t spre_units(uint32_t n_pod, uint32_t n_pair, uint32_t max_victims) {
+    return 1 + (size_t)n_pod * (2 + ((size_t)max_victims + 3) / 4) + ((size_t)n_pair + 1) / 2;
+}
+
+// The sharded preemption call's own buffers for these sizes (the pair and running-pod groups as dra_preempt_batch grows them)
+int spre_buffers(dra_ctx* ctx, uint32_t n_pod, uint32_t n_pair, uint32_t max_victims, uint32_t rn_pod) {
+    int rc;
+    if ((rc = grow(ctx, ctx->d_spre_part, ctx->cap_spre_part, spre_units(n_pod, n_pair, max_victims)))) return rc;
+    if ((rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, std::max(n_pair, 1u)))) return rc;
+    if ((size_t)n_pair + 8 > ctx->cap_pre_pairs) {
+        const size_t need = (size_t)n_pair + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_psum, need)) || (rc = grow_pre(ctx, ctx->d_pre_psum64, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_pairst, need)) || (rc = grow_pre(ctx, ctx->d_pre_pairvic, need))) return rc;
+        ctx->cap_pre_pairs = need + need / 2 + 64;
+    }
+    if ((size_t)rn_pod + 8 > ctx->cap_pre_rpods) {
+        const size_t need = (size_t)rn_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rpodoff, need)) || (rc = grow_pre(ctx, ctx->d_pre_rprio, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_rrec, need)) || (rc = grow_pre(ctx, ctx->d_pre_vlist, need))) return rc;
+        ctx->cap_pre_rpods = need + need / 2 + 64;
+    }
+    return DRA_OK;
+}
+
 // (Re)allocates this rank's gather buffer:  [layout][table x2][staging x2: world slices of cap packets][headers x2][rendezvous flags]
 // and, after dra_set_shard_pairs(max_pairs > 0), [UnsuitableNodes staging x2: world slices of uns_stride words][their flags]
 // and, for dra_shard_export with an inventory loaded, [inventory staging x2: n_gpu records][their flags + election words]
 // and, after dra_set_shard_place(max_pods > 0), [place pods: progress counter, 64 bytes][max_pods state words of 8 bytes]
+// and, after dra_set_shard_preempt(max_pods > 0), [preemption partials x2: world slices of spre_units][their flags]
 int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, uint32_t cap) {
     if (ctx->world > (int)PEER_MAX) return fail(ctx, DRA_E_INVAL, "world %d > %u", ctx->world, PEER_MAX);
     CU(cudaSetDevice(ctx->device));
@@ -1792,6 +1844,16 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
         if (int rc = preload_place_shard(ctx)) return rc;
         // the sort's scan-status words for the loaded inventory now: ensure_batch grows them with a cudaFree, which waits
         // for the whole device — where, inside a call, a peer's walk may be waiting for this rank
+        if (ctx->d_inv_live) { if (int rc = ensure_batch(ctx, 1, 1, false)) return rc; }
+    }
+    // sharded preemption, after dra_set_shard_preempt: the partials' exchange, and the call's scratch at full size now (no
+    // cudaFree inside a call while a peer's merge waits for this rank)
+    ctx->peer_pre_pods = ctx->pre_max_pods; ctx->peer_pre_pairs = ctx->pre_max_pairs; ctx->peer_pre_victims = ctx->pre_max_victims;
+    if (ctx->peer_pre_pods) {
+        const size_t slice = spre_units(ctx->peer_pre_pods, ctx->peer_pre_pairs, ctx->peer_pre_victims) * 16;
+        reserve(ctx->pre_x, (size_t)ctx->world * slice, slice, (size_t)PEER_MAX * 4);
+        if (int rc = preload_preempt_shard(ctx)) return rc;
+        if (int rc = spre_buffers(ctx, ctx->peer_pre_pods, ctx->peer_pre_pairs, ctx->peer_pre_victims, 0)) return rc;
         if (ctx->d_inv_live) { if (int rc = ensure_batch(ctx, 1, 1, false)) return rc; }
     }
     ctx->splace_seq = 0;
@@ -2445,6 +2507,144 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded place pods launch: %s", cudaGetErrorString(e));
     ctx->gather_table = (const dra_out_rec*)table; ctx->gather_n_per = n_out; ctx->gather_len = n_out;
+    return DRA_OK;
+}
+
+int dra_set_shard_preempt(dra_ctx* ctx, uint32_t max_pods, uint32_t max_pairs, uint32_t max_victims) {
+    if (!ctx) return DRA_E_INVAL;
+    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "dra_set_shard_preempt: call it before dra_shard_export");
+    if (max_pods > (1u << 26) || max_pairs > 0xFFFFFFF0u || max_victims > (1u << 20))
+        return fail(ctx, DRA_E_INVAL, "dra_set_shard_preempt: sizes too large (max_pods <= 2^26, max_victims <= 2^20)");
+    if (spre_units(max_pods, max_pairs, max_victims) > ((size_t)1 << 32) / 16)
+        return fail(ctx, DRA_E_INVAL, "dra_set_shard_preempt: one rank's slice would exceed 4 GiB");
+    ctx->pre_max_pods = max_pods; ctx->pre_max_pairs = max_pairs; ctx->pre_max_victims = max_victims;
+    return DRA_OK;
+}
+
+// Sharded preemption: offset checks and pair -> pod (k_uns_prep) -> the running pods, their bucketing and victim lists on
+// the whole inventory (k_pre_running, the counting sort, k_pre_vsort) -> the window's pairs (k_pods_preempt_win) -> per-pod
+// partials (k_spre_reduce, k_pods_preempt_victims_win) -> push to every peer -> wait + merge into the caller's buffers (k_spre_merge).
+// Enqueues only.
+int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                    const uint32_t* d_pod_off, const int32_t* d_prio, uint32_t n_pod,
+                                    const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                    const dra_running_pods* running,
+                                    uint8_t* d_pair_status, uint32_t* d_pair_victims,
+                                    uint32_t* d_pod_node, uint8_t* d_pod_status, uint32_t* d_n_victims,
+                                    uint32_t* d_victims, uint32_t max_victims, uint32_t flags) {
+    if (!ctx || !d_pod_off || !running || !running->pod_off || (n_claim && !d_claims) ||
+        (n_pod && (!d_prio || !d_pod_node || !d_pod_status || !d_n_victims)))
+        return DRA_E_INVAL;
+    const dra_running_pods& R = *running;
+    if ((R.n_claim && !R.claims) || (R.n_pod && !R.prio) || (R.n_out && !R.out)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_preempt_batch_global_device: unknown flags 0x%x", flags);
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (max_victims && !d_victims) return fail(ctx, DRA_E_INVAL, "max_victims %u without a victims buffer", max_victims);
+    const bool dense = d_cand_nodes == nullptr && d_cand_off == nullptr;
+    if (!dense && (!d_cand_nodes || !d_cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
+    if (dense && (uint64_t)n_pod * ctx->n_node != n_pair)
+        return fail(ctx, DRA_E_INVAL, "dense form: n_pair %u != n_pod %u x n_node %u", n_pair, n_pod, ctx->n_node);
+    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    if (n_pod > (1u << 26) || max_victims > (1u << 20)) return fail(ctx, DRA_E_INVAL, "n_pod or max_victims too large for the sharded call");
+    const bool gather = ctx->world > 1;
+    if (gather) {
+        if (!ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the merge needs every rank's range)");
+        if (int rc = need_peers(ctx)) return rc;
+        if (ctx->shard_bounds[ctx->world] != ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard map does not span the inventory's %u nodes", ctx->n_node);
+        if (n_pod > ctx->peer_pre_pods || n_pair > ctx->peer_pre_pairs || max_victims > ctx->peer_pre_victims)
+            return fail(ctx, DRA_E_INVAL, "n_pod %u / n_pair %u / max_victims %u exceed the sizes of dra_set_shard_preempt before dra_shard_export "
+                        "(%u / %u / %u)", n_pod, n_pair, max_victims, ctx->peer_pre_pods, ctx->peer_pre_pairs, ctx->peer_pre_victims);
+    }
+    ctx->chain = DRA_K_PREEMPT_SHARD; ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
+    CU(cudaSetDevice(ctx->device));
+    // peers on this device may already wait for this rank: no buffer this call outgrows is freed before the next sync
+    struct DeferFree { dra_ctx* c; ~DeferFree() { c->defer_free = false; } } defer{ctx};
+    ctx->defer_free = gather;
+    int rc = upload_table(ctx);
+    if (rc) return rc;
+    if ((rc = ensure_batch(ctx, std::max(R.n_pod, 1u), 1, false))) return rc;
+    if ((rc = spre_buffers(ctx, n_pod, n_pair, max_victims, R.n_pod))) return rc;
+    if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, ctx->stream)); }
+    cudaStream_t st = ctx->stream;
+    const uint32_t lo = gather ? ctx->shard_lo : 0u, hi = gather ? ctx->shard_hi : ctx->n_node;   // world 1: every node
+    const bool want_pairs = d_pair_status || d_pair_victims;
+    PreShard s; memset(&s, 0, sizeof s);
+    s.node_lo = lo; s.node_hi = hi; s.n_walk = dense ? n_pod * (hi - lo) : n_pair;
+    s.stride = 2 + (max_victims + 3) / 4; s.part = ctx->d_spre_part;
+    s.pairs = want_pairs ? reinterpret_cast<uint2*>(ctx->d_spre_part + 1 + (size_t)n_pod * s.stride) : nullptr;
+
+    PreArgs a; memset(&a, 0, sizeof a);
+    a.claims = (const uint4*)d_claims; a.pod_off = d_pod_off; a.prio = d_prio; a.n_pod = n_pod;
+    a.cand_nodes = dense ? nullptr : d_cand_nodes; a.cand_off = dense ? nullptr : d_cand_off;
+    a.pair_pod = dense ? nullptr : ctx->d_upair_pod; a.n_pair = n_pair;
+    a.rclaims = (const uint4*)R.claims; a.rn_claim = R.n_claim; a.rpod_off = R.pod_off; a.rprio = R.prio; a.rn_pod = R.n_pod;
+    a.rout_off = R.out_off; a.rout = (const uint2*)R.out; a.rn_out = R.n_out;
+    a.rrec = ctx->d_pre_rrec; a.rsorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.vlist = ctx->d_pre_vlist;
+    a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.n_gpu = ctx->n_gpu; a.tbl = ctx->d_tbl;
+    a.sel = sel_of(ctx); a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
+    a.psum = ctx->d_pre_psum; a.psum64 = ctx->d_pre_psum64; a.max_victims = max_victims;
+    a.work = ctx->d_ticket + 13;
+    a.gate = ctx->d_err + ERR_BAD_OFFSETS; a.err = err_of(ctx);
+    Prof prof(ctx);
+    CU(cudaMemsetAsync(a.work, 0, 4, st));
+    k_uns_prep<<<std::max(1u, (n_pod + 7) / 8), 256, 0, st>>>(d_pod_off, dense ? nullptr : d_cand_off, n_pod, n_claim, n_pair,
+                                                              ctx->d_upair_pod, a.err);
+    k_pre_running<<<std::max(1u, (R.n_pod + 255) / 256), 256, 0, st>>>(a);
+    ctx->launches += 2;
+    if (R.n_pod) {
+        if ((rc = launch_sort(ctx, ctx->d_pre_rrec, R.n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, ctx->n_node, ctx->d_node_off)))
+            return rc;
+    } else {
+        CU(cudaMemsetAsync(ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, st));
+    }
+    const uint32_t W = ctx->max_width <= 8 ? 8u : (ctx->max_width <= 16 ? 16u : 32u);
+    if (ctx->n_node) {
+        k_pre_vsort<<<std::min(ctx->n_node, (uint32_t)ctx->n_sm * 8u), 256, 0, st>>>(a);
+        ctx->launches += 1;
+    }
+    const uint32_t per_cta = 8 * (32 / W);
+    if (s.n_walk) {
+        const uint32_t grid = std::max(1u, std::min((s.n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
+        if (W == 8) k_pods_preempt_win<8, 8><<<grid, 256, 0, st>>>(a, s);
+        else if (W == 16) k_pods_preempt_win<8, 16><<<grid, 256, 0, st>>>(a, s);
+        else k_pods_preempt_win<8, 32><<<grid, 256, 0, st>>>(a, s);
+        ctx->launches += 1;
+    }
+    k_spre_reduce<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, s);
+    ctx->launches += 1;
+    if (max_victims && hi > lo) {
+        const uint32_t grid = std::max(1u, std::min((n_pod + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
+        if (W == 8) k_pods_preempt_victims_win<8, 8><<<grid, 256, 0, st>>>(a, s);
+        else if (W == 16) k_pods_preempt_victims_win<8, 16><<<grid, 256, 0, st>>>(a, s);
+        else k_pods_preempt_victims_win<8, 32><<<grid, 256, 0, st>>>(a, s);
+        ctx->launches += 1;
+    }
+    prof.mark();
+    PreMerge m; memset(&m, 0, sizeof m);
+    m.part = s.part; m.pairs = s.pairs; m.stride = s.stride;
+    m.claims = a.claims; m.pod_off = d_pod_off; m.n_pod = n_pod;
+    m.cand_nodes = a.cand_nodes; m.cand_off = a.cand_off; m.n_pair = n_pair; m.n_node = ctx->n_node;
+    m.sel = a.sel; m.max_victims = max_victims; m.gate = a.gate;
+    m.bounds[0] = 0; m.bounds[1] = ctx->n_node;
+    if (gather) for (int r = 0; r <= ctx->world; ++r) m.bounds[r] = ctx->shard_bounds[r];
+    m.pair_status = d_pair_status; m.pair_victims = d_pair_victims;
+    m.pod_node = d_pod_node; m.pod_status = d_pod_status; m.n_victims = d_n_victims; m.victims = max_victims ? d_victims : nullptr;
+    const PeerExchange x = gather ? bind_exchange(ctx, ctx->pre_x) : PeerExchange{};   // world 1: no peers
+    if (gather) {
+        m.slice4 = (uint32_t)(ctx->pre_x.slice / 16);
+        const uint32_t n4 = (uint32_t)(1 + (size_t)n_pod * s.stride + (want_pairs ? ((size_t)n_pair + 1) / 2 : 0));
+        k_peer_push<<<std::max(1u, std::min((n4 + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, st>>>(x, s.part, 0u, n4);
+        ctx->launches += 1;
+    }
+    // a small grid: it waits for its peers, and ranks sharing one device must not find their evaluation's SMs held by it
+    const size_t work = std::max(((size_t)n_pod + 7) / 8, want_pairs ? ((size_t)n_pair + 255) / 256 : 0);
+    const uint32_t merge_grid = (uint32_t)std::max<size_t>(1, std::min<size_t>(work, (size_t)std::max(1, ctx->n_sm / 4)));
+    k_spre_merge<<<merge_grid, 256, 0, st>>>(x, m);
+    ctx->launches += 1;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded preemption launch: %s", cudaGetErrorString(e));
     return DRA_OK;
 }
 

@@ -12,7 +12,8 @@
 //   k_unsuitable     one warp per (pod, candidate node) pair, same step function on a snapshot
 //   k_pods_place     place pods (spec §13): persistent, a warp walks each of its nodes' visit lists with a cursor;
 //                    sharded (<4, true>): the rank's node window, pod states replicated on every rank (k_splace_*)
-//   k_pods_preempt   preemption (spec §14): per (pod, candidate) pair, W lanes, the victims by remove-all-then-reprieve
+//   k_pods_preempt   preemption (spec §14): per (pod, candidate) pair, W lanes, the victims by remove-all-then-reprieve;
+//                    sharded (k_pods_preempt_win): the rank's node window, per-pod partials merged on every rank (k_spre_*)
 //   k_dealloc        inverse updates with atomics (sharded: behind k_dealloc_check, on the rank's GPU range only)
 //
 // What this replaces in the reference: the per-node search behind Allocate()/UnsuitableNodes() that
@@ -3796,6 +3797,236 @@ k_pods_preempt_victims(const PreArgs a) {
         if (k == DRA_GPU_NONE) continue;
         const uint32_t node = a.cand_off ? __ldg(&a.cand_nodes[k]) : k - p * a.n_node;
         (void)pre_pair<W>(a, tbl_s, p, node, lane, gmask, gbase, true, a.victims + (size_t)p * a.max_victims);
+    }
+}
+
+// ---- sharded preemption (dra_preempt_batch_global_device) ----------------------------------------------------------
+// Every rank gets the same pending pods, candidates and running pods.  k_uns_prep checks pod_off / cand_off and writes
+// pair -> pod; k_pre_running, the counting sort and k_pre_vsort run unchanged on the whole inventory (their checks are
+// on global GPU indices, so every rank finds the same fault).  Then, on this rank's node window only:
+//   k_pods_preempt_win    k_pods_preempt's pair evaluation for the pairs whose node lies in the window
+//   k_spre_reduce   warp per pod: k_pre_choose's reduction over the window's pairs, keeping list positions, into this
+//                   rank's partial of the pod (and the rank's fault word into the partials' header)
+//   k_pods_preempt_victims_win  W lanes per pod whose partial holds an EVICT pair and no FITS pair: that pair's victim row
+//   k_peer_push     the partials (and, when the caller asked for them, the window's pair results) to every peer
+//   k_spre_merge    flags, wait, then per pod the minimum over the ranks' partials; writes the caller's buffers only if
+//                   no rank reported a fault
+// The partials, in uint4 units: [0] header {fault word}; pod p at 1 + p * stride: {fit position, best EVICT position,
+// its victim count, its highest victim priority}, {index of its first victim, SEARCH_LIMIT seen, its priority sum lo,
+// hi}, then the best pair's row of max_victims words; after the pods the window's pairs as {status, victims} (uint2).
+// A position is the pair's index in the call's pair list, so the merge's choice is the minimum over the ranks of a total
+// order — (FITS first, then pre_better, then position) — which is the single-inventory choice for any partition.
+struct PreShard {
+    uint32_t node_lo, node_hi;    // this rank's window
+    uint32_t n_walk;              // pairs the evaluation walks: dense n_pod * (node_hi - node_lo), else n_pair
+    uint32_t stride;              // uint4 units per pod partial: 2 + ceil(max_victims / 4)
+    uint4* part;                  // the partials (header, pods)
+    uint2* pairs;                 // the window's pair results (nullptr: the caller asked for none)
+};
+
+__device__ __forceinline__ uint4* spre_pod(const PreShard& s, uint32_t p) { return s.part + 1 + (size_t)p * s.stride; }
+
+template <int WPC, int W>
+__global__ void __launch_bounds__(WPC * 32, 2)
+k_pods_preempt_win(const PreArgs a, const PreShard s) {
+    __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
+    if (__ldcg(a.gate)) return;
+    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
+    __syncthreads();
+    constexpr uint32_t G = 32 / W;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t grp = lane / W, gbase = grp * W;
+    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
+    const uint32_t n_win = s.node_hi - s.node_lo;
+    while (true) {
+        uint32_t nxt = 0;
+        if (lane == 0) nxt = atomicAdd(a.work, G);
+        const uint32_t pw = __shfl_sync(FULLMASK, nxt, 0);
+        if (pw >= s.n_walk) break;
+        const uint32_t walk = pw + grp;
+        if (walk >= s.n_walk) continue;                                  // whole group skips together
+        uint32_t pod, node, pair;
+        if (!a.cand_off) { pod = walk / n_win; node = s.node_lo + (walk - pod * n_win); pair = pod * a.n_node + node; }
+        else {
+            pair = walk; node = __ldg(&a.cand_nodes[pair]);
+            if (node - s.node_lo >= n_win) continue;                     // another rank's node, or none
+            pod = __ldg(&a.pair_pod[pair]);
+        }
+        const PreSum r = pre_pair<W>(a, tbl_s, pod, node, lane, gmask, gbase, false, nullptr);
+        if (lane == gbase) {
+            a.psum[pair] = make_uint4(r.st, r.count, r.hi, r.hi_idx);
+            a.psum64[pair] = r.sum;
+            if (s.pairs) s.pairs[pair] = make_uint2(r.st, r.st == DRA_PRE_EVICT ? r.count : 0u);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256)
+k_spre_reduce(const PreArgs a, const PreShard s) {
+    const uint32_t gate = __ldcg(a.gate);
+    if (blockIdx.x == 0 && threadIdx.x == 0) s.part[0] = make_uint4(gate, 0u, 0u, 0u);
+    if (gate) return;
+    const uint32_t lane = threadIdx.x & 31, p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (p >= a.n_pod) return;
+    const bool dense = a.cand_off == nullptr;
+    const uint32_t n_win = s.node_hi - s.node_lo;
+    const uint32_t k0 = dense ? p * a.n_node + s.node_lo : __ldg(&a.cand_off[p]);
+    const uint32_t k1 = dense ? k0 + n_win : __ldg(&a.cand_off[p + 1]);
+    uint32_t fit = DRA_GPU_NONE, best = DRA_GPU_NONE;
+    uint4 bs = make_uint4(0, 0, 0, 0); unsigned long long b64 = 0;
+    bool lim = false;
+    for (uint32_t k = k0 + lane; k < k1; k += 32) {                      // each lane in list order: ties keep the earlier
+        if (!dense && __ldg(&a.cand_nodes[k]) - s.node_lo >= n_win) continue;
+        const uint4 v = __ldcg(&a.psum[k]);
+        if (v.x == DRA_PRE_FITS) fit = min(fit, k);
+        else if (v.x == DRA_PRE_SEARCH_LIMIT) lim = true;
+        else if (v.x == DRA_PRE_EVICT) {
+            const unsigned long long v64 = __ldcg(&a.psum64[k]);
+            if (best == DRA_GPU_NONE || pre_better(v, v64, bs, b64)) { best = k; bs = v; b64 = v64; }
+        }
+    }
+    fit = __reduce_min_sync(FULLMASK, fit);
+    lim = __any_sync(FULLMASK, lim);
+    for (uint32_t d = 16; d; d >>= 1) {
+        const uint32_t ob = __shfl_xor_sync(FULLMASK, best, d);
+        uint4 os;
+        os.x = __shfl_xor_sync(FULLMASK, bs.x, d); os.y = __shfl_xor_sync(FULLMASK, bs.y, d);
+        os.z = __shfl_xor_sync(FULLMASK, bs.z, d); os.w = __shfl_xor_sync(FULLMASK, bs.w, d);
+        const unsigned long long o64 = __shfl_xor_sync(FULLMASK, b64, d);
+        const bool take = ob != DRA_GPU_NONE &&
+                          (best == DRA_GPU_NONE || pre_better(os, o64, bs, b64) || (!pre_better(bs, b64, os, o64) && ob < best));
+        if (take) { best = ob; bs = os; b64 = o64; }
+    }
+    if (lane != 0) return;
+    if (fit != DRA_GPU_NONE) best = DRA_GPU_NONE;                        // a FITS pair anywhere beats every EVICT pair
+    uint4* q = spre_pod(s, p);
+    q[0] = make_uint4(fit, best, bs.y, bs.z);
+    q[1] = make_uint4(bs.w, lim ? 1u : 0u, (uint32_t)b64, (uint32_t)(b64 >> 32));
+}
+
+// W lanes per pod: the reprieve of the pod's best local EVICT pair once more, writing its row into the partial (only the
+// first min(count, max_victims) words; the merge fills the rest)
+template <int WPC, int W>
+__global__ void __launch_bounds__(WPC * 32, 2)
+k_pods_preempt_victims_win(const PreArgs a, const PreShard s) {
+    __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
+    if (__ldcg(a.gate)) return;
+    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
+    __syncthreads();
+    constexpr uint32_t G = 32 / W;
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t grp = lane / W, gbase = grp * W;
+    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
+    for (uint32_t pw = (blockIdx.x * WPC + wid) * G; pw < a.n_pod; pw += gridDim.x * WPC * G) {
+        const uint32_t p = pw + grp;
+        if (p >= a.n_pod) continue;
+        uint4* q = spre_pod(s, p);
+        const uint32_t k = __ldcg(&q[0]).y;
+        if (k == DRA_GPU_NONE) continue;
+        const uint32_t node = a.cand_off ? __ldg(&a.cand_nodes[k]) : k - p * a.n_node;
+        (void)pre_pair<W>(a, tbl_s, p, node, lane, gmask, gbase, true, reinterpret_cast<uint32_t*>(q + 2));
+    }
+}
+
+struct PreMerge {
+    const uint4* part;            // this rank's partials (PreShard::part); a peer's are at my_stage + sender * slice4
+    const uint2* pairs;           // this rank's pair results; a peer's follow its partials in its slice
+    uint32_t slice4, stride;      // uint4 units of one sender's slice; of one pod's partial
+    const uint4* claims; const uint32_t* pod_off; uint32_t n_pod;
+    const uint32_t* cand_nodes; const uint32_t* cand_off; uint32_t n_pair, n_node;
+    SelCtx sel;
+    uint32_t max_victims;
+    uint32_t bounds[PEER_MAX + 1];   // rank r owns nodes [bounds[r], bounds[r + 1])
+    const uint32_t* gate;            // this rank's fault word
+    uint8_t* pair_status; uint32_t* pair_victims;                  // the caller's (pair outputs: nullptr unless asked)
+    uint32_t* pod_node; uint8_t* pod_status; uint32_t* n_victims; uint32_t* victims;
+};
+
+// At most SMs / 4 CTAs, launched after the evaluation: ranks sharing one device must not find their evaluation's SMs
+// held by a peer's waiting CTAs.  Block 0 raises this rank's flags, every block waits; then a warp per pod (lane s reads
+// rank s's partial) and a thread per pair.  With world 1 (an all-zero PeerExchange) nothing is waited for.
+__global__ void __launch_bounds__(256)
+k_spre_merge(const PeerExchange x, const PreMerge m) {
+    __shared__ uint32_t s_ok;
+    const uint32_t tid = threadIdx.x;
+    if (tid == 0) s_ok = 1u;
+    __syncthreads();
+    if (blockIdx.x == 0) peer_raise(x, tid);
+    if (!peer_wait(x, tid, clock64())) s_ok = 0u;
+    const uint32_t world = x.world ? x.world : 1u, rank = x.rank;
+    if (tid < world) {
+        const uint32_t f = tid == rank ? __ldcg(m.gate) : __ldcg(&x.my_stage[(size_t)tid * m.slice4]).x;
+        if (f) {
+            s_ok = 0u;
+            if (blockIdx.x == 0 && tid != rank) x.err.set(ERR_BAD_OFFSETS);   // a peer's fault fails the call here too
+        }
+    }
+    __syncthreads();
+    if (!s_ok) return;
+    const uint32_t lane = tid & 31;
+    const uint32_t warp = (blockIdx.x * blockDim.x + tid) >> 5, n_warp = (gridDim.x * blockDim.x) >> 5;
+    const bool dense = m.cand_off == nullptr;
+    for (uint32_t p = warp; p < m.n_pod; p += n_warp) {
+        const uint4* src = nullptr;
+        uint4 A = make_uint4(DRA_GPU_NONE, DRA_GPU_NONE, 0u, 0u), B = make_uint4(0u, 0u, 0u, 0u);
+        if (lane < world) {
+            src = (lane == rank ? m.part : x.my_stage + (size_t)lane * m.slice4) + 1 + (size_t)p * m.stride;
+            A = __ldcg(&src[0]); B = __ldcg(&src[1]);
+        }
+        const uint32_t fit = __reduce_min_sync(FULLMASK, A.x);
+        const bool lim = __any_sync(FULLMASK, B.y != 0u);
+        uint32_t best = A.y, win = lane;
+        uint4 bs = make_uint4(0u, A.z, A.w, B.x);
+        unsigned long long b64 = (unsigned long long)B.z | ((unsigned long long)B.w << 32);
+        for (uint32_t d = 16; d; d >>= 1) {
+            const uint32_t ob = __shfl_xor_sync(FULLMASK, best, d), ow = __shfl_xor_sync(FULLMASK, win, d);
+            uint4 os;
+            os.x = 0u; os.y = __shfl_xor_sync(FULLMASK, bs.y, d);
+            os.z = __shfl_xor_sync(FULLMASK, bs.z, d); os.w = __shfl_xor_sync(FULLMASK, bs.w, d);
+            const unsigned long long o64 = __shfl_xor_sync(FULLMASK, b64, d);
+            const bool take = ob != DRA_GPU_NONE &&
+                              (best == DRA_GPU_NONE || pre_better(os, o64, bs, b64) || (!pre_better(bs, b64, os, o64) && ob < best));
+            if (take) { best = ob; bs = os; b64 = o64; win = ow; }
+        }
+        const uint32_t c0 = __ldg(&m.pod_off[p]), cnt = __ldg(&m.pod_off[p + 1]) - c0;
+        bool inv = cnt > DRA_MAX_POD;
+        for (uint32_t i = lane; i < cnt && !inv; i += 32) {
+            const uint4 c = __ldg(&m.claims[c0 + i]);
+            const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
+            inv = claim_invalid(kind, prof, count, true) || claim_sel(kind, c.z, c.w) > m.sel.n_sel;
+        }
+        inv = __any_sync(FULLMASK, inv);
+        uint32_t st, k = DRA_GPU_NONE;
+        if (fit != DRA_GPU_NONE) { st = DRA_PRE_FITS; k = fit; }
+        else if (best != DRA_GPU_NONE) { st = DRA_PRE_EVICT; k = best; }
+        else st = inv ? DRA_PRE_INVALID : lim ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO;
+        const uint32_t nv = st == DRA_PRE_EVICT ? bs.y : 0u;
+        if (lane == 0) {
+            m.pod_status[p] = (uint8_t)st;
+            m.pod_node[p] = k == DRA_GPU_NONE ? DRA_GPU_NONE : dense ? k - p * m.n_node : __ldg(&m.cand_nodes[k]);
+            m.n_victims[p] = nv;
+        }
+        if (m.max_victims) {
+            const uint32_t* row = reinterpret_cast<const uint32_t*>(
+                (win == rank ? m.part : x.my_stage + (size_t)win * m.slice4) + 1 + (size_t)p * m.stride + 2);
+            const uint32_t n = min(nv, m.max_victims);
+            for (uint32_t j = lane; j < m.max_victims; j += 32)
+                m.victims[(size_t)p * m.max_victims + j] = j < n ? __ldcg(&row[j]) : DRA_GPU_NONE;
+        }
+    }
+    if (!m.pair_status && !m.pair_victims) return;
+    const size_t pair4 = 1 + (size_t)m.n_pod * m.stride;                 // a slice's pair results follow its partials
+    for (uint32_t k = blockIdx.x * blockDim.x + tid; k < m.n_pair; k += gridDim.x * blockDim.x) {
+        const uint32_t node = dense ? k % m.n_node : __ldg(&m.cand_nodes[k]);
+        uint2 v = make_uint2(DRA_PRE_NO, 0u);                             // a candidate naming no node
+        if (node < m.n_node) {
+            uint32_t r = 0;
+            while (r + 1 < world && m.bounds[r + 1] <= node) ++r;
+            const uint2* src = r == rank ? m.pairs : reinterpret_cast<const uint2*>(x.my_stage + (size_t)r * m.slice4 + pair4);
+            v = __ldcg(&src[k]);
+        }
+        if (m.pair_status) m.pair_status[k] = (uint8_t)v.x;
+        if (m.pair_victims) m.pair_victims[k] = v.y;
     }
 }
 
