@@ -311,7 +311,8 @@ typedef struct dra_running_pods {
  *                    order (priority descending, then index); the rest of the row 0xFFFFFFFF.
  * DRA_E_INVAL with nothing written: unknown flags, pod_off / cand_off / running->pod_off not monotone or not spanning,
  * dense n_pod * n_node >= 2^32, a running slot range outside running->n_out, a running pod whose OK slots name a GPU
- * index >= n_gpu or GPUs of two nodes, max_victims > 0 without victims.  Host buffers; flags: 0 or DRA_F_EXHAUSTIVE. */
+ * index >= n_gpu or GPUs of two nodes, max_victims > 0 without victims.  n_pod == 0 returns DRA_OK once flags, pod_off,
+ * cand_off and max_victims pass, without examining the running pods.  Host buffers; flags: 0 or DRA_F_EXHAUSTIVE. */
 int  dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
                        const uint32_t* pod_off, const int32_t* prio, uint32_t n_pod,
                        const uint32_t* cand_nodes, const uint32_t* cand_off,

@@ -147,9 +147,10 @@ PREEMPT_API int preempt_oracle_preempt(const dra_gpu_rec* gpus, uint32_t n_gpu, 
         if (!cand_off || cand_off[0] != 0) return -1;
         for (uint32_t p = 0; p < n_pod; p++) if (cand_off[p + 1] < cand_off[p]) return -1;
     } else if ((uint64_t)n_pod * n_node >= (1ull << 32)) return -1;
+    if (max_victims && !victims) return -1;
+    if (n_pod == 0) return 0;                            /* no pending pods: the running pods are not examined */
     if (rpod_off[0] != 0 || rpod_off[rn_pod] != rn_claim) return -1;
     for (uint32_t r = 0; r < rn_pod; r++) if (rpod_off[r + 1] < rpod_off[r]) return -1;
-    if (max_victims && !victims) return -1;
     running R = { rclaims, rpod_off, rprio, rout_off, rout, n_node };
     /* where each running pod is: the node of its OK slots' GPUs */
     uint32_t* rnode = (uint32_t*)malloc(((size_t)rn_pod + 1) * sizeof(uint32_t));

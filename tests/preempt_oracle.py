@@ -129,6 +129,8 @@ def preempt_naive(gpus, node_off, table, claims, pod_off, prio, cands, exhaustiv
     lists of dicts as naive.py takes them; run_out: list of (gpu, start, size, profile, status); cands: one list of node
     indices per pod, or None for every node ascending.  Returns the six outputs as lists."""
     from oracle import naive as N
+    if len(pod_off) == 1:                                # no pending pods: the running pods are not examined
+        return [], [], [], [], [], []
     n_node = len(node_off) - 1
     G0 = N._state(gpus)
     prio, run_prio = [int(x) for x in prio], [int(x) for x in run_prio]

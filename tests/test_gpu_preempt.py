@@ -153,13 +153,14 @@ def test_the_full_flow(pkg, pctx, oracle):
         assert done
 
 
-def _raw(pkg, ctx, g, a, sentinel):
-    """dra_preempt_batch on sentinel-filled outputs; returns (rc, outputs)"""
+def _raw(pkg, ctx, g, a, sentinel, slack=0):
+    """dra_preempt_batch on sentinel-filled outputs (each `slack` elements longer than the call needs); returns (rc,
+    outputs)"""
     A = pkg.api
     n_pod = len(a["po"]) - 1
     n_pair = n_pod * ctx.n_node if a["co"] is None else int(a["co"][-1])
     def filled(n, dtype):                                 # every byte = sentinel
-        return np.full(max(n, 1) * np.dtype(dtype).itemsize, sentinel, np.uint8).view(dtype)
+        return np.full((max(n, 1) + slack) * np.dtype(dtype).itemsize, sentinel, np.uint8).view(dtype)
     outs = [filled(n_pair, np.uint8), filled(n_pair, np.uint32)] + \
            [filled(n_pod, d) for d in (np.uint32, np.uint8, np.uint32)] + [filled(n_pod * a["mv"], np.uint32)]
     keep = [np.ascontiguousarray(a[k], dtype=d) if a[k] is not None else None for k, d in
