@@ -1930,7 +1930,7 @@ k_pack(const PackArgs a) {
 // n_node SMs and every byte after the first CTA's touch comes from L2.
 // dynamic smem: [tbl 1024][bars 16][inv 512][live 1024+128][counts 64][index lists: n_claim u32, warp w at w*chunk]
 constexpr uint32_t FU_TBL = 0, FU_TBAR = 1024, FU_IBAR = 1032, FU_INV = 1040, FU_LIVE = 1552, FU_CNT = 2704, FU_LIST = 2832;   // counts: up to 32 warps
-constexpr uint32_t FU_PIECE = 256;          // claims per staged piece (4 KiB bulk copy, own mbarrier)
+constexpr uint32_t FU_PIECE = 256;          // claims per staged piece: one warp's 8 loads of 32 claims
 constexpr uint32_t FU_MAXPIECE = 8;         // pieces per warp part => staging needs n_claim <= NW * 2048
 // per-warp part of the claim array: a multiple of 32 claims, of a whole piece when the array is staged
 __host__ __device__ constexpr uint32_t fused_chunk(uint32_t n_claim, int nw, bool stage) {
@@ -1940,6 +1940,7 @@ __host__ __device__ constexpr uint32_t fused_chunk(uint32_t n_claim, int nw, boo
 __host__ __device__ constexpr size_t fused_list_bytes(uint32_t n_claim, int nw, bool stage) {
     return (size_t)fused_chunk(n_claim, nw, stage) * nw * 4;
 }
+// (staged: the NW * FU_MAXPIECE * 8 bytes in front of the index lists are unused, kept so the staged capacity stays 11,117 claims)
 __host__ __device__ constexpr size_t fused_smem_bytes(uint32_t n_claim, int nw, bool stage) {
     return FU_LIST + (stage ? (size_t)nw * FU_MAXPIECE * 8 : 0) + fused_list_bytes(n_claim, nw, stage) + 16 + (stage ? (size_t)n_claim * 16 + 16 : 0);
 }
@@ -2003,7 +2004,7 @@ __device__ __forceinline__ void grid_barrier(uint32_t* gbar, uint32_t n_cta, con
 // (`again`: the shared-memory barriers of the previous batch are invalidated first).
 // What differs from batch to batch (resident mode keeps everything else in the kernel's parameter space)
 struct Batch {
-    uint32_t n_claim, n_out, have_off, serve;
+    uint32_t n_claim, n_out, have_off;
     const uint4* inv_src;
     const uint32_t* out_off;
     const uint4* h_claims; const uint32_t* h_out_off; uint2* h_out;
@@ -2019,7 +2020,6 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
     const uint32_t tbar = sbase + FU_TBAR, ibar = sbase + FU_IBAR;
     const uint32_t list_addr = sbase + FU_LIST + (STAGE ? (uint32_t)NW * FU_MAXPIECE * 8u : 0u);
     const uint32_t stage_addr = STAGE ? ((list_addr + (uint32_t)fused_list_bytes(b.n_claim, NW, STAGE) + 15u) & ~15u) : 0u;
-    const uint32_t sbar = sbase + FU_LIST;       // STAGE: one mbarrier per 4 KiB piece of the claim array
     // multi-GPU send queue: behind everything else of the layout; [q_cap entries of 16 B]; its counter and end marker
     // live in the spare words of the counts area
     const uint32_t q_base = (sbase + (uint32_t)fused_smem_bytes(b.n_claim, NW, STAGE) + 15u) & ~15u;
@@ -2033,33 +2033,27 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
     // round trip 1: extents (needed for the inventory copy); table copy goes out immediately
     uint32_t g0 = 0, g1 = 0;
     if (has_node) { g0 = __ldg(&a.node_off[node]); g1 = __ldg(&a.node_off[node + 1]); }
-    // barrier init spread over the threads (one mbarrier.init each), then one fence + sync
+    // the table and inventory barriers, then one fence + sync
     if (again) {                                   // resident mode: the previous batch's barriers are dead objects now
         // warp 0 wrote this node's GpuRecs with generic stores in the previous batch; the bulk copy below reads them
         // through the async proxy
         asm volatile("fence.proxy.async;" ::: "memory");
         __syncthreads();
         if (threadIdx.x == 0) { mbar_inval_a(tbar); mbar_inval_a(ibar); }
-        if (STAGE && threadIdx.x < NW * FU_MAXPIECE) mbar_inval_a(sbar + threadIdx.x * 8);
         __syncthreads();
     }
     if (threadIdx.x == 0) { mbar_init_a(tbar, 1); mbar_init_a(ibar, 1); }
-    if (STAGE) {                                   // (resident mode initialises all of them: the next batch may be larger)
-        const uint32_t npt_ = again || b.serve ? NW * FU_MAXPIECE : (b.n_claim + FU_PIECE - 1) / FU_PIECE;
-        if (threadIdx.x < npt_) mbar_init_a(sbar + threadIdx.x * 8, 1);
-    }
     mbar_fence_init();
     __syncthreads();
     if (threadIdx.x == 0) tma_load_a(sbase + FU_TBL, a.tbl, 1024u, tbar);
     const uint32_t ng = g1 - g0;
-    if (threadIdx.x == 32 && ng) tma_load_a(sbase + FU_INV, b.inv_src + g0, ng * 16u, ibar);     // (issuing it after the claim pieces instead: measured, no gain)
+    if (threadIdx.x == 32 && ng) tma_load_a(sbase + FU_INV, b.inv_src + g0, ng * 16u, ibar);
     // sharded call: the claim list was compacted on the device by the kernel before this one; b.n_claim is its capacity
     if (a.sh_on) {
         // ... or right here: one 1024-claim tile per CTA (cooperative launch), a grid barrier, and the list is there —
         // no second launch; the table and inventory copies above are already in flight behind it
         if (blockIdx.x < a.sh.n_tiles) shard_tile_flat<SC_IN_ROWS>(a.sh, blockIdx.x);
         grid_barrier(a.dio.gbar, gridDim.x, a.err);
-        asm volatile("fence.proxy.async;" ::: "memory");     // generic-proxy stores (other SMs) -> bulk-copy reads
     }
     else if (a.n_dev) pdl_wait();                            // (launched as a programmatic dependent of the compaction)
     const uint32_t n_claim = a.n_dev ? min(b.n_claim, __ldcg(a.n_dev)) : b.n_claim;
@@ -2073,37 +2067,37 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
 
     if (STAGE && b.h_claims) {
         // direct ingest: one 16-byte load from the caller's pinned buffer per thread (a single PCIe round trip for
-        // the whole grid), stored to the device copy that everybody's bulk copies below read from L2.
-        // (Per-piece ready flags instead of the grid barrier were tried: slower to the first bulk copy — every
-        // producer then pays its own fence on the critical path.)
+        // the whole grid), stored to the device copy that every CTA's filter below reads from L2.
+        // (Per-piece ready flags instead of the grid barrier were tried while the stage was filled by bulk copies: slower
+        // — every producer then pays its own fence on the critical path.)
         DRA_DSTAMP(0);
         const uint32_t nthr = gridDim.x * (NW * 32), t0 = blockIdx.x * (NW * 32) + threadIdx.x;
         for (uint32_t i = t0; i < b.n_claim; i += nthr) a.dio.d_claims[i] = __ldcs(b.h_claims + i);
         if (b.h_out_off) for (uint32_t i = t0; i < b.n_claim; i += nthr) a.dio.d_out_off[i] = __ldcs(b.h_out_off + i);
         DRA_DSTAMP(1);
         grid_barrier(a.dio.gbar, gridDim.x, a.err);
-        asm volatile("fence.proxy.async;" ::: "memory");       // generic-proxy stores (other SMs) -> bulk-copy reads
         DRA_DSTAMP(2);
-    }
-    if (STAGE) {
-        // every warp arms and issues the pieces of its own part of the filter, in order: TMA issues from one warp
-        // serialise, so they are spread over the 8 warps' lane 0, and the copies land about in issue order — each
-        // warp's first piece is among the first to arrive.  (Dealt round-robin over the warps, the pieces land in array
-        // order: the last warp's part lands last and the CTA waits ~3,400 cycles for it on cfg2, profiles/timeline.py.)
-        const uint32_t part = fused_chunk(n_claim, NW, true);
-        const uint32_t g_end = (min(n_claim, (wid + 1) * part) + FU_PIECE - 1) / FU_PIECE;
-        if (lane == 0)
-            for (uint32_t g = wid * part / FU_PIECE; g < g_end; ++g) {
-                const uint32_t c0 = g * FU_PIECE, bytes = min(FU_PIECE, n_claim - c0) * 16u;
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sbar + g * 8), "r"(bytes) : "memory");
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                             ::"r"(stage_addr + (c0 << 4)), "l"(a.claims + c0), "r"(bytes), "r"(sbar + g * 8) : "memory");
-            }
     }
     DRA_STAMP(2);
 
-    // warp 0 sets up the node (inventory, table row properties) NOW: it needs only the table and the GpuRecs, which
-    // land long before the claim pieces — after the filter this would sit on the critical path
+    const uint32_t chunk = fused_chunk(n_claim, NW, STAGE);            // per-warp part of the filter
+    const uint32_t lo = wid * chunk, hi = min(n_claim, lo + chunk);
+    // STAGE: each lane loads whole claims into registers, tests the key there and stores the claim into the stage, from
+    // which the pack, the stray CTA and the tail read it after the filter's __syncthreads.  (Filling the stage with
+    // 4 KiB bulk copies instead left the filter waiting for them to be issued and land: profiles/timeline.py.)
+    // L2-coherent loads only: the array may have been written inside this launch by other CTAs (direct-I/O ingest,
+    // in-kernel compaction) or, in k_serve, rewritten for this batch while the kernel stayed up.
+    // The first 8 claims of every lane go out now, so warp 0's are in flight while it waits for the table and GpuRecs.
+    constexpr int U = 8;
+    const uint4 none = make_uint4(0u, 0xFFFFFFFFu, 0u, 0u);
+    uint4 cur[U];
+    if (STAGE) {
+        #pragma unroll
+        for (int u = 0; u < U; ++u) { const uint32_t i = lo + u * 32 + lane; cur[u] = i < hi ? __ldcg(a.claims + i) : none; }
+    }
+
+    // warp 0 sets up the node (inventory, table row properties) NOW: it needs only the table and the GpuRecs, in flight
+    // since the entry — after the filter this would sit on the critical path
     NodeCtx x;
     uint4 rec = make_uint4(0, 0, 0, 0);
     if (wid == 0 && has_node) {
@@ -2120,15 +2114,14 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
     }
 
     // ---- filter: which claims select this node (all warps) ------------------------------------------
-    const uint32_t chunk = fused_chunk(n_claim, NW, STAGE);            // per-warp part
-    const uint32_t lo = wid * chunk, hi = min(n_claim, lo + chunk);
     const uint32_t ltmask = lanemask_lt();
     const uint32_t my_list = list_addr + (lo << 2);
     const uint32_t want = has_node ? node : 0xFFFFFFFEu;
     const bool stray_cta = node == a.n_node;
     uint32_t cntw = 0, slot_l = 0;                                     // slot_l: OutRec slots of this lane's matches (gather only)
     const bool gather = a.peer.world != 0;
-    auto scan = [&](const uint32_t i, const uint32_t keyv) {          // one claim per lane; warp-uniform control flow
+    // one claim per lane; warp-uniform control flow.  xv: the claim's first word (STAGE only, loaded with the key)
+    auto scan = [&](const uint32_t i, const uint32_t keyv, const uint32_t xv) {
         // CTA n_node collects the claims that name no node of the inventory (they become INVALID, spec §3)
         const bool m = has_node ? keyv == want : (stray_cta && i < hi && keyv >= a.n_node);
         const uint32_t bm = __ballot_sync(FULLMASK, m);
@@ -2136,7 +2129,7 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
             if (m) {
                 sts32(my_list + ((cntw + (uint32_t)__popc(bm & ltmask)) << 2), i);
                 if (gather) {                                          // the packet range is reserved while the pack runs
-                    const uint32_t x_ = STAGE ? lds32(stage_addr + (i << 4)) : __ldg(reinterpret_cast<const uint32_t*>(a.claims) + 4 * (size_t)i);
+                    const uint32_t x_ = STAGE ? xv : __ldg(reinterpret_cast<const uint32_t*>(a.claims) + 4 * (size_t)i);
                     const uint32_t kind = x_ & 0xFFu, count = x_ >> 16;
                     slot_l += (!stray_cta && kind == DRA_KIND_GPU && !claim_invalid(kind, 0, count, b.have_off != 0)) ? count : 1u;
                 }
@@ -2144,22 +2137,22 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
             cntw += (uint32_t)__popc(bm);
         }
     };
-    constexpr int U = 8;
-    if (STAGE) {
-        // the whole array is in flight as 4 KiB TMA bulk copies (issued above); each warp scans the pieces of its
-        // part from shared memory as they land, and the pack phase later reads the claims from the same copy
-        const uint32_t npiece = hi > lo ? (hi - lo + FU_PIECE - 1) / FU_PIECE : 0;
-        const uint32_t g_first = lo / FU_PIECE;                         // parts are whole pieces (fused_chunk)
-        for (uint32_t q = 0; q < npiece; ++q) {
-            mbar_wait_a(sbar + (g_first + q) * 8, 0);
-            uint32_t kv[U];
+    if (STAGE) {                                                       // (the first 8 claims were issued above)
+        uint4 nxt[U];
+        for (uint32_t base = lo; base < hi; base += 32 * U) {
             #pragma unroll
-            for (int u = 0; u < U; ++u) {                      // all 8 shared loads in flight before the first test
-                const uint32_t i = lo + q * FU_PIECE + u * 32 + lane;
-                kv[u] = i < hi ? lds32(stage_addr + (i << 4) + 4) : 0xFFFFFFFFu;
+            for (int u = 0; u < U; ++u) {                      // next batch goes out before this one is looked at
+                const uint32_t i = base + 32 * U + u * 32 + lane;
+                nxt[u] = i < hi ? __ldcg(a.claims + i) : none;
             }
             #pragma unroll
-            for (int u = 0; u < U; ++u) scan(lo + q * FU_PIECE + u * 32 + lane, kv[u]);
+            for (int u = 0; u < U; ++u) {
+                const uint32_t i = base + u * 32 + lane;
+                if (i < hi) sts128(stage_addr + (i << 4), cur[u]);
+                scan(i, cur[u].y, cur[u].x);
+            }
+            #pragma unroll
+            for (int u = 0; u < U; ++u) cur[u] = nxt[u];
         }
     } else {
         const uint32_t* keyp = reinterpret_cast<const uint32_t*>(a.claims) + 1;      // .y of claim i at keyp[4*i]
@@ -2173,7 +2166,7 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
                 nxt[u] = i < hi ? __ldg(keyp + 4 * (size_t)i) : 0xFFFFFFFFu;
             }
             #pragma unroll
-            for (int u = 0; u < U; ++u) scan(base + u * 32 + lane, key[u]);
+            for (int u = 0; u < U; ++u) scan(base + u * 32 + lane, key[u], 0u);
             #pragma unroll
             for (int u = 0; u < U; ++u) key[u] = nxt[u];
         }
@@ -2334,7 +2327,7 @@ template <int NW, bool STAGE>
 __global__ void __launch_bounds__(NW * 32, 1)
 k_fused(const PackArgs a) {
     extern __shared__ __align__(16) uint8_t dyn_smem[];
-    const Batch b{a.n_claim, a.n_out, a.have_off, 0u, a.inv_src, a.out_off, a.dio.h_claims, a.dio.h_out_off, a.dio.h_out};
+    const Batch b{a.n_claim, a.n_out, a.have_off, a.inv_src, a.out_off, a.dio.h_claims, a.dio.h_out_off, a.dio.h_out};
     fused_body<NW, STAGE>(a, b, dyn_smem, false);
 }
 
@@ -2406,7 +2399,7 @@ k_serve(const ServeArgs s) {
         }
         const PackArgs& a = s.base;
         Batch b;
-        b.n_claim = n_claim; b.n_out = n_out; b.serve = 1u;
+        b.n_claim = n_claim; b.n_out = n_out;
         b.inv_src = (flags & DRA_F_FRESH_INVENTORY) ? s.inv_pristine : const_cast<const uint4*>(s.base.inv_dst);
         b.h_claims = reinterpret_cast<const uint4*>(((unsigned long long)cmd_s[5] << 32) | cmd_s[4]);
         b.h_out_off = reinterpret_cast<const uint32_t*>(((unsigned long long)cmd_s[7] << 32) | cmd_s[6]);

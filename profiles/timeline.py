@@ -18,7 +18,7 @@ for it in range(6):
     ctx.sync()
 tl = ctx.debug_timeline(w.n_node + 1).astype(np.uint64)
 node = tl[: w.n_node]
-names = ["entry -> barriers/TMA issued", "filter", "sync", "table/inventory wait + first fetch", "pack (warp 0)"]
+names = ["entry: table/inventory copies issued", "filter", "sync", "table/inventory wait + first fetch", "pack (warp 0)"]
 for k, nm in enumerate(names):
     d = (node[:, k + 2] - node[:, k + 1]).astype(np.int64)
     print(f"{nm:36s} cycles: median {int(np.median(d)):6d}  p90 {int(np.percentile(d, 90)):6d}  max {int(d.max()):6d}")
