@@ -255,9 +255,10 @@ CONFIGS = {"cfg1": cfg1, "cfg2": cfg2, "cfg3": cfg3, "cfg4": cfg4, "cfg5": cfg5}
 def homog(n_claim: int = 3000, n_node: int = 24, seed: int = 1, model: int = 0, wide16: bool = False,
           max_width: int = 32) -> Workload:
     """Homogeneous all-MIG nodes of widths 1..max_width with pre-occupied, fully-allocated and unavailable
-    GPUs, MIG-only claims incl. unsupported profiles: the workload class of the packers' fast loops (the
-    64-bit SWAR form for <= 8 GPUs x <= 8 slices, the ballot form for anything wider).  ``wide16`` swaps in a
-    synthetic 16-slice part so that occupancy masks do not fit a byte."""
+    GPUs, MIG-only claims incl. unsupported profiles: the workload class of the packers' lean plain-MIG loop
+    (one lane per GPU, a ballot picks the lowest GPU; 3 shift steps when the table row has no shape above
+    8 slices, 4 otherwise).  ``wide16`` swaps in a synthetic 16-slice part so that occupancy masks do not fit
+    a byte and the 4-step form runs."""
     r = splitmix64(BASE_SEED + 900 + seed, 8 * (n_node * 40 + n_claim) + 64)
     sizes = 1 + (r[:n_node] % np.uint64(max_width)).astype(np.int64)
     sizes[::3] = np.minimum(sizes[::3], 8)

@@ -106,7 +106,7 @@ def test_large_batch_through_a_replayed_graph(pkg, oracle):
         pc.free(); po.free()
 
 
-# ---- the packers' fast loops: 64-bit SWAR node state (<= 8 GPUs x <= 8 slices) and the ballot form (wider) ----
+# ---- the packers' lean plain-MIG loop: one lane per GPU and a ballot; 3 shift steps for rows of <= 8 slices, 4 wider ----
 @pytest.mark.parametrize("seed,model,wide16,max_width", [
     (0, 0, False, 8), (1, 0, False, 32), (2, 1, False, 8), (3, 0, True, 8), (4, 0, True, 32), (5, 1, False, 32),
     (6, 0, False, 1), (7, 0, False, 9)])
