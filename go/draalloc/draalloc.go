@@ -330,6 +330,81 @@ func (c *Context) PreemptBatch(claims []ClaimRec, podOff []uint32, prio []int32,
 	return r, nil
 }
 
+// Preempt-and-place answer (spec §15).  Per pod: the node chosen (0xFFFFFFFF: none) and its status (DRA_PRE_*).  Per
+// running pod: the pending pod that evicted it, 0xFFFFFFFF when none.
+type PreemptPlacement struct {
+	Out       []OutRec
+	PodNode   []uint32
+	PodStatus []uint8
+	EvictedBy []uint32
+}
+
+// PreemptPlaceBatch runs PostFilter and Reserve for a whole batch in one call (dra_preempt_place_batch, spec §15): pods
+// in input order, each judged as PreemptBatch judges it on the inventory the pods before it left, then applied — its
+// victims released, the pod allocated on the chosen node.  Candidates as PlaceBatch (cands == candOff == nil: every
+// node, ascending); outOff / nOut as PlaceBatch.  The call releases the victims itself: do not pass them to
+// DeallocateBatch again.  Unbuilt, like the rest of this file.
+func (c *Context) PreemptPlaceBatch(claims []ClaimRec, podOff []uint32, prio []int32, cands, candOff []uint32,
+	run RunningPods, outOff []uint32, nOut int, flags uint32) (*PreemptPlacement, error) {
+	nPod := len(podOff) - 1
+	if nPod <= 0 || len(run.PodOff) == 0 {
+		return &PreemptPlacement{Out: make([]OutRec, nOut)}, nil
+	}
+	r := &PreemptPlacement{make([]OutRec, nOut+1), make([]uint32, nPod), make([]uint8, nPod), make([]uint32, len(run.PodOff))}
+	var cp, rcp *C.dra_claim_rec
+	var oo, cn, co, roo *C.uint32_t
+	if len(claims) > 0 {
+		cp = (*C.dra_claim_rec)(unsafe.Pointer(&claims[0]))
+	}
+	if outOff != nil {
+		oo = (*C.uint32_t)(unsafe.Pointer(&outOff[0]))
+	}
+	if candOff != nil {
+		co = (*C.uint32_t)(unsafe.Pointer(&candOff[0]))
+		if len(cands) == 0 {
+			cands = []uint32{0} // an empty list still needs an address (nil means the dense form)
+		}
+		cn = (*C.uint32_t)(unsafe.Pointer(&cands[0]))
+	}
+	if len(run.Claims) > 0 {
+		rcp = (*C.dra_claim_rec)(unsafe.Pointer(&run.Claims[0]))
+	}
+	var rp *C.int32_t
+	if len(run.Prio) > 0 {
+		rp = (*C.int32_t)(unsafe.Pointer(&run.Prio[0]))
+	}
+	if run.OutOff != nil {
+		roo = (*C.uint32_t)(unsafe.Pointer(&run.OutOff[0]))
+	}
+	var rop *C.dra_out_rec
+	if len(run.Out) > 0 {
+		rop = (*C.dra_out_rec)(unsafe.Pointer(&run.Out[0]))
+	}
+	// the struct handed to C holds Go pointers: cgo accepts that only for pinned memory
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, q := range []unsafe.Pointer{unsafe.Pointer(rcp), unsafe.Pointer(&run.PodOff[0]), unsafe.Pointer(rp),
+		unsafe.Pointer(roo), unsafe.Pointer(rop)} {
+		if q != nil {
+			pin.Pin(q)
+		}
+	}
+	cr := C.dra_running_pods{claims: rcp, n_claim: C.uint32_t(len(run.Claims)),
+		pod_off: (*C.uint32_t)(unsafe.Pointer(&run.PodOff[0])), n_pod: C.uint32_t(len(run.PodOff) - 1), prio: rp,
+		out_off: roo, out: rop, n_out: C.uint32_t(len(run.Out))}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_preempt_place_batch(c.h, cp, C.uint32_t(len(claims)), (*C.uint32_t)(unsafe.Pointer(&podOff[0])),
+		(*C.int32_t)(unsafe.Pointer(&prio[0])), C.uint32_t(nPod), cn, co, &cr, oo,
+		(*C.dra_out_rec)(unsafe.Pointer(&r.Out[0])), C.uint32_t(nOut), (*C.uint32_t)(unsafe.Pointer(&r.PodNode[0])),
+		(*C.uint8_t)(unsafe.Pointer(&r.PodStatus[0])), (*C.uint32_t)(unsafe.Pointer(&r.EvictedBy[0])), C.uint32_t(flags))
+	if rc != 0 {
+		return nil, lastError(c.h)
+	}
+	r.Out, r.EvictedBy = r.Out[:nOut], r.EvictedBy[:len(run.PodOff)-1]
+	return r, nil
+}
+
 func (c *Context) DeallocateBatch(claims []ClaimRec, outOff []uint32, out []OutRec) error {
 	if len(claims) == 0 {
 		return nil

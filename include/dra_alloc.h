@@ -321,6 +321,37 @@ int  dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
                        uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
                        uint32_t* victims, uint32_t max_victims, uint32_t flags);
 
+/* Preempt and place (spec §15): dra_preempt_batch's question for a batch that sees itself, answered and applied.  Pods
+ * are taken in input order; pod p is judged as dra_preempt_batch judges it, but on the inventory as the pods before it
+ * left it (their placements held, their victims gone), with only the running pods no earlier pod evicted as possible
+ * victims; the pods of the call are never victims.  Its choice is then applied: for EVICT the victims are released from
+ * the live inventory as dra_deallocate_batch releases them; for FITS or EVICT the pod is allocated on the chosen node as
+ * dra_allocate_pods_batch allocates it, OutRecs written.  The result is byte for byte the host loop, per pod:
+ * dra_preempt_batch with that one pod and the running pods not yet evicted, dra_deallocate_batch of its victims,
+ * dra_allocate_pods_batch of its claims on the chosen node.
+ *   claims / pod_off / prio / candidates   as dra_preempt_batch (cand_nodes == cand_off == NULL: dense form); each
+ *                    claim's node field is ignored and never written
+ *   running          the running pods, as dra_preempt_batch takes them
+ *   out_off / out[n_out]  as dra_place_pods_batch: slots counted as if each claim named a node of the inventory
+ *   pod_node[p]      the node chosen (FITS or EVICT), else 0xFFFFFFFF     pod_status[p]  DRA_PRE_*
+ *   evicted_by[r]    the pod that evicted running pod r, else 0xFFFFFFFF (each pod's victims in eviction order:
+ *                    priority descending, then index)
+ * A pod placed nowhere takes nothing: its slots carry DRA_ST_SEARCH_LIMIT when its status is DRA_PRE_SEARCH_LIMIT, else
+ * DRA_ST_POD (DRA_ST_INVALID for claims invalid by §3/§10, every claim of a pod of more than DRA_MAX_POD).  An empty pod
+ * is FITS on its first candidate naming a node, with nothing written.  The call RELEASES THE VICTIMS ITSELF: their
+ * allocations are gone from the live inventory when it returns, so the caller must not pass them to
+ * dra_deallocate_batch again.  DRA_E_INVAL, with no output and no inventory word written: unknown flags, pod_off /
+ * cand_off / running->pod_off not monotone or not spanning, more than 2^30 - 1 candidates for a pod or nodes in the
+ * inventory, dense n_pod * n_node >= 2^32, a pending slot outside n_out, a running slot range outside running->n_out, a
+ * running pod whose OK slots name a GPU index >= n_gpu or GPUs of two nodes.  n_pod == 0 returns DRA_OK after the
+ * checks of the pending arrays, without examining the running pods.  Host buffers; flags: 0 or DRA_F_EXHAUSTIVE. */
+int  dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
+                             const uint32_t* pod_off, const int32_t* prio, uint32_t n_pod,
+                             const uint32_t* cand_nodes, const uint32_t* cand_off,
+                             const dra_running_pods* running,
+                             const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
+                             uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, uint32_t flags);
+
 /* Deallocate(): stands in for controller.Driver.Deallocate(ctx, claim).  Inverse update from the
  * claims and the OutRecs dra_allocate_batch produced for them (same out_off convention). */
 int  dra_deallocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
@@ -590,6 +621,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_PLACE_SHARD       0x400000u /* sharded place pods: prep, gate, walk of the node window, finalisers (+ all-gather) */
 #define DRA_K_PREEMPT           0x800000u /* preemption: running-pod prep, victim lists, pairs, choice, victim rows */
 #define DRA_K_PREEMPT_SHARD    0x1000000u /* sharded preemption: prep, victim lists, the window's pairs, partials, merge */
+#define DRA_K_PREEMPT_PLACE    0x2000000u /* preempt and place: running-pod prep, victim lists, visit lists, persistent walk */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

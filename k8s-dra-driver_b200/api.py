@@ -24,7 +24,8 @@ KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x0
            "hist_warp": 0x00100, "scan8": 0x00200, "scan_rows": 0x00400, "scan": 0x00800, "scatter": 0x01000,
            "pack1": 0x02000, "pack4": 0x04000, "compact_flat1": 0x08000, "compact_flat8": 0x10000,
            "compact_lookback": 0x20000, "compact_in_kernel": 0x40000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000,
-           "place_shard": 0x400000, "preempt": 0x800000, "preempt_shard": 0x1000000}
+           "place_shard": 0x400000, "preempt": 0x800000, "preempt_shard": 0x1000000,
+           "preempt_place": 0x2000000}
 
 
 class DraError(RuntimeError):
@@ -65,6 +66,7 @@ SYMBOLS = {
     "dra_place_pods_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u32]),
     "dra_deallocate_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_preempt_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32]),
+    "dra_preempt_place_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _u32]),
     "dra_comm_unique_id": (_i32, [_vp]),
     "dra_comm_init": (_i32, [_vp, _vp, _i32, _i32]),
     "dra_allocate_batch_gather_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _u32, _u32]),
@@ -370,6 +372,44 @@ class Context:
                                                 max_victims, flags))
         return (pair_status[:n_pair], pair_victims[:n_pair], pod_node[:n_pod], pod_status[:n_pod], n_victims[:n_pod],
                 victims[:n_pod * max_victims].reshape(n_pod, max_victims))
+
+    def preempt_place(self, claims, pod_off, prio, run_claims, run_pod_off, run_prio, run_out, run_out_off=None,
+                      cand_nodes=None, cand_off=None, out_off=None, n_out=None, flags: int = 0):
+        """Preempt and place (spec §15): pods in input order, each judged as preempt() judges it on the inventory the pods
+        before it left (their placements held, their victims gone), then applied: its victims released, the pod allocated
+        on the chosen node.  Running pods as preempt() takes them; candidates and out_off / n_out as place_pods().  The
+        call releases the victims itself: do not deallocate them again.  Returns (out, pod_node, pod_status, evicted_by);
+        evicted_by[r] = the pod that evicted running pod r, 0xFFFFFFFF when none.  flags: 0 or F_EXHAUSTIVE."""
+        c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
+        po = np.ascontiguousarray(pod_off, dtype=np.uint32)
+        pr = np.ascontiguousarray(prio, dtype=np.int32)
+        n_pod = len(po) - 1
+        oo = None if out_off is None else np.ascontiguousarray(out_off, dtype=np.uint32)
+        if n_out is None:
+            placed = c.copy()
+            placed["node"] = 0                         # slots as if every claim named a node of the inventory
+            n_out = len(c) if oo is None else int(R.claim_slots(placed, 1).sum())
+        rc_ = np.ascontiguousarray(run_claims, dtype=R.CLAIM_DTYPE)
+        rpo = np.ascontiguousarray(run_pod_off, dtype=np.uint32)
+        rpr = np.ascontiguousarray(run_prio, dtype=np.int32)
+        ro = np.ascontiguousarray(run_out, dtype=R.OUT_DTYPE)
+        roo = None if run_out_off is None else np.ascontiguousarray(run_out_off, dtype=np.uint32)
+        cn = co = None
+        if cand_nodes is not None or cand_off is not None:
+            co = np.ascontiguousarray(cand_off, dtype=np.uint32)
+            cn = np.ascontiguousarray(cand_nodes if cand_nodes is not None else [], dtype=np.uint32)
+            if len(cn) == 0:
+                cn = np.zeros(1, np.uint32)            # NULL would mean the dense form
+        run = RunningPods(rc_.ctypes.data, len(rc_), rpo.ctypes.data, len(rpo) - 1, rpr.ctypes.data,
+                          None if roo is None else roo.ctypes.data, ro.ctypes.data, len(ro))
+        out = np.zeros(max(n_out, 1), dtype=R.OUT_DTYPE)
+        pod_node = np.zeros(max(n_pod, 1), dtype=np.uint32)
+        pod_status = np.zeros(max(n_pod, 1), dtype=np.uint8)
+        evicted_by = np.zeros(max(len(rpo) - 1, 1), dtype=np.uint32)
+        self._check(self._lib.dra_preempt_place_batch(self._h, _ptr(c), len(c), _ptr(po), _ptr(pr), n_pod, _ptr(cn), _ptr(co),
+                                                      C.byref(run), _ptr(oo), _ptr(out), n_out, _ptr(pod_node),
+                                                      _ptr(pod_status), _ptr(evicted_by), flags))
+        return out[:n_out], pod_node[:n_pod], pod_status[:n_pod], evicted_by[:len(rpo) - 1]
 
     def deallocate(self, claims, out, out_off=None):
         c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)

@@ -110,6 +110,12 @@ struct dra_ctx {
     uint32_t *d_pre_rpodoff = nullptr, *d_pre_rprio = nullptr; uint4 *d_pre_rrec = nullptr, *d_pre_vlist = nullptr; size_t cap_pre_rpods = 0;
     uint2* d_pre_rout = nullptr; size_t cap_pre_rout = 0;
     uint32_t* d_pre_vic = nullptr; size_t cap_pre_vic = 0;
+    // preempt and place (spec §15): per pending pod, per running pod, per node (the running lists' offsets, the last pod
+    // judged there)
+    uint32_t* d_pp_pending = nullptr; size_t cap_pp_pods = 0;
+    uint32_t* d_pp_evicted = nullptr; size_t cap_pp_rpods = 0;
+    uint32_t *d_pp_runoff = nullptr, *d_pp_judged = nullptr; size_t cap_pp_nodes = 0;
+    int pp_occ = -1;                      // resident CTAs of k_pods_preempt_place<4> per SM (occupancy query, once)
 
     // error flags
     uint32_t* d_err = nullptr;            // device memory
@@ -679,6 +685,9 @@ int check_err(dra_ctx* ctx) {
     cudaStreamSynchronize(ctx->stream);
     if (sp) return fail(ctx, DRA_E_STATE, "sharded call: %u claims fell into this shard, more than the launch was laid out for; nothing was changed, call again", ctx->h_sc_counts ? ctx->h_sc_counts[0] : 0u);
     if (dw) return fail(ctx, DRA_E_CUDA, "a device-side wait inside one kernel (grid barrier / look-back over CTAs) timed out: CTAs were not scheduled together; state is undefined, reload the inventory");
+    if (bo && (ctx->chain & DRA_K_PREEMPT_PLACE))
+        return fail(ctx, DRA_E_INVAL, "dra_preempt_place_batch: running pods: pod_off not monotone or not spanning the claims, a slot range "
+                                      "outside n_out, or OK slots naming a GPU index >= n_gpu or GPUs of two nodes; nothing was written");
     if (bo && (ctx->chain & DRA_K_PREEMPT))
         return fail(ctx, DRA_E_INVAL, "dra_preempt_batch: running pods: pod_off not monotone or not spanning the claims, a slot range outside "
                                       "n_out, or OK slots naming a GPU index >= n_gpu or GPUs of two nodes; nothing was written");
@@ -902,7 +911,8 @@ void dra_ctx_destroy(dra_ctx* c) {
                    c->d_place_state, c->d_place_node, c->d_place_cursor, c->d_splace_local, c->d_splace_rec,
                    c->d_pre_prio, c->d_pre_node, c->d_pre_nvic, c->d_pre_choice, c->d_pre_pst, c->d_pre_psum, c->d_pre_psum64,
                    c->d_pre_pairst, c->d_pre_pairvic, c->d_pre_rclaims, c->d_pre_routoff, c->d_pre_rpodoff, c->d_pre_rprio,
-                   c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic, c->d_spre_part};
+                   c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic, c->d_spre_part,
+                   c->d_pp_pending, c->d_pp_evicted, c->d_pp_runoff, c->d_pp_judged};
     for (void* p : dev) if (p) cudaFree(p);
     for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
@@ -1662,6 +1672,246 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
     memcpy(pod_status, o2 + onb, n_pod);
     memcpy(n_victims, o2 + onb + opb, (size_t)n_pod * 4);
     if (vb) memcpy(victims, o2 + onb + opb + ocb, vb);
+    return DRA_OK;
+}
+
+// Preempt and place (spec §15): the pending-pod arrays are checked here, the running pods on the device (k_pre_running),
+// whose fault gates the walk, so a rejected call writes no inventory word.  Running lists as in dra_preempt_batch (their
+// offsets kept aside, since the visit lists reuse the sort's buffers), visit lists as in dra_place_pods_batch, then one
+// persistent cooperative launch; the outputs are copied back after ONE synchronise and reach the caller only without a
+// fault.
+int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off,
+                            const int32_t* prio, uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off,
+                            const dra_running_pods* running, const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
+                            uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, uint32_t flags) {
+    if (!ctx || !pod_off || !running || !running->pod_off || (n_claim && (!claims || !out)) ||
+        (n_pod && (!prio || !pod_node || !pod_status)))
+        return DRA_E_INVAL;
+    const dra_running_pods& R = *running;
+    if ((R.n_claim && !R.claims) || (R.n_pod && (!R.prio || !evicted_by)) || (R.n_out && !R.out)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_preempt_place_batch: unknown flags 0x%x", flags);
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (pod_off[0] != 0 || pod_off[n_pod] != n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]");
+    for (uint32_t q = 0; q < n_pod; ++q)
+        if (pod_off[q + 1] < pod_off[q]) return fail(ctx, DRA_E_INVAL, "pod_off not monotone at pod %u", q);
+    const bool dense = cand_nodes == nullptr && cand_off == nullptr;
+    if (!dense && !cand_off) return fail(ctx, DRA_E_INVAL, "cand_nodes without cand_off");
+    if (!dense && cand_off[0] != 0) return fail(ctx, DRA_E_INVAL, "cand_off[0] must be 0");
+    for (uint32_t q = 0; !dense && q < n_pod; ++q) {
+        if (cand_off[q + 1] < cand_off[q]) return fail(ctx, DRA_E_INVAL, "cand_off not monotone at pod %u", q);
+        if (cand_off[q + 1] - cand_off[q] > PL_POS) return fail(ctx, DRA_E_INVAL, "pod %u has more than %u candidates", q, PL_POS);
+    }
+    const uint64_t n_pair64 = dense ? (uint64_t)n_pod * ctx->n_node : cand_off[n_pod];
+    if (dense && n_pair64 >= (1ull << 32)) return fail(ctx, DRA_E_INVAL, "dense form: n_pod * n_node must stay below 2^32");
+    const uint32_t n_pair = (uint32_t)n_pair64;
+    if (!dense && n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    if (n_pair && !dense && !cand_nodes) return fail(ctx, DRA_E_INVAL, "cand_off lists candidates but cand_nodes is NULL");
+    if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
+    if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    for (uint32_t i = 0; i < n_claim; ++i) {                              // slots as if the claim named a node of the inventory
+        const dra_claim_rec& c = claims[i];
+        const bool gpu = c.kind == DRA_KIND_GPU && c.count >= 1 && c.count <= DRA_MAX_COUNT && (out_off || c.count == 1);
+        const uint32_t slots = gpu ? c.count : 1u, dst = out_off ? out_off[i] : i;
+        if (dst > n_out || slots > n_out - dst) return fail(ctx, DRA_E_INVAL, "claim %u: slots [%u, %u) outside n_out %u", i, dst, dst + slots, n_out);
+    }
+    ctx->chain = DRA_K_PREEMPT_PLACE; ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;
+    if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "dra_preempt_place_batch needs cooperative launches, which this device does not offer");
+    CU(cudaSetDevice(ctx->device));
+    int rc = ensure_batch(ctx, std::max(std::max(n_claim, R.n_pod), n_pair), n_out, true);
+    if (rc) return rc;
+    if ((rc = upload_table(ctx))) return rc;
+    if (n_pod + 8 > ctx->cap_pods) {
+        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_pod_off, 0, cap))) return rc;
+        if ((rc = grow_nc(ctx, ctx->d_cand_off, 0, cap))) return rc;
+        ctx->cap_pods = cap;
+    }
+    if (!dense && (size_t)n_pair + 64 > ctx->cap_pairs) {
+        size_t cap = (size_t)n_pair + n_pair / 2 + 128;
+        if ((rc = grow_nc(ctx, ctx->d_cand_nodes, 0, cap))) return rc;
+        if ((rc = grow_nc(ctx, ctx->d_pair_pod, 0, cap))) return rc;
+        ctx->cap_pairs = cap;
+    }
+    if ((size_t)n_pair + 8 > ctx->cap_podrec) {
+        size_t cap = (size_t)n_pair + n_pair / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_podrec, 0, cap))) return rc;
+        ctx->cap_podrec = cap;
+    }
+    if ((size_t)n_pod + 8 > ctx->cap_place_pods) {
+        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_place_state, 0, cap))) return rc;
+        if ((rc = grow_nc(ctx, ctx->d_place_node, 0, cap))) return rc;
+        ctx->cap_place_pods = cap;
+    }
+    if ((size_t)ctx->n_node + 8 > ctx->cap_place_cursor) {
+        size_t cap = (size_t)ctx->n_node + ctx->n_node / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_place_cursor, 0, cap))) return rc;
+        ctx->cap_place_cursor = cap;
+    }
+    if ((size_t)n_pod + 8 > ctx->cap_pre_pods) {
+        const size_t need = (size_t)n_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_prio, need)) || (rc = grow_pre(ctx, ctx->d_pre_node, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_nvic, need)) || (rc = grow_pre(ctx, ctx->d_pre_choice, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_pst, need))) return rc;
+        ctx->cap_pre_pods = need + need / 2 + 64;
+    }
+    if ((size_t)n_pair + 8 > ctx->cap_pre_pairs) {
+        const size_t need = (size_t)n_pair + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_psum, need)) || (rc = grow_pre(ctx, ctx->d_pre_psum64, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_pairst, need)) || (rc = grow_pre(ctx, ctx->d_pre_pairvic, need))) return rc;
+        ctx->cap_pre_pairs = need + need / 2 + 64;
+    }
+    if ((size_t)R.n_claim + 8 > ctx->cap_pre_rclaims) {
+        const size_t need = (size_t)R.n_claim + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rclaims, need)) || (rc = grow_pre(ctx, ctx->d_pre_routoff, need))) return rc;
+        ctx->cap_pre_rclaims = need + need / 2 + 64;
+    }
+    if ((size_t)R.n_pod + 8 > ctx->cap_pre_rpods) {
+        const size_t need = (size_t)R.n_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rpodoff, need)) || (rc = grow_pre(ctx, ctx->d_pre_rprio, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_rrec, need)) || (rc = grow_pre(ctx, ctx->d_pre_vlist, need))) return rc;
+        ctx->cap_pre_rpods = need + need / 2 + 64;
+    }
+    if ((size_t)R.n_out + 8 > ctx->cap_pre_rout) {
+        const size_t need = (size_t)R.n_out + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rout, need))) return rc;
+        ctx->cap_pre_rout = need + need / 2 + 64;
+    }
+    if ((size_t)n_pod + 8 > ctx->cap_pp_pods) {
+        const size_t need = (size_t)n_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pp_pending, need))) return rc;
+        ctx->cap_pp_pods = need + need / 2 + 64;
+    }
+    if ((size_t)R.n_pod + 8 > ctx->cap_pp_rpods) {
+        const size_t need = (size_t)R.n_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pp_evicted, need))) return rc;
+        ctx->cap_pp_rpods = need + need / 2 + 64;
+    }
+    if ((size_t)ctx->n_node + 8 > ctx->cap_pp_nodes) {
+        const size_t need = (size_t)ctx->n_node + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pp_runoff, need)) || (rc = grow_pre(ctx, ctx->d_pp_judged, need))) return rc;
+        ctx->cap_pp_nodes = need + need / 2 + 64;
+    }
+    // staging: claims | pod_off | out_off | prio | cand_off | cand_nodes | running claims | pod_off | prio | out_off | out
+    auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    const size_t cb = al((size_t)n_claim * 16), pb = al(((size_t)n_pod + 1) * 4), ob = out_off ? al((size_t)n_claim * 4) : 0;
+    const size_t prb = al((size_t)n_pod * 4), kb = dense ? 0 : al(((size_t)n_pod + 1) * 4), nb = dense ? 0 : al((size_t)n_pair * 4);
+    const size_t rcb = al((size_t)R.n_claim * 16), rpb = al(((size_t)R.n_pod + 1) * 4), rprb = al((size_t)R.n_pod * 4);
+    const size_t rob = R.out_off ? al((size_t)R.n_claim * 4) : 0, routb = al((size_t)R.n_out * 8);
+    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + ob + prb + kb + nb + rcb + rpb + rprb + rob + routb + 16))) return rc;
+    uint8_t* h = ctx->h_in;
+    auto put = [&](const void* src, size_t bytes, size_t room) { uint8_t* d = h; if (bytes) memcpy(d, src, bytes); h += room; return d; };
+    uint8_t* h_c = put(claims, (size_t)n_claim * 16, cb);
+    uint8_t* h_po = put(pod_off, ((size_t)n_pod + 1) * 4, pb);
+    uint8_t* h_oo = out_off ? put(out_off, (size_t)n_claim * 4, ob) : nullptr;
+    uint8_t* h_pr = put(prio, (size_t)n_pod * 4, prb);
+    uint8_t* h_co = dense ? nullptr : put(cand_off, ((size_t)n_pod + 1) * 4, kb);
+    uint8_t* h_cn = dense ? nullptr : put(cand_nodes, (size_t)n_pair * 4, nb);
+    uint8_t* h_rc = put(R.claims, (size_t)R.n_claim * 16, rcb);
+    uint8_t* h_rpo = put(R.pod_off, ((size_t)R.n_pod + 1) * 4, rpb);
+    uint8_t* h_rpr = put(R.prio, (size_t)R.n_pod * 4, rprb);
+    uint8_t* h_roo = R.out_off ? put(R.out_off, (size_t)R.n_claim * 4, rob) : nullptr;
+    uint8_t* h_ro = put(R.out, (size_t)R.n_out * 8, routb);
+    cudaStream_t st = ctx->stream;
+    if (n_claim) CU(cudaMemcpyAsync(ctx->d_claims, h_c, (size_t)n_claim * 16, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pod_off, h_po, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (h_oo && n_claim) CU(cudaMemcpyAsync(ctx->d_out_off, h_oo, (size_t)n_claim * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pre_prio, h_pr, (size_t)n_pod * 4, cudaMemcpyHostToDevice, st));
+    if (!dense) {
+        CU(cudaMemcpyAsync(ctx->d_cand_off, h_co, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
+        if (n_pair) CU(cudaMemcpyAsync(ctx->d_cand_nodes, h_cn, (size_t)n_pair * 4, cudaMemcpyHostToDevice, st));
+    }
+    if (R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_rclaims, h_rc, (size_t)R.n_claim * 16, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pre_rpodoff, h_rpo, ((size_t)R.n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (R.n_pod) CU(cudaMemcpyAsync(ctx->d_pre_rprio, h_rpr, (size_t)R.n_pod * 4, cudaMemcpyHostToDevice, st));
+    if (h_roo && R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_routoff, h_roo, (size_t)R.n_claim * 4, cudaMemcpyHostToDevice, st));
+    if (R.n_out) CU(cudaMemcpyAsync(ctx->d_pre_rout, h_ro, (size_t)R.n_out * 8, cudaMemcpyHostToDevice, st));
+    const size_t rb = (size_t)n_out * 8;
+    if (rb) CU(cudaMemsetAsync(ctx->d_out, 0, rb, st));
+    CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)ctx->n_node + 1) * 4, st));
+    CU(cudaMemsetAsync(ctx->d_pp_judged, 0, ((size_t)ctx->n_node + 1) * 4, st));
+    if (R.n_pod) CU(cudaMemsetAsync(ctx->d_pp_evicted, 0xFF, (size_t)R.n_pod * 4, st));
+
+    PreArgs a; memset(&a, 0, sizeof a);
+    a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.prio = (const int32_t*)ctx->d_pre_prio; a.n_pod = n_pod;
+    a.cand_nodes = dense ? nullptr : ctx->d_cand_nodes; a.cand_off = dense ? nullptr : ctx->d_cand_off; a.n_pair = n_pair;
+    a.rclaims = ctx->d_pre_rclaims; a.rn_claim = R.n_claim; a.rpod_off = ctx->d_pre_rpodoff; a.rprio = (const int32_t*)ctx->d_pre_rprio;
+    a.rn_pod = R.n_pod; a.rout_off = R.out_off ? ctx->d_pre_routoff : nullptr; a.rout = ctx->d_pre_rout; a.rn_out = R.n_out;
+    a.rrec = ctx->d_pre_rrec; a.rsorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.vlist = ctx->d_pre_vlist;
+    a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.n_gpu = ctx->n_gpu; a.tbl = ctx->d_tbl;
+    a.sel = sel_of(ctx); a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
+    a.psum = ctx->d_pre_psum; a.psum64 = ctx->d_pre_psum64;
+    a.pod_node = ctx->d_pre_node; a.pod_status = ctx->d_pre_pst;
+    a.gate = ctx->d_err + ERR_BAD_OFFSETS; a.err = err_of(ctx);
+    Prof prof(ctx);
+    // the running lists (§14)
+    k_pre_running<<<std::max(1u, (R.n_pod + 255) / 256), 256, 0, st>>>(a);
+    ctx->launches += 1;
+    if (R.n_pod) {
+        if ((rc = launch_sort(ctx, ctx->d_pre_rrec, R.n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, ctx->n_node, ctx->d_node_off)))
+            return rc;
+        if (ctx->n_node) {
+            k_pre_vsort<<<std::min(ctx->n_node, (uint32_t)ctx->n_sm * 8u), 256, 0, st>>>(a);
+            ctx->launches += 1;
+        }
+        CU(cudaMemcpyAsync(ctx->d_pp_runoff, ctx->d_claim_off, ((size_t)ctx->n_node + 1) * 4, cudaMemcpyDeviceToDevice, st));
+    } else {
+        CU(cudaMemsetAsync(ctx->d_pp_runoff, 0, ((size_t)ctx->n_node + 1) * 4, st));
+    }
+    a.list_off = ctx->d_pp_runoff;
+    // the visit lists (§13)
+    PlaceArgs pl; memset(&pl, 0, sizeof pl);
+    pl.claims = ctx->d_claims; pl.pod_off = ctx->d_pod_off; pl.n_pod = n_pod;
+    pl.cand_nodes = a.cand_nodes; pl.cand_off = a.cand_off;
+    pl.out_off = out_off ? ctx->d_out_off : nullptr; pl.out = ctx->d_out;
+    pl.state = ctx->d_place_state; pl.pairs = ctx->d_podrec;
+    pl.sorted = ctx->d_sorted; pl.list_off = ctx->d_claim_off; pl.cursor = ctx->d_place_cursor;
+    pl.inv_src = ctx->d_inv_live; pl.inv_dst = ctx->d_inv_live; pl.node_off = ctx->d_node_off; pl.tbl = ctx->d_tbl;
+    pl.n_node = ctx->n_node; pl.exhaustive = a.exhaustive; pl.sel = a.sel; pl.err = a.err;
+    PpArgs pp{ctx->d_pp_pending, ctx->d_pp_evicted, ctx->d_pp_judged};
+    k_pp_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, pl, pp);
+    ctx->launches += 1;
+    if (!dense && n_pair &&
+        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, ctx->n_node, ctx->d_node_off)))
+        return rc;
+    if (ctx->n_node) {
+        if (ctx->pp_occ < 0) {
+            int occ = 0;
+            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_preempt_place<4>, 128, 0));
+            ctx->pp_occ = occ;
+        }
+        if (ctx->pp_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_preempt_place: no CTA can be resident");
+        const uint32_t grid = std::max(1u, std::min((ctx->n_node + 3) / 4, (uint32_t)(ctx->pp_occ * ctx->n_sm)));
+        cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
+        lc.gridDim = dim3(grid); lc.blockDim = dim3(128); lc.dynamicSmemBytes = 0; lc.stream = st;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
+        lc.attrs = at; lc.numAttrs = 1;
+        CU(cudaLaunchKernelEx(&lc, k_pods_preempt_place<4>, a, pl, pp));
+        ctx->launches += 1;
+    }
+    ctx->chain |= DRA_K_PREEMPT_PLACE;
+    prof.mark();
+    // outputs: out | pod_node | pod_status | evicted_by
+    const size_t onb = al((size_t)n_pod * 4), opb = al(n_pod), oeb = (size_t)R.n_pod * 4;
+    if ((rc = grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, al(rb) + onb + opb + oeb + 16))) return rc;
+    uint8_t* o = ctx->h_out;
+    uint8_t* o2 = o + al(rb);
+    if (rb) CU(cudaMemcpyAsync(o, ctx->d_out, rb, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(o2, ctx->d_pre_node, (size_t)n_pod * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(o2 + onb, ctx->d_pre_pst, n_pod, cudaMemcpyDeviceToHost, st));
+    if (oeb) CU(cudaMemcpyAsync(o2 + onb + opb, ctx->d_pp_evicted, oeb, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "preempt-and-place kernels: %s", cudaGetErrorString(e));
+    collect_timings(ctx, 1);
+    if ((rc = check_err(ctx))) return rc;
+    if (rb) memcpy(out, o, rb);
+    memcpy(pod_node, o2, (size_t)n_pod * 4);
+    memcpy(pod_status, o2 + onb, n_pod);
+    if (oeb) memcpy(evicted_by, o2 + onb + opb, oeb);
     return DRA_OK;
 }
 

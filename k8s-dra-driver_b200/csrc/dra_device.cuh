@@ -3619,10 +3619,13 @@ struct PreSum { uint32_t st, count, hi, hi_idx; unsigned long long sum; };
 
 // Pair (pod, node) on the W lanes gbase.. of the warp.  skip_first: the pair is known to be EVICT (k_pods_preempt_victims), so the
 // evaluation on the node as it is and the validity check are left out.  row: where the victims go (lane gbase writes).
-template <int W>
+// LIVE (spec §15, k_pods_preempt_place): the node as it stands is *live, the walk's working state, instead of a.inv; `row` is
+// then the call's evicted-by word per running pod: running pods whose word is set are gone and left out of V, and with
+// skip_first each victim's word is set to `pod`.  Lane gbase writes the words and its reading decides for the group.
+template <int W, bool LIVE = false>
 __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __restrict__ tbl_s, const uint32_t pod,
                                            const uint32_t node, const uint32_t lane, const uint32_t gmask, const uint32_t gbase,
-                                           const bool skip_first, uint32_t* row) {
+                                           const bool skip_first, uint32_t* row, const Lane* live = nullptr) {
     PreSum s{DRA_PRE_NO, 0u, 0x80000000u, 0xFFFFFFFFu, 0ull};
     if (node >= a.n_node) return s;
     const uint32_t c0 = __ldg(&a.pod_off[pod]), cnt = __ldg(&a.pod_off[pod + 1]) - c0;
@@ -3631,7 +3634,9 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
     const uint32_t g0 = __ldg(&a.node_off[node]), ng = __ldg(&a.node_off[node + 1]) - g0;
     if (ng > W) return s;                                             // cannot happen: W is chosen from the inventory
     const uint32_t gidx = gl < ng ? g0 + gl : DRA_GPU_NONE;
-    Lane L; L.load(gl < ng ? __ldg(&a.inv[g0 + gl]) : make_uint4(0, 0, 0, 0), gl < ng);
+    Lane L;
+    if constexpr (LIVE) L = *live;
+    else L.load(gl < ng ? __ldg(&a.inv[g0 + gl]) : make_uint4(0, 0, 0, 0), gl < ng);
     const PodGet get{a.claims + c0, nullptr, 0};
     const bool exh = a.exhaustive != 0;
     uint32_t st1 = DRA_ST_POD;
@@ -3657,7 +3662,13 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
         if ((int32_t)__ldcg(&a.vlist[mid]).w >= P) v0 = mid + 1; else hi = mid;
     }
     if (v0 == v1) { s.st = st1 == DRA_ST_SEARCH_LIMIT ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO; return s; }   // S' = S
-    for (uint32_t v = v0; v < v1; ++v) pre_apply(L, a, __ldcg(&a.vlist[v]), gidx, false);
+    bool any = !LIVE;
+    for (uint32_t v = v0; v < v1; ++v) {
+        const uint4 r = __ldcg(&a.vlist[v]);
+        if constexpr (LIVE) { if (__shfl_sync(gmask, __ldcg(&row[r.y]), gbase) != DRA_GPU_NONE) continue; any = true; }
+        pre_apply(L, a, r, gidx, false);
+    }
+    if (!any) { s.st = st1 == DRA_ST_SEARCH_LIMIT ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO; return s; }   // every member gone: S' = S
     {
         Lt = L;
         const uint32_t st = pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr);
@@ -3666,13 +3677,15 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
     s.st = DRA_PRE_EVICT;
     for (uint32_t v = v0; v < v1; ++v) {                            // the reprieve, most important first
         const uint4 r = __ldcg(&a.vlist[v]);
+        if constexpr (LIVE) { if (__shfl_sync(gmask, __ldcg(&row[r.y]), gbase) != DRA_GPU_NONE) continue; }
         Lane Lk = L;
         pre_apply(Lk, a, r, gidx, true);
         Lt = Lk;
         if (pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr) == 0) { L = Lk; continue; }
         if (s.count == 0) { s.hi = r.w; s.hi_idx = r.y; }            // V order: the first victim has the highest priority
         s.sum += (unsigned long long)((long long)(int32_t)r.w + 2147483648ll);
-        if (row && s.count < a.max_victims && lane == gbase) row[s.count] = r.y;
+        if constexpr (LIVE) { if (skip_first && lane == gbase) row[r.y] = pod; }
+        else { if (row && s.count < a.max_victims && lane == gbase) row[s.count] = r.y; }
         ++s.count;
     }
     return s;
@@ -3719,24 +3732,20 @@ __device__ __forceinline__ bool pre_better(const uint4 xs, const unsigned long l
     return xs.w > ys.w;                                                  // latest "start" among the highest-priority victims
 }
 
-// Warp per pod: FITS at the first such candidate, else the preferred EVICT pair, else INVALID / SEARCH_LIMIT / NO.
-__global__ void __launch_bounds__(256)
-k_pre_choose(const PreArgs a) {
-    if (__ldcg(a.gate)) return;
-    const uint32_t lane = threadIdx.x & 31, p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (p >= a.n_pod) return;
-    const bool dense = a.cand_off == nullptr;
-    const uint32_t k0 = dense ? p * a.n_node : __ldg(&a.cand_off[p]), k1 = dense ? k0 + a.n_node : __ldg(&a.cand_off[p + 1]);
+// Warp-wide, pod p's pair summaries psum[k0 .. k1) in list order: FITS at the first such pair, else the preferred EVICT
+// pair, else INVALID / SEARCH_LIMIT / NO.  Returns the status; k = the chosen pair (NONE without one), bs = its summary.
+__device__ __forceinline__ uint32_t pre_reduce(const PreArgs& a, const uint32_t p, const uint32_t k0, const uint32_t k1,
+                                               const uint32_t lane, uint32_t& k, uint4& bs) {
     uint32_t fit = DRA_GPU_NONE, best = DRA_GPU_NONE;
-    uint4 bs = make_uint4(0, 0, 0, 0); unsigned long long b64 = 0;
+    bs = make_uint4(0, 0, 0, 0); unsigned long long b64 = 0;
     bool lim = false;
-    for (uint32_t k = k0 + lane; k < k1; k += 32) {                      // each lane in list order: ties keep the earlier
-        const uint4 s = __ldcg(&a.psum[k]);
-        if (s.x == DRA_PRE_FITS) fit = min(fit, k);
+    for (uint32_t j = k0 + lane; j < k1; j += 32) {                      // each lane in list order: ties keep the earlier
+        const uint4 s = __ldcg(&a.psum[j]);
+        if (s.x == DRA_PRE_FITS) fit = min(fit, j);
         else if (s.x == DRA_PRE_SEARCH_LIMIT) lim = true;
         else if (s.x == DRA_PRE_EVICT) {
-            const unsigned long long v = __ldcg(&a.psum64[k]);
-            if (best == DRA_GPU_NONE || pre_better(s, v, bs, b64)) { best = k; bs = s; b64 = v; }
+            const unsigned long long v = __ldcg(&a.psum64[j]);
+            if (best == DRA_GPU_NONE || pre_better(s, v, bs, b64)) { best = j; bs = s; b64 = v; }
         }
     }
     fit = __reduce_min_sync(FULLMASK, fit);
@@ -3759,11 +3768,23 @@ k_pre_choose(const PreArgs a) {
         inv = claim_invalid(kind, prof, count, true) || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
     }
     inv = __any_sync(FULLMASK, inv);
+    k = DRA_GPU_NONE;
+    if (fit != DRA_GPU_NONE) { k = fit; return DRA_PRE_FITS; }
+    if (best != DRA_GPU_NONE) { k = best; return DRA_PRE_EVICT; }
+    return inv ? DRA_PRE_INVALID : lim ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO;
+}
+
+// Warp per pod: its pairs reduced by pre_reduce.
+__global__ void __launch_bounds__(256)
+k_pre_choose(const PreArgs a) {
+    if (__ldcg(a.gate)) return;
+    const uint32_t lane = threadIdx.x & 31, p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (p >= a.n_pod) return;
+    const bool dense = a.cand_off == nullptr;
+    const uint32_t k0 = dense ? p * a.n_node : __ldg(&a.cand_off[p]), k1 = dense ? k0 + a.n_node : __ldg(&a.cand_off[p + 1]);
+    uint32_t k; uint4 bs;
+    const uint32_t st = pre_reduce(a, p, k0, k1, lane, k, bs);
     if (lane != 0) return;
-    uint32_t st, k = DRA_GPU_NONE;
-    if (fit != DRA_GPU_NONE) { st = DRA_PRE_FITS; k = fit; }
-    else if (best != DRA_GPU_NONE) { st = DRA_PRE_EVICT; k = best; }
-    else st = inv ? DRA_PRE_INVALID : lim ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO;
     a.pod_status[p] = (uint8_t)st;
     a.pod_node[p] = k == DRA_GPU_NONE ? DRA_GPU_NONE : dense ? k - k0 : __ldg(&a.cand_nodes[k]);
     a.n_victims[p] = st == DRA_PRE_EVICT ? bs.y : 0u;
@@ -3790,6 +3811,213 @@ k_pods_preempt_victims(const PreArgs a) {
         if (k == DRA_GPU_NONE) continue;
         const uint32_t node = a.cand_off ? __ldg(&a.cand_nodes[k]) : k - p * a.n_node;
         (void)pre_pair<W>(a, tbl_s, p, node, lane, gmask, gbase, true, a.victims + (size_t)p * a.max_victims);
+    }
+}
+
+// ---- preempt and place (spec §15, dra_preempt_place_batch) ---------------------------------------------------------
+// §14's pair judgement and choice inside §13's walk: pods in input order, each judged on the nodes as the pods before it
+// left them.  k_pre_running, the counting sort and k_pre_vsort build each node's running list as for §14; k_pp_prep and
+// the counting sort build each node's visit list as for §13.  Then k_pods_preempt_place: a warp owns whole nodes, one lane
+// per GPU, with a cursor into each node's visit list.  At pod q's entry the owner judges the pair on the node as it
+// stands (pre_pair<32, true>: V without the running pods that earlier pods evicted), publishes the summary into q's psum
+// slots and counts q's open pairs down; the warp that publishes the last one reduces them (pre_reduce, list order) and
+// releases the decision into q's state word.  A node passes q only once q is decided.  The chosen node first applies q:
+// the chosen pair's reprieve once more (deterministic: nothing changed the node since), which marks the victims, §9 for
+// each of them, then the §12 evaluation with OutRecs.  q's entries on a node are consecutive after the stable sort and are
+// judged once: nothing changes the node between them.
+//   Exact: a node judges or applies q only after every earlier pod that lists the node is decided and, if it chose the
+//   node, applied there; a pod changes no node but the one it chose.
+//   Progress: every node that lists the lowest undecided pod can reach it (every entry before it belongs to a decided pod),
+//   so with every CTA resident its last pair is always judged.
+// State word: PP_OPEN undecided; PP_NOWHERE decided, applied nowhere; else the chosen position (the node in the dense form)
+// | PP_EVICT for an EVICT choice.
+constexpr uint32_t PP_OPEN = 0xFFFFFFFFu, PP_NOWHERE = 0x80000000u, PP_EVICT = 0x40000000u;
+
+struct PpArgs {
+    uint32_t* pending;            // [n_pod] the pod's pairs not judged yet
+    uint32_t* evicted_by;         // [rn_pod] the pod that evicted the running pod, or NONE (the caller's output)
+    uint32_t* judged;             // [n_node] 1 + the last pod judged at the node
+};
+
+// Warp per pod: state word, open-pair count, pair records (candidate form; pairs naming no node are NO and carry node
+// NONE, so the sort drops them, as do every pair of a pod that is never judged).  A pod that is never judged is decided
+// here: an empty pod is FITS on its first candidate naming a node, with nothing written; a pod of more than 32 claims is
+// INVALID; a pod with no candidate naming a node is INVALID or NO.
+__global__ void __launch_bounds__(256)
+k_pp_prep(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (p >= pl.n_pod) return;
+    const uint32_t c0 = __ldg(&pl.pod_off[p]), cnt = __ldg(&pl.pod_off[p + 1]) - c0;
+    const bool live = cnt != 0 && cnt <= DRA_MAX_POD;
+    uint32_t first = DRA_GPU_NONE, usable = 0;
+    if (!pl.cand_off) {
+        usable = pl.n_node;
+        if (pl.n_node) first = 0;
+    } else {
+        const uint32_t k0 = __ldg(&pl.cand_off[p]), nk = __ldg(&pl.cand_off[p + 1]) - k0;
+        for (uint32_t j0 = 0; j0 < nk; j0 += 32) {
+            const uint32_t j = j0 + lane;
+            const uint32_t n = j < nk ? __ldg(&pl.cand_nodes[k0 + j]) : DRA_GPU_NONE;
+            const bool ok = n < pl.n_node;
+            if (j < nk) {
+                pl.pairs[k0 + j] = make_uint4(p, live && ok ? n : DRA_GPU_NONE, j, 0);
+                if (!ok) { a.psum[k0 + j] = make_uint4(DRA_PRE_NO, 0, 0x80000000u, DRA_GPU_NONE); a.psum64[k0 + j] = 0; }
+            }
+            const uint32_t b = __ballot_sync(FULLMASK, ok);
+            usable += (uint32_t)__popc(b);
+            if (b && first == DRA_GPU_NONE) first = __shfl_sync(FULLMASK, n, __ffs(b) - 1);
+        }
+    }
+    const bool judged = live && usable != 0;
+    bool inv = cnt > DRA_MAX_POD;
+    if (live && !usable) {
+        for (uint32_t i = lane; i < cnt; i += 32) {
+            const uint4 c = __ldg(&pl.claims[c0 + i]);
+            const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
+            inv = inv || claim_invalid(kind, prof, count, true) || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
+        }
+        inv = __any_sync(FULLMASK, inv);
+    }
+    if (lane == 0) {
+        pp.pending[p] = usable;
+        pl.state[p] = judged ? PP_OPEN : PP_NOWHERE;
+        if (!judged) {
+            a.pod_node[p] = cnt == 0 ? first : DRA_GPU_NONE;
+            a.pod_status[p] = (uint8_t)(cnt == 0 ? (first != DRA_GPU_NONE ? DRA_PRE_FITS : DRA_PRE_NO)
+                                                 : inv ? DRA_PRE_INVALID : DRA_PRE_NO);
+        }
+    }
+    if (cnt != 0 && !judged) place_fail(pl, c0, cnt, DRA_ST_POD, lane);
+}
+
+// Persistent: every CTA resident (cooperative launch); warp w owns nodes w, w + warps, ... and cycles over them.  Minimum
+// one CTA per SM in the bounds: the walk's state beside pre_pair's then fits in registers without spilling (the stack
+// holds only the two Lane copies handed to pod_eval).
+template <int WPC>
+__global__ void __launch_bounds__(WPC * 32, 1)
+k_pods_preempt_place(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
+    __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
+    if (__ldcg(a.gate)) return;
+    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&pl.tbl[i]);
+    __syncthreads();
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t w0 = blockIdx.x * WPC + (threadIdx.x >> 5), n_warp = gridDim.x * WPC;
+    const bool dense = pl.cand_off == nullptr, have_off = pl.out_off != nullptr;
+    uint32_t seen = 0;
+    long long t0 = clock64();
+    while (true) {
+        bool left = false, moved = false;
+        for (uint32_t node = w0; node < pl.n_node; node += n_warp) {
+            const uint32_t l0 = dense ? 0u : __ldcg(&pl.list_off[node]), l1 = dense ? pl.n_pod : __ldcg(&pl.list_off[node + 1]);
+            const uint32_t cur0 = l0 + __ldcg(&pl.cursor[node]);
+            uint32_t cur = cur0;
+            if (cur >= l1) continue;
+            const uint32_t g0 = __ldg(&pl.node_off[node]), ng = __ldg(&pl.node_off[node + 1]) - g0;
+            Lane L;
+            bool loaded = false, dirty = false;
+            while (cur < l1) {
+                // 32 entries at once: the first one that is not to be skipped (decided, and not for this entry)
+                const uint32_t e = cur + lane;
+                uint32_t q = 0, k = 0, s = PP_NOWHERE;
+                if (e < l1) {
+                    if (dense) { q = e; k = node; }
+                    else { const uint4 r = __ldcg(&pl.sorted[e]); q = r.x; k = r.z; }
+                    s = ld_acquire_u32(&pl.state[q]);
+                }
+                const bool skip = s != PP_OPEN && ((s & PP_NOWHERE) || (s & PL_POS) != k);
+                const uint32_t act = __ballot_sync(FULLMASK, !skip);
+                if (!act) { cur = min(cur + 32u, l1); continue; }
+                const uint32_t f = (uint32_t)__ffs(act) - 1u;
+                cur += f;
+                const uint32_t qf = __shfl_sync(FULLMASK, q, f), sf = __shfl_sync(FULLMASK, s, f);
+                if (!loaded) {
+                    L.load(lane < ng ? pl.inv_dst[g0 + lane] : make_uint4(0, 0, 0, 0), lane < ng);
+                    loaded = true;
+                }
+                if (sf == PP_OPEN) {
+                    if (__shfl_sync(FULLMASK, __ldcg(&pp.judged[node]), 0) == qf + 1u) break;   // judged, undecided: wait
+                    // judge q here once, for each of its consecutive entries
+                    const PreSum r = pre_pair<32, true>(a, tbl_s, qf, node, lane, FULLMASK, 0u, false, pp.evicted_by, &L);
+                    const uint32_t kb = dense ? qf * pl.n_node : __ldg(&pl.cand_off[qf]);
+                    uint32_t n_here = 0;
+                    for (uint32_t e2 = cur; e2 < l1; ++e2) {
+                        uint32_t pos = node;
+                        if (!dense) { const uint4 r2 = __ldcg(&pl.sorted[e2]); if (r2.x != qf) break; pos = r2.z; }
+                        else if (e2 != cur) break;
+                        if (lane == 0) { a.psum[kb + pos] = make_uint4(r.st, r.count, r.hi, r.hi_idx); a.psum64[kb + pos] = r.sum; }
+                        ++n_here;
+                    }
+                    __threadfence();
+                    __syncwarp();
+                    uint32_t last = 0;
+                    if (lane == 0) {
+                        pp.judged[node] = qf + 1u;
+                        last = atomicSub(&pp.pending[qf], n_here) == n_here ? 1u : 0u;
+                        atomicAdd(&pl.cursor[pl.n_node], 1u);
+                    }
+                    if (__shfl_sync(FULLMASK, last, 0)) {
+                        // every pair of q is judged: the decision
+                        __threadfence();
+                        const uint32_t k0 = dense ? qf * pl.n_node : __ldg(&pl.cand_off[qf]);
+                        const uint32_t k1 = dense ? k0 + pl.n_node : __ldg(&pl.cand_off[qf + 1]);
+                        uint32_t kc; uint4 bs;
+                        const uint32_t st = pre_reduce(a, qf, k0, k1, lane, kc, bs);
+                        if (lane == 0) {
+                            a.pod_status[qf] = (uint8_t)st;
+                            a.pod_node[qf] = kc == DRA_GPU_NONE ? DRA_GPU_NONE : dense ? kc - k0 : __ldg(&pl.cand_nodes[kc]);
+                        }
+                        if (kc == DRA_GPU_NONE) {
+                            const uint32_t c0 = __ldg(&pl.pod_off[qf]), cnt = __ldg(&pl.pod_off[qf + 1]) - c0;
+                            place_fail(pl, c0, cnt, st == DRA_PRE_SEARCH_LIMIT ? (uint32_t)DRA_ST_SEARCH_LIMIT : (uint32_t)DRA_ST_POD, lane);
+                        }
+                        __threadfence();
+                        __syncwarp();
+                        if (lane == 0)
+                            st_release_u32(&pl.state[qf], kc == DRA_GPU_NONE ? PP_NOWHERE : (kc - k0) | (st == DRA_PRE_EVICT ? PP_EVICT : 0u));
+                    }
+                    moved = true;
+                    continue;                                        // q's state again: decided now, or this node waits
+                }
+                // q is decided, for this entry of this node: apply it
+                const uint32_t c0 = __ldg(&pl.pod_off[qf]), cnt = __ldg(&pl.pod_off[qf + 1]) - c0;
+                if (sf & PP_EVICT) {
+                    (void)pre_pair<32, true>(a, tbl_s, qf, node, lane, FULLMASK, 0u, true, pp.evicted_by, &L);   // marks the victims
+                    __syncwarp();
+                    const uint32_t gidx = lane < ng ? g0 + lane : DRA_GPU_NONE;
+                    const uint32_t v0 = __ldcg(&a.list_off[node]), v1 = __ldcg(&a.list_off[node + 1]);
+                    for (uint32_t v = v0; v < v1; ++v) {             // §9 for each victim
+                        const uint4 r = __ldcg(&a.vlist[v]);
+                        if (__shfl_sync(FULLMASK, __ldcg(&pp.evicted_by[r.y]), 0) == qf) pre_apply(L, a, r, gidx, false);
+                    }
+                }
+                {
+                    const PodGet get{pl.claims + c0, have_off ? pl.out_off + c0 : nullptr, c0};
+                    Lane Lt = L;
+                    if (pod_eval<32>(Lt, lane, FULLMASK, 0, g0, tbl_s, get, cnt, pl.sel, pl.exhaustive != 0, have_off, pl.out) == 0) L = Lt;
+                }
+                dirty = true;
+                __threadfence();
+                __syncwarp();
+                if (lane == 0) atomicAdd(&pl.cursor[pl.n_node], 1u);
+                moved = true;
+                ++cur;
+            }
+            if (dirty && lane < ng) pl.inv_dst[g0 + lane] = L.store(pl.inv_dst[g0 + lane]);    // (only this warp writes the node)
+            if (cur != cur0) { moved = true; pl.cursor[node] = cur - l0; }
+            if (cur < l1) left = true;
+        }
+        if (!left) break;
+        if (moved) { t0 = clock64(); continue; }
+        // nothing moved on this warp's nodes: back off, and give up when nothing moved anywhere for a long time (cannot
+        // happen with every CTA resident)
+        __nanosleep(256);
+        const uint32_t pr = __shfl_sync(FULLMASK, ld_acquire_u32(&pl.cursor[pl.n_node]), 0);
+        if (pr != seen) { seen = pr; t0 = clock64(); }
+        else if (clock64() - t0 > 4000000000ll) {
+            if (lane == 0) pl.err.set(ERR_DEVICE_WAIT);
+            break;
+        }
     }
 }
 
