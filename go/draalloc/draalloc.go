@@ -600,6 +600,44 @@ func (c *Context) PreemptBatchGlobalDevice(pinnedClaims unsafe.Pointer, nClaim i
 	return nil
 }
 
+// SetShardPreemptPlace reserves room for the sharded preempt-and-place call (pending pods, judged pairs, running pods):
+// after SetInventory, before ShardExport, the same on every context.  Unbuilt, like the rest of this file.
+func (c *Context) SetShardPreemptPlace(maxPods, maxPairs, maxRun uint32) error {
+	if rc := C.dra_set_shard_preempt_place(c.h, C.uint32_t(maxPods), C.uint32_t(maxPairs), C.uint32_t(maxRun)); rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
+// PreemptPlaceGlobal: preempt and place (spec §15) on a sharded world (dra_preempt_place_batch_global_device).  The same
+// pending pods, candidates (pinnedCandNodes == pinnedCandOff == nil and nPair == 0: dense form), running pods, out_off,
+// nOut and flags on every context, every array in dra_host_alloc'ed (pinned) memory.  Every context ends with the whole
+// table (GatherRead), pod_node, pod_status and evicted_by; the victims are released by the call on the contexts that own
+// them.  Returns at once; Sync reports completion and errors found on the device.  Unbuilt, like the rest of this file.
+func (c *Context) PreemptPlaceGlobal(pinnedClaims unsafe.Pointer, nClaim int, pinnedPodOff, pinnedPrio unsafe.Pointer,
+	nPod int, pinnedCandNodes, pinnedCandOff unsafe.Pointer, nPair int, run PinnedRunningPods, pinnedOutOff unsafe.Pointer,
+	nOut int, pinnedPodNode, pinnedPodStatus, pinnedEvictedBy unsafe.Pointer, flags uint32) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var r C.dra_running_pods
+	r.claims = (*C.dra_claim_rec)(run.Claims)
+	r.n_claim = C.uint32_t(run.NClaim)
+	r.pod_off = (*C.uint32_t)(run.PodOff)
+	r.n_pod = C.uint32_t(run.NPod)
+	r.prio = (*C.int32_t)(run.Prio)
+	r.out_off = (*C.uint32_t)(run.OutOff)
+	r.out = (*C.dra_out_rec)(run.Out)
+	r.n_out = C.uint32_t(run.NOut)
+	rc := C.dra_preempt_place_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
+		(*C.uint32_t)(pinnedPodOff), (*C.int32_t)(pinnedPrio), C.uint32_t(nPod), (*C.uint32_t)(pinnedCandNodes),
+		(*C.uint32_t)(pinnedCandOff), C.uint32_t(nPair), &r, (*C.uint32_t)(pinnedOutOff), C.uint32_t(nOut),
+		(*C.uint32_t)(pinnedPodNode), (*C.uint8_t)(pinnedPodStatus), (*C.uint32_t)(pinnedEvictedBy), C.uint32_t(flags))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
 // DeallocateGlobal: Deallocate on a sharded world (dra_deallocate_batch_global_device), the step after AllocatePodsGlobal.
 // The same claims, out_off and OutRecs on every context, in dra_host_alloc'ed (pinned) memory (pinnedOutOff may be nil);
 // each context applies the OK records whose GPU lies in its own range and writes no other GPU.  Needs SetShardMap (or

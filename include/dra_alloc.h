@@ -536,6 +536,39 @@ int  dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
  * blocked thread has not made yet, and the sync times out. */
 int dra_shard_sync_inventory_device(dra_ctx* ctx);
 
+/* Room for the sharded preempt-and-place call: at most max_pods pending pods, max_pairs judged pairs (n_pair in the
+ * candidate form, n_pod * n_node in the dense form) and max_run running pods per call.  World > 1: call before
+ * dra_shard_export (afterwards: DRA_E_STATE), every rank with the same sizes; the peer import refuses a peer set up
+ * differently.  Load the inventory first: the export then loads every kernel of the call and sizes its scratch (about
+ * 16 bytes per GPU, 40 bytes per pair, 40 per pod and running pod) and its sort, so that no call loads a module or frees a
+ * buffer while a peer waits for it.  World 1 needs no call. */
+int dra_set_shard_preempt_place(dra_ctx* ctx, uint32_t max_pods, uint32_t max_pairs, uint32_t max_run);
+/* Preempt and place over a sharded world (spec §15, "Sharded form"): dra_preempt_place_batch applied to the world's state,
+ * the inventory made of every rank's own node range as that rank holds it.  The SAME claims, pod_off, prio, candidates
+ * (cand_nodes == cand_off == NULL and n_pair == 0: the dense form), running pods, out_off, n_out and flags on every rank
+ * (device pointers, or dra_host_alloc'ed buffers; `running` itself is a host struct whose pointers are device-visible).
+ * Every rank ends with the WHOLE table (dra_gather_table / dra_gather_read: n_out records) and the whole d_pod_node[n_pod],
+ * d_pod_status[n_pod] and d_evicted_by[running->n_pod]: byte for byte what dra_preempt_place_batch answers on that one
+ * inventory.  Each rank's own GPU range ends as that call leaves it (the victims are released by the call); no rank writes
+ * a GPU record outside its range, and none touches the pristine copy.  The ranks exchange their own ranges once, through
+ * the inventory sync's staging, and then every rank runs the §15 walk on a private copy of the world's state.
+ * Prerequisites as for dra_place_pods_batch_global_device: dra_set_shard (world 1: every node is the rank's) or, world > 1,
+ * dra_set_shard_map; dra_set_shard_preempt_place and the inventory loaded before dra_shard_export; dra_peer_import or
+ * dra_peer_import_local (else DRA_E_STATE).  n_pod, pairs or running pods above the reserved sizes, n_out above the exported
+ * table: DRA_E_INVAL.  World 1 needs no export.  Host-side argument errors return before anything is enqueued.  Enqueues on
+ * ctx's stream and returns; n_pod == 0 enqueues nothing.  Completion and device-detected errors surface at dra_ctx_sync:
+ * pod_off / cand_off not monotone or not spanning their arrays, more than 2^30 - 1 candidates for a pod, a pending slot
+ * outside n_out, or the running pods' faults of dra_preempt_place_batch give DRA_E_INVAL on EVERY rank, with no output
+ * and no inventory word written; a peer that does not deliver its range within DRA_PEER_TIMEOUT_MS gives DRA_E_NCCL on
+ * EVERY rank, also with nothing written (after the exchange the ranks agree on one verdict: the call fails everywhere or
+ * nowhere).  The table is this context's own buffer, written by no peer; after a failed call its contents are undefined.
+ * flags: 0 or DRA_F_EXHAUSTIVE. */
+int dra_preempt_place_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                          const uint32_t* d_pod_off, const int32_t* d_prio, uint32_t n_pod,
+                                          const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                          const dra_running_pods* running, const uint32_t* d_out_off, uint32_t n_out,
+                                          uint32_t* d_pod_node, uint8_t* d_pod_status, uint32_t* d_evicted_by, uint32_t flags);
+
 /* Deallocate over a sharded world (spec §9, "Sharded form"): the classic flow's last step.  The SAME claims, out_off and
  * OutRecs on every rank (device pointers, or dra_host_alloc'ed buffers; d_out may be the table dra_gather_table returns).
  * slots(c) is counted as by dra_deallocate_batch, on the whole inventory's node indices.  A rank applies only the OK slots
@@ -622,6 +655,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_PREEMPT           0x800000u /* preemption: running-pod prep, victim lists, pairs, choice, victim rows */
 #define DRA_K_PREEMPT_SHARD    0x1000000u /* sharded preemption: prep, victim lists, the window's pairs, partials, merge */
 #define DRA_K_PREEMPT_PLACE    0x2000000u /* preempt and place: running-pod prep, victim lists, visit lists, persistent walk */
+#define DRA_K_PREEMPT_PLACE_SHARD 0x4000000u /* sharded preempt and place: state exchange, the §15 chain on it, own range back */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

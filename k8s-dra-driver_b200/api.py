@@ -25,7 +25,7 @@ KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x0
            "pack1": 0x02000, "pack4": 0x04000, "compact_flat1": 0x08000, "compact_flat8": 0x10000,
            "compact_lookback": 0x20000, "compact_in_kernel": 0x40000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000,
            "place_shard": 0x400000, "preempt": 0x800000, "preempt_shard": 0x1000000,
-           "preempt_place": 0x2000000}
+           "preempt_place": 0x2000000, "preempt_place_shard": 0x4000000}
 
 
 class DraError(RuntimeError):
@@ -89,6 +89,9 @@ SYMBOLS = {
     "dra_set_shard_preempt": (_i32, [_vp, _u32, _u32, _u32]),
     "dra_preempt_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp,
                                                _vp, _u32, _u32]),
+    "dra_set_shard_preempt_place": (_i32, [_vp, _u32, _u32, _u32]),
+    "dra_preempt_place_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp,
+                                                     _vp, _u32]),
     "dra_shard_sync_inventory_device": (_i32, [_vp]),
     "dra_deallocate_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_mps_limits_batch": (_i32, [_vp, _vp, _u32, _vp, _vp]),
@@ -542,6 +545,25 @@ class Context:
             self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), _ptr(d_prio), n_pod, _ptr(d_cand_nodes), _ptr(d_cand_off),
             n_pair, C.byref(running), _ptr(d_pair_status), _ptr(d_pair_victims), _ptr(d_pod_node), _ptr(d_pod_status),
             _ptr(d_n_victims), _ptr(d_victims), max_victims, flags))
+
+    def set_shard_preempt_place(self, max_pods: int, max_pairs: int, max_run: int) -> None:
+        """Room for the sharded preempt-and-place call (pending pods, judged pairs, running pods); world > 1: before
+        shard_export, with the inventory loaded, the same on every rank."""
+        self._check(self._lib.dra_set_shard_preempt_place(self._h, max_pods, max_pairs, max_run))
+
+    def preempt_place_global_device(self, d_claims: int, n_claim: int, d_pod_off: int, d_prio: int, n_pod: int,
+                                    d_cand_nodes: int | None, d_cand_off: int | None, n_pair: int, running: "RunningPods",
+                                    d_out_off: int | None, n_out: int, d_pod_node: int, d_pod_status: int,
+                                    d_evicted_by: int | None, flags: int = 0) -> None:
+        """Sharded preempt and place (spec §15): the SAME pending pods, candidates and running pods on every rank (device
+        pointers; `running` a RunningPods whose pointers are device-visible); d_cand_nodes / d_cand_off None and n_pair 0 =
+        dense form.  Every rank receives the whole table (gather_read()) and the whole pod_node (n_pod uint32), pod_status
+        (n_pod uint8) and evicted_by (one uint32 per running pod); each rank's own GPU range ends as preempt_place() leaves
+        it.  flags: F_EXHAUSTIVE.  Enqueues, no synchronisation; errors found on the device surface at sync()."""
+        self._check(self._lib.dra_preempt_place_batch_global_device(
+            self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), _ptr(d_prio), n_pod, _ptr(d_cand_nodes), _ptr(d_cand_off),
+            n_pair, C.byref(running), _ptr(d_out_off), n_out, _ptr(d_pod_node), _ptr(d_pod_status), _ptr(d_evicted_by),
+            flags))
 
     def shard_sync_inventory_device(self) -> None:
         """Every rank's live inventory becomes the world's state (each GPU as its owning rank holds it), so get_inventory()

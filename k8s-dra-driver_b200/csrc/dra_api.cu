@@ -212,6 +212,12 @@ struct dra_ctx {
     uint32_t peer_pre_pods = 0, peer_pre_pairs = 0, peer_pre_victims = 0;
     PeerRegion pre_x;
     uint4* d_spre_part = nullptr; size_t cap_spre_part = 0;           // this rank's partials and pair results (uint4 units)
+    // sharded preempt and place: the world's state assembled for the call (scratch inventory), and the call's gate word
+    uint32_t spp_max_pods = 0, spp_max_pairs = 0, spp_max_run = 0;     // dra_set_shard_preempt_place, reserved by the next peer_setup
+    uint32_t peer_spp_pods = 0, peer_spp_pairs = 0, peer_spp_run = 0;
+    uint4* d_spp_inv = nullptr; size_t cap_spp_inv = 0;
+    uint32_t* d_spp_gate = nullptr;
+    PeerRegion spp_x;                           // the verdict agreement's flags (k_spp_agree), after the exchange
     int splace_occ = -1;                        // resident CTAs of k_pods_place<4, true> per SM (occupancy query, once)
     int peers_on_device = 1;                    // ranks whose contexts share this device (dra_peer_import_local)
     // inventory sync: records in the peer buffer ([staging x2: peer_inv_gpus records][flags[PEER_MAX], elect[2]])
@@ -684,6 +690,9 @@ int check_err(dra_ctx* ctx) {
     cudaMemsetAsync(ctx->d_err, 0, ERR_WORDS * sizeof(uint32_t), ctx->stream);
     cudaStreamSynchronize(ctx->stream);
     if (sp) return fail(ctx, DRA_E_STATE, "sharded call: %u claims fell into this shard, more than the launch was laid out for; nothing was changed, call again", ctx->h_sc_counts ? ctx->h_sc_counts[0] : 0u);
+    if (dw && (ctx->chain & DRA_K_PREEMPT_PLACE_SHARD))
+        return fail(ctx, DRA_E_CUDA, "sharded preempt and place: the walk's wait timed out (its CTAs were not resident together); nothing was "
+                                     "written: no output, and every inventory is as it was");
     if (dw) return fail(ctx, DRA_E_CUDA, "a device-side wait inside one kernel (grid barrier / look-back over CTAs) timed out: CTAs were not scheduled together; state is undefined, reload the inventory");
     if (bo && (ctx->chain & DRA_K_PREEMPT_PLACE))
         return fail(ctx, DRA_E_INVAL, "dra_preempt_place_batch: running pods: pod_off not monotone or not spanning the claims, a slot range "
@@ -695,6 +704,11 @@ int check_err(dra_ctx* ctx) {
         return fail(ctx, DRA_E_INVAL, "sharded preemption: pod_off / cand_off not monotone or not spanning their arrays, or running pods: pod_off "
                                       "not monotone or not spanning the claims, a slot range outside n_out, or OK slots naming a GPU index "
                                       ">= n_gpu or GPUs of two nodes (on this rank or a peer); nothing was written");
+    if (bo && (ctx->chain & DRA_K_PREEMPT_PLACE_SHARD))
+        return fail(ctx, DRA_E_INVAL, "sharded preempt and place: pod_off / cand_off not monotone or not spanning their arrays, more than %u "
+                                      "candidates for a pod, a pending slot outside n_out, or running pods: pod_off not monotone or not "
+                                      "spanning the claims, a slot range outside n_out, or OK slots naming a GPU index >= n_gpu or GPUs of "
+                                      "two nodes; nothing was written", PL_POS);
     if (bo) return fail(ctx, DRA_E_INVAL, "sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays; nothing was evaluated");
     if (bp && (ctx->chain & DRA_K_PLACE_SHARD))
         return fail(ctx, DRA_E_INVAL, "sharded place pods: pod_off / cand_off not monotone or not spanning their arrays, more than %u candidates for a pod, "
@@ -706,6 +720,63 @@ int check_err(dra_ctx* ctx) {
     if (pt) return fail(ctx, DRA_E_NCCL, "all-gather: a rank did not deliver its records in time (or aborted its batch)");
     if (ns) return fail(ctx, DRA_E_INVAL, "DRA_F_NODE_SORTED given but claims are not sorted by node; inventory unchanged");
     return fail(ctx, DRA_E_INVAL, "out_off/n_out: a claim's slots fall outside out[]; inventory state is undefined, reset it");
+}
+
+// The device buffers of a §15 walk (dra_preempt_place_batch and its sharded form) for n_pod pending pods, n_pair judged
+// pairs (n_pod * n_node in the dense form) and rn_pod running pods
+int pp_buffers(dra_ctx* ctx, uint32_t n_pod, uint32_t n_pair, uint32_t rn_pod) {
+    int rc;
+    if ((size_t)n_pair + 8 > ctx->cap_podrec) {
+        size_t cap = (size_t)n_pair + n_pair / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_podrec, 0, cap))) return rc;
+        ctx->cap_podrec = cap;
+    }
+    if ((size_t)n_pod + 8 > ctx->cap_place_pods) {
+        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_place_state, 0, cap))) return rc;
+        if ((rc = grow_nc(ctx, ctx->d_place_node, 0, cap))) return rc;
+        ctx->cap_place_pods = cap;
+    }
+    if ((size_t)ctx->n_node + 8 > ctx->cap_place_cursor) {
+        size_t cap = (size_t)ctx->n_node + ctx->n_node / 2 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_place_cursor, 0, cap))) return rc;
+        ctx->cap_place_cursor = cap;
+    }
+    if ((size_t)n_pod + 8 > ctx->cap_pre_pods) {
+        const size_t need = (size_t)n_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_prio, need)) || (rc = grow_pre(ctx, ctx->d_pre_node, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_nvic, need)) || (rc = grow_pre(ctx, ctx->d_pre_choice, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_pst, need))) return rc;
+        ctx->cap_pre_pods = need + need / 2 + 64;
+    }
+    if ((size_t)n_pair + 8 > ctx->cap_pre_pairs) {
+        const size_t need = (size_t)n_pair + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_psum, need)) || (rc = grow_pre(ctx, ctx->d_pre_psum64, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_pairst, need)) || (rc = grow_pre(ctx, ctx->d_pre_pairvic, need))) return rc;
+        ctx->cap_pre_pairs = need + need / 2 + 64;
+    }
+    if ((size_t)rn_pod + 8 > ctx->cap_pre_rpods) {
+        const size_t need = (size_t)rn_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rpodoff, need)) || (rc = grow_pre(ctx, ctx->d_pre_rprio, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_rrec, need)) || (rc = grow_pre(ctx, ctx->d_pre_vlist, need))) return rc;
+        ctx->cap_pre_rpods = need + need / 2 + 64;
+    }
+    if ((size_t)n_pod + 8 > ctx->cap_pp_pods) {
+        const size_t need = (size_t)n_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pp_pending, need))) return rc;
+        ctx->cap_pp_pods = need + need / 2 + 64;
+    }
+    if ((size_t)rn_pod + 8 > ctx->cap_pp_rpods) {
+        const size_t need = (size_t)rn_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pp_evicted, need))) return rc;
+        ctx->cap_pp_rpods = need + need / 2 + 64;
+    }
+    if ((size_t)ctx->n_node + 8 > ctx->cap_pp_nodes) {
+        const size_t need = (size_t)ctx->n_node + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pp_runoff, need)) || (rc = grow_pre(ctx, ctx->d_pp_judged, need))) return rc;
+        ctx->cap_pp_nodes = need + need / 2 + 64;
+    }
+    return DRA_OK;
 }
 
 }  // namespace
@@ -912,7 +983,7 @@ void dra_ctx_destroy(dra_ctx* c) {
                    c->d_pre_prio, c->d_pre_node, c->d_pre_nvic, c->d_pre_choice, c->d_pre_pst, c->d_pre_psum, c->d_pre_psum64,
                    c->d_pre_pairst, c->d_pre_pairvic, c->d_pre_rclaims, c->d_pre_routoff, c->d_pre_rpodoff, c->d_pre_rprio,
                    c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic, c->d_spre_part,
-                   c->d_pp_pending, c->d_pp_evicted, c->d_pp_runoff, c->d_pp_judged};
+                   c->d_pp_pending, c->d_pp_evicted, c->d_pp_runoff, c->d_pp_judged, c->d_spp_inv, c->d_spp_gate};
     for (void* p : dev) if (p) cudaFree(p);
     for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
@@ -1734,65 +1805,16 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
         if ((rc = grow_nc(ctx, ctx->d_pair_pod, 0, cap))) return rc;
         ctx->cap_pairs = cap;
     }
-    if ((size_t)n_pair + 8 > ctx->cap_podrec) {
-        size_t cap = (size_t)n_pair + n_pair / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_podrec, 0, cap))) return rc;
-        ctx->cap_podrec = cap;
-    }
-    if ((size_t)n_pod + 8 > ctx->cap_place_pods) {
-        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_place_state, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_place_node, 0, cap))) return rc;
-        ctx->cap_place_pods = cap;
-    }
-    if ((size_t)ctx->n_node + 8 > ctx->cap_place_cursor) {
-        size_t cap = (size_t)ctx->n_node + ctx->n_node / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_place_cursor, 0, cap))) return rc;
-        ctx->cap_place_cursor = cap;
-    }
-    if ((size_t)n_pod + 8 > ctx->cap_pre_pods) {
-        const size_t need = (size_t)n_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_prio, need)) || (rc = grow_pre(ctx, ctx->d_pre_node, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_nvic, need)) || (rc = grow_pre(ctx, ctx->d_pre_choice, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_pst, need))) return rc;
-        ctx->cap_pre_pods = need + need / 2 + 64;
-    }
-    if ((size_t)n_pair + 8 > ctx->cap_pre_pairs) {
-        const size_t need = (size_t)n_pair + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_psum, need)) || (rc = grow_pre(ctx, ctx->d_pre_psum64, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_pairst, need)) || (rc = grow_pre(ctx, ctx->d_pre_pairvic, need))) return rc;
-        ctx->cap_pre_pairs = need + need / 2 + 64;
-    }
+    if ((rc = pp_buffers(ctx, n_pod, n_pair, R.n_pod))) return rc;
     if ((size_t)R.n_claim + 8 > ctx->cap_pre_rclaims) {
         const size_t need = (size_t)R.n_claim + 8;
         if ((rc = grow_pre(ctx, ctx->d_pre_rclaims, need)) || (rc = grow_pre(ctx, ctx->d_pre_routoff, need))) return rc;
         ctx->cap_pre_rclaims = need + need / 2 + 64;
     }
-    if ((size_t)R.n_pod + 8 > ctx->cap_pre_rpods) {
-        const size_t need = (size_t)R.n_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rpodoff, need)) || (rc = grow_pre(ctx, ctx->d_pre_rprio, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_rrec, need)) || (rc = grow_pre(ctx, ctx->d_pre_vlist, need))) return rc;
-        ctx->cap_pre_rpods = need + need / 2 + 64;
-    }
     if ((size_t)R.n_out + 8 > ctx->cap_pre_rout) {
         const size_t need = (size_t)R.n_out + 8;
         if ((rc = grow_pre(ctx, ctx->d_pre_rout, need))) return rc;
         ctx->cap_pre_rout = need + need / 2 + 64;
-    }
-    if ((size_t)n_pod + 8 > ctx->cap_pp_pods) {
-        const size_t need = (size_t)n_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pp_pending, need))) return rc;
-        ctx->cap_pp_pods = need + need / 2 + 64;
-    }
-    if ((size_t)R.n_pod + 8 > ctx->cap_pp_rpods) {
-        const size_t need = (size_t)R.n_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pp_evicted, need))) return rc;
-        ctx->cap_pp_rpods = need + need / 2 + 64;
-    }
-    if ((size_t)ctx->n_node + 8 > ctx->cap_pp_nodes) {
-        const size_t need = (size_t)ctx->n_node + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pp_runoff, need)) || (rc = grow_pre(ctx, ctx->d_pp_judged, need))) return rc;
-        ctx->cap_pp_nodes = need + need / 2 + 64;
     }
     // staging: claims | pod_off | out_off | prio | cand_off | cand_nodes | running claims | pod_off | prio | out_off | out
     auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
@@ -1979,6 +2001,7 @@ namespace {
 struct PeerLayout {
     uint32_t world, rank, form, cap, tab_len, uns_pairs, inv_gpus, rsvd;      // rsvd: dra_set_shard_place's max_pods
     uint32_t pre_pods, pre_pairs, pre_victims, pad;                           // dra_set_shard_preempt's sizes
+    uint32_t spp_pods, spp_pairs, spp_run, pad2;                              // dra_set_shard_preempt_place's sizes
     bool operator==(const PeerLayout& o) const { return memcmp(this, &o, sizeof o) == 0; }
 };
 PeerLayout layout_of(const dra_ctx* c, int rank) {
@@ -1986,6 +2009,7 @@ PeerLayout layout_of(const dra_ctx* c, int rank) {
     l.world = (uint32_t)c->world; l.rank = (uint32_t)rank; l.form = c->peer_form; l.cap = c->peer_cap; l.tab_len = c->peer_tab_len;
     l.uns_pairs = c->peer_uns_pairs; l.inv_gpus = c->peer_inv_gpus; l.rsvd = c->peer_place_pods;
     l.pre_pods = c->peer_pre_pods; l.pre_pairs = c->peer_pre_pairs; l.pre_victims = c->peer_pre_victims;
+    l.spp_pods = c->peer_spp_pods; l.spp_pairs = c->peer_spp_pairs; l.spp_run = c->peer_spp_run;
     return l;
 }
 
@@ -2019,6 +2043,33 @@ int preload_preempt_shard(dra_ctx* ctx) {
                         (const void*)k_bucket_scan, (const void*)k_bucket_scatter};
     for (const void* k : ks) { cudaFuncAttributes fa; CU(cudaFuncGetAttributes(&fa, k)); }
     CU(cudaFuncSetAttribute((const void*)k_spre_merge, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    return DRA_OK;
+}
+
+// The same for the sharded preempt-and-place chain, and the walk's occupancy query (which loads it too).  Its one wait is
+// the inventory exchange (k_isync_copy), before the walk.
+int preload_preempt_place_shard(dra_ctx* ctx) {
+    const void* ks[] = {(const void*)k_peer_push, (const void*)k_isync_copy, (const void*)k_spp_agree, (const void*)k_pre_running, (const void*)k_pre_vsort,
+                        (const void*)k_spp_prep, (const void*)k_pods_preempt_place<4>, (const void*)k_spp_final,
+                        (const void*)k_bucket_small, (const void*)k_bucket_hist8<false>, (const void*)k_bucket_hist8<true>,
+                        (const void*)k_bucket_scan_rows, (const void*)k_bucket_scan8, (const void*)k_bucket_hist,
+                        (const void*)k_bucket_scan, (const void*)k_bucket_scatter};
+    for (const void* k : ks) { cudaFuncAttributes fa; CU(cudaFuncGetAttributes(&fa, k)); }
+    if (ctx->pp_occ < 0) {
+        int occ = 0;
+        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_preempt_place<4>, 128, 0));
+        ctx->pp_occ = occ;
+    }
+    return DRA_OK;
+}
+
+// The sharded preempt-and-place call's buffers for these sizes: the §15 walk's, the sort's, and the scratch inventory
+int spp_buffers(dra_ctx* ctx, uint32_t n_pod, uint32_t n_pair, uint32_t rn_pod) {
+    int rc;
+    if ((rc = ensure_batch(ctx, std::max(std::max(rn_pod, n_pair), 1u), 1, false))) return rc;
+    if ((rc = pp_buffers(ctx, n_pod, n_pair, rn_pod))) return rc;
+    if ((rc = grow(ctx, ctx->d_spp_inv, ctx->cap_spp_inv, std::max(ctx->n_gpu, 1u)))) return rc;
+    if (!ctx->d_spp_gate) CU(cudaMalloc((void**)&ctx->d_spp_gate, 16));
     return DRA_OK;
 }
 
@@ -2105,6 +2156,19 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
         if (int rc = preload_preempt_shard(ctx)) return rc;
         if (int rc = spre_buffers(ctx, ctx->peer_pre_pods, ctx->peer_pre_pairs, ctx->peer_pre_victims, 0)) return rc;
         if (ctx->d_inv_live) { if (int rc = ensure_batch(ctx, 1, 1, false)) return rc; }
+    }
+    // sharded preempt and place, after dra_set_shard_preempt_place: its kernels loaded and its buffers at full size now (no
+    // module load and no cudaFree inside a call while a peer's exchange waits for this rank)
+    ctx->peer_spp_pods = ctx->spp_max_pods; ctx->peer_spp_pairs = ctx->spp_max_pairs; ctx->peer_spp_run = ctx->spp_max_run;
+    if (ctx->peer_spp_pods) {
+        reserve(ctx->spp_x, 0, 0, (size_t)PEER_MAX * 4);
+        if (int rc = preload_preempt_place_shard(ctx)) return rc;
+        if (ctx->d_inv_live) { if (int rc = spp_buffers(ctx, ctx->peer_spp_pods, ctx->peer_spp_pairs, ctx->peer_spp_run)) return rc; }
+        if ((size_t)tab_len + 16 > ctx->cap_gtable) {                     // the call's table, at the exported size
+            const size_t ncap = (size_t)tab_len + 16;
+            if (int rc = grow_nc(ctx, ctx->d_gtable, 0, ncap)) return rc;
+            ctx->cap_gtable = ncap;
+        }
     }
     ctx->splace_seq = 0;
     if (ctx->d_splace_local) CU(cudaMemset(ctx->d_splace_local, 0, 64 + ctx->cap_splace_local * 8));
@@ -2895,6 +2959,172 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     ctx->launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded preemption launch: %s", cudaGetErrorString(e));
+    return DRA_OK;
+}
+
+int dra_set_shard_preempt_place(dra_ctx* ctx, uint32_t max_pods, uint32_t max_pairs, uint32_t max_run) {
+    if (!ctx) return DRA_E_INVAL;
+    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "dra_set_shard_preempt_place: call it before dra_shard_export");
+    if (max_pods > (1u << 26) || max_pairs > 0xFFFFFFF0u || max_run > (1u << 26))
+        return fail(ctx, DRA_E_INVAL, "dra_set_shard_preempt_place: sizes too large (max_pods, max_run <= 2^26, max_pairs <= 2^32 - 16)");
+    ctx->spp_max_pods = max_pods; ctx->spp_max_pairs = max_pairs; ctx->spp_max_run = max_run;
+    return DRA_OK;
+}
+
+// Sharded preempt and place: the world's state into the scratch inventory (own range from the live copy, the others over
+// the inventory sync's exchange: k_peer_push, k_isync_copy) -> §15's chain on the scratch copy, identical on every rank
+// (k_pre_running, the counting sort, k_pre_vsort, k_spp_prep, the counting sort of the pairs, k_pods_preempt_place) ->
+// the caller's outputs and the own GPU range back into the live copy (k_spp_final).  Enqueues only.
+int dra_preempt_place_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                          const uint32_t* d_pod_off, const int32_t* d_prio, uint32_t n_pod,
+                                          const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                          const dra_running_pods* running, const uint32_t* d_out_off, uint32_t n_out,
+                                          uint32_t* d_pod_node, uint8_t* d_pod_status, uint32_t* d_evicted_by, uint32_t flags) {
+    if (!ctx || !d_pod_off || !running || !running->pod_off || (n_claim && !d_claims) ||
+        (n_pod && (!d_prio || !d_pod_node || !d_pod_status)))
+        return DRA_E_INVAL;
+    const dra_running_pods& R = *running;
+    if ((R.n_claim && !R.claims) || (R.n_pod && (!R.prio || !d_evicted_by)) || (R.n_out && !R.out)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~DRA_F_EXHAUSTIVE)
+        return fail(ctx, DRA_E_INVAL, "dra_preempt_place_batch_global_device: unknown flags 0x%x (DRA_F_FRESH_INVENTORY is not taken)", flags);
+    if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (n_pod > (1u << 26) || R.n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
+    if (int rc = check_slots(ctx, n_claim, n_out, d_out_off != nullptr)) return rc;
+    if (!n_pod && n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]: no pods for %u claims", n_claim);
+    const bool dense = d_cand_nodes == nullptr && d_cand_off == nullptr;
+    if (!dense && (!d_cand_nodes || !d_cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
+    if (dense && n_pair) return fail(ctx, DRA_E_INVAL, "dense form: n_pair must be 0");
+    if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
+    const uint64_t walk64 = dense ? (uint64_t)n_pod * ctx->n_node : n_pair;     // the pairs the walk judges
+    if (walk64 > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    const uint32_t walk = (uint32_t)walk64;
+    const bool gather = ctx->world > 1;
+    if (gather) {
+        if (!ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the exchange needs every rank's range)");
+        if (int rc = need_peers(ctx)) return rc;
+        if (ctx->shard_bounds[ctx->world] != ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard map does not span the inventory's %u nodes", ctx->n_node);
+        if (!ctx->peer_inv_gpus) return fail(ctx, DRA_E_STATE, "the inventory was not loaded before dra_shard_export: the export reserved no staging for it");
+        if (ctx->n_gpu > ctx->peer_inv_gpus)
+            return fail(ctx, DRA_E_STATE, "the inventory grew to %u GPUs after dra_shard_export reserved staging for %u", ctx->n_gpu, ctx->peer_inv_gpus);
+        if (!ctx->peer_spp_pods) return fail(ctx, DRA_E_STATE, "dra_set_shard_preempt_place was not called before dra_shard_export");
+        if (n_pod > ctx->peer_spp_pods || walk > ctx->peer_spp_pairs || R.n_pod > ctx->peer_spp_run)
+            return fail(ctx, DRA_E_INVAL, "n_pod %u / pairs %u / running pods %u exceed the sizes of dra_set_shard_preempt_place before "
+                        "dra_shard_export (%u / %u / %u)", n_pod, walk, R.n_pod, ctx->peer_spp_pods, ctx->peer_spp_pairs, ctx->peer_spp_run);
+        if (n_out > ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", n_out, ctx->peer_tab_len);
+    }
+    ctx->chain = DRA_K_PREEMPT_PLACE_SHARD; ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
+    CU(cudaSetDevice(ctx->device));
+    // peers on this device may already wait for this rank: no buffer this call outgrows is freed before the next sync
+    struct DeferFree { dra_ctx* c; ~DeferFree() { c->defer_free = false; } } defer{ctx};
+    ctx->defer_free = gather;
+    int rc = upload_table(ctx);
+    if (rc) return rc;
+    if ((rc = spp_buffers(ctx, n_pod, walk, R.n_pod))) return rc;
+    if (ctx->pp_occ < 0 && (rc = preload_preempt_place_shard(ctx))) return rc;
+    if (ctx->pp_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_preempt_place: no CTA can be resident");
+    // The table is this context's own: every rank computes the whole of it, so no packet moves and the gather's epochs,
+    // parities and cursors are left to the calls that gather
+    if ((size_t)n_out + 16 > ctx->cap_gtable) {
+        const size_t ncap = (size_t)n_out + n_out / 4 + 64;
+        if ((rc = grow_nc(ctx, ctx->d_gtable, 0, ncap))) return rc;
+        ctx->cap_gtable = ncap;
+    }
+    uint2* table = ctx->d_gtable;
+    cudaStream_t st = ctx->stream;
+    const Err err = err_of(ctx);
+    // world 1: the rank owns every GPU
+    const uint32_t gpu_lo = gather ? ctx->h_node_off[ctx->shard_bounds[ctx->rank]] : 0u;
+    const uint32_t gpu_hi = gather ? ctx->h_node_off[ctx->shard_bounds[ctx->rank + 1]] : ctx->n_gpu;
+    Prof prof(ctx);
+    CU(cudaMemsetAsync(ctx->d_spp_gate, 0, 4, st));
+    CU(cudaMemcpyAsync(ctx->d_spp_inv, ctx->d_inv_live, (size_t)ctx->n_gpu * 16, cudaMemcpyDeviceToDevice, st));
+    if (gather) {
+        const PeerExchange x = bind_exchange(ctx, ctx->isync_x);
+        InvSync s; memset(&s, 0, sizeof s);
+        s.inv = ctx->d_spp_inv; s.n_gpu = ctx->n_gpu; s.own_lo = gpu_lo; s.own_hi = gpu_hi;
+        s.elect = (uint32_t*)(ctx->peer_local + ctx->isync_x.flags) + PEER_MAX;
+        k_peer_push<<<std::max(1u, std::min((gpu_hi - gpu_lo + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, st>>>(x, ctx->d_inv_live, gpu_lo, gpu_hi);
+        // a small grid: it waits for its peers, and ranks sharing one device must not find their walk's SMs held by it
+        k_isync_copy<<<std::max(1u, std::min((ctx->n_gpu + 255) / 256, (uint32_t)std::max(1, ctx->n_sm / 4))), 256, 0, st>>>(x, s);
+        // one verdict for the world: the call fails on every rank or on none
+        k_spp_agree<<<1, 32, 0, st>>>(bind_exchange(ctx, ctx->spp_x), s.elect, x.seq, ctx->d_spp_gate);
+        ctx->launches += 3;
+    }
+    if (n_out) CU(cudaMemsetAsync(table, 0, (size_t)n_out * 8, st));
+    CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)ctx->n_node + 1) * 4, st));
+    CU(cudaMemsetAsync(ctx->d_pp_judged, 0, ((size_t)ctx->n_node + 1) * 4, st));
+    if (R.n_pod) CU(cudaMemsetAsync(ctx->d_pp_evicted, 0xFF, (size_t)R.n_pod * 4, st));
+
+    PreArgs a; memset(&a, 0, sizeof a);
+    a.claims = (const uint4*)d_claims; a.pod_off = d_pod_off; a.prio = d_prio; a.n_pod = n_pod;
+    a.cand_nodes = dense ? nullptr : d_cand_nodes; a.cand_off = dense ? nullptr : d_cand_off; a.n_pair = walk;
+    a.rclaims = (const uint4*)R.claims; a.rn_claim = R.n_claim; a.rpod_off = R.pod_off; a.rprio = R.prio; a.rn_pod = R.n_pod;
+    a.rout_off = R.out_off; a.rout = (const uint2*)R.out; a.rn_out = R.n_out;
+    a.rrec = ctx->d_pre_rrec; a.rsorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.vlist = ctx->d_pre_vlist;
+    a.inv = ctx->d_spp_inv; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.n_gpu = ctx->n_gpu; a.tbl = ctx->d_tbl;
+    a.sel = sel_of(ctx); a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
+    a.psum = ctx->d_pre_psum; a.psum64 = ctx->d_pre_psum64;
+    a.pod_node = ctx->d_pre_node; a.pod_status = ctx->d_pre_pst;
+    a.gate = ctx->d_err + ERR_BAD_OFFSETS; a.err = err;
+    // the running lists (§14), on global GPU indices: every rank finds the same faults
+    k_pre_running<<<std::max(1u, (R.n_pod + 255) / 256), 256, 0, st>>>(a);
+    ctx->launches += 1;
+    if (R.n_pod) {
+        if ((rc = launch_sort(ctx, ctx->d_pre_rrec, R.n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_spp_inv, false, ctx->n_node, ctx->d_node_off)))
+            return rc;
+        if (ctx->n_node) {
+            k_pre_vsort<<<std::min(ctx->n_node, (uint32_t)ctx->n_sm * 8u), 256, 0, st>>>(a);
+            ctx->launches += 1;
+        }
+        CU(cudaMemcpyAsync(ctx->d_pp_runoff, ctx->d_claim_off, ((size_t)ctx->n_node + 1) * 4, cudaMemcpyDeviceToDevice, st));
+    } else {
+        CU(cudaMemsetAsync(ctx->d_pp_runoff, 0, ((size_t)ctx->n_node + 1) * 4, st));
+    }
+    a.list_off = ctx->d_pp_runoff;
+    // the checks of the pending arrays and the visit lists (§13)
+    PlaceArgs pl; memset(&pl, 0, sizeof pl);
+    pl.claims = a.claims; pl.pod_off = d_pod_off; pl.n_pod = n_pod;
+    pl.cand_nodes = a.cand_nodes; pl.cand_off = a.cand_off;
+    pl.out_off = d_out_off; pl.out = table;
+    pl.state = ctx->d_place_state; pl.pairs = ctx->d_podrec;
+    pl.sorted = ctx->d_sorted; pl.list_off = ctx->d_claim_off; pl.cursor = ctx->d_place_cursor;
+    pl.inv_src = ctx->d_spp_inv; pl.inv_dst = ctx->d_spp_inv; pl.node_off = ctx->d_node_off; pl.tbl = ctx->d_tbl;
+    pl.n_node = ctx->n_node; pl.exhaustive = a.exhaustive; pl.sel = a.sel; pl.err = err;
+    PpArgs pp{ctx->d_pp_pending, ctx->d_pp_evicted, ctx->d_pp_judged};
+    SppArgs s; memset(&s, 0, sizeof s);
+    s.n_claim = n_claim; s.n_pair = n_pair; s.n_out = n_out; s.gate = ctx->d_spp_gate; s.err_dev = ctx->d_err;
+    s.pod_node_src = ctx->d_pre_node; s.pod_status_src = ctx->d_pre_pst; s.evicted_src = ctx->d_pp_evicted;
+    s.pod_node = d_pod_node; s.pod_status = d_pod_status; s.evicted_by = d_evicted_by; s.n_pod = n_pod; s.rn_pod = R.n_pod;
+    s.inv_src = ctx->d_spp_inv; s.inv_dst = ctx->d_inv_live; s.gpu_lo = gpu_lo; s.gpu_hi = gpu_hi;
+    k_spp_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, pl, pp, s);
+    ctx->launches += 1;
+    if (!dense && n_pair &&
+        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_spp_inv, false, ctx->n_node, ctx->d_node_off)))
+        return rc;
+    if (ctx->n_node) {
+        // Every CTA resident, but not a cooperative launch: ranks sharing this device run their walks side by side (each
+        // takes its share of the residency, less one CTA per SM left for a peer's waiting exchange).  The walk itself waits
+        // for no peer.
+        const int k = gather ? std::max(1, ctx->peers_on_device) : 1;
+        const int per_sm = k > 1 ? std::max(1, ctx->pp_occ - 1) : ctx->pp_occ;
+        const uint32_t share = (uint32_t)std::max(1, per_sm * ctx->n_sm / k);
+        const uint32_t grid = std::max(1u, std::min((ctx->n_node + 3) / 4, share));
+        PreArgs aw = a;
+        aw.gate = ctx->d_spp_gate;
+        k_pods_preempt_place<4><<<grid, 128, 0, st>>>(aw, pl, pp);
+        ctx->launches += 1;
+    }
+    const uint32_t fin = std::max(std::max(n_pod, R.n_pod), gpu_hi - gpu_lo);
+    k_spp_final<<<std::max(1u, std::min((fin + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, st>>>(s);
+    ctx->launches += 1;
+    ctx->chain |= DRA_K_PREEMPT_PLACE_SHARD;
+    prof.mark();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded preempt-and-place launch: %s", cudaGetErrorString(e));
+    ctx->gather_table = (const dra_out_rec*)table; ctx->gather_n_per = n_out; ctx->gather_len = n_out;
     return DRA_OK;
 }
 

@@ -3843,11 +3843,7 @@ struct PpArgs {
 // NONE, so the sort drops them, as do every pair of a pod that is never judged).  A pod that is never judged is decided
 // here: an empty pod is FITS on its first candidate naming a node, with nothing written; a pod of more than 32 claims is
 // INVALID; a pod with no candidate naming a node is INVALID or NO.
-__global__ void __launch_bounds__(256)
-k_pp_prep(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (p >= pl.n_pod) return;
+__device__ __forceinline__ void pp_prep_pod(const PreArgs& a, const PlaceArgs& pl, const PpArgs& pp, uint32_t p, uint32_t lane) {
     const uint32_t c0 = __ldg(&pl.pod_off[p]), cnt = __ldg(&pl.pod_off[p + 1]) - c0;
     const bool live = cnt != 0 && cnt <= DRA_MAX_POD;
     uint32_t first = DRA_GPU_NONE, usable = 0;
@@ -3889,6 +3885,14 @@ k_pp_prep(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
         }
     }
     if (cnt != 0 && !judged) place_fail(pl, c0, cnt, DRA_ST_POD, lane);
+}
+
+__global__ void __launch_bounds__(256)
+k_pp_prep(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (p >= pl.n_pod) return;
+    pp_prep_pod(a, pl, pp, p, lane);
 }
 
 // Persistent: every CTA resident (cooperative launch); warp w owns nodes w, w + warps, ... and cycles over them.  Minimum
@@ -4019,6 +4023,93 @@ k_pods_preempt_place(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
             break;
         }
     }
+}
+
+// ---- preempt and place on a sharded world (dra_preempt_place_batch_global_device) -----------------------------------
+// Every rank gets the same pending pods, candidates and running pods.  Each rank assembles the world's state in a scratch
+// copy of the inventory: its own GPU range from its live copy, every other range from the owning rank over the inventory
+// sync's exchange (k_peer_push of the live own range, k_isync_copy into the scratch copy).  Then every rank runs §15's
+// chain on the scratch copy — k_pre_running, the counting sort, k_pre_vsort, k_spp_prep, the counting sort of the pairs and
+// k_pods_preempt_place — so every rank takes the same decisions in the same order, and k_spp_final hands the caller the
+// outputs and copies the rank's own GPU range back into its live copy.  The walk waits for no peer: the only wait is the
+// exchange, before anything is judged.
+struct SppArgs {
+    uint32_t n_claim, n_pair, n_out;             // the pending arrays' lengths (n_pair 0: dense form)
+    uint32_t* gate;                              // non-zero: a pending or running fault, or a peer missing; nothing is written
+    const uint32_t* err_dev;                     // the context's device error words
+    const uint32_t* pod_node_src; const uint8_t* pod_status_src; const uint32_t* evicted_src;   // the walk's outputs
+    uint32_t* pod_node; uint8_t* pod_status; uint32_t* evicted_by;                          // the caller's
+    uint32_t n_pod, rn_pod;
+    const uint4* inv_src; uint4* inv_dst; uint32_t gpu_lo, gpu_hi;   // scratch -> live over this rank's GPU range
+};
+
+// One warp, after k_isync_copy: the world agrees on the exchange's verdict, so that the call fails on every rank or on
+// none.  Lane p publishes this rank's verdict (its copy kernel's, `elect`[1], and no timeout here) to peer p as the flag
+// {seq : ok}, then waits for peer p's.  A peer's failure, or a peer whose verdict does not arrive within the spin limit,
+// closes the gate and sets ERR_PEER_TIMEOUT.  A rank that timed out in the exchange publishes its failure at once, before
+// any peer that received everything can stop waiting for it here, so a late peer fails the call everywhere.
+__global__ void __launch_bounds__(32)
+k_spp_agree(const PeerExchange x, const uint32_t* __restrict__ elect, uint32_t sync_seq, uint32_t* gate) {
+    const uint32_t tid = threadIdx.x;
+    uint32_t v1;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v1) : "l"(elect + 1) : "memory");
+    const uint32_t ok = (v1 == (sync_seq << 1 | 1u) && !__ldcg(&x.err.dev[ERR_PEER_TIMEOUT])) ? 1u : 0u;
+    const uint32_t mine = x.seq << 1 | ok;
+    bool fail = ok == 0u;
+    if (tid < x.world && tid != x.rank) {
+        asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(x.flag[tid]), "r"(mine) : "memory");
+        const long long t0 = clock64();
+        uint32_t v;
+        while (true) {
+            asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(x.my_flags + tid) : "memory");
+            if ((int32_t)((v >> 1) - x.seq) >= 0) { fail = fail || (v >> 1) != x.seq || !(v & 1u); break; }
+            if (clock64() - t0 > x.spin_limit) { fail = true; break; }
+        }
+    }
+    if (__any_sync(FULLMASK, fail) && tid == 0) { *gate = 1u; x.err.set(ERR_PEER_TIMEOUT); }
+}
+
+// Warp per pod: k_splace_prep's device-side checks of the pending arrays (pod_off and cand_off monotone and spanning them,
+// at most PL_POS candidates, every claim's slots inside n_out, counted as dra_preempt_place_batch counts them), then
+// k_pp_prep's work for a pod that passes.  A faulty pod sets ERR_BAD_OFFSETS and the gate and writes nothing.  Warp 0 also
+// closes the gate on the faults found before it: the running pods' (k_pre_running) and a peer missing from the exchange.
+__global__ void __launch_bounds__(256)
+k_spp_prep(const PreArgs a, const PlaceArgs pl, const PpArgs pp, const SppArgs s) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (p == 0 && lane == 0 && (__ldcg(&s.err_dev[ERR_BAD_OFFSETS]) || __ldcg(&s.err_dev[ERR_PEER_TIMEOUT]))) *s.gate = 1u;
+    if (p >= pl.n_pod) return;
+    const bool have_off = pl.out_off != nullptr;
+    const uint32_t c0 = __ldg(&pl.pod_off[p]), c1 = __ldg(&pl.pod_off[p + 1]);
+    bool fault = c1 < c0 || c1 > s.n_claim || (p == 0 && (c0 != 0 || __ldg(&pl.pod_off[pl.n_pod]) != s.n_claim));
+    if (pl.cand_off) {
+        const uint32_t k0 = __ldg(&pl.cand_off[p]), k1 = __ldg(&pl.cand_off[p + 1]);
+        fault = fault || k1 < k0 || k1 > s.n_pair || k1 - k0 > PL_POS || (p == 0 && (k0 != 0 || __ldg(&pl.cand_off[pl.n_pod]) != s.n_pair));
+    }
+    if (!fault)
+        for (uint32_t i = c0 + lane; i < c1; i += 32) {
+            const uint4 c = __ldg(&pl.claims[i]);
+            const uint32_t kind = c.x & 0xFFu, count = c.x >> 16;
+            const bool gpu = kind == DRA_KIND_GPU && count >= 1 && count <= DRA_MAX_COUNT && (have_off || count == 1);
+            const uint32_t slots = gpu ? count : 1u, dst = have_off ? __ldg(&pl.out_off[i]) : i;
+            fault = fault || dst > s.n_out || slots > s.n_out - dst;
+        }
+    if (__any_sync(FULLMASK, fault)) {
+        if (lane == 0) { *s.gate = 1u; a.err.set(ERR_BAD_OFFSETS); }
+        return;
+    }
+    pp_prep_pod(a, pl, pp, p, lane);
+}
+
+// Grid-stride, after the walk: with the gate open and the walk complete, the caller's pod_node, pod_status and evicted_by
+// from the walk's, and this rank's own GPU range from the scratch copy into the live one.  Otherwise nothing.
+__global__ void __launch_bounds__(256)
+k_spp_final(const SppArgs s) {
+    if (__ldcg(s.gate) || __ldcg(&s.err_dev[ERR_DEVICE_WAIT])) return;
+    const uint32_t t0 = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
+    for (uint32_t i = t0; i < s.n_pod; i += nt) { s.pod_node[i] = __ldcg(&s.pod_node_src[i]); s.pod_status[i] = __ldcg(&s.pod_status_src[i]); }
+    for (uint32_t i = t0; i < s.rn_pod; i += nt) s.evicted_by[i] = __ldcg(&s.evicted_src[i]);
+    for (uint32_t i = s.gpu_lo + t0; i < s.gpu_hi; i += nt) s.inv_dst[i] = __ldcg(&s.inv_src[i]);
 }
 
 // ---- sharded preemption (dra_preempt_batch_global_device) ----------------------------------------------------------
