@@ -337,10 +337,11 @@ int  dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
  *   evicted_by[r]    the pod that evicted running pod r, else 0xFFFFFFFF (each pod's victims in eviction order:
  *                    priority descending, then index)
  * A pod placed nowhere takes nothing: its slots carry DRA_ST_SEARCH_LIMIT when its status is DRA_PRE_SEARCH_LIMIT, else
- * DRA_ST_POD (DRA_ST_INVALID for claims invalid by §3/§10, every claim of a pod of more than DRA_MAX_POD).  An empty pod
- * is FITS on its first candidate naming a node, with nothing written.  The call RELEASES THE VICTIMS ITSELF: their
- * allocations are gone from the live inventory when it returns, so the caller must not pass them to
- * dra_deallocate_batch again.  DRA_E_INVAL, with no output and no inventory word written: unknown flags, pod_off /
+ * DRA_ST_POD (DRA_ST_INVALID for claims invalid by §3/§10, every claim of a pod of more than DRA_MAX_POD).  A pod with
+ * a claim invalid in the call's slot mode (without out_off, a GPU claim of count != 1) is DRA_PRE_INVALID and evicts
+ * nothing.  An empty pod is FITS on its first candidate naming a node, with nothing written.  The call RELEASES THE
+ * VICTIMS ITSELF: their allocations are gone from the live inventory when it returns, so the caller must not pass them
+ * to dra_deallocate_batch again.  DRA_E_INVAL, with no output and no inventory word written: unknown flags, pod_off /
  * cand_off / running->pod_off not monotone or not spanning, more than 2^30 - 1 candidates for a pod or nodes in the
  * inventory, dense n_pod * n_node >= 2^32, a pending slot outside n_out, a running slot range outside running->n_out, a
  * running pod whose OK slots name a GPU index >= n_gpu or GPUs of two nodes.  n_pod == 0 returns DRA_OK after the

@@ -3841,11 +3841,22 @@ struct PpArgs {
 
 // Warp per pod: state word, open-pair count, pair records (candidate form; pairs naming no node are NO and carry node
 // NONE, so the sort drops them, as do every pair of a pod that is never judged).  A pod that is never judged is decided
-// here: an empty pod is FITS on its first candidate naming a node, with nothing written; a pod of more than 32 claims is
-// INVALID; a pod with no candidate naming a node is INVALID or NO.
+// here: an empty pod is FITS on its first candidate naming a node, with nothing written; a pod of more than 32 claims, or
+// with a claim invalid in the call's slot mode (a GPU claim of count != 1 without out_off), is INVALID; a pod with no
+// candidate naming a node is NO.  (The pair judgement assumes out_off: it must never see a pod the apply would reject.)
 __device__ __forceinline__ void pp_prep_pod(const PreArgs& a, const PlaceArgs& pl, const PpArgs& pp, uint32_t p, uint32_t lane) {
     const uint32_t c0 = __ldg(&pl.pod_off[p]), cnt = __ldg(&pl.pod_off[p + 1]) - c0;
-    const bool live = cnt != 0 && cnt <= DRA_MAX_POD;
+    const bool have_off = pl.out_off != nullptr;
+    bool inv = cnt > DRA_MAX_POD;
+    if (!inv) {
+        for (uint32_t i = lane; i < cnt; i += 32) {
+            const uint4 c = __ldg(&pl.claims[c0 + i]);
+            const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
+            inv = inv || claim_invalid(kind, prof, count, have_off) || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
+        }
+        inv = __any_sync(FULLMASK, inv);
+    }
+    const bool live = cnt != 0 && !inv;
     uint32_t first = DRA_GPU_NONE, usable = 0;
     if (!pl.cand_off) {
         usable = pl.n_node;
@@ -3866,15 +3877,6 @@ __device__ __forceinline__ void pp_prep_pod(const PreArgs& a, const PlaceArgs& p
         }
     }
     const bool judged = live && usable != 0;
-    bool inv = cnt > DRA_MAX_POD;
-    if (live && !usable) {
-        for (uint32_t i = lane; i < cnt; i += 32) {
-            const uint4 c = __ldg(&pl.claims[c0 + i]);
-            const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
-            inv = inv || claim_invalid(kind, prof, count, true) || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
-        }
-        inv = __any_sync(FULLMASK, inv);
-    }
     if (lane == 0) {
         pp.pending[p] = usable;
         pl.state[p] = judged ? PP_OPEN : PP_NOWHERE;

@@ -89,6 +89,10 @@ PREEMPT_API int pp_oracle_preempt_place(dra_gpu_rec* gpus, uint32_t n_gpu, const
         uint32_t k0 = dense ? 0 : cand_off[p], k1 = dense ? n_node : cand_off[p + 1];
         int have_best = 0, any_lim = 0; uint32_t fit_k = DRA_GPU_NONE, best_k = 0;
         pair_sum best = { 0 };
+        /* a claim invalid in the call's slot mode: INVALID, judged nowhere (judge() assumes out_off) */
+        int inv = cnt > DRA_MAX_POD;
+        for (uint32_t i = 0; i < cnt && !inv; i++) { dra_claim_rec t = claims[c0 + i]; t.node = 0; inv = claim_invalid(&t, 1, have_off); }
+        if (inv) k1 = k0;
         for (uint32_t k = k0; k < k1; k++) {              /* §14's pairs on the current state */
             uint32_t n = dense ? k : cand_nodes[k];
             if (n < n_node && cnt <= DRA_MAX_POD)
@@ -102,11 +106,7 @@ PREEMPT_API int pp_oracle_preempt_place(dra_gpu_rec* gpus, uint32_t n_gpu, const
         uint32_t n = DRA_GPU_NONE;
         if (fit_k != DRA_GPU_NONE) { n = dense ? fit_k : cand_nodes[fit_k]; pod_status[p] = PRE_FITS; }
         else if (have_best) { n = dense ? best_k : cand_nodes[best_k]; pod_status[p] = PRE_EVICT; }
-        else {
-            int inv = cnt > DRA_MAX_POD;
-            for (uint32_t i = 0; i < cnt && !inv; i++) { dra_claim_rec t = claims[c0 + i]; t.node = 0; inv = claim_invalid(&t, 1, 1); }
-            pod_status[p] = inv ? PRE_INVALID : any_lim ? PRE_LIMIT : PRE_NO;
-        }
+        else pod_status[p] = inv ? PRE_INVALID : any_lim ? PRE_LIMIT : PRE_NO;
         pod_node[p] = n;
         if (n == DRA_GPU_NONE) {                          /* placed nowhere: the inventory is unchanged */
             for (uint32_t i = c0; i < c0 + cnt; i++) {

@@ -80,9 +80,12 @@ def pending_slots(claims, out_off=None):
 
 
 def preempt_place(gpus, node_off, table, claims, pod_off, prio, run_claims, run_pod_off, run_prio, run_out,
-                  run_out_off=None, cand_nodes=None, cand_off=None, out_off=None, n_out=None, flags: int = 0):
+                  run_out_off=None, cand_nodes=None, cand_off=None, out_off=None, n_out=None, flags: int = 0,
+                  fill: int | None = None):
     """spec §15.  cand_nodes/cand_off None = every pod against every node, ascending.  Returns (out, pod_node,
-    pod_status, evicted_by, gpus_after).  Raises ValueError on the arguments §15 rejects.  Inputs are not modified."""
+    pod_status, evicted_by, gpus_after).  Raises ValueError on the arguments §15 rejects.  Inputs are not modified.
+    fill: every byte of the four outputs starts as `fill`, so what the call does not write (slots no claim owns, and
+    evicted_by when there are no pending pods) keeps it; None: zeros, and evicted_by 0xFFFFFFFF."""
     g = np.ascontiguousarray(gpus, dtype=O.GPU_DTYPE).copy()
     off = np.ascontiguousarray(node_off, dtype=np.uint32)
     t = np.ascontiguousarray(table)
@@ -105,10 +108,16 @@ def preempt_place(gpus, node_off, table, claims, pod_off, prio, run_claims, run_
     n_rout = len(run_out) if run_out is not None else 0
     roo = None if run_out_off is None else _nz(run_out_off, np.uint32)
     n_run = len(rpo) - 1
-    out = np.zeros(max(n_out, 1), O.OUT_DTYPE)
-    pnode = np.zeros(max(n_pod, 1), np.uint32)
-    pstat = np.zeros(max(n_pod, 1), np.uint8)
-    ev = np.full(max(n_run, 1), NONE, np.uint32)
+    def filled(n, dtype):
+        return np.full(max(n, 1) * np.dtype(dtype).itemsize, fill, np.uint8).view(dtype)
+    if fill is None:
+        out = np.zeros(max(n_out, 1), O.OUT_DTYPE)
+        pnode = np.zeros(max(n_pod, 1), np.uint32)
+        pstat = np.zeros(max(n_pod, 1), np.uint8)
+        ev = np.full(max(n_run, 1), NONE, np.uint32)
+    else:
+        out, pnode, pstat, ev = (filled(n_out, O.OUT_DTYPE), filled(n_pod, np.uint32), filled(n_pod, np.uint8),
+                                 filled(n_run, np.uint32))
     rc = lib().pp_oracle_preempt_place(_p(g), len(g), _p(off), len(off) - 1, _p(t), _p(c), n_claim, _p(po), _p(pr), n_pod,
                                        _p(cn), _p(co), _p(rc_), len(run_claims) if run_claims is not None else 0, _p(rpo),
                                        _p(rpr), n_run, _p(roo), _p(ro), n_rout, _p(oo), _p(out), n_out, _p(pnode),
@@ -169,21 +178,25 @@ def preempt_place_naive(gpus, node_off, table, claims, pod_off, prio, cands, exh
     for p in range(len(pod_off) - 1):
         c0, c1 = pod_off[p], pod_off[p + 1]
         pod = claims[c0:c1]
-        alive = [r for r in range(n_run) if evicted_by[r] == NONE]
-        idx = [i for r in alive for i in range(run_pod_off[r], run_pod_off[r + 1])]
-        rpo = [0]
-        for r in alive:
-            rpo.append(rpo[-1] + run_pod_off[r + 1] - run_pod_off[r])
-        _, _, node, st, nv, rows = preempt_naive(
-            N._dump(gpus, G), node_off, table, pod, [0, len(pod)], [prio[p]], None if cands is None else [cands[p]],
-            exhaustive, [run_claims[i] for i in idx], rpo, [run_prio[r] for r in alive], [run_out[i] for i in idx],
-            None, max(len(alive), 1))
-        node, st = node[0], st[0]
+        if len(pod) > N.MAX_POD or any(N._invalid(dict(c, node=0), 1, have_off) for c in pod):
+            # invalid in the call's slot mode: not handed to §14, which judges as if out_off were given
+            node, st = NONE, INVALID
+        else:
+            alive = [r for r in range(n_run) if evicted_by[r] == NONE]
+            idx = [i for r in alive for i in range(run_pod_off[r], run_pod_off[r + 1])]
+            rpo = [0]
+            for r in alive:
+                rpo.append(rpo[-1] + run_pod_off[r + 1] - run_pod_off[r])
+            _, _, node, st, nv, rows = preempt_naive(
+                N._dump(gpus, G), node_off, table, pod, [0, len(pod)], [prio[p]], None if cands is None else [cands[p]],
+                exhaustive, [run_claims[i] for i in idx], rpo, [run_prio[r] for r in alive], [run_out[i] for i in idx],
+                None, max(len(alive), 1))
+            node, st = node[0], st[0]
+            for v in rows[0][: nv[0]]:
+                evicted_by[alive[v]] = p
+                release(alive[v])
         pod_node.append(node)
         pod_status.append(st)
-        for v in rows[0][: nv[0]]:
-            evicted_by[alive[v]] = p
-            release(alive[v])
         if node != NONE:
             if pod:
                 _, recs = N.eval_pod(G, node_off[node], node_off[node + 1], table, [dict(c, node=node) for c in pod],

@@ -5,9 +5,11 @@ records.default_table(), now and then an UNAVAILABLE GPU), running pods placed o
 their records match the inventory), optionally perturbed afterwards into records that do not match it, priorities drawn
 from a pool with the int32 extremes and many ties, pending pods of 0 to 33 claims, and candidate lists with duplicates,
 strays and more than 32 entries.  The same builder draws from hypothesis (`problems()`) or from a seeded numpy generator
-(`random_problem`), so the GPU suite can also make larger problems of the same kind without hypothesis."""
+(`random_problem`), so the GPU suite can also make larger problems of the same kind without hypothesis.  `build_place`
+makes spec §15 (preempt and place) problems of the same kind, with the pending pods' out_off in one of four forms."""
 from __future__ import annotations
 
+import dataclasses
 import importlib
 from dataclasses import dataclass
 
@@ -323,3 +325,82 @@ def problems(draw):
 
 def random_problem(seed: int, scale: int = 1) -> Problem:
     return build(_Rng(np.random.default_rng(seed)), scale)
+
+
+# ---- spec §15 (preempt and place) -----------------------------------------------------------------------------------
+OUT_FORMS = ("none", "packed", "gaps", "spare")
+
+
+@dataclass
+class PlaceProblem(Problem):
+    """A §15 problem: a §14 problem with the pending pods' out_off (None: the call passes none) and n_out.  `error` is
+    the §15 oracle's verdict on the call."""
+    out_off: np.ndarray | None = None
+    n_out: int = 0
+    form: str = "none"
+
+    def pp_oracle(self, gpus=None, flags=None, fill=None):
+        """preempt_place_oracle.preempt_place on this problem (on `gpus` when given); raises ValueError on a call-level
+        error"""
+        import preempt_place_oracle as PP
+        cn, co = self.cand_arrays()
+        return PP.preempt_place(self.gpus if gpus is None else gpus, self.node_off, self.table, self.claims, self.pod_off,
+                                self.prio, self.run_claims, self.run_pod_off, self.run_prio, self.run_out,
+                                self.run_out_off, cn, co, self.out_off, self.n_out, self.flags if flags is None else flags,
+                                fill)
+
+
+def pending_out_off(D, claims, form):
+    """(out_off, n_out) of the pending claims in one of OUT_FORMS; slots never overlap (where overlapping slots end up
+    depends on the order in which pods on different nodes are applied, which §13 and §15 leave open)"""
+    if form == "none":
+        return None, len(claims)
+    placed = claims.copy()
+    placed["node"] = 0
+    sl = R.claim_slots(placed, 1, True).astype(np.int64)
+    if form == "gaps":                                   # claims laid out in a random order, with holes between them
+        order = list(range(len(claims)))
+        for i in range(len(order) - 1, 0, -1):
+            j = D.int(0, i)
+            order[i], order[j] = order[j], order[i]
+        oo = np.zeros(len(claims), np.uint32)
+        cur = 0
+        for i in order:
+            cur += D.pick((0, 0, 1, 3))
+            oo[i] = cur
+            cur += int(sl[i])
+        return oo, cur + D.pick((0, 2))
+    oo = np.concatenate([[0], np.cumsum(sl)[:-1]]).astype(np.uint32) if len(claims) else np.zeros(0, np.uint32)
+    return oo, int(sl.sum()) + (D.int(1, 5) if form == "spare" else 0)
+
+
+def as_place(pb: Problem, D, form: str, short: bool = False, judge: bool = True) -> PlaceProblem:
+    """pb as a §15 problem, the pending out_off in `form` (drawn through D); short: n_out one slot short.  judge: set
+    `error` from the oracle (otherwise pb's is kept)"""
+    oo, n_out = pending_out_off(D, pb.claims, form)
+    d = {f.name: getattr(pb, f.name) for f in dataclasses.fields(Problem)}
+    x = PlaceProblem(**d, out_off=oo, n_out=max(n_out - 1, 0) if short else n_out, form=form)
+    if judge:
+        try:
+            x.pp_oracle()
+            x.error = False
+        except ValueError:
+            x.error = True
+    x.what = f"{x.what} out_off {form}{' short' if short else ''}"
+    return x
+
+
+def build_place(D, scale: int = 1) -> PlaceProblem:
+    """One §15 problem drawn through D: build()'s inventory, running pods, priorities, pending pods and candidates, and
+    the pending out_off in one of OUT_FORMS.  Now and then n_out is one slot short (a call-level error)."""
+    pb = build(D, scale)
+    return as_place(pb, D, D.pick(OUT_FORMS), D.int(0, 15) == 0)
+
+
+@st.composite
+def place_problems(draw):
+    return build_place(_Hyp(draw))
+
+
+def random_place_problem(seed: int, scale: int = 1) -> PlaceProblem:
+    return build_place(_Rng(np.random.default_rng(seed)), scale)

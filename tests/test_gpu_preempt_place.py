@@ -189,13 +189,15 @@ def test_equals_place_pods_when_nothing_is_evictable(pkg, ctx):
         assert (node[nonempty] == pnode[nonempty]).all() and (ev == NONE).all()
 
 
-def _raw(pkg, ctx, a, sentinel):
-    """dra_preempt_place_batch on sentinel-filled outputs; returns (rc, outputs)"""
+def _raw(pkg, ctx, a, sentinel, slack=0):
+    """dra_preempt_place_batch on sentinel-filled outputs, each `slack` elements longer than the call may write (n_out:
+    a["n_out"], default 1); returns (rc, outputs)"""
     A = pkg.api
     n_pod = len(a["po"]) - 1
+    n_out = a.get("n_out", 1)
     def filled(n, dtype):                                 # every byte = sentinel
-        return np.full(max(n, 1) * np.dtype(dtype).itemsize, sentinel, np.uint8).view(dtype)
-    outs = [filled(4, A.R.OUT_DTYPE), filled(n_pod, np.uint32), filled(n_pod, np.uint8), filled(len(a["rpo"]) - 1, np.uint32)]
+        return np.full((max(n, 1) + slack) * np.dtype(dtype).itemsize, sentinel, np.uint8).view(dtype)
+    outs = [filled(n_out, A.R.OUT_DTYPE), filled(n_pod, np.uint32), filled(n_pod, np.uint8), filled(len(a["rpo"]) - 1, np.uint32)]
     keep = [np.ascontiguousarray(a[k], dtype=d) if a.get(k) is not None else None for k, d in
             (("c", A.R.CLAIM_DTYPE), ("po", np.uint32), ("prio", np.int32), ("rc", A.R.CLAIM_DTYPE), ("rpo", np.uint32),
              ("rpr", np.int32), ("ro", A.R.OUT_DTYPE), ("roo", np.uint32), ("cn", np.uint32), ("co", np.uint32),
@@ -205,7 +207,7 @@ def _raw(pkg, ctx, a, sentinel):
                         None if roo is None else roo.ctypes.data, ro.ctypes.data, len(ro))
     p = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)      # noqa: E731
     rc_ = ctx._lib.dra_preempt_place_batch(ctx._h, p(c), len(c), p(po), p(prio), n_pod, p(cn), p(co), C.byref(run),
-                                           p(oo), p(outs[0]), 1, p(outs[1]), p(outs[2]), p(outs[3]), a["fl"])
+                                           p(oo), p(outs[0]), n_out, p(outs[1]), p(outs[2]), p(outs[3]), a["fl"])
     return rc_, outs
 
 

@@ -78,12 +78,14 @@ class World:
             g[a:b] = c.get_inventory()[a:b]
         return g
 
-    def enqueue(self, claims, pod_off, prio, run, cands=None, flags=0):
+    def enqueue(self, claims, pod_off, prio, run, cands=None, flags=0, slots=None):
+        """slots: (out_off or None, n_out) of the pending claims; None: packed, as _slots lays them out"""
         import torch
         n_pod, n_run = len(pod_off) - 1, run.struct.n_pod
         cn, co = (None, None) if cands is None else cands
-        oo, n_out = _slots(self.pkg, claims)
-        keep = [_dev(claims), _dev(pod_off), _dev(prio), _dev(oo)] + ([None, None] if cn is None else [_dev(cn), _dev(co)])
+        oo, n_out = _slots(self.pkg, claims) if slots is None else slots
+        keep = [_dev(claims), _dev(pod_off), _dev(prio), None if oo is None else _dev(oo)] + \
+            ([None, None] if cn is None else [_dev(cn), _dev(co)])
         sizes = (n_pod * 4, n_pod, n_run * 4)
         outs = [[torch.full((s + PAD,), SENTINEL, dtype=torch.uint8, device="cuda:0") for s in sizes] for _ in self.ctxs]
         torch.cuda.synchronize()                         # (the contexts' streams do not wait for torch's)
@@ -91,7 +93,7 @@ class World:
         for c, o in zip(self.ctxs, outs):
             c.preempt_place_global_device(keep[0].data_ptr(), len(claims), keep[1].data_ptr(), keep[2].data_ptr(), n_pod,
                                           ptr(keep[4]), ptr(keep[5]), 0 if co is None else int(co[-1]), run.struct,
-                                          keep[3].data_ptr(), n_out, o[0].data_ptr(), o[1].data_ptr(), o[2].data_ptr(), flags)
+                                          ptr(keep[3]), n_out, o[0].data_ptr(), o[1].data_ptr(), o[2].data_ptr(), flags)
         return outs, (keep, sizes, n_out)
 
     def read(self, outs, meta):
@@ -102,28 +104,38 @@ class World:
             hs = [t.cpu().numpy() for t in o]
             for h, s, name in zip(hs, sizes, ("pod_node", "pod_status", "evicted_by")):
                 assert (h[s:] == SENTINEL).all(), f"rank {r} wrote past {name}"
-            table = c.gather_read(np.zeros(n_out, dtype=self.pkg.records.OUT_DTYPE)) if n_out else np.zeros(0, self.pkg.records.OUT_DTYPE)
+            # (a call without pending pods writes nothing, the table included)
+            table = c.gather_read(np.zeros(n_out, dtype=self.pkg.records.OUT_DTYPE)) if n_out and sizes[1] else \
+                np.zeros(n_out, self.pkg.records.OUT_DTYPE)
             res.append((table, hs[0][:sizes[0]].view(np.uint32), hs[1][:sizes[1]], hs[2][:sizes[2]].view(np.uint32)))
         return res
 
-    def call(self, claims, pod_off, prio, run, cands=None, flags=0):
-        outs, meta = self.enqueue(claims, pod_off, prio, run, cands, flags)
+    def call(self, claims, pod_off, prio, run, cands=None, flags=0, slots=None):
+        outs, meta = self.enqueue(claims, pod_off, prio, run, cands, flags, slots)
         for c in self.ctxs:
             c.sync()
         return self.read(outs, meta)
 
-    def check(self, claims, pod_off, prio, run_arrays, run, cands=None, flags=0, what=""):
-        """one call against the oracle on the world's state; the ranges, the rest of each copy and the pristine copies"""
+    def check(self, claims, pod_off, prio, run_arrays, run, cands=None, flags=0, what="", slots=None, run_out_off=None):
+        """one call against the oracle on the world's state; the ranges, the rest of each copy and the pristine copies.
+        Nothing may be written past pod_node, pod_status and evicted_by, nor into evicted_by without pending pods.
+        slots as for enqueue; run_out_off: the running pods' out_off (`run` must carry the same)."""
         before = [c.get_inventory() for c in self.ctxs]
         state = self.state()
         cn, co = (None, None) if cands is None else cands
-        oo, n_out = _slots(self.pkg, claims)
+        oo, n_out = _slots(self.pkg, claims) if slots is None else slots
         rc, rpo, rpr, ro = run_arrays
-        ref = PP.preempt_place(state, self.w.node_off, self.w.table, claims, pod_off, prio, rc, rpo, rpr, ro, None, cn, co,
-                               oo, n_out, PP.F_EXHAUSTIVE if flags & self.pkg.api.F_EXHAUSTIVE else 0)
-        got = self.call(claims, pod_off, prio, run, cands, flags)
+        oracle = lambda fill: PP.preempt_place(state, self.w.node_off, self.w.table, claims, pod_off, prio, rc, rpo, rpr,  # noqa: E731
+                                               ro, run_out_off, cn, co, oo, n_out,
+                                               PP.F_EXHAUSTIVE if flags & self.pkg.api.F_EXHAUSTIVE else 0, fill)
+        ref = oracle(SENTINEL)                           # what the call must not write keeps the sentinel
+        # the table's slots that no claim owns hold whatever the gathered table held: only the written bytes count
+        written = ref[0].view(np.uint8) == oracle(SENTINEL ^ 0xFF)[0].view(np.uint8) if slots is not None else None
+        got = self.call(claims, pod_off, prio, run, cands, flags, (oo, n_out))
         for r, g in enumerate(got):
             for name, x, y in zip(("out", "pod_node", "pod_status", "evicted_by"), g, ref[:4]):
+                if name == "out" and written is not None:
+                    x, y = x.view(np.uint8)[written], y.view(np.uint8)[written]
                 if x.tobytes() != y.tobytes():
                     bad = np.flatnonzero(x.view(np.uint8) != y.view(np.uint8))[:5]
                     pytest.fail(f"{what} rank {r}: {name} differs at bytes {bad}")

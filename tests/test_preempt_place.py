@@ -152,6 +152,65 @@ def test_search_limit():
     assert list(st) == [PP.NO] and (out["status"] == R.ST_POD).all()
 
 
+def _two_gpu_node(running=True):
+    """One node of two non-MIG GPUs; with `running`, GPU 0 held by a one-GPU running pod of priority 1.  Pending: one
+    pod of a single GPU claim of count 2, priority 10."""
+    g, off = R.make_inventory([2], mig=False)
+    rc = np.zeros(1 if running else 0, R.CLAIM_DTYPE)
+    rc["kind"], rc["count"], rc["node"] = R.KIND_GPU, 1, 0
+    ro = np.zeros(len(rc), R.OUT_DTYPE)
+    ro["gpu"], ro["profile"], ro["status"] = 0, R.PROFILE_GPU, R.ST_OK
+    if running:
+        g["flags"][0] |= R.GPU_FULL_ALLOCATED
+    c = np.zeros(1, R.CLAIM_DTYPE)
+    c["kind"], c["count"] = R.KIND_GPU, 2
+    return g, off, R.default_table(), c, np.array([0, 1], np.uint32), np.array([10], np.int32), rc, \
+        np.arange(len(rc) + 1, dtype=np.uint32), np.ones(len(rc), np.int32), ro
+
+
+@pytest.mark.parametrize("cands", [None, [[0]], [[5, 0, 0]]])
+@pytest.mark.parametrize("flags", [0, PP.F_EXHAUSTIVE])
+def test_slot_mode_decides_validity(cands, flags):
+    """A GPU claim of count 2 is valid only with out_off (§1).  With it, the pod evicts the running pod and takes both
+    GPUs.  Without it the pod is INVALID: judged nowhere, nothing evicted, the inventory unchanged, and podNode is
+    §13's (nowhere) also on an empty node."""
+    g, off, t, c, po, prio, rc, rpo, rpr, ro = _two_gpu_node()
+    out, node, st, ev, after = run_both(g, off, t, c, po, prio, rc, rpo, rpr, ro, cands=cands, flags=flags,
+                                        out_off=np.zeros(1, np.uint32))
+    assert list(node) == [0] and list(st) == [PP.EVICT] and list(ev) == [0]
+    assert _outs(out) == [(0, 0, 0, R.PROFILE_GPU, R.ST_OK), (1, 0, 0, R.PROFILE_GPU, R.ST_OK)]
+    assert list(after["flags"] & R.GPU_FULL_ALLOCATED) == [R.GPU_FULL_ALLOCATED] * 2
+    out, node, st, ev, after = run_both(g, off, t, c, po, prio, rc, rpo, rpr, ro, cands=cands, flags=flags)
+    assert list(node) == [NONE] and list(st) == [PP.INVALID] and list(ev) == [NONE]
+    assert _outs(out) == [(NONE, 0, 0, R.PROFILE_GPU, R.ST_INVALID)] and after.tobytes() == g.tobytes()
+    # nothing to evict: without out_off, place pods' answer
+    g, off, t, c, po, prio, rc, rpo, rpr, ro = _two_gpu_node(running=False)
+    cn, co = (None, None) if cands is None else _flat(cands)
+    for oo in (None, np.zeros(1, np.uint32)):
+        out, node, st, ev, after = run_both(g, off, t, c, po, prio, rc, rpo, rpr, ro, cands=cands, flags=flags, out_off=oo)
+        pout, pnode, pafter = PL.place_pods(g, off, t, c, po, cn, co, oo, len(out), flags)
+        assert out.tobytes() == pout.tobytes() and list(node) == list(pnode) and after.tobytes() == pafter.tobytes()
+        assert list(st) == ([PP.FITS] if oo is not None else [PP.INVALID])
+
+
+@pytest.mark.parametrize("cands", [None, [[0]], [[5, 0, 0]]])
+def test_slot_mode_decides_validity_on_a_sharded_world(cands):
+    """The same under the model of the sharded exchange: every rank, whatever the partition, gives the single call's
+    answer (the sharded form's prep is the single form's)."""
+    from test_preempt_place_shard_model import _check_world
+    g, off, t, c, po, prio, rc, rpo, rpr, ro = _two_gpu_node()
+    stale, _ = R.make_inventory([2], mig=False)
+    cn = None if cands is None else _flat(cands)
+    for flags in (0, PP.F_EXHAUSTIVE):
+        rng = np.random.default_rng(flags)
+        for oo in (None, np.zeros(1, np.uint32)):
+            ref = _check_world(rng, g, stale, off, t, c, po, prio, (rc, rpo, rpr, ro), cn, flags, out_off=oo)
+            if oo is None:
+                assert list(ref[2]) == [PP.INVALID] and list(ref[3]) == [NONE] and ref[4].tobytes() == g.tobytes()
+            else:
+                assert list(ref[1]) == [0] and list(ref[2]) == [PP.EVICT] and list(ref[3]) == [0]
+
+
 def test_call_errors():
     g, off = R.make_inventory([1, 1], mig=True)
     t = R.default_table()
@@ -304,15 +363,50 @@ def _apply(g, claims, out, have_off, oo, add):
     return g
 
 
+def check_matched(gpus, node_off, claims, pod_off, out, node, st, ev, oo):
+    """§15's answer when the running records match the inventory: every non-empty pod placed (FITS or EVICT) has every
+    slot OK on podNode's GPUs, and every other pod has none OK; only EVICT pods evict.  oo None: no out_off."""
+    node_of = np.searchsorted(node_off, np.arange(len(gpus)), side="right") - 1
+    assert all(st[p] == PP.EVICT for p in set(int(p) for p in ev[ev != NONE]))
+    placed = claims.copy()
+    placed["node"] = 0
+    sl = R.claim_slots(placed, 1, oo is not None)
+    for p in range(len(pod_off) - 1):
+        recs = [out[(int(oo[i]) if oo is not None else i) + k] for i in range(int(pod_off[p]), int(pod_off[p + 1]))
+                for k in range(int(sl[i]))]
+        if st[p] in (PP.FITS, PP.EVICT):
+            assert node[p] < len(node_off) - 1, p
+            assert all(o["status"] == R.ST_OK and node_of[o["gpu"]] == node[p] for o in recs), p
+        else:
+            assert node[p] == NONE and not any(o["status"] == R.ST_OK for o in recs), p
+
+
 @pytest.mark.parametrize("seed", range(4))
 def test_properties(seed):
+    _check_properties(seed, have_off=True)
+
+
+@pytest.mark.parametrize("seed", range(4))
+def test_properties_without_out_off(seed):
+    """the same with no out_off: a pod with a multi-GPU claim is INVALID, and nothing is evicted for it"""
+    _check_properties(seed, have_off=False)
+
+
+def _check_properties(seed, have_off):
     w, oo, n_out = _world(seed)
+    if not have_off:
+        oo, n_out = None, len(w.claims)
     n_node = len(w.node_off) - 1
     node_of = np.searchsorted(w.node_off, np.arange(len(w.gpus)), side="right") - 1
     for flags in (0, PP.F_EXHAUSTIVE):
         out, node, st, ev, after = PP.preempt_place(w.gpus, w.node_off, w.table, w.claims, w.pod_off, w.prio, w.run_claims,
                                                     w.run_pod_off, w.run_prio, w.run_out, None, None, None, oo, n_out, flags)
         assert (st == PP.EVICT).any()
+        check_matched(w.gpus, w.node_off, w.claims, w.pod_off, out, node, st, ev, oo)
+        if not have_off:                                 # a pod with a multi-GPU claim is INVALID without out_off
+            multi = [(w.claims["kind"][w.pod_off[p]:w.pod_off[p + 1]] == R.KIND_GPU).any() and
+                     (w.claims["count"][w.pod_off[p]:w.pod_off[p + 1]] > 1).any() for p in range(len(w.prio))]
+            assert any(multi) and all(st[p] == PP.INVALID for p in np.flatnonzero(multi))
         # every victim is on its evictor's node, at a lower priority
         for r in np.flatnonzero(ev != NONE):
             p = ev[r]
@@ -324,13 +418,13 @@ def test_properties(seed):
         for r in np.flatnonzero(ev != NONE):
             vk[w.run_pod_off[r]: w.run_pod_off[r + 1]] = True
         g = _apply(w.gpus, w.run_claims[vk], w.run_out[vk], False, None, False)
-        g = _apply(g, w.claims, out, True, oo, True)
+        g = _apply(g, w.claims, out, have_off, oo, True)
         assert g.tobytes() == after.tobytes()
         # no two MIG placements overlap: the placed pods' and the running pods that stay
         used = {}
         keep = ~vk
         recs = [(o, c) for c, o in zip(w.run_claims[keep], w.run_out[keep])]
-        recs += [(out[oo[i]], w.claims[i]) for i in range(len(w.claims)) if w.claims[i]["kind"] == R.KIND_MIG]
+        recs += [(out[oo[i] if have_off else i], w.claims[i]) for i in range(len(w.claims)) if w.claims[i]["kind"] == R.KIND_MIG]
         for o, c in recs:
             if c["kind"] != R.KIND_MIG or o["status"] != R.ST_OK:
                 continue
@@ -338,3 +432,25 @@ def test_properties(seed):
             assert used.get(int(o["gpu"]), 0) & m == 0
             used[int(o["gpu"])] = used.get(int(o["gpu"]), 0) | m
         assert all(node[p] < n_node for p in np.flatnonzero(st <= PP.EVICT))
+
+
+# ---- random §15 problems (tests/preempt_problems.py) ----------------------------------------------------------------
+def test_random_place_problems():
+    """Every out_off form, mismatched records and run_out_off included: the call fails exactly when the builder says so,
+    and on matched records the answer has check_matched's properties and the inventory is the one the OutRecs and the
+    victims' releases make."""
+    from hypothesis import HealthCheck, given, settings
+    from preempt_problems import place_problems
+
+    @settings(max_examples=150, deadline=None, suppress_health_check=list(HealthCheck), derandomize=True, database=None)
+    @given(place_problems())
+    def run(pb):
+        if pb.error:
+            with pytest.raises(ValueError):
+                pb.pp_oracle()
+            return
+        out, node, st, ev, after = pb.pp_oracle()
+        assert len(out) == pb.n_out and len(node) == len(pb.prio) and len(ev) == len(pb.run_prio)
+        if pb.matched:
+            check_matched(pb.gpus, pb.node_off, pb.claims, pb.pod_off, out, node, st, ev, pb.out_off)
+    run()

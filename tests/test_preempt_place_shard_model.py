@@ -67,11 +67,11 @@ def run_protocol(rng, state, stale, off, bounds, call):
     return done, rng_of
 
 
-def _check_world(rng, w_gpus, stale, off, table, claims, pod_off, prio, run, cands, flags, n_parts=4):
+def _check_world(rng, w_gpus, stale, off, table, claims, pod_off, prio, run, cands, flags, n_parts=4, out_off=None):
     rc, rpo, rpr, ro = run
     cn, co = (None, None) if cands is None else cands
-    ref = PP.preempt_place(w_gpus, off, table, claims, pod_off, prio, rc, rpo, rpr, ro, None, cn, co, None, None, flags)
-    call = lambda g: PP.preempt_place(g, off, table, claims, pod_off, prio, rc, rpo, rpr, ro, None, cn, co, None, None, flags)  # noqa: E731
+    ref = PP.preempt_place(w_gpus, off, table, claims, pod_off, prio, rc, rpo, rpr, ro, None, cn, co, out_off, None, flags)
+    call = lambda g: PP.preempt_place(g, off, table, claims, pod_off, prio, rc, rpo, rpr, ro, None, cn, co, out_off, None, flags)  # noqa: E731
     n_node = len(off) - 1
     for _ in range(n_parts):
         world = int(rng.integers(1, 6))
