@@ -639,6 +639,9 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
     return DRA_OK;
 }
 
+// Lanes per (pod, node) pair for k_unsuitable and the preemption pair kernels: one per GPU of the widest node
+uint32_t pair_width(const dra_ctx* ctx) { return ctx->max_width <= 8 ? 8u : (ctx->max_width <= 16 ? 16u : 32u); }
+
 template <bool WIN>
 void launch_unsuitable_w(dra_ctx* ctx, const UnsArgs& a, uint32_t W, uint32_t grid) {
     if (a.exhaustive) {
@@ -655,7 +658,7 @@ void launch_unsuitable_w(dra_ctx* ctx, const UnsArgs& a, uint32_t W, uint32_t gr
 // k_unsuitable over n_walk pairs (win: the sharded call's node window, n_walk = a.n_walk; else n_walk = a.n_pair); lanes per
 // pair from the widest node: 8 lanes = 4 pairs per warp.  Enqueues only.
 int launch_unsuitable(dra_ctx* ctx, UnsArgs& a, bool win) {
-    const uint32_t W = ctx->max_width <= 8 ? 8u : (ctx->max_width <= 16 ? 16u : 32u);
+    const uint32_t W = pair_width(ctx);
     const uint32_t per_cta = 8 * (32 / W);
     const uint32_t n_walk = win ? a.n_walk : a.n_pair;
     const uint32_t grid = std::max(1u, std::min((n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
@@ -777,6 +780,121 @@ int pp_buffers(dra_ctx* ctx, uint32_t n_pod, uint32_t n_pair, uint32_t rn_pod) {
         ctx->cap_pp_nodes = need + need / 2 + 64;
     }
     return DRA_OK;
+}
+
+size_t al16(size_t b) { return (b + 15) & ~(size_t)15; }
+
+// Pinned staging bytes of the running pods: claims | pod_off | prio | out_off | out, each rounded up to 16 bytes
+size_t running_room(const dra_running_pods& R) {
+    return al16((size_t)R.n_claim * 16) + al16(((size_t)R.n_pod + 1) * 4) + al16((size_t)R.n_pod * 4) +
+           (R.out_off ? al16((size_t)R.n_claim * 4) : 0) + al16((size_t)R.n_out * 8);
+}
+
+// The caller's running pods R into the d_pre_r* buffers (grown as needed) through the pinned staging at h
+// (running_room(R) bytes); dev = R with those device pointers.  Enqueues only.
+int upload_running(dra_ctx* ctx, const dra_running_pods& R, uint8_t* h, dra_running_pods& dev) {
+    int rc;
+    if ((size_t)R.n_claim + 8 > ctx->cap_pre_rclaims) {
+        const size_t need = (size_t)R.n_claim + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rclaims, need)) || (rc = grow_pre(ctx, ctx->d_pre_routoff, need))) return rc;
+        ctx->cap_pre_rclaims = need + need / 2 + 64;
+    }
+    if ((size_t)R.n_pod + 8 > ctx->cap_pre_rpods) {
+        const size_t need = (size_t)R.n_pod + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rpodoff, need)) || (rc = grow_pre(ctx, ctx->d_pre_rprio, need)) ||
+            (rc = grow_pre(ctx, ctx->d_pre_rrec, need)) || (rc = grow_pre(ctx, ctx->d_pre_vlist, need))) return rc;
+        ctx->cap_pre_rpods = need + need / 2 + 64;
+    }
+    if ((size_t)R.n_out + 8 > ctx->cap_pre_rout) {
+        const size_t need = (size_t)R.n_out + 8;
+        if ((rc = grow_pre(ctx, ctx->d_pre_rout, need))) return rc;
+        ctx->cap_pre_rout = need + need / 2 + 64;
+    }
+    auto put = [&](const void* src, size_t bytes) { uint8_t* d = h; if (bytes) memcpy(d, src, bytes); h += al16(bytes); return d; };
+    uint8_t* h_rc = put(R.claims, (size_t)R.n_claim * 16);
+    uint8_t* h_rpo = put(R.pod_off, ((size_t)R.n_pod + 1) * 4);
+    uint8_t* h_rpr = put(R.prio, (size_t)R.n_pod * 4);
+    uint8_t* h_roo = R.out_off ? put(R.out_off, (size_t)R.n_claim * 4) : nullptr;
+    uint8_t* h_ro = put(R.out, (size_t)R.n_out * 8);
+    cudaStream_t st = ctx->stream;
+    if (R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_rclaims, h_rc, (size_t)R.n_claim * 16, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pre_rpodoff, h_rpo, ((size_t)R.n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (R.n_pod) CU(cudaMemcpyAsync(ctx->d_pre_rprio, h_rpr, (size_t)R.n_pod * 4, cudaMemcpyHostToDevice, st));
+    if (h_roo && R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_routoff, h_roo, (size_t)R.n_claim * 4, cudaMemcpyHostToDevice, st));
+    if (R.n_out) CU(cudaMemcpyAsync(ctx->d_pre_rout, h_ro, (size_t)R.n_out * 8, cudaMemcpyHostToDevice, st));
+    dev = R;
+    dev.claims = (const dra_claim_rec*)ctx->d_pre_rclaims; dev.pod_off = ctx->d_pre_rpodoff;
+    dev.prio = (const int32_t*)ctx->d_pre_rprio; dev.out_off = R.out_off ? ctx->d_pre_routoff : nullptr;
+    dev.out = (const dra_out_rec*)ctx->d_pre_rout;
+    return DRA_OK;
+}
+
+// The PreArgs fields every preemption call sets: the pending pods (cand_nodes and cand_off nullptr in the dense form), the
+// running pods R (device pointers), the running lists' buffers, the inventory copy inv that is judged, psum, the pod
+// outputs and the fault gate
+PreArgs pre_args(dra_ctx* ctx, const uint4* claims, const uint32_t* pod_off, const int32_t* prio, uint32_t n_pod,
+                 const uint32_t* cand_nodes, const uint32_t* cand_off, uint32_t n_pair, const dra_running_pods& R,
+                 const uint4* inv, uint32_t flags) {
+    PreArgs a; memset(&a, 0, sizeof a);
+    a.claims = claims; a.pod_off = pod_off; a.prio = prio; a.n_pod = n_pod;
+    a.cand_nodes = cand_nodes; a.cand_off = cand_off; a.n_pair = n_pair;
+    a.rclaims = (const uint4*)R.claims; a.rn_claim = R.n_claim; a.rpod_off = R.pod_off; a.rprio = R.prio; a.rn_pod = R.n_pod;
+    a.rout_off = R.out_off; a.rout = (const uint2*)R.out; a.rn_out = R.n_out;
+    a.rrec = ctx->d_pre_rrec; a.rsorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.vlist = ctx->d_pre_vlist;
+    a.inv = inv; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.n_gpu = ctx->n_gpu; a.tbl = ctx->d_tbl;
+    a.sel = sel_of(ctx); a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
+    a.psum = ctx->d_pre_psum; a.psum64 = ctx->d_pre_psum64;
+    a.pod_node = ctx->d_pre_node; a.pod_status = ctx->d_pre_pst;
+    a.gate = ctx->d_err + ERR_BAD_OFFSETS; a.err = err_of(ctx);
+    return a;
+}
+
+// The running lists: k_pre_running, its records bucketed by node with the counting sort (without running pods the
+// offsets are zeroed instead) and k_pre_vsort.  walk (§15): the visit lists reuse the sort's buffers, so the offsets are
+// kept in d_pp_runoff, which becomes a.list_off; and without running pods there is no list to sort.  Enqueues only.
+int launch_running_lists(dra_ctx* ctx, PreArgs& a, Prof& prof, bool walk) {
+    cudaStream_t st = ctx->stream;
+    k_pre_running<<<std::max(1u, (a.rn_pod + 255) / 256), 256, 0, st>>>(a);
+    ctx->launches += 1;
+    if (!a.rn_pod) CU(cudaMemsetAsync(walk ? ctx->d_pp_runoff : ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, st));
+    else if (int rc = launch_sort(ctx, a.rrec, a.rn_pod, nullptr, nullptr, 0, 0, prof, a.inv, false, ctx->n_node, ctx->d_node_off))
+        return rc;
+    if (ctx->n_node && (a.rn_pod || !walk)) {
+        k_pre_vsort<<<std::min(ctx->n_node, (uint32_t)ctx->n_sm * 8u), 256, 0, st>>>(a);
+        ctx->launches += 1;
+    }
+    if (walk) {
+        if (a.rn_pod) CU(cudaMemcpyAsync(ctx->d_pp_runoff, ctx->d_claim_off, ((size_t)ctx->n_node + 1) * 4, cudaMemcpyDeviceToDevice, st));
+        a.list_off = ctx->d_pp_runoff;
+    }
+    return DRA_OK;
+}
+
+// k_pods_preempt over s's pairs (none: no launch), pair_width lanes per pair, 8 warps per CTA.  Enqueues only.
+int launch_preempt_pairs(dra_ctx* ctx, PreArgs a, const PreShard& s) {
+    if (!s.n_walk) return DRA_OK;
+    cudaStream_t st = ctx->stream;
+    if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, st)); }
+    a.work = ctx->d_ticket + 13;
+    CU(cudaMemsetAsync(a.work, 0, 4, st));
+    const uint32_t W = pair_width(ctx), per_cta = 8 * (32 / W);
+    const uint32_t grid = std::max(1u, std::min((s.n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
+    if (W == 8) k_pods_preempt<8, 8><<<grid, 256, 0, st>>>(a, s);
+    else if (W == 16) k_pods_preempt<8, 16><<<grid, 256, 0, st>>>(a, s);
+    else k_pods_preempt<8, 32><<<grid, 256, 0, st>>>(a, s);
+    ctx->launches += 1;
+    return DRA_OK;
+}
+
+// k_pods_preempt_victims for a's pods: pod p's chosen pair at choice[p * cstride], its row at rows + p * rstride.  Enqueues only.
+void launch_preempt_victims(dra_ctx* ctx, const PreArgs& a, const uint32_t* choice, uint32_t cstride, uint32_t* rows, uint32_t rstride) {
+    const uint32_t W = pair_width(ctx), per_cta = 8 * (32 / W);
+    const uint32_t grid = std::max(1u, std::min((a.n_pod + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
+    cudaStream_t st = ctx->stream;
+    if (W == 8) k_pods_preempt_victims<8, 8><<<grid, 256, 0, st>>>(a, choice, cstride, rows, rstride);
+    else if (W == 16) k_pods_preempt_victims<8, 16><<<grid, 256, 0, st>>>(a, choice, cstride, rows, rstride);
+    else k_pods_preempt_victims<8, 32><<<grid, 256, 0, st>>>(a, choice, cstride, rows, rstride);
+    ctx->launches += 1;
 }
 
 }  // namespace
@@ -1608,35 +1726,17 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
             (rc = grow_pre(ctx, ctx->d_pre_pairst, need)) || (rc = grow_pre(ctx, ctx->d_pre_pairvic, need))) return rc;
         ctx->cap_pre_pairs = need + need / 2 + 64;
     }
-    if ((size_t)R.n_claim + 8 > ctx->cap_pre_rclaims) {
-        const size_t need = (size_t)R.n_claim + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rclaims, need)) || (rc = grow_pre(ctx, ctx->d_pre_routoff, need))) return rc;
-        ctx->cap_pre_rclaims = need + need / 2 + 64;
-    }
-    if ((size_t)R.n_pod + 8 > ctx->cap_pre_rpods) {
-        const size_t need = (size_t)R.n_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rpodoff, need)) || (rc = grow_pre(ctx, ctx->d_pre_rprio, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_rrec, need)) || (rc = grow_pre(ctx, ctx->d_pre_vlist, need))) return rc;
-        ctx->cap_pre_rpods = need + need / 2 + 64;
-    }
-    if ((size_t)R.n_out + 8 > ctx->cap_pre_rout) {
-        const size_t need = (size_t)R.n_out + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rout, need))) return rc;
-        ctx->cap_pre_rout = need + need / 2 + 64;
-    }
     const size_t vb = (size_t)n_pod * max_victims * 4;
     if (vb / 4 + 8 > ctx->cap_pre_vic) {
         const size_t need = vb / 4 + 8;
         if ((rc = grow_pre(ctx, ctx->d_pre_vic, need))) return rc;
         ctx->cap_pre_vic = need + need / 2 + 64;
     }
-    // staging: claims | pod_off | prio | cand_off | cand_nodes | pair -> pod | running claims | pod_off | prio | out_off | out
-    auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    // staging: claims | pod_off | prio | cand_off | cand_nodes | pair -> pod | the running pods
+    auto al = al16;
     const size_t cb = al((size_t)n_claim * 16), pb = al(((size_t)n_pod + 1) * 4), prb = al((size_t)n_pod * 4);
     const size_t kb = dense ? 0 : al(((size_t)n_pod + 1) * 4), nb = dense ? 0 : al((size_t)n_pair * 4);
-    const size_t rcb = al((size_t)R.n_claim * 16), rpb = al(((size_t)R.n_pod + 1) * 4), rprb = al((size_t)R.n_pod * 4);
-    const size_t rob = R.out_off ? al((size_t)R.n_claim * 4) : 0, routb = al((size_t)R.n_out * 8);
-    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + prb + kb + 2 * nb + rcb + rpb + rprb + rob + routb + 16))) return rc;
+    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + prb + kb + 2 * nb + running_room(R) + 16))) return rc;
     uint8_t* h = ctx->h_in;
     auto put = [&](const void* src, size_t bytes, size_t room) { uint8_t* d = h; if (bytes) memcpy(d, src, bytes); h += room; return d; };
     uint8_t* h_c = put(claims, (size_t)n_claim * 16, cb);
@@ -1647,11 +1747,6 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
     uint8_t* h_pp = dense ? nullptr : put(nullptr, 0, nb);
     for (uint32_t q = 0; !dense && q < n_pod; ++q)
         for (uint32_t k = cand_off[q]; k < cand_off[q + 1]; ++k) ((uint32_t*)h_pp)[k] = q;
-    uint8_t* h_rc = put(R.claims, (size_t)R.n_claim * 16, rcb);
-    uint8_t* h_rpo = put(R.pod_off, ((size_t)R.n_pod + 1) * 4, rpb);
-    uint8_t* h_rpr = put(R.prio, (size_t)R.n_pod * 4, rprb);
-    uint8_t* h_roo = R.out_off ? put(R.out_off, (size_t)R.n_claim * 4, rob) : nullptr;
-    uint8_t* h_ro = put(R.out, (size_t)R.n_out * 8, routb);
     cudaStream_t st = ctx->stream;
     if (n_claim) CU(cudaMemcpyAsync(ctx->d_claims, h_c, (size_t)n_claim * 16, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(ctx->d_pod_off, h_po, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
@@ -1663,61 +1758,23 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
             CU(cudaMemcpyAsync(ctx->d_pair_pod, h_pp, (size_t)n_pair * 4, cudaMemcpyHostToDevice, st));
         }
     }
-    if (R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_rclaims, h_rc, (size_t)R.n_claim * 16, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pre_rpodoff, h_rpo, ((size_t)R.n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (R.n_pod) CU(cudaMemcpyAsync(ctx->d_pre_rprio, h_rpr, (size_t)R.n_pod * 4, cudaMemcpyHostToDevice, st));
-    if (h_roo && R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_routoff, h_roo, (size_t)R.n_claim * 4, cudaMemcpyHostToDevice, st));
-    if (R.n_out) CU(cudaMemcpyAsync(ctx->d_pre_rout, h_ro, (size_t)R.n_out * 8, cudaMemcpyHostToDevice, st));
+    dra_running_pods Rd;
+    if ((rc = upload_running(ctx, R, h, Rd))) return rc;
 
-    PreArgs a; memset(&a, 0, sizeof a);
-    a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.prio = (const int32_t*)ctx->d_pre_prio; a.n_pod = n_pod;
-    a.cand_nodes = dense ? nullptr : ctx->d_cand_nodes; a.cand_off = dense ? nullptr : ctx->d_cand_off;
-    a.pair_pod = dense ? nullptr : ctx->d_pair_pod; a.n_pair = n_pair;
-    a.rclaims = ctx->d_pre_rclaims; a.rn_claim = R.n_claim; a.rpod_off = ctx->d_pre_rpodoff; a.rprio = (const int32_t*)ctx->d_pre_rprio;
-    a.rn_pod = R.n_pod; a.rout_off = R.out_off ? ctx->d_pre_routoff : nullptr; a.rout = ctx->d_pre_rout; a.rn_out = R.n_out;
-    a.rrec = ctx->d_pre_rrec; a.rsorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.vlist = ctx->d_pre_vlist;
-    a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.n_gpu = ctx->n_gpu; a.tbl = ctx->d_tbl;
-    a.sel = sel_of(ctx); a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
-    a.psum = ctx->d_pre_psum; a.psum64 = ctx->d_pre_psum64;
+    PreArgs a = pre_args(ctx, ctx->d_claims, ctx->d_pod_off, (const int32_t*)ctx->d_pre_prio, n_pod, dense ? nullptr : ctx->d_cand_nodes,
+                         dense ? nullptr : ctx->d_cand_off, n_pair, Rd, ctx->d_inv_live, flags);
+    a.pair_pod = dense ? nullptr : ctx->d_pair_pod;
     a.pair_status = pair_status ? ctx->d_pre_pairst : nullptr; a.pair_victims = pair_victims ? ctx->d_pre_pairvic : nullptr;
-    a.pod_node = ctx->d_pre_node; a.pod_status = ctx->d_pre_pst; a.n_victims = ctx->d_pre_nvic; a.choice = ctx->d_pre_choice;
-    a.victims = ctx->d_pre_vic; a.max_victims = max_victims;
-    a.gate = ctx->d_err + ERR_BAD_OFFSETS; a.err = err_of(ctx);
-    if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, st)); }
-    a.work = ctx->d_ticket + 13;
-    CU(cudaMemsetAsync(a.work, 0, 4, st));
+    a.n_victims = ctx->d_pre_nvic; a.choice = ctx->d_pre_choice; a.max_victims = max_victims;
     Prof prof(ctx);
-    k_pre_running<<<std::max(1u, (R.n_pod + 255) / 256), 256, 0, st>>>(a);
-    ctx->launches += 1;
-    if (R.n_pod) {
-        if ((rc = launch_sort(ctx, ctx->d_pre_rrec, R.n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, ctx->n_node, ctx->d_node_off)))
-            return rc;
-    } else {
-        CU(cudaMemsetAsync(ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, st));
-    }
-    const uint32_t W = ctx->max_width <= 8 ? 8u : (ctx->max_width <= 16 ? 16u : 32u);
-    if (ctx->n_node) {
-        k_pre_vsort<<<std::min(ctx->n_node, (uint32_t)ctx->n_sm * 8u), 256, 0, st>>>(a);
-        ctx->launches += 1;
-    }
-    if (n_pair) {
-        const uint32_t per_cta = 8 * (32 / W);
-        const uint32_t grid = std::max(1u, std::min((n_pair + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
-        if (W == 8) k_pods_preempt<8, 8><<<grid, 256, 0, st>>>(a);
-        else if (W == 16) k_pods_preempt<8, 16><<<grid, 256, 0, st>>>(a);
-        else k_pods_preempt<8, 32><<<grid, 256, 0, st>>>(a);
-        ctx->launches += 1;
-    }
+    if ((rc = launch_running_lists(ctx, a, prof, false))) return rc;
+    const PreShard whole{0u, ctx->n_node, n_pair, 0u, nullptr, nullptr};
+    if ((rc = launch_preempt_pairs(ctx, a, whole))) return rc;
     k_pre_choose<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a);
     ctx->launches += 1;
     if (max_victims) {
         CU(cudaMemsetAsync(ctx->d_pre_vic, 0xFF, vb, st));
-        const uint32_t per_cta = 8 * (32 / W);
-        const uint32_t grid = std::max(1u, std::min((n_pod + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
-        if (W == 8) k_pods_preempt_victims<8, 8><<<grid, 256, 0, st>>>(a);
-        else if (W == 16) k_pods_preempt_victims<8, 16><<<grid, 256, 0, st>>>(a);
-        else k_pods_preempt_victims<8, 32><<<grid, 256, 0, st>>>(a);
-        ctx->launches += 1;
+        launch_preempt_victims(ctx, a, ctx->d_pre_choice, 1u, ctx->d_pre_vic, max_victims);
     }
     prof.mark();
     // outputs: pair_status | pair_victims | pod_node | pod_status | n_victims | victims
@@ -1806,23 +1863,11 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
         ctx->cap_pairs = cap;
     }
     if ((rc = pp_buffers(ctx, n_pod, n_pair, R.n_pod))) return rc;
-    if ((size_t)R.n_claim + 8 > ctx->cap_pre_rclaims) {
-        const size_t need = (size_t)R.n_claim + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rclaims, need)) || (rc = grow_pre(ctx, ctx->d_pre_routoff, need))) return rc;
-        ctx->cap_pre_rclaims = need + need / 2 + 64;
-    }
-    if ((size_t)R.n_out + 8 > ctx->cap_pre_rout) {
-        const size_t need = (size_t)R.n_out + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rout, need))) return rc;
-        ctx->cap_pre_rout = need + need / 2 + 64;
-    }
-    // staging: claims | pod_off | out_off | prio | cand_off | cand_nodes | running claims | pod_off | prio | out_off | out
-    auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    // staging: claims | pod_off | out_off | prio | cand_off | cand_nodes | the running pods
+    auto al = al16;
     const size_t cb = al((size_t)n_claim * 16), pb = al(((size_t)n_pod + 1) * 4), ob = out_off ? al((size_t)n_claim * 4) : 0;
     const size_t prb = al((size_t)n_pod * 4), kb = dense ? 0 : al(((size_t)n_pod + 1) * 4), nb = dense ? 0 : al((size_t)n_pair * 4);
-    const size_t rcb = al((size_t)R.n_claim * 16), rpb = al(((size_t)R.n_pod + 1) * 4), rprb = al((size_t)R.n_pod * 4);
-    const size_t rob = R.out_off ? al((size_t)R.n_claim * 4) : 0, routb = al((size_t)R.n_out * 8);
-    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + ob + prb + kb + nb + rcb + rpb + rprb + rob + routb + 16))) return rc;
+    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + ob + prb + kb + nb + running_room(R) + 16))) return rc;
     uint8_t* h = ctx->h_in;
     auto put = [&](const void* src, size_t bytes, size_t room) { uint8_t* d = h; if (bytes) memcpy(d, src, bytes); h += room; return d; };
     uint8_t* h_c = put(claims, (size_t)n_claim * 16, cb);
@@ -1831,11 +1876,6 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     uint8_t* h_pr = put(prio, (size_t)n_pod * 4, prb);
     uint8_t* h_co = dense ? nullptr : put(cand_off, ((size_t)n_pod + 1) * 4, kb);
     uint8_t* h_cn = dense ? nullptr : put(cand_nodes, (size_t)n_pair * 4, nb);
-    uint8_t* h_rc = put(R.claims, (size_t)R.n_claim * 16, rcb);
-    uint8_t* h_rpo = put(R.pod_off, ((size_t)R.n_pod + 1) * 4, rpb);
-    uint8_t* h_rpr = put(R.prio, (size_t)R.n_pod * 4, rprb);
-    uint8_t* h_roo = R.out_off ? put(R.out_off, (size_t)R.n_claim * 4, rob) : nullptr;
-    uint8_t* h_ro = put(R.out, (size_t)R.n_out * 8, routb);
     cudaStream_t st = ctx->stream;
     if (n_claim) CU(cudaMemcpyAsync(ctx->d_claims, h_c, (size_t)n_claim * 16, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(ctx->d_pod_off, h_po, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
@@ -1845,44 +1885,18 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
         CU(cudaMemcpyAsync(ctx->d_cand_off, h_co, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
         if (n_pair) CU(cudaMemcpyAsync(ctx->d_cand_nodes, h_cn, (size_t)n_pair * 4, cudaMemcpyHostToDevice, st));
     }
-    if (R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_rclaims, h_rc, (size_t)R.n_claim * 16, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pre_rpodoff, h_rpo, ((size_t)R.n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (R.n_pod) CU(cudaMemcpyAsync(ctx->d_pre_rprio, h_rpr, (size_t)R.n_pod * 4, cudaMemcpyHostToDevice, st));
-    if (h_roo && R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_routoff, h_roo, (size_t)R.n_claim * 4, cudaMemcpyHostToDevice, st));
-    if (R.n_out) CU(cudaMemcpyAsync(ctx->d_pre_rout, h_ro, (size_t)R.n_out * 8, cudaMemcpyHostToDevice, st));
+    dra_running_pods Rd;
+    if ((rc = upload_running(ctx, R, h, Rd))) return rc;
     const size_t rb = (size_t)n_out * 8;
     if (rb) CU(cudaMemsetAsync(ctx->d_out, 0, rb, st));
     CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)ctx->n_node + 1) * 4, st));
     CU(cudaMemsetAsync(ctx->d_pp_judged, 0, ((size_t)ctx->n_node + 1) * 4, st));
     if (R.n_pod) CU(cudaMemsetAsync(ctx->d_pp_evicted, 0xFF, (size_t)R.n_pod * 4, st));
 
-    PreArgs a; memset(&a, 0, sizeof a);
-    a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.prio = (const int32_t*)ctx->d_pre_prio; a.n_pod = n_pod;
-    a.cand_nodes = dense ? nullptr : ctx->d_cand_nodes; a.cand_off = dense ? nullptr : ctx->d_cand_off; a.n_pair = n_pair;
-    a.rclaims = ctx->d_pre_rclaims; a.rn_claim = R.n_claim; a.rpod_off = ctx->d_pre_rpodoff; a.rprio = (const int32_t*)ctx->d_pre_rprio;
-    a.rn_pod = R.n_pod; a.rout_off = R.out_off ? ctx->d_pre_routoff : nullptr; a.rout = ctx->d_pre_rout; a.rn_out = R.n_out;
-    a.rrec = ctx->d_pre_rrec; a.rsorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.vlist = ctx->d_pre_vlist;
-    a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.n_gpu = ctx->n_gpu; a.tbl = ctx->d_tbl;
-    a.sel = sel_of(ctx); a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
-    a.psum = ctx->d_pre_psum; a.psum64 = ctx->d_pre_psum64;
-    a.pod_node = ctx->d_pre_node; a.pod_status = ctx->d_pre_pst;
-    a.gate = ctx->d_err + ERR_BAD_OFFSETS; a.err = err_of(ctx);
+    PreArgs a = pre_args(ctx, ctx->d_claims, ctx->d_pod_off, (const int32_t*)ctx->d_pre_prio, n_pod, dense ? nullptr : ctx->d_cand_nodes,
+                         dense ? nullptr : ctx->d_cand_off, n_pair, Rd, ctx->d_inv_live, flags);
     Prof prof(ctx);
-    // the running lists (§14)
-    k_pre_running<<<std::max(1u, (R.n_pod + 255) / 256), 256, 0, st>>>(a);
-    ctx->launches += 1;
-    if (R.n_pod) {
-        if ((rc = launch_sort(ctx, ctx->d_pre_rrec, R.n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, ctx->n_node, ctx->d_node_off)))
-            return rc;
-        if (ctx->n_node) {
-            k_pre_vsort<<<std::min(ctx->n_node, (uint32_t)ctx->n_sm * 8u), 256, 0, st>>>(a);
-            ctx->launches += 1;
-        }
-        CU(cudaMemcpyAsync(ctx->d_pp_runoff, ctx->d_claim_off, ((size_t)ctx->n_node + 1) * 4, cudaMemcpyDeviceToDevice, st));
-    } else {
-        CU(cudaMemsetAsync(ctx->d_pp_runoff, 0, ((size_t)ctx->n_node + 1) * 4, st));
-    }
-    a.list_off = ctx->d_pp_runoff;
+    if ((rc = launch_running_lists(ctx, a, prof, true))) return rc;
     // the visit lists (§13)
     PlaceArgs pl; memset(&pl, 0, sizeof pl);
     pl.claims = ctx->d_claims; pl.pod_off = ctx->d_pod_off; pl.n_pod = n_pod;
@@ -2035,9 +2049,9 @@ int preload_place_shard(dra_ctx* ctx) {
 // The same for the sharded preemption chain, whose merge waits for its peers: it also takes the all-shared split.
 int preload_preempt_shard(dra_ctx* ctx) {
     const void* ks[] = {(const void*)k_uns_prep, (const void*)k_pre_running, (const void*)k_pre_vsort,
-                        (const void*)k_pods_preempt_win<8, 8>, (const void*)k_pods_preempt_win<8, 16>, (const void*)k_pods_preempt_win<8, 32>,
-                        (const void*)k_spre_reduce, (const void*)k_pods_preempt_victims_win<8, 8>, (const void*)k_pods_preempt_victims_win<8, 16>,
-                        (const void*)k_pods_preempt_victims_win<8, 32>, (const void*)k_peer_push, (const void*)k_spre_merge,
+                        (const void*)k_pods_preempt<8, 8>, (const void*)k_pods_preempt<8, 16>, (const void*)k_pods_preempt<8, 32>,
+                        (const void*)k_spre_reduce, (const void*)k_pods_preempt_victims<8, 8>, (const void*)k_pods_preempt_victims<8, 16>,
+                        (const void*)k_pods_preempt_victims<8, 32>, (const void*)k_peer_push, (const void*)k_spre_merge,
                         (const void*)k_bucket_small, (const void*)k_bucket_hist8<false>, (const void*)k_bucket_hist8<true>,
                         (const void*)k_bucket_scan_rows, (const void*)k_bucket_scan8, (const void*)k_bucket_hist,
                         (const void*)k_bucket_scan, (const void*)k_bucket_scatter};
@@ -2836,8 +2850,8 @@ int dra_set_shard_preempt(dra_ctx* ctx, uint32_t max_pods, uint32_t max_pairs, u
 }
 
 // Sharded preemption: offset checks and pair -> pod (k_uns_prep) -> the running pods, their bucketing and victim lists on
-// the whole inventory (k_pre_running, the counting sort, k_pre_vsort) -> the window's pairs (k_pods_preempt_win) -> per-pod
-// partials (k_spre_reduce, k_pods_preempt_victims_win) -> push to every peer -> wait + merge into the caller's buffers (k_spre_merge).
+// the whole inventory (k_pre_running, the counting sort, k_pre_vsort) -> the window's pairs (k_pods_preempt) -> per-pod
+// partials (k_spre_reduce, k_pods_preempt_victims) -> push to every peer -> wait + merge into the caller's buffers (k_spre_merge).
 // Enqueues only.
 int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
                                     const uint32_t* d_pod_off, const int32_t* d_prio, uint32_t n_pod,
@@ -2880,7 +2894,6 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     if (rc) return rc;
     if ((rc = ensure_batch(ctx, std::max(R.n_pod, 1u), 1, false))) return rc;
     if ((rc = spre_buffers(ctx, n_pod, n_pair, max_victims, R.n_pod))) return rc;
-    if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, ctx->stream)); }
     cudaStream_t st = ctx->stream;
     const uint32_t lo = gather ? ctx->shard_lo : 0u, hi = gather ? ctx->shard_hi : ctx->n_node;   // world 1: every node
     const bool want_pairs = d_pair_status || d_pair_victims;
@@ -2889,51 +2902,21 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     s.stride = 2 + (max_victims + 3) / 4; s.part = ctx->d_spre_part;
     s.pairs = want_pairs ? reinterpret_cast<uint2*>(ctx->d_spre_part + 1 + (size_t)n_pod * s.stride) : nullptr;
 
-    PreArgs a; memset(&a, 0, sizeof a);
-    a.claims = (const uint4*)d_claims; a.pod_off = d_pod_off; a.prio = d_prio; a.n_pod = n_pod;
-    a.cand_nodes = dense ? nullptr : d_cand_nodes; a.cand_off = dense ? nullptr : d_cand_off;
-    a.pair_pod = dense ? nullptr : ctx->d_upair_pod; a.n_pair = n_pair;
-    a.rclaims = (const uint4*)R.claims; a.rn_claim = R.n_claim; a.rpod_off = R.pod_off; a.rprio = R.prio; a.rn_pod = R.n_pod;
-    a.rout_off = R.out_off; a.rout = (const uint2*)R.out; a.rn_out = R.n_out;
-    a.rrec = ctx->d_pre_rrec; a.rsorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.vlist = ctx->d_pre_vlist;
-    a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.n_gpu = ctx->n_gpu; a.tbl = ctx->d_tbl;
-    a.sel = sel_of(ctx); a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
-    a.psum = ctx->d_pre_psum; a.psum64 = ctx->d_pre_psum64; a.max_victims = max_victims;
-    a.work = ctx->d_ticket + 13;
-    a.gate = ctx->d_err + ERR_BAD_OFFSETS; a.err = err_of(ctx);
+    PreArgs a = pre_args(ctx, (const uint4*)d_claims, d_pod_off, d_prio, n_pod, dense ? nullptr : d_cand_nodes,
+                         dense ? nullptr : d_cand_off, n_pair, R, ctx->d_inv_live, flags);
+    a.pair_pod = dense ? nullptr : ctx->d_upair_pod; a.max_victims = max_victims;
     Prof prof(ctx);
-    CU(cudaMemsetAsync(a.work, 0, 4, st));
     k_uns_prep<<<std::max(1u, (n_pod + 7) / 8), 256, 0, st>>>(d_pod_off, dense ? nullptr : d_cand_off, n_pod, n_claim, n_pair,
                                                               ctx->d_upair_pod, a.err);
-    k_pre_running<<<std::max(1u, (R.n_pod + 255) / 256), 256, 0, st>>>(a);
-    ctx->launches += 2;
-    if (R.n_pod) {
-        if ((rc = launch_sort(ctx, ctx->d_pre_rrec, R.n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, ctx->n_node, ctx->d_node_off)))
-            return rc;
-    } else {
-        CU(cudaMemsetAsync(ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, st));
-    }
-    const uint32_t W = ctx->max_width <= 8 ? 8u : (ctx->max_width <= 16 ? 16u : 32u);
-    if (ctx->n_node) {
-        k_pre_vsort<<<std::min(ctx->n_node, (uint32_t)ctx->n_sm * 8u), 256, 0, st>>>(a);
-        ctx->launches += 1;
-    }
-    const uint32_t per_cta = 8 * (32 / W);
-    if (s.n_walk) {
-        const uint32_t grid = std::max(1u, std::min((s.n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
-        if (W == 8) k_pods_preempt_win<8, 8><<<grid, 256, 0, st>>>(a, s);
-        else if (W == 16) k_pods_preempt_win<8, 16><<<grid, 256, 0, st>>>(a, s);
-        else k_pods_preempt_win<8, 32><<<grid, 256, 0, st>>>(a, s);
-        ctx->launches += 1;
-    }
+    ctx->launches += 1;
+    if ((rc = launch_running_lists(ctx, a, prof, false))) return rc;
+    if ((rc = launch_preempt_pairs(ctx, a, s))) return rc;
     k_spre_reduce<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, s);
     ctx->launches += 1;
     if (max_victims && hi > lo) {
-        const uint32_t grid = std::max(1u, std::min((n_pod + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
-        if (W == 8) k_pods_preempt_victims_win<8, 8><<<grid, 256, 0, st>>>(a, s);
-        else if (W == 16) k_pods_preempt_victims_win<8, 16><<<grid, 256, 0, st>>>(a, s);
-        else k_pods_preempt_victims_win<8, 32><<<grid, 256, 0, st>>>(a, s);
-        ctx->launches += 1;
+        // in words from pod 0's partial: the best EVICT position at 1, the row from 8 (unit 2); 4 * stride words per pod
+        uint32_t* part = reinterpret_cast<uint32_t*>(s.part + 1);
+        launch_preempt_victims(ctx, a, part + 1, 4 * s.stride, part + 8, 4 * s.stride);
     }
     prof.mark();
     PreMerge m; memset(&m, 0, sizeof m);
@@ -3058,32 +3041,10 @@ int dra_preempt_place_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     CU(cudaMemsetAsync(ctx->d_pp_judged, 0, ((size_t)ctx->n_node + 1) * 4, st));
     if (R.n_pod) CU(cudaMemsetAsync(ctx->d_pp_evicted, 0xFF, (size_t)R.n_pod * 4, st));
 
-    PreArgs a; memset(&a, 0, sizeof a);
-    a.claims = (const uint4*)d_claims; a.pod_off = d_pod_off; a.prio = d_prio; a.n_pod = n_pod;
-    a.cand_nodes = dense ? nullptr : d_cand_nodes; a.cand_off = dense ? nullptr : d_cand_off; a.n_pair = walk;
-    a.rclaims = (const uint4*)R.claims; a.rn_claim = R.n_claim; a.rpod_off = R.pod_off; a.rprio = R.prio; a.rn_pod = R.n_pod;
-    a.rout_off = R.out_off; a.rout = (const uint2*)R.out; a.rn_out = R.n_out;
-    a.rrec = ctx->d_pre_rrec; a.rsorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.vlist = ctx->d_pre_vlist;
-    a.inv = ctx->d_spp_inv; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.n_gpu = ctx->n_gpu; a.tbl = ctx->d_tbl;
-    a.sel = sel_of(ctx); a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
-    a.psum = ctx->d_pre_psum; a.psum64 = ctx->d_pre_psum64;
-    a.pod_node = ctx->d_pre_node; a.pod_status = ctx->d_pre_pst;
-    a.gate = ctx->d_err + ERR_BAD_OFFSETS; a.err = err;
+    PreArgs a = pre_args(ctx, (const uint4*)d_claims, d_pod_off, d_prio, n_pod, dense ? nullptr : d_cand_nodes,
+                         dense ? nullptr : d_cand_off, walk, R, ctx->d_spp_inv, flags);
     // the running lists (§14), on global GPU indices: every rank finds the same faults
-    k_pre_running<<<std::max(1u, (R.n_pod + 255) / 256), 256, 0, st>>>(a);
-    ctx->launches += 1;
-    if (R.n_pod) {
-        if ((rc = launch_sort(ctx, ctx->d_pre_rrec, R.n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_spp_inv, false, ctx->n_node, ctx->d_node_off)))
-            return rc;
-        if (ctx->n_node) {
-            k_pre_vsort<<<std::min(ctx->n_node, (uint32_t)ctx->n_sm * 8u), 256, 0, st>>>(a);
-            ctx->launches += 1;
-        }
-        CU(cudaMemcpyAsync(ctx->d_pp_runoff, ctx->d_claim_off, ((size_t)ctx->n_node + 1) * 4, cudaMemcpyDeviceToDevice, st));
-    } else {
-        CU(cudaMemsetAsync(ctx->d_pp_runoff, 0, ((size_t)ctx->n_node + 1) * 4, st));
-    }
-    a.list_off = ctx->d_pp_runoff;
+    if ((rc = launch_running_lists(ctx, a, prof, true))) return rc;
     // the checks of the pending arrays and the visit lists (§13)
     PlaceArgs pl; memset(&pl, 0, sizeof pl);
     pl.claims = a.claims; pl.pod_off = d_pod_off; pl.n_pod = n_pod;

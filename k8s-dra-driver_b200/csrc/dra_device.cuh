@@ -13,7 +13,7 @@
 //   k_pods_place     place pods (spec §13): persistent, a warp walks each of its nodes' visit lists with a cursor;
 //                    sharded (<4, true>): the rank's node window, pod states replicated on every rank (k_splace_*)
 //   k_pods_preempt   preemption (spec §14): per (pod, candidate) pair, W lanes, the victims by remove-all-then-reprieve;
-//                    sharded (k_pods_preempt_win): the rank's node window, per-pod partials merged on every rank (k_spre_*)
+//                    sharded: the same kernel on the rank's node window, per-pod partials merged on every rank (k_spre_*)
 //   k_dealloc        inverse updates with atomics (sharded: behind k_dealloc_check, on the rank's GPU range only)
 //
 // What this replaces in the reference: the per-node search behind Allocate()/UnsuitableNodes() that
@@ -3519,6 +3519,7 @@ k_imex_offsets(const int* __restrict__ used, const uint32_t* __restrict__ dom_of
 //   k_pods_preempt  W lanes per pair, one per GPU of the node: dry pod_eval, remove V, pod_eval, the reprieve loop
 //   k_pre_choose    warp per pod: the pod's pairs reduced in list order
 //   k_pods_preempt_victims  W lanes per pod: the reprieve of the chosen pair again, this time writing the victims
+// The sharded call (below) runs the same two pair kernels on its rank's node window.
 // ====================================================================================================
 struct PreArgs {
     const uint4* claims; const uint32_t* pod_off; const int32_t* prio; uint32_t n_pod;
@@ -3536,10 +3537,20 @@ struct PreArgs {
     unsigned long long* psum64;   // [n_pair] sum over the victims of (priority + 2^31)
     uint8_t* pair_status; uint32_t* pair_victims;                   // caller's per-pair outputs (may be nullptr)
     uint32_t* pod_node; uint8_t* pod_status; uint32_t* n_victims; uint32_t* choice;
-    uint32_t* victims; uint32_t max_victims;
+    uint32_t max_victims;
     uint32_t* work;               // next unclaimed pair (zeroed by the host)
     const uint32_t* gate;         // non-zero: the running pods failed their check, nothing is evaluated
     Err err;
+};
+
+// The pair kernel's node window and the sharded call's partials (layout at k_spre_reduce).  The single-inventory call:
+// the window [0, n_node), n_walk = n_pair, no partials.
+struct PreShard {
+    uint32_t node_lo, node_hi;    // the pairs to judge are those of the nodes in [node_lo, node_hi), or of no node
+    uint32_t n_walk;              // pairs the evaluation walks: dense n_pod * (node_hi - node_lo), else n_pair
+    uint32_t stride;              // uint4 units per pod partial: 2 + ceil(max_victims / 4)
+    uint4* part;                  // the partials (header, pods)
+    uint2* pairs;                 // the window's pair results (nullptr: the caller asked for none)
 };
 
 // Thread per running pod.  Its node is the node of the GPUs its OK slots name (slots counted as §9 counts them); a pod
@@ -3617,6 +3628,20 @@ __device__ __forceinline__ void pre_apply(Lane& L, const PreArgs& a, const uint4
 
 struct PreSum { uint32_t st, count, hi, hi_idx; unsigned long long sum; };
 
+// Is the pod of cnt claims at `claims` INVALID: more than DRA_MAX_POD claims, or one invalid in slot mode have_off (§1) or
+// naming a selector past n_sel?  On the W lanes gbase.. (gl = lane - gbase; gmask the group's lanes), answered on each.
+template <int W>
+__device__ __forceinline__ bool pod_invalid(const uint4* claims, const uint32_t cnt, const uint32_t n_sel, const bool have_off,
+                                            const uint32_t gl, const uint32_t gmask) {
+    bool inv = cnt > DRA_MAX_POD;
+    for (uint32_t i = gl; i < cnt && !inv; i += W) {
+        const uint4 c = __ldg(&claims[i]);
+        const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
+        inv = claim_invalid(kind, prof, count, have_off) || claim_sel(kind, c.z, c.w) > n_sel;
+    }
+    return (__ballot_sync(gmask, inv) & gmask) != 0u;
+}
+
 // Pair (pod, node) on the W lanes gbase.. of the warp.  skip_first: the pair is known to be EVICT (k_pods_preempt_victims), so the
 // evaluation on the node as it is and the validity check are left out.  row: where the victims go (lane gbase writes).
 // LIVE (spec §15, k_pods_preempt_place): the node as it stands is *live, the walk's working state, instead of a.inv; `row` is
@@ -3645,13 +3670,7 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
         Lt = L;
         st1 = pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr);
         if (st1 == 0) { s.st = DRA_PRE_FITS; return s; }
-        bool inv = false;
-        for (uint32_t i = gl; i < cnt; i += W) {
-            const uint4 c = get(i);
-            const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
-            inv = inv || claim_invalid(kind, prof, count, true) || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
-        }
-        if (__ballot_sync(gmask, inv) & gmask) { s.st = DRA_PRE_INVALID; return s; }
+        if (pod_invalid<W>(a.claims + c0, cnt, a.sel.n_sel, true, gl, gmask)) { s.st = DRA_PRE_INVALID; return s; }
     }
     // V: the tail of the node's list below the pod's priority (the list is by priority descending)
     const int32_t P = __ldg(&a.prio[pod]);
@@ -3692,10 +3711,12 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
 }
 
 // W lanes per (pod, candidate) pair, 32/W pairs per warp, in k_unsuitable's layout; pairs are taken from a counter, since
-// a pair costs from one evaluation to |V| + 2 of them.
+// a pair costs from one evaluation to |V| + 2 of them.  The pairs of s's node window: dense, the window's columns; with
+// candidates, every pair but those naming another rank's node (a pair naming no node is judged NO, as k_pre_choose
+// reads every pair).
 template <int WPC, int W>
 __global__ void __launch_bounds__(WPC * 32, 2)
-k_pods_preempt(const PreArgs a) {
+k_pods_preempt(const PreArgs a, const PreShard s) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
     if (__ldcg(a.gate)) return;
     for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
@@ -3704,22 +3725,29 @@ k_pods_preempt(const PreArgs a) {
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t grp = lane / W, gbase = grp * W;
     const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
+    const uint32_t n_win = s.node_hi - s.node_lo;
     while (true) {
         uint32_t nxt = 0;
         if (lane == 0) nxt = atomicAdd(a.work, G);
         const uint32_t pw = __shfl_sync(FULLMASK, nxt, 0);
-        if (pw >= a.n_pair) break;
-        const uint32_t pair = pw + grp;
-        if (pair >= a.n_pair) continue;                                  // whole group skips together
-        uint32_t pod, node;
-        if (!a.cand_off) { pod = pair / a.n_node; node = pair - pod * a.n_node; }
-        else { pod = __ldg(&a.pair_pod[pair]); node = __ldg(&a.cand_nodes[pair]); }
-        const PreSum s = pre_pair<W>(a, tbl_s, pod, node, lane, gmask, gbase, false, nullptr);
+        if (pw >= s.n_walk) break;
+        const uint32_t walk = pw + grp;
+        if (walk >= s.n_walk) continue;                                  // whole group skips together
+        uint32_t pod, node, pair;
+        if (!a.cand_off) { pod = walk / n_win; node = s.node_lo + (walk - pod * n_win); pair = pod * a.n_node + node; }
+        else {
+            pair = walk; node = __ldg(&a.cand_nodes[pair]);
+            if (node < a.n_node && node - s.node_lo >= n_win) continue;   // another rank's node
+            pod = __ldg(&a.pair_pod[pair]);
+        }
+        const PreSum r = pre_pair<W>(a, tbl_s, pod, node, lane, gmask, gbase, false, nullptr);
         if (lane == gbase) {
-            a.psum[pair] = make_uint4(s.st, s.count, s.hi, s.hi_idx);
-            a.psum64[pair] = s.sum;
-            if (a.pair_status) a.pair_status[pair] = (uint8_t)s.st;
-            if (a.pair_victims) a.pair_victims[pair] = s.st == DRA_PRE_EVICT ? s.count : 0u;
+            const uint32_t nv = r.st == DRA_PRE_EVICT ? r.count : 0u;
+            a.psum[pair] = make_uint4(r.st, r.count, r.hi, r.hi_idx);
+            a.psum64[pair] = r.sum;
+            if (a.pair_status) a.pair_status[pair] = (uint8_t)r.st;
+            if (a.pair_victims) a.pair_victims[pair] = nv;
+            if (s.pairs) s.pairs[pair] = make_uint2(r.st, nv);
         }
     }
 }
@@ -3732,24 +3760,9 @@ __device__ __forceinline__ bool pre_better(const uint4 xs, const unsigned long l
     return xs.w > ys.w;                                                  // latest "start" among the highest-priority victims
 }
 
-// Warp-wide, pod p's pair summaries psum[k0 .. k1) in list order: FITS at the first such pair, else the preferred EVICT
-// pair, else INVALID / SEARCH_LIMIT / NO.  Returns the status; k = the chosen pair (NONE without one), bs = its summary.
-__device__ __forceinline__ uint32_t pre_reduce(const PreArgs& a, const uint32_t p, const uint32_t k0, const uint32_t k1,
-                                               const uint32_t lane, uint32_t& k, uint4& bs) {
-    uint32_t fit = DRA_GPU_NONE, best = DRA_GPU_NONE;
-    bs = make_uint4(0, 0, 0, 0); unsigned long long b64 = 0;
-    bool lim = false;
-    for (uint32_t j = k0 + lane; j < k1; j += 32) {                      // each lane in list order: ties keep the earlier
-        const uint4 s = __ldcg(&a.psum[j]);
-        if (s.x == DRA_PRE_FITS) fit = min(fit, j);
-        else if (s.x == DRA_PRE_SEARCH_LIMIT) lim = true;
-        else if (s.x == DRA_PRE_EVICT) {
-            const unsigned long long v = __ldcg(&a.psum64[j]);
-            if (best == DRA_GPU_NONE || pre_better(s, v, bs, b64)) { best = j; bs = s; b64 = v; }
-        }
-    }
-    fit = __reduce_min_sync(FULLMASK, fit);
-    lim = __any_sync(FULLMASK, lim);
+// Warp-wide: every lane ends with the warp's preferred EVICT candidate (position best, NONE for none; summary bs; sum
+// b64), ties to the lower position.  bs.x, which pre_better does not read, travels with the candidate.
+__device__ __forceinline__ void pre_best_warp(uint32_t& best, uint4& bs, unsigned long long& b64) {
     for (uint32_t d = 16; d; d >>= 1) {
         const uint32_t ob = __shfl_xor_sync(FULLMASK, best, d);
         uint4 os;
@@ -3760,18 +3773,49 @@ __device__ __forceinline__ uint32_t pre_reduce(const PreArgs& a, const uint32_t 
                           (best == DRA_GPU_NONE || pre_better(os, o64, bs, b64) || (!pre_better(bs, b64, os, o64) && ob < best));
         if (take) { best = ob; bs = os; b64 = o64; }
     }
-    const uint32_t c0 = __ldg(&a.pod_off[p]), cnt = __ldg(&a.pod_off[p + 1]) - c0;
-    bool inv = cnt > DRA_MAX_POD;
-    for (uint32_t i = lane; i < cnt && !inv; i += 32) {
-        const uint4 c = __ldg(&a.claims[c0 + i]);
-        const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
-        inv = claim_invalid(kind, prof, count, true) || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
+}
+
+struct PreScan { uint32_t fit, best; uint4 bs; unsigned long long b64; bool lim; };
+
+// Warp-wide, the pair summaries psum[k0 .. k1) in list order (with win_nodes, only the pairs k whose node win_nodes[k] lies
+// in [lo, lo + n_win)): the first FITS position, the preferred EVICT position with its summary and sum, and whether a
+// SEARCH_LIMIT was seen.  The same on every lane.
+__device__ __forceinline__ PreScan pre_scan(const PreArgs& a, const uint32_t k0, const uint32_t k1, const uint32_t lane,
+                                            const uint32_t* win_nodes = nullptr, const uint32_t lo = 0, const uint32_t n_win = 0) {
+    PreScan r{DRA_GPU_NONE, DRA_GPU_NONE, make_uint4(0, 0, 0, 0), 0ull, false};
+    for (uint32_t j = k0 + lane; j < k1; j += 32) {                      // each lane in list order: ties keep the earlier
+        if (win_nodes && __ldg(&win_nodes[j]) - lo >= n_win) continue;
+        const uint4 s = __ldcg(&a.psum[j]);
+        if (s.x == DRA_PRE_FITS) r.fit = min(r.fit, j);
+        else if (s.x == DRA_PRE_SEARCH_LIMIT) r.lim = true;
+        else if (s.x == DRA_PRE_EVICT) {
+            const unsigned long long v = __ldcg(&a.psum64[j]);
+            if (r.best == DRA_GPU_NONE || pre_better(s, v, r.bs, r.b64)) { r.best = j; r.bs = s; r.b64 = v; }
+        }
     }
-    inv = __any_sync(FULLMASK, inv);
+    r.fit = __reduce_min_sync(FULLMASK, r.fit);
+    r.lim = __any_sync(FULLMASK, r.lim);
+    pre_best_warp(r.best, r.bs, r.b64);
+    return r;
+}
+
+// The pod's status from its reduced pairs: FITS at the first such pair, else the preferred EVICT pair, else INVALID /
+// SEARCH_LIMIT / NO.  k = the chosen position (NONE without one).
+__device__ __forceinline__ uint32_t pre_decide(const uint32_t fit, const uint32_t best, const bool lim, const bool inv, uint32_t& k) {
     k = DRA_GPU_NONE;
     if (fit != DRA_GPU_NONE) { k = fit; return DRA_PRE_FITS; }
     if (best != DRA_GPU_NONE) { k = best; return DRA_PRE_EVICT; }
     return inv ? DRA_PRE_INVALID : lim ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO;
+}
+
+// Warp-wide, pod p's pairs psum[k0 .. k1) reduced and decided.  Returns the status; k = the chosen pair, bs = its summary.
+__device__ __forceinline__ uint32_t pre_reduce(const PreArgs& a, const uint32_t p, const uint32_t k0, const uint32_t k1,
+                                               const uint32_t lane, uint32_t& k, uint4& bs) {
+    const PreScan r = pre_scan(a, k0, k1, lane);
+    const uint32_t c0 = __ldg(&a.pod_off[p]), cnt = __ldg(&a.pod_off[p + 1]) - c0;
+    const bool inv = pod_invalid<32>(a.claims + c0, cnt, a.sel.n_sel, true, lane, FULLMASK);
+    bs = r.bs;
+    return pre_decide(r.fit, r.best, r.lim, inv, k);
 }
 
 // Warp per pod: its pairs reduced by pre_reduce.
@@ -3791,11 +3835,12 @@ k_pre_choose(const PreArgs a) {
     a.choice[p] = st == DRA_PRE_EVICT ? k : DRA_GPU_NONE;
 }
 
-// W lanes per pod whose choice is an EVICT pair: its reprieve once more, writing the victims into the pod's row (the rows
-// are filled with 0xFFFFFFFF by the host first).  Deterministic, so the victims are the ones k_pods_preempt counted.
+// W lanes per pod p whose chosen EVICT pair is choice[p * cstride] (NONE: none): its reprieve once more, writing the first
+// min(count, max_victims) victims into the row at rows + p * rstride (the rest is filled by the caller).  Deterministic, so
+// the victims are the ones k_pods_preempt counted.
 template <int WPC, int W>
 __global__ void __launch_bounds__(WPC * 32, 2)
-k_pods_preempt_victims(const PreArgs a) {
+k_pods_preempt_victims(const PreArgs a, const uint32_t* choice, const uint32_t cstride, uint32_t* rows, const uint32_t rstride) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
     if (__ldcg(a.gate)) return;
     for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
@@ -3807,10 +3852,10 @@ k_pods_preempt_victims(const PreArgs a) {
     for (uint32_t pw = (blockIdx.x * WPC + wid) * G; pw < a.n_pod; pw += gridDim.x * WPC * G) {
         const uint32_t p = pw + grp;
         if (p >= a.n_pod) continue;
-        const uint32_t k = __ldcg(&a.choice[p]);
+        const uint32_t k = __ldcg(&choice[(size_t)p * cstride]);
         if (k == DRA_GPU_NONE) continue;
         const uint32_t node = a.cand_off ? __ldg(&a.cand_nodes[k]) : k - p * a.n_node;
-        (void)pre_pair<W>(a, tbl_s, p, node, lane, gmask, gbase, true, a.victims + (size_t)p * a.max_victims);
+        (void)pre_pair<W>(a, tbl_s, p, node, lane, gmask, gbase, true, rows + (size_t)p * rstride);
     }
 }
 
@@ -3846,16 +3891,7 @@ struct PpArgs {
 // candidate naming a node is NO.  (The pair judgement assumes out_off: it must never see a pod the apply would reject.)
 __device__ __forceinline__ void pp_prep_pod(const PreArgs& a, const PlaceArgs& pl, const PpArgs& pp, uint32_t p, uint32_t lane) {
     const uint32_t c0 = __ldg(&pl.pod_off[p]), cnt = __ldg(&pl.pod_off[p + 1]) - c0;
-    const bool have_off = pl.out_off != nullptr;
-    bool inv = cnt > DRA_MAX_POD;
-    if (!inv) {
-        for (uint32_t i = lane; i < cnt; i += 32) {
-            const uint4 c = __ldg(&pl.claims[c0 + i]);
-            const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
-            inv = inv || claim_invalid(kind, prof, count, have_off) || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
-        }
-        inv = __any_sync(FULLMASK, inv);
-    }
+    const bool inv = pod_invalid<32>(pl.claims + c0, cnt, a.sel.n_sel, pl.out_off != nullptr, lane, FULLMASK);
     const bool live = cnt != 0 && !inv;
     uint32_t first = DRA_GPU_NONE, usable = 0;
     if (!pl.cand_off) {
@@ -4118,10 +4154,11 @@ k_spp_final(const SppArgs s) {
 // Every rank gets the same pending pods, candidates and running pods.  k_uns_prep checks pod_off / cand_off and writes
 // pair -> pod; k_pre_running, the counting sort and k_pre_vsort run unchanged on the whole inventory (their checks are
 // on global GPU indices, so every rank finds the same fault).  Then, on this rank's node window only:
-//   k_pods_preempt_win    k_pods_preempt's pair evaluation for the pairs whose node lies in the window
+//   k_pods_preempt  the pair evaluation for the pairs whose node lies in the window (PreShard)
 //   k_spre_reduce   warp per pod: k_pre_choose's reduction over the window's pairs, keeping list positions, into this
 //                   rank's partial of the pod (and the rank's fault word into the partials' header)
-//   k_pods_preempt_victims_win  W lanes per pod whose partial holds an EVICT pair and no FITS pair: that pair's victim row
+//   k_pods_preempt_victims  W lanes per pod whose partial holds an EVICT pair and no FITS pair: that pair's victim row,
+//                   the first min(count, max_victims) words (the merge fills the rest)
 //   k_peer_push     the partials (and, when the caller asked for them, the window's pair results) to every peer
 //   k_spre_merge    flags, wait, then per pod the minimum over the ranks' partials; writes the caller's buffers only if
 //                   no rank reported a fault
@@ -4130,51 +4167,7 @@ k_spp_final(const SppArgs s) {
 // hi}, then the best pair's row of max_victims words; after the pods the window's pairs as {status, victims} (uint2).
 // A position is the pair's index in the call's pair list, so the merge's choice is the minimum over the ranks of a total
 // order — (FITS first, then pre_better, then position) — which is the single-inventory choice for any partition.
-struct PreShard {
-    uint32_t node_lo, node_hi;    // this rank's window
-    uint32_t n_walk;              // pairs the evaluation walks: dense n_pod * (node_hi - node_lo), else n_pair
-    uint32_t stride;              // uint4 units per pod partial: 2 + ceil(max_victims / 4)
-    uint4* part;                  // the partials (header, pods)
-    uint2* pairs;                 // the window's pair results (nullptr: the caller asked for none)
-};
-
-__device__ __forceinline__ uint4* spre_pod(const PreShard& s, uint32_t p) { return s.part + 1 + (size_t)p * s.stride; }
-
-template <int WPC, int W>
-__global__ void __launch_bounds__(WPC * 32, 2)
-k_pods_preempt_win(const PreArgs a, const PreShard s) {
-    __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
-    if (__ldcg(a.gate)) return;
-    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
-    __syncthreads();
-    constexpr uint32_t G = 32 / W;
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t grp = lane / W, gbase = grp * W;
-    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
-    const uint32_t n_win = s.node_hi - s.node_lo;
-    while (true) {
-        uint32_t nxt = 0;
-        if (lane == 0) nxt = atomicAdd(a.work, G);
-        const uint32_t pw = __shfl_sync(FULLMASK, nxt, 0);
-        if (pw >= s.n_walk) break;
-        const uint32_t walk = pw + grp;
-        if (walk >= s.n_walk) continue;                                  // whole group skips together
-        uint32_t pod, node, pair;
-        if (!a.cand_off) { pod = walk / n_win; node = s.node_lo + (walk - pod * n_win); pair = pod * a.n_node + node; }
-        else {
-            pair = walk; node = __ldg(&a.cand_nodes[pair]);
-            if (node - s.node_lo >= n_win) continue;                     // another rank's node, or none
-            pod = __ldg(&a.pair_pod[pair]);
-        }
-        const PreSum r = pre_pair<W>(a, tbl_s, pod, node, lane, gmask, gbase, false, nullptr);
-        if (lane == gbase) {
-            a.psum[pair] = make_uint4(r.st, r.count, r.hi, r.hi_idx);
-            a.psum64[pair] = r.sum;
-            if (s.pairs) s.pairs[pair] = make_uint2(r.st, r.st == DRA_PRE_EVICT ? r.count : 0u);
-        }
-    }
-}
-
+// k_pods_preempt also judges a candidate naming no node (NO); the reduce leaves it out and the merge writes it itself.
 __global__ void __launch_bounds__(256)
 k_spre_reduce(const PreArgs a, const PreShard s) {
     const uint32_t gate = __ldcg(a.gate);
@@ -4186,60 +4179,12 @@ k_spre_reduce(const PreArgs a, const PreShard s) {
     const uint32_t n_win = s.node_hi - s.node_lo;
     const uint32_t k0 = dense ? p * a.n_node + s.node_lo : __ldg(&a.cand_off[p]);
     const uint32_t k1 = dense ? k0 + n_win : __ldg(&a.cand_off[p + 1]);
-    uint32_t fit = DRA_GPU_NONE, best = DRA_GPU_NONE;
-    uint4 bs = make_uint4(0, 0, 0, 0); unsigned long long b64 = 0;
-    bool lim = false;
-    for (uint32_t k = k0 + lane; k < k1; k += 32) {                      // each lane in list order: ties keep the earlier
-        if (!dense && __ldg(&a.cand_nodes[k]) - s.node_lo >= n_win) continue;
-        const uint4 v = __ldcg(&a.psum[k]);
-        if (v.x == DRA_PRE_FITS) fit = min(fit, k);
-        else if (v.x == DRA_PRE_SEARCH_LIMIT) lim = true;
-        else if (v.x == DRA_PRE_EVICT) {
-            const unsigned long long v64 = __ldcg(&a.psum64[k]);
-            if (best == DRA_GPU_NONE || pre_better(v, v64, bs, b64)) { best = k; bs = v; b64 = v64; }
-        }
-    }
-    fit = __reduce_min_sync(FULLMASK, fit);
-    lim = __any_sync(FULLMASK, lim);
-    for (uint32_t d = 16; d; d >>= 1) {
-        const uint32_t ob = __shfl_xor_sync(FULLMASK, best, d);
-        uint4 os;
-        os.x = __shfl_xor_sync(FULLMASK, bs.x, d); os.y = __shfl_xor_sync(FULLMASK, bs.y, d);
-        os.z = __shfl_xor_sync(FULLMASK, bs.z, d); os.w = __shfl_xor_sync(FULLMASK, bs.w, d);
-        const unsigned long long o64 = __shfl_xor_sync(FULLMASK, b64, d);
-        const bool take = ob != DRA_GPU_NONE &&
-                          (best == DRA_GPU_NONE || pre_better(os, o64, bs, b64) || (!pre_better(bs, b64, os, o64) && ob < best));
-        if (take) { best = ob; bs = os; b64 = o64; }
-    }
+    PreScan r = pre_scan(a, k0, k1, lane, dense ? nullptr : a.cand_nodes, s.node_lo, n_win);
     if (lane != 0) return;
-    if (fit != DRA_GPU_NONE) best = DRA_GPU_NONE;                        // a FITS pair anywhere beats every EVICT pair
-    uint4* q = spre_pod(s, p);
-    q[0] = make_uint4(fit, best, bs.y, bs.z);
-    q[1] = make_uint4(bs.w, lim ? 1u : 0u, (uint32_t)b64, (uint32_t)(b64 >> 32));
-}
-
-// W lanes per pod: the reprieve of the pod's best local EVICT pair once more, writing its row into the partial (only the
-// first min(count, max_victims) words; the merge fills the rest)
-template <int WPC, int W>
-__global__ void __launch_bounds__(WPC * 32, 2)
-k_pods_preempt_victims_win(const PreArgs a, const PreShard s) {
-    __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
-    if (__ldcg(a.gate)) return;
-    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
-    __syncthreads();
-    constexpr uint32_t G = 32 / W;
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const uint32_t grp = lane / W, gbase = grp * W;
-    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
-    for (uint32_t pw = (blockIdx.x * WPC + wid) * G; pw < a.n_pod; pw += gridDim.x * WPC * G) {
-        const uint32_t p = pw + grp;
-        if (p >= a.n_pod) continue;
-        uint4* q = spre_pod(s, p);
-        const uint32_t k = __ldcg(&q[0]).y;
-        if (k == DRA_GPU_NONE) continue;
-        const uint32_t node = a.cand_off ? __ldg(&a.cand_nodes[k]) : k - p * a.n_node;
-        (void)pre_pair<W>(a, tbl_s, p, node, lane, gmask, gbase, true, reinterpret_cast<uint32_t*>(q + 2));
-    }
+    if (r.fit != DRA_GPU_NONE) r.best = DRA_GPU_NONE;                    // a FITS pair anywhere beats every EVICT pair
+    uint4* q = s.part + 1 + (size_t)p * s.stride;
+    q[0] = make_uint4(r.fit, r.best, r.bs.y, r.bs.z);
+    q[1] = make_uint4(r.bs.w, r.lim ? 1u : 0u, (uint32_t)r.b64, (uint32_t)(r.b64 >> 32));
 }
 
 struct PreMerge {
@@ -4289,31 +4234,15 @@ k_spre_merge(const PeerExchange x, const PreMerge m) {
         }
         const uint32_t fit = __reduce_min_sync(FULLMASK, A.x);
         const bool lim = __any_sync(FULLMASK, B.y != 0u);
-        uint32_t best = A.y, win = lane;
-        uint4 bs = make_uint4(0u, A.z, A.w, B.x);
+        uint32_t best = A.y;
+        uint4 bs = make_uint4(lane, A.z, A.w, B.x);                     // .x: the rank whose partial holds the candidate
         unsigned long long b64 = (unsigned long long)B.z | ((unsigned long long)B.w << 32);
-        for (uint32_t d = 16; d; d >>= 1) {
-            const uint32_t ob = __shfl_xor_sync(FULLMASK, best, d), ow = __shfl_xor_sync(FULLMASK, win, d);
-            uint4 os;
-            os.x = 0u; os.y = __shfl_xor_sync(FULLMASK, bs.y, d);
-            os.z = __shfl_xor_sync(FULLMASK, bs.z, d); os.w = __shfl_xor_sync(FULLMASK, bs.w, d);
-            const unsigned long long o64 = __shfl_xor_sync(FULLMASK, b64, d);
-            const bool take = ob != DRA_GPU_NONE &&
-                              (best == DRA_GPU_NONE || pre_better(os, o64, bs, b64) || (!pre_better(bs, b64, os, o64) && ob < best));
-            if (take) { best = ob; bs = os; b64 = o64; win = ow; }
-        }
+        pre_best_warp(best, bs, b64);
+        const uint32_t win = bs.x;
         const uint32_t c0 = __ldg(&m.pod_off[p]), cnt = __ldg(&m.pod_off[p + 1]) - c0;
-        bool inv = cnt > DRA_MAX_POD;
-        for (uint32_t i = lane; i < cnt && !inv; i += 32) {
-            const uint4 c = __ldg(&m.claims[c0 + i]);
-            const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
-            inv = claim_invalid(kind, prof, count, true) || claim_sel(kind, c.z, c.w) > m.sel.n_sel;
-        }
-        inv = __any_sync(FULLMASK, inv);
-        uint32_t st, k = DRA_GPU_NONE;
-        if (fit != DRA_GPU_NONE) { st = DRA_PRE_FITS; k = fit; }
-        else if (best != DRA_GPU_NONE) { st = DRA_PRE_EVICT; k = best; }
-        else st = inv ? DRA_PRE_INVALID : lim ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO;
+        const bool inv = pod_invalid<32>(m.claims + c0, cnt, m.sel.n_sel, true, lane, FULLMASK);
+        uint32_t k;
+        const uint32_t st = pre_decide(fit, best, lim, inv, k);
         const uint32_t nv = st == DRA_PRE_EVICT ? bs.y : 0u;
         if (lane == 0) {
             m.pod_status[p] = (uint8_t)st;
