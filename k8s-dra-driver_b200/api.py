@@ -141,6 +141,36 @@ def load(build_if_stale: bool = True) -> C.CDLL:
     return lib
 
 
+def _cands(cand_nodes, cand_off):
+    """(cand_nodes, cand_off) as the C calls take them: both None in the dense form, else uint32 arrays with an empty
+    cand_nodes made one element long, since NULL would mean the dense form."""
+    if cand_nodes is None and cand_off is None:
+        return None, None
+    cn = np.ascontiguousarray(cand_nodes if cand_nodes is not None else [], dtype=np.uint32)
+    return (cn if len(cn) else np.zeros(1, np.uint32)), np.ascontiguousarray(cand_off, dtype=np.uint32)
+
+
+def _running(claims, pod_off, prio, out, out_off=None) -> RunningPods:
+    """RunningPods over contiguous copies of the arrays, which it keeps alive."""
+    keep = (np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE), np.ascontiguousarray(pod_off, dtype=np.uint32),
+            np.ascontiguousarray(prio, dtype=np.int32), np.ascontiguousarray(out, dtype=R.OUT_DTYPE),
+            None if out_off is None else np.ascontiguousarray(out_off, dtype=np.uint32))
+    c, po, pr, o, oo = keep
+    run = RunningPods(c.ctypes.data, len(c), po.ctypes.data, len(po) - 1, pr.ctypes.data,
+                      None if oo is None else oo.ctypes.data, o.ctypes.data, len(o))
+    run._keep = keep
+    return run
+
+
+def _placed_n_out(claims, out_off) -> int:
+    """n_out for claims whose node is still to be chosen: their slots as if every claim named a node of the inventory."""
+    if out_off is None:
+        return len(claims)
+    placed = claims.copy()
+    placed["node"] = 0
+    return int(R.claim_slots(placed, 1).sum())
+
+
 def _ptr(a):
     if a is None:
         return None
@@ -304,15 +334,8 @@ class Context:
         po = np.ascontiguousarray(pod_off, dtype=np.uint32)
         oo = None if out_off is None else np.ascontiguousarray(out_off, dtype=np.uint32)
         if n_out is None:
-            placed = c.copy()
-            placed["node"] = 0                         # slots as if every claim named a node of the inventory
-            n_out = len(c) if oo is None else int(R.claim_slots(placed, 1).sum())
-        cn = co = None
-        if cand_nodes is not None or cand_off is not None:
-            co = np.ascontiguousarray(cand_off, dtype=np.uint32)
-            cn = np.ascontiguousarray(cand_nodes if cand_nodes is not None else [], dtype=np.uint32)
-            if len(cn) == 0:
-                cn = np.zeros(1, np.uint32)            # NULL would mean the dense form
+            n_out = _placed_n_out(c, oo)
+        cn, co = _cands(cand_nodes, cand_off)
         n_pod = len(po) - 1
         out = np.zeros(n_out, dtype=R.OUT_DTYPE)
         pod_node = np.zeros(max(n_pod, 1), dtype=np.uint32)
@@ -349,20 +372,9 @@ class Context:
         po = np.ascontiguousarray(pod_off, dtype=np.uint32)
         pr = np.ascontiguousarray(prio, dtype=np.int32)
         n_pod = len(po) - 1
-        rc_ = np.ascontiguousarray(run_claims, dtype=R.CLAIM_DTYPE)
-        rpo = np.ascontiguousarray(run_pod_off, dtype=np.uint32)
-        rpr = np.ascontiguousarray(run_prio, dtype=np.int32)
-        ro = np.ascontiguousarray(run_out, dtype=R.OUT_DTYPE)
-        roo = None if run_out_off is None else np.ascontiguousarray(run_out_off, dtype=np.uint32)
-        cn = co = None
-        if cand_nodes is not None or cand_off is not None:
-            co = np.ascontiguousarray(cand_off, dtype=np.uint32)
-            cn = np.ascontiguousarray(cand_nodes if cand_nodes is not None else [], dtype=np.uint32)
-            if len(cn) == 0:
-                cn = np.zeros(1, np.uint32)            # NULL would mean the dense form
+        run = _running(run_claims, run_pod_off, run_prio, run_out, run_out_off)
+        cn, co = _cands(cand_nodes, cand_off)
         n_pair = n_pod * self.n_node if co is None else int(co[-1])
-        run = RunningPods(rc_.ctypes.data, len(rc_), rpo.ctypes.data, len(rpo) - 1, rpr.ctypes.data,
-                          None if roo is None else roo.ctypes.data, ro.ctypes.data, len(ro))
         pair_status = np.zeros(max(n_pair, 1), dtype=np.uint8)
         pair_victims = np.zeros(max(n_pair, 1), dtype=np.uint32)
         pod_node = np.zeros(max(n_pod, 1), dtype=np.uint32)
@@ -389,30 +401,17 @@ class Context:
         n_pod = len(po) - 1
         oo = None if out_off is None else np.ascontiguousarray(out_off, dtype=np.uint32)
         if n_out is None:
-            placed = c.copy()
-            placed["node"] = 0                         # slots as if every claim named a node of the inventory
-            n_out = len(c) if oo is None else int(R.claim_slots(placed, 1).sum())
-        rc_ = np.ascontiguousarray(run_claims, dtype=R.CLAIM_DTYPE)
-        rpo = np.ascontiguousarray(run_pod_off, dtype=np.uint32)
-        rpr = np.ascontiguousarray(run_prio, dtype=np.int32)
-        ro = np.ascontiguousarray(run_out, dtype=R.OUT_DTYPE)
-        roo = None if run_out_off is None else np.ascontiguousarray(run_out_off, dtype=np.uint32)
-        cn = co = None
-        if cand_nodes is not None or cand_off is not None:
-            co = np.ascontiguousarray(cand_off, dtype=np.uint32)
-            cn = np.ascontiguousarray(cand_nodes if cand_nodes is not None else [], dtype=np.uint32)
-            if len(cn) == 0:
-                cn = np.zeros(1, np.uint32)            # NULL would mean the dense form
-        run = RunningPods(rc_.ctypes.data, len(rc_), rpo.ctypes.data, len(rpo) - 1, rpr.ctypes.data,
-                          None if roo is None else roo.ctypes.data, ro.ctypes.data, len(ro))
+            n_out = _placed_n_out(c, oo)
+        run = _running(run_claims, run_pod_off, run_prio, run_out, run_out_off)
+        cn, co = _cands(cand_nodes, cand_off)
         out = np.zeros(max(n_out, 1), dtype=R.OUT_DTYPE)
         pod_node = np.zeros(max(n_pod, 1), dtype=np.uint32)
         pod_status = np.zeros(max(n_pod, 1), dtype=np.uint8)
-        evicted_by = np.zeros(max(len(rpo) - 1, 1), dtype=np.uint32)
+        evicted_by = np.zeros(max(run.n_pod, 1), dtype=np.uint32)
         self._check(self._lib.dra_preempt_place_batch(self._h, _ptr(c), len(c), _ptr(po), _ptr(pr), n_pod, _ptr(cn), _ptr(co),
                                                       C.byref(run), _ptr(oo), _ptr(out), n_out, _ptr(pod_node),
                                                       _ptr(pod_status), _ptr(evicted_by), flags))
-        return out[:n_out], pod_node[:n_pod], pod_status[:n_pod], evicted_by[:len(rpo) - 1]
+        return out[:n_out], pod_node[:n_pod], pod_status[:n_pod], evicted_by[:run.n_pod]
 
     def deallocate(self, claims, out, out_off=None):
         c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)

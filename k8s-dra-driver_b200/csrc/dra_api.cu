@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <map>
 #include <mutex>
 #include <string>
@@ -273,9 +274,18 @@ int grow_nc(dra_ctx* ctx, T*& p, size_t have_cap, size_t new_cap) {   // compani
     return DRA_OK;
 }
 
-template <class T>
-int grow_pre(dra_ctx* ctx, T*& p, size_t need) {            // a buffer of the preemption call, capacity tracked by the caller
-    return grow_nc(ctx, p, 0, need + need / 2 + 64);
+// A group of buffers that share the capacity cap (elements): once need exceeds it, every one of them is reallocated for
+// need + need / 2 + 64 elements.  A sharded call and its dra_shard_export compute need through the same function, so the
+// export leaves nothing for the call to outgrow.
+template <class... T>
+int grow_set(dra_ctx* ctx, size_t& cap, size_t need, T*&... bufs) {
+    if (need <= cap) return DRA_OK;
+    const size_t ncap = need + need / 2 + 64;
+    int rc = DRA_OK;
+    ((rc = rc ? rc : grow_nc(ctx, bufs, 0, ncap)), ...);
+    if (rc) return rc;
+    cap = ncap;
+    return DRA_OK;
 }
 
 int grow_pinned(dra_ctx* ctx, uint8_t*& p, size_t& cap, size_t need) {
@@ -728,105 +738,187 @@ int check_err(dra_ctx* ctx) {
 // The device buffers of a §15 walk (dra_preempt_place_batch and its sharded form) for n_pod pending pods, n_pair judged
 // pairs (n_pod * n_node in the dense form) and rn_pod running pods
 int pp_buffers(dra_ctx* ctx, uint32_t n_pod, uint32_t n_pair, uint32_t rn_pod) {
+    const size_t pods = (size_t)n_pod + 8, pairs = (size_t)n_pair + 8, rpods = (size_t)rn_pod + 8, nodes = (size_t)ctx->n_node + 8;
     int rc;
-    if ((size_t)n_pair + 8 > ctx->cap_podrec) {
-        size_t cap = (size_t)n_pair + n_pair / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_podrec, 0, cap))) return rc;
-        ctx->cap_podrec = cap;
-    }
-    if ((size_t)n_pod + 8 > ctx->cap_place_pods) {
-        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_place_state, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_place_node, 0, cap))) return rc;
-        ctx->cap_place_pods = cap;
-    }
-    if ((size_t)ctx->n_node + 8 > ctx->cap_place_cursor) {
-        size_t cap = (size_t)ctx->n_node + ctx->n_node / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_place_cursor, 0, cap))) return rc;
-        ctx->cap_place_cursor = cap;
-    }
-    if ((size_t)n_pod + 8 > ctx->cap_pre_pods) {
-        const size_t need = (size_t)n_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_prio, need)) || (rc = grow_pre(ctx, ctx->d_pre_node, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_nvic, need)) || (rc = grow_pre(ctx, ctx->d_pre_choice, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_pst, need))) return rc;
-        ctx->cap_pre_pods = need + need / 2 + 64;
-    }
-    if ((size_t)n_pair + 8 > ctx->cap_pre_pairs) {
-        const size_t need = (size_t)n_pair + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_psum, need)) || (rc = grow_pre(ctx, ctx->d_pre_psum64, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_pairst, need)) || (rc = grow_pre(ctx, ctx->d_pre_pairvic, need))) return rc;
-        ctx->cap_pre_pairs = need + need / 2 + 64;
-    }
-    if ((size_t)rn_pod + 8 > ctx->cap_pre_rpods) {
-        const size_t need = (size_t)rn_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rpodoff, need)) || (rc = grow_pre(ctx, ctx->d_pre_rprio, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_rrec, need)) || (rc = grow_pre(ctx, ctx->d_pre_vlist, need))) return rc;
-        ctx->cap_pre_rpods = need + need / 2 + 64;
-    }
-    if ((size_t)n_pod + 8 > ctx->cap_pp_pods) {
-        const size_t need = (size_t)n_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pp_pending, need))) return rc;
-        ctx->cap_pp_pods = need + need / 2 + 64;
-    }
-    if ((size_t)rn_pod + 8 > ctx->cap_pp_rpods) {
-        const size_t need = (size_t)rn_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pp_evicted, need))) return rc;
-        ctx->cap_pp_rpods = need + need / 2 + 64;
-    }
-    if ((size_t)ctx->n_node + 8 > ctx->cap_pp_nodes) {
-        const size_t need = (size_t)ctx->n_node + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pp_runoff, need)) || (rc = grow_pre(ctx, ctx->d_pp_judged, need))) return rc;
-        ctx->cap_pp_nodes = need + need / 2 + 64;
-    }
+    if ((rc = grow_set(ctx, ctx->cap_podrec, pairs, ctx->d_podrec)) ||
+        (rc = grow_set(ctx, ctx->cap_place_pods, pods, ctx->d_place_state, ctx->d_place_node)) ||
+        (rc = grow_set(ctx, ctx->cap_place_cursor, nodes, ctx->d_place_cursor)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_pods, pods, ctx->d_pre_prio, ctx->d_pre_node, ctx->d_pre_nvic, ctx->d_pre_choice, ctx->d_pre_pst)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_pairs, pairs, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_rpods, rpods, ctx->d_pre_rpodoff, ctx->d_pre_rprio, ctx->d_pre_rrec, ctx->d_pre_vlist)) ||
+        (rc = grow_set(ctx, ctx->cap_pp_pods, pods, ctx->d_pp_pending)) ||
+        (rc = grow_set(ctx, ctx->cap_pp_rpods, rpods, ctx->d_pp_evicted)) ||
+        (rc = grow_set(ctx, ctx->cap_pp_nodes, nodes, ctx->d_pp_runoff, ctx->d_pp_judged))) return rc;
     return DRA_OK;
 }
 
 size_t al16(size_t b) { return (b + 15) & ~(size_t)15; }
 
-// Pinned staging bytes of the running pods: claims | pod_off | prio | out_off | out, each rounded up to 16 bytes
-size_t running_room(const dra_running_pods& R) {
-    return al16((size_t)R.n_claim * 16) + al16(((size_t)R.n_pod + 1) * 4) + al16((size_t)R.n_pod * 4) +
-           (R.out_off ? al16((size_t)R.n_claim * 4) : 0) + al16((size_t)R.n_out * 8);
-}
+// The inputs of a synchronous call, each part from the host at src to the device at dst.  A part without src is written
+// by the caller (stage_in's fill).  A fixed array, nothing allocated per call: a part beyond CAP is not kept, and
+// stage_in refuses the call.
+struct Staging {
+    static constexpr int CAP = 12;
+    struct Part { void* dst; const void* src; size_t bytes; };
+    Part part[CAP];
+    int n = 0;
+    bool overflow = false;
+    void add(void* dst, const void* src, size_t bytes) {
+        if (n < CAP) part[n++] = Part{dst, src, bytes};
+        else overflow = true;
+    }
+};
 
-// The caller's running pods R into the d_pre_r* buffers (grown as needed) through the pinned staging at h
-// (running_room(R) bytes); dev = R with those device pointers.  Enqueues only.
-int upload_running(dra_ctx* ctx, const dra_running_pods& R, uint8_t* h, dra_running_pods& dev) {
+// s's parts through the pinned h_in (grown once), each at a 16-byte boundary; parts of no bytes are skipped.  Each part is
+// copied in, or for the part without src written by fill(its staging), before its copy to the device is enqueued.
+template <class Fill>
+int stage_in(dra_ctx* ctx, const Staging& s, Fill fill) {
+    if (s.overflow) return fail(ctx, DRA_E_STATE, "more than %d staged inputs in one call", Staging::CAP);
+    size_t total = 0;
+    for (int i = 0; i < s.n; ++i) total += al16(s.part[i].bytes);
+    if (int rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, total)) return rc;
+    uint8_t* h = ctx->h_in;
+    for (int i = 0; i < s.n; ++i) {
+        const Staging::Part& p = s.part[i];
+        if (!p.bytes) continue;
+        if (p.src) memcpy(h, p.src, p.bytes);
+        else fill(h);
+        CU(cudaMemcpyAsync(p.dst, h, p.bytes, cudaMemcpyHostToDevice, ctx->stream));
+        h += al16(p.bytes);
+    }
+    return DRA_OK;
+}
+int stage_in(dra_ctx* ctx, const Staging& s) { return stage_in(ctx, s, [](uint8_t*) {}); }
+
+// The caller's running pods R as parts of s, into the d_pre_r* buffers (grown as needed); dev = R with those device pointers
+int running_parts(dra_ctx* ctx, const dra_running_pods& R, Staging& s, dra_running_pods& dev) {
     int rc;
-    if ((size_t)R.n_claim + 8 > ctx->cap_pre_rclaims) {
-        const size_t need = (size_t)R.n_claim + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rclaims, need)) || (rc = grow_pre(ctx, ctx->d_pre_routoff, need))) return rc;
-        ctx->cap_pre_rclaims = need + need / 2 + 64;
-    }
-    if ((size_t)R.n_pod + 8 > ctx->cap_pre_rpods) {
-        const size_t need = (size_t)R.n_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rpodoff, need)) || (rc = grow_pre(ctx, ctx->d_pre_rprio, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_rrec, need)) || (rc = grow_pre(ctx, ctx->d_pre_vlist, need))) return rc;
-        ctx->cap_pre_rpods = need + need / 2 + 64;
-    }
-    if ((size_t)R.n_out + 8 > ctx->cap_pre_rout) {
-        const size_t need = (size_t)R.n_out + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rout, need))) return rc;
-        ctx->cap_pre_rout = need + need / 2 + 64;
-    }
-    auto put = [&](const void* src, size_t bytes) { uint8_t* d = h; if (bytes) memcpy(d, src, bytes); h += al16(bytes); return d; };
-    uint8_t* h_rc = put(R.claims, (size_t)R.n_claim * 16);
-    uint8_t* h_rpo = put(R.pod_off, ((size_t)R.n_pod + 1) * 4);
-    uint8_t* h_rpr = put(R.prio, (size_t)R.n_pod * 4);
-    uint8_t* h_roo = R.out_off ? put(R.out_off, (size_t)R.n_claim * 4) : nullptr;
-    uint8_t* h_ro = put(R.out, (size_t)R.n_out * 8);
-    cudaStream_t st = ctx->stream;
-    if (R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_rclaims, h_rc, (size_t)R.n_claim * 16, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pre_rpodoff, h_rpo, ((size_t)R.n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (R.n_pod) CU(cudaMemcpyAsync(ctx->d_pre_rprio, h_rpr, (size_t)R.n_pod * 4, cudaMemcpyHostToDevice, st));
-    if (h_roo && R.n_claim) CU(cudaMemcpyAsync(ctx->d_pre_routoff, h_roo, (size_t)R.n_claim * 4, cudaMemcpyHostToDevice, st));
-    if (R.n_out) CU(cudaMemcpyAsync(ctx->d_pre_rout, h_ro, (size_t)R.n_out * 8, cudaMemcpyHostToDevice, st));
+    if ((rc = grow_set(ctx, ctx->cap_pre_rclaims, (size_t)R.n_claim + 8, ctx->d_pre_rclaims, ctx->d_pre_routoff)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_rpods, (size_t)R.n_pod + 8, ctx->d_pre_rpodoff, ctx->d_pre_rprio, ctx->d_pre_rrec, ctx->d_pre_vlist)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_rout, (size_t)R.n_out + 8, ctx->d_pre_rout))) return rc;
+    s.add(ctx->d_pre_rclaims, R.claims, (size_t)R.n_claim * 16);
+    s.add(ctx->d_pre_rpodoff, R.pod_off, ((size_t)R.n_pod + 1) * 4);
+    s.add(ctx->d_pre_rprio, R.prio, (size_t)R.n_pod * 4);
+    s.add(ctx->d_pre_routoff, R.out_off, R.out_off ? (size_t)R.n_claim * 4 : 0);
+    s.add(ctx->d_pre_rout, R.out, (size_t)R.n_out * 8);
     dev = R;
     dev.claims = (const dra_claim_rec*)ctx->d_pre_rclaims; dev.pod_off = ctx->d_pre_rpodoff;
     dev.prio = (const int32_t*)ctx->d_pre_rprio; dev.out_off = R.out_off ? ctx->d_pre_routoff : nullptr;
     dev.out = (const dra_out_rec*)ctx->d_pre_rout;
     return DRA_OK;
+}
+
+// pair -> pod of the candidate form: pair_pod[k] = q for every k in [cand_off[q], cand_off[q + 1])
+void expand_pairs(uint32_t* pair_pod, const uint32_t* cand_off, uint32_t n_pod) {
+    for (uint32_t q = 0; q < n_pod; ++q)
+        for (uint32_t k = cand_off[q]; k < cand_off[q + 1]; ++k) pair_pod[k] = q;
+}
+
+// One output of a synchronous call: bytes from the device at src to the caller's dst
+struct ReadBack { void* dst; const void* src; size_t bytes; };
+using Outputs = std::initializer_list<ReadBack>;
+
+size_t out_bytes(Outputs outs) {
+    size_t total = 0;
+    for (const ReadBack& o : outs) total += al16(o.bytes);
+    return total;
+}
+
+// The pinned h_out for outs, grown before the call enqueues anything: a failed allocation leaves the inventory as it was
+int reserve_out(dra_ctx* ctx, Outputs outs) { return grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, out_bytes(outs)); }
+
+// The tail of a synchronous call: the outputs into h_out (reserve_out), one synchronise, the launch error as DRA_E_CUDA
+// "<name>: ...", the times of n_marks stages, the device's fault words; the caller's buffers are written only when all passed
+int read_back(dra_ctx* ctx, const char* name, int n_marks, Outputs outs) {
+    if (out_bytes(outs) > ctx->h_out_cap) return fail(ctx, DRA_E_STATE, "%s: outputs not reserved before the launch", name);
+    uint8_t* h = ctx->h_out;
+    for (const ReadBack& o : outs) {
+        if (o.bytes) CU(cudaMemcpyAsync(h, o.src, o.bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        h += al16(o.bytes);
+    }
+    CU(cudaStreamSynchronize(ctx->stream));
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "%s: %s", name, cudaGetErrorString(e));
+    collect_timings(ctx, n_marks);
+    if (int rc = check_err(ctx)) return rc;
+    h = ctx->h_out;
+    for (const ReadBack& o : outs) {
+        if (o.bytes) memcpy(o.dst, h, o.bytes);
+        h += al16(o.bytes);
+    }
+    return DRA_OK;
+}
+
+// The pending pods' pod_off [n_pod + 1]: spans [0, n_claim] and is monotone
+int check_pod_off(dra_ctx* ctx, const uint32_t* pod_off, uint32_t n_pod, uint32_t n_claim) {
+    if (pod_off[0] != 0 || pod_off[n_pod] != n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]");
+    for (uint32_t q = 0; q < n_pod; ++q)
+        if (pod_off[q + 1] < pod_off[q]) return fail(ctx, DRA_E_INVAL, "pod_off not monotone at pod %u", q);
+    return DRA_OK;
+}
+
+// The pending pods' candidates: the dense form (cand_nodes and cand_off both NULL: every pod against every node), or
+// cand_off [n_pod + 1] from 0 and monotone with at most per_pod candidates a pod, and cand_nodes when it lists any.
+// n_pair: the pairs, n_pod * dense_nodes in the dense form; more than max_pairs fails.
+int check_cands(dra_ctx* ctx, uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, uint32_t per_pod,
+                uint32_t dense_nodes, uint64_t max_pairs, bool& dense, uint32_t& n_pair) {
+    dense = cand_nodes == nullptr && cand_off == nullptr;
+    if (!dense && !cand_off) return fail(ctx, DRA_E_INVAL, "cand_nodes without cand_off");
+    if (!dense && cand_off[0] != 0) return fail(ctx, DRA_E_INVAL, "cand_off[0] must be 0");
+    for (uint32_t q = 0; !dense && q < n_pod; ++q) {
+        if (cand_off[q + 1] < cand_off[q]) return fail(ctx, DRA_E_INVAL, "cand_off not monotone at pod %u", q);
+        if (cand_off[q + 1] - cand_off[q] > per_pod) return fail(ctx, DRA_E_INVAL, "pod %u has more than %u candidates", q, per_pod);
+    }
+    const uint64_t n = dense ? (uint64_t)n_pod * dense_nodes : cand_off[n_pod];
+    if (n > max_pairs) return fail(ctx, DRA_E_INVAL, "%llu (pod, node) pairs: more than %llu", (unsigned long long)n, (unsigned long long)max_pairs);
+    n_pair = (uint32_t)n;
+    if (n_pair && !dense && !cand_nodes) return fail(ctx, DRA_E_INVAL, "cand_off lists candidates but cand_nodes is NULL");
+    return DRA_OK;
+}
+
+// Spec §13's slots: n_out >= n_claim without out_off, and each claim's OutRec slots within n_out as if the claim named a
+// node of the inventory
+int check_place_slots(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* out_off, uint32_t n_out) {
+    if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    for (uint32_t i = 0; i < n_claim; ++i) {
+        const dra_claim_rec& c = claims[i];
+        const bool gpu = c.kind == DRA_KIND_GPU && c.count >= 1 && c.count <= DRA_MAX_COUNT && (out_off || c.count == 1);
+        const uint32_t slots = gpu ? c.count : 1u, dst = out_off ? out_off[i] : i;
+        if (dst > n_out || slots > n_out - dst) return fail(ctx, DRA_E_INVAL, "claim %u: slots [%u, %u) outside n_out %u", i, dst, dst + slots, n_out);
+    }
+    return DRA_OK;
+}
+
+// A persistent walk k over the inventory's nodes (none: no launch): CTAs of 4 warps, one per 4 nodes up to all that can be
+// resident at once (occ per SM, queried once), launched cooperatively so that every one of them is.  Enqueues only.
+template <typename... KA, typename... A>
+int launch_walk(dra_ctx* ctx, int& occ, const char* name, void (*k)(KA...), A&&... args) {
+    if (!ctx->n_node) return DRA_OK;
+    if (occ < 0) {
+        int nb = 0;
+        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, 128, 0));
+        occ = nb;
+    }
+    if (occ < 1) return fail(ctx, DRA_E_CUDA, "%s: no CTA can be resident", name);
+    const uint32_t grid = std::max(1u, std::min((ctx->n_node + 3) / 4, (uint32_t)(occ * ctx->n_sm)));
+    cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
+    lc.gridDim = dim3(grid); lc.blockDim = dim3(128); lc.dynamicSmemBytes = 0; lc.stream = ctx->stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
+    lc.attrs = at; lc.numAttrs = 1;
+    CU(cudaLaunchKernelEx(&lc, k, static_cast<KA>(args)...));
+    ctx->launches += 1;
+    return DRA_OK;
+}
+
+// The grid of a sharded walk over n_walk nodes with every CTA resident (occ per SM).  Not a cooperative launch: ranks
+// sharing this device run their walks side by side, so each takes its share of the residency, less one CTA per SM left
+// for a peer's waiting kernel.
+uint32_t shard_walk_grid(const dra_ctx* ctx, int occ, bool gather, uint32_t n_walk) {
+    const int k = gather ? std::max(1, ctx->peers_on_device) : 1;
+    const int per_sm = k > 1 ? std::max(1, occ - 1) : occ;
+    const uint32_t share = (uint32_t)std::max(1, per_sm * ctx->n_sm / k);
+    return std::max(1u, std::min((n_walk + 3) / 4, share));
 }
 
 // The PreArgs fields every preemption call sets: the pending pods (cand_nodes and cand_off nullptr in the dense form), the
@@ -1394,63 +1486,27 @@ int dra_unsuitable_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     QUIESCE();
     if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_unsuitable_batch: unknown flags 0x%x", flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
-    if (pod_off[0] != 0 || pod_off[n_pod] != n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]");
-    const bool dense = cand_nodes == nullptr && cand_off == nullptr;      // every pod against every node
-    if (!dense && !cand_off) return DRA_E_INVAL;
-    if (!dense && cand_off[0] != 0) return fail(ctx, DRA_E_INVAL, "cand_off[0] must be 0");
-    const uint64_t n_pair64 = dense ? (uint64_t)n_pod * ctx->n_node : cand_off[n_pod];
-    if (n_pair64 > 0xFFFFFFF0ull) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
-    const uint32_t n_pair = (uint32_t)n_pair64;
-    if (n_pair && (!suitable_bits || (!dense && !cand_nodes))) return DRA_E_INVAL;
+    bool dense; uint32_t n_pair;
+    int rc;
+    if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
+        (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, 0xFFFFFFFFu, ctx->n_node, 0xFFFFFFF0ull, dense, n_pair))) return rc;
+    if (n_pair && !suitable_bits) return fail(ctx, DRA_E_INVAL, "suitable_bits is NULL");
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_batch(ctx, n_claim, 1, true);
-    if (rc) return rc;
+    if ((rc = ensure_batch(ctx, n_claim, 1, true))) return rc;
     if ((rc = upload_table(ctx))) return rc;
-    if (n_pod + 8 > ctx->cap_pods) {
-        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_pod_off, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_cand_off, 0, cap))) return rc;
-        ctx->cap_pods = cap;
-    }
     const size_t words = ((size_t)n_pair + 31) / 32;
-    if (!dense && (size_t)n_pair + 64 > ctx->cap_pairs) {
-        size_t cap = (size_t)n_pair + n_pair / 2 + 128;
-        if ((rc = grow_nc(ctx, ctx->d_cand_nodes, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_pair_pod, 0, cap))) return rc;
-        ctx->cap_pairs = cap;
-    }
-    if (words + 8 > ctx->cap_bits_only) {
-        size_t cap = words + words / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_bits, 0, cap))) return rc;
-        ctx->cap_bits_only = cap;
-    }
-    // staging: claims | pod_off | (cand_off | cand_nodes | pair->pod expansion)
-    const size_t stage = (size_t)n_claim * 16 + ((size_t)n_pod + 1) * 8 + (dense ? 0 : (size_t)n_pair * 8) + 64;
-    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, stage))) return rc;
-    uint8_t* p = ctx->h_in;
-    if (n_claim) memcpy(p, claims, (size_t)n_claim * 16);
-    uint8_t* h_claims = p; p += (size_t)n_claim * 16;
-    memcpy(p, pod_off, ((size_t)n_pod + 1) * 4); uint8_t* h_pod = p; p += ((size_t)n_pod + 1) * 4;
-    for (uint32_t q = 0; q < n_pod; ++q)
-        if (pod_off[q + 1] < pod_off[q]) return fail(ctx, DRA_E_INVAL, "pod_off not monotone at pod %u", q);
-    uint8_t *h_cn = nullptr; uint32_t* h_pp = nullptr;
+    if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
+        (!dense && (rc = grow_set(ctx, ctx->cap_pairs, (size_t)n_pair + 64, ctx->d_cand_nodes, ctx->d_pair_pod))) ||
+        (rc = grow_set(ctx, ctx->cap_bits_only, words + 8, ctx->d_bits))) return rc;
+    Staging s;                                            // (cand_off is only needed on the host)
+    s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
+    s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
     if (!dense) {
-        p += ((size_t)n_pod + 1) * 4;                    // (cand_off is only needed on the host)
-        if (n_pair) memcpy(p, cand_nodes, (size_t)n_pair * 4);
-        h_cn = p; p += (size_t)n_pair * 4;
-        h_pp = (uint32_t*)p;
-        for (uint32_t q = 0; q < n_pod; ++q) {
-            if (cand_off[q + 1] < cand_off[q] || cand_off[q + 1] > n_pair) return fail(ctx, DRA_E_INVAL, "cand_off not monotone at pod %u", q);
-            for (uint32_t k = cand_off[q]; k < cand_off[q + 1]; ++k) h_pp[k] = q;
-        }
+        s.add(ctx->d_cand_nodes, cand_nodes, (size_t)n_pair * 4);
+        s.add(ctx->d_pair_pod, nullptr, (size_t)n_pair * 4);
     }
-    if (n_claim) CU(cudaMemcpyAsync(ctx->d_claims, h_claims, (size_t)n_claim * 16, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->d_pod_off, h_pod, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = stage_in(ctx, s, [&](uint8_t* h) { expand_pairs((uint32_t*)h, cand_off, n_pod); }))) return rc;
     if (n_pair) {
-        if (!dense) {
-            CU(cudaMemcpyAsync(ctx->d_cand_nodes, h_cn, (size_t)n_pair * 4, cudaMemcpyHostToDevice, ctx->stream));
-            CU(cudaMemcpyAsync(ctx->d_pair_pod, h_pp, (size_t)n_pair * 4, cudaMemcpyHostToDevice, ctx->stream));
-        }
         CU(cudaMemsetAsync(ctx->d_bits, 0, words * 4, ctx->stream));
         UnsArgs a; memset(&a, 0, sizeof a);
         a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.n_pod = n_pod;
@@ -1465,6 +1521,7 @@ int dra_unsuitable_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
         if ((rc = grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, words * 4))) return rc;
         CU(cudaMemcpyAsync(ctx->h_out, ctx->d_bits, words * 4, cudaMemcpyDeviceToHost, ctx->stream));
     }
+    // k_unsuitable sets no fault word (one left by an earlier enqueue-only call is dra_ctx_sync's to report)
     CU(cudaStreamSynchronize(ctx->stream));
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "k_unsuitable: %s", cudaGetErrorString(e));
@@ -1481,36 +1538,23 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     QUIESCE();
     if (flags & ~(DRA_F_EXHAUSTIVE | DRA_F_FRESH_INVENTORY)) return fail(ctx, DRA_E_INVAL, "dra_allocate_pods_batch: unknown flags 0x%x", flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
-    if (pod_off[0] != 0 || pod_off[n_pod] != n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]");
+    int rc;
+    if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim))) return rc;
     if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
-    for (uint32_t q = 0; q < n_pod; ++q)
-        if (pod_off[q + 1] < pod_off[q]) return fail(ctx, DRA_E_INVAL, "pod_off not monotone at pod %u", q);
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_batch(ctx, std::max(n_claim, n_pod), n_out, true);
-    if (rc) return rc;
+    if ((rc = ensure_batch(ctx, std::max(n_claim, n_pod), n_out, true))) return rc;
     if ((rc = upload_table(ctx))) return rc;
-    if (n_pod + 8 > ctx->cap_pods) {
-        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_pod_off, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_cand_off, 0, cap))) return rc;
-        ctx->cap_pods = cap;
-    }
-    if (n_pod + 8 > ctx->cap_podrec) {
-        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_podrec, 0, cap))) return rc;
-        ctx->cap_podrec = cap;
-    }
-    const size_t cb = (size_t)n_claim * 16, pb = ((size_t)n_pod + 1) * 4, ob = out_off ? (size_t)n_claim * 4 : 0, rb = (size_t)n_out * 8;
-    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + ob))) return rc;
-    if ((rc = grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, rb + 16))) return rc;
-    if (cb) memcpy(ctx->h_in, claims, cb);
-    memcpy(ctx->h_in + cb, pod_off, pb);
-    if (ob) memcpy(ctx->h_in + cb + pb, out_off, ob);
-    if (cb) CU(cudaMemcpyAsync(ctx->d_claims, ctx->h_in, cb, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->d_pod_off, ctx->h_in + cb, pb, cudaMemcpyHostToDevice, ctx->stream));
-    if (ob) CU(cudaMemcpyAsync(ctx->d_out_off, ctx->h_in + cb + pb, ob, cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
+        (rc = grow_set(ctx, ctx->cap_podrec, (size_t)n_pod + 8, ctx->d_podrec))) return rc;
+    const Outputs outs = {{out, ctx->d_out, (size_t)n_out * 8}};
+    if ((rc = reserve_out(ctx, outs))) return rc;
+    Staging s;
+    s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
+    s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
+    if (out_off) s.add(ctx->d_out_off, out_off, (size_t)n_claim * 4);
+    if ((rc = stage_in(ctx, s))) return rc;
     Err err = err_of(ctx);
     Prof prof(ctx);
     uint2* d_out = ctx->d_out;
@@ -1531,13 +1575,8 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
         CU(launch_k(k_pods<4>, dim3(grid), dim3(128), 0, ctx->stream, pdl, a));
         ctx->launches += 1;
     }
-    if (rb) CU(cudaMemcpyAsync(ctx->h_out, d_out, rb, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "pod kernels: %s", cudaGetErrorString(e));
-    if ((rc = check_err(ctx))) return rc;
-    if (rb) memcpy(out, ctx->h_out, rb);
-    return DRA_OK;
+    prof.mark();                                          // the walk: the pack stage of the timings
+    return read_back(ctx, "pod kernels", 4, outs);
 }
 
 // Place pods (spec §13): pod records -> (candidate form) the pair records stably sorted by node with the claim path's
@@ -1550,78 +1589,35 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     QUIESCE();
     if (flags & ~(DRA_F_EXHAUSTIVE | DRA_F_FRESH_INVENTORY)) return fail(ctx, DRA_E_INVAL, "dra_place_pods_batch: unknown flags 0x%x", flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
-    if (pod_off[0] != 0 || pod_off[n_pod] != n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]");
-    for (uint32_t q = 0; q < n_pod; ++q)
-        if (pod_off[q + 1] < pod_off[q]) return fail(ctx, DRA_E_INVAL, "pod_off not monotone at pod %u", q);
-    const bool dense = cand_nodes == nullptr && cand_off == nullptr;      // every pod against every node, ascending
-    if (!dense && !cand_off) return fail(ctx, DRA_E_INVAL, "cand_nodes without cand_off");
-    if (!dense && cand_off[0] != 0) return fail(ctx, DRA_E_INVAL, "cand_off[0] must be 0");
-    for (uint32_t q = 0; !dense && q < n_pod; ++q) {
-        if (cand_off[q + 1] < cand_off[q]) return fail(ctx, DRA_E_INVAL, "cand_off not monotone at pod %u", q);
-        if (cand_off[q + 1] - cand_off[q] > PL_POS) return fail(ctx, DRA_E_INVAL, "pod %u has more than %u candidates", q, PL_POS);
-    }
-    const uint32_t n_pair = dense ? 0u : cand_off[n_pod];
-    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
-    if (n_pair && !cand_nodes) return fail(ctx, DRA_E_INVAL, "cand_off lists candidates but cand_nodes is NULL");
+    bool dense; uint32_t n_pair;                          // the dense form walks every node, ascending: no pair records
+    int rc;
+    if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
+        (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, PL_POS, 0, 0xFFFFFFF0ull, dense, n_pair))) return rc;
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
-    if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
-    for (uint32_t i = 0; i < n_claim; ++i) {                              // slots as if the claim named a node of the inventory
-        const dra_claim_rec& c = claims[i];
-        const bool gpu = c.kind == DRA_KIND_GPU && c.count >= 1 && c.count <= DRA_MAX_COUNT && (out_off || c.count == 1);
-        const uint32_t slots = gpu ? c.count : 1u, dst = out_off ? out_off[i] : i;
-        if (dst > n_out || slots > n_out - dst) return fail(ctx, DRA_E_INVAL, "claim %u: slots [%u, %u) outside n_out %u", i, dst, dst + slots, n_out);
-    }
+    if ((rc = check_place_slots(ctx, claims, n_claim, out_off, n_out))) return rc;
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "dra_place_pods_batch needs cooperative launches, which this device does not offer");
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_batch(ctx, std::max(std::max(n_claim, n_pod), n_pair), n_out, true);
-    if (rc) return rc;
+    if ((rc = ensure_batch(ctx, std::max(std::max(n_claim, n_pod), n_pair), n_out, true))) return rc;
     if ((rc = upload_table(ctx))) return rc;
-    if (n_pod + 8 > ctx->cap_pods) {
-        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_pod_off, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_cand_off, 0, cap))) return rc;
-        ctx->cap_pods = cap;
+    if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
+        (rc = grow_set(ctx, ctx->cap_pairs, (size_t)n_pair + 64, ctx->d_cand_nodes, ctx->d_pair_pod)) ||
+        (rc = grow_set(ctx, ctx->cap_podrec, (size_t)n_pair + 8, ctx->d_podrec)) ||
+        (rc = grow_set(ctx, ctx->cap_place_pods, (size_t)n_pod + 8, ctx->d_place_state, ctx->d_place_node)) ||
+        (rc = grow_set(ctx, ctx->cap_place_cursor, (size_t)ctx->n_node + 8, ctx->d_place_cursor))) return rc;
+    const size_t rb = (size_t)n_out * 8;
+    const Outputs outs = {{out, ctx->d_out, rb}, {pod_node, ctx->d_place_node, (size_t)n_pod * 4}};
+    if ((rc = reserve_out(ctx, outs))) return rc;
+    Staging s;
+    s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
+    s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
+    if (out_off) s.add(ctx->d_out_off, out_off, (size_t)n_claim * 4);
+    if (!dense) {
+        s.add(ctx->d_cand_off, cand_off, ((size_t)n_pod + 1) * 4);
+        s.add(ctx->d_cand_nodes, cand_nodes, (size_t)n_pair * 4);
     }
-    if ((size_t)n_pair + 64 > ctx->cap_pairs) {
-        size_t cap = (size_t)n_pair + n_pair / 2 + 128;
-        if ((rc = grow_nc(ctx, ctx->d_cand_nodes, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_pair_pod, 0, cap))) return rc;
-        ctx->cap_pairs = cap;
-    }
-    if ((size_t)n_pair + 8 > ctx->cap_podrec) {
-        size_t cap = (size_t)n_pair + n_pair / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_podrec, 0, cap))) return rc;
-        ctx->cap_podrec = cap;
-    }
-    if ((size_t)n_pod + 8 > ctx->cap_place_pods) {
-        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_place_state, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_place_node, 0, cap))) return rc;
-        ctx->cap_place_pods = cap;
-    }
-    if ((size_t)ctx->n_node + 8 > ctx->cap_place_cursor) {
-        size_t cap = (size_t)ctx->n_node + ctx->n_node / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_place_cursor, 0, cap))) return rc;
-        ctx->cap_place_cursor = cap;
-    }
-    // staging: claims | pod_off | out_off | cand_off | cand_nodes
-    const size_t cb = (size_t)n_claim * 16, pb = ((size_t)n_pod + 1) * 4, ob = out_off ? (size_t)n_claim * 4 : 0;
-    const size_t kb = dense ? 0 : ((size_t)n_pod + 1) * 4, nb = (size_t)n_pair * 4, rb = (size_t)n_out * 8, qb = (size_t)n_pod * 4;
-    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + ob + kb + nb + 16))) return rc;
-    if ((rc = grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, rb + qb + 16))) return rc;
-    uint8_t* h = ctx->h_in;
-    if (cb) memcpy(h, claims, cb);
-    memcpy(h + cb, pod_off, pb);
-    if (ob) memcpy(h + cb + pb, out_off, ob);
-    if (kb) memcpy(h + cb + pb + ob, cand_off, kb);
-    if (nb) memcpy(h + cb + pb + ob + kb, cand_nodes, nb);
-    if (cb) CU(cudaMemcpyAsync(ctx->d_claims, h, cb, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->d_pod_off, h + cb, pb, cudaMemcpyHostToDevice, ctx->stream));
-    if (ob) CU(cudaMemcpyAsync(ctx->d_out_off, h + cb + pb, ob, cudaMemcpyHostToDevice, ctx->stream));
-    if (kb) CU(cudaMemcpyAsync(ctx->d_cand_off, h + cb + pb + ob, kb, cudaMemcpyHostToDevice, ctx->stream));
-    if (nb) CU(cudaMemcpyAsync(ctx->d_cand_nodes, h + cb + pb + ob + kb, nb, cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = stage_in(ctx, s))) return rc;
     if (rb) CU(cudaMemsetAsync(ctx->d_out, 0, rb, ctx->stream));
     CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)ctx->n_node + 1) * 4, ctx->stream));
     Prof prof(ctx);
@@ -1639,33 +1635,10 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     if (!dense && n_pair &&
         (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, a.inv_src, false, ctx->n_node, ctx->d_node_off)))
         return rc;
-    if (ctx->n_node) {
-        if (ctx->place_occ < 0) {
-            int occ = 0;
-            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_place<4>, 128, 0));
-            ctx->place_occ = occ;
-        }
-        if (ctx->place_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_place: no CTA can be resident");
-        const uint32_t grid = std::max(1u, std::min((ctx->n_node + 3) / 4, (uint32_t)(ctx->place_occ * ctx->n_sm)));
-        cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
-        lc.gridDim = dim3(grid); lc.blockDim = dim3(128); lc.dynamicSmemBytes = 0; lc.stream = ctx->stream;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
-        lc.attrs = at; lc.numAttrs = 1;
-        CU(cudaLaunchKernelEx(&lc, k_pods_place<4>, a, PlaceShard{}));
-        ctx->launches += 1;
-    }
+    if ((rc = launch_walk(ctx, ctx->place_occ, "k_pods_place", k_pods_place<4>, a, PlaceShard{}))) return rc;
     ctx->chain |= DRA_K_PLACE;
     prof.mark();
-    if (rb) CU(cudaMemcpyAsync(ctx->h_out, ctx->d_out, rb, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->h_out + rb, ctx->d_place_node, qb, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "place kernels: %s", cudaGetErrorString(e));
-    if ((rc = check_err(ctx))) return rc;
-    if (rb) memcpy(out, ctx->h_out, rb);
-    memcpy(pod_node, ctx->h_out + rb, qb);
-    return DRA_OK;
+    return read_back(ctx, "place kernels", 4, outs);
 }
 
 // Preemption (spec §14): the pending-pod arrays are checked here; the running pods on the device (k_pre_running), whose
@@ -1683,83 +1656,40 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
     if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_preempt_batch: unknown flags 0x%x", flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     if (max_victims && !victims) return fail(ctx, DRA_E_INVAL, "max_victims %u without a victims buffer", max_victims);
-    if (pod_off[0] != 0 || pod_off[n_pod] != n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]");
-    for (uint32_t q = 0; q < n_pod; ++q)
-        if (pod_off[q + 1] < pod_off[q]) return fail(ctx, DRA_E_INVAL, "pod_off not monotone at pod %u", q);
-    const bool dense = cand_nodes == nullptr && cand_off == nullptr;
-    if (!dense && !cand_off) return fail(ctx, DRA_E_INVAL, "cand_nodes without cand_off");
-    if (!dense && cand_off[0] != 0) return fail(ctx, DRA_E_INVAL, "cand_off[0] must be 0");
-    for (uint32_t q = 0; !dense && q < n_pod; ++q)
-        if (cand_off[q + 1] < cand_off[q]) return fail(ctx, DRA_E_INVAL, "cand_off not monotone at pod %u", q);
-    const uint64_t n_pair64 = dense ? (uint64_t)n_pod * ctx->n_node : cand_off[n_pod];
-    if (dense && n_pair64 >= (1ull << 32)) return fail(ctx, DRA_E_INVAL, "dense form: n_pod * n_node must stay below 2^32");
-    const uint32_t n_pair = (uint32_t)n_pair64;
-    if (n_pair && !dense && !cand_nodes) return fail(ctx, DRA_E_INVAL, "cand_off lists candidates but cand_nodes is NULL");
+    bool dense; uint32_t n_pair;
+    int rc;
+    if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
+        (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, 0xFFFFFFFFu, ctx->n_node, 0xFFFFFFFFull, dense, n_pair))) return rc;
     ctx->chain = DRA_K_PREEMPT; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_batch(ctx, std::max(n_claim, R.n_pod), 1, true);
-    if (rc) return rc;
+    if ((rc = ensure_batch(ctx, std::max(n_claim, R.n_pod), 1, true))) return rc;
     if ((rc = upload_table(ctx))) return rc;
-    if (n_pod + 8 > ctx->cap_pods) {
-        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_pod_off, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_cand_off, 0, cap))) return rc;
-        ctx->cap_pods = cap;
-    }
-    if (!dense && (size_t)n_pair + 64 > ctx->cap_pairs) {
-        size_t cap = (size_t)n_pair + n_pair / 2 + 128;
-        if ((rc = grow_nc(ctx, ctx->d_cand_nodes, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_pair_pod, 0, cap))) return rc;
-        ctx->cap_pairs = cap;
-    }
-    if ((size_t)n_pod + 8 > ctx->cap_pre_pods) {
-        const size_t need = (size_t)n_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_prio, need)) || (rc = grow_pre(ctx, ctx->d_pre_node, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_nvic, need)) || (rc = grow_pre(ctx, ctx->d_pre_choice, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_pst, need))) return rc;
-        ctx->cap_pre_pods = need + need / 2 + 64;
-    }
-    if ((size_t)n_pair + 8 > ctx->cap_pre_pairs) {
-        const size_t need = (size_t)n_pair + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_psum, need)) || (rc = grow_pre(ctx, ctx->d_pre_psum64, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_pairst, need)) || (rc = grow_pre(ctx, ctx->d_pre_pairvic, need))) return rc;
-        ctx->cap_pre_pairs = need + need / 2 + 64;
-    }
     const size_t vb = (size_t)n_pod * max_victims * 4;
-    if (vb / 4 + 8 > ctx->cap_pre_vic) {
-        const size_t need = vb / 4 + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_vic, need))) return rc;
-        ctx->cap_pre_vic = need + need / 2 + 64;
-    }
-    // staging: claims | pod_off | prio | cand_off | cand_nodes | pair -> pod | the running pods
-    auto al = al16;
-    const size_t cb = al((size_t)n_claim * 16), pb = al(((size_t)n_pod + 1) * 4), prb = al((size_t)n_pod * 4);
-    const size_t kb = dense ? 0 : al(((size_t)n_pod + 1) * 4), nb = dense ? 0 : al((size_t)n_pair * 4);
-    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + prb + kb + 2 * nb + running_room(R) + 16))) return rc;
-    uint8_t* h = ctx->h_in;
-    auto put = [&](const void* src, size_t bytes, size_t room) { uint8_t* d = h; if (bytes) memcpy(d, src, bytes); h += room; return d; };
-    uint8_t* h_c = put(claims, (size_t)n_claim * 16, cb);
-    uint8_t* h_po = put(pod_off, ((size_t)n_pod + 1) * 4, pb);
-    uint8_t* h_pr = put(prio, (size_t)n_pod * 4, prb);
-    uint8_t* h_co = dense ? nullptr : put(cand_off, ((size_t)n_pod + 1) * 4, kb);
-    uint8_t* h_cn = dense ? nullptr : put(cand_nodes, (size_t)n_pair * 4, nb);
-    uint8_t* h_pp = dense ? nullptr : put(nullptr, 0, nb);
-    for (uint32_t q = 0; !dense && q < n_pod; ++q)
-        for (uint32_t k = cand_off[q]; k < cand_off[q + 1]; ++k) ((uint32_t*)h_pp)[k] = q;
-    cudaStream_t st = ctx->stream;
-    if (n_claim) CU(cudaMemcpyAsync(ctx->d_claims, h_c, (size_t)n_claim * 16, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pod_off, h_po, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pre_prio, h_pr, (size_t)n_pod * 4, cudaMemcpyHostToDevice, st));
+    if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
+        (!dense && (rc = grow_set(ctx, ctx->cap_pairs, (size_t)n_pair + 64, ctx->d_cand_nodes, ctx->d_pair_pod))) ||
+        (rc = grow_set(ctx, ctx->cap_pre_pods, (size_t)n_pod + 8, ctx->d_pre_prio, ctx->d_pre_node, ctx->d_pre_nvic, ctx->d_pre_choice, ctx->d_pre_pst)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_pairs, (size_t)n_pair + 8, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_vic, vb / 4 + 8, ctx->d_pre_vic))) return rc;
+    const Outputs outs = {{pair_status, ctx->d_pre_pairst, pair_status ? (size_t)n_pair : 0},
+                          {pair_victims, ctx->d_pre_pairvic, pair_victims ? (size_t)n_pair * 4 : 0},
+                          {pod_node, ctx->d_pre_node, (size_t)n_pod * 4},
+                          {pod_status, ctx->d_pre_pst, n_pod},
+                          {n_victims, ctx->d_pre_nvic, (size_t)n_pod * 4},
+                          {victims, ctx->d_pre_vic, vb}};
+    if ((rc = reserve_out(ctx, outs))) return rc;
+    Staging s;
+    s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
+    s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
+    s.add(ctx->d_pre_prio, prio, (size_t)n_pod * 4);
     if (!dense) {
-        CU(cudaMemcpyAsync(ctx->d_cand_off, h_co, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
-        if (n_pair) {
-            CU(cudaMemcpyAsync(ctx->d_cand_nodes, h_cn, (size_t)n_pair * 4, cudaMemcpyHostToDevice, st));
-            CU(cudaMemcpyAsync(ctx->d_pair_pod, h_pp, (size_t)n_pair * 4, cudaMemcpyHostToDevice, st));
-        }
+        s.add(ctx->d_cand_off, cand_off, ((size_t)n_pod + 1) * 4);
+        s.add(ctx->d_cand_nodes, cand_nodes, (size_t)n_pair * 4);
+        s.add(ctx->d_pair_pod, nullptr, (size_t)n_pair * 4);
     }
     dra_running_pods Rd;
-    if ((rc = upload_running(ctx, R, h, Rd))) return rc;
+    if ((rc = running_parts(ctx, R, s, Rd)) ||
+        (rc = stage_in(ctx, s, [&](uint8_t* h) { expand_pairs((uint32_t*)h, cand_off, n_pod); }))) return rc;
 
     PreArgs a = pre_args(ctx, ctx->d_claims, ctx->d_pod_off, (const int32_t*)ctx->d_pre_prio, n_pod, dense ? nullptr : ctx->d_cand_nodes,
                          dense ? nullptr : ctx->d_cand_off, n_pair, Rd, ctx->d_inv_live, flags);
@@ -1770,6 +1700,7 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
     if ((rc = launch_running_lists(ctx, a, prof, false))) return rc;
     const PreShard whole{0u, ctx->n_node, n_pair, 0u, nullptr, nullptr};
     if ((rc = launch_preempt_pairs(ctx, a, whole))) return rc;
+    cudaStream_t st = ctx->stream;
     k_pre_choose<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a);
     ctx->launches += 1;
     if (max_victims) {
@@ -1777,30 +1708,7 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
         launch_preempt_victims(ctx, a, ctx->d_pre_choice, 1u, ctx->d_pre_vic, max_victims);
     }
     prof.mark();
-    // outputs: pair_status | pair_victims | pod_node | pod_status | n_victims | victims
-    const size_t osb = pair_status ? al(n_pair) : 0, ovb = pair_victims ? al((size_t)n_pair * 4) : 0;
-    const size_t onb = al((size_t)n_pod * 4), opb = al(n_pod), ocb = al((size_t)n_pod * 4);
-    if ((rc = grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, osb + ovb + onb + opb + ocb + vb + 16))) return rc;
-    uint8_t* o = ctx->h_out;
-    if (osb && n_pair) CU(cudaMemcpyAsync(o, ctx->d_pre_pairst, n_pair, cudaMemcpyDeviceToHost, st));
-    if (ovb && n_pair) CU(cudaMemcpyAsync(o + osb, ctx->d_pre_pairvic, (size_t)n_pair * 4, cudaMemcpyDeviceToHost, st));
-    uint8_t* o2 = o + osb + ovb;
-    CU(cudaMemcpyAsync(o2, ctx->d_pre_node, (size_t)n_pod * 4, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(o2 + onb, ctx->d_pre_pst, n_pod, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(o2 + onb + opb, ctx->d_pre_nvic, (size_t)n_pod * 4, cudaMemcpyDeviceToHost, st));
-    if (vb) CU(cudaMemcpyAsync(o2 + onb + opb + ocb, ctx->d_pre_vic, vb, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "preemption kernels: %s", cudaGetErrorString(e));
-    collect_timings(ctx, 1);
-    if ((rc = check_err(ctx))) return rc;
-    if (pair_status && n_pair) memcpy(pair_status, o, n_pair);
-    if (pair_victims && n_pair) memcpy(pair_victims, o + osb, (size_t)n_pair * 4);
-    memcpy(pod_node, o2, (size_t)n_pod * 4);
-    memcpy(pod_status, o2 + onb, n_pod);
-    memcpy(n_victims, o2 + onb + opb, (size_t)n_pod * 4);
-    if (vb) memcpy(victims, o2 + onb + opb + ocb, vb);
-    return DRA_OK;
+    return read_back(ctx, "preemption kernels", 1, outs);
 }
 
 // Preempt and place (spec §15): the pending-pod arrays are checked here, the running pods on the device (k_pre_running),
@@ -1820,74 +1728,38 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     QUIESCE();
     if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_preempt_place_batch: unknown flags 0x%x", flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
-    if (pod_off[0] != 0 || pod_off[n_pod] != n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]");
-    for (uint32_t q = 0; q < n_pod; ++q)
-        if (pod_off[q + 1] < pod_off[q]) return fail(ctx, DRA_E_INVAL, "pod_off not monotone at pod %u", q);
-    const bool dense = cand_nodes == nullptr && cand_off == nullptr;
-    if (!dense && !cand_off) return fail(ctx, DRA_E_INVAL, "cand_nodes without cand_off");
-    if (!dense && cand_off[0] != 0) return fail(ctx, DRA_E_INVAL, "cand_off[0] must be 0");
-    for (uint32_t q = 0; !dense && q < n_pod; ++q) {
-        if (cand_off[q + 1] < cand_off[q]) return fail(ctx, DRA_E_INVAL, "cand_off not monotone at pod %u", q);
-        if (cand_off[q + 1] - cand_off[q] > PL_POS) return fail(ctx, DRA_E_INVAL, "pod %u has more than %u candidates", q, PL_POS);
-    }
-    const uint64_t n_pair64 = dense ? (uint64_t)n_pod * ctx->n_node : cand_off[n_pod];
-    if (dense && n_pair64 >= (1ull << 32)) return fail(ctx, DRA_E_INVAL, "dense form: n_pod * n_node must stay below 2^32");
-    const uint32_t n_pair = (uint32_t)n_pair64;
-    if (!dense && n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
-    if (n_pair && !dense && !cand_nodes) return fail(ctx, DRA_E_INVAL, "cand_off lists candidates but cand_nodes is NULL");
+    bool dense; uint32_t n_pair;
+    int rc;
+    if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
+        (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, PL_POS, ctx->n_node, 0xFFFFFFFFull, dense, n_pair))) return rc;
+    if (!dense && n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");   // (the dense form: below 2^32)
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
-    if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
-    for (uint32_t i = 0; i < n_claim; ++i) {                              // slots as if the claim named a node of the inventory
-        const dra_claim_rec& c = claims[i];
-        const bool gpu = c.kind == DRA_KIND_GPU && c.count >= 1 && c.count <= DRA_MAX_COUNT && (out_off || c.count == 1);
-        const uint32_t slots = gpu ? c.count : 1u, dst = out_off ? out_off[i] : i;
-        if (dst > n_out || slots > n_out - dst) return fail(ctx, DRA_E_INVAL, "claim %u: slots [%u, %u) outside n_out %u", i, dst, dst + slots, n_out);
-    }
+    if ((rc = check_place_slots(ctx, claims, n_claim, out_off, n_out))) return rc;
     ctx->chain = DRA_K_PREEMPT_PLACE; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "dra_preempt_place_batch needs cooperative launches, which this device does not offer");
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_batch(ctx, std::max(std::max(n_claim, R.n_pod), n_pair), n_out, true);
-    if (rc) return rc;
+    if ((rc = ensure_batch(ctx, std::max(std::max(n_claim, R.n_pod), n_pair), n_out, true))) return rc;
     if ((rc = upload_table(ctx))) return rc;
-    if (n_pod + 8 > ctx->cap_pods) {
-        size_t cap = (size_t)n_pod + n_pod / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_pod_off, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_cand_off, 0, cap))) return rc;
-        ctx->cap_pods = cap;
-    }
-    if (!dense && (size_t)n_pair + 64 > ctx->cap_pairs) {
-        size_t cap = (size_t)n_pair + n_pair / 2 + 128;
-        if ((rc = grow_nc(ctx, ctx->d_cand_nodes, 0, cap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_pair_pod, 0, cap))) return rc;
-        ctx->cap_pairs = cap;
-    }
-    if ((rc = pp_buffers(ctx, n_pod, n_pair, R.n_pod))) return rc;
-    // staging: claims | pod_off | out_off | prio | cand_off | cand_nodes | the running pods
-    auto al = al16;
-    const size_t cb = al((size_t)n_claim * 16), pb = al(((size_t)n_pod + 1) * 4), ob = out_off ? al((size_t)n_claim * 4) : 0;
-    const size_t prb = al((size_t)n_pod * 4), kb = dense ? 0 : al(((size_t)n_pod + 1) * 4), nb = dense ? 0 : al((size_t)n_pair * 4);
-    if ((rc = grow_pinned(ctx, ctx->h_in, ctx->h_in_cap, cb + pb + ob + prb + kb + nb + running_room(R) + 16))) return rc;
-    uint8_t* h = ctx->h_in;
-    auto put = [&](const void* src, size_t bytes, size_t room) { uint8_t* d = h; if (bytes) memcpy(d, src, bytes); h += room; return d; };
-    uint8_t* h_c = put(claims, (size_t)n_claim * 16, cb);
-    uint8_t* h_po = put(pod_off, ((size_t)n_pod + 1) * 4, pb);
-    uint8_t* h_oo = out_off ? put(out_off, (size_t)n_claim * 4, ob) : nullptr;
-    uint8_t* h_pr = put(prio, (size_t)n_pod * 4, prb);
-    uint8_t* h_co = dense ? nullptr : put(cand_off, ((size_t)n_pod + 1) * 4, kb);
-    uint8_t* h_cn = dense ? nullptr : put(cand_nodes, (size_t)n_pair * 4, nb);
-    cudaStream_t st = ctx->stream;
-    if (n_claim) CU(cudaMemcpyAsync(ctx->d_claims, h_c, (size_t)n_claim * 16, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pod_off, h_po, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (h_oo && n_claim) CU(cudaMemcpyAsync(ctx->d_out_off, h_oo, (size_t)n_claim * 4, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pre_prio, h_pr, (size_t)n_pod * 4, cudaMemcpyHostToDevice, st));
+    if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
+        (!dense && (rc = grow_set(ctx, ctx->cap_pairs, (size_t)n_pair + 64, ctx->d_cand_nodes, ctx->d_pair_pod))) ||
+        (rc = pp_buffers(ctx, n_pod, n_pair, R.n_pod))) return rc;
+    const size_t rb = (size_t)n_out * 8;
+    const Outputs outs = {{out, ctx->d_out, rb}, {pod_node, ctx->d_pre_node, (size_t)n_pod * 4}, {pod_status, ctx->d_pre_pst, n_pod},
+                          {evicted_by, ctx->d_pp_evicted, (size_t)R.n_pod * 4}};
+    if ((rc = reserve_out(ctx, outs))) return rc;
+    Staging s;
+    s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
+    s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
+    if (out_off) s.add(ctx->d_out_off, out_off, (size_t)n_claim * 4);
+    s.add(ctx->d_pre_prio, prio, (size_t)n_pod * 4);
     if (!dense) {
-        CU(cudaMemcpyAsync(ctx->d_cand_off, h_co, ((size_t)n_pod + 1) * 4, cudaMemcpyHostToDevice, st));
-        if (n_pair) CU(cudaMemcpyAsync(ctx->d_cand_nodes, h_cn, (size_t)n_pair * 4, cudaMemcpyHostToDevice, st));
+        s.add(ctx->d_cand_off, cand_off, ((size_t)n_pod + 1) * 4);
+        s.add(ctx->d_cand_nodes, cand_nodes, (size_t)n_pair * 4);
     }
     dra_running_pods Rd;
-    if ((rc = upload_running(ctx, R, h, Rd))) return rc;
-    const size_t rb = (size_t)n_out * 8;
+    if ((rc = running_parts(ctx, R, s, Rd)) || (rc = stage_in(ctx, s))) return rc;
+    cudaStream_t st = ctx->stream;
     if (rb) CU(cudaMemsetAsync(ctx->d_out, 0, rb, st));
     CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)ctx->n_node + 1) * 4, st));
     CU(cudaMemsetAsync(ctx->d_pp_judged, 0, ((size_t)ctx->n_node + 1) * 4, st));
@@ -1912,43 +1784,10 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     if (!dense && n_pair &&
         (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, ctx->n_node, ctx->d_node_off)))
         return rc;
-    if (ctx->n_node) {
-        if (ctx->pp_occ < 0) {
-            int occ = 0;
-            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_preempt_place<4>, 128, 0));
-            ctx->pp_occ = occ;
-        }
-        if (ctx->pp_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_preempt_place: no CTA can be resident");
-        const uint32_t grid = std::max(1u, std::min((ctx->n_node + 3) / 4, (uint32_t)(ctx->pp_occ * ctx->n_sm)));
-        cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
-        lc.gridDim = dim3(grid); lc.blockDim = dim3(128); lc.dynamicSmemBytes = 0; lc.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
-        lc.attrs = at; lc.numAttrs = 1;
-        CU(cudaLaunchKernelEx(&lc, k_pods_preempt_place<4>, a, pl, pp));
-        ctx->launches += 1;
-    }
+    if ((rc = launch_walk(ctx, ctx->pp_occ, "k_pods_preempt_place", k_pods_preempt_place<4>, a, pl, pp))) return rc;
     ctx->chain |= DRA_K_PREEMPT_PLACE;
     prof.mark();
-    // outputs: out | pod_node | pod_status | evicted_by
-    const size_t onb = al((size_t)n_pod * 4), opb = al(n_pod), oeb = (size_t)R.n_pod * 4;
-    if ((rc = grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, al(rb) + onb + opb + oeb + 16))) return rc;
-    uint8_t* o = ctx->h_out;
-    uint8_t* o2 = o + al(rb);
-    if (rb) CU(cudaMemcpyAsync(o, ctx->d_out, rb, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(o2, ctx->d_pre_node, (size_t)n_pod * 4, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(o2 + onb, ctx->d_pre_pst, n_pod, cudaMemcpyDeviceToHost, st));
-    if (oeb) CU(cudaMemcpyAsync(o2 + onb + opb, ctx->d_pp_evicted, oeb, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "preempt-and-place kernels: %s", cudaGetErrorString(e));
-    collect_timings(ctx, 1);
-    if ((rc = check_err(ctx))) return rc;
-    if (rb) memcpy(out, o, rb);
-    memcpy(pod_node, o2, (size_t)n_pod * 4);
-    memcpy(pod_status, o2 + onb, n_pod);
-    if (oeb) memcpy(evicted_by, o2 + onb + opb, oeb);
-    return DRA_OK;
+    return read_back(ctx, "preempt-and-place kernels", 1, outs);
 }
 
 int dra_deallocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* out_off,
@@ -2098,18 +1937,8 @@ int spre_buffers(dra_ctx* ctx, uint32_t n_pod, uint32_t n_pair, uint32_t max_vic
     int rc;
     if ((rc = grow(ctx, ctx->d_spre_part, ctx->cap_spre_part, spre_units(n_pod, n_pair, max_victims)))) return rc;
     if ((rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, std::max(n_pair, 1u)))) return rc;
-    if ((size_t)n_pair + 8 > ctx->cap_pre_pairs) {
-        const size_t need = (size_t)n_pair + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_psum, need)) || (rc = grow_pre(ctx, ctx->d_pre_psum64, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_pairst, need)) || (rc = grow_pre(ctx, ctx->d_pre_pairvic, need))) return rc;
-        ctx->cap_pre_pairs = need + need / 2 + 64;
-    }
-    if ((size_t)rn_pod + 8 > ctx->cap_pre_rpods) {
-        const size_t need = (size_t)rn_pod + 8;
-        if ((rc = grow_pre(ctx, ctx->d_pre_rpodoff, need)) || (rc = grow_pre(ctx, ctx->d_pre_rprio, need)) ||
-            (rc = grow_pre(ctx, ctx->d_pre_rrec, need)) || (rc = grow_pre(ctx, ctx->d_pre_vlist, need))) return rc;
-        ctx->cap_pre_rpods = need + need / 2 + 64;
-    }
+    if ((rc = grow_set(ctx, ctx->cap_pre_pairs, (size_t)n_pair + 8, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_rpods, (size_t)rn_pod + 8, ctx->d_pre_rpodoff, ctx->d_pre_rprio, ctx->d_pre_rrec, ctx->d_pre_vlist))) return rc;
     return DRA_OK;
 }
 
@@ -2178,11 +2007,7 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
         reserve(ctx->spp_x, 0, 0, (size_t)PEER_MAX * 4);
         if (int rc = preload_preempt_place_shard(ctx)) return rc;
         if (ctx->d_inv_live) { if (int rc = spp_buffers(ctx, ctx->peer_spp_pods, ctx->peer_spp_pairs, ctx->peer_spp_run)) return rc; }
-        if ((size_t)tab_len + 16 > ctx->cap_gtable) {                     // the call's table, at the exported size
-            const size_t ncap = (size_t)tab_len + 16;
-            if (int rc = grow_nc(ctx, ctx->d_gtable, 0, ncap)) return rc;
-            ctx->cap_gtable = ncap;
-        }
+        if (int rc = grow_set(ctx, ctx->cap_gtable, (size_t)tab_len + 16, ctx->d_gtable)) return rc;   // the call's table, at the exported size
     }
     ctx->splace_seq = 0;
     if (ctx->d_splace_local) CU(cudaMemset(ctx->d_splace_local, 0, 64 + ctx->cap_splace_local * 8));
@@ -2235,10 +2060,8 @@ int result_table(dra_ctx* ctx, uint32_t n_out, const uint32_t* count_dev, PktGat
     if (ctx->world > 1) {
         ctx->peer_epoch += 1;
         g = make_gather(ctx, ctx->peer_epoch, 0, 0, 0, count_dev);
-    } else if ((size_t)n_out + 16 > ctx->cap_gtable) {
-        const size_t ncap = (size_t)n_out + n_out / 4 + 64;
-        if (int rc = grow_nc(ctx, ctx->d_gtable, 0, ncap)) return rc;
-        ctx->cap_gtable = ncap;
+    } else if (int rc = grow_set(ctx, ctx->cap_gtable, (size_t)n_out + 16, ctx->d_gtable)) {
+        return rc;
     }
     table = ctx->world > 1 ? g.table : ctx->d_gtable;
     return DRA_OK;
@@ -2466,12 +2289,7 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
     ctx->shard_last_n = n_claim;
     int rc = ensure_batch(ctx, std::max(cap, 1u), n_out, false);
     if (rc) return rc;
-    if ((size_t)n_claim + 64 > ctx->cap_cclaims) {
-        const size_t ncap = (size_t)n_claim + n_claim / 4 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_cclaims, 0, ncap))) return rc;
-        if ((rc = grow_nc(ctx, ctx->d_coff, 0, ncap))) return rc;
-        ctx->cap_cclaims = ncap;
-    }
+    if ((rc = grow_set(ctx, ctx->cap_cclaims, (size_t)n_claim + 64, ctx->d_cclaims, ctx->d_coff))) return rc;
     // tiles: 256 claims while that keeps them within 1024 (one round of predecessor reads), else 2048; beyond 2M claims
     // the look-back kernel
     const uint32_t sc_rows = n_claim <= 256u * 1024u ? 1u : 8u;
@@ -2635,11 +2453,7 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     if ((rc = ensure_batch(ctx, n_pod, 1, false))) return rc;
     const Tiling t = tiling(n_pod, n_win, ctx->n_sm);                 // the sort's tiles are laid out on the window
     if ((rc = grow(ctx, ctx->d_hist, ctx->cap_hist, (size_t)t.n_tiles * (n_win + 1), 64))) return rc;
-    if (n_pod + 8 > ctx->cap_podrec) {
-        const size_t cap = (size_t)n_pod + n_pod / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_podrec, ctx->cap_podrec, cap))) return rc;
-        ctx->cap_podrec = cap;
-    }
+    if ((rc = grow_set(ctx, ctx->cap_podrec, (size_t)n_pod + 8, ctx->d_podrec))) return rc;
     if (!ctx->d_spod) CU(cudaMalloc((void**)&ctx->d_spod, SP_WORDS * 4));
     uint2* table = nullptr; PktGather g; memset(&g, 0, sizeof g);
     if ((rc = result_table(ctx, n_out, nullptr, g, table))) return rc;
@@ -2735,17 +2549,9 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     if ((rc = ensure_batch(ctx, std::max(n_pod, n_pair), 1, false))) return rc;
     const Tiling t = tiling(n_pair, n_win, ctx->n_sm);                // the sort's tiles are laid out on the window
     if ((rc = grow(ctx, ctx->d_hist, ctx->cap_hist, (size_t)t.n_tiles * (n_win + 1), 64))) return rc;
-    if ((size_t)n_pair + 8 > ctx->cap_podrec) {
-        const size_t cap = (size_t)n_pair + n_pair / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_podrec, ctx->cap_podrec, cap))) return rc;
-        ctx->cap_podrec = cap;
-    }
-    if ((rc = grow(ctx, ctx->d_splace_rec, ctx->cap_splace_rec, n_pod))) return rc;
-    if ((size_t)n_win + 8 > ctx->cap_place_cursor) {
-        const size_t cap = (size_t)n_win + n_win / 2 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_place_cursor, ctx->cap_place_cursor, cap))) return rc;
-        ctx->cap_place_cursor = cap;
-    }
+    if ((rc = grow_set(ctx, ctx->cap_podrec, (size_t)n_pair + 8, ctx->d_podrec)) ||
+        (rc = grow(ctx, ctx->d_splace_rec, ctx->cap_splace_rec, n_pod)) ||
+        (rc = grow_set(ctx, ctx->cap_place_cursor, (size_t)n_win + 8, ctx->d_place_cursor))) return rc;
     if (!gather && n_pod > ctx->cap_splace_local) {          // world 1: the state words in plain device memory, zeroed
         const size_t cap = (size_t)n_pod + n_pod / 2 + 64;
         if (ctx->d_splace_local) CU(cudaFree(ctx->d_splace_local));
@@ -2805,23 +2611,16 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     // before the walk: after it, this thread launches only kernels preload_place_shard loaded, since anything it waits for
     // there would hold back the peers' calls that the walk waits for.)
     CU(cudaMemsetAsync(ctx->d_spod, 0, PEER_MAX * 4, ctx->stream));
-    {
-        // Every CTA resident.  Ranks sharing this device run their walks side by side, so each takes its share of the
-        // residency, less one CTA per SM left for a peer's waiting gather kernel.  Not a cooperative launch: cooperative
-        // grids do not run beside each other, and a rank's walk waits for its peers' walks.
-        if (ctx->splace_occ < 0) {
-            int occ = 0;
-            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_place<4, true>, 128, 0));
-            ctx->splace_occ = occ;
-        }
-        if (ctx->splace_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_place<4, true>: no CTA can be resident");
-        const int k = gather ? std::max(1, ctx->peers_on_device) : 1;
-        const int per_sm = k > 1 ? std::max(1, ctx->splace_occ - 1) : ctx->splace_occ;
-        const uint32_t share = (uint32_t)std::max(1, per_sm * ctx->n_sm / k);
-        const uint32_t grid = std::max(1u, std::min((n_win + 3) / 4, share));
-        k_pods_place<4, true><<<grid, 128, 0, ctx->stream>>>(a, sh);
-        ctx->launches += 1;
+    // Every CTA resident, not a cooperative launch: cooperative grids do not run beside each other, and a rank's walk waits
+    // for its peers' walks
+    if (ctx->splace_occ < 0) {
+        int occ = 0;
+        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_place<4, true>, 128, 0));
+        ctx->splace_occ = occ;
     }
+    if (ctx->splace_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_place<4, true>: no CTA can be resident");
+    k_pods_place<4, true><<<shard_walk_grid(ctx, ctx->splace_occ, gather, n_win), 128, 0, ctx->stream>>>(a, sh);
+    ctx->launches += 1;
     k_splace_final<<<(n_pod + 255) / 256, 256, 0, ctx->stream>>>(a, sh);
     ctx->launches += 1; ctx->chain |= DRA_K_PLACE_SHARD;
     prof.mark();
@@ -3010,11 +2809,7 @@ int dra_preempt_place_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     if (ctx->pp_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_preempt_place: no CTA can be resident");
     // The table is this context's own: every rank computes the whole of it, so no packet moves and the gather's epochs,
     // parities and cursors are left to the calls that gather
-    if ((size_t)n_out + 16 > ctx->cap_gtable) {
-        const size_t ncap = (size_t)n_out + n_out / 4 + 64;
-        if ((rc = grow_nc(ctx, ctx->d_gtable, 0, ncap))) return rc;
-        ctx->cap_gtable = ncap;
-    }
+    if ((rc = grow_set(ctx, ctx->cap_gtable, (size_t)n_out + 16, ctx->d_gtable))) return rc;
     uint2* table = ctx->d_gtable;
     cudaStream_t st = ctx->stream;
     const Err err = err_of(ctx);
@@ -3065,17 +2860,10 @@ int dra_preempt_place_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     if (!dense && n_pair &&
         (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_spp_inv, false, ctx->n_node, ctx->d_node_off)))
         return rc;
-    if (ctx->n_node) {
-        // Every CTA resident, but not a cooperative launch: ranks sharing this device run their walks side by side (each
-        // takes its share of the residency, less one CTA per SM left for a peer's waiting exchange).  The walk itself waits
-        // for no peer.
-        const int k = gather ? std::max(1, ctx->peers_on_device) : 1;
-        const int per_sm = k > 1 ? std::max(1, ctx->pp_occ - 1) : ctx->pp_occ;
-        const uint32_t share = (uint32_t)std::max(1, per_sm * ctx->n_sm / k);
-        const uint32_t grid = std::max(1u, std::min((ctx->n_node + 3) / 4, share));
+    if (ctx->n_node) {                 // every CTA resident (shard_walk_grid); the walk itself waits for no peer
         PreArgs aw = a;
         aw.gate = ctx->d_spp_gate;
-        k_pods_preempt_place<4><<<grid, 128, 0, st>>>(aw, pl, pp);
+        k_pods_preempt_place<4><<<shard_walk_grid(ctx, ctx->pp_occ, gather, ctx->n_node), 128, 0, st>>>(aw, pl, pp);
         ctx->launches += 1;
     }
     const uint32_t fin = std::max(std::max(n_pod, R.n_pod), gpu_hi - gpu_lo);
