@@ -255,8 +255,9 @@ int  dra_unsuitable_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
  * pod_off[p] .. pod_off[p+1], all naming the same node, at most DRA_MAX_POD) is placed atomically; with
  * DRA_F_EXHAUSTIVE its MIG claims are placed by the backtracking search over the placement enumeration of
  * nvlib.go:244-295 (multi-request shape: demo/specs/quickstart/gpu-test4.yaml:19-44).  A pod that does not fit
- * takes nothing: its slots carry DRA_ST_POD (or DRA_ST_SEARCH_LIMIT).  Host buffers; flags: DRA_F_EXHAUSTIVE,
- * DRA_F_FRESH_INVENTORY. */
+ * takes nothing: its slots carry DRA_ST_POD (or DRA_ST_SEARCH_LIMIT).  The pods are sorted by node with
+ * dra_allocate_batch's counting sort: n_pod > 0 on an inventory of 102,400 nodes or more is DRA_E_INVAL, refused
+ * before anything runs.  Host buffers; flags: DRA_F_EXHAUSTIVE, DRA_F_FRESH_INVENTORY. */
 int  dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
                              const uint32_t* pod_off, uint32_t n_pod,
                              const uint32_t* out_off, dra_out_rec* out, uint32_t n_out, uint32_t flags);
@@ -274,8 +275,9 @@ int  dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t
  * out of budget (DRA_ST_INVALID for claims invalid by §3/§10); a pod of more than DRA_MAX_POD claims is INVALID; an
  * empty pod is skipped.  Slots are counted as if each claim named a node of the inventory.  With one candidate per pod,
  * the node its claims name, the result is byte for byte dra_allocate_pods_batch's.  pod_off / cand_off not monotone or
- * not spanning, a slot outside n_out, or unknown flags: DRA_E_INVAL, nothing changed.  Host buffers; flags:
- * DRA_F_EXHAUSTIVE, DRA_F_FRESH_INVENTORY. */
+ * not spanning, a slot outside n_out, unknown flags, or candidates (cand_off[n_pod] > 0) on an inventory of 102,400
+ * nodes or more (the pairs are sorted by node as dra_allocate_pods_batch's pods are; the dense form has no such limit):
+ * DRA_E_INVAL, nothing changed.  Host buffers; flags: DRA_F_EXHAUSTIVE, DRA_F_FRESH_INVENTORY. */
 int  dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
                           const uint32_t* pod_off, uint32_t n_pod,
                           const uint32_t* cand_nodes, const uint32_t* cand_off,
@@ -311,7 +313,8 @@ typedef struct dra_running_pods {
  *                    order (priority descending, then index); the rest of the row 0xFFFFFFFF.
  * DRA_E_INVAL with nothing written: unknown flags, pod_off / cand_off / running->pod_off not monotone or not spanning,
  * dense n_pod * n_node >= 2^32, a running slot range outside running->n_out, a running pod whose OK slots name a GPU
- * index >= n_gpu or GPUs of two nodes, max_victims > 0 without victims.  n_pod == 0 returns DRA_OK once flags, pod_off,
+ * index >= n_gpu or GPUs of two nodes, max_victims > 0 without victims, running pods on an inventory of 102,400 nodes
+ * or more (they are sorted by node as dra_allocate_pods_batch's pods are).  n_pod == 0 returns DRA_OK once flags, pod_off,
  * cand_off and max_victims pass, without examining the running pods.  Host buffers; flags: 0 or DRA_F_EXHAUSTIVE. */
 int  dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
                        const uint32_t* pod_off, const int32_t* prio, uint32_t n_pod,
@@ -344,7 +347,8 @@ int  dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
  * to dra_deallocate_batch again.  DRA_E_INVAL, with no output and no inventory word written: unknown flags, pod_off /
  * cand_off / running->pod_off not monotone or not spanning, more than 2^30 - 1 candidates for a pod or nodes in the
  * inventory, dense n_pod * n_node >= 2^32, a pending slot outside n_out, a running slot range outside running->n_out, a
- * running pod whose OK slots name a GPU index >= n_gpu or GPUs of two nodes.  n_pod == 0 returns DRA_OK after the
+ * running pod whose OK slots name a GPU index >= n_gpu or GPUs of two nodes, running pods or candidates (cand_off[n_pod]
+ * > 0) on an inventory of 102,400 nodes or more (both are sorted by node).  n_pod == 0 returns DRA_OK after the
  * checks of the pending arrays, without examining the running pods.  Host buffers; flags: 0 or DRA_F_EXHAUSTIVE. */
 int  dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
                              const uint32_t* pod_off, const int32_t* prio, uint32_t n_pod,

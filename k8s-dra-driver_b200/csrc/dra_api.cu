@@ -401,6 +401,11 @@ FusedPlan fused_plan(const dra_ctx* ctx, uint32_t n_claim, uint32_t flags, uint3
     return p;
 }
 
+// The counting sort's widest node range: its one-warp histogram (the form for ranges too wide for the CTA-wide one)
+// keeps (n_node + 1) u16 counters in shared memory, at most SORT_SMEM_MAX bytes of them
+constexpr size_t SORT_SMEM_MAX = 200 * 1024;
+size_t sort_warp_hist_smem(uint32_t n_node) { return ((size_t)n_node + 1) * sizeof(uint16_t); }
+
 // Stable counting sort of 16-byte records by their node key (.y) into ctx->d_sorted + ctx->d_claim_off — the
 // front half of the sort path.  Records naming no node get an INVALID OutRec (d_out != nullptr) or are dropped
 // (d_out == nullptr: pod records).  Enqueues only.
@@ -464,8 +469,8 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
                 prof.mark();
             } else {
                 if (n_dev) return fail(ctx, DRA_E_INVAL, "sharded call: node range too wide for the CTA-wide histogram");
-                size_t smem = ((size_t)n_node + 1) * sizeof(uint16_t);
-                if (smem > 200 * 1024) return fail(ctx, DRA_E_INVAL, "n_node=%u exceeds the bucketing limit", n_node);
+                size_t smem = sort_warp_hist_smem(n_node);
+                if (smem > SORT_SMEM_MAX) return fail(ctx, DRA_E_INVAL, "n_node=%u exceeds the bucketing limit", n_node);
                 if (smem > 48 * 1024 && ctx->hist_smem_set < (int)smem) {
                     CU(cudaFuncSetAttribute(k_bucket_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                     ctx->hist_smem_set = (int)smem;
@@ -886,6 +891,15 @@ int check_place_slots(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
         const uint32_t slots = gpu ? c.count : 1u, dst = out_off ? out_off[i] : i;
         if (dst > n_out || slots > n_out - dst) return fail(ctx, DRA_E_INVAL, "claim %u: slots [%u, %u) outside n_out %u", i, dst, dst + slots, n_out);
     }
+    return DRA_OK;
+}
+
+// A call that will sort n_rec records (pod or pair records, running pods) by node over the whole inventory: a node range
+// wider than the counting sort takes (launch_sort) fails here, before anything is staged or launched, so the refusal
+// leaves no kernel behind and no fault word set for the next call
+int check_sortable(dra_ctx* ctx, uint32_t n_rec) {
+    if (n_rec && sort_warp_hist_smem(ctx->n_node) > SORT_SMEM_MAX)
+        return fail(ctx, DRA_E_INVAL, "n_node=%u exceeds the bucketing limit", ctx->n_node);
     return DRA_OK;
 }
 
@@ -1541,6 +1555,7 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     int rc;
     if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim))) return rc;
     if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+    if ((rc = check_sortable(ctx, n_pod))) return rc;
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     CU(cudaSetDevice(ctx->device));
@@ -1594,7 +1609,8 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
         (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, PL_POS, 0, 0xFFFFFFF0ull, dense, n_pair))) return rc;
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
-    if ((rc = check_place_slots(ctx, claims, n_claim, out_off, n_out))) return rc;
+    if ((rc = check_place_slots(ctx, claims, n_claim, out_off, n_out)) ||
+        (rc = check_sortable(ctx, dense ? 0 : n_pair))) return rc;
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "dra_place_pods_batch needs cooperative launches, which this device does not offer");
@@ -1659,7 +1675,8 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
     bool dense; uint32_t n_pair;
     int rc;
     if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
-        (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, 0xFFFFFFFFu, ctx->n_node, 0xFFFFFFFFull, dense, n_pair))) return rc;
+        (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, 0xFFFFFFFFu, ctx->n_node, 0xFFFFFFFFull, dense, n_pair)) ||
+        (rc = check_sortable(ctx, n_pod ? R.n_pod : 0))) return rc;
     ctx->chain = DRA_K_PREEMPT; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     CU(cudaSetDevice(ctx->device));
@@ -1734,7 +1751,9 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
         (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, PL_POS, ctx->n_node, 0xFFFFFFFFull, dense, n_pair))) return rc;
     if (!dense && n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");   // (the dense form: below 2^32)
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
-    if ((rc = check_place_slots(ctx, claims, n_claim, out_off, n_out))) return rc;
+    if ((rc = check_place_slots(ctx, claims, n_claim, out_off, n_out)) ||
+        (rc = check_sortable(ctx, n_pod ? R.n_pod : 0)) ||
+        (rc = check_sortable(ctx, n_pod && !dense ? n_pair : 0))) return rc;
     ctx->chain = DRA_K_PREEMPT_PLACE; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "dra_preempt_place_batch needs cooperative launches, which this device does not offer");
