@@ -257,7 +257,10 @@ int  dra_unsuitable_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
  * nvlib.go:244-295 (multi-request shape: demo/specs/quickstart/gpu-test4.yaml:19-44).  A pod that does not fit
  * takes nothing: its slots carry DRA_ST_POD (or DRA_ST_SEARCH_LIMIT).  The pods are sorted by node with
  * dra_allocate_batch's counting sort: n_pod > 0 on an inventory of 102,400 nodes or more is DRA_E_INVAL, refused
- * before anything runs.  Host buffers; flags: DRA_F_EXHAUSTIVE, DRA_F_FRESH_INVENTORY. */
+ * before anything runs.  Slots are counted from each claim's own fields (a GPU claim naming no node of the inventory has
+ * one); slots no claim owns read back as 0.  pod_off not monotone or not spanning [0, n_claim], a slot range outside
+ * n_out, or unknown flags: DRA_E_INVAL, refused before anything runs, with no output written and no state changed.
+ * Host buffers; flags: DRA_F_EXHAUSTIVE, DRA_F_FRESH_INVENTORY. */
 int  dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
                              const uint32_t* pod_off, uint32_t n_pod,
                              const uint32_t* out_off, dra_out_rec* out, uint32_t n_out, uint32_t flags);

@@ -331,8 +331,13 @@ int ensure_batch(dra_ctx* ctx, uint32_t n_claim, uint32_t n_out, bool own_io) {
         ctx->cap_claims = ncap;
     }
     if (own_io) { int rc = grow(ctx, ctx->d_out, ctx->cap_out, need_o, 64); if (rc) return rc; }
+    // d_hist for a sort of any record count up to n_claim (the pod calls sort fewer records than they stage claims).  The
+    // tile count is not monotone in the count: tiles grow once there would be more than n_sm CTA-wide tiles (or 64
+    // one-warp tiles), so n_sm * 2048 records take n_sm tiles where more records can take fewer.
     Tiling t = tiling(n_claim, ctx->n_node, ctx->n_sm);
-    size_t need_h = (size_t)t.n_tiles * (ctx->n_node + 1);
+    const size_t knee = t.cta_wide ? std::min<size_t>(ctx->n_sm, ((size_t)n_claim + H8_TILE - 1) / H8_TILE)
+                                   : std::min<size_t>(64, ((size_t)n_claim + 255) / 256);
+    size_t need_h = std::max<size_t>(t.n_tiles, knee) * (ctx->n_node + 1);
     int rc = grow(ctx, ctx->d_hist, ctx->cap_hist, need_h, 64);
     if (rc) return rc;
     // k_bucket_scan_rows: one status word per CTA of 32 nodes, zeroed once (here, never inside a stream capture)
@@ -881,14 +886,20 @@ int check_cands(dra_ctx* ctx, uint32_t n_pod, const uint32_t* cand_nodes, const 
     return DRA_OK;
 }
 
-// Spec §13's slots: n_out >= n_claim without out_off, and each claim's OutRec slots within n_out as if the claim named a
-// node of the inventory
-int check_place_slots(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* out_off, uint32_t n_out) {
-    if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+// The pod calls' slots: n_out >= n_claim without out_off, and each claim's OutRec slots within n_out.  A GPU claim of
+// count 1 .. DRA_MAX_COUNT (more than 1 only with out_off) has count slots, every other claim one.  any_node (spec §13):
+// counted as if the claim named a node of the inventory; otherwise (spec §12, as k_pod_records counts them) only a GPU
+// claim naming a node < n_node has count slots.
+int check_slots(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* out_off, uint32_t n_out,
+                bool any_node) {
+    if (!out_off) {                                       // one slot per claim: claim i owns slot i
+        if (n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
+        return DRA_OK;
+    }
     for (uint32_t i = 0; i < n_claim; ++i) {
         const dra_claim_rec& c = claims[i];
-        const bool gpu = c.kind == DRA_KIND_GPU && c.count >= 1 && c.count <= DRA_MAX_COUNT && (out_off || c.count == 1);
-        const uint32_t slots = gpu ? c.count : 1u, dst = out_off ? out_off[i] : i;
+        const bool gpu = c.kind == DRA_KIND_GPU && (any_node || c.node < ctx->n_node) && c.count >= 1 && c.count <= DRA_MAX_COUNT;
+        const uint32_t slots = gpu ? c.count : 1u, dst = out_off[i];
         if (dst > n_out || slots > n_out - dst) return fail(ctx, DRA_E_INVAL, "claim %u: slots [%u, %u) outside n_out %u", i, dst, dst + slots, n_out);
     }
     return DRA_OK;
@@ -1545,7 +1556,9 @@ int dra_unsuitable_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
 }
 
 // Allocate with pod boundaries (spec §12): pod records -> stable counting sort of the PODS by node (the claim path's
-// bucketing kernels, the record has a ClaimRec's layout) -> one warp per node walks its pods in input order.
+// bucketing kernels, the record has a ClaimRec's layout) -> one warp per node walks its pods in input order.  The slot
+// ranges are checked here, before anything is enqueued (k_pod_records checks them again): k_pods does not look at the
+// fault word, so a bad range found only on the device would leave every other pod applied and no OutRec returned.
 int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, uint32_t n_pod,
                             const uint32_t* out_off, dra_out_rec* out, uint32_t n_out, uint32_t flags) {
     if (!ctx || !pod_off || (n_claim && (!claims || !out))) return DRA_E_INVAL;
@@ -1553,9 +1566,9 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     if (flags & ~(DRA_F_EXHAUSTIVE | DRA_F_FRESH_INVENTORY)) return fail(ctx, DRA_E_INVAL, "dra_allocate_pods_batch: unknown flags 0x%x", flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     int rc;
-    if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim))) return rc;
-    if (!out_off && n_out < n_claim) return fail(ctx, DRA_E_INVAL, "n_out %u < n_claim %u without out_off", n_out, n_claim);
-    if ((rc = check_sortable(ctx, n_pod))) return rc;
+    if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
+        (rc = check_slots(ctx, claims, n_claim, out_off, n_out, false)) ||
+        (rc = check_sortable(ctx, n_pod))) return rc;
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     CU(cudaSetDevice(ctx->device));
@@ -1570,6 +1583,8 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
     if (out_off) s.add(ctx->d_out_off, out_off, (size_t)n_claim * 4);
     if ((rc = stage_in(ctx, s))) return rc;
+    const uint32_t owned_lo = out_off ? 0u : n_claim;    // slots no claim owns read back as 0 (without out_off: past n_claim)
+    if (n_out > owned_lo) CU(cudaMemsetAsync(ctx->d_out + owned_lo, 0, (size_t)(n_out - owned_lo) * 8, ctx->stream));
     Err err = err_of(ctx);
     Prof prof(ctx);
     uint2* d_out = ctx->d_out;
@@ -1609,7 +1624,7 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
         (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, PL_POS, 0, 0xFFFFFFF0ull, dense, n_pair))) return rc;
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
-    if ((rc = check_place_slots(ctx, claims, n_claim, out_off, n_out)) ||
+    if ((rc = check_slots(ctx, claims, n_claim, out_off, n_out, true)) ||
         (rc = check_sortable(ctx, dense ? 0 : n_pair))) return rc;
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
@@ -1751,7 +1766,7 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
         (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, PL_POS, ctx->n_node, 0xFFFFFFFFull, dense, n_pair))) return rc;
     if (!dense && n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");   // (the dense form: below 2^32)
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
-    if ((rc = check_place_slots(ctx, claims, n_claim, out_off, n_out)) ||
+    if ((rc = check_slots(ctx, claims, n_claim, out_off, n_out, true)) ||
         (rc = check_sortable(ctx, n_pod ? R.n_pod : 0)) ||
         (rc = check_sortable(ctx, n_pod && !dense ? n_pair : 0))) return rc;
     ctx->chain = DRA_K_PREEMPT_PLACE; ctx->chain_tile = 0;

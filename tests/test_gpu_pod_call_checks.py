@@ -115,7 +115,7 @@ CASES = [
     ("cand_off[0] != 0", CANDS, dict(cn=[0, 1], co=[1, 1, 2])),
     ("cand_off decreasing", CANDS, dict(cn=[0, 1], co=[0, 2, 1])),
     ("n_out < n_claim without out_off", (PODS, PLACE, PREPL), dict(n_out=1)),
-    ("a claim's slots past n_out", (PLACE, PREPL), dict(oo=[0, 5])),
+    ("a claim's slots past n_out", (PODS, PLACE, PREPL), dict(oo=[0, 5])),
     ("max_victims without victims", (PRE,), dict(victims=False)),
 ]
 
