@@ -405,6 +405,54 @@ func (c *Context) PreemptPlaceBatch(claims []ClaimRec, podOff []uint32, prio []i
 	return r, nil
 }
 
+// Pod-capacity answer (spec §16).  Per pair (candOff order; dense: pod*nNode + node): the copies of the pod the node
+// still takes and why counting stopped (DRA_ST_OK: maxCopies reached, DRA_ST_POD, DRA_ST_SEARCH_LIMIT, DRA_ST_INVALID).
+// Per pod: the sum over its pairs and how many of them take at least one copy.
+type PodCapacity struct {
+	PairCopies []uint16
+	PairStop   []uint8
+	PodTotal   []uint64
+	PodNodes   []uint32
+}
+
+// PodCapacityBatch counts, for each pod and each of its candidate nodes, how many copies of the pod the node still takes,
+// placed as AllocatePodsBatch would place them with the same flags, at most maxCopies (1 .. 65535) per node
+// (dra_pod_capacity_batch, spec §16).  Pure.  Candidates as PlaceBatch (cands == candOff == nil: every node, ascending,
+// nNode of them).  Unbuilt, like the rest of this file.
+func (c *Context) PodCapacityBatch(claims []ClaimRec, podOff []uint32, cands, candOff []uint32, nNode int,
+	maxCopies uint32, flags uint32) (*PodCapacity, error) {
+	nPod := len(podOff) - 1
+	if nPod <= 0 {
+		return &PodCapacity{}, nil
+	}
+	nPair := nPod * nNode
+	var cp *C.dra_claim_rec
+	var cn, co *C.uint32_t
+	if len(claims) > 0 {
+		cp = (*C.dra_claim_rec)(unsafe.Pointer(&claims[0]))
+	}
+	if candOff != nil {
+		nPair = int(candOff[nPod])
+		co = (*C.uint32_t)(unsafe.Pointer(&candOff[0]))
+		if len(cands) == 0 {
+			cands = []uint32{0} // an empty list still needs an address (nil means the dense form)
+		}
+		cn = (*C.uint32_t)(unsafe.Pointer(&cands[0]))
+	}
+	r := &PodCapacity{make([]uint16, nPair+1), make([]uint8, nPair+1), make([]uint64, nPod), make([]uint32, nPod)}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_pod_capacity_batch(c.h, cp, C.uint32_t(len(claims)), (*C.uint32_t)(unsafe.Pointer(&podOff[0])),
+		C.uint32_t(nPod), cn, co, C.uint32_t(maxCopies), (*C.uint16_t)(unsafe.Pointer(&r.PairCopies[0])),
+		(*C.uint8_t)(unsafe.Pointer(&r.PairStop[0])), (*C.uint64_t)(unsafe.Pointer(&r.PodTotal[0])),
+		(*C.uint32_t)(unsafe.Pointer(&r.PodNodes[0])), C.uint32_t(flags))
+	if rc != 0 {
+		return nil, lastError(c.h)
+	}
+	r.PairCopies, r.PairStop = r.PairCopies[:nPair], r.PairStop[:nPair]
+	return r, nil
+}
+
 func (c *Context) DeallocateBatch(claims []ClaimRec, outOff []uint32, out []OutRec) error {
 	if len(claims) == 0 {
 		return nil

@@ -360,6 +360,36 @@ int  dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t
                              const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
                              uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, uint32_t flags);
 
+/* Pod capacity (spec §16): how many copies of each pod every candidate node still takes — the question asked about a
+ * workload rather than a pod (replicas of a Deployment that fit and where, an autoscaler's simulation, "free 3g.40gb
+ * instances per node", a figure to order dra_place_pods_batch's candidates by).  Pure: nothing is written to the
+ * inventory.  Pods and candidates as dra_unsuitable_batch takes them (cand_nodes == cand_off == NULL: dense form, pair
+ * k = pod * n_node + node); each claim's node field is ignored.  For pair k = (pod, node): the pod is evaluated on a
+ * private copy of the node as dra_allocate_pods_batch evaluates it with the same flags (spec §12, slots as if out_off
+ * were given: a GPU claim may have count up to DRA_MAX_COUNT), the placement kept each time it succeeds, until an
+ * evaluation fails or max_copies (1 .. 65535) copies are placed.
+ *   pair_copies[k]   copies placed: the number of OK pods dra_allocate_pods_batch gives for max_copies identical copies
+ *                    of the pod naming that node.  With DRA_F_EXHAUSTIVE, >= 1 exactly when dra_unsuitable_batch sets
+ *                    the pair's bit with that flag; without it the evaluation is §12's, not §8's claim walk.
+ *   pair_stop[k]     (may be NULL) why counting stopped: DRA_ST_OK max_copies reached (the count is "at least");
+ *                    DRA_ST_POD the next copy does not fit; DRA_ST_SEARCH_LIMIT the next copy's search ran out of
+ *                    DRA_EXH_BUDGET (the count is a lower bound); DRA_ST_INVALID more than DRA_MAX_POD claims or a claim
+ *                    invalid by §3/§10 (copies 0)
+ *   pod_total[p]     (may be NULL) the sum of the pod's pair_copies: with each node listed once, the copies the whole
+ *                    candidate set takes (nodes are independent); a node listed twice is counted twice
+ *   pod_nodes[p]     (may be NULL) how many of the pod's pairs take at least one copy
+ * A candidate naming no node of the inventory: copies 0, DRA_ST_POD.  Otherwise an empty pod: copies max_copies,
+ * DRA_ST_OK.  DRA_E_INVAL with nothing written: unknown flags, max_copies 0 or above 65535, pod_off / cand_off not
+ * monotone or not spanning, dense n_pod * n_node >= 2^32, pair_copies NULL with pairs to answer.  n_pod == 0 returns
+ * DRA_OK after those checks.  On a sharded world the call is exact on any rank after dra_shard_sync_inventory_device,
+ * which makes that rank's live copy the world's state.  Host buffers; flags: 0 or DRA_F_EXHAUSTIVE. */
+int  dra_pod_capacity_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
+                            const uint32_t* pod_off, uint32_t n_pod,
+                            const uint32_t* cand_nodes, const uint32_t* cand_off,
+                            uint32_t max_copies,
+                            uint16_t* pair_copies, uint8_t* pair_stop,
+                            uint64_t* pod_total, uint32_t* pod_nodes, uint32_t flags);
+
 /* Deallocate(): stands in for controller.Driver.Deallocate(ctx, claim).  Inverse update from the
  * claims and the OutRecs dra_allocate_batch produced for them (same out_off convention). */
 int  dra_deallocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
@@ -664,6 +694,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_PREEMPT_SHARD    0x1000000u /* sharded preemption: prep, victim lists, the window's pairs, partials, merge */
 #define DRA_K_PREEMPT_PLACE    0x2000000u /* preempt and place: running-pod prep, victim lists, visit lists, persistent walk */
 #define DRA_K_PREEMPT_PLACE_SHARD 0x4000000u /* sharded preempt and place: state exchange, the §15 chain on it, own range back */
+#define DRA_K_POD_CAPACITY     0x8000000u /* pod capacity: the pairs' copy counts, the per-pod sums */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

@@ -116,6 +116,11 @@ public:
     // on none of its nodes.  Each pod is atomic (spec §12), its MIG claims by the backtracking search when
     // SetExhaustive(true).  Placed claims can be given back with Deallocate.
     void PlaceBatch(const std::vector<PodRequest>& pods);
+    // how many copies of each pod every one of its PotentialNodes still takes (spec §16, dra_pod_capacity_batch), counted
+    // as AllocateBatch would place them under SetExhaustive, at most maxCopies (1 .. 65535) per node; pure.  Result q:
+    // node name -> copies for pod q; a node the inventory does not know counts 0, and a pod whose claims cannot be
+    // lowered gets an empty map (each claim's Error says why).  SelectedNode is not read.
+    std::vector<std::map<std::string, uint32_t>> PodCapacityBatch(const std::vector<PodRequest>& pods, uint32_t maxCopies);
 
     // live occupancy of one GPU (memory-slice mask), for inspection
     uint16_t BusyMask(const std::string& node, uint32_t gpuIndex);

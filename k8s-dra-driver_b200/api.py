@@ -25,7 +25,7 @@ KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x0
            "pack1": 0x02000, "pack4": 0x04000, "compact_flat1": 0x08000, "compact_flat8": 0x10000,
            "compact_lookback": 0x20000, "compact_in_kernel": 0x40000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000,
            "place_shard": 0x400000, "preempt": 0x800000, "preempt_shard": 0x1000000,
-           "preempt_place": 0x2000000, "preempt_place_shard": 0x4000000}
+           "preempt_place": 0x2000000, "preempt_place_shard": 0x4000000, "pod_capacity": 0x8000000}
 
 
 class DraError(RuntimeError):
@@ -67,6 +67,7 @@ SYMBOLS = {
     "dra_deallocate_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_preempt_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32]),
     "dra_preempt_place_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _u32]),
+    "dra_pod_capacity_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _u32]),
     "dra_comm_unique_id": (_i32, [_vp]),
     "dra_comm_init": (_i32, [_vp, _vp, _i32, _i32]),
     "dra_allocate_batch_gather_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _u32, _u32]),
@@ -412,6 +413,28 @@ class Context:
                                                       C.byref(run), _ptr(oo), _ptr(out), n_out, _ptr(pod_node),
                                                       _ptr(pod_status), _ptr(evicted_by), flags))
         return out[:n_out], pod_node[:n_pod], pod_status[:n_pod], evicted_by[:run.n_pod]
+
+    def pod_capacity(self, claims, pod_off, cand_nodes=None, cand_off=None, max_copies: int = 64, exhaustive: bool = False,
+                     want_stop: bool = True, want_totals: bool = True):
+        """Pod capacity (spec §16): how many copies of each pod every candidate node still takes, counted as
+        allocate_pods() would place them (at most max_copies, 1 .. 65535).  cand_nodes/cand_off None = every node, pair
+        k = pod * n_node + node.  Pure.  Returns (pair_copies u16, pair_stop u8 or None, pod_total u64 or None, pod_nodes
+        u32 or None); pair_stop: ST_OK max_copies reached, ST_POD the next copy does not fit, ST_SEARCH_LIMIT its search
+        ran out of budget, ST_INVALID."""
+        c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
+        po = np.ascontiguousarray(pod_off, dtype=np.uint32)
+        n_pod = len(po) - 1
+        cn, co = _cands(cand_nodes, cand_off)
+        n_pair = n_pod * self.n_node if co is None else int(co[-1])
+        copies = np.zeros(max(n_pair, 1), dtype=np.uint16)
+        stop = np.zeros(max(n_pair, 1), dtype=np.uint8) if want_stop else None
+        total = np.zeros(max(n_pod, 1), dtype=np.uint64) if want_totals else None
+        nodes = np.zeros(max(n_pod, 1), dtype=np.uint32) if want_totals else None
+        self._check(self._lib.dra_pod_capacity_batch(self._h, _ptr(c), len(c), _ptr(po), n_pod, _ptr(cn), _ptr(co), max_copies,
+                                                     _ptr(copies), _ptr(stop), _ptr(total), _ptr(nodes),
+                                                     F_EXHAUSTIVE if exhaustive else 0))
+        return (copies[:n_pair], None if stop is None else stop[:n_pair], None if total is None else total[:n_pod],
+                None if nodes is None else nodes[:n_pod])
 
     def deallocate(self, claims, out, out_off=None):
         c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)

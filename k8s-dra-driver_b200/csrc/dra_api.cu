@@ -117,6 +117,9 @@ struct dra_ctx {
     uint32_t* d_pp_evicted = nullptr; size_t cap_pp_rpods = 0;
     uint32_t *d_pp_runoff = nullptr, *d_pp_judged = nullptr; size_t cap_pp_nodes = 0;
     int pp_occ = -1;                      // resident CTAs of k_pods_preempt_place<4> per SM (occupancy query, once)
+    // pod capacity (spec §16): per pair, per pod
+    uint16_t* d_cap_copies = nullptr; uint8_t* d_cap_stop = nullptr; size_t cap_cap_pairs = 0;
+    unsigned long long* d_cap_total = nullptr; uint32_t* d_cap_nodes = nullptr; size_t cap_cap_pods = 0;
 
     // error flags
     uint32_t* d_err = nullptr;            // device memory
@@ -1014,6 +1017,28 @@ void launch_preempt_victims(dra_ctx* ctx, const PreArgs& a, const uint32_t* choi
     ctx->launches += 1;
 }
 
+// k_pods_capacity over a's pairs (none: no launch), pair_width lanes per pair, 8 warps per CTA, then k_pods_capacity_sum
+// over its pods when a per-pod output is asked for.  Enqueues only.
+int launch_capacity(dra_ctx* ctx, CapArgs a) {
+    cudaStream_t st = ctx->stream;
+    if (a.n_pair) {
+        if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, st)); }
+        a.work = ctx->d_ticket + 14;
+        CU(cudaMemsetAsync(a.work, 0, 4, st));
+        const uint32_t W = pair_width(ctx), per_cta = 8 * (32 / W);
+        const uint32_t grid = std::max(1u, std::min((a.n_pair + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
+        if (W == 8) k_pods_capacity<8, 8><<<grid, 256, 0, st>>>(a);
+        else if (W == 16) k_pods_capacity<8, 16><<<grid, 256, 0, st>>>(a);
+        else k_pods_capacity<8, 32><<<grid, 256, 0, st>>>(a);
+        ctx->launches += 1;
+    }
+    if (a.pod_total || a.pod_nodes) {
+        k_pods_capacity_sum<<<(a.n_pod + 7) / 8, 256, 0, st>>>(a);
+        ctx->launches += 1;
+    }
+    return DRA_OK;
+}
+
 }  // namespace
 
 namespace {
@@ -1218,7 +1243,8 @@ void dra_ctx_destroy(dra_ctx* c) {
                    c->d_pre_prio, c->d_pre_node, c->d_pre_nvic, c->d_pre_choice, c->d_pre_pst, c->d_pre_psum, c->d_pre_psum64,
                    c->d_pre_pairst, c->d_pre_pairvic, c->d_pre_rclaims, c->d_pre_routoff, c->d_pre_rpodoff, c->d_pre_rprio,
                    c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic, c->d_spre_part,
-                   c->d_pp_pending, c->d_pp_evicted, c->d_pp_runoff, c->d_pp_judged, c->d_spp_inv, c->d_spp_gate};
+                   c->d_pp_pending, c->d_pp_evicted, c->d_pp_runoff, c->d_pp_judged, c->d_spp_inv, c->d_spp_gate,
+                   c->d_cap_copies, c->d_cap_stop, c->d_cap_total, c->d_cap_nodes};
     for (void* p : dev) if (p) cudaFree(p);
     for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
@@ -1741,6 +1767,58 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
     }
     prof.mark();
     return read_back(ctx, "preemption kernels", 1, outs);
+}
+
+// Pod capacity (spec §16): every argument is checked here, before anything is staged or launched, so a rejected call
+// writes nothing; the kernels read the live inventory and write only the call's own buffers.
+int dra_pod_capacity_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, uint32_t n_pod,
+                           const uint32_t* cand_nodes, const uint32_t* cand_off, uint32_t max_copies, uint16_t* pair_copies,
+                           uint8_t* pair_stop, uint64_t* pod_total, uint32_t* pod_nodes, uint32_t flags) {
+    if (!ctx || !pod_off || (n_claim && !claims)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_pod_capacity_batch: unknown flags 0x%x", flags);
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (max_copies < 1 || max_copies > 65535) return fail(ctx, DRA_E_INVAL, "max_copies %u outside [1, 65535]", max_copies);
+    bool dense; uint32_t n_pair;
+    int rc;
+    if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
+        (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, 0xFFFFFFFFu, ctx->n_node, 0xFFFFFFFFull, dense, n_pair))) return rc;
+    if (n_pair && !pair_copies) return fail(ctx, DRA_E_INVAL, "pair_copies is NULL");
+    ctx->chain = DRA_K_POD_CAPACITY; ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;
+    CU(cudaSetDevice(ctx->device));
+    if ((rc = ensure_batch(ctx, n_claim, 1, true))) return rc;
+    if ((rc = upload_table(ctx))) return rc;
+    if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
+        (!dense && (rc = grow_set(ctx, ctx->cap_pairs, (size_t)n_pair + 64, ctx->d_cand_nodes, ctx->d_pair_pod))) ||
+        (rc = grow_set(ctx, ctx->cap_cap_pairs, (size_t)n_pair + 8, ctx->d_cap_copies, ctx->d_cap_stop)) ||
+        (rc = grow_set(ctx, ctx->cap_cap_pods, (size_t)n_pod + 8, ctx->d_cap_total, ctx->d_cap_nodes))) return rc;
+    const Outputs outs = {{pair_copies, ctx->d_cap_copies, (size_t)n_pair * 2},
+                          {pair_stop, ctx->d_cap_stop, pair_stop ? (size_t)n_pair : 0},
+                          {pod_total, ctx->d_cap_total, pod_total ? (size_t)n_pod * 8 : 0},
+                          {pod_nodes, ctx->d_cap_nodes, pod_nodes ? (size_t)n_pod * 4 : 0}};
+    if ((rc = reserve_out(ctx, outs))) return rc;
+    Staging s;
+    s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
+    s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
+    if (!dense) {
+        s.add(ctx->d_cand_off, cand_off, ((size_t)n_pod + 1) * 4);
+        s.add(ctx->d_cand_nodes, cand_nodes, (size_t)n_pair * 4);
+        s.add(ctx->d_pair_pod, nullptr, (size_t)n_pair * 4);
+    }
+    if ((rc = stage_in(ctx, s, [&](uint8_t* h) { expand_pairs((uint32_t*)h, cand_off, n_pod); }))) return rc;
+    CapArgs a; memset(&a, 0, sizeof a);
+    a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.n_pod = n_pod;
+    a.cand_nodes = dense ? nullptr : ctx->d_cand_nodes; a.cand_off = dense ? nullptr : ctx->d_cand_off;
+    a.pair_pod = dense ? nullptr : ctx->d_pair_pod; a.n_pair = n_pair;
+    a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.tbl = ctx->d_tbl; a.sel = sel_of(ctx);
+    a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.max_copies = max_copies;
+    a.pair_copies = ctx->d_cap_copies; a.pair_stop = pair_stop ? ctx->d_cap_stop : nullptr;
+    a.pod_total = pod_total ? ctx->d_cap_total : nullptr; a.pod_nodes = pod_nodes ? ctx->d_cap_nodes : nullptr;
+    Prof prof(ctx);
+    if ((rc = launch_capacity(ctx, a))) return rc;
+    prof.mark();
+    return read_back(ctx, "capacity kernels", 1, outs);
 }
 
 // Preempt and place (spec §15): the pending-pod arrays are checked here, the running pods on the device (k_pre_running),

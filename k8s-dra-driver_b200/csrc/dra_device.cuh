@@ -4273,4 +4273,97 @@ k_spre_merge(const PeerExchange x, const PreMerge m) {
     }
 }
 
+// ====================================================================================================
+// Pod capacity (spec §16): how many copies of a pod each candidate node still takes
+//   k_pods_capacity      W lanes per (pod, node) pair: pod_eval on a register copy of the node, the placement kept each
+//                        time it succeeds, until one fails or max_copies are placed
+//   k_pods_capacity_sum  warp per pod: the pod's pairs summed, and those with a copy counted
+// ====================================================================================================
+struct CapArgs {
+    const uint4* claims; const uint32_t* pod_off; uint32_t n_pod;
+    const uint32_t* cand_nodes; const uint32_t* cand_off; const uint32_t* pair_pod;   // cand_off == nullptr: dense form
+    uint32_t n_pair;
+    const uint4* inv; const uint32_t* node_off; uint32_t n_node; const uint32_t* tbl; SelCtx sel;
+    uint32_t exhaustive, max_copies;
+    uint16_t* pair_copies; uint8_t* pair_stop;            // pair_stop: nullptr unless asked for
+    unsigned long long* pod_total; uint32_t* pod_nodes;   // each nullptr unless asked for
+    uint32_t* work;                                       // next unclaimed pair (zeroed by the host)
+};
+
+// k_pods_preempt's layout: W lanes per pair, 32/W pairs per warp, pairs taken from a counter, since a pair costs from one
+// evaluation to max_copies of them.  One writer per pair, so the results are plain stores and nothing is zeroed first.
+// A candidate naming no node, an empty pod and a pod of more than DRA_MAX_POD claims are answered without loading a node.
+template <int WPC, int W>
+__global__ void __launch_bounds__(WPC * 32, 2)
+k_pods_capacity(const CapArgs a) {
+    __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
+    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
+    __syncthreads();
+    constexpr uint32_t G = 32 / W;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t grp = lane / W, gbase = grp * W, gl = lane - gbase;
+    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
+    while (true) {
+        uint32_t nxt = 0;
+        if (lane == 0) nxt = atomicAdd(a.work, G);
+        const uint32_t pw = __shfl_sync(FULLMASK, nxt, 0);
+        if (pw >= a.n_pair) break;
+        const uint32_t pair = pw + grp;
+        if (pair >= a.n_pair) continue;                                  // whole group skips together
+        uint32_t pod, node;
+        if (!a.cand_off) { pod = pair / a.n_node; node = pair - pod * a.n_node; }
+        else { pod = __ldg(&a.pair_pod[pair]); node = __ldg(&a.cand_nodes[pair]); }
+        const uint32_t c0 = __ldg(&a.pod_off[pod]), cnt = __ldg(&a.pod_off[pod + 1]) - c0;
+        uint32_t copies = 0, stop = DRA_ST_POD;                           // a candidate naming no node: unsuitable (§8)
+        if (node >= a.n_node) {}
+        else if (cnt == 0) { copies = a.max_copies; stop = DRA_ST_OK; }
+        else if (cnt > DRA_MAX_POD) stop = DRA_ST_INVALID;
+        else {
+            const uint32_t g0 = __ldg(&a.node_off[node]), ng = __ldg(&a.node_off[node + 1]) - g0;
+            if (ng <= W) {                                                // always: W is chosen from the inventory
+                Lane L; L.load(gl < ng ? __ldg(&a.inv[g0 + gl]) : make_uint4(0, 0, 0, 0), gl < ng);
+                const PodGet get{a.claims + c0, nullptr, 0};
+                Lane Lt;                                                  // ONE copy handed to every pod_eval: one stack slot
+                stop = DRA_ST_OK;
+                while (copies < a.max_copies) {
+                    Lt = L;
+                    const uint32_t st = pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, a.exhaustive != 0, true, nullptr);
+                    if (st) { stop = st; break; }
+                    L = Lt; ++copies;
+                }
+                // validity does not depend on the node's state: an invalid pod fails its first evaluation
+                if (stop == DRA_ST_POD && copies == 0 && pod_invalid<W>(a.claims + c0, cnt, a.sel.n_sel, true, gl, gmask))
+                    stop = DRA_ST_INVALID;
+            }
+        }
+        if (lane == gbase) {
+            a.pair_copies[pair] = (uint16_t)copies;
+            if (a.pair_stop) a.pair_stop[pair] = (uint8_t)stop;
+        }
+    }
+}
+
+// Warp per pod: the lanes stride the pod's pairs (dense: its row of n_node).  The counts are 16 bits each, so a lane's
+// sum needs 64 bits only beyond 65,537 pairs per lane; it is kept in 64 bits throughout and reduced with a shuffle tree.
+__global__ void __launch_bounds__(256)
+k_pods_capacity_sum(const CapArgs a) {
+    const uint32_t lane = threadIdx.x & 31, p = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (p >= a.n_pod) return;
+    const unsigned long long k0 = a.cand_off ? __ldg(&a.cand_off[p]) : (unsigned long long)p * a.n_node;
+    const unsigned long long k1 = a.cand_off ? __ldg(&a.cand_off[p + 1]) : k0 + a.n_node;
+    unsigned long long sum = 0;
+    uint32_t nodes = 0;
+    for (unsigned long long k = k0; k < k1; k += 32) {
+        const uint32_t c = k + lane < k1 ? (uint32_t)a.pair_copies[k + lane] : 0u;
+        sum += c;
+        nodes += __popc(__ballot_sync(FULLMASK, c != 0u));
+    }
+    #pragma unroll
+    for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(FULLMASK, sum, d);
+    if (lane == 0) {
+        if (a.pod_total) a.pod_total[p] = sum;
+        if (a.pod_nodes) a.pod_nodes[p] = nodes;
+    }
+}
+
 }  // namespace dra

@@ -313,6 +313,48 @@ void Driver::PlaceBatch(const std::vector<PodRequest>& pods) {
                 if (ca->Error == status_text(DRA_ST_POD)) ca->Error = "the pod's claims fit together on none of its potential nodes";
 }
 
+std::vector<std::map<std::string, uint32_t>> Driver::PodCapacityBatch(const std::vector<PodRequest>& pods, uint32_t maxCopies) {
+    std::vector<std::map<std::string, uint32_t>> res(pods.size());
+    Lowered lo;
+    std::vector<uint32_t> podOff(1, 0), candOff(1, 0), cand;
+    std::vector<size_t> podOf;                                  // lowered pod -> index in pods
+    for (size_t pi = 0; pi < pods.size(); ++pi) {
+        const auto& pod = pods[pi];
+        uint32_t model = 0;                                     // profile names: as in UnsuitableNodesBatch
+        for (const auto& nn : pod.PotentialNodes) { const uint32_t n = nodeIndex(nn); if (n != 0xFFFFFFFFu) { model = nodeModel_[n]; break; } }
+        std::map<std::string, uint32_t> groups;
+        bool ok = true;
+        const size_t mark = lo.recs.size();
+        const uint32_t markOut = lo.nOut;
+        for (ClaimAllocation* ca : groupAdjacent(pod.Claims)) {
+            uint32_t g = 0;
+            if (ca->IsMig && !ca->Mig.GpuClaimName.empty()) {
+                auto it = groups.find(ca->Mig.GpuClaimName);
+                g = it == groups.end() ? (groups[ca->Mig.GpuClaimName] = nextGroup_++) : it->second;
+                if (nextGroup_ == 0) nextGroup_ = 1;
+            }
+            ok = lower(*ca, 0, g, lo, model) && ok;
+        }
+        if (!ok) {
+            lo.recs.resize(mark); lo.outOff.resize(mark); lo.owner.resize(mark); lo.nOut = markOut;
+            continue;
+        }
+        podOff.push_back((uint32_t)lo.recs.size());
+        for (const auto& nn : pod.PotentialNodes) cand.push_back(nodeIndex(nn));
+        candOff.push_back((uint32_t)cand.size());
+        podOf.push_back(pi);
+    }
+    if (podOf.empty()) return res;
+    std::vector<uint16_t> copies(cand.size() + 1, 0);
+    check(dra_pod_capacity_batch(ctx_, lo.recs.data(), (uint32_t)lo.recs.size(), podOff.data(), (uint32_t)podOf.size(),
+                                 cand.data(), candOff.data(), maxCopies, copies.data(), nullptr, nullptr, nullptr,
+                                 exhaustive_ ? DRA_F_EXHAUSTIVE : 0u), "dra_pod_capacity_batch");
+    for (size_t q = 0; q < podOf.size(); ++q)
+        for (uint32_t k = candOff[q]; k < candOff[q + 1]; ++k)
+            res[podOf[q]][pods[podOf[q]].PotentialNodes[k - candOff[q]]] = copies[k];
+    return res;
+}
+
 void Driver::UnsuitableNodes(const std::vector<ClaimAllocation*>& claims, const std::vector<std::string>& potentialNodes) {
     PodRequest p; p.Claims = claims; p.PotentialNodes = potentialNodes;
     UnsuitableNodesBatch({p});
