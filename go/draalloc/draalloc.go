@@ -648,6 +648,35 @@ func (c *Context) PreemptBatchGlobalDevice(pinnedClaims unsafe.Pointer, nClaim i
 	return nil
 }
 
+// SetShardCapacity reserves room for the sharded pod-capacity call's pair results: before ShardExport, the same on every
+// context.  Unbuilt, like the rest of this file.
+func (c *Context) SetShardCapacity(maxPairs uint32) error {
+	if rc := C.dra_set_shard_capacity(c.h, C.uint32_t(maxPairs)); rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
+// PodCapacityBatchGlobalDevice: pod capacity (spec §16) on a sharded world (dra_pod_capacity_batch_global_device).  The
+// same pods, candidates (pinnedCandNodes == pinnedCandOff == nil: dense form, nPair = nPod * nNode), maxCopies and flags
+// on every context, every array in dra_host_alloc'ed (pinned) memory; each context counts the pairs of its own nodes, and
+// every context ends with the whole outputs (all but pinnedPairCopies may be nil).  Returns at once; Sync reports
+// completion and errors found on the device.  Unbuilt, like the rest of this file.
+func (c *Context) PodCapacityBatchGlobalDevice(pinnedClaims unsafe.Pointer, nClaim int, pinnedPodOff unsafe.Pointer, nPod int,
+	pinnedCandNodes, pinnedCandOff unsafe.Pointer, nPair int, maxCopies int,
+	pinnedPairCopies, pinnedPairStop, pinnedPodTotal, pinnedPodNodes unsafe.Pointer, flags uint32) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_pod_capacity_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
+		(*C.uint32_t)(pinnedPodOff), C.uint32_t(nPod), (*C.uint32_t)(pinnedCandNodes), (*C.uint32_t)(pinnedCandOff),
+		C.uint32_t(nPair), C.uint32_t(maxCopies), (*C.uint16_t)(pinnedPairCopies), (*C.uint8_t)(pinnedPairStop),
+		(*C.uint64_t)(pinnedPodTotal), (*C.uint32_t)(pinnedPodNodes), C.uint32_t(flags))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
 // SetShardPreemptPlace reserves room for the sharded preempt-and-place call (pending pods, judged pairs, running pods):
 // after SetInventory, before ShardExport, the same on every context.  Unbuilt, like the rest of this file.
 func (c *Context) SetShardPreemptPlace(maxPods, maxPairs, maxRun uint32) error {

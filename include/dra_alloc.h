@@ -382,7 +382,8 @@ int  dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t
  * DRA_ST_OK.  DRA_E_INVAL with nothing written: unknown flags, max_copies 0 or above 65535, pod_off / cand_off not
  * monotone or not spanning, dense n_pod * n_node >= 2^32, pair_copies NULL with pairs to answer.  n_pod == 0 returns
  * DRA_OK after those checks.  On a sharded world the call is exact on any rank after dra_shard_sync_inventory_device,
- * which makes that rank's live copy the world's state.  Host buffers; flags: 0 or DRA_F_EXHAUSTIVE. */
+ * which makes that rank's live copy the world's state; dra_pod_capacity_batch_global_device answers across the ranks
+ * without the sync, each rank counting the pairs of its own nodes.  Host buffers; flags: 0 or DRA_F_EXHAUSTIVE. */
 int  dra_pod_capacity_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
                             const uint32_t* pod_off, uint32_t n_pod,
                             const uint32_t* cand_nodes, const uint32_t* cand_off,
@@ -418,7 +419,7 @@ int  dra_gather_read(dra_ctx* ctx, dra_out_rec* out_all, uint32_t n_rec);
  *                                              cudaIpcMemHandle_t;  the host runtime all-gathers the handles;
  *   dra_peer_import(ctx, handles)              world * 64 bytes, in rank order.
  * Requires all ranks on one node with P2P access; on failure the NCCL path stays in use.  Every rank must export alike (the
- * same sizes, dra_set_shard_pairs, dra_set_shard_place, dra_set_shard_preempt and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
+ * same sizes, dra_set_shard_pairs, dra_set_shard_place, dra_set_shard_preempt, dra_set_shard_capacity and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
  * own layout, so dra_peer_import / dra_peer_import_local refuse a peer set up differently with DRA_E_INVAL.
  * dra_peer_export(ctx, 0, NULL) switches the peer path off again. */
 int  dra_peer_export(dra_ctx* ctx, uint32_t n_per_rank, void* handle64);
@@ -560,6 +561,37 @@ int  dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
                                      uint32_t* d_pod_node, uint8_t* d_pod_status, uint32_t* d_n_victims,
                                      uint32_t* d_victims, uint32_t max_victims, uint32_t flags);
 
+/* Room for the sharded pod-capacity call in the buffer dra_shard_export maps: each rank's slice holds a 16-byte header,
+ * then a u16 count and a u8 stop per pair, each part padded to 16 bytes, so 16 * (1 + ceil(max_pairs / 8) +
+ * ceil(max_pairs / 16)) bytes, one slice per rank and call parity: world * 2 slices per rank (about 61 MB for 1.28 M pairs
+ * at world 8).  World > 1: call before dra_shard_export (afterwards: DRA_E_STATE), every rank with the same max_pairs; the
+ * peer import refuses a peer set up differently.  The export also sizes the call's scratch for max_pairs (one slice and 4
+ * bytes a pair), so that no call frees a buffer while a peer waits for it.  World 1 needs no call. */
+int  dra_set_shard_capacity(dra_ctx* ctx, uint32_t max_pairs);
+/* Pod capacity over a sharded world (spec §16, "Sharded form"): dra_pod_capacity_batch answered on the world's state.  The
+ * SAME claims, pod_off, candidates (cand_nodes == cand_off == NULL: the dense form, n_pair = n_pod * n_node), max_copies and
+ * flags on every rank (device pointers, or dra_host_alloc'ed buffers).  A pair is counted by the rank whose node range
+ * holds its candidate node, against that rank's live inventory; a candidate naming no node of the inventory gets 0 copies
+ * and DRA_ST_POD.  Every rank ends with the WHOLE outputs, laid out as dra_pod_capacity_batch's, byte for byte what that
+ * call answers on ONE inventory made of every rank's own nodes; d_pair_stop, d_pod_total and d_pod_nodes may be NULL.
+ * Nothing is written to any inventory, live or pristine.  Needs dra_set_shard (else DRA_E_STATE); world > 1 needs
+ * dra_set_shard_map spanning the inventory (a bare dra_set_shard: DRA_E_STATE), dra_shard_export after
+ * dra_set_shard_capacity with max_pairs > 0 (even for a call with no pairs), and dra_peer_import /
+ * dra_peer_import_local (else DRA_E_STATE).  World 1 needs no export,
+ * counts every node, and answers byte for byte as dra_pod_capacity_batch.  Host-side argument errors (DRA_E_INVAL) return
+ * before anything is enqueued: unknown flags, max_copies outside [1, 65535], one candidate array without the other, a
+ * dense n_pair other than n_pod * n_node, n_pair above 2^32 - 16 or (world > 1) above max_pairs, n_pod above 2^26, NULL
+ * d_pair_copies with pairs to answer.  Enqueues on ctx's stream and returns; n_pod == 0 enqueues nothing.  Completion and
+ * device-detected errors surface at dra_ctx_sync: pod_off / cand_off not monotone or not spanning their arrays give
+ * DRA_E_INVAL on EVERY rank with none of the outputs written; a peer that does not arrive within DRA_PEER_TIMEOUT_MS
+ * gives DRA_E_NCCL, also with nothing written.  flags: 0 or DRA_F_EXHAUSTIVE. */
+int  dra_pod_capacity_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                          const uint32_t* d_pod_off, uint32_t n_pod,
+                                          const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                          uint32_t max_copies,
+                                          uint16_t* d_pair_copies, uint8_t* d_pair_stop,
+                                          uint64_t* d_pod_total, uint32_t* d_pod_nodes, uint32_t flags);
+
 /* Every rank's live inventory becomes the world's state: for each GPU, the record its owning rank holds (the rank whose
  * node range contains the GPU's node, per the current dra_set_shard_map).  Own range untouched, pristine copy untouched.
  * Afterwards dra_get_inventory on any rank returns the whole world, and dra_set_shard_map may move node ranges between
@@ -695,6 +727,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_PREEMPT_PLACE    0x2000000u /* preempt and place: running-pod prep, victim lists, visit lists, persistent walk */
 #define DRA_K_PREEMPT_PLACE_SHARD 0x4000000u /* sharded preempt and place: state exchange, the §15 chain on it, own range back */
 #define DRA_K_POD_CAPACITY     0x8000000u /* pod capacity: the pairs' copy counts, the per-pod sums */
+#define DRA_K_POD_CAPACITY_SHARD 0x10000000u /* sharded pod capacity: prep, the window's pairs, exchange, merge with the sums */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

@@ -25,7 +25,8 @@ KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x0
            "pack1": 0x02000, "pack4": 0x04000, "compact_flat1": 0x08000, "compact_flat8": 0x10000,
            "compact_lookback": 0x20000, "compact_in_kernel": 0x40000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000,
            "place_shard": 0x400000, "preempt": 0x800000, "preempt_shard": 0x1000000,
-           "preempt_place": 0x2000000, "preempt_place_shard": 0x4000000, "pod_capacity": 0x8000000}
+           "preempt_place": 0x2000000, "preempt_place_shard": 0x4000000, "pod_capacity": 0x8000000,
+           "pod_capacity_shard": 0x10000000}
 
 
 class DraError(RuntimeError):
@@ -93,6 +94,9 @@ SYMBOLS = {
     "dra_set_shard_preempt_place": (_i32, [_vp, _u32, _u32, _u32]),
     "dra_preempt_place_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp,
                                                      _vp, _u32]),
+    "dra_set_shard_capacity": (_i32, [_vp, _u32]),
+    "dra_pod_capacity_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp,
+                                                    _u32]),
     "dra_shard_sync_inventory_device": (_i32, [_vp]),
     "dra_deallocate_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_mps_limits_batch": (_i32, [_vp, _vp, _u32, _vp, _vp]),
@@ -567,6 +571,22 @@ class Context:
             self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), _ptr(d_prio), n_pod, _ptr(d_cand_nodes), _ptr(d_cand_off),
             n_pair, C.byref(running), _ptr(d_pair_status), _ptr(d_pair_victims), _ptr(d_pod_node), _ptr(d_pod_status),
             _ptr(d_n_victims), _ptr(d_victims), max_victims, flags))
+
+    def set_shard_capacity(self, max_pairs: int) -> None:
+        """Room for the sharded pod-capacity call's pair results; world > 1: before shard_export, the same on every rank."""
+        self._check(self._lib.dra_set_shard_capacity(self._h, max_pairs))
+
+    def pod_capacity_global_device(self, d_claims: int, n_claim: int, d_pod_off: int, n_pod: int, d_cand_nodes: int | None,
+                                   d_cand_off: int | None, n_pair: int, max_copies: int, d_pair_copies: int | None,
+                                   d_pair_stop: int | None = None, d_pod_total: int | None = None,
+                                   d_pod_nodes: int | None = None, flags: int = 0) -> None:
+        """Sharded pod capacity (spec §16): the SAME pods and candidates on every rank (device pointers); d_cand_nodes /
+        d_cand_off None = dense form (n_pair = n_pod * n_node).  Each rank counts the pairs of its own nodes; every rank
+        receives the whole outputs, laid out as pod_capacity()'s (u16 copies, u8 stops, u64 totals, u32 node counts); all
+        but d_pair_copies may be None.  Enqueues, no synchronisation; errors found on the device surface at sync()."""
+        self._check(self._lib.dra_pod_capacity_batch_global_device(
+            self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod, _ptr(d_cand_nodes), _ptr(d_cand_off), n_pair,
+            max_copies, _ptr(d_pair_copies), _ptr(d_pair_stop), _ptr(d_pod_total), _ptr(d_pod_nodes), flags))
 
     def set_shard_preempt_place(self, max_pods: int, max_pairs: int, max_run: int) -> None:
         """Room for the sharded preempt-and-place call (pending pods, judged pairs, running pods); world > 1: before

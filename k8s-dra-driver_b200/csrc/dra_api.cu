@@ -222,6 +222,10 @@ struct dra_ctx {
     uint4* d_spp_inv = nullptr; size_t cap_spp_inv = 0;
     uint32_t* d_spp_gate = nullptr;
     PeerRegion spp_x;                           // the verdict agreement's flags (k_spp_agree), after the exchange
+    // sharded pod capacity: a region [slices x2: world slices][flags] (dra_device.cuh CapMerge) in the peer buffer
+    uint32_t scap_max_pairs = 0, peer_scap_pairs = 0;   // dra_set_shard_capacity; reserved by the next peer_setup
+    PeerRegion scap_x;
+    uint4* d_scap_part = nullptr; size_t cap_scap_part = 0;           // this rank's slice (uint4 units)
     int splace_occ = -1;                        // resident CTAs of k_pods_place<4, true> per SM (occupancy query, once)
     int peers_on_device = 1;                    // ranks whose contexts share this device (dra_peer_import_local)
     // inventory sync: records in the peer buffer ([staging x2: peer_inv_gpus records][flags[PEER_MAX], elect[2]])
@@ -1017,16 +1021,16 @@ void launch_preempt_victims(dra_ctx* ctx, const PreArgs& a, const uint32_t* choi
     ctx->launches += 1;
 }
 
-// k_pods_capacity over a's pairs (none: no launch), pair_width lanes per pair, 8 warps per CTA, then k_pods_capacity_sum
+// k_pods_capacity over a's walk (none: no launch), pair_width lanes per pair, 8 warps per CTA, then k_pods_capacity_sum
 // over its pods when a per-pod output is asked for.  Enqueues only.
 int launch_capacity(dra_ctx* ctx, CapArgs a) {
     cudaStream_t st = ctx->stream;
-    if (a.n_pair) {
+    if (a.n_walk) {
         if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, st)); }
         a.work = ctx->d_ticket + 14;
         CU(cudaMemsetAsync(a.work, 0, 4, st));
         const uint32_t W = pair_width(ctx), per_cta = 8 * (32 / W);
-        const uint32_t grid = std::max(1u, std::min((a.n_pair + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
+        const uint32_t grid = std::max(1u, std::min((a.n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
         if (W == 8) k_pods_capacity<8, 8><<<grid, 256, 0, st>>>(a);
         else if (W == 16) k_pods_capacity<8, 16><<<grid, 256, 0, st>>>(a);
         else k_pods_capacity<8, 32><<<grid, 256, 0, st>>>(a);
@@ -1244,7 +1248,7 @@ void dra_ctx_destroy(dra_ctx* c) {
                    c->d_pre_pairst, c->d_pre_pairvic, c->d_pre_rclaims, c->d_pre_routoff, c->d_pre_rpodoff, c->d_pre_rprio,
                    c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic, c->d_spre_part,
                    c->d_pp_pending, c->d_pp_evicted, c->d_pp_runoff, c->d_pp_judged, c->d_spp_inv, c->d_spp_gate,
-                   c->d_cap_copies, c->d_cap_stop, c->d_cap_total, c->d_cap_nodes};
+                   c->d_cap_copies, c->d_cap_stop, c->d_cap_total, c->d_cap_nodes, c->d_scap_part};
     for (void* p : dev) if (p) cudaFree(p);
     for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
@@ -1813,6 +1817,7 @@ int dra_pod_capacity_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n
     a.pair_pod = dense ? nullptr : ctx->d_pair_pod; a.n_pair = n_pair;
     a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.tbl = ctx->d_tbl; a.sel = sel_of(ctx);
     a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.max_copies = max_copies;
+    a.node_lo = 0; a.n_win = ctx->n_node; a.n_walk = n_pair;           // every node: the walk index is the pair index
     a.pair_copies = ctx->d_cap_copies; a.pair_stop = pair_stop ? ctx->d_cap_stop : nullptr;
     a.pod_total = pod_total ? ctx->d_cap_total : nullptr; a.pod_nodes = pod_nodes ? ctx->d_cap_nodes : nullptr;
     Prof prof(ctx);
@@ -1965,7 +1970,7 @@ namespace {
 // every rank to be set up alike; the export writes this at offset 0 of the buffer for importers in other processes to read.
 struct PeerLayout {
     uint32_t world, rank, form, cap, tab_len, uns_pairs, inv_gpus, rsvd;      // rsvd: dra_set_shard_place's max_pods
-    uint32_t pre_pods, pre_pairs, pre_victims, pad;                           // dra_set_shard_preempt's sizes
+    uint32_t pre_pods, pre_pairs, pre_victims, scap_pairs;                    // dra_set_shard_preempt's sizes, dra_set_shard_capacity's
     uint32_t spp_pods, spp_pairs, spp_run, pad2;                              // dra_set_shard_preempt_place's sizes
     bool operator==(const PeerLayout& o) const { return memcmp(this, &o, sizeof o) == 0; }
 };
@@ -1973,7 +1978,7 @@ PeerLayout layout_of(const dra_ctx* c, int rank) {
     PeerLayout l; memset(&l, 0, sizeof l);
     l.world = (uint32_t)c->world; l.rank = (uint32_t)rank; l.form = c->peer_form; l.cap = c->peer_cap; l.tab_len = c->peer_tab_len;
     l.uns_pairs = c->peer_uns_pairs; l.inv_gpus = c->peer_inv_gpus; l.rsvd = c->peer_place_pods;
-    l.pre_pods = c->peer_pre_pods; l.pre_pairs = c->peer_pre_pairs; l.pre_victims = c->peer_pre_victims;
+    l.pre_pods = c->peer_pre_pods; l.pre_pairs = c->peer_pre_pairs; l.pre_victims = c->peer_pre_victims; l.scap_pairs = c->peer_scap_pairs;
     l.spp_pods = c->peer_spp_pods; l.spp_pairs = c->peer_spp_pairs; l.spp_run = c->peer_spp_run;
     return l;
 }
@@ -2010,6 +2015,19 @@ int preload_preempt_shard(dra_ctx* ctx) {
     CU(cudaFuncSetAttribute((const void*)k_spre_merge, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     return DRA_OK;
 }
+
+// The same for the sharded pod-capacity chain, whose merge waits for its peers: it also takes the all-shared split.
+int preload_capacity_shard(dra_ctx* ctx) {
+    const void* ks[] = {(const void*)k_uns_prep, (const void*)k_pods_capacity<8, 8>, (const void*)k_pods_capacity<8, 16>,
+                        (const void*)k_pods_capacity<8, 32>, (const void*)k_peer_push, (const void*)k_scap_merge};
+    for (const void* k : ks) { cudaFuncAttributes fa; CU(cudaFuncGetAttributes(&fa, k)); }
+    CU(cudaFuncSetAttribute((const void*)k_scap_merge, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    return DRA_OK;
+}
+
+// uint4 units of one rank's pod-capacity slice for n walked pairs (dra_device.cuh CapMerge): the header, n u16 copies and
+// n u8 stops, each padded to 16 bytes
+size_t scap_units(uint32_t n) { return 1 + ((size_t)n + 7) / 8 + ((size_t)n + 15) / 16; }
 
 // The same for the sharded preempt-and-place chain, and the walk's occupancy query (which loads it too).  Its one wait is
 // the inventory exchange (k_isync_copy), before the walk.
@@ -2059,6 +2077,7 @@ int spre_buffers(dra_ctx* ctx, uint32_t n_pod, uint32_t n_pair, uint32_t max_vic
 // and, for dra_shard_export with an inventory loaded, [inventory staging x2: n_gpu records][their flags + election words]
 // and, after dra_set_shard_place(max_pods > 0), [place pods: progress counter, 64 bytes][max_pods state words of 8 bytes]
 // and, after dra_set_shard_preempt(max_pods > 0), [preemption partials x2: world slices of spre_units][their flags]
+// and, after dra_set_shard_capacity(max_pairs > 0), [pod-capacity slices x2: world slices of scap_units][their flags]
 int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, uint32_t cap) {
     if (ctx->world > (int)PEER_MAX) return fail(ctx, DRA_E_INVAL, "world %d > %u", ctx->world, PEER_MAX);
     CU(cudaSetDevice(ctx->device));
@@ -2111,6 +2130,16 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
         if (int rc = preload_preempt_shard(ctx)) return rc;
         if (int rc = spre_buffers(ctx, ctx->peer_pre_pods, ctx->peer_pre_pairs, ctx->peer_pre_victims, 0)) return rc;
         if (ctx->d_inv_live) { if (int rc = ensure_batch(ctx, 1, 1, false)) return rc; }
+    }
+    // sharded pod capacity, after dra_set_shard_capacity: the slices' exchange, and the call's scratch at full size now (no
+    // cudaFree inside a call while a peer's merge waits for this rank)
+    ctx->peer_scap_pairs = ctx->scap_max_pairs;
+    if (ctx->peer_scap_pairs) {
+        const size_t slice = scap_units(ctx->peer_scap_pairs) * 16;
+        reserve(ctx->scap_x, (size_t)ctx->world * slice, slice, (size_t)PEER_MAX * 4);
+        if (int rc = preload_capacity_shard(ctx)) return rc;
+        if (int rc = grow(ctx, ctx->d_scap_part, ctx->cap_scap_part, scap_units(ctx->peer_scap_pairs))) return rc;
+        if (int rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, ctx->peer_scap_pairs)) return rc;
     }
     // sharded preempt and place, after dra_set_shard_preempt_place: its kernels loaded and its buffers at full size now (no
     // module load and no cudaFree inside a call while a peer's exchange waits for this rank)
@@ -2853,6 +2882,105 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     ctx->launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded preemption launch: %s", cudaGetErrorString(e));
+    return DRA_OK;
+}
+
+int dra_set_shard_capacity(dra_ctx* ctx, uint32_t max_pairs) {
+    if (!ctx) return DRA_E_INVAL;
+    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "dra_set_shard_capacity: call it before dra_shard_export");
+    if (max_pairs > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "dra_set_shard_capacity: max_pairs %u above 2^32 - 16", max_pairs);
+    if (scap_units(max_pairs) > ((size_t)1 << 32) / 16)
+        return fail(ctx, DRA_E_INVAL, "dra_set_shard_capacity: one rank's slice would exceed 4 GiB");
+    ctx->scap_max_pairs = max_pairs;
+    return DRA_OK;
+}
+
+// Sharded pod capacity: offset checks and pair -> pod (k_uns_prep) -> the window's pairs into this rank's slice
+// (k_pods_capacity) -> push to every peer -> wait + merge into the caller's buffers, with the per-pod sums (k_scap_merge).
+// Enqueues only.
+int dra_pod_capacity_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                         const uint32_t* d_pod_off, uint32_t n_pod,
+                                         const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                         uint32_t max_copies, uint16_t* d_pair_copies, uint8_t* d_pair_stop,
+                                         uint64_t* d_pod_total, uint32_t* d_pod_nodes, uint32_t flags) {
+    if (!ctx || !d_pod_off || (n_claim && !d_claims)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_pod_capacity_batch_global_device: unknown flags 0x%x", flags);
+    if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (max_copies < 1 || max_copies > 65535) return fail(ctx, DRA_E_INVAL, "max_copies %u outside [1, 65535]", max_copies);
+    const bool dense = d_cand_nodes == nullptr && d_cand_off == nullptr;
+    if (!dense && (!d_cand_nodes || !d_cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
+    if (dense && (uint64_t)n_pod * ctx->n_node != n_pair)
+        return fail(ctx, DRA_E_INVAL, "dense form: n_pair %u != n_pod %u x n_node %u", n_pair, n_pod, ctx->n_node);
+    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    if (n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "n_pod %u too large for the sharded call (2^26)", n_pod);
+    const bool gather = ctx->world > 1;
+    if (gather) {
+        if (!ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the merge needs every rank's range)");
+        if (int rc = need_peers(ctx)) return rc;
+        if (ctx->shard_bounds[ctx->world] != ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard map does not span the inventory's %u nodes", ctx->n_node);
+        // no exchange reserved: even a call with no pairs pushes a header and raises flags, which would land in the
+        // peers' buffers at offset 0
+        if (!ctx->peer_scap_pairs)
+            return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_capacity(max_pairs > 0) was not called before dra_shard_export");
+        if (n_pair > ctx->peer_scap_pairs)
+            return fail(ctx, DRA_E_INVAL, "n_pair %u exceeds the max_pairs (%u) of dra_set_shard_capacity before dra_shard_export", n_pair, ctx->peer_scap_pairs);
+    }
+    if (n_pair && !d_pair_copies) return fail(ctx, DRA_E_INVAL, "pair_copies is NULL");
+    ctx->chain = DRA_K_POD_CAPACITY_SHARD; ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
+    CU(cudaSetDevice(ctx->device));
+    // peers on this device may already wait for this rank: no buffer this call outgrows is freed before the next sync
+    struct DeferFree { dra_ctx* c; ~DeferFree() { c->defer_free = false; } } defer{ctx};
+    ctx->defer_free = gather;
+    int rc = upload_table(ctx);
+    if (rc) return rc;
+    // world > 1: peer_setup sized both for max_pairs, so these never reallocate there
+    if ((rc = grow(ctx, ctx->d_scap_part, ctx->cap_scap_part, scap_units(n_pair)))) return rc;
+    if (!dense && (rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, n_pair))) return rc;
+    cudaStream_t st = ctx->stream;
+    const uint32_t lo = gather ? ctx->shard_lo : 0u, hi = gather ? ctx->shard_hi : ctx->n_node;   // world 1: every node
+    const uint32_t* gate = ctx->d_err + ERR_BAD_OFFSETS;
+    CapArgs a; memset(&a, 0, sizeof a);
+    a.claims = (const uint4*)d_claims; a.pod_off = d_pod_off; a.n_pod = n_pod;
+    a.cand_nodes = dense ? nullptr : d_cand_nodes; a.cand_off = dense ? nullptr : d_cand_off;
+    a.pair_pod = dense ? nullptr : ctx->d_upair_pod; a.n_pair = n_pair;
+    a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.tbl = ctx->d_tbl; a.sel = sel_of(ctx);
+    a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.max_copies = max_copies;
+    a.node_lo = lo; a.n_win = hi - lo; a.n_walk = dense ? n_pod * a.n_win : n_pair;   // (n_pod * n_win <= n_pair)
+    uint4* part = ctx->d_scap_part;
+    const size_t copies4 = ((size_t)a.n_walk + 7) / 8, stops4 = d_pair_stop ? ((size_t)a.n_walk + 15) / 16 : 0;
+    a.pair_copies = reinterpret_cast<uint16_t*>(part + 1);
+    a.pair_stop = d_pair_stop ? reinterpret_cast<uint8_t*>(part + 1 + copies4) : nullptr;
+    a.gate = gate;
+    Prof prof(ctx);
+    k_uns_prep<<<std::max(1u, (n_pod + 7) / 8), 256, 0, st>>>(d_pod_off, dense ? nullptr : d_cand_off, n_pod, n_claim, n_pair,
+                                                              ctx->d_upair_pod, err_of(ctx));
+    ctx->launches += 1;
+    if ((rc = launch_capacity(ctx, a))) return rc;
+    prof.mark();
+    CapMerge m; memset(&m, 0, sizeof m);
+    m.part = part; m.cand_nodes = a.cand_nodes; m.cand_off = a.cand_off;
+    m.n_pod = n_pod; m.n_pair = n_pair; m.n_node = ctx->n_node;
+    m.bounds[0] = 0; m.bounds[1] = ctx->n_node;
+    if (gather) for (int r = 0; r <= ctx->world; ++r) m.bounds[r] = ctx->shard_bounds[r];
+    m.gate = gate;
+    m.pair_copies = d_pair_copies; m.pair_stop = d_pair_stop; m.pod_total = (unsigned long long*)d_pod_total; m.pod_nodes = d_pod_nodes;
+    const PeerExchange x = gather ? bind_exchange(ctx, ctx->scap_x) : PeerExchange{};   // world 1: no peers
+    if (gather) {
+        m.slice4 = (uint32_t)(ctx->scap_x.slice / 16);
+        CU(cudaMemcpyAsync(part, gate, 4, cudaMemcpyDeviceToDevice, st));   // the header: this rank's fault word
+        const uint32_t n4 = (uint32_t)(1 + copies4 + stops4);
+        k_peer_push<<<std::max(1u, std::min((n4 + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, st>>>(x, part, 0u, n4);
+        ctx->launches += 1;
+    }
+    // a small grid: it waits for its peers, and ranks sharing one device must not find their evaluation's SMs held by it
+    const uint32_t merge_grid = std::max(1u, std::min((n_pod + 7) / 8, (uint32_t)std::max(1, ctx->n_sm / 4)));
+    k_scap_merge<<<merge_grid, 256, 0, st>>>(x, m);
+    ctx->launches += 1;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded pod capacity launch: %s", cudaGetErrorString(e));
     return DRA_OK;
 }
 

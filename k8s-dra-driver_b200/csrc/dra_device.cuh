@@ -4278,6 +4278,7 @@ k_spre_merge(const PeerExchange x, const PreMerge m) {
 //   k_pods_capacity      W lanes per (pod, node) pair: pod_eval on a register copy of the node, the placement kept each
 //                        time it succeeds, until one fails or max_copies are placed
 //   k_pods_capacity_sum  warp per pod: the pod's pairs summed, and those with a copy counted
+// The sharded call (dra_pod_capacity_batch_global_device) runs k_pods_capacity on its node window and k_scap_merge below.
 // ====================================================================================================
 struct CapArgs {
     const uint4* claims; const uint32_t* pod_off; uint32_t n_pod;
@@ -4285,18 +4286,26 @@ struct CapArgs {
     uint32_t n_pair;
     const uint4* inv; const uint32_t* node_off; uint32_t n_node; const uint32_t* tbl; SelCtx sel;
     uint32_t exhaustive, max_copies;
-    uint16_t* pair_copies; uint8_t* pair_stop;            // pair_stop: nullptr unless asked for
+    // the node window: the pairs of the nodes in [node_lo, node_lo + n_win), or of no node.  n_walk: the pairs walked,
+    // dense n_pod * n_win, else n_pair.  The single-inventory call: [0, n_node), n_walk = n_pair.
+    uint32_t node_lo, n_win, n_walk;
+    uint16_t* pair_copies; uint8_t* pair_stop;            // at the walk index; pair_stop: nullptr unless asked for
     unsigned long long* pod_total; uint32_t* pod_nodes;   // each nullptr unless asked for
     uint32_t* work;                                       // next unclaimed pair (zeroed by the host)
+    const uint32_t* gate;                                 // non-zero: the offsets failed their check (nullptr: none)
 };
 
 // k_pods_preempt's layout: W lanes per pair, 32/W pairs per warp, pairs taken from a counter, since a pair costs from one
 // evaluation to max_copies of them.  One writer per pair, so the results are plain stores and nothing is zeroed first.
 // A candidate naming no node, an empty pod and a pod of more than DRA_MAX_POD claims are answered without loading a node.
+// The results go to the walk index: dense walk w is pod w / n_win at node node_lo + w % n_win; in the candidate form the
+// walk index is the pair index, and a pair on a node outside the window is skipped.  With the window [0, n_node) the walk
+// index is the pair index in both forms.
 template <int WPC, int W>
 __global__ void __launch_bounds__(WPC * 32, 2)
 k_pods_capacity(const CapArgs a) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
+    if (a.gate && __ldcg(a.gate)) return;
     for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
     __syncthreads();
     constexpr uint32_t G = 32 / W;
@@ -4307,12 +4316,16 @@ k_pods_capacity(const CapArgs a) {
         uint32_t nxt = 0;
         if (lane == 0) nxt = atomicAdd(a.work, G);
         const uint32_t pw = __shfl_sync(FULLMASK, nxt, 0);
-        if (pw >= a.n_pair) break;
-        const uint32_t pair = pw + grp;
-        if (pair >= a.n_pair) continue;                                  // whole group skips together
+        if (pw >= a.n_walk) break;
+        const uint32_t pair = pw + grp;                                  // the walk index
+        if (pair >= a.n_walk) continue;                                  // whole group skips together
         uint32_t pod, node;
-        if (!a.cand_off) { pod = pair / a.n_node; node = pair - pod * a.n_node; }
-        else { pod = __ldg(&a.pair_pod[pair]); node = __ldg(&a.cand_nodes[pair]); }
+        if (!a.cand_off) { pod = pair / a.n_win; node = a.node_lo + (pair - pod * a.n_win); }
+        else {
+            node = __ldg(&a.cand_nodes[pair]);
+            if (node < a.n_node && node - a.node_lo >= a.n_win) continue;   // another rank's node
+            pod = __ldg(&a.pair_pod[pair]);
+        }
         const uint32_t c0 = __ldg(&a.pod_off[pod]), cnt = __ldg(&a.pod_off[pod + 1]) - c0;
         uint32_t copies = 0, stop = DRA_ST_POD;                           // a candidate naming no node: unsuitable (§8)
         if (node >= a.n_node) {}
@@ -4343,26 +4356,102 @@ k_pods_capacity(const CapArgs a) {
     }
 }
 
-// Warp per pod: the lanes stride the pod's pairs (dense: its row of n_node).  The counts are 16 bits each, so a lane's
-// sum needs 64 bits only beyond 65,537 pairs per lane; it is kept in 64 bits throughout and reduced with a shuffle tree.
-__global__ void __launch_bounds__(256)
-k_pods_capacity_sum(const CapArgs a) {
-    const uint32_t lane = threadIdx.x & 31, p = blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (p >= a.n_pod) return;
-    const unsigned long long k0 = a.cand_off ? __ldg(&a.cand_off[p]) : (unsigned long long)p * a.n_node;
-    const unsigned long long k1 = a.cand_off ? __ldg(&a.cand_off[p + 1]) : k0 + a.n_node;
+// A warp's sums over pod p's pairs [k0, k1), the lanes striding them: copies(k) gives pair k's count.  The counts are 16
+// bits each, so a lane's sum needs 64 bits only beyond 65,537 pairs per lane; it is kept in 64 bits throughout and reduced
+// with a shuffle tree.
+template <class F>
+__device__ __forceinline__ void cap_pod_sums(uint32_t p, uint32_t lane, unsigned long long k0, unsigned long long k1, F copies,
+                                             unsigned long long* pod_total, uint32_t* pod_nodes) {
     unsigned long long sum = 0;
     uint32_t nodes = 0;
     for (unsigned long long k = k0; k < k1; k += 32) {
-        const uint32_t c = k + lane < k1 ? (uint32_t)a.pair_copies[k + lane] : 0u;
+        const uint32_t c = k + lane < k1 ? copies(k + lane) : 0u;
         sum += c;
         nodes += __popc(__ballot_sync(FULLMASK, c != 0u));
     }
     #pragma unroll
     for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(FULLMASK, sum, d);
     if (lane == 0) {
-        if (a.pod_total) a.pod_total[p] = sum;
-        if (a.pod_nodes) a.pod_nodes[p] = nodes;
+        if (pod_total) pod_total[p] = sum;
+        if (pod_nodes) pod_nodes[p] = nodes;
+    }
+}
+
+// Warp per pod: the lanes stride the pod's pairs (dense: its row of n_node).
+__global__ void __launch_bounds__(256)
+k_pods_capacity_sum(const CapArgs a) {
+    const uint32_t lane = threadIdx.x & 31, p = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (p >= a.n_pod) return;
+    const unsigned long long k0 = a.cand_off ? __ldg(&a.cand_off[p]) : (unsigned long long)p * a.n_node;
+    const unsigned long long k1 = a.cand_off ? __ldg(&a.cand_off[p + 1]) : k0 + a.n_node;
+    cap_pod_sums(p, lane, k0, k1, [&](unsigned long long k) { return (uint32_t)a.pair_copies[k]; }, a.pod_total, a.pod_nodes);
+}
+
+// ---- sharded pod capacity (dra_pod_capacity_batch_global_device) --------------------------------------------------
+// Every rank gets the same pods and candidates.  k_uns_prep checks pod_off / cand_off and writes pair -> pod; its fault
+// word gates k_pods_capacity, which evaluates this rank's window into its slice; k_peer_push sends the slice to every
+// peer; k_scap_merge waits and writes the caller's buffers.  A rank's slice, in uint4 units, for its nw walked pairs
+// (dense n_pod * its window's width, else n_pair): [0] header {fault word}, then nw u16 copies padded to 16 bytes, then
+// (only when the caller asked for them) nw u8 stops padded to 16 bytes.  A pair's count depends on its own node's state
+// alone, so taking each pair from the rank that owns its node gives the single-inventory answer on the world's state for
+// any partition.
+struct CapMerge {
+    const uint4* part;            // this rank's slice; a peer's is at my_stage + sender * slice4
+    uint32_t slice4;              // uint4 units of one sender's slice in the exchange
+    const uint32_t* cand_nodes; const uint32_t* cand_off;   // cand_off == nullptr: dense form
+    uint32_t n_pod, n_pair, n_node;
+    uint32_t bounds[PEER_MAX + 1];   // rank r owns nodes [bounds[r], bounds[r + 1])
+    const uint32_t* gate;            // this rank's fault word
+    uint16_t* pair_copies; uint8_t* pair_stop;                   // the caller's (pair_stop: nullptr unless asked)
+    unsigned long long* pod_total; uint32_t* pod_nodes;          // the caller's (each nullptr unless asked)
+};
+
+// At most SMs / 4 CTAs, launched after the evaluation: ranks sharing one device must not find their evaluation's SMs
+// held by a peer's waiting CTAs.  Block 0 raises this rank's flags, every block waits and checks every rank's fault word;
+// then a warp per pod: each lane takes a pair from the slice of the rank owning its node (a candidate naming no node: 0
+// copies, POD), writes the pair's outputs and feeds the pod's sums.  Nothing is written after a fault or a timeout.  With
+// world 1 (an all-zero PeerExchange) nothing is waited for.
+__global__ void __launch_bounds__(256)
+k_scap_merge(const PeerExchange x, const CapMerge m) {
+    __shared__ uint32_t s_ok;
+    const uint32_t tid = threadIdx.x;
+    if (tid == 0) s_ok = 1u;
+    __syncthreads();
+    if (blockIdx.x == 0) peer_raise(x, tid);
+    if (!peer_wait(x, tid, clock64())) s_ok = 0u;
+    const uint32_t world = x.world ? x.world : 1u, rank = x.rank;
+    if (tid < world) {
+        const uint32_t f = tid == rank ? __ldcg(m.gate) : __ldcg(&x.my_stage[(size_t)tid * m.slice4]).x;
+        if (f) {
+            s_ok = 0u;
+            if (blockIdx.x == 0 && tid != rank) x.err.set(ERR_BAD_OFFSETS);   // a peer's fault fails the call here too
+        }
+    }
+    __syncthreads();
+    if (!s_ok) return;
+    const uint32_t lane = tid & 31;
+    const uint32_t warp = (blockIdx.x * blockDim.x + tid) >> 5, n_warp = (gridDim.x * blockDim.x) >> 5;
+    const bool dense = m.cand_off == nullptr;
+    for (uint32_t p = warp; p < m.n_pod; p += n_warp) {
+        const unsigned long long k0 = dense ? (unsigned long long)p * m.n_node : __ldg(&m.cand_off[p]);
+        const unsigned long long k1 = dense ? k0 + m.n_node : __ldg(&m.cand_off[p + 1]);
+        cap_pod_sums(p, lane, k0, k1, [&](unsigned long long k) {
+            const uint32_t node = dense ? (uint32_t)(k - k0) : __ldg(&m.cand_nodes[k]);
+            uint32_t copies = 0, stop = DRA_ST_POD;                        // a candidate naming no node
+            if (node < m.n_node) {
+                uint32_t r = 0;
+                while (r + 1 < world && m.bounds[r + 1] <= node) ++r;
+                const uint32_t lo = m.bounds[r], n_win = m.bounds[r + 1] - lo;
+                const uint32_t w = dense ? p * n_win + (node - lo) : (uint32_t)k;
+                const uint32_t nw = dense ? m.n_pod * n_win : m.n_pair;
+                const uint4* src = r == rank ? m.part : x.my_stage + (size_t)r * m.slice4;
+                copies = __ldcg(reinterpret_cast<const unsigned short*>(src + 1) + w);
+                if (m.pair_stop) stop = __ldcg(reinterpret_cast<const unsigned char*>(src + 1 + ((size_t)nw + 7) / 8) + w);
+            }
+            m.pair_copies[k] = (uint16_t)copies;
+            if (m.pair_stop) m.pair_stop[k] = (uint8_t)stop;
+            return copies;
+        }, m.pod_total, m.pod_nodes);
     }
 }
 
