@@ -419,7 +419,7 @@ int  dra_gather_read(dra_ctx* ctx, dra_out_rec* out_all, uint32_t n_rec);
  *                                              cudaIpcMemHandle_t;  the host runtime all-gathers the handles;
  *   dra_peer_import(ctx, handles)              world * 64 bytes, in rank order.
  * Requires all ranks on one node with P2P access; on failure the NCCL path stays in use.  Every rank must export alike (the
- * same sizes, dra_set_shard_pairs, dra_set_shard_place, dra_set_shard_preempt, dra_set_shard_capacity and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
+ * same sizes, dra_set_shard_pairs, dra_set_shard_place, dra_set_shard_preempt, dra_set_shard_capacity, dra_set_shard_preempt_place and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
  * own layout, so dra_peer_import / dra_peer_import_local refuse a peer set up differently with DRA_E_INVAL.
  * dra_peer_export(ctx, 0, NULL) switches the peer path off again. */
 int  dra_peer_export(dra_ctx* ctx, uint32_t n_per_rank, void* handle64);

@@ -71,6 +71,15 @@ struct PeerRegion {
     uint32_t seq = 0;             // the exchange's last call
 };
 
+// The sizes the sharded calls' peer exchanges are reserved for, one group per dra_set_shard_* setter
+struct ShardSizes {
+    uint32_t uns_pairs;                             // dra_set_shard_pairs
+    uint32_t place_pods;                            // dra_set_shard_place
+    uint32_t pre_pods, pre_pairs, pre_victims;      // dra_set_shard_preempt
+    uint32_t scap_pairs;                            // dra_set_shard_capacity
+    uint32_t spp_pods, spp_pairs, spp_run;          // dra_set_shard_preempt_place
+};
+
 struct dra_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -197,33 +206,28 @@ struct dra_ctx {
     uint32_t* h_sc_counts_dev = nullptr;
     uint2* d_gtable = nullptr; size_t cap_gtable = 0;   // result table when no peers are set up (world 1)
     uint32_t* d_ticket = nullptr;
+    ShardSizes shard_req{};                     // the sizes the setters asked for, reserved by the next peer_setup
+    ShardSizes shard_rsv{};                     // the sizes the last peer_setup reserved
     // sharded UnsuitableNodes: bit exchange in the peer buffer ([staging x2: world slices of uns_stride words][flags])
-    uint32_t uns_max_pairs = 0;                 // dra_set_shard_pairs, reserved by the next peer_setup
-    uint32_t peer_uns_pairs = 0, uns_stride = 0;
+    uint32_t uns_stride = 0;
     uint32_t* d_ubits = nullptr; size_t cap_ubits = 0;   // this rank's words of the call
     uint32_t* d_upair_pod = nullptr; size_t cap_upair_pod = 0;   // candidate form: pair -> pod (k_uns_prep)
     // sharded pods Allocate
     uint32_t* d_spod = nullptr;                 // [SP_WORDS] call words (dra_device.cuh SPodArgs)
     // sharded place pods: a region [progress counter, 64 bytes][state words: u64 per pod] (dra_device.cuh PlaceShard) in
     // the peer buffer at world > 1, in d_splace_local at world 1
-    uint32_t place_max_pods = 0;                // dra_set_shard_place, reserved by the next peer_setup
-    uint32_t peer_place_pods = 0; size_t off_splace = 0;
+    size_t off_splace = 0;
     uint8_t* d_splace_local = nullptr; size_t cap_splace_local = 0;    // pods
     uint32_t splace_seq = 0;                    // the last call's sequence number (peer_setup starts over: fresh words)
     uint4* d_splace_rec = nullptr; size_t cap_splace_rec = 0;          // [n_pod] finaliser records for k_spod_gather
     // sharded preemption: a region [partials x2: world slices][flags] (dra_device.cuh PreShard) in the peer buffer
-    uint32_t pre_max_pods = 0, pre_max_pairs = 0, pre_max_victims = 0;   // dra_set_shard_preempt, reserved by the next peer_setup
-    uint32_t peer_pre_pods = 0, peer_pre_pairs = 0, peer_pre_victims = 0;
     PeerRegion pre_x;
     uint4* d_spre_part = nullptr; size_t cap_spre_part = 0;           // this rank's partials and pair results (uint4 units)
     // sharded preempt and place: the world's state assembled for the call (scratch inventory), and the call's gate word
-    uint32_t spp_max_pods = 0, spp_max_pairs = 0, spp_max_run = 0;     // dra_set_shard_preempt_place, reserved by the next peer_setup
-    uint32_t peer_spp_pods = 0, peer_spp_pairs = 0, peer_spp_run = 0;
     uint4* d_spp_inv = nullptr; size_t cap_spp_inv = 0;
     uint32_t* d_spp_gate = nullptr;
     PeerRegion spp_x;                           // the verdict agreement's flags (k_spp_agree), after the exchange
     // sharded pod capacity: a region [slices x2: world slices][flags] (dra_device.cuh CapMerge) in the peer buffer
-    uint32_t scap_max_pairs = 0, peer_scap_pairs = 0;   // dra_set_shard_capacity; reserved by the next peer_setup
     PeerRegion scap_x;
     uint4* d_scap_part = nullptr; size_t cap_scap_part = 0;           // this rank's slice (uint4 units)
     int splace_occ = -1;                        // resident CTAs of k_pods_place<4, true> per SM (occupancy query, once)
@@ -1042,6 +1046,80 @@ int launch_capacity(dra_ctx* ctx, CapArgs a) {
     }
     return DRA_OK;
 }
+
+// A sharded call at world > 1 needs the sharded form of the peer buffer, exported and imported
+int need_peers(dra_ctx* ctx) {
+    if (ctx->world <= 1 || (ctx->peer_ready && ctx->peer_form == 2)) return DRA_OK;
+    return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
+}
+
+// k_peer_push's grid for n units: a CTA per 256, at most two per SM
+uint32_t push_grid(const dra_ctx* ctx, uint32_t n) { return std::max(1u, std::min((n + 255) / 256, (uint32_t)ctx->n_sm * 2u)); }
+
+// The grid of a kernel that waits for its peers, for work CTAs' worth of work: at most SMs / 4 CTAs, because ranks
+// sharing one device must not find the SMs of their own evaluation, walk, sort or push held by a peer's waiting CTAs
+uint32_t wait_grid(const dra_ctx* ctx, size_t work) {
+    return (uint32_t)std::max<size_t>(1, std::min<size_t>(work, (size_t)std::max(1, ctx->n_sm / 4)));
+}
+
+// A setter of the sizes dra_shard_export reserves: at world > 1, only before the export
+int check_before_export(dra_ctx* ctx, const char* setter) {
+    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "%s: call it before dra_shard_export", setter);
+    return DRA_OK;
+}
+
+// The candidates of a sharded call, as device pointers: cand_nodes and cand_off both or neither (the dense form), at most
+// 0xFFFFFFF0 pairs.  dense_all: the dense form has n_pair == n_pod * n_node pairs, else it gives n_pair 0.
+int check_dev_cands(dra_ctx* ctx, const uint32_t* cand_nodes, const uint32_t* cand_off, uint32_t n_pod, uint32_t n_pair,
+                    bool dense_all, bool& dense) {
+    dense = cand_nodes == nullptr && cand_off == nullptr;
+    if (!dense && (!cand_nodes || !cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
+    if (dense && dense_all && (uint64_t)n_pod * ctx->n_node != n_pair)
+        return fail(ctx, DRA_E_INVAL, "dense form: n_pair %u != n_pod %u x n_node %u", n_pair, n_pod, ctx->n_node);
+    if (dense && !dense_all && n_pair) return fail(ctx, DRA_E_INVAL, "dense form: n_pair must be 0");
+    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    return DRA_OK;
+}
+
+// The inventory sync's exchange: reserved by dra_shard_export for the inventory loaded then, which has not grown since
+int check_inv_exchange(dra_ctx* ctx) {
+    if (!ctx->peer_inv_gpus) return fail(ctx, DRA_E_STATE, "the inventory was not loaded before dra_shard_export: the export reserved no staging for it");
+    if (ctx->n_gpu > ctx->peer_inv_gpus)
+        return fail(ctx, DRA_E_STATE, "the inventory grew to %u GPUs after dra_shard_export reserved staging for %u", ctx->n_gpu, ctx->peer_inv_gpus);
+    return DRA_OK;
+}
+
+constexpr auto no_check = [] { return (int)DRA_OK; };
+
+// What a sharded call needs at world > 1 besides its arguments, in this order: dra_set_shard_map (map_use: what needs every
+// rank's range; nullptr: nothing does), a map spanning the inventory (spanning), the peers, reserved() (the call's
+// exchange reserved by its setter before the export), n_out within the exported table (n_out < 0: the call has no table),
+// fits() (the call within the reserved sizes).
+template <class Reserved, class Fits>
+int check_world(dra_ctx* ctx, const char* map_use, bool spanning, Reserved reserved, int64_t n_out, Fits fits) {
+    if (ctx->world <= 1) return DRA_OK;
+    if (map_use && !ctx->shard_map_on)
+        return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (%s every rank's range)", map_use);
+    if (int rc = need_peers(ctx)) return rc;
+    if (spanning && ctx->shard_bounds[ctx->world] != ctx->n_node)
+        return fail(ctx, DRA_E_STATE, "the shard map does not span the inventory's %u nodes", ctx->n_node);
+    if (int rc = reserved()) return rc;
+    if (n_out > (int64_t)ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", (uint32_t)n_out, ctx->peer_tab_len);
+    return fits();
+}
+
+// The scope of a sharded call that enqueues: open() sets its device, and uploads the table.  Peers on this device may
+// already wait for this rank (gather: world > 1), so no buffer the call outgrows is freed before the next dra_ctx_sync
+// (defer_free, cleared when the scope ends).
+struct CallScope {
+    dra_ctx* ctx;
+    ~CallScope() { ctx->defer_free = false; }
+    int open(bool gather) {
+        CU(cudaSetDevice(ctx->device));
+        ctx->defer_free = gather;
+        return upload_table(ctx);
+    }
+};
 
 }  // namespace
 
@@ -1969,59 +2047,38 @@ namespace {
 // What a peer buffer's layout depends on.  Every rank computes its peers' offsets from its OWN layout, so an import requires
 // every rank to be set up alike; the export writes this at offset 0 of the buffer for importers in other processes to read.
 struct PeerLayout {
-    uint32_t world, rank, form, cap, tab_len, uns_pairs, inv_gpus, rsvd;      // rsvd: dra_set_shard_place's max_pods
-    uint32_t pre_pods, pre_pairs, pre_victims, scap_pairs;                    // dra_set_shard_preempt's sizes, dra_set_shard_capacity's
-    uint32_t spp_pods, spp_pairs, spp_run, pad2;                              // dra_set_shard_preempt_place's sizes
+    uint32_t world, rank, form, cap, tab_len, inv_gpus;
+    ShardSizes sizes;
+    uint32_t pad;
     bool operator==(const PeerLayout& o) const { return memcmp(this, &o, sizeof o) == 0; }
 };
 PeerLayout layout_of(const dra_ctx* c, int rank) {
     PeerLayout l; memset(&l, 0, sizeof l);
     l.world = (uint32_t)c->world; l.rank = (uint32_t)rank; l.form = c->peer_form; l.cap = c->peer_cap; l.tab_len = c->peer_tab_len;
-    l.uns_pairs = c->peer_uns_pairs; l.inv_gpus = c->peer_inv_gpus; l.rsvd = c->peer_place_pods;
-    l.pre_pods = c->peer_pre_pods; l.pre_pairs = c->peer_pre_pairs; l.pre_victims = c->peer_pre_victims; l.scap_pairs = c->peer_scap_pairs;
-    l.spp_pods = c->peer_spp_pods; l.spp_pairs = c->peer_spp_pairs; l.spp_run = c->peer_spp_run;
+    l.inv_gpus = c->peer_inv_gpus; l.sizes = c->shard_rsv;
     return l;
 }
 
-// Loads every kernel of the sharded place-pods chain now.  With lazy module loading (CUDA's default) the first launch of a
-// kernel loads it, and the load waits for the kernels running on the device.  A rank's walk waits for its peers' walks, so
-// a host thread that enqueues the ranks of one process one after the other would stall at rank 0's first launch after
-// the walk until the walk gives up.  Called while no call of the world is in flight.
-int preload_place_shard(dra_ctx* ctx) {
-    const void* ks[] = {(const void*)k_splace_prep, (const void*)k_spod_gate, (const void*)k_pods_place<4, true>,
-                        (const void*)k_splace_final, (const void*)k_spod_gather<true>, (const void*)k_bucket_small,
-                        (const void*)k_bucket_hist8<false>, (const void*)k_bucket_hist8<true>, (const void*)k_bucket_scan_rows,
-                        (const void*)k_bucket_scan8, (const void*)k_bucket_hist, (const void*)k_bucket_scan,
-                        (const void*)k_bucket_scatter};
-    for (const void* k : ks) { cudaFuncAttributes fa; CU(cudaFuncGetAttributes(&fa, k)); }
-    // An SM holds CTAs of one L1/shared split at a time.  With ranks on one device, a rank's walk (and its waiting gather)
-    // may sit on every SM while a peer's counting sort still has to run, and the sort's CTA-wide histogram wants most of
-    // the shared memory: the kernels that wait take the all-shared split too, so the sort's CTAs fit beside them.
-    const void* waiting[] = {(const void*)k_pods_place<4, true>, (const void*)k_spod_gather<true>};
+using Kernels = std::initializer_list<const void*>;
+
+// The counting sort's kernels (launch_sort), for the sharded chains that sort
+const Kernels SORT_KERNELS = {(const void*)k_bucket_small, (const void*)k_bucket_hist8<false>, (const void*)k_bucket_hist8<true>,
+                              (const void*)k_bucket_scan_rows, (const void*)k_bucket_scan8, (const void*)k_bucket_hist,
+                              (const void*)k_bucket_scan, (const void*)k_bucket_scatter};
+
+// Loads the kernels of a sharded chain now: ks, and waiting, those of its kernels that wait for its peers.  With lazy module
+// loading (CUDA's default) the first launch of a kernel loads it, and the load waits for the kernels running on the
+// device.  A rank's walk, merge or gather waits for its peers, so a host thread that enqueues the ranks of one process one
+// after the other would stall at rank 0's first launch after such a kernel until the wait gives up.  Called while no call
+// of the world is in flight.
+// An SM holds CTAs of one L1/shared split at a time.  With ranks on one device, a rank's waiting kernels may sit on every
+// SM while a peer's counting sort still has to run, and the sort's CTA-wide histogram wants most of the shared memory:
+// the kernels that wait take the all-shared split, so the sort's CTAs fit beside them.
+// sorts: the chain runs the counting sort.
+int preload(dra_ctx* ctx, Kernels ks, Kernels waiting, bool sorts) {
+    for (Kernels l : {ks, waiting, sorts ? SORT_KERNELS : Kernels{}})
+        for (const void* k : l) { cudaFuncAttributes fa; CU(cudaFuncGetAttributes(&fa, k)); }
     for (const void* k : waiting) CU(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    return DRA_OK;
-}
-
-// The same for the sharded preemption chain, whose merge waits for its peers: it also takes the all-shared split.
-int preload_preempt_shard(dra_ctx* ctx) {
-    const void* ks[] = {(const void*)k_uns_prep, (const void*)k_pre_running, (const void*)k_pre_vsort,
-                        (const void*)k_pods_preempt<8, 8>, (const void*)k_pods_preempt<8, 16>, (const void*)k_pods_preempt<8, 32>,
-                        (const void*)k_spre_reduce, (const void*)k_pods_preempt_victims<8, 8>, (const void*)k_pods_preempt_victims<8, 16>,
-                        (const void*)k_pods_preempt_victims<8, 32>, (const void*)k_peer_push, (const void*)k_spre_merge,
-                        (const void*)k_bucket_small, (const void*)k_bucket_hist8<false>, (const void*)k_bucket_hist8<true>,
-                        (const void*)k_bucket_scan_rows, (const void*)k_bucket_scan8, (const void*)k_bucket_hist,
-                        (const void*)k_bucket_scan, (const void*)k_bucket_scatter};
-    for (const void* k : ks) { cudaFuncAttributes fa; CU(cudaFuncGetAttributes(&fa, k)); }
-    CU(cudaFuncSetAttribute((const void*)k_spre_merge, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    return DRA_OK;
-}
-
-// The same for the sharded pod-capacity chain, whose merge waits for its peers: it also takes the all-shared split.
-int preload_capacity_shard(dra_ctx* ctx) {
-    const void* ks[] = {(const void*)k_uns_prep, (const void*)k_pods_capacity<8, 8>, (const void*)k_pods_capacity<8, 16>,
-                        (const void*)k_pods_capacity<8, 32>, (const void*)k_peer_push, (const void*)k_scap_merge};
-    for (const void* k : ks) { cudaFuncAttributes fa; CU(cudaFuncGetAttributes(&fa, k)); }
-    CU(cudaFuncSetAttribute((const void*)k_scap_merge, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     return DRA_OK;
 }
 
@@ -2029,15 +2086,13 @@ int preload_capacity_shard(dra_ctx* ctx) {
 // n u8 stops, each padded to 16 bytes
 size_t scap_units(uint32_t n) { return 1 + ((size_t)n + 7) / 8 + ((size_t)n + 15) / 16; }
 
-// The same for the sharded preempt-and-place chain, and the walk's occupancy query (which loads it too).  Its one wait is
-// the inventory exchange (k_isync_copy), before the walk.
+// The sharded preempt-and-place chain's kernels (preload), and the walk's occupancy query (which loads it too).  Its one
+// wait is the inventory exchange (k_isync_copy), before the walk, and it keeps its split.
 int preload_preempt_place_shard(dra_ctx* ctx) {
-    const void* ks[] = {(const void*)k_peer_push, (const void*)k_isync_copy, (const void*)k_spp_agree, (const void*)k_pre_running, (const void*)k_pre_vsort,
-                        (const void*)k_spp_prep, (const void*)k_pods_preempt_place<4>, (const void*)k_spp_final,
-                        (const void*)k_bucket_small, (const void*)k_bucket_hist8<false>, (const void*)k_bucket_hist8<true>,
-                        (const void*)k_bucket_scan_rows, (const void*)k_bucket_scan8, (const void*)k_bucket_hist,
-                        (const void*)k_bucket_scan, (const void*)k_bucket_scatter};
-    for (const void* k : ks) { cudaFuncAttributes fa; CU(cudaFuncGetAttributes(&fa, k)); }
+    if (int rc = preload(ctx, {(const void*)k_peer_push, (const void*)k_isync_copy, (const void*)k_spp_agree,
+                               (const void*)k_pre_running, (const void*)k_pre_vsort, (const void*)k_spp_prep,
+                               (const void*)k_pods_preempt_place<4>, (const void*)k_spp_final}, {}, true))
+        return rc;
     if (ctx->pp_occ < 0) {
         int occ = 0;
         CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_preempt_place<4>, 128, 0));
@@ -2099,55 +2154,63 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
     for (int p = 0; p < 2; ++p) ctx->off_stage[p] = take((size_t)ctx->world * cap * 16);
     for (int p = 0; p < 2; ++p) ctx->off_hdr[p] = take((size_t)ctx->world * 16);
     reserve(ctx->rendezvous_x, 0, 0, (size_t)PEER_MAX * 4);
-    ctx->peer_uns_pairs = ctx->uns_max_pairs;
-    ctx->uns_stride = (uint32_t)(((size_t)ctx->uns_max_pairs + 127) / 128 * 4);     // words, whole 16-byte units
+    ctx->shard_rsv = ctx->shard_req;
+    const ShardSizes& z = ctx->shard_rsv;
+    ctx->uns_stride = (uint32_t)(((size_t)z.uns_pairs + 127) / 128 * 4);     // words, whole 16-byte units
     if (ctx->uns_stride) {
         reserve(ctx->uns_x, (size_t)ctx->world * ctx->uns_stride * 4, (size_t)ctx->uns_stride * 4, (size_t)PEER_MAX * 4);
         // the call's own buffers at full size now: growing one inside the call would cudaFree the old one, which waits for
         // the whole device — where a peer's merge may already be spinning for this rank's push (ranks sharing a device)
         int rc;
         if ((rc = grow(ctx, ctx->d_ubits, ctx->cap_ubits, ctx->uns_stride))) return rc;
-        if ((rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, ctx->uns_max_pairs))) return rc;
+        if ((rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, z.uns_pairs))) return rc;
     }
     // the inventory sync's staging, sized for the inventory loaded now (sharded form only); its flags, then `elect` [2]
     ctx->peer_inv_gpus = form == 2 && ctx->d_inv_live ? ctx->n_gpu : 0u;
     if (ctx->peer_inv_gpus) reserve(ctx->isync_x, (size_t)ctx->peer_inv_gpus * 16, 0, (size_t)(PEER_MAX + 2) * 4);
     // sharded place pods, after dra_set_shard_place: the replicated state words (zeroed below, so the sequence starts over)
-    ctx->peer_place_pods = ctx->place_max_pods;
-    if (ctx->peer_place_pods) {
-        ctx->off_splace = take(64 + (size_t)ctx->peer_place_pods * 8);
-        if (int rc = preload_place_shard(ctx)) return rc;
+    if (z.place_pods) {
+        ctx->off_splace = take(64 + (size_t)z.place_pods * 8);
+        if (int rc = preload(ctx, {(const void*)k_splace_prep, (const void*)k_spod_gate, (const void*)k_splace_final},
+                             {(const void*)k_pods_place<4, true>, (const void*)k_spod_gather<true>}, true))
+            return rc;
         // the sort's scan-status words for the loaded inventory now: ensure_batch grows them with a cudaFree, which waits
         // for the whole device — where, inside a call, a peer's walk may be waiting for this rank
         if (ctx->d_inv_live) { if (int rc = ensure_batch(ctx, 1, 1, false)) return rc; }
     }
     // sharded preemption, after dra_set_shard_preempt: the partials' exchange, and the call's scratch at full size now (no
     // cudaFree inside a call while a peer's merge waits for this rank)
-    ctx->peer_pre_pods = ctx->pre_max_pods; ctx->peer_pre_pairs = ctx->pre_max_pairs; ctx->peer_pre_victims = ctx->pre_max_victims;
-    if (ctx->peer_pre_pods) {
-        const size_t slice = spre_units(ctx->peer_pre_pods, ctx->peer_pre_pairs, ctx->peer_pre_victims) * 16;
+    if (z.pre_pods) {
+        const size_t slice = spre_units(z.pre_pods, z.pre_pairs, z.pre_victims) * 16;
         reserve(ctx->pre_x, (size_t)ctx->world * slice, slice, (size_t)PEER_MAX * 4);
-        if (int rc = preload_preempt_shard(ctx)) return rc;
-        if (int rc = spre_buffers(ctx, ctx->peer_pre_pods, ctx->peer_pre_pairs, ctx->peer_pre_victims, 0)) return rc;
+        if (int rc = preload(ctx, {(const void*)k_uns_prep, (const void*)k_pre_running, (const void*)k_pre_vsort,
+                                   (const void*)k_pods_preempt<8, 8>, (const void*)k_pods_preempt<8, 16>,
+                                   (const void*)k_pods_preempt<8, 32>, (const void*)k_spre_reduce,
+                                   (const void*)k_pods_preempt_victims<8, 8>, (const void*)k_pods_preempt_victims<8, 16>,
+                                   (const void*)k_pods_preempt_victims<8, 32>, (const void*)k_peer_push},
+                             {(const void*)k_spre_merge}, true))
+            return rc;
+        if (int rc = spre_buffers(ctx, z.pre_pods, z.pre_pairs, z.pre_victims, 0)) return rc;
         if (ctx->d_inv_live) { if (int rc = ensure_batch(ctx, 1, 1, false)) return rc; }
     }
     // sharded pod capacity, after dra_set_shard_capacity: the slices' exchange, and the call's scratch at full size now (no
     // cudaFree inside a call while a peer's merge waits for this rank)
-    ctx->peer_scap_pairs = ctx->scap_max_pairs;
-    if (ctx->peer_scap_pairs) {
-        const size_t slice = scap_units(ctx->peer_scap_pairs) * 16;
+    if (z.scap_pairs) {
+        const size_t slice = scap_units(z.scap_pairs) * 16;
         reserve(ctx->scap_x, (size_t)ctx->world * slice, slice, (size_t)PEER_MAX * 4);
-        if (int rc = preload_capacity_shard(ctx)) return rc;
-        if (int rc = grow(ctx, ctx->d_scap_part, ctx->cap_scap_part, scap_units(ctx->peer_scap_pairs))) return rc;
-        if (int rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, ctx->peer_scap_pairs)) return rc;
+        if (int rc = preload(ctx, {(const void*)k_uns_prep, (const void*)k_pods_capacity<8, 8>, (const void*)k_pods_capacity<8, 16>,
+                                   (const void*)k_pods_capacity<8, 32>, (const void*)k_peer_push},
+                             {(const void*)k_scap_merge}, false))
+            return rc;
+        if (int rc = grow(ctx, ctx->d_scap_part, ctx->cap_scap_part, scap_units(z.scap_pairs))) return rc;
+        if (int rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, z.scap_pairs)) return rc;
     }
     // sharded preempt and place, after dra_set_shard_preempt_place: its kernels loaded and its buffers at full size now (no
     // module load and no cudaFree inside a call while a peer's exchange waits for this rank)
-    ctx->peer_spp_pods = ctx->spp_max_pods; ctx->peer_spp_pairs = ctx->spp_max_pairs; ctx->peer_spp_run = ctx->spp_max_run;
-    if (ctx->peer_spp_pods) {
+    if (z.spp_pods) {
         reserve(ctx->spp_x, 0, 0, (size_t)PEER_MAX * 4);
         if (int rc = preload_preempt_place_shard(ctx)) return rc;
-        if (ctx->d_inv_live) { if (int rc = spp_buffers(ctx, ctx->peer_spp_pods, ctx->peer_spp_pairs, ctx->peer_spp_run)) return rc; }
+        if (ctx->d_inv_live) { if (int rc = spp_buffers(ctx, z.spp_pods, z.spp_pairs, z.spp_run)) return rc; }
         if (int rc = grow_set(ctx, ctx->cap_gtable, (size_t)tab_len + 16, ctx->d_gtable)) return rc;   // the call's table, at the exported size
     }
     ctx->splace_seq = 0;
@@ -2206,12 +2269,6 @@ int result_table(dra_ctx* ctx, uint32_t n_out, const uint32_t* count_dev, PktGat
     }
     table = ctx->world > 1 ? g.table : ctx->d_gtable;
     return DRA_OK;
-}
-
-// A sharded call at world > 1 needs the sharded form of the peer buffer, exported and imported
-int need_peers(dra_ctx* ctx) {
-    if (ctx->world <= 1 || (ctx->peer_ready && ctx->peer_form == 2)) return DRA_OK;
-    return fail(ctx, DRA_E_STATE, "dra_shard_export + dra_peer_import have not been called");
 }
 
 // A sharded call's claims and OutRec slots: at most 2^26 of each, and without out_off one slot per claim at least
@@ -2493,9 +2550,9 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
 
 int dra_set_shard_pairs(dra_ctx* ctx, uint32_t max_pairs) {
     if (!ctx) return DRA_E_INVAL;
-    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "dra_set_shard_pairs: call it before dra_shard_export");
+    if (int rc = check_before_export(ctx, "dra_set_shard_pairs")) return rc;
     if (max_pairs > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "max_pairs %u: too many (pod, node) pairs", max_pairs);
-    ctx->uns_max_pairs = max_pairs;
+    ctx->shard_req.uns_pairs = max_pairs;
     return DRA_OK;
 }
 
@@ -2510,19 +2567,19 @@ int dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_unsuitable_batch_global_device: unknown flags 0x%x", flags);
     if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
-    const bool dense = d_cand_nodes == nullptr && d_cand_off == nullptr;
-    if (!dense && (!d_cand_nodes || !d_cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
-    if (dense && (uint64_t)n_pod * ctx->n_node != n_pair)
-        return fail(ctx, DRA_E_INVAL, "dense form: n_pair %u != n_pod %u x n_node %u", n_pair, n_pod, ctx->n_node);
-    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    bool dense;
+    if (int rc = check_dev_cands(ctx, d_cand_nodes, d_cand_off, n_pod, n_pair, true, dense)) return rc;
     const bool gather = ctx->world > 1;
-    if (int rc = need_peers(ctx)) return rc;
-    if (gather && n_pair > ctx->peer_uns_pairs)
-        return fail(ctx, DRA_E_INVAL, "n_pair %u exceeds the max_pairs (%u) of dra_set_shard_pairs before dra_shard_export", n_pair, ctx->peer_uns_pairs);
+    const uint32_t max_pairs = ctx->shard_rsv.uns_pairs;
+    if (int rc = check_world(ctx, nullptr, false, no_check, -1, [&] {
+            if (n_pair <= max_pairs) return (int)DRA_OK;
+            return fail(ctx, DRA_E_INVAL, "n_pair %u exceeds the max_pairs (%u) of dra_set_shard_pairs before dra_shard_export", n_pair, max_pairs);
+        }))
+        return rc;
     if (n_pair && !d_suitable_bits) return DRA_E_INVAL;
     if (!n_pair) return DRA_OK;                        // every rank sees the same n_pair: none of them exchanges anything
-    CU(cudaSetDevice(ctx->device));
-    int rc = upload_table(ctx);
+    CallScope scope{ctx};
+    int rc = scope.open(gather);
     if (rc) return rc;
     const size_t n_words = ((size_t)n_pair + 31) / 32, n_words4 = ((size_t)n_pair + 127) / 128 * 4;
     // world > 1: peer_setup sized both for max_pairs, so these never reallocate there (no cudaFree while peers wait)
@@ -2552,11 +2609,10 @@ int dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     const PeerExchange x = gather ? bind_exchange(ctx, ctx->uns_x) : PeerExchange{};   // world 1: no peers
     if (gather) {
         const uint32_t n4 = (uint32_t)(n_words4 / 4);
-        k_peer_push<<<std::max(1u, std::min((n4 + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, ctx->stream>>>(x, (const uint4*)ctx->d_ubits, 0u, n4);
+        k_peer_push<<<push_grid(ctx, n4), 256, 0, ctx->stream>>>(x, (const uint4*)ctx->d_ubits, 0u, n4);
         ctx->launches += 1;
     }
-    const uint32_t merge_grid = std::max(1u, std::min((uint32_t)((n_words + 1023) / 1024), (uint32_t)std::max(1, ctx->n_sm / 4)));
-    k_uns_merge<<<merge_grid, 256, 0, ctx->stream>>>(x, m);
+    k_uns_merge<<<wait_grid(ctx, (n_words + 1023) / 1024), 256, 0, ctx->stream>>>(x, m);
     ctx->launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded UnsuitableNodes launch: %s", cudaGetErrorString(e));
@@ -2579,16 +2635,11 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     if (int rc = check_slots(ctx, n_claim, n_out, d_out_off != nullptr)) return rc;
     if (!n_pod && n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]: no pods for %u claims", n_claim);
     const bool gather = ctx->world > 1;
-    if (gather && !ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the gather needs every rank's range)");
-    if (int rc = need_peers(ctx)) return rc;
-    if (gather && n_out > ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", n_out, ctx->peer_tab_len);
+    if (int rc = check_world(ctx, "the gather needs", false, no_check, n_out, no_check)) return rc;
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
-    CU(cudaSetDevice(ctx->device));
-    // peers on this device may already wait for this rank: no buffer this call outgrows is freed before the next sync
-    struct DeferFree { dra_ctx* c; ~DeferFree() { c->defer_free = false; } } defer{ctx};
-    ctx->defer_free = gather;
-    int rc = upload_table(ctx);
+    CallScope scope{ctx};
+    int rc = scope.open(gather);
     if (rc) return rc;
     const uint32_t n_win = ctx->shard_hi - ctx->shard_lo;
     if ((rc = ensure_batch(ctx, n_pod, 1, false))) return rc;
@@ -2631,9 +2682,7 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     }
     prof.mark();
     if (gather) {
-        // a small grid: it waits for its peers, and ranks sharing one device must not find their sort / k_pods SMs held by it
-        const uint32_t blocks = std::max(1u, std::min((uint32_t)std::max(1, ctx->n_sm / 4), (std::max(n_pod, g.world * g.cap / 4u) + 255u) / 256u));
-        k_spod_gather<false><<<blocks, 256, 0, ctx->stream>>>(g, sa, ctx->peer_tab_len);
+        k_spod_gather<false><<<wait_grid(ctx, (std::max(n_pod, g.world * g.cap / 4u) + 255u) / 256u), 256, 0, ctx->stream>>>(g, sa, ctx->peer_tab_len);
         ctx->launches += 1; ctx->chain |= DRA_K_POD_GATHER;
     }
     cudaError_t e = cudaGetLastError();
@@ -2644,9 +2693,9 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
 
 int dra_set_shard_place(dra_ctx* ctx, uint32_t max_pods) {
     if (!ctx) return DRA_E_INVAL;
-    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "dra_set_shard_place: call it before dra_shard_export");
+    if (int rc = check_before_export(ctx, "dra_set_shard_place")) return rc;
     if (max_pods > (1u << 26)) return fail(ctx, DRA_E_INVAL, "max_pods %u exceeds 2^26", max_pods);
-    ctx->place_max_pods = max_pods;
+    ctx->shard_req.place_pods = max_pods;
     return DRA_OK;
 }
 
@@ -2667,24 +2716,20 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     if (n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
     if (int rc = check_slots(ctx, n_claim, n_out, d_out_off != nullptr)) return rc;
     if (!n_pod && n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]: no pods for %u claims", n_claim);
-    const bool dense = d_cand_nodes == nullptr && d_cand_off == nullptr;
-    if (!dense && (!d_cand_nodes || !d_cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
-    if (dense && n_pair) return fail(ctx, DRA_E_INVAL, "dense form: n_pair must be 0");
-    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    bool dense;
+    if (int rc = check_dev_cands(ctx, d_cand_nodes, d_cand_off, n_pod, n_pair, false, dense)) return rc;
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
     const bool gather = ctx->world > 1;
-    if (gather && !ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the walk and the gather need every rank's range)");
-    if (int rc = need_peers(ctx)) return rc;
-    if (gather && n_out > ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", n_out, ctx->peer_tab_len);
-    if (gather && n_pod > ctx->peer_place_pods)
-        return fail(ctx, DRA_E_STATE, "n_pod %u exceeds the max_pods (%u) of dra_set_shard_place before dra_shard_export", n_pod, ctx->peer_place_pods);
+    const uint32_t max_pods = ctx->shard_rsv.place_pods;
+    if (int rc = check_world(ctx, "the walk and the gather need", false, no_check, n_out, [&] {
+            if (n_pod <= max_pods) return (int)DRA_OK;
+            return fail(ctx, DRA_E_STATE, "n_pod %u exceeds the max_pods (%u) of dra_set_shard_place before dra_shard_export", n_pod, max_pods);
+        }))
+        return rc;
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
-    CU(cudaSetDevice(ctx->device));
-    // peers on this device may already wait for this rank: no buffer this call outgrows is freed before the next sync
-    struct DeferFree { dra_ctx* c; ~DeferFree() { c->defer_free = false; } } defer{ctx};
-    ctx->defer_free = gather;
-    int rc = upload_table(ctx);
+    CallScope scope{ctx};
+    int rc = scope.open(gather);
     if (rc) return rc;
     const uint32_t n_win = ctx->shard_hi - ctx->shard_lo;
     if ((rc = ensure_batch(ctx, std::max(n_pod, n_pair), 1, false))) return rc;
@@ -2767,9 +2812,7 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     prof.mark();
     if (gather) {
         k_spod_gate<<<1, 256, 0, ctx->stream>>>(sa, ctx->peer_cap, nullptr, ctx->d_inv_live, ctx->d_node_off);
-        // a small grid: it waits for its peers, and ranks sharing one device must not find their walk's SMs held by it
-        const uint32_t blocks = std::max(1u, std::min((uint32_t)std::max(1, ctx->n_sm / 4), (std::max(n_pod, g.world * g.cap / 4u) + 255u) / 256u));
-        k_spod_gather<true><<<blocks, 256, 0, ctx->stream>>>(g, sa, ctx->peer_tab_len);
+        k_spod_gather<true><<<wait_grid(ctx, (std::max(n_pod, g.world * g.cap / 4u) + 255u) / 256u), 256, 0, ctx->stream>>>(g, sa, ctx->peer_tab_len);
         ctx->launches += 2;
     }
     cudaError_t e = cudaGetLastError();
@@ -2780,12 +2823,13 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
 
 int dra_set_shard_preempt(dra_ctx* ctx, uint32_t max_pods, uint32_t max_pairs, uint32_t max_victims) {
     if (!ctx) return DRA_E_INVAL;
-    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "dra_set_shard_preempt: call it before dra_shard_export");
+    if (int rc = check_before_export(ctx, "dra_set_shard_preempt")) return rc;
     if (max_pods > (1u << 26) || max_pairs > 0xFFFFFFF0u || max_victims > (1u << 20))
         return fail(ctx, DRA_E_INVAL, "dra_set_shard_preempt: sizes too large (max_pods <= 2^26, max_victims <= 2^20)");
     if (spre_units(max_pods, max_pairs, max_victims) > ((size_t)1 << 32) / 16)
         return fail(ctx, DRA_E_INVAL, "dra_set_shard_preempt: one rank's slice would exceed 4 GiB");
-    ctx->pre_max_pods = max_pods; ctx->pre_max_pairs = max_pairs; ctx->pre_max_victims = max_victims;
+    ShardSizes& z = ctx->shard_req;
+    z.pre_pods = max_pods; z.pre_pairs = max_pairs; z.pre_victims = max_victims;
     return DRA_OK;
 }
 
@@ -2809,28 +2853,21 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_preempt_batch_global_device: unknown flags 0x%x", flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     if (max_victims && !d_victims) return fail(ctx, DRA_E_INVAL, "max_victims %u without a victims buffer", max_victims);
-    const bool dense = d_cand_nodes == nullptr && d_cand_off == nullptr;
-    if (!dense && (!d_cand_nodes || !d_cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
-    if (dense && (uint64_t)n_pod * ctx->n_node != n_pair)
-        return fail(ctx, DRA_E_INVAL, "dense form: n_pair %u != n_pod %u x n_node %u", n_pair, n_pod, ctx->n_node);
-    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    bool dense;
+    if (int rc = check_dev_cands(ctx, d_cand_nodes, d_cand_off, n_pod, n_pair, true, dense)) return rc;
     if (n_pod > (1u << 26) || max_victims > (1u << 20)) return fail(ctx, DRA_E_INVAL, "n_pod or max_victims too large for the sharded call");
     const bool gather = ctx->world > 1;
-    if (gather) {
-        if (!ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the merge needs every rank's range)");
-        if (int rc = need_peers(ctx)) return rc;
-        if (ctx->shard_bounds[ctx->world] != ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard map does not span the inventory's %u nodes", ctx->n_node);
-        if (n_pod > ctx->peer_pre_pods || n_pair > ctx->peer_pre_pairs || max_victims > ctx->peer_pre_victims)
+    const ShardSizes& z = ctx->shard_rsv;
+    if (int rc = check_world(ctx, "the merge needs", true, no_check, -1, [&] {
+            if (n_pod <= z.pre_pods && n_pair <= z.pre_pairs && max_victims <= z.pre_victims) return (int)DRA_OK;
             return fail(ctx, DRA_E_INVAL, "n_pod %u / n_pair %u / max_victims %u exceed the sizes of dra_set_shard_preempt before dra_shard_export "
-                        "(%u / %u / %u)", n_pod, n_pair, max_victims, ctx->peer_pre_pods, ctx->peer_pre_pairs, ctx->peer_pre_victims);
-    }
+                        "(%u / %u / %u)", n_pod, n_pair, max_victims, z.pre_pods, z.pre_pairs, z.pre_victims);
+        }))
+        return rc;
     ctx->chain = DRA_K_PREEMPT_SHARD; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
-    CU(cudaSetDevice(ctx->device));
-    // peers on this device may already wait for this rank: no buffer this call outgrows is freed before the next sync
-    struct DeferFree { dra_ctx* c; ~DeferFree() { c->defer_free = false; } } defer{ctx};
-    ctx->defer_free = gather;
-    int rc = upload_table(ctx);
+    CallScope scope{ctx};
+    int rc = scope.open(gather);
     if (rc) return rc;
     if ((rc = ensure_batch(ctx, std::max(R.n_pod, 1u), 1, false))) return rc;
     if ((rc = spre_buffers(ctx, n_pod, n_pair, max_victims, R.n_pod))) return rc;
@@ -2872,13 +2909,11 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     if (gather) {
         m.slice4 = (uint32_t)(ctx->pre_x.slice / 16);
         const uint32_t n4 = (uint32_t)(1 + (size_t)n_pod * s.stride + (want_pairs ? ((size_t)n_pair + 1) / 2 : 0));
-        k_peer_push<<<std::max(1u, std::min((n4 + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, st>>>(x, s.part, 0u, n4);
+        k_peer_push<<<push_grid(ctx, n4), 256, 0, st>>>(x, s.part, 0u, n4);
         ctx->launches += 1;
     }
-    // a small grid: it waits for its peers, and ranks sharing one device must not find their evaluation's SMs held by it
     const size_t work = std::max(((size_t)n_pod + 7) / 8, want_pairs ? ((size_t)n_pair + 255) / 256 : 0);
-    const uint32_t merge_grid = (uint32_t)std::max<size_t>(1, std::min<size_t>(work, (size_t)std::max(1, ctx->n_sm / 4)));
-    k_spre_merge<<<merge_grid, 256, 0, st>>>(x, m);
+    k_spre_merge<<<wait_grid(ctx, work), 256, 0, st>>>(x, m);
     ctx->launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded preemption launch: %s", cudaGetErrorString(e));
@@ -2887,11 +2922,11 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
 
 int dra_set_shard_capacity(dra_ctx* ctx, uint32_t max_pairs) {
     if (!ctx) return DRA_E_INVAL;
-    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "dra_set_shard_capacity: call it before dra_shard_export");
+    if (int rc = check_before_export(ctx, "dra_set_shard_capacity")) return rc;
     if (max_pairs > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "dra_set_shard_capacity: max_pairs %u above 2^32 - 16", max_pairs);
     if (scap_units(max_pairs) > ((size_t)1 << 32) / 16)
         return fail(ctx, DRA_E_INVAL, "dra_set_shard_capacity: one rank's slice would exceed 4 GiB");
-    ctx->scap_max_pairs = max_pairs;
+    ctx->shard_req.scap_pairs = max_pairs;
     return DRA_OK;
 }
 
@@ -2909,32 +2944,26 @@ int dra_pod_capacity_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cl
     if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     if (max_copies < 1 || max_copies > 65535) return fail(ctx, DRA_E_INVAL, "max_copies %u outside [1, 65535]", max_copies);
-    const bool dense = d_cand_nodes == nullptr && d_cand_off == nullptr;
-    if (!dense && (!d_cand_nodes || !d_cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
-    if (dense && (uint64_t)n_pod * ctx->n_node != n_pair)
-        return fail(ctx, DRA_E_INVAL, "dense form: n_pair %u != n_pod %u x n_node %u", n_pair, n_pod, ctx->n_node);
-    if (n_pair > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
+    bool dense;
+    if (int rc = check_dev_cands(ctx, d_cand_nodes, d_cand_off, n_pod, n_pair, true, dense)) return rc;
     if (n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "n_pod %u too large for the sharded call (2^26)", n_pod);
     const bool gather = ctx->world > 1;
-    if (gather) {
-        if (!ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the merge needs every rank's range)");
-        if (int rc = need_peers(ctx)) return rc;
-        if (ctx->shard_bounds[ctx->world] != ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard map does not span the inventory's %u nodes", ctx->n_node);
-        // no exchange reserved: even a call with no pairs pushes a header and raises flags, which would land in the
-        // peers' buffers at offset 0
-        if (!ctx->peer_scap_pairs)
+    const uint32_t max_pairs = ctx->shard_rsv.scap_pairs;
+    // no exchange reserved: even a call with no pairs pushes a header and raises flags, which would land in the peers'
+    // buffers at offset 0
+    if (int rc = check_world(ctx, "the merge needs", true, [&] {
+            if (max_pairs) return (int)DRA_OK;
             return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_capacity(max_pairs > 0) was not called before dra_shard_export");
-        if (n_pair > ctx->peer_scap_pairs)
-            return fail(ctx, DRA_E_INVAL, "n_pair %u exceeds the max_pairs (%u) of dra_set_shard_capacity before dra_shard_export", n_pair, ctx->peer_scap_pairs);
-    }
+        }, -1, [&] {
+            if (n_pair <= max_pairs) return (int)DRA_OK;
+            return fail(ctx, DRA_E_INVAL, "n_pair %u exceeds the max_pairs (%u) of dra_set_shard_capacity before dra_shard_export", n_pair, max_pairs);
+        }))
+        return rc;
     if (n_pair && !d_pair_copies) return fail(ctx, DRA_E_INVAL, "pair_copies is NULL");
     ctx->chain = DRA_K_POD_CAPACITY_SHARD; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
-    CU(cudaSetDevice(ctx->device));
-    // peers on this device may already wait for this rank: no buffer this call outgrows is freed before the next sync
-    struct DeferFree { dra_ctx* c; ~DeferFree() { c->defer_free = false; } } defer{ctx};
-    ctx->defer_free = gather;
-    int rc = upload_table(ctx);
+    CallScope scope{ctx};
+    int rc = scope.open(gather);
     if (rc) return rc;
     // world > 1: peer_setup sized both for max_pairs, so these never reallocate there
     if ((rc = grow(ctx, ctx->d_scap_part, ctx->cap_scap_part, scap_units(n_pair)))) return rc;
@@ -2972,12 +3001,10 @@ int dra_pod_capacity_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cl
         m.slice4 = (uint32_t)(ctx->scap_x.slice / 16);
         CU(cudaMemcpyAsync(part, gate, 4, cudaMemcpyDeviceToDevice, st));   // the header: this rank's fault word
         const uint32_t n4 = (uint32_t)(1 + copies4 + stops4);
-        k_peer_push<<<std::max(1u, std::min((n4 + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, st>>>(x, part, 0u, n4);
+        k_peer_push<<<push_grid(ctx, n4), 256, 0, st>>>(x, part, 0u, n4);
         ctx->launches += 1;
     }
-    // a small grid: it waits for its peers, and ranks sharing one device must not find their evaluation's SMs held by it
-    const uint32_t merge_grid = std::max(1u, std::min((n_pod + 7) / 8, (uint32_t)std::max(1, ctx->n_sm / 4)));
-    k_scap_merge<<<merge_grid, 256, 0, st>>>(x, m);
+    k_scap_merge<<<wait_grid(ctx, (n_pod + 7) / 8), 256, 0, st>>>(x, m);
     ctx->launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded pod capacity launch: %s", cudaGetErrorString(e));
@@ -2986,10 +3013,11 @@ int dra_pod_capacity_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cl
 
 int dra_set_shard_preempt_place(dra_ctx* ctx, uint32_t max_pods, uint32_t max_pairs, uint32_t max_run) {
     if (!ctx) return DRA_E_INVAL;
-    if (ctx->world > 1 && ctx->peer_local) return fail(ctx, DRA_E_STATE, "dra_set_shard_preempt_place: call it before dra_shard_export");
+    if (int rc = check_before_export(ctx, "dra_set_shard_preempt_place")) return rc;
     if (max_pods > (1u << 26) || max_pairs > 0xFFFFFFF0u || max_run > (1u << 26))
         return fail(ctx, DRA_E_INVAL, "dra_set_shard_preempt_place: sizes too large (max_pods, max_run <= 2^26, max_pairs <= 2^32 - 16)");
-    ctx->spp_max_pods = max_pods; ctx->spp_max_pairs = max_pairs; ctx->spp_max_run = max_run;
+    ShardSizes& z = ctx->shard_req;
+    z.spp_pods = max_pods; z.spp_pairs = max_pairs; z.spp_run = max_run;
     return DRA_OK;
 }
 
@@ -3015,34 +3043,28 @@ int dra_preempt_place_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     if (n_pod > (1u << 26) || R.n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
     if (int rc = check_slots(ctx, n_claim, n_out, d_out_off != nullptr)) return rc;
     if (!n_pod && n_claim) return fail(ctx, DRA_E_INVAL, "pod_off must span [0, n_claim]: no pods for %u claims", n_claim);
-    const bool dense = d_cand_nodes == nullptr && d_cand_off == nullptr;
-    if (!dense && (!d_cand_nodes || !d_cand_off)) return fail(ctx, DRA_E_INVAL, "cand_nodes and cand_off: both or neither");
-    if (dense && n_pair) return fail(ctx, DRA_E_INVAL, "dense form: n_pair must be 0");
+    bool dense;
+    if (int rc = check_dev_cands(ctx, d_cand_nodes, d_cand_off, n_pod, n_pair, false, dense)) return rc;
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
     const uint64_t walk64 = dense ? (uint64_t)n_pod * ctx->n_node : n_pair;     // the pairs the walk judges
     if (walk64 > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "too many (pod, node) pairs");
     const uint32_t walk = (uint32_t)walk64;
     const bool gather = ctx->world > 1;
-    if (gather) {
-        if (!ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the exchange needs every rank's range)");
-        if (int rc = need_peers(ctx)) return rc;
-        if (ctx->shard_bounds[ctx->world] != ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard map does not span the inventory's %u nodes", ctx->n_node);
-        if (!ctx->peer_inv_gpus) return fail(ctx, DRA_E_STATE, "the inventory was not loaded before dra_shard_export: the export reserved no staging for it");
-        if (ctx->n_gpu > ctx->peer_inv_gpus)
-            return fail(ctx, DRA_E_STATE, "the inventory grew to %u GPUs after dra_shard_export reserved staging for %u", ctx->n_gpu, ctx->peer_inv_gpus);
-        if (!ctx->peer_spp_pods) return fail(ctx, DRA_E_STATE, "dra_set_shard_preempt_place was not called before dra_shard_export");
-        if (n_pod > ctx->peer_spp_pods || walk > ctx->peer_spp_pairs || R.n_pod > ctx->peer_spp_run)
+    const ShardSizes& z = ctx->shard_rsv;
+    if (int rc = check_world(ctx, "the exchange needs", true, [&] {
+            if (int rc = check_inv_exchange(ctx)) return rc;
+            if (z.spp_pods) return (int)DRA_OK;
+            return fail(ctx, DRA_E_STATE, "dra_set_shard_preempt_place was not called before dra_shard_export");
+        }, n_out, [&] {
+            if (n_pod <= z.spp_pods && walk <= z.spp_pairs && R.n_pod <= z.spp_run) return (int)DRA_OK;
             return fail(ctx, DRA_E_INVAL, "n_pod %u / pairs %u / running pods %u exceed the sizes of dra_set_shard_preempt_place before "
-                        "dra_shard_export (%u / %u / %u)", n_pod, walk, R.n_pod, ctx->peer_spp_pods, ctx->peer_spp_pairs, ctx->peer_spp_run);
-        if (n_out > ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", n_out, ctx->peer_tab_len);
-    }
+                        "dra_shard_export (%u / %u / %u)", n_pod, walk, R.n_pod, z.spp_pods, z.spp_pairs, z.spp_run);
+        }))
+        return rc;
     ctx->chain = DRA_K_PREEMPT_PLACE_SHARD; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
-    CU(cudaSetDevice(ctx->device));
-    // peers on this device may already wait for this rank: no buffer this call outgrows is freed before the next sync
-    struct DeferFree { dra_ctx* c; ~DeferFree() { c->defer_free = false; } } defer{ctx};
-    ctx->defer_free = gather;
-    int rc = upload_table(ctx);
+    CallScope scope{ctx};
+    int rc = scope.open(gather);
     if (rc) return rc;
     if ((rc = spp_buffers(ctx, n_pod, walk, R.n_pod))) return rc;
     if (ctx->pp_occ < 0 && (rc = preload_preempt_place_shard(ctx))) return rc;
@@ -3064,9 +3086,8 @@ int dra_preempt_place_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
         InvSync s; memset(&s, 0, sizeof s);
         s.inv = ctx->d_spp_inv; s.n_gpu = ctx->n_gpu; s.own_lo = gpu_lo; s.own_hi = gpu_hi;
         s.elect = (uint32_t*)(ctx->peer_local + ctx->isync_x.flags) + PEER_MAX;
-        k_peer_push<<<std::max(1u, std::min((gpu_hi - gpu_lo + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, st>>>(x, ctx->d_inv_live, gpu_lo, gpu_hi);
-        // a small grid: it waits for its peers, and ranks sharing one device must not find their walk's SMs held by it
-        k_isync_copy<<<std::max(1u, std::min((ctx->n_gpu + 255) / 256, (uint32_t)std::max(1, ctx->n_sm / 4))), 256, 0, st>>>(x, s);
+        k_peer_push<<<push_grid(ctx, gpu_hi - gpu_lo), 256, 0, st>>>(x, ctx->d_inv_live, gpu_lo, gpu_hi);
+        k_isync_copy<<<wait_grid(ctx, (ctx->n_gpu + 255) / 256), 256, 0, st>>>(x, s);
         // one verdict for the world: the call fails on every rank or on none
         k_spp_agree<<<1, 32, 0, st>>>(bind_exchange(ctx, ctx->spp_x), s.elect, x.seq, ctx->d_spp_gate);
         ctx->launches += 3;
@@ -3123,21 +3144,15 @@ int dra_shard_sync_inventory_device(dra_ctx* ctx) {
     if (!ctx) return DRA_E_INVAL;
     QUIESCE();
     if (ctx->world <= 1) return DRA_OK;
-    if (!ctx->shard_map_on) return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_map has not been called (the sync needs every rank's range)");
-    if (int rc = need_peers(ctx)) return rc;
-    if (!ctx->peer_inv_gpus) return fail(ctx, DRA_E_STATE, "the inventory was not loaded before dra_shard_export: the export reserved no staging for it");
-    if (ctx->n_gpu > ctx->peer_inv_gpus)
-        return fail(ctx, DRA_E_STATE, "the inventory grew to %u GPUs after dra_shard_export reserved staging for %u", ctx->n_gpu, ctx->peer_inv_gpus);
-    if (ctx->shard_bounds[ctx->world] != ctx->n_node) return fail(ctx, DRA_E_STATE, "the shard map does not span the inventory's %u nodes", ctx->n_node);
+    if (int rc = check_world(ctx, "the sync needs", true, [ctx] { return check_inv_exchange(ctx); }, -1, no_check)) return rc;
     CU(cudaSetDevice(ctx->device));
     const PeerExchange x = bind_exchange(ctx, ctx->isync_x);
     InvSync s; memset(&s, 0, sizeof s);
     s.inv = ctx->d_inv_live; s.n_gpu = ctx->n_gpu;
     s.elect = (uint32_t*)(ctx->peer_local + ctx->isync_x.flags) + PEER_MAX;
     s.own_lo = ctx->h_node_off[ctx->shard_bounds[ctx->rank]]; s.own_hi = ctx->h_node_off[ctx->shard_bounds[ctx->rank + 1]];
-    k_peer_push<<<std::max(1u, std::min((s.own_hi - s.own_lo + 255) / 256, (uint32_t)ctx->n_sm * 2u)), 256, 0, ctx->stream>>>(x, s.inv, s.own_lo, s.own_hi);
-    // a small grid: it waits for its peers, and ranks sharing one device must not find their push's SMs held by it
-    k_isync_copy<<<std::max(1u, std::min((ctx->n_gpu + 255) / 256, (uint32_t)std::max(1, ctx->n_sm / 4))), 256, 0, ctx->stream>>>(x, s);
+    k_peer_push<<<push_grid(ctx, s.own_hi - s.own_lo), 256, 0, ctx->stream>>>(x, s.inv, s.own_lo, s.own_hi);
+    k_isync_copy<<<wait_grid(ctx, (ctx->n_gpu + 255) / 256), 256, 0, ctx->stream>>>(x, s);
     ctx->launches += 2;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "inventory sync launch: %s", cudaGetErrorString(e));

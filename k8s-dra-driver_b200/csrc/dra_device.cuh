@@ -4201,27 +4201,42 @@ struct PreMerge {
     uint32_t* pod_node; uint8_t* pod_status; uint32_t* n_victims; uint32_t* victims;
 };
 
+// The start of a merge that waits for its peers (k_spre_merge, k_scap_merge): block 0 raises this rank's flags, every
+// block waits, then every rank's fault word is read (this rank's at gate, a peer's in the first word of its slice, slice4
+// uint4 units apart in x's staging).  A peer's fault fails the call here too.  False in every thread after a fault or a
+// timeout: the merge writes nothing then.  world (at least 1), rank and tid as the kernel has them.
+__device__ __forceinline__ bool merge_start(const PeerExchange& x, const uint32_t* gate, uint32_t slice4, uint32_t world,
+                                            uint32_t rank, uint32_t tid) {
+    __shared__ uint32_t s_ok;
+    if (tid == 0) s_ok = 1u;
+    __syncthreads();
+    if (blockIdx.x == 0) peer_raise(x, tid);
+    if (!peer_wait(x, tid, clock64())) s_ok = 0u;
+    if (tid < world) {
+        const uint32_t f = tid == rank ? __ldcg(gate) : __ldcg(&x.my_stage[(size_t)tid * slice4]).x;
+        if (f) {
+            s_ok = 0u;
+            if (blockIdx.x == 0 && tid != rank) x.err.set(ERR_BAD_OFFSETS);
+        }
+    }
+    __syncthreads();
+    return s_ok != 0u;
+}
+
+// The rank whose node range [bounds[r], bounds[r + 1]) of the shard map holds node, in a world of world ranks
+__device__ __forceinline__ uint32_t node_owner(const uint32_t* bounds, uint32_t world, uint32_t node) {
+    uint32_t r = 0;
+    while (r + 1 < world && bounds[r + 1] <= node) ++r;
+    return r;
+}
+
 // At most SMs / 4 CTAs, launched after the evaluation: ranks sharing one device must not find their evaluation's SMs
 // held by a peer's waiting CTAs.  Block 0 raises this rank's flags, every block waits; then a warp per pod (lane s reads
 // rank s's partial) and a thread per pair.  With world 1 (an all-zero PeerExchange) nothing is waited for.
 __global__ void __launch_bounds__(256)
 k_spre_merge(const PeerExchange x, const PreMerge m) {
-    __shared__ uint32_t s_ok;
-    const uint32_t tid = threadIdx.x;
-    if (tid == 0) s_ok = 1u;
-    __syncthreads();
-    if (blockIdx.x == 0) peer_raise(x, tid);
-    if (!peer_wait(x, tid, clock64())) s_ok = 0u;
-    const uint32_t world = x.world ? x.world : 1u, rank = x.rank;
-    if (tid < world) {
-        const uint32_t f = tid == rank ? __ldcg(m.gate) : __ldcg(&x.my_stage[(size_t)tid * m.slice4]).x;
-        if (f) {
-            s_ok = 0u;
-            if (blockIdx.x == 0 && tid != rank) x.err.set(ERR_BAD_OFFSETS);   // a peer's fault fails the call here too
-        }
-    }
-    __syncthreads();
-    if (!s_ok) return;
+    const uint32_t tid = threadIdx.x, world = x.world ? x.world : 1u, rank = x.rank;
+    if (!merge_start(x, m.gate, m.slice4, world, rank, tid)) return;
     const uint32_t lane = tid & 31;
     const uint32_t warp = (blockIdx.x * blockDim.x + tid) >> 5, n_warp = (gridDim.x * blockDim.x) >> 5;
     const bool dense = m.cand_off == nullptr;
@@ -4263,8 +4278,7 @@ k_spre_merge(const PeerExchange x, const PreMerge m) {
         const uint32_t node = dense ? k % m.n_node : __ldg(&m.cand_nodes[k]);
         uint2 v = make_uint2(DRA_PRE_NO, 0u);                             // a candidate naming no node
         if (node < m.n_node) {
-            uint32_t r = 0;
-            while (r + 1 < world && m.bounds[r + 1] <= node) ++r;
+            const uint32_t r = node_owner(m.bounds, world, node);
             const uint2* src = r == rank ? m.pairs : reinterpret_cast<const uint2*>(x.my_stage + (size_t)r * m.slice4 + pair4);
             v = __ldcg(&src[k]);
         }
@@ -4413,22 +4427,8 @@ struct CapMerge {
 // world 1 (an all-zero PeerExchange) nothing is waited for.
 __global__ void __launch_bounds__(256)
 k_scap_merge(const PeerExchange x, const CapMerge m) {
-    __shared__ uint32_t s_ok;
-    const uint32_t tid = threadIdx.x;
-    if (tid == 0) s_ok = 1u;
-    __syncthreads();
-    if (blockIdx.x == 0) peer_raise(x, tid);
-    if (!peer_wait(x, tid, clock64())) s_ok = 0u;
-    const uint32_t world = x.world ? x.world : 1u, rank = x.rank;
-    if (tid < world) {
-        const uint32_t f = tid == rank ? __ldcg(m.gate) : __ldcg(&x.my_stage[(size_t)tid * m.slice4]).x;
-        if (f) {
-            s_ok = 0u;
-            if (blockIdx.x == 0 && tid != rank) x.err.set(ERR_BAD_OFFSETS);   // a peer's fault fails the call here too
-        }
-    }
-    __syncthreads();
-    if (!s_ok) return;
+    const uint32_t tid = threadIdx.x, world = x.world ? x.world : 1u, rank = x.rank;
+    if (!merge_start(x, m.gate, m.slice4, world, rank, tid)) return;
     const uint32_t lane = tid & 31;
     const uint32_t warp = (blockIdx.x * blockDim.x + tid) >> 5, n_warp = (gridDim.x * blockDim.x) >> 5;
     const bool dense = m.cand_off == nullptr;
@@ -4439,8 +4439,7 @@ k_scap_merge(const PeerExchange x, const CapMerge m) {
             const uint32_t node = dense ? (uint32_t)(k - k0) : __ldg(&m.cand_nodes[k]);
             uint32_t copies = 0, stop = DRA_ST_POD;                        // a candidate naming no node
             if (node < m.n_node) {
-                uint32_t r = 0;
-                while (r + 1 < world && m.bounds[r + 1] <= node) ++r;
+                const uint32_t r = node_owner(m.bounds, world, node);
                 const uint32_t lo = m.bounds[r], n_win = m.bounds[r + 1] - lo;
                 const uint32_t w = dense ? p * n_win + (node - lo) : (uint32_t)k;
                 const uint32_t nw = dense ? m.n_pod * n_win : m.n_pair;
