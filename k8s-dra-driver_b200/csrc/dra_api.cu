@@ -205,6 +205,9 @@ struct dra_ctx {
     volatile uint32_t* h_sc_counts = nullptr;   // mapped host copy of the last call's counts
     uint32_t* h_sc_counts_dev = nullptr;
     uint2* d_gtable = nullptr; size_t cap_gtable = 0;   // result table when no peers are set up (world 1)
+    // 16 words, zeroed when allocated: [4] the shard compaction's tile ticket, [8] k_bucket_scan8's, [10, 11]
+    // k_bucket_scan_rows' ticket and epoch; and the 64-bit counters of the counter walks (walk_counter), each zeroed
+    // before its launch: [6, 7] preemption, [12, 13] UnsuitableNodes, [14, 15] pod capacity
     uint32_t* d_ticket = nullptr;
     ShardSizes shard_req{};                     // the sizes the setters asked for, reserved by the next peer_setup
     ShardSizes shard_rsv{};                     // the sizes the last peer_setup reserved
@@ -686,6 +689,10 @@ void launch_unsuitable_w(dra_ctx* ctx, const UnsArgs& a, uint32_t W, uint32_t gr
     }
 }
 
+// The 64-bit walk counter at d_ticket word `word` (even: 8-aligned).  64 bits because a walk may cover up to 2^32 - 1
+// pairs and every warp takes one more value past its end: a 32-bit counter would wrap and walk the pairs again.
+unsigned long long* walk_counter(dra_ctx* ctx, int word) { return reinterpret_cast<unsigned long long*>(ctx->d_ticket + word); }
+
 // k_unsuitable over n_walk pairs (win: the sharded call's node window, n_walk = a.n_walk; else n_walk = a.n_pair); lanes per
 // pair from the widest node: 8 lanes = 4 pairs per warp.  Enqueues only.
 int launch_unsuitable(dra_ctx* ctx, UnsArgs& a, bool win) {
@@ -694,8 +701,8 @@ int launch_unsuitable(dra_ctx* ctx, UnsArgs& a, bool win) {
     const uint32_t n_walk = win ? a.n_walk : a.n_pair;
     const uint32_t grid = std::max(1u, std::min((n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
     if (a.exhaustive) {
-        a.work = ctx->d_ticket + 12;
-        CU(cudaMemsetAsync(a.work, 0, 4, ctx->stream));
+        a.work = walk_counter(ctx, 12);
+        CU(cudaMemsetAsync(a.work, 0, 8, ctx->stream));
     }
     if (win) launch_unsuitable_w<true>(ctx, a, W, grid);
     else launch_unsuitable_w<false>(ctx, a, W, grid);
@@ -1003,8 +1010,8 @@ int launch_preempt_pairs(dra_ctx* ctx, PreArgs a, const PreShard& s) {
     if (!s.n_walk) return DRA_OK;
     cudaStream_t st = ctx->stream;
     if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, st)); }
-    a.work = ctx->d_ticket + 13;
-    CU(cudaMemsetAsync(a.work, 0, 4, st));
+    a.work = walk_counter(ctx, 6);
+    CU(cudaMemsetAsync(a.work, 0, 8, st));
     const uint32_t W = pair_width(ctx), per_cta = 8 * (32 / W);
     const uint32_t grid = std::max(1u, std::min((s.n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
     if (W == 8) k_pods_preempt<8, 8><<<grid, 256, 0, st>>>(a, s);
@@ -1031,8 +1038,8 @@ int launch_capacity(dra_ctx* ctx, CapArgs a) {
     cudaStream_t st = ctx->stream;
     if (a.n_walk) {
         if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, st)); }
-        a.work = ctx->d_ticket + 14;
-        CU(cudaMemsetAsync(a.work, 0, 4, st));
+        a.work = walk_counter(ctx, 14);
+        CU(cudaMemsetAsync(a.work, 0, 8, st));
         const uint32_t W = pair_width(ctx), per_cta = 8 * (32 / W);
         const uint32_t grid = std::max(1u, std::min((a.n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
         if (W == 8) k_pods_capacity<8, 8><<<grid, 256, 0, st>>>(a);

@@ -2940,8 +2940,8 @@ struct UnsArgs {
     SelCtx sel;
     uint32_t dense;     // 1: every pod x every node, pair = pod * n_node + node (cand arrays unused)
     uint32_t exhaustive; // spec §12: pod evaluation with the backtracking search
-    uint32_t* work;      // EXH: next unclaimed pair (zeroed by the caller) — searches differ by orders of magnitude in length,
-                         //      so the warps take their pairs from a counter instead of a fixed stride
+    unsigned long long* work;   // EXH: next unclaimed pair (zeroed by the caller) — searches differ by orders of magnitude
+                                //      in length, so the warps take their pairs from a counter instead of a fixed stride
     // sharded call only (k_unsuitable<..., WIN = true>):
     uint32_t node_lo, n_win;   // node window: only pairs whose node lies in [node_lo, node_lo + n_win) are evaluated
     uint32_t n_walk;           // pairs the kernel walks: dense n_pod * n_win (mapped back to pod * n_node + node), else n_pair
@@ -2952,6 +2952,17 @@ struct GlobalGet {
     const uint4* base;
     __device__ __forceinline__ uint4 operator()(uint32_t m) const { return __ldg(&base[m]); }
 };
+
+// A counter walk's next G walk indices, for the whole warp: lane 0 takes them from the 64-bit counter (zeroed by the host)
+// and every lane gets the first.  Every warp takes one value at or past the end, so the counter itself passes 2^32 on a
+// walk near 2^32 pairs; the value is handed on clamped to 0xFFFFFFFF, which is at or past every walk's end.  A walk
+// index below the end is a multiple of G below 2^32, so pw + grp never wraps.
+template <uint32_t G>
+__device__ __forceinline__ uint32_t walk_fetch(unsigned long long* work, uint32_t lane) {
+    uint32_t nxt = 0;
+    if (lane == 0) nxt = (uint32_t)min(atomicAdd(work, (unsigned long long)G), 0xFFFFFFFFull);
+    return __shfl_sync(FULLMASK, nxt, 0);
+}
 
 // W lanes per (pod, candidate) pair: 32/W pairs share a warp (W = 8 for the usual <= 8 GPUs per node), each
 // group running its own claim loop with group-wide ballots.  dense = every pod against every node
@@ -2970,13 +2981,10 @@ k_unsuitable(const UnsArgs a) {
     const uint32_t grp = lane / W, gl = lane % W, gbase = grp * W;
     const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
     const uint32_t stride = gridDim.x * WPC * G;
-    for (uint32_t pw = (blockIdx.x * WPC + wid) * G; ; pw += stride) {
-        if (EXH) {
-            uint32_t nxt = 0;
-            if (lane == 0) nxt = atomicAdd(a.work, G);
-            pw = __shfl_sync(FULLMASK, nxt, 0);
-        }
-        const uint32_t n_walk = WIN ? a.n_walk : a.n_pair;
+    const uint32_t n_walk = WIN ? a.n_walk : a.n_pair;
+    // the stride steps at most to n_walk: a plain pw += stride wraps past 2^32 near the top of the range and walks again
+    for (uint32_t pw = (blockIdx.x * WPC + wid) * G; ; pw += min(stride, n_walk - pw)) {
+        if (EXH) pw = walk_fetch<G>(a.work, lane);
         if (pw >= n_walk) break;
         const uint32_t walk = pw + grp;
         if (walk >= n_walk) continue;                                    // whole group skips together
@@ -3029,7 +3037,7 @@ k_uns_prep(const uint32_t* __restrict__ pod_off, const uint32_t* __restrict__ ca
     if (cand_off) {
         const uint32_t k0 = __ldg(&cand_off[p]), k1 = __ldg(&cand_off[p + 1]);
         bad = bad || k1 < k0 || k1 > n_pair;
-        if (!bad) for (uint32_t k = k0 + lane; k < k1; k += 32) pair_pod[k] = p;
+        if (!bad) for (unsigned long long k = (unsigned long long)k0 + lane; k < k1; k += 32) pair_pod[k] = p;   // 64 bits: k1 may lie within 32 of 2^32
     }
     if (bad && lane == 0) err.set(ERR_BAD_OFFSETS);
 }
@@ -3538,7 +3546,7 @@ struct PreArgs {
     uint8_t* pair_status; uint32_t* pair_victims;                   // caller's per-pair outputs (may be nullptr)
     uint32_t* pod_node; uint8_t* pod_status; uint32_t* n_victims; uint32_t* choice;
     uint32_t max_victims;
-    uint32_t* work;               // next unclaimed pair (zeroed by the host)
+    unsigned long long* work;     // next unclaimed pair (zeroed by the host)
     const uint32_t* gate;         // non-zero: the running pods failed their check, nothing is evaluated
     Err err;
 };
@@ -3727,9 +3735,7 @@ k_pods_preempt(const PreArgs a, const PreShard s) {
     const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
     const uint32_t n_win = s.node_hi - s.node_lo;
     while (true) {
-        uint32_t nxt = 0;
-        if (lane == 0) nxt = atomicAdd(a.work, G);
-        const uint32_t pw = __shfl_sync(FULLMASK, nxt, 0);
+        const uint32_t pw = walk_fetch<G>(a.work, lane);
         if (pw >= s.n_walk) break;
         const uint32_t walk = pw + grp;
         if (walk >= s.n_walk) continue;                                  // whole group skips together
@@ -4305,7 +4311,7 @@ struct CapArgs {
     uint32_t node_lo, n_win, n_walk;
     uint16_t* pair_copies; uint8_t* pair_stop;            // at the walk index; pair_stop: nullptr unless asked for
     unsigned long long* pod_total; uint32_t* pod_nodes;   // each nullptr unless asked for
-    uint32_t* work;                                       // next unclaimed pair (zeroed by the host)
+    unsigned long long* work;                             // next unclaimed pair (zeroed by the host)
     const uint32_t* gate;                                 // non-zero: the offsets failed their check (nullptr: none)
 };
 
@@ -4327,9 +4333,7 @@ k_pods_capacity(const CapArgs a) {
     const uint32_t grp = lane / W, gbase = grp * W, gl = lane - gbase;
     const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
     while (true) {
-        uint32_t nxt = 0;
-        if (lane == 0) nxt = atomicAdd(a.work, G);
-        const uint32_t pw = __shfl_sync(FULLMASK, nxt, 0);
+        const uint32_t pw = walk_fetch<G>(a.work, lane);
         if (pw >= a.n_walk) break;
         const uint32_t pair = pw + grp;                                  // the walk index
         if (pair >= a.n_walk) continue;                                  // whole group skips together
