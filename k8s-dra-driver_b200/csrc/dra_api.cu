@@ -358,7 +358,8 @@ int ensure_batch(dra_ctx* ctx, uint32_t n_claim, uint32_t n_out, bool own_io) {
     const uint32_t n_cta = (ctx->n_node + 1 + 31) / 32;
     if (ctx->cap_scan_status < n_cta) {
         CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_scan_status) CU(cudaFree(ctx->d_scan_status));
+        if (ctx->d_scan_status && ctx->defer_free) ctx->retired.push_back(ctx->d_scan_status);
+        else if (ctx->d_scan_status) CU(cudaFree(ctx->d_scan_status));
         ctx->d_scan_status = nullptr; ctx->cap_scan_status = 0;
         const uint32_t ncap = n_cta + n_cta / 2 + 64;
         CU(cudaMalloc((void**)&ctx->d_scan_status, (size_t)ncap * 8));
@@ -2463,7 +2464,10 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
     if (int rc = need_peers(ctx)) return rc;
     if (gather && n_out > ctx->peer_tab_len) return fail(ctx, DRA_E_INVAL, "n_out %u exceeds the exported table (%u)", n_out, ctx->peer_tab_len);
     ctx->chain = ctx->chain_tile = 0;
-    CU(cudaSetDevice(ctx->device));
+    // world > 1: a peer on this device may already be waiting for this rank's packets, so a buffer this call outgrows
+    // is freed at the next dra_ctx_sync (a cudaFree now would wait for that peer, which waits for this call)
+    CallScope scope{ctx};
+    if (int rc = scope.open(gather)) return rc;
     const uint32_t n_local_node = ctx->shard_hi - ctx->shard_lo;
     // Plan.  The single-launch kernel lays its shared memory out for a CAPACITY of claims; the real number is only known
     // on the device (the compaction's count).  First call of a shape: capacity = the whole batch (always safe).  Later

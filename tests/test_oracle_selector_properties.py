@@ -43,45 +43,51 @@ def sel_eval(prog, a):
     return stack[-1] if seen else True
 
 
-@st.composite
-def selector_problems(draw):
+def selector_programs(D, n_gpu):
+    """Random attributes for n_gpu GPUs, a table of 1-3 random selector programs and a selector id (the table's size + 1:
+    beyond it).  D draws integers and picks (preempt_problems._Hyp from hypothesis, _Rng from a seeded generator)."""
     import importlib
     R = importlib.import_module("k8s-dra-driver_b200").records
-    g, off, t, c, out_off, n_out = draw(problems())
-    a = np.zeros(len(g), dtype=R.ATTR_DTYPE)
-    for i in range(len(g)):
-        a[i] = (draw(st.sampled_from([16384, 40960, 81920])), draw(st.sampled_from([0x0705, 0x0800, 0x0900])),
-                draw(st.integers(0, 9)), draw(st.integers(0, 5)), draw(st.sampled_from([535, 550, 570])))
-    n_sel = draw(st.integers(1, 3))
+    a = np.zeros(n_gpu, dtype=R.ATTR_DTYPE)
+    for i in range(n_gpu):
+        a[i] = (D.pick([16384, 40960, 81920]), D.pick([0x0705, 0x0800, 0x0900]), D.int(0, 9), D.int(0, 5),
+                D.pick([535, 550, 570]))
+    n_sel = D.int(1, 3)
     sels = np.zeros((n_sel, R.SEL_MAX_INS), dtype=R.SEL_INS_DTYPE)
     domain = {0: [16384, 40960, 81920], 1: [0x0705, 0x0800, 0x0900], 2: list(range(10)), 3: list(range(6)), 4: [535, 550, 570]}
 
     def leaf():
-        attr = draw(st.integers(0, 4))
-        if attr in (2, 3) and draw(st.booleans()):
-            return [(1, attr, 6, 0, draw(st.integers(0, 1023)))]             # IN_MASK over small ids
-        return [(1, attr, draw(st.integers(0, 5)), 0, draw(st.sampled_from(domain[attr])))]
+        attr = D.int(0, 4)
+        if attr in (2, 3) and D.int(0, 1):
+            return [(1, attr, 6, 0, D.int(0, 1023))]                         # IN_MASK over small ids
+        return [(1, attr, D.int(0, 5), 0, D.pick(domain[attr]))]
 
     def tree(depth):
-        if depth == 0 or draw(st.integers(0, 2)) == 0:
+        if depth == 0 or D.int(0, 2) == 0:
             return leaf()
-        k = draw(st.sampled_from([2, 3, 4]))
+        k = D.pick([2, 3, 4])
         if k == 4:
             return tree(depth - 1) + [(4, 0, 0, 0, 0)]
         return tree(depth - 1) + tree(depth - 1) + [(k, 0, 0, 0, 0)]
 
     for s in range(n_sel):
-        if draw(st.integers(0, 4)) != 0:                   # mostly well-formed trees that split the GPUs ...
+        if D.int(0, 4) != 0:                               # mostly well-formed trees that split the GPUs ...
             prog = tree(2)[: R.SEL_MAX_INS]
             for k, ins in enumerate(prog):
                 sels[s, k] = ins
         else:                                              # ... and some garbage: unknown codes, underflow, early END
-            for k in range(draw(st.integers(0, R.SEL_MAX_INS))):
-                sels[s, k] = (draw(st.sampled_from([1, 1, 1, 2, 3, 4, 0, 9])), draw(st.sampled_from([0, 1, 2, 3, 4, 7])),
-                              draw(st.sampled_from([0, 1, 2, 3, 4, 5, 6, 8])), 0,
-                              draw(st.sampled_from([0, 1, 3, 0b101010, 535, 0x0800, 40960, 0xFFFFFFFF])))
-    sid = draw(st.integers(1, n_sel + 1))                 # n_sel + 1: beyond the table -> INVALID
-    return g, off, t, c, out_off, n_out, a, sels, sid
+            for k in range(D.int(0, R.SEL_MAX_INS)):
+                sels[s, k] = (D.pick([1, 1, 1, 2, 3, 4, 0, 9]), D.pick([0, 1, 2, 3, 4, 7]), D.pick([0, 1, 2, 3, 4, 5, 6, 8]), 0,
+                              D.pick([0, 1, 3, 0b101010, 535, 0x0800, 40960, 0xFFFFFFFF]))
+    sid = D.int(1, n_sel + 1)                             # n_sel + 1: beyond the table -> INVALID
+    return a, sels, sid
+
+
+@st.composite
+def selector_problems(draw):
+    from preempt_problems import _Hyp
+    g, off, t, c, out_off, n_out = draw(problems())
+    return (g, off, t, c, out_off, n_out) + selector_programs(_Hyp(draw), len(g))
 
 
 @settings(max_examples=300, deadline=None, suppress_health_check=list(HealthCheck), derandomize=True)
