@@ -330,6 +330,107 @@ func (c *Context) PreemptBatch(claims []ClaimRec, podOff []uint32, prio []int32,
 	return r, nil
 }
 
+// PdbNone: a running pod that counts against no disruption budget.
+const PdbNone = 0xFFFFFFFF
+
+// DisruptionBudgets for PreemptPdbBatch (spec §14, "Disruption budgets"): RunPdb[r] the budget running pod r counts
+// against (PdbNone for none, also for a pod in its budget's DisruptedPods), Allowed[b] each budget's
+// status.disruptionsAllowed.  Both empty: no budgets.
+type DisruptionBudgets struct {
+	RunPdb  []uint32
+	Allowed []int32
+}
+
+// Preemption answer with disruption budgets: Preemption, plus per pair the violating victims of an EVICT pair and per
+// pod the chosen pair's.
+type PreemptionPdb struct {
+	Preemption
+	PairViolations []uint32
+	PodViolations  []uint32
+}
+
+// PreemptPdbBatch is PreemptBatch honouring PodDisruptionBudgets (dra_preempt_pdb_batch): on each candidate node the
+// running pods whose eviction would violate their budget are reprieved first, and a pod's node is the one with the fewest
+// violating victims before any other criterion.  Unbuilt, like the rest of this file.
+func (c *Context) PreemptPdbBatch(claims []ClaimRec, podOff []uint32, prio []int32, cands, candOff []uint32, nNode int,
+	run RunningPods, budgets DisruptionBudgets, maxVictims int, flags uint32) (*PreemptionPdb, error) {
+	nPod := len(podOff) - 1
+	if nPod <= 0 || len(run.PodOff) == 0 {
+		return &PreemptionPdb{}, nil
+	}
+	nPair := nPod * nNode
+	var cn, co *C.uint32_t
+	if candOff != nil {
+		nPair = int(candOff[nPod])
+		co = (*C.uint32_t)(unsafe.Pointer(&candOff[0]))
+		if len(cands) == 0 {
+			cands = []uint32{0} // an empty list still needs an address (nil means the dense form)
+		}
+		cn = (*C.uint32_t)(unsafe.Pointer(&cands[0]))
+	}
+	r := &PreemptionPdb{Preemption{make([]uint8, nPair+1), make([]uint32, nPair+1), make([]uint32, nPod),
+		make([]uint8, nPod), make([]uint32, nPod), make([]uint32, nPod*maxVictims+1)},
+		make([]uint32, nPair+1), make([]uint32, nPod)}
+	var cp, rcp *C.dra_claim_rec
+	if len(claims) > 0 {
+		cp = (*C.dra_claim_rec)(unsafe.Pointer(&claims[0]))
+	}
+	if len(run.Claims) > 0 {
+		rcp = (*C.dra_claim_rec)(unsafe.Pointer(&run.Claims[0]))
+	}
+	var rp *C.int32_t
+	if len(run.Prio) > 0 {
+		rp = (*C.int32_t)(unsafe.Pointer(&run.Prio[0]))
+	}
+	var roo *C.uint32_t
+	if run.OutOff != nil {
+		roo = (*C.uint32_t)(unsafe.Pointer(&run.OutOff[0]))
+	}
+	var rop *C.dra_out_rec
+	if len(run.Out) > 0 {
+		rop = (*C.dra_out_rec)(unsafe.Pointer(&run.Out[0]))
+	}
+	var bpdb *C.uint32_t
+	if len(budgets.RunPdb) > 0 {
+		bpdb = (*C.uint32_t)(unsafe.Pointer(&budgets.RunPdb[0]))
+	}
+	var bal *C.int32_t
+	if len(budgets.Allowed) > 0 {
+		bal = (*C.int32_t)(unsafe.Pointer(&budgets.Allowed[0]))
+	}
+	// the structs handed to C hold Go pointers: cgo accepts that only for pinned memory
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, q := range []unsafe.Pointer{unsafe.Pointer(rcp), unsafe.Pointer(&run.PodOff[0]), unsafe.Pointer(rp),
+		unsafe.Pointer(roo), unsafe.Pointer(rop), unsafe.Pointer(bpdb), unsafe.Pointer(bal)} {
+		if q != nil {
+			pin.Pin(q)
+		}
+	}
+	cr := C.dra_running_pods{claims: rcp, n_claim: C.uint32_t(len(run.Claims)),
+		pod_off: (*C.uint32_t)(unsafe.Pointer(&run.PodOff[0])), n_pod: C.uint32_t(len(run.PodOff) - 1), prio: rp,
+		out_off: roo, out: rop, n_out: C.uint32_t(len(run.Out))}
+	cb := C.dra_disruption_budgets{run_pdb: bpdb, allowed: bal, n_pdb: C.uint32_t(len(budgets.Allowed))}
+	var vp *C.uint32_t
+	if maxVictims > 0 {
+		vp = (*C.uint32_t)(unsafe.Pointer(&r.Victims[0]))
+	}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_preempt_pdb_batch(c.h, cp, C.uint32_t(len(claims)), (*C.uint32_t)(unsafe.Pointer(&podOff[0])),
+		(*C.int32_t)(unsafe.Pointer(&prio[0])), C.uint32_t(nPod), cn, co, &cr, &cb,
+		(*C.uint8_t)(unsafe.Pointer(&r.PairStatus[0])), (*C.uint32_t)(unsafe.Pointer(&r.PairVictims[0])),
+		(*C.uint32_t)(unsafe.Pointer(&r.PairViolations[0])), (*C.uint32_t)(unsafe.Pointer(&r.PodNode[0])),
+		(*C.uint8_t)(unsafe.Pointer(&r.PodStatus[0])), (*C.uint32_t)(unsafe.Pointer(&r.NVictims[0])),
+		(*C.uint32_t)(unsafe.Pointer(&r.PodViolations[0])), vp, C.uint32_t(maxVictims), C.uint32_t(flags))
+	if rc != 0 {
+		return nil, lastError(c.h)
+	}
+	r.PairStatus, r.PairVictims, r.Victims = r.PairStatus[:nPair], r.PairVictims[:nPair], r.Victims[:nPod*maxVictims]
+	r.PairViolations = r.PairViolations[:nPair]
+	return r, nil
+}
+
 // Preempt-and-place answer (spec §15).  Per pod: the node chosen (0xFFFFFFFF: none) and its status (DRA_PRE_*).  Per
 // running pod: the pending pod that evicted it, 0xFFFFFFFF when none.
 type PreemptPlacement struct {
@@ -642,6 +743,45 @@ func (c *Context) PreemptBatchGlobalDevice(pinnedClaims unsafe.Pointer, nClaim i
 		(*C.uint32_t)(pinnedCandOff), C.uint32_t(nPair), &r, (*C.uint8_t)(pinnedPairStatus), (*C.uint32_t)(pinnedPairVictims),
 		(*C.uint32_t)(pinnedPodNode), (*C.uint8_t)(pinnedPodStatus), (*C.uint32_t)(pinnedNVictims), (*C.uint32_t)(pinnedVictims),
 		C.uint32_t(maxVictims), C.uint32_t(flags))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
+// PinnedDisruptionBudgets: the budgets of PreemptPdbBatchGlobalDevice in dra_host_alloc'ed (pinned) or device memory.
+type PinnedDisruptionBudgets struct {
+	RunPdb  unsafe.Pointer
+	Allowed unsafe.Pointer
+	NPdb    int
+}
+
+// PreemptPdbBatchGlobalDevice is PreemptBatchGlobalDevice honouring PodDisruptionBudgets
+// (dra_preempt_pdb_batch_global_device), the same budgets on every context; the violation outputs may be nil.  Returns at
+// once; Sync reports completion and errors found on the device.  Unbuilt, like the rest of this file.
+func (c *Context) PreemptPdbBatchGlobalDevice(pinnedClaims unsafe.Pointer, nClaim int, pinnedPodOff, pinnedPrio unsafe.Pointer,
+	nPod int, pinnedCandNodes, pinnedCandOff unsafe.Pointer, nPair int, run PinnedRunningPods, budgets PinnedDisruptionBudgets,
+	pinnedPairStatus, pinnedPairVictims, pinnedPairViolations, pinnedPodNode, pinnedPodStatus, pinnedNVictims,
+	pinnedPodViolations, pinnedVictims unsafe.Pointer, maxVictims int, flags uint32) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var r C.dra_running_pods
+	r.claims = (*C.dra_claim_rec)(run.Claims)
+	r.n_claim = C.uint32_t(run.NClaim)
+	r.pod_off = (*C.uint32_t)(run.PodOff)
+	r.n_pod = C.uint32_t(run.NPod)
+	r.prio = (*C.int32_t)(run.Prio)
+	r.out_off = (*C.uint32_t)(run.OutOff)
+	r.out = (*C.dra_out_rec)(run.Out)
+	r.n_out = C.uint32_t(run.NOut)
+	b := C.dra_disruption_budgets{run_pdb: (*C.uint32_t)(budgets.RunPdb), allowed: (*C.int32_t)(budgets.Allowed),
+		n_pdb: C.uint32_t(budgets.NPdb)}
+	rc := C.dra_preempt_pdb_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
+		(*C.uint32_t)(pinnedPodOff), (*C.int32_t)(pinnedPrio), C.uint32_t(nPod), (*C.uint32_t)(pinnedCandNodes),
+		(*C.uint32_t)(pinnedCandOff), C.uint32_t(nPair), &r, &b, (*C.uint8_t)(pinnedPairStatus),
+		(*C.uint32_t)(pinnedPairVictims), (*C.uint32_t)(pinnedPairViolations), (*C.uint32_t)(pinnedPodNode),
+		(*C.uint8_t)(pinnedPodStatus), (*C.uint32_t)(pinnedNVictims), (*C.uint32_t)(pinnedPodViolations),
+		(*C.uint32_t)(pinnedVictims), C.uint32_t(maxVictims), C.uint32_t(flags))
 	if rc != 0 {
 		return lastError(c.h)
 	}

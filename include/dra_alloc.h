@@ -289,7 +289,7 @@ int  dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
 
 /* Preemption (spec §14): for pods that fit nowhere, which lower-priority running pods to evict on each candidate node,
  * and which node to evict them on — kube-scheduler's DefaultPreemption (SelectVictimsOnNode, pickOneNodeForPreemption)
- * without PodDisruptionBudgets.  Pure: nothing is written to the inventory. */
+ * without start times; PodDisruptionBudgets through dra_preempt_pdb_batch.  Pure: nothing is written to the inventory. */
 #define DRA_PRE_FITS         0u   /* the pod fits on the node as it is: no victims */
 #define DRA_PRE_EVICT        1u   /* the pod fits once the victims are gone */
 #define DRA_PRE_NO           2u   /* it does not fit even with every lower-priority pod gone (or: no such node) */
@@ -326,6 +326,35 @@ int  dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
                        uint8_t* pair_status, uint32_t* pair_victims,
                        uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
                        uint32_t* victims, uint32_t max_victims, uint32_t flags);
+
+/* Disruption budgets (spec §14, "Disruption budgets"): PodDisruptionBudgets lowered by the caller.  Running pod r counts
+ * against budget run_pdb[r] (at most one; DRA_PDB_NONE for none, also for a pod listed in its budget's DisruptedPods),
+ * whose status.disruptionsAllowed is allowed[b].  NULL, n_pdb == 0 or every run_pdb DRA_PDB_NONE: no budgets. */
+#define DRA_PDB_NONE 0xFFFFFFFFu
+#define DRA_PDB_MAX_RUNNING (1u << 29)   /* with n_pdb > 0, fewer running pods than this (a violation count takes 29 bits) */
+typedef struct dra_disruption_budgets {
+    const uint32_t* run_pdb;   /* [running->n_pod]: budget of each running pod, DRA_PDB_NONE for none */
+    const int32_t*  allowed;   /* [n_pdb]: disruptionsAllowed of each budget */
+    uint32_t        n_pdb;
+} dra_disruption_budgets;
+
+/* dra_preempt_batch with disruption budgets (NULL: none): on each pair, V's members whose eviction would take their
+ * budget below zero (counted over V in order, from allowed afresh for every pair) are reprieved first, then the others;
+ * the pod's EVICT pair is the one with the fewest violating victims first, then dra_preempt_batch's order.  Victim rows
+ * stay in V order.  Two more outputs, each may be NULL:
+ *   pair_violations[k]  the violating victims of an EVICT pair, else 0
+ *   pod_violations[p]   the chosen pair's (EVICT), else 0
+ * With no budgets every output is byte for byte dra_preempt_batch's, every violation count 0.  DRA_E_INVAL with nothing
+ * written: dra_preempt_batch's errors, n_pdb > 0 without allowed, and, when n_pod > 0: a run_pdb[r] neither DRA_PDB_NONE
+ * nor below n_pdb, running pods with n_pdb > 0 and no run_pdb, n_pdb > 0 with DRA_PDB_MAX_RUNNING running pods or more.
+ * n_pod == 0 returns DRA_OK without examining the running pods or run_pdb.  Host buffers. */
+int  dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
+                           const uint32_t* pod_off, const int32_t* prio, uint32_t n_pod,
+                           const uint32_t* cand_nodes, const uint32_t* cand_off,
+                           const dra_running_pods* running, const dra_disruption_budgets* budgets,
+                           uint8_t* pair_status, uint32_t* pair_victims, uint32_t* pair_violations,
+                           uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims, uint32_t* pod_violations,
+                           uint32_t* victims, uint32_t max_victims, uint32_t flags);
 
 /* Preempt and place (spec §15): dra_preempt_batch's question for a batch that sees itself, answered and applied.  Pods
  * are taken in input order; pod p is judged as dra_preempt_batch judges it, but on the inventory as the pods before it
@@ -560,6 +589,20 @@ int  dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
                                      uint8_t* d_pair_status, uint32_t* d_pair_victims,
                                      uint32_t* d_pod_node, uint8_t* d_pod_status, uint32_t* d_n_victims,
                                      uint32_t* d_victims, uint32_t max_victims, uint32_t flags);
+/* dra_preempt_batch_global_device with disruption budgets, as dra_preempt_pdb_batch answers them: `budgets` (NULL: none)
+ * is a host struct whose pointers are device-visible, the SAME on every rank; d_pair_violations and d_pod_violations may
+ * be NULL.  The sizes of dra_set_shard_preempt are unchanged: the violation counts share the partials' and the pair
+ * results' words.  Host-side, before anything is enqueued: n_pdb > 0 without allowed, and with n_pod > 0 running pods
+ * with n_pdb > 0 and no run_pdb, or DRA_PDB_MAX_RUNNING running pods or more, give DRA_E_INVAL.  A run_pdb[r] neither
+ * DRA_PDB_NONE nor below n_pdb is a running-pod fault: DRA_E_INVAL on EVERY rank at dra_ctx_sync, no output written.
+ * With no budgets every output is byte for byte dra_preempt_batch_global_device's. */
+int  dra_preempt_pdb_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                         const uint32_t* d_pod_off, const int32_t* d_prio, uint32_t n_pod,
+                                         const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                         const dra_running_pods* running, const dra_disruption_budgets* budgets,
+                                         uint8_t* d_pair_status, uint32_t* d_pair_victims, uint32_t* d_pair_violations,
+                                         uint32_t* d_pod_node, uint8_t* d_pod_status, uint32_t* d_n_victims,
+                                         uint32_t* d_pod_violations, uint32_t* d_victims, uint32_t max_victims, uint32_t flags);
 
 /* Room for the sharded pod-capacity call in the buffer dra_shard_export maps: each rank's slice holds a 16-byte header,
  * then a u16 count and a u8 stop per pair, each part padded to 16 bytes, so 16 * (1 + ceil(max_pairs / 8) +

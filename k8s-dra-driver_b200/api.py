@@ -18,6 +18,7 @@ OK, E_INVAL, E_CUDA, E_NCCL, E_NOMEM, E_STATE = 0, -1, -2, -3, -4, -5
 CFG_USE_GRAPH, CFG_NO_FUSED, CFG_NO_DIRECT, CFG_RESIDENT = 0x1, 0x2, 0x4, 0x8
 F_NODE_SORTED, F_FRESH_INVENTORY, F_EXHAUSTIVE = 0x1, 0x2, 0x4
 PRE_FITS, PRE_EVICT, PRE_NO, PRE_SEARCH_LIMIT, PRE_INVALID = 0, 1, 2, 3, 4     # dra_preempt_batch statuses (spec §14)
+PDB_NONE = 0xFFFFFFFF                                                           # a running pod under no disruption budget
 # DRA_K_*: the kernels an Allocate-family call enqueued (dra_debug_last_chain)
 KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x00004, "serve": 0x00008,
            "sorted_prep": 0x00010, "bucket_small": 0x00020, "hist8": 0x00040, "hist8_multi": 0x00080,
@@ -46,6 +47,11 @@ class RunningPods(C.Structure):
                 ("prio", C.c_void_p), ("out_off", C.c_void_p), ("out", C.c_void_p), ("n_out", C.c_uint32)]
 
 
+class DisruptionBudgets(C.Structure):
+    """dra_disruption_budgets: the budget of each running pod (PDB_NONE for none) and each budget's disruptionsAllowed."""
+    _fields_ = [("run_pdb", C.c_void_p), ("allowed", C.c_void_p), ("n_pdb", C.c_uint32)]
+
+
 # every symbol include/dra_alloc.h declares: name -> (restype, argtypes)
 _vp, _u32, _i32, _u64 = C.c_void_p, C.c_uint32, C.c_int, C.c_uint64
 SYMBOLS = {
@@ -67,6 +73,8 @@ SYMBOLS = {
     "dra_place_pods_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u32]),
     "dra_deallocate_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_preempt_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32]),
+    "dra_preempt_pdb_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                     _u32, _u32]),
     "dra_preempt_place_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _u32]),
     "dra_pod_capacity_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _u32]),
     "dra_comm_unique_id": (_i32, [_vp]),
@@ -91,6 +99,8 @@ SYMBOLS = {
     "dra_set_shard_preempt": (_i32, [_vp, _u32, _u32, _u32]),
     "dra_preempt_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp,
                                                _vp, _u32, _u32]),
+    "dra_preempt_pdb_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp,
+                                                   _vp, _vp, _vp, _vp, _vp, _u32, _u32]),
     "dra_set_shard_preempt_place": (_i32, [_vp, _u32, _u32, _u32]),
     "dra_preempt_place_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp,
                                                      _vp, _u32]),
@@ -393,6 +403,37 @@ class Context:
         return (pair_status[:n_pair], pair_victims[:n_pair], pod_node[:n_pod], pod_status[:n_pod], n_victims[:n_pod],
                 victims[:n_pod * max_victims].reshape(n_pod, max_victims))
 
+    def preempt_pdb(self, claims, pod_off, prio, run_claims, run_pod_off, run_prio, run_out, run_pdb, pdb_allowed,
+                    run_out_off=None, cand_nodes=None, cand_off=None, max_victims: int = 8, flags: int = 0):
+        """preempt() with disruption budgets (spec §14, "Disruption budgets"): run_pdb[r] the budget running pod r counts
+        against (PDB_NONE for none; None: no array), pdb_allowed[b] each budget's disruptionsAllowed (None: no budgets).
+        Returns preempt()'s six outputs, then pair_violations and pod_violations (uint32)."""
+        c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
+        po = np.ascontiguousarray(pod_off, dtype=np.uint32)
+        pr = np.ascontiguousarray(prio, dtype=np.int32)
+        n_pod = len(po) - 1
+        run = _running(run_claims, run_pod_off, run_prio, run_out, run_out_off)
+        rp = None if run_pdb is None else np.ascontiguousarray(run_pdb, dtype=np.uint32)
+        al = None if pdb_allowed is None else np.ascontiguousarray(pdb_allowed, dtype=np.int32)
+        bud = DisruptionBudgets(None if rp is None or not len(rp) else rp.ctypes.data,
+                                None if al is None or not len(al) else al.ctypes.data, 0 if al is None else len(al))
+        cn, co = _cands(cand_nodes, cand_off)
+        n_pair = n_pod * self.n_node if co is None else int(co[-1])
+        pair_status = np.zeros(max(n_pair, 1), dtype=np.uint8)
+        pair_victims = np.zeros(max(n_pair, 1), dtype=np.uint32)
+        pair_viol = np.zeros(max(n_pair, 1), dtype=np.uint32)
+        pod_node = np.zeros(max(n_pod, 1), dtype=np.uint32)
+        pod_status = np.zeros(max(n_pod, 1), dtype=np.uint8)
+        n_victims = np.zeros(max(n_pod, 1), dtype=np.uint32)
+        pod_viol = np.zeros(max(n_pod, 1), dtype=np.uint32)
+        victims = np.zeros(max(n_pod * max_victims, 1), dtype=np.uint32)
+        self._check(self._lib.dra_preempt_pdb_batch(
+            self._h, _ptr(c), len(c), _ptr(po), _ptr(pr), n_pod, _ptr(cn), _ptr(co), C.byref(run), C.byref(bud),
+            _ptr(pair_status), _ptr(pair_victims), _ptr(pair_viol), _ptr(pod_node), _ptr(pod_status), _ptr(n_victims),
+            _ptr(pod_viol), _ptr(victims) if max_victims else None, max_victims, flags))
+        return (pair_status[:n_pair], pair_victims[:n_pair], pod_node[:n_pod], pod_status[:n_pod], n_victims[:n_pod],
+                victims[:n_pod * max_victims].reshape(n_pod, max_victims), pair_viol[:n_pair], pod_viol[:n_pod])
+
     def preempt_place(self, claims, pod_off, prio, run_claims, run_pod_off, run_prio, run_out, run_out_off=None,
                       cand_nodes=None, cand_off=None, out_off=None, n_out=None, flags: int = 0):
         """Preempt and place (spec §15): pods in input order, each judged as preempt() judges it on the inventory the pods
@@ -571,6 +612,21 @@ class Context:
             self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), _ptr(d_prio), n_pod, _ptr(d_cand_nodes), _ptr(d_cand_off),
             n_pair, C.byref(running), _ptr(d_pair_status), _ptr(d_pair_victims), _ptr(d_pod_node), _ptr(d_pod_status),
             _ptr(d_n_victims), _ptr(d_victims), max_victims, flags))
+
+    def preempt_pdb_global_device(self, d_claims: int, n_claim: int, d_pod_off: int, d_prio: int, n_pod: int,
+                                  d_cand_nodes: int | None, d_cand_off: int | None, n_pair: int, running: "RunningPods",
+                                  budgets: "DisruptionBudgets | None", d_pair_status: int | None, d_pair_victims: int | None,
+                                  d_pair_violations: int | None, d_pod_node: int, d_pod_status: int, d_n_victims: int,
+                                  d_pod_violations: int | None, d_victims: int | None, max_victims: int,
+                                  flags: int = 0) -> None:
+        """preempt_global_device() with disruption budgets, as preempt_pdb() answers them: `budgets` a DisruptionBudgets
+        whose pointers are device-visible (None: none), the same on every rank; the violation outputs (uint32) may be
+        None.  Enqueues, no synchronisation; errors found on the device surface at sync()."""
+        self._check(self._lib.dra_preempt_pdb_batch_global_device(
+            self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), _ptr(d_prio), n_pod, _ptr(d_cand_nodes), _ptr(d_cand_off),
+            n_pair, C.byref(running), None if budgets is None else C.byref(budgets), _ptr(d_pair_status),
+            _ptr(d_pair_victims), _ptr(d_pair_violations), _ptr(d_pod_node), _ptr(d_pod_status), _ptr(d_n_victims),
+            _ptr(d_pod_violations), _ptr(d_victims), max_victims, flags))
 
     def set_shard_capacity(self, max_pairs: int) -> None:
         """Room for the sharded pod-capacity call's pair results; world > 1: before shard_export, the same on every rank."""

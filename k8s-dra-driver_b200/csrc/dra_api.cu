@@ -113,11 +113,13 @@ struct dra_ctx {
     int place_occ = -1;                   // resident CTAs of k_pods_place<4> per SM (occupancy query, once)
     // preemption (spec §14): per pending pod, per pair, the running pods and the victim rows
     uint32_t *d_pre_prio = nullptr, *d_pre_node = nullptr, *d_pre_nvic = nullptr, *d_pre_choice = nullptr; uint8_t* d_pre_pst = nullptr;
-    size_t cap_pre_pods = 0;
+    uint32_t* d_pre_podviol = nullptr; size_t cap_pre_pods = 0;
     uint4* d_pre_psum = nullptr; unsigned long long* d_pre_psum64 = nullptr; uint8_t* d_pre_pairst = nullptr;
-    uint32_t* d_pre_pairvic = nullptr; size_t cap_pre_pairs = 0;
+    uint32_t *d_pre_pairvic = nullptr, *d_pre_pairviol = nullptr; size_t cap_pre_pairs = 0;
     uint4* d_pre_rclaims = nullptr; uint32_t* d_pre_routoff = nullptr; size_t cap_pre_rclaims = 0;
-    uint32_t *d_pre_rpodoff = nullptr, *d_pre_rprio = nullptr; uint4 *d_pre_rrec = nullptr, *d_pre_vlist = nullptr; size_t cap_pre_rpods = 0;
+    uint32_t *d_pre_rpodoff = nullptr, *d_pre_rprio = nullptr; uint4 *d_pre_rrec = nullptr, *d_pre_vlist = nullptr;
+    uint32_t *d_pre_rpdb = nullptr, *d_pre_vprev = nullptr; size_t cap_pre_rpods = 0;   // budgets: run_pdb, vprev
+    int32_t* d_pre_allowed = nullptr; size_t cap_pre_allowed = 0;                        // budgets: disruptionsAllowed
     uint2* d_pre_rout = nullptr; size_t cap_pre_rout = 0;
     uint32_t* d_pre_vic = nullptr; size_t cap_pre_vic = 0;
     // preempt and place (spec §15): per pending pod, per running pod, per node (the running lists' offsets, the last pod
@@ -741,11 +743,13 @@ int check_err(dra_ctx* ctx) {
                                       "outside n_out, or OK slots naming a GPU index >= n_gpu or GPUs of two nodes; nothing was written");
     if (bo && (ctx->chain & DRA_K_PREEMPT))
         return fail(ctx, DRA_E_INVAL, "dra_preempt_batch: running pods: pod_off not monotone or not spanning the claims, a slot range outside "
-                                      "n_out, or OK slots naming a GPU index >= n_gpu or GPUs of two nodes; nothing was written");
+                                      "n_out, OK slots naming a GPU index >= n_gpu or GPUs of two nodes, or a budget neither "
+                                      "DRA_PDB_NONE nor below n_pdb; nothing was written");
     if (bo && (ctx->chain & DRA_K_PREEMPT_SHARD))
         return fail(ctx, DRA_E_INVAL, "sharded preemption: pod_off / cand_off not monotone or not spanning their arrays, or running pods: pod_off "
-                                      "not monotone or not spanning the claims, a slot range outside n_out, or OK slots naming a GPU index "
-                                      ">= n_gpu or GPUs of two nodes (on this rank or a peer); nothing was written");
+                                      "not monotone or not spanning the claims, a slot range outside n_out, OK slots naming a GPU index "
+                                      ">= n_gpu or GPUs of two nodes, or a budget neither DRA_PDB_NONE nor below n_pdb (on this rank "
+                                      "or a peer); nothing was written");
     if (bo && (ctx->chain & DRA_K_PREEMPT_PLACE_SHARD))
         return fail(ctx, DRA_E_INVAL, "sharded preempt and place: pod_off / cand_off not monotone or not spanning their arrays, more than %u "
                                       "candidates for a pod, a pending slot outside n_out, or running pods: pod_off not monotone or not "
@@ -772,9 +776,12 @@ int pp_buffers(dra_ctx* ctx, uint32_t n_pod, uint32_t n_pair, uint32_t rn_pod) {
     if ((rc = grow_set(ctx, ctx->cap_podrec, pairs, ctx->d_podrec)) ||
         (rc = grow_set(ctx, ctx->cap_place_pods, pods, ctx->d_place_state, ctx->d_place_node)) ||
         (rc = grow_set(ctx, ctx->cap_place_cursor, nodes, ctx->d_place_cursor)) ||
-        (rc = grow_set(ctx, ctx->cap_pre_pods, pods, ctx->d_pre_prio, ctx->d_pre_node, ctx->d_pre_nvic, ctx->d_pre_choice, ctx->d_pre_pst)) ||
-        (rc = grow_set(ctx, ctx->cap_pre_pairs, pairs, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic)) ||
-        (rc = grow_set(ctx, ctx->cap_pre_rpods, rpods, ctx->d_pre_rpodoff, ctx->d_pre_rprio, ctx->d_pre_rrec, ctx->d_pre_vlist)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_pods, pods, ctx->d_pre_prio, ctx->d_pre_node, ctx->d_pre_nvic, ctx->d_pre_choice, ctx->d_pre_pst,
+                       ctx->d_pre_podviol)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_pairs, pairs, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic,
+                       ctx->d_pre_pairviol)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_rpods, rpods, ctx->d_pre_rpodoff, ctx->d_pre_rprio, ctx->d_pre_rrec, ctx->d_pre_vlist,
+                       ctx->d_pre_rpdb, ctx->d_pre_vprev)) ||
         (rc = grow_set(ctx, ctx->cap_pp_pods, pods, ctx->d_pp_pending)) ||
         (rc = grow_set(ctx, ctx->cap_pp_rpods, rpods, ctx->d_pp_evicted)) ||
         (rc = grow_set(ctx, ctx->cap_pp_nodes, nodes, ctx->d_pp_runoff, ctx->d_pp_judged))) return rc;
@@ -787,7 +794,7 @@ size_t al16(size_t b) { return (b + 15) & ~(size_t)15; }
 // by the caller (stage_in's fill).  A fixed array, nothing allocated per call: a part beyond CAP is not kept, and
 // stage_in refuses the call.
 struct Staging {
-    static constexpr int CAP = 12;
+    static constexpr int CAP = 14;
     struct Part { void* dst; const void* src; size_t bytes; };
     Part part[CAP];
     int n = 0;
@@ -819,11 +826,14 @@ int stage_in(dra_ctx* ctx, const Staging& s, Fill fill) {
 }
 int stage_in(dra_ctx* ctx, const Staging& s) { return stage_in(ctx, s, [](uint8_t*) {}); }
 
-// The caller's running pods R as parts of s, into the d_pre_r* buffers (grown as needed); dev = R with those device pointers
-int running_parts(dra_ctx* ctx, const dra_running_pods& R, Staging& s, dra_running_pods& dev) {
+// The caller's running pods R as parts of s, into the d_pre_r* buffers (grown as needed); dev = R with those device pointers.
+// B (NULL: none): the budgets too, Bd = B with device pointers.
+int running_parts(dra_ctx* ctx, const dra_running_pods& R, Staging& s, dra_running_pods& dev,
+                  const dra_disruption_budgets* B = nullptr, dra_disruption_budgets* Bd = nullptr) {
     int rc;
     if ((rc = grow_set(ctx, ctx->cap_pre_rclaims, (size_t)R.n_claim + 8, ctx->d_pre_rclaims, ctx->d_pre_routoff)) ||
-        (rc = grow_set(ctx, ctx->cap_pre_rpods, (size_t)R.n_pod + 8, ctx->d_pre_rpodoff, ctx->d_pre_rprio, ctx->d_pre_rrec, ctx->d_pre_vlist)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_rpods, (size_t)R.n_pod + 8, ctx->d_pre_rpodoff, ctx->d_pre_rprio, ctx->d_pre_rrec, ctx->d_pre_vlist,
+                       ctx->d_pre_rpdb, ctx->d_pre_vprev)) ||
         (rc = grow_set(ctx, ctx->cap_pre_rout, (size_t)R.n_out + 8, ctx->d_pre_rout))) return rc;
     s.add(ctx->d_pre_rclaims, R.claims, (size_t)R.n_claim * 16);
     s.add(ctx->d_pre_rpodoff, R.pod_off, ((size_t)R.n_pod + 1) * 4);
@@ -834,6 +844,12 @@ int running_parts(dra_ctx* ctx, const dra_running_pods& R, Staging& s, dra_runni
     dev.claims = (const dra_claim_rec*)ctx->d_pre_rclaims; dev.pod_off = ctx->d_pre_rpodoff;
     dev.prio = (const int32_t*)ctx->d_pre_rprio; dev.out_off = R.out_off ? ctx->d_pre_routoff : nullptr;
     dev.out = (const dra_out_rec*)ctx->d_pre_rout;
+    if (!B) return DRA_OK;
+    if ((rc = grow_set(ctx, ctx->cap_pre_allowed, (size_t)B->n_pdb + 8, ctx->d_pre_allowed))) return rc;
+    s.add(ctx->d_pre_rpdb, B->run_pdb, B->run_pdb ? (size_t)R.n_pod * 4 : 0);
+    s.add(ctx->d_pre_allowed, B->allowed, B->n_pdb ? (size_t)B->n_pdb * 4 : 0);
+    *Bd = *B;
+    Bd->run_pdb = B->run_pdb ? ctx->d_pre_rpdb : nullptr; Bd->allowed = B->n_pdb ? ctx->d_pre_allowed : nullptr;
     return DRA_OK;
 }
 
@@ -983,6 +999,25 @@ PreArgs pre_args(dra_ctx* ctx, const uint4* claims, const uint32_t* pod_off, con
     a.pod_node = ctx->d_pre_node; a.pod_status = ctx->d_pre_pst;
     a.gate = ctx->d_err + ERR_BAD_OFFSETS; a.err = err_of(ctx);
     return a;
+}
+
+// a's disruption budgets from B (pointers the device reads; NULL: none): run_pdb checked whenever given, the budgets in
+// force when n_pdb > 0 and there are running pods
+void pre_budgets(dra_ctx* ctx, PreArgs& a, const dra_disruption_budgets* B) {
+    if (!B) return;
+    a.run_pdb = a.rn_pod ? B->run_pdb : nullptr; a.pdb_allowed = B->allowed; a.n_pdb = B->n_pdb;
+    a.pdb = B->n_pdb && a.rn_pod ? 1u : 0u;
+    a.vprev = ctx->d_pre_vprev;
+}
+
+// The budget arguments of a preemption call that has pending pods (spec §14, "Disruption budgets"; NULL: none)
+int check_budgets(dra_ctx* ctx, const char* name, const dra_disruption_budgets* B, uint32_t rn_pod) {
+    if (!B || !B->n_pdb) return DRA_OK;
+    if (!B->allowed) return fail(ctx, DRA_E_INVAL, "%s: n_pdb %u without allowed", name, B->n_pdb);
+    if (rn_pod && !B->run_pdb) return fail(ctx, DRA_E_INVAL, "%s: %u running pods and %u budgets without run_pdb", name, rn_pod, B->n_pdb);
+    if (rn_pod >= DRA_PDB_MAX_RUNNING)
+        return fail(ctx, DRA_E_INVAL, "%s: %u running pods with budgets: at most %u", name, rn_pod, DRA_PDB_MAX_RUNNING - 1);
+    return DRA_OK;
 }
 
 // The running lists: k_pre_running, its records bucketed by node with the counting sort (without running pods the
@@ -1332,7 +1367,8 @@ void dra_ctx_destroy(dra_ctx* c) {
                    c->d_place_state, c->d_place_node, c->d_place_cursor, c->d_splace_local, c->d_splace_rec,
                    c->d_pre_prio, c->d_pre_node, c->d_pre_nvic, c->d_pre_choice, c->d_pre_pst, c->d_pre_psum, c->d_pre_psum64,
                    c->d_pre_pairst, c->d_pre_pairvic, c->d_pre_rclaims, c->d_pre_routoff, c->d_pre_rpodoff, c->d_pre_rprio,
-                   c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic, c->d_spre_part,
+                   c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic, c->d_spre_part, c->d_pre_podviol,
+                   c->d_pre_pairviol, c->d_pre_rpdb, c->d_pre_vprev, c->d_pre_allowed,
                    c->d_pp_pending, c->d_pp_evicted, c->d_pp_runoff, c->d_pp_judged, c->d_spp_inv, c->d_spp_gate,
                    c->d_cap_copies, c->d_cap_stop, c->d_cap_total, c->d_cap_nodes, c->d_scap_part};
     for (void* p : dev) if (p) cudaFree(p);
@@ -1791,10 +1827,11 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
 // Preemption (spec §14): the pending-pod arrays are checked here; the running pods on the device (k_pre_running), whose
 // fault gates every later kernel.  Inputs are staged in, the kernels launched, the outputs copied back after ONE
 // synchronise, and the caller's buffers are written only when no fault was found.
-int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, const int32_t* prio,
-                      uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, const dra_running_pods* running,
-                      uint8_t* pair_status, uint32_t* pair_victims, uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
-                      uint32_t* victims, uint32_t max_victims, uint32_t flags) {
+int dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, const int32_t* prio,
+                          uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, const dra_running_pods* running,
+                          const dra_disruption_budgets* budgets, uint8_t* pair_status, uint32_t* pair_victims,
+                          uint32_t* pair_violations, uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
+                          uint32_t* pod_violations, uint32_t* victims, uint32_t max_victims, uint32_t flags) {
     if (!ctx || !pod_off || !running || !running->pod_off || (n_claim && !claims) || (n_pod && (!prio || !pod_node || !pod_status || !n_victims)))
         return DRA_E_INVAL;
     const dra_running_pods& R = *running;
@@ -1803,6 +1840,8 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
     if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_preempt_batch: unknown flags 0x%x", flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     if (max_victims && !victims) return fail(ctx, DRA_E_INVAL, "max_victims %u without a victims buffer", max_victims);
+    if (budgets && budgets->n_pdb && !budgets->allowed)
+        return fail(ctx, DRA_E_INVAL, "dra_preempt_pdb_batch: n_pdb %u without allowed", budgets->n_pdb);
     bool dense; uint32_t n_pair;
     int rc;
     if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
@@ -1810,21 +1849,26 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
         (rc = check_sortable(ctx, n_pod ? R.n_pod : 0))) return rc;
     ctx->chain = DRA_K_PREEMPT; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
+    if ((rc = check_budgets(ctx, "dra_preempt_pdb_batch", budgets, R.n_pod))) return rc;
     CU(cudaSetDevice(ctx->device));
     if ((rc = ensure_batch(ctx, std::max(n_claim, R.n_pod), 1, true))) return rc;
     if ((rc = upload_table(ctx))) return rc;
     const size_t vb = (size_t)n_pod * max_victims * 4;
     if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
         (!dense && (rc = grow_set(ctx, ctx->cap_pairs, (size_t)n_pair + 64, ctx->d_cand_nodes, ctx->d_pair_pod))) ||
-        (rc = grow_set(ctx, ctx->cap_pre_pods, (size_t)n_pod + 8, ctx->d_pre_prio, ctx->d_pre_node, ctx->d_pre_nvic, ctx->d_pre_choice, ctx->d_pre_pst)) ||
-        (rc = grow_set(ctx, ctx->cap_pre_pairs, (size_t)n_pair + 8, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_pods, (size_t)n_pod + 8, ctx->d_pre_prio, ctx->d_pre_node, ctx->d_pre_nvic, ctx->d_pre_choice, ctx->d_pre_pst,
+                       ctx->d_pre_podviol)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_pairs, (size_t)n_pair + 8, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic,
+                       ctx->d_pre_pairviol)) ||
         (rc = grow_set(ctx, ctx->cap_pre_vic, vb / 4 + 8, ctx->d_pre_vic))) return rc;
     const Outputs outs = {{pair_status, ctx->d_pre_pairst, pair_status ? (size_t)n_pair : 0},
                           {pair_victims, ctx->d_pre_pairvic, pair_victims ? (size_t)n_pair * 4 : 0},
                           {pod_node, ctx->d_pre_node, (size_t)n_pod * 4},
                           {pod_status, ctx->d_pre_pst, n_pod},
                           {n_victims, ctx->d_pre_nvic, (size_t)n_pod * 4},
-                          {victims, ctx->d_pre_vic, vb}};
+                          {victims, ctx->d_pre_vic, vb},
+                          {pair_violations, ctx->d_pre_pairviol, pair_violations ? (size_t)n_pair * 4 : 0},
+                          {pod_violations, ctx->d_pre_podviol, pod_violations ? (size_t)n_pod * 4 : 0}};
     if ((rc = reserve_out(ctx, outs))) return rc;
     Staging s;
     s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
@@ -1836,7 +1880,8 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
         s.add(ctx->d_pair_pod, nullptr, (size_t)n_pair * 4);
     }
     dra_running_pods Rd;
-    if ((rc = running_parts(ctx, R, s, Rd)) ||
+    dra_disruption_budgets Bd;
+    if ((rc = running_parts(ctx, R, s, Rd, budgets, &Bd)) ||
         (rc = stage_in(ctx, s, [&](uint8_t* h) { expand_pairs((uint32_t*)h, cand_off, n_pod); }))) return rc;
 
     PreArgs a = pre_args(ctx, ctx->d_claims, ctx->d_pod_off, (const int32_t*)ctx->d_pre_prio, n_pod, dense ? nullptr : ctx->d_cand_nodes,
@@ -1844,6 +1889,8 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
     a.pair_pod = dense ? nullptr : ctx->d_pair_pod;
     a.pair_status = pair_status ? ctx->d_pre_pairst : nullptr; a.pair_victims = pair_victims ? ctx->d_pre_pairvic : nullptr;
     a.n_victims = ctx->d_pre_nvic; a.choice = ctx->d_pre_choice; a.max_victims = max_victims;
+    pre_budgets(ctx, a, budgets ? &Bd : nullptr);
+    a.pair_viol = pair_violations ? ctx->d_pre_pairviol : nullptr; a.pod_viol = pod_violations ? ctx->d_pre_podviol : nullptr;
     Prof prof(ctx);
     if ((rc = launch_running_lists(ctx, a, prof, false))) return rc;
     const PreShard whole{0u, ctx->n_node, n_pair, 0u, nullptr, nullptr};
@@ -1857,6 +1904,14 @@ int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_clai
     }
     prof.mark();
     return read_back(ctx, "preemption kernels", 1, outs);
+}
+
+int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, const int32_t* prio,
+                      uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, const dra_running_pods* running,
+                      uint8_t* pair_status, uint32_t* pair_victims, uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
+                      uint32_t* victims, uint32_t max_victims, uint32_t flags) {
+    return dra_preempt_pdb_batch(ctx, claims, n_claim, pod_off, prio, n_pod, cand_nodes, cand_off, running, nullptr, pair_status,
+                                 pair_victims, nullptr, pod_node, pod_status, n_victims, nullptr, victims, max_victims, flags);
 }
 
 // Pod capacity (spec §16): every argument is checked here, before anything is staged or launched, so a rejected call
@@ -2130,8 +2185,10 @@ int spre_buffers(dra_ctx* ctx, uint32_t n_pod, uint32_t n_pair, uint32_t max_vic
     int rc;
     if ((rc = grow(ctx, ctx->d_spre_part, ctx->cap_spre_part, spre_units(n_pod, n_pair, max_victims)))) return rc;
     if ((rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, std::max(n_pair, 1u)))) return rc;
-    if ((rc = grow_set(ctx, ctx->cap_pre_pairs, (size_t)n_pair + 8, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic)) ||
-        (rc = grow_set(ctx, ctx->cap_pre_rpods, (size_t)rn_pod + 8, ctx->d_pre_rpodoff, ctx->d_pre_rprio, ctx->d_pre_rrec, ctx->d_pre_vlist))) return rc;
+    if ((rc = grow_set(ctx, ctx->cap_pre_pairs, (size_t)n_pair + 8, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic,
+                       ctx->d_pre_pairviol)) ||
+        (rc = grow_set(ctx, ctx->cap_pre_rpods, (size_t)rn_pod + 8, ctx->d_pre_rpodoff, ctx->d_pre_rprio, ctx->d_pre_rrec, ctx->d_pre_vlist,
+                       ctx->d_pre_rpdb, ctx->d_pre_vprev))) return rc;
     return DRA_OK;
 }
 
@@ -2848,13 +2905,13 @@ int dra_set_shard_preempt(dra_ctx* ctx, uint32_t max_pods, uint32_t max_pairs, u
 // the whole inventory (k_pre_running, the counting sort, k_pre_vsort) -> the window's pairs (k_pods_preempt) -> per-pod
 // partials (k_spre_reduce, k_pods_preempt_victims) -> push to every peer -> wait + merge into the caller's buffers (k_spre_merge).
 // Enqueues only.
-int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
-                                    const uint32_t* d_pod_off, const int32_t* d_prio, uint32_t n_pod,
-                                    const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
-                                    const dra_running_pods* running,
-                                    uint8_t* d_pair_status, uint32_t* d_pair_victims,
-                                    uint32_t* d_pod_node, uint8_t* d_pod_status, uint32_t* d_n_victims,
-                                    uint32_t* d_victims, uint32_t max_victims, uint32_t flags) {
+int dra_preempt_pdb_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                        const uint32_t* d_pod_off, const int32_t* d_prio, uint32_t n_pod,
+                                        const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                        const dra_running_pods* running, const dra_disruption_budgets* budgets,
+                                        uint8_t* d_pair_status, uint32_t* d_pair_victims, uint32_t* d_pair_violations,
+                                        uint32_t* d_pod_node, uint8_t* d_pod_status, uint32_t* d_n_victims,
+                                        uint32_t* d_pod_violations, uint32_t* d_victims, uint32_t max_victims, uint32_t flags) {
     if (!ctx || !d_pod_off || !running || !running->pod_off || (n_claim && !d_claims) ||
         (n_pod && (!d_prio || !d_pod_node || !d_pod_status || !d_n_victims)))
         return DRA_E_INVAL;
@@ -2864,6 +2921,8 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_preempt_batch_global_device: unknown flags 0x%x", flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     if (max_victims && !d_victims) return fail(ctx, DRA_E_INVAL, "max_victims %u without a victims buffer", max_victims);
+    if (budgets && budgets->n_pdb && !budgets->allowed)
+        return fail(ctx, DRA_E_INVAL, "dra_preempt_pdb_batch_global_device: n_pdb %u without allowed", budgets->n_pdb);
     bool dense;
     if (int rc = check_dev_cands(ctx, d_cand_nodes, d_cand_off, n_pod, n_pair, true, dense)) return rc;
     if (n_pod > (1u << 26) || max_victims > (1u << 20)) return fail(ctx, DRA_E_INVAL, "n_pod or max_victims too large for the sharded call");
@@ -2877,6 +2936,7 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
         return rc;
     ctx->chain = DRA_K_PREEMPT_SHARD; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
+    if (int rc = check_budgets(ctx, "dra_preempt_pdb_batch_global_device", budgets, R.n_pod)) return rc;
     CallScope scope{ctx};
     int rc = scope.open(gather);
     if (rc) return rc;
@@ -2884,7 +2944,7 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     if ((rc = spre_buffers(ctx, n_pod, n_pair, max_victims, R.n_pod))) return rc;
     cudaStream_t st = ctx->stream;
     const uint32_t lo = gather ? ctx->shard_lo : 0u, hi = gather ? ctx->shard_hi : ctx->n_node;   // world 1: every node
-    const bool want_pairs = d_pair_status || d_pair_victims;
+    const bool want_pairs = d_pair_status || d_pair_victims || d_pair_violations;
     PreShard s; memset(&s, 0, sizeof s);
     s.node_lo = lo; s.node_hi = hi; s.n_walk = dense ? n_pod * (hi - lo) : n_pair;
     s.stride = 2 + (max_victims + 3) / 4; s.part = ctx->d_spre_part;
@@ -2893,6 +2953,7 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     PreArgs a = pre_args(ctx, (const uint4*)d_claims, d_pod_off, d_prio, n_pod, dense ? nullptr : d_cand_nodes,
                          dense ? nullptr : d_cand_off, n_pair, R, ctx->d_inv_live, flags);
     a.pair_pod = dense ? nullptr : ctx->d_upair_pod; a.max_victims = max_victims;
+    pre_budgets(ctx, a, budgets);
     Prof prof(ctx);
     k_uns_prep<<<std::max(1u, (n_pod + 7) / 8), 256, 0, st>>>(d_pod_off, dense ? nullptr : d_cand_off, n_pod, n_claim, n_pair,
                                                               ctx->d_upair_pod, a.err);
@@ -2916,6 +2977,7 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     if (gather) for (int r = 0; r <= ctx->world; ++r) m.bounds[r] = ctx->shard_bounds[r];
     m.pair_status = d_pair_status; m.pair_victims = d_pair_victims;
     m.pod_node = d_pod_node; m.pod_status = d_pod_status; m.n_victims = d_n_victims; m.victims = max_victims ? d_victims : nullptr;
+    m.pair_viol = d_pair_violations; m.pod_viol = d_pod_violations;
     const PeerExchange x = gather ? bind_exchange(ctx, ctx->pre_x) : PeerExchange{};   // world 1: no peers
     if (gather) {
         m.slice4 = (uint32_t)(ctx->pre_x.slice / 16);
@@ -2929,6 +2991,18 @@ int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims,
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded preemption launch: %s", cudaGetErrorString(e));
     return DRA_OK;
+}
+
+int dra_preempt_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                    const uint32_t* d_pod_off, const int32_t* d_prio, uint32_t n_pod,
+                                    const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                    const dra_running_pods* running,
+                                    uint8_t* d_pair_status, uint32_t* d_pair_victims,
+                                    uint32_t* d_pod_node, uint8_t* d_pod_status, uint32_t* d_n_victims,
+                                    uint32_t* d_victims, uint32_t max_victims, uint32_t flags) {
+    return dra_preempt_pdb_batch_global_device(ctx, d_claims, n_claim, d_pod_off, d_prio, n_pod, d_cand_nodes, d_cand_off, n_pair,
+                                               running, nullptr, d_pair_status, d_pair_victims, nullptr, d_pod_node,
+                                               d_pod_status, d_n_victims, nullptr, d_victims, max_victims, flags);
 }
 
 int dra_set_shard_capacity(dra_ctx* ctx, uint32_t max_pairs) {

@@ -3541,7 +3541,8 @@ struct PreArgs {
     uint4* vlist;                 // each node's list by priority descending, then index: {claims, index, first claim, prio}
     const uint4* inv; const uint32_t* node_off; uint32_t n_node, n_gpu; const uint32_t* tbl; SelCtx sel;
     uint32_t exhaustive;
-    uint4* psum;                  // [n_pair] {status, victims, highest victim priority, running index of the first victim}
+    uint4* psum;                  // [n_pair] {status | violations << PRE_VSHIFT, victims, highest victim priority, lowest
+                                  //  running index among the victims of that priority}
     unsigned long long* psum64;   // [n_pair] sum over the victims of (priority + 2^31)
     uint8_t* pair_status; uint32_t* pair_victims;                   // caller's per-pair outputs (may be nullptr)
     uint32_t* pod_node; uint8_t* pod_status; uint32_t* n_victims; uint32_t* choice;
@@ -3549,7 +3550,18 @@ struct PreArgs {
     unsigned long long* work;     // next unclaimed pair (zeroed by the host)
     const uint32_t* gate;         // non-zero: the running pods failed their check, nothing is evaluated
     Err err;
+    // disruption budgets (spec §14, "Disruption budgets"; dra_preempt_pdb_batch), all nullptr / 0 without them
+    const uint32_t* run_pdb;      // [rn_pod] each running pod's budget, or DRA_PDB_NONE (checked by k_pre_running)
+    const int32_t* pdb_allowed;   // [n_pdb] disruptionsAllowed
+    uint32_t n_pdb;
+    uint32_t pdb;                 // non-zero: budgets in force (n_pdb > 0, running pods): vprev is built and read
+    uint32_t* vprev;              // [rn_pod] per vlist position, the previous position of its node's list with the same budget
+    uint32_t* pair_viol; uint32_t* pod_viol;                        // caller's violation outputs (may be nullptr)
 };
+
+// psum[k].x and the sharded call's pair records hold status | violations << PRE_VSHIFT (a status takes 3 bits; the
+// violations fit the other 29 because a budgeted call has fewer than 2^29 running pods)
+constexpr uint32_t PRE_VSHIFT = 3, PRE_ST_MASK = (1u << PRE_VSHIFT) - 1u;
 
 // The pair kernel's node window and the sharded call's partials (layout at k_spre_reduce).  The single-inventory call:
 // the window [0, n_node), n_walk = n_pair, no partials.
@@ -3563,7 +3575,8 @@ struct PreShard {
 
 // Thread per running pod.  Its node is the node of the GPUs its OK slots name (slots counted as §9 counts them); a pod
 // without an OK slot is on no node.  Offsets not monotone or not spanning, a slot range outside rn_out, a GPU index
-// >= n_gpu or GPUs of two nodes set ERR_BAD_OFFSETS, which gates every kernel after the sort.
+// >= n_gpu or GPUs of two nodes set ERR_BAD_OFFSETS, which gates every kernel after the sort; so does a budget that is
+// neither DRA_PDB_NONE nor below n_pdb.
 __global__ void __launch_bounds__(256)
 k_pre_running(const PreArgs a) {
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
@@ -3573,6 +3586,10 @@ k_pre_running(const PreArgs a) {
     const bool have_off = a.rout_off != nullptr;
     uint32_t node = DRA_GPU_NONE;
     bool bad = c1 < c0 || c1 > a.rn_claim;
+    if (a.run_pdb) {
+        const uint32_t b = __ldg(&a.run_pdb[r]);
+        bad = bad || (b != DRA_PDB_NONE && b >= a.n_pdb);
+    }
     for (uint32_t i = c0; !bad && i < c1; ++i) {
         const uint4 c = __ldg(&a.rclaims[i]);
         const uint32_t base = have_off ? __ldg(&a.rout_off[i]) : i, slots = dealloc_slots(c, a.n_node, have_off);
@@ -3592,6 +3609,8 @@ k_pre_running(const PreArgs a) {
 
 // CTA per node: the node's running pods (index order after the stable bucketing) ranked by (priority descending, index
 // ascending), a total order, so each pod's rank is the number of pods before it.  Quadratic in the pods of one node.
+// With budgets, then each list position's previous position with the same budget (vprev; NONE for none or no budget),
+// also quadratic at worst.
 __global__ void __launch_bounds__(256)
 k_pre_vsort(const PreArgs a) {
     if (__ldcg(a.gate)) return;
@@ -3605,6 +3624,15 @@ k_pre_vsort(const PreArgs a) {
                 rank += ((int32_t)o.w > (int32_t)me.w || ((int32_t)o.w == (int32_t)me.w && o.y < me.y)) ? 1u : 0u;
             }
             a.vlist[l0 + rank] = me;
+        }
+        if (!a.pdb) continue;
+        __syncthreads();                                                 // the node's list is in place
+        for (uint32_t e = l0 + threadIdx.x; e < l1; e += blockDim.x) {
+            const uint32_t b = __ldg(&a.run_pdb[__ldcg(&a.vlist[e]).y]);
+            uint32_t prev = DRA_GPU_NONE;
+            for (uint32_t f = e; b != DRA_PDB_NONE && f-- > l0;)
+                if (__ldg(&a.run_pdb[__ldcg(&a.vlist[f]).y]) == b) { prev = f; break; }
+            a.vprev[e] = prev;
         }
     }
 }
@@ -3634,7 +3662,24 @@ __device__ __forceinline__ void pre_apply(Lane& L, const PreArgs& a, const uint4
     }
 }
 
-struct PreSum { uint32_t st, count, hi, hi_idx; unsigned long long sum; };
+// A pair's summary: status, victims, the highest victim priority and the lowest running index among the victims of that
+// priority, the sum of (priority + 2^31) over the victims, and the victims whose eviction violates a budget
+struct PreSum { uint32_t st, count, hi, hi_idx; unsigned long long sum; uint32_t viol; };
+
+// Is V's member at list position v (running pod y) violating (spec §14, "Disruption budgets"): do the members in the list
+// positions [v0, v] that count against its budget b number more than allowed[b]?  Walks b's chain back from v through
+// vprev, at most allowed[b] steps.  The same on every lane.
+__device__ __forceinline__ bool pre_violating(const PreArgs& a, const uint32_t v0, uint32_t v, const uint32_t y) {
+    const uint32_t b = __ldg(&a.run_pdb[y]);
+    if (b == DRA_PDB_NONE) return false;
+    const int32_t allowed = __ldg(&a.pdb_allowed[b]);
+    if (allowed < 0) return true;
+    for (uint32_t n = 0; n < (uint32_t)allowed; ++n) {                   // n + 1 members of b found in [v, v1)
+        v = __ldcg(&a.vprev[v]);
+        if (v == DRA_GPU_NONE || v < v0) return false;
+    }
+    return true;
+}
 
 // Is the pod of cnt claims at `claims` INVALID: more than DRA_MAX_POD claims, or one invalid in slot mode have_off (§1) or
 // naming a selector past n_sel?  On the W lanes gbase.. (gl = lane - gbase; gmask the group's lanes), answered on each.
@@ -3659,7 +3704,7 @@ template <int W, bool LIVE = false>
 __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __restrict__ tbl_s, const uint32_t pod,
                                            const uint32_t node, const uint32_t lane, const uint32_t gmask, const uint32_t gbase,
                                            const bool skip_first, uint32_t* row, const Lane* live = nullptr) {
-    PreSum s{DRA_PRE_NO, 0u, 0x80000000u, 0xFFFFFFFFu, 0ull};
+    PreSum s{DRA_PRE_NO, 0u, 0x80000000u, 0xFFFFFFFFu, 0ull, 0u};
     if (node >= a.n_node) return s;
     const uint32_t c0 = __ldg(&a.pod_off[pod]), cnt = __ldg(&a.pod_off[pod + 1]) - c0;
     if (cnt > DRA_MAX_POD) { s.st = DRA_PRE_INVALID; return s; }
@@ -3702,6 +3747,51 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
         if (st != 0) { s.st = st == DRA_ST_SEARCH_LIMIT ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO; return s; }
     }
     s.st = DRA_PRE_EVICT;
+    if constexpr (!LIVE) {
+        if (a.pdb) {
+            // Budgets: the reprieve over V's violating members first, then over the others, each phase in V order.
+            // keep(S, r): r re-applied to S; true, with S updated, if the pod still fits there.
+            auto keep = [&](Lane& S, const uint4 r) {
+                Lane Lk = S;
+                pre_apply(Lk, a, r, gidx, true);
+                Lt = Lk;
+                if (pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr) != 0) return false;
+                S = Lk;
+                return true;
+            };
+            auto victim = [&](const uint4 r, const bool vf) {           // victims come out of V order: true max / min
+                if (s.count == 0 || (int32_t)r.w > (int32_t)s.hi || (r.w == s.hi && r.y < s.hi_idx)) { s.hi = r.w; s.hi_idx = r.y; }
+                s.sum += (unsigned long long)((long long)(int32_t)r.w + 2147483648ll);
+                if (row && s.count < a.max_victims && lane == gbase) row[s.count] = r.y;
+                s.viol += vf ? 1u : 0u;
+                ++s.count;
+            };
+            if (!row) {                                              // the counts: both phases on L
+                for (uint32_t v = v0; v < v1; ++v) {
+                    const uint4 r = __ldcg(&a.vlist[v]);
+                    if (pre_violating(a, v0, v, r.y) && !keep(L, r)) victim(r, true);
+                }
+                for (uint32_t v = v0; v < v1; ++v) {
+                    const uint4 r = __ldcg(&a.vlist[v]);
+                    if (!pre_violating(a, v0, v, r.y) && !keep(L, r)) victim(r, false);
+                }
+            } else {
+                // The victims in V order: the violating phase once for its end state Lb, then V once with two states,
+                // L replaying the violating phase and Lb the other one, each member deciding on its own phase's state
+                Lane Lb = L;
+                for (uint32_t v = v0; v < v1; ++v) {
+                    const uint4 r = __ldcg(&a.vlist[v]);
+                    if (pre_violating(a, v0, v, r.y)) (void)keep(Lb, r);
+                }
+                for (uint32_t v = v0; v < v1; ++v) {
+                    const uint4 r = __ldcg(&a.vlist[v]);
+                    const bool vf = pre_violating(a, v0, v, r.y);
+                    if (!(vf ? keep(L, r) : keep(Lb, r))) victim(r, vf);
+                }
+            }
+            return s;
+        }
+    }
     for (uint32_t v = v0; v < v1; ++v) {                            // the reprieve, most important first
         const uint4 r = __ldcg(&a.vlist[v]);
         if constexpr (LIVE) { if (__shfl_sync(gmask, __ldcg(&row[r.y]), gbase) != DRA_GPU_NONE) continue; }
@@ -3748,26 +3838,28 @@ k_pods_preempt(const PreArgs a, const PreShard s) {
         }
         const PreSum r = pre_pair<W>(a, tbl_s, pod, node, lane, gmask, gbase, false, nullptr);
         if (lane == gbase) {
-            const uint32_t nv = r.st == DRA_PRE_EVICT ? r.count : 0u;
-            a.psum[pair] = make_uint4(r.st, r.count, r.hi, r.hi_idx);
+            const uint32_t nv = r.st == DRA_PRE_EVICT ? r.count : 0u;   // (r.viol is 0 unless EVICT)
+            a.psum[pair] = make_uint4(r.st | r.viol << PRE_VSHIFT, r.count, r.hi, r.hi_idx);
             a.psum64[pair] = r.sum;
             if (a.pair_status) a.pair_status[pair] = (uint8_t)r.st;
             if (a.pair_victims) a.pair_victims[pair] = nv;
-            if (s.pairs) s.pairs[pair] = make_uint2(r.st, nv);
+            if (a.pair_viol) a.pair_viol[pair] = r.viol;
+            if (s.pairs) s.pairs[pair] = make_uint2(r.st | r.viol << PRE_VSHIFT, nv);
         }
     }
 }
 
 // is EVICT pair x (summary xs, sum x64) preferred to y?  Equal summaries: neither (list position decides)
 __device__ __forceinline__ bool pre_better(const uint4 xs, const unsigned long long x64, const uint4 ys, const unsigned long long y64) {
+    if (xs.x >> PRE_VSHIFT != ys.x >> PRE_VSHIFT) return xs.x >> PRE_VSHIFT < ys.x >> PRE_VSHIFT;   // fewest violations
     if (xs.z != ys.z) return (int32_t)xs.z < (int32_t)ys.z;             // lowest highest victim priority
     if (x64 != y64) return x64 < y64;                                    // lowest sum of priorities
     if (xs.y != ys.y) return xs.y < ys.y;                                // fewest victims
     return xs.w > ys.w;                                                  // latest "start" among the highest-priority victims
 }
 
-// Warp-wide: every lane ends with the warp's preferred EVICT candidate (position best, NONE for none; summary bs; sum
-// b64), ties to the lower position.  bs.x, which pre_better does not read, travels with the candidate.
+// Warp-wide: every lane ends with the warp's preferred EVICT candidate (position best, NONE for none; summary bs, its
+// .x the violations << PRE_VSHIFT with any status bits; sum b64), ties to the lower position.
 __device__ __forceinline__ void pre_best_warp(uint32_t& best, uint4& bs, unsigned long long& b64) {
     for (uint32_t d = 16; d; d >>= 1) {
         const uint32_t ob = __shfl_xor_sync(FULLMASK, best, d);
@@ -3792,9 +3884,10 @@ __device__ __forceinline__ PreScan pre_scan(const PreArgs& a, const uint32_t k0,
     for (uint32_t j = k0 + lane; j < k1; j += 32) {                      // each lane in list order: ties keep the earlier
         if (win_nodes && __ldg(&win_nodes[j]) - lo >= n_win) continue;
         const uint4 s = __ldcg(&a.psum[j]);
-        if (s.x == DRA_PRE_FITS) r.fit = min(r.fit, j);
-        else if (s.x == DRA_PRE_SEARCH_LIMIT) r.lim = true;
-        else if (s.x == DRA_PRE_EVICT) {
+        const uint32_t st = s.x & PRE_ST_MASK;
+        if (st == DRA_PRE_FITS) r.fit = min(r.fit, j);
+        else if (st == DRA_PRE_SEARCH_LIMIT) r.lim = true;
+        else if (st == DRA_PRE_EVICT) {
             const unsigned long long v = __ldcg(&a.psum64[j]);
             if (r.best == DRA_GPU_NONE || pre_better(s, v, r.bs, r.b64)) { r.best = j; r.bs = s; r.b64 = v; }
         }
@@ -3838,6 +3931,7 @@ k_pre_choose(const PreArgs a) {
     a.pod_status[p] = (uint8_t)st;
     a.pod_node[p] = k == DRA_GPU_NONE ? DRA_GPU_NONE : dense ? k - k0 : __ldg(&a.cand_nodes[k]);
     a.n_victims[p] = st == DRA_PRE_EVICT ? bs.y : 0u;
+    if (a.pod_viol) a.pod_viol[p] = st == DRA_PRE_EVICT ? bs.x >> PRE_VSHIFT : 0u;
     a.choice[p] = st == DRA_PRE_EVICT ? k : DRA_GPU_NONE;
 }
 
@@ -4169,8 +4263,9 @@ k_spp_final(const SppArgs s) {
 //   k_spre_merge    flags, wait, then per pod the minimum over the ranks' partials; writes the caller's buffers only if
 //                   no rank reported a fault
 // The partials, in uint4 units: [0] header {fault word}; pod p at 1 + p * stride: {fit position, best EVICT position,
-// its victim count, its highest victim priority}, {index of its first victim, SEARCH_LIMIT seen, its priority sum lo,
-// hi}, then the best pair's row of max_victims words; after the pods the window's pairs as {status, victims} (uint2).
+// its victim count, its highest victim priority}, {its lowest victim index of that priority, SEARCH_LIMIT seen | its
+// violations << 1, its priority sum lo, hi}, then the best pair's row of max_victims words; after the pods the window's
+// pairs as {status | violations << PRE_VSHIFT, victims} (uint2).
 // A position is the pair's index in the call's pair list, so the merge's choice is the minimum over the ranks of a total
 // order — (FITS first, then pre_better, then position) — which is the single-inventory choice for any partition.
 // k_pods_preempt also judges a candidate naming no node (NO); the reduce leaves it out and the merge writes it itself.
@@ -4190,7 +4285,7 @@ k_spre_reduce(const PreArgs a, const PreShard s) {
     if (r.fit != DRA_GPU_NONE) r.best = DRA_GPU_NONE;                    // a FITS pair anywhere beats every EVICT pair
     uint4* q = s.part + 1 + (size_t)p * s.stride;
     q[0] = make_uint4(r.fit, r.best, r.bs.y, r.bs.z);
-    q[1] = make_uint4(r.bs.w, r.lim ? 1u : 0u, (uint32_t)r.b64, (uint32_t)(r.b64 >> 32));
+    q[1] = make_uint4(r.bs.w, (r.lim ? 1u : 0u) | (r.bs.x >> PRE_VSHIFT) << 1, (uint32_t)r.b64, (uint32_t)(r.b64 >> 32));
 }
 
 struct PreMerge {
@@ -4205,6 +4300,7 @@ struct PreMerge {
     const uint32_t* gate;            // this rank's fault word
     uint8_t* pair_status; uint32_t* pair_victims;                  // the caller's (pair outputs: nullptr unless asked)
     uint32_t* pod_node; uint8_t* pod_status; uint32_t* n_victims; uint32_t* victims;
+    uint32_t* pair_viol; uint32_t* pod_viol;                        // the caller's violation outputs (nullptr: none)
 };
 
 // The start of a merge that waits for its peers (k_spre_merge, k_scap_merge): block 0 raises this rank's flags, every
@@ -4254,23 +4350,26 @@ k_spre_merge(const PeerExchange x, const PreMerge m) {
             A = __ldcg(&src[0]); B = __ldcg(&src[1]);
         }
         const uint32_t fit = __reduce_min_sync(FULLMASK, A.x);
-        const bool lim = __any_sync(FULLMASK, B.y != 0u);
+        const bool lim = __any_sync(FULLMASK, (B.y & 1u) != 0u);
         uint32_t best = A.y;
-        uint4 bs = make_uint4(lane, A.z, A.w, B.x);                     // .x: the rank whose partial holds the candidate
+        uint4 bs = make_uint4((B.y >> 1) << PRE_VSHIFT, A.z, A.w, B.x);
         unsigned long long b64 = (unsigned long long)B.z | ((unsigned long long)B.w << 32);
         pre_best_warp(best, bs, b64);
-        const uint32_t win = bs.x;
         const uint32_t c0 = __ldg(&m.pod_off[p]), cnt = __ldg(&m.pod_off[p + 1]) - c0;
         const bool inv = pod_invalid<32>(m.claims + c0, cnt, m.sel.n_sel, true, lane, FULLMASK);
         uint32_t k;
         const uint32_t st = pre_decide(fit, best, lim, inv, k);
         const uint32_t nv = st == DRA_PRE_EVICT ? bs.y : 0u;
+        const uint32_t node = k == DRA_GPU_NONE ? DRA_GPU_NONE : dense ? k - p * m.n_node : __ldg(&m.cand_nodes[k]);
         if (lane == 0) {
             m.pod_status[p] = (uint8_t)st;
-            m.pod_node[p] = k == DRA_GPU_NONE ? DRA_GPU_NONE : dense ? k - p * m.n_node : __ldg(&m.cand_nodes[k]);
+            m.pod_node[p] = node;
             m.n_victims[p] = nv;
+            if (m.pod_viol) m.pod_viol[p] = st == DRA_PRE_EVICT ? bs.x >> PRE_VSHIFT : 0u;
         }
         if (m.max_victims) {
+            // the chosen EVICT pair's partial is its node's owner's (no row is read for any other status)
+            const uint32_t win = st == DRA_PRE_EVICT ? node_owner(m.bounds, world, node) : rank;
             const uint32_t* row = reinterpret_cast<const uint32_t*>(
                 (win == rank ? m.part : x.my_stage + (size_t)win * m.slice4) + 1 + (size_t)p * m.stride + 2);
             const uint32_t n = min(nv, m.max_victims);
@@ -4278,7 +4377,7 @@ k_spre_merge(const PeerExchange x, const PreMerge m) {
                 m.victims[(size_t)p * m.max_victims + j] = j < n ? __ldcg(&row[j]) : DRA_GPU_NONE;
         }
     }
-    if (!m.pair_status && !m.pair_victims) return;
+    if (!m.pair_status && !m.pair_victims && !m.pair_viol) return;
     const size_t pair4 = 1 + (size_t)m.n_pod * m.stride;                 // a slice's pair results follow its partials
     for (uint32_t k = blockIdx.x * blockDim.x + tid; k < m.n_pair; k += gridDim.x * blockDim.x) {
         const uint32_t node = dense ? k % m.n_node : __ldg(&m.cand_nodes[k]);
@@ -4288,8 +4387,9 @@ k_spre_merge(const PeerExchange x, const PreMerge m) {
             const uint2* src = r == rank ? m.pairs : reinterpret_cast<const uint2*>(x.my_stage + (size_t)r * m.slice4 + pair4);
             v = __ldcg(&src[k]);
         }
-        if (m.pair_status) m.pair_status[k] = (uint8_t)v.x;
+        if (m.pair_status) m.pair_status[k] = (uint8_t)(v.x & PRE_ST_MASK);
         if (m.pair_victims) m.pair_victims[k] = v.y;
+        if (m.pair_viol) m.pair_viol[k] = v.x >> PRE_VSHIFT;
     }
 }
 
