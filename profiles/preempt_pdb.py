@@ -4,7 +4,7 @@ calls on the same seeded problem, timed alternately in one loop:
   dra_preempt_batch                     the budget-free call
   dra_preempt_pdb_batch, no budgets     NULL budgets: must cost what the budget-free call costs
   dra_preempt_pdb_batch, budgets        8 budgets over the running pods (1 in 4 pods in none), allowed 0..3
-Each output is first checked byte for byte against the CPU oracle (tests/preempt_pdb_oracle.c).  Times are medians (min, max)
+Each output is first checked byte for byte against the CPU oracle (tests/pod_oracles.c).  Times are medians (min, max)
 of CUDA events around the host-buffer call.  Prints the card and its power limit."""
 import importlib
 import os
@@ -20,7 +20,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))                # the CPU oracle of spec §14 (test infrastructure)
 pkg = importlib.import_module("k8s-dra-driver_b200")
 import preempt_oracle as P  # noqa: E402
-import preempt_pdb_oracle as PB  # noqa: E402
+import preempt_oracle as PB  # noqa: E402
 
 A, S, R = pkg.api, pkg.synth, pkg.records
 REPS = int(os.environ.get("PREEMPT_REPS", "10"))

@@ -1,66 +1,19 @@
 """ctypes wrapper of the CPU oracle of spec §16 (pod capacity) — TEST INFRASTRUCTURE ONLY.
 
-tests/capacity_oracle.c counts the copies of each pod a candidate node takes with the §12 evaluation of
-oracle/dra_oracle.c (which it includes); it is compiled on first use into a cache file in the temporary directory, named
-by a hash of its sources, so a read-only tree works too.  `capacity_naive` below is the independent restatement on top of
-oracle/naive.py's `eval_pod`: the two share no code, and the CPU suite checks one against the other."""
+pod_oracle_capacity (tests/pod_oracles.c, loaded by tests/pod_oracles.py) counts the copies of each pod a candidate
+node takes with the §12 evaluation of oracle/dra_oracle.c.  `capacity_naive` below is the independent restatement on
+top of oracle/naive.py's `eval_pod`: the two share no code, and the CPU suite checks one against the other."""
 from __future__ import annotations
 
 import copy
-import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 from oracle import oracle as O
+from pod_oracles import _nz, _p, lib, set_selectors  # noqa: F401  (set_selectors: the selectors of every pod oracle)
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_SRCS = [os.path.join(_HERE, "capacity_oracle.c"), os.path.join(_ROOT, "oracle", "dra_oracle.c"),
-         os.path.join(_ROOT, "oracle", "dra_oracle.h"), os.path.join(_ROOT, "include", "dra_alloc.h")]
 F_EXHAUSTIVE = O.F_EXHAUSTIVE
 ST_OK, ST_INVALID, ST_POD, ST_SEARCH_LIMIT = 0, 5, 6, 7
-
-_lib = None
-
-
-def build() -> str:
-    h = hashlib.sha256()
-    for s in _SRCS:
-        with open(s, "rb") as f:
-            h.update(f.read())
-    so = os.path.join(tempfile.gettempdir(), f"dra_capacity_oracle_{os.getuid()}_{h.hexdigest()[:16]}.so")
-    if not os.path.exists(so):
-        tmp = f"{so}.{os.getpid()}.tmp"
-        subprocess.run([os.environ.get("CC", "gcc"), "-O2", "-std=c11", "-Wall", "-fPIC", "-pthread", "-shared",
-                        "-fvisibility=hidden", "-o", tmp, _SRCS[0]], check=True)
-        os.replace(tmp, so)
-    return so
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        _lib = C.CDLL(build())
-        vp, u32 = C.c_void_p, C.c_uint32
-        _lib.capacity_oracle_capacity.argtypes = [vp, u32, vp, u32, vp, vp, u32, vp, u32, vp, vp, u32, vp, vp, vp, vp, u32]
-        _lib.capacity_oracle_capacity.restype = C.c_int
-        _lib.capacity_oracle_set_selectors.argtypes = [vp, u32, vp, u32]
-        _lib.capacity_oracle_set_selectors.restype = None
-    return _lib
-
-
-def _p(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
-
-
-def _nz(a, dtype):
-    """an array that is never NULL (NULL means something else to the callee)"""
-    a = np.ascontiguousarray(a if a is not None else [], dtype=dtype)
-    return a if len(a) else np.zeros(1, dtype)
 
 
 def capacity(gpus, node_off, table, claims, pod_off, cand_nodes=None, cand_off=None, max_copies: int = 64, flags: int = 0):
@@ -83,26 +36,11 @@ def capacity(gpus, node_off, table, claims, pod_off, cand_nodes=None, cand_off=N
     stop = np.zeros(max(n_pair, 1), np.uint8)
     total = np.zeros(max(n_pod, 1), np.uint64)
     nodes = np.zeros(max(n_pod, 1), np.uint32)
-    rc = lib().capacity_oracle_capacity(_p(g), len(g), _p(off), n_node, _p(t), _p(c), n_claim, _p(po), n_pod, _p(cn), _p(co),
-                                        max_copies, _p(copies), _p(stop), _p(total), _p(nodes), flags)
+    rc = lib().pod_oracle_capacity(_p(g), len(g), _p(off), n_node, _p(t), _p(c), n_claim, _p(po), n_pod, _p(cn), _p(co),
+                                   max_copies, _p(copies), _p(stop), _p(total), _p(nodes), flags)
     if rc != 0:
-        raise ValueError(f"capacity_oracle_capacity: rc={rc}")
+        raise ValueError(f"pod_oracle_capacity: rc={rc}")
     return copies[:n_pair], stop[:n_pair], total[:n_pod], nodes[:n_pod]
-
-
-_sel_keep = []
-
-
-def set_selectors(attrs=None, sels=None):
-    """Selector context for the following calls (spec §10); call with no arguments to clear."""
-    _sel_keep.clear()
-    if sels is None or len(sels) == 0:
-        lib().capacity_oracle_set_selectors(None, 0, None, 0)
-        return
-    a = np.ascontiguousarray(attrs) if attrs is not None else np.zeros(0, dtype=np.uint8)
-    s_ = np.ascontiguousarray(sels).reshape(-1, 8)
-    _sel_keep.extend([a, s_])                          # the C side keeps the pointers
-    lib().capacity_oracle_set_selectors(_p(a) if len(a) else None, len(a), _p(s_), len(s_))
 
 
 def capacity_naive(gpus, node_off, table, claims, pod_off, cands, exhaustive, max_copies: int = 64):

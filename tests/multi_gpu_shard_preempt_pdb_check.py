@@ -17,7 +17,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 pkg = importlib.import_module("k8s-dra-driver_b200")
 import preempt_oracle as P
-import preempt_pdb_oracle as PB
+import preempt_oracle as PB
 R = pkg.records
 F_EXH = pkg.api.F_EXHAUSTIVE
 

@@ -1,59 +1,18 @@
 """ctypes wrapper of the CPU oracle of spec §13 (place pods) — TEST INFRASTRUCTURE ONLY.
 
-tests/place_oracle.c walks the candidates of each pod and evaluates the pod with the §12 evaluation of
-oracle/dra_oracle.c (which it includes); it is compiled on first use into a cache file in the temporary directory,
-named by a hash of its sources, so a read-only tree works too.  `place_pods_naive` below is the independent restatement
-on top of oracle/naive.py's `eval_pod`: the two share no code, and the CPU suite checks one against the other."""
+pod_oracle_place_pods (tests/pod_oracles.c, loaded by tests/pod_oracles.py) walks the candidates of each pod and
+evaluates the pod with the §12 evaluation of oracle/dra_oracle.c.  `place_pods_naive` below is the independent
+restatement on top of oracle/naive.py's `eval_pod`: the two share no code, and the CPU suite checks one against the
+other."""
 from __future__ import annotations
-
-import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 from oracle import oracle as O
+from pod_oracles import _p, lib, set_selectors  # noqa: F401  (set_selectors: the selectors of every pod oracle)
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_SRCS = [os.path.join(_HERE, "place_oracle.c"), os.path.join(_ROOT, "oracle", "dra_oracle.c"),
-         os.path.join(_ROOT, "oracle", "dra_oracle.h"), os.path.join(_ROOT, "include", "dra_alloc.h")]
 NONE = 0xFFFFFFFF
 F_EXHAUSTIVE = O.F_EXHAUSTIVE
-
-_lib = None
-
-
-def build() -> str:
-    h = hashlib.sha256()
-    for s in _SRCS:
-        with open(s, "rb") as f:
-            h.update(f.read())
-    so = os.path.join(tempfile.gettempdir(), f"dra_place_oracle_{os.getuid()}_{h.hexdigest()[:16]}.so")
-    if not os.path.exists(so):
-        tmp = f"{so}.{os.getpid()}.tmp"
-        subprocess.run([os.environ.get("CC", "gcc"), "-O2", "-std=c11", "-Wall", "-fPIC", "-pthread", "-shared",
-                        "-fvisibility=hidden", "-o", tmp, _SRCS[0]], check=True)
-        os.replace(tmp, so)
-    return so
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        _lib = C.CDLL(build())
-        vp, u32 = C.c_void_p, C.c_uint32
-        _lib.place_oracle_place_pods.argtypes = [vp, u32, vp, u32, vp, vp, u32, vp, u32, vp, vp, vp, vp, u32, vp, u32]
-        _lib.place_oracle_place_pods.restype = C.c_int
-        _lib.place_oracle_set_selectors.argtypes = [vp, u32, vp, u32]
-        _lib.place_oracle_set_selectors.restype = None
-    return _lib
-
-
-def _p(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
 def place_pods(gpus, node_off, table, claims, pod_off, cand_nodes=None, cand_off=None, out_off=None, n_out=None,
@@ -74,26 +33,11 @@ def place_pods(gpus, node_off, table, claims, pod_off, cand_nodes=None, cand_off
         n_out = len(c) if oo is None else 0
     out = np.zeros(max(n_out, 1), dtype=O.OUT_DTYPE)
     pod_node = np.zeros(max(len(po) - 1, 1), dtype=np.uint32)
-    rc = lib().place_oracle_place_pods(_p(g), len(g), _p(off), len(off) - 1, _p(t), _p(c), len(c), _p(po), len(po) - 1,
-                                       _p(cn), _p(co), _p(oo), _p(out), n_out, _p(pod_node), flags)
+    rc = lib().pod_oracle_place_pods(_p(g), len(g), _p(off), len(off) - 1, _p(t), _p(c), len(c), _p(po), len(po) - 1,
+                                     _p(cn), _p(co), _p(oo), _p(out), n_out, _p(pod_node), flags)
     if rc != 0:
-        raise ValueError(f"place_oracle_place_pods: rc={rc}")
+        raise ValueError(f"pod_oracle_place_pods: rc={rc}")
     return out[:n_out], pod_node[:len(po) - 1], g
-
-
-_sel_keep = []
-
-
-def set_selectors(attrs=None, sels=None):
-    """Selector context for the following calls (spec §10); call with no arguments to clear."""
-    _sel_keep.clear()
-    if sels is None or len(sels) == 0:
-        lib().place_oracle_set_selectors(None, 0, None, 0)
-        return
-    a = np.ascontiguousarray(attrs) if attrs is not None else np.zeros(0, dtype=np.uint8)
-    s_ = np.ascontiguousarray(sels).reshape(-1, 8)
-    _sel_keep.extend([a, s_])                          # the C side keeps the pointers
-    lib().place_oracle_set_selectors(_p(a) if len(a) else None, len(a), _p(s_), len(s_))
 
 
 def place_pods_naive(gpus, node_off, table, claims, pod_off, cands, exhaustive, out_off=None):

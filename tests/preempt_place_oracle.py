@@ -1,71 +1,20 @@
 """ctypes wrapper of the CPU oracle of spec §15 (preempt and place) — TEST INFRASTRUCTURE ONLY.
 
-tests/preempt_place_oracle.c runs the sequential schedule on tests/preempt_oracle.c's pair judgement and oracle/dra_oracle.c's
-pod evaluation (which it includes); it is compiled on first use into a cache file in the temporary directory, named by
-a hash of its sources, so a read-only tree works too.  `preempt_place_naive` below is the independent restatement: the
-host loop itself, per pod preempt_oracle.preempt_naive with that one pod against the running pods not evicted yet, §9 for
-its victims and oracle/naive.py's `eval_pod` on the chosen node.  The two share no code, and the CPU suite checks one
-against the other."""
+pod_oracle_preempt_place (tests/pod_oracles.c, loaded by tests/pod_oracles.py) runs the sequential schedule on the §14
+pair judgement without budgets and oracle/dra_oracle.c's pod evaluation.  `preempt_place_naive` below is the
+independent restatement: the host loop itself, per pod preempt_oracle.preempt_naive with that one pod against the
+running pods not evicted yet, §9 for its victims and oracle/naive.py's `eval_pod` on the chosen node.  The two share no
+code, and the CPU suite checks one against the other."""
 from __future__ import annotations
-
-import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 from oracle import oracle as O
+from pod_oracles import _nz, _p, lib, set_selectors  # noqa: F401  (set_selectors: the selectors of every pod oracle)
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
-_SRCS = [os.path.join(_HERE, "preempt_place_oracle.c"), os.path.join(_HERE, "preempt_oracle.c"),
-         os.path.join(_ROOT, "oracle", "dra_oracle.c"), os.path.join(_ROOT, "oracle", "dra_oracle.h"),
-         os.path.join(_ROOT, "include", "dra_alloc.h")]
 NONE = 0xFFFFFFFF
 F_EXHAUSTIVE = O.F_EXHAUSTIVE
 FITS, EVICT, NO, SEARCH_LIMIT, INVALID = 0, 1, 2, 3, 4
-
-_lib = None
-
-
-def build() -> str:
-    h = hashlib.sha256()
-    for s in _SRCS:
-        with open(s, "rb") as f:
-            h.update(f.read())
-    so = os.path.join(tempfile.gettempdir(), f"dra_preempt_place_oracle_{os.getuid()}_{h.hexdigest()[:16]}.so")
-    if not os.path.exists(so):
-        tmp = f"{so}.{os.getpid()}.tmp"
-        subprocess.run([os.environ.get("CC", "gcc"), "-O2", "-std=c11", "-Wall", "-fPIC", "-pthread", "-shared",
-                        "-fvisibility=hidden", "-o", tmp, _SRCS[0]], check=True)
-        os.replace(tmp, so)
-    return so
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        _lib = C.CDLL(build())
-        vp, u32 = C.c_void_p, C.c_uint32
-        _lib.pp_oracle_preempt_place.argtypes = [vp, u32, vp, u32, vp, vp, u32, vp, vp, u32, vp, vp,
-                                                 vp, u32, vp, vp, u32, vp, vp, u32,
-                                                 vp, vp, u32, vp, vp, vp, u32]
-        _lib.pp_oracle_preempt_place.restype = C.c_int
-        _lib.pp_oracle_set_selectors.argtypes = [vp, u32, vp, u32]
-        _lib.pp_oracle_set_selectors.restype = None
-    return _lib
-
-
-def _p(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
-
-
-def _nz(a, dtype):
-    """an array that is never NULL (NULL means something else to the callee)"""
-    a = np.ascontiguousarray(a if a is not None else [], dtype=dtype)
-    return a if len(a) else np.zeros(1, dtype)
 
 
 def pending_slots(claims, out_off=None):
@@ -118,28 +67,14 @@ def preempt_place(gpus, node_off, table, claims, pod_off, prio, run_claims, run_
     else:
         out, pnode, pstat, ev = (filled(n_out, O.OUT_DTYPE), filled(n_pod, np.uint32), filled(n_pod, np.uint8),
                                  filled(n_run, np.uint32))
-    rc = lib().pp_oracle_preempt_place(_p(g), len(g), _p(off), len(off) - 1, _p(t), _p(c), n_claim, _p(po), _p(pr), n_pod,
-                                       _p(cn), _p(co), _p(rc_), len(run_claims) if run_claims is not None else 0, _p(rpo),
-                                       _p(rpr), n_run, _p(roo), _p(ro), n_rout, _p(oo), _p(out), n_out, _p(pnode),
-                                       _p(pstat), _p(ev), flags)
+    rc = lib().pod_oracle_preempt_place(_p(g), len(g), _p(off), len(off) - 1, _p(t), _p(c), n_claim, _p(po), _p(pr),
+                                        n_pod, _p(cn), _p(co), _p(rc_),
+                                        len(run_claims) if run_claims is not None else 0, _p(rpo), _p(rpr), n_run,
+                                        _p(roo), _p(ro), n_rout, _p(oo), _p(out), n_out, _p(pnode), _p(pstat), _p(ev),
+                                        flags)
     if rc != 0:
-        raise ValueError(f"pp_oracle_preempt_place: rc={rc}")
+        raise ValueError(f"pod_oracle_preempt_place: rc={rc}")
     return out[:n_out], pnode[:n_pod], pstat[:n_pod], ev[:n_run], g
-
-
-_sel_keep = []
-
-
-def set_selectors(attrs=None, sels=None):
-    """Selector context for the following calls (spec §10); call with no arguments to clear."""
-    _sel_keep.clear()
-    if sels is None or len(sels) == 0:
-        lib().pp_oracle_set_selectors(None, 0, None, 0)
-        return
-    a = np.ascontiguousarray(attrs) if attrs is not None else np.zeros(0, dtype=np.uint8)
-    s_ = np.ascontiguousarray(sels).reshape(-1, 8)
-    _sel_keep.extend([a, s_])                          # the C side keeps the pointers
-    lib().pp_oracle_set_selectors(_p(a) if len(a) else None, len(a), _p(s_), len(s_))
 
 
 def preempt_place_naive(gpus, node_off, table, claims, pod_off, prio, cands, exhaustive, run_claims, run_pod_off,

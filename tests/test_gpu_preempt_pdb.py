@@ -1,5 +1,5 @@
 """GPU suite: preemption with disruption budgets on one inventory (dra_preempt_pdb_batch, spec §14 "Disruption budgets").
-Every call's eight outputs are compared byte for byte with preempt_pdb_oracle.preempt_pdb on the context's live inventory:
+Every call's eight outputs are compared byte for byte with preempt_oracle.preempt_pdb on the context's live inventory:
 random problems at every lane width the pair kernel instantiates, with and without DRA_F_EXHAUSTIVE, with selectors,
 victim rows shorter than the victim count, and running records that do not match the inventory.  With no budgets the
 call is dra_preempt_batch, kernel chain included; a bad budget index fails with nothing written."""
@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 import preempt_oracle as P
-import preempt_pdb_oracle as PB
+import preempt_oracle as PB
 from preempt_problems import I32_MAX, I32_MIN, random_problem
 
 pytestmark = pytest.mark.gpu

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 import preempt_oracle as P
-import preempt_pdb_oracle as PB
+import preempt_oracle as PB
 from test_gpu_preempt_pdb import NAMES, budgets
 from test_gpu_shard_preempt import World, _cands, _dev, _nn, _running
 from test_gpu_shard_unsuitable import _bounds

@@ -1,8 +1,9 @@
 """CPU suite: spec §13 — place a batch of pods on the first candidate node each one fits, given what the pods before it
 took (the batched form of the classic controller's pending allocations, SURVEY App. A).
 
-The C oracle (tests/place_oracle.c, on oracle/dra_oracle.c's pod evaluation) and the pure-Python restatement
-(place_oracle.place_pods_naive, on oracle/naive.py's) share no code, so agreement between them pins the sequential rule."""
+The C oracle (pod_oracle_place_pods in tests/pod_oracles.c, on oracle/dra_oracle.c's pod evaluation) and the pure-Python
+restatement (place_oracle.place_pods_naive, on oracle/naive.py's) share no code, so agreement between them pins the
+sequential rule."""
 import numpy as np
 from hypothesis import HealthCheck, given, settings
 from hypothesis import strategies as st

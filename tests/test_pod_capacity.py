@@ -1,9 +1,9 @@
 """CPU suite: spec §16 — pod capacity: how many copies of a pod each candidate node still takes, counted as the pods
 Allocate (§12) would place them.
 
-The C oracle (tests/capacity_oracle.c, on oracle/dra_oracle.c's pod evaluation) and the pure-Python restatement
-(capacity_oracle.capacity_naive, on oracle/naive.py's) share no code, so agreement between them pins the rule; the two
-consequences §16 states tie it to the pods Allocate and to the exhaustive UnsuitableNodes."""
+The C oracle (pod_oracle_capacity in tests/pod_oracles.c, on oracle/dra_oracle.c's pod evaluation) and the pure-Python
+restatement (capacity_oracle.capacity_naive, on oracle/naive.py's) share no code, so agreement between them pins the
+rule; the two consequences §16 states tie it to the pods Allocate and to the exhaustive UnsuitableNodes."""
 import importlib
 import json
 import os

@@ -1,8 +1,9 @@
 """CPU suite: spec §14 — preemption: for a pod that fits nowhere, the lower-priority running pods to evict on each
 candidate node, and the node to evict them on (kube-scheduler's DefaultPreemption without PodDisruptionBudgets).
 
-The C oracle (tests/preempt_oracle.c, on oracle/dra_oracle.c's pod evaluation) and the pure-Python restatement
-(preempt_oracle.preempt_naive, on oracle/naive.py's) share no code, so agreement between them pins the rule."""
+The C oracle (pod_oracle_preempt in tests/pod_oracles.c, on oracle/dra_oracle.c's pod evaluation) and the pure-Python
+restatement (preempt_oracle.preempt_naive, on oracle/naive.py's) share no code, so agreement between them pins the
+rule."""
 import importlib
 
 import numpy as np
@@ -223,10 +224,11 @@ def test_call_errors():
     # max_victims > 0 without a victims buffer
     out = [np.zeros(4, np.uint32) for _ in range(5)]
     prio = np.array([1], np.int32)
-    assert P.lib().preempt_oracle_preempt(P._p(g), len(g), P._p(off), len(off) - 1, P._p(t), P._p(ok["c"]), 1,
-                                          P._p(ok["po"]), P._p(prio), 1, None, None, P._p(ok["rc"]), 2, P._p(ok["rpo"]),
-                                          P._p(ok["rpr"]), 2, None, P._p(ok["ro"]), 2, P._p(out[0]), P._p(out[1]),
-                                          P._p(out[2]), P._p(out[3]), P._p(out[4]), None, 3, 0) == -1
+    assert P.lib().pod_oracle_preempt(P._p(g), len(g), P._p(off), len(off) - 1, P._p(t), P._p(ok["c"]), 1,
+                                      P._p(ok["po"]), P._p(prio), 1, None, None, P._p(ok["rc"]), 2, P._p(ok["rpo"]),
+                                      P._p(ok["rpr"]), 2, None, P._p(ok["ro"]), 2, None, None, 0, P._p(out[0]),
+                                      P._p(out[1]), None, P._p(out[2]), P._p(out[3]), P._p(out[4]), None, None, 3,
+                                      0) == -1
 
 
 def test_dense_form_over_two_to_the_32_pairs():

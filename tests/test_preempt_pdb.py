@@ -1,9 +1,9 @@
 """CPU suite: spec §14 with disruption budgets — V's members whose eviction would take their budget below zero are
 reprieved first, and the pod's EVICT pair is the one with the fewest such victims before any other key.
 
-The C oracle (tests/preempt_pdb_oracle.c, budgets in the "members of V up to v" form) and the naive restatement
-(preempt_pdb_oracle.preempt_naive_pdb, kube-scheduler's decrement-then-below-zero loop) share no code, so agreement between
-them pins the rule."""
+The C oracle (pod_oracle_preempt in tests/pod_oracles.c, budgets in the "members of V up to v" form) and the naive
+restatement (preempt_oracle.preempt_naive_pdb, kube-scheduler's decrement-then-below-zero loop) share no code, so
+agreement between them pins the rule."""
 import importlib
 
 import numpy as np
@@ -17,7 +17,7 @@ from test_pod_mode import _mig, _tbl
 from test_preempt import _flat, _outs, _small_world, mig_running, occupied
 
 import preempt_oracle as P
-import preempt_pdb_oracle as PB
+import preempt_oracle as PB
 
 R = importlib.import_module("k8s-dra-driver_b200").records
 NONE = 0xFFFFFFFF

@@ -1,7 +1,7 @@
 """CPU suite: the partition-and-merge of the sharded preemption call with disruption budgets, modelled in Python as
 test_preempt_shard_model.py models it without them.
 
-Each (pod, candidate) pair is judged alone (preempt_pdb_oracle.preempt_naive_pdb with one pod and one candidate: every pair
+Each (pod, candidate) pair is judged alone (preempt_oracle.preempt_naive_pdb with one pod and one candidate: every pair
 copies the budgets afresh) by the rank that owns the candidate's node.  Each rank keeps per pod its first FITS position
 and its best EVICT pair under the order with the fewest violations first, then the list position; the merge takes the
 minimum over the ranks.  For every partition, worlds 1 to 5, the answer must be the single-inventory one of both
@@ -16,7 +16,7 @@ from test_preempt_shard_model import _partitions
 
 import importlib
 import preempt_oracle as P
-import preempt_pdb_oracle as PB
+import preempt_oracle as PB
 from oracle import naive as N
 
 R = importlib.import_module("k8s-dra-driver_b200").records

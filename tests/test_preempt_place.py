@@ -1,8 +1,8 @@
 """CPU suite: spec §15 — preempt and place: the pods of a batch in input order, each judged as §14 judges it on the
 inventory the pods before it left (their placements held, their victims gone), then applied.
 
-The C oracle (tests/preempt_place_oracle.c, on tests/preempt_oracle.c's pair judgement and oracle/dra_oracle.c's pod
-evaluation) and the Python restatement (preempt_place_oracle.preempt_place_naive: the host loop over
+The C oracle (pod_oracle_preempt_place in tests/pod_oracles.c, on its §14 pair judgement and oracle/dra_oracle.c's
+pod evaluation) and the Python restatement (preempt_place_oracle.preempt_place_naive: the host loop over
 preempt_oracle.preempt_naive, §9 and oracle/naive.py's eval_pod) share no code, so agreement between them pins the rule."""
 import importlib
 
