@@ -7,23 +7,15 @@ fused kernel + packet-gather tail, sort path + gather kernel, ncclAllGather, and
 
   python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 tests/multi_gpu_check.py
 """
-import importlib, os, sys
 import numpy as np
 import torch
 import torch.distributed as dist
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-pkg = importlib.import_module("k8s-dra-driver_b200")
+from multi_gpu_rank import finish, pkg, report, start
 from oracle import oracle as O
 R = pkg.records
 
-rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-os.environ.setdefault("NCCL_DEBUG", "WARN")
-torch.cuda.set_device(local)
-dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", local))
-dev = torch.device("cuda", local)
-stream = torch.cuda.Stream(device=dev); torch.cuda.set_stream(stream)
-fails = 0
+rank, world, dev, stream = start()
 for name, w, ctx_flags, use_peer in [
         ("fused+peer, mixed with counts/groups/invalid", pkg.synth.mixed(9000, 97, 21), 0, True),
         ("sort path+peer push/wait", pkg.synth.mixed(9000, 97, 22), pkg.api.CFG_NO_FUSED, True),
@@ -33,7 +25,7 @@ for name, w, ctx_flags, use_peer in [
     lbs = [pkg.shard.local_batch(w.gpus, w.node_off, w.claims, r, ranges) for r in range(world)]
     lb = lbs[rank]
     n_per = max(b.n_out for b in lbs); n_per += n_per & 1
-    ctx = pkg.api.Context(device=local, stream=stream.cuda_stream, flags=ctx_flags)
+    ctx = pkg.api.Context(device=dev.index, stream=stream.cuda_stream, flags=ctx_flags)
     ctx.set_table(w.table); ctx.set_inventory(lb.gpus, lb.node_off)
     uid = [pkg.api.Context.comm_unique_id() if rank == 0 else None]      # one NCCL unique id per communicator
     dist.broadcast_object_list(uid, src=0)
@@ -52,10 +44,7 @@ for name, w, ctx_flags, use_peer in [
         parts = [(b.sel, b.out_off, table[r * n_per: r * n_per + b.n_out], b.gpu_base) for r, b in enumerate(lbs)]
         merged = pkg.shard.merge(w.n_out, w.out_off if w.out_off is not None else np.arange(w.n_claim, dtype=np.uint32), parts)
         ref, _ = O.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out)
-        ok = merged.tobytes() == ref.tobytes()
-        fails += not ok
-        if rank == 0:
-            print(f"{name} rep {rep}: {'OK' if ok else 'MISMATCH'} ({w.n_claim} claims, {world} ranks)")
+        report(f"{name} rep {rep}", merged.tobytes() == ref.tobytes(), f"{w.n_claim} claims, {world} ranks")
     ctx.close()
 # ---- the sharded GLOBAL batch: the same claim array on every rank, device-side range filter, global slots ----
 for name, w, ctx_flags in [("global batch, fused, mixed", pkg.synth.mixed(9000, 97, 31), 0),
@@ -64,7 +53,7 @@ for name, w, ctx_flags in [("global batch, fused, mixed", pkg.synth.mixed(9000, 
                            # large: every shard goes through wave-sized hist tiles, the row-wise scan and the stand-alone gather
                            ("global batch, 1M claims x 10k nodes", pkg.synth.cfg2(1_000_000, 10_000), 0)]:
     ranges = pkg.shard.plan(w.claims["node"], w.n_node, world)
-    ctx = pkg.api.Context(device=local, stream=stream.cuda_stream, flags=ctx_flags)
+    ctx = pkg.api.Context(device=dev.index, stream=stream.cuda_stream, flags=ctx_flags)
     ctx.set_table(w.table); ctx.set_inventory(w.gpus, w.node_off)
     uid = [pkg.api.Context.comm_unique_id() if rank == 0 else None]
     dist.broadcast_object_list(uid, src=0)
@@ -81,14 +70,8 @@ for name, w, ctx_flags in [("global batch, fused, mixed", pkg.synth.mixed(9000, 
         ctx.allocate_global_device(d_claims.data_ptr(), w.n_claim, None if d_off is None else d_off.data_ptr(), w.n_out, pkg.api.F_FRESH_INVENTORY)
         table = ctx.gather_read(np.zeros(w.n_out, dtype=R.OUT_DTYPE))
         g0, g1 = int(w.node_off[ranges[rank][0]]), int(w.node_off[ranges[rank][1]])
-        ok = table.tobytes() == ref.tobytes() and ctx.get_inventory()[g0:g1].tobytes() == ref_inv[g0:g1].tobytes()
-        fails += not ok
-        if rank == 0:
-            print(f"{name} rep {rep}: {'OK' if ok else 'MISMATCH'} ({w.n_claim} claims, {world} ranks)")
+        report(f"{name} rep {rep}", table.tobytes() == ref.tobytes()
+               and ctx.get_inventory()[g0:g1].tobytes() == ref_inv[g0:g1].tobytes(), f"{w.n_claim} claims, {world} ranks")
     dist.barrier()
     ctx.close()
-t = torch.tensor([fails], device=dev); dist.all_reduce(t)
-if rank == 0:
-    print("ALL OK" if int(t.item()) == 0 else f"{int(t.item())} FAILURES")
-dist.destroy_process_group()
-sys.exit(1 if int(t.item()) else 0)
+finish()

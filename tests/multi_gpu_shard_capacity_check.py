@@ -7,25 +7,14 @@ the real world, and no rank's inventory may change.
 
   python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tests/multi_gpu_shard_capacity_check.py
 """
-import importlib, os, sys
 import numpy as np
 import torch
-import torch.distributed as dist
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-pkg = importlib.import_module("k8s-dra-driver_b200")
+from multi_gpu_rank import dv, finish, join, pkg, report, start
 import capacity_oracle as K
 F_EXH = pkg.api.F_EXHAUSTIVE
 
-rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-os.environ.setdefault("NCCL_DEBUG", "WARN")
-torch.cuda.set_device(local)
-dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", local))
-dev = torch.device("cuda", local)
-stream = torch.cuda.Stream(device=dev); torch.cuda.set_stream(stream)
-fails = 0
-
+rank, world, dev, stream = start()
 w = pkg.synth.preempt(n_node=32 * world, gpus_per_node=8, n_pending=200, seed=23)
 n_node = len(w.node_off) - 1
 n_pod = len(w.pod_off) - 1
@@ -33,28 +22,13 @@ bounds = [n_node * r // world for r in range(world)] + [n_node]
 g0, g1 = int(w.node_off[bounds[rank]]), int(w.node_off[bounds[rank + 1]])
 mine = w.empty.copy()
 mine[g0:g1] = w.gpus[g0:g1]
-ctx = pkg.api.Context(device=local, stream=stream.cuda_stream)
+ctx = pkg.api.Context(device=dev.index, stream=stream.cuda_stream)
 ctx.set_table(w.table); ctx.set_inventory(mine, w.node_off)
-uid = [pkg.api.Context.comm_unique_id() if rank == 0 else None]
-dist.broadcast_object_list(uid, src=0)
-ctx.comm_init(uid[0], rank, world)
-ctx.set_shard_map(bounds, stray_rank=0)
-ctx.set_shard_capacity(n_pod * n_node)
-hs = [None] * world
-dist.all_gather_object(hs, ctx.shard_export(64))
-ctx.peer_import(hs)
-
-
-def dv(a):
-    a = np.ascontiguousarray(a)
-    return torch.from_numpy(a.view(np.uint8).reshape(-1).copy()).to(dev) if a.nbytes else torch.zeros(16, dtype=torch.uint8, device=dev)
-
-
+join(ctx, bounds, 0, 64, capacity=(n_pod * n_node,))
 keep = [dv(w.claims), dv(w.pod_off)]
 
 
 def check(what, cn, co, flags):
-    global fails
     ref = K.capacity(w.gpus, w.node_off, w.table, w.claims, w.pod_off, cn, co, 64, K.F_EXHAUSTIVE if flags & F_EXH else 0)
     n_pair = n_pod * n_node if co is None else int(co[-1])
     d_n = dv(cn) if cn is not None else None
@@ -69,11 +43,7 @@ def check(what, cn, co, flags):
     dt = (np.uint16, np.uint8, np.uint64, np.uint32)
     got = [o.cpu().numpy()[:s].view(d) for o, s, d in zip(outs, sizes, dt)]
     ok = all(x.tobytes() == y.tobytes() for x, y in zip(got, ref)) and ctx.get_inventory().tobytes() == mine.tobytes()
-    t = torch.tensor([0 if ok else 1], device=dev); dist.all_reduce(t)
-    fails += int(t.item()) != 0
-    if rank == 0:
-        print(f"sharded pod capacity, {what}: {'OK' if int(t.item()) == 0 else 'MISMATCH'} "
-              f"({n_pod} pods, {int(ref[2].sum())} copies in all, {world} ranks)")
+    report(f"sharded pod capacity, {what}", ok, f"{n_pod} pods, {int(ref[2].sum())} copies in all, {world} ranks")
 
 
 rng = np.random.default_rng(5)
@@ -82,10 +52,4 @@ forms = {"dense": (None, None),
 for name, (cn, co) in forms.items():
     for flags, fname in ((0, "first-fit"), (F_EXH, "exhaustive")):
         check(f"{name}, {fname}", cn, co, flags)
-dist.barrier()
-ctx.close()
-t = torch.tensor([fails], device=dev); dist.all_reduce(t)
-if rank == 0:
-    print("ALL OK" if int(t.item()) == 0 else f"{int(t.item())} FAILURES")
-dist.destroy_process_group()
-sys.exit(1 if int(t.item()) else 0)
+finish([ctx])

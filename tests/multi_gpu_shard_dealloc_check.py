@@ -9,24 +9,16 @@ released the same way, which must give back the loaded inventory.
   python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tests/multi_gpu_shard_dealloc_check.py
 """
 import ctypes as C
-import importlib, os, sys
+
 import numpy as np
 import torch
 import torch.distributed as dist
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-pkg = importlib.import_module("k8s-dra-driver_b200")
+from multi_gpu_rank import dv, finish, join, pkg, report, start
 from oracle import oracle as O
 R = pkg.records
 
-rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-os.environ.setdefault("NCCL_DEBUG", "WARN")
-torch.cuda.set_device(local)
-dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", local))
-dev = torch.device("cuda", local)
-stream = torch.cuda.Stream(device=dev); torch.cuda.set_stream(stream)
-fails = 0
-
+rank, world, dev, stream = start()
 w = pkg.synth.mixed(4000, 200 * world + 5, 31, invalid=True)
 rng = np.random.default_rng(31)
 claims = w.claims.copy()
@@ -35,25 +27,12 @@ claims["kind"][sh], claims["count"][sh], claims["group"][sh] = R.KIND_SHARED, 1,
 claims["mem_limit_mib"][sh] = rng.choice(np.array([1024, 4096, 10240], dtype=np.uint32), int(sh.sum()))
 out_off, n_out = R.out_offsets(claims, w.n_node)
 n_out = int(n_out)
-ctx = pkg.api.Context(device=local, stream=stream.cuda_stream)
+ctx = pkg.api.Context(device=dev.index, stream=stream.cuda_stream)
 ctx.set_table(w.table); ctx.set_inventory(w.gpus, w.node_off)
-uid = [pkg.api.Context.comm_unique_id() if rank == 0 else None]
-dist.broadcast_object_list(uid, src=0)
-ctx.comm_init(uid[0], rank, world)
 bounds = [0] + [min(w.n_node, 1 + 3 * r * r) for r in range(1, world)] + [w.n_node]     # uneven ranges
-ctx.set_shard_map(bounds, stray_rank=world - 1)
-hs = [None] * world
-dist.all_gather_object(hs, ctx.shard_export(n_out))
-ctx.peer_import(hs)
+join(ctx, bounds, world - 1, n_out)
 g0, g1 = int(w.node_off[bounds[rank]]), int(w.node_off[bounds[rank + 1]])
-
-
-def report(what, ok):
-    global fails
-    t = torch.tensor([0 if ok else 1], device=dev); dist.all_reduce(t)
-    fails += int(t.item()) != 0
-    if rank == 0:
-        print(f"{what}: {'OK' if int(t.item()) == 0 else 'MISMATCH'} ({world} ranks, {w.n_gpu} GPUs)")
+detail = f"{world} ranks, {w.n_gpu} GPUs"
 
 
 def table_ptr():
@@ -63,38 +42,30 @@ def table_ptr():
 
 
 def release(sub, sub_off, state, what):
-    d_c = torch.from_numpy(sub.view(np.uint8).copy()).to(dev)
-    d_o = torch.from_numpy(sub_off.view(np.uint8).copy()).to(dev)
+    d_c, d_o = dv(sub), dv(sub_off)
     torch.cuda.synchronize()
     before = ctx.get_inventory()
     ctx.deallocate_global_device(d_c.data_ptr(), len(sub), d_o.data_ptr(), table_ptr(), n_out)
     ctx.sync()
     inv = ctx.get_inventory()
     report(what, inv[g0:g1].tobytes() == state[g0:g1].tobytes() and inv[:g0].tobytes() == before[:g0].tobytes()
-           and inv[g1:].tobytes() == before[g1:].tobytes())
+           and inv[g1:].tobytes() == before[g1:].tobytes(), detail)
     dist.barrier()
     ctx.shard_sync_inventory_device()
     ctx.sync()
-    report(f"{what}, then the sync", ctx.get_inventory().tobytes() == state.tobytes())
+    report(f"{what}, then the sync", ctx.get_inventory().tobytes() == state.tobytes(), detail)
 
 
-d_c = torch.from_numpy(claims.view(np.uint8).copy()).to(dev)
-d_o = torch.from_numpy(out_off.view(np.uint8).copy()).to(dev)
+d_c, d_o = dv(claims), dv(out_off)
 torch.cuda.synchronize()
 ref, state = O.allocate(w.gpus, w.node_off, w.table, claims, out_off, n_out)
 ctx.allocate_global_device(d_c.data_ptr(), len(claims), d_o.data_ptr(), n_out, 0)
 ctx.sync()
-report("sharded Allocate", ctx.gather_read(np.zeros(n_out, dtype=R.OUT_DTYPE)).tobytes() == ref.tobytes())
+report("sharded Allocate", ctx.gather_read(np.zeros(n_out, dtype=R.OUT_DTYPE)).tobytes() == ref.tobytes(), detail)
 sel = rng.random(len(claims)) < 0.4
 state = O.deallocate(state, claims[sel], ref, out_off[sel], n_node=w.n_node)
 release(claims[sel], out_off[sel].copy(), state, "sharded Deallocate of 40% of the claims")
 state = O.deallocate(state, claims[~sel], ref, out_off[~sel], n_node=w.n_node)
 release(claims[~sel], out_off[~sel].copy(), state, "sharded Deallocate of the rest")
-report("every record released gives back the loaded inventory", state.tobytes() == w.gpus.tobytes())
-dist.barrier()
-ctx.close()
-t = torch.tensor([fails], device=dev); dist.all_reduce(t)
-if rank == 0:
-    print("ALL OK" if int(t.item()) == 0 else f"{int(t.item())} FAILURES")
-dist.destroy_process_group()
-sys.exit(1 if int(t.item()) else 0)
+report("every record released gives back the loaded inventory", state.tobytes() == w.gpus.tobytes(), detail)
+finish([ctx])

@@ -7,26 +7,16 @@ Every rank's whole table, pod_node and own inventory range must equal the CPU or
 
   python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tests/multi_gpu_shard_place_check.py
 """
-import importlib, os, sys
 import numpy as np
 import torch
 import torch.distributed as dist
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-pkg = importlib.import_module("k8s-dra-driver_b200")
+from multi_gpu_rank import dv, finish, join, pkg, report, start
 import place_oracle as P
 R = pkg.records
 F_EXH, F_FRESH = pkg.api.F_EXHAUSTIVE, pkg.api.F_FRESH_INVENTORY
 
-rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-os.environ.setdefault("NCCL_DEBUG", "WARN")
-torch.cuda.set_device(local)
-dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", local))
-dev = torch.device("cuda", local)
-stream = torch.cuda.Stream(device=dev); torch.cuda.set_stream(stream)
-fails = 0
-
+rank, world, dev, stream = start()
 w, pod_off = pkg.synth.pods(2000, 24 * world, 17)
 bounds = [w.n_node * r // world for r in range(world)] + [w.n_node]
 g0, g1 = int(w.node_off[bounds[rank]]), int(w.node_off[bounds[rank + 1]])
@@ -34,20 +24,9 @@ first = int(pod_off[300])
 claims = w.claims[first:].copy()
 po = (pod_off[300:] - first).astype(np.uint32)
 n_pod = len(po) - 1
-ctx = pkg.api.Context(device=local, stream=stream.cuda_stream)
+ctx = pkg.api.Context(device=dev.index, stream=stream.cuda_stream)
 ctx.set_table(w.table); ctx.set_inventory(w.gpus, w.node_off)
-uid = [pkg.api.Context.comm_unique_id() if rank == 0 else None]
-dist.broadcast_object_list(uid, src=0)
-ctx.comm_init(uid[0], rank, world)
-ctx.set_shard_map(bounds, stray_rank=world - 1)
-ctx.set_shard_place(n_pod)
-hs = [None] * world
-dist.all_gather_object(hs, ctx.shard_export(max(w.n_claim, 1)))
-ctx.peer_import(hs)
-
-
-def dv(a):
-    return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).copy()).to(dev)
+join(ctx, bounds, world - 1, max(w.n_claim, 1), place=(n_pod,))
 
 
 def real_state():
@@ -61,7 +40,6 @@ def real_state():
 
 
 def check(what, cn, co, flags):
-    global fails
     src = w.gpus if flags & F_FRESH else real_state()
     ref, ref_node, ref_inv = P.place_pods(src, w.node_off, w.table, claims, po, cn, co, None, len(claims),
                                           P.F_EXHAUSTIVE if flags & F_EXH else 0)
@@ -78,11 +56,7 @@ def check(what, cn, co, flags):
     node = d_pn.cpu().numpy().view(np.uint32)
     inv = ctx.get_inventory()
     ok = got.tobytes() == ref.tobytes() and node.tobytes() == ref_node.tobytes() and inv[g0:g1].tobytes() == ref_inv[g0:g1].tobytes()
-    t = torch.tensor([0 if ok else 1], device=dev); dist.all_reduce(t)
-    fails += int(t.item()) != 0
-    if rank == 0:
-        print(f"sharded place pods, {what}: {'OK' if int(t.item()) == 0 else 'MISMATCH'} "
-              f"({n_pod} pods, {int((ref_node != 0xFFFFFFFF).sum())} placed, {world} ranks)")
+    report(f"sharded place pods, {what}", ok, f"{n_pod} pods, {int((ref_node != 0xFFFFFFFF).sum())} placed, {world} ranks")
 
 
 d_first = dv(w.claims[:first])
@@ -97,10 +71,4 @@ forms = {"dense": (None, None),
 for name, (cn, co) in forms.items():
     for flags, fname in ((0, "first-fit"), (F_EXH, "exhaustive"), (F_FRESH, "fresh first-fit"), (F_EXH | F_FRESH, "fresh exhaustive")):
         check(f"{name}, {fname}", cn, co, flags)
-dist.barrier()
-ctx.close()
-t = torch.tensor([fails], device=dev); dist.all_reduce(t)
-if rank == 0:
-    print("ALL OK" if int(t.item()) == 0 else f"{int(t.item())} FAILURES")
-dist.destroy_process_group()
-sys.exit(1 if int(t.item()) else 0)
+finish([ctx])

@@ -8,26 +8,15 @@ real world, its own range must equal the oracle's final inventory, and the rest 
 
   python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tests/multi_gpu_shard_preempt_place_check.py
 """
-import importlib, os, sys
 import numpy as np
 import torch
-import torch.distributed as dist
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-pkg = importlib.import_module("k8s-dra-driver_b200")
+from multi_gpu_rank import dv, finish, join, pkg, report, start
 import preempt_place_oracle as PP
 R = pkg.records
 F_EXH = pkg.api.F_EXHAUSTIVE
 
-rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-os.environ.setdefault("NCCL_DEBUG", "WARN")
-torch.cuda.set_device(local)
-dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", local))
-dev = torch.device("cuda", local)
-stream = torch.cuda.Stream(device=dev); torch.cuda.set_stream(stream)
-fails = 0
-
+rank, world, dev, stream = start()
 w = pkg.synth.preempt(n_node=32 * world, gpus_per_node=8, n_pending=200, seed=29)
 n_node = len(w.node_off) - 1
 n_pod = len(w.pod_off) - 1
@@ -40,30 +29,15 @@ placed = w.claims.copy(); placed["node"] = 0
 sl = R.claim_slots(placed, 1).astype(np.int64)
 out_off = np.concatenate([[0], np.cumsum(sl)[:-1]]).astype(np.uint32)
 n_out = int(sl.sum())
-ctx = pkg.api.Context(device=local, stream=stream.cuda_stream)
+ctx = pkg.api.Context(device=dev.index, stream=stream.cuda_stream)
 ctx.set_table(w.table); ctx.set_inventory(mine, w.node_off)
-uid = [pkg.api.Context.comm_unique_id() if rank == 0 else None]
-dist.broadcast_object_list(uid, src=0)
-ctx.comm_init(uid[0], rank, world)
-ctx.set_shard_map(bounds, stray_rank=0)
-ctx.set_shard_preempt_place(n_pod, n_pod * n_node, n_run)
-hs = [None] * world
-dist.all_gather_object(hs, ctx.shard_export(n_out))
-ctx.peer_import(hs)
-
-
-def dv(a):
-    a = np.ascontiguousarray(a)
-    return torch.from_numpy(a.view(np.uint8).reshape(-1).copy()).to(dev) if a.nbytes else torch.zeros(16, dtype=torch.uint8, device=dev)
-
-
+join(ctx, bounds, 0, n_out, preempt_place=(n_pod, n_pod * n_node, n_run))
 keep = [dv(x) for x in (w.claims, w.pod_off, w.prio, w.run_claims, w.run_pod_off, w.run_prio, w.run_out, out_off)]
 run = pkg.api.RunningPods(keep[3].data_ptr(), len(w.run_claims), keep[4].data_ptr(), n_run,
                           keep[5].data_ptr(), None, keep[6].data_ptr(), len(w.run_out))
 
 
 def check(what, cn, co, flags):
-    global fails
     ref = PP.preempt_place(w.gpus, w.node_off, w.table, w.claims, w.pod_off, w.prio, w.run_claims, w.run_pod_off,
                            w.run_prio, w.run_out, None, cn, co, out_off, n_out, PP.F_EXHAUSTIVE if flags & F_EXH else 0)
     ctx.set_inventory(mine, w.node_off)                        # every call from the world as loaded
@@ -82,11 +56,7 @@ def check(what, cn, co, flags):
     ok = all(x.tobytes() == y.tobytes() for x, y in zip(got, ref[:4]))
     ok = ok and inv[g0:g1].tobytes() == ref[4][g0:g1].tobytes()
     ok = ok and inv[:g0].tobytes() == mine[:g0].tobytes() and inv[g1:].tobytes() == mine[g1:].tobytes()
-    t = torch.tensor([0 if ok else 1], device=dev); dist.all_reduce(t)
-    fails += int(t.item()) != 0
-    if rank == 0:
-        print(f"sharded preempt and place, {what}: {'OK' if int(t.item()) == 0 else 'MISMATCH'} "
-              f"({n_pod} pods, {int((ref[2] == PP.EVICT).sum())} evicting, {world} ranks)")
+    report(f"sharded preempt and place, {what}", ok, f"{n_pod} pods, {int((ref[2] == PP.EVICT).sum())} evicting, {world} ranks")
 
 
 rng = np.random.default_rng(5)
@@ -95,10 +65,4 @@ forms = {"dense": (None, None),
 for name, (cn, co) in forms.items():
     for flags, fname in ((0, "first-fit"), (F_EXH, "exhaustive")):
         check(f"{name}, {fname}", cn, co, flags)
-dist.barrier()
-ctx.close()
-t = torch.tensor([fails], device=dev); dist.all_reduce(t)
-if rank == 0:
-    print("ALL OK" if int(t.item()) == 0 else f"{int(t.item())} FAILURES")
-dist.destroy_process_group()
-sys.exit(1 if int(t.item()) else 0)
+finish([ctx])

@@ -8,47 +8,25 @@ table and state.
 
   python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tests/multi_gpu_shard_sync_check.py
 """
-import importlib, os, sys
 import numpy as np
 import torch
 import torch.distributed as dist
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-pkg = importlib.import_module("k8s-dra-driver_b200")
+from multi_gpu_rank import dv, finish, join, pkg, report, start
 from oracle import oracle as O
 R = pkg.records
 
-rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-os.environ.setdefault("NCCL_DEBUG", "WARN")
-torch.cuda.set_device(local)
-dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", local))
-dev = torch.device("cuda", local)
-stream = torch.cuda.Stream(device=dev); torch.cuda.set_stream(stream)
-fails = 0
-
+rank, world, dev, stream = start()
 w = pkg.synth.mixed(4000, 200 * world + 5, 21, invalid=True)      # 2,900-5,900 GPUs: k_isync_copy runs 12-23 CTAs
-ctx = pkg.api.Context(device=local, stream=stream.cuda_stream)
+ctx = pkg.api.Context(device=dev.index, stream=stream.cuda_stream)
 ctx.set_table(w.table); ctx.set_inventory(w.gpus, w.node_off)
-uid = [pkg.api.Context.comm_unique_id() if rank == 0 else None]
-dist.broadcast_object_list(uid, src=0)
-ctx.comm_init(uid[0], rank, world)
 bounds = [0] + [min(w.n_node, 1 + 3 * r * r) for r in range(1, world)] + [w.n_node]     # uneven ranges
-ctx.set_shard_map(bounds, stray_rank=world - 1)
-hs = [None] * world
-dist.all_gather_object(hs, ctx.shard_export(w.n_out))
-ctx.peer_import(hs)
-
-
-def report(what, ok):
-    global fails
-    t = torch.tensor([0 if ok else 1], device=dev); dist.all_reduce(t)
-    fails += int(t.item()) != 0
-    if rank == 0:
-        print(f"{what}: {'OK' if int(t.item()) == 0 else 'MISMATCH'} ({world} ranks, {w.n_gpu} GPUs)")
+join(ctx, bounds, world - 1, w.n_out)
+detail = f"{world} ranks, {w.n_gpu} GPUs"
 
 
 def allocate(claims, out_off, n_out):
-    d_c, d_o = torch.from_numpy(claims.view(np.uint8).copy()).to(dev), torch.from_numpy(out_off.view(np.uint8).copy()).to(dev)
+    d_c, d_o = dv(claims), dv(out_off)
     torch.cuda.synchronize()
     ctx.allocate_global_device(d_c.data_ptr(), len(claims), d_o.data_ptr(), n_out, 0)
     ctx.sync()
@@ -62,13 +40,13 @@ def sync_and_check(what, state):
     ctx.shard_sync_inventory_device()
     ctx.sync()
     inv = ctx.get_inventory()
-    report(what, inv.tobytes() == state.tobytes() and inv[g0:g1].tobytes() == before[g0:g1].tobytes())
+    report(what, inv.tobytes() == state.tobytes() and inv[g0:g1].tobytes() == before[g0:g1].tobytes(), detail)
 
 
 # 1. sharded Allocate, then every rank deallocates the first half of the claims' records
 claims, out_off, n_out = w.claims, w.out_off, int(w.n_out)
 ref, state = O.allocate(w.gpus, w.node_off, w.table, claims, out_off, n_out)
-report("sharded Allocate", allocate(claims, out_off, n_out).tobytes() == ref.tobytes())
+report("sharded Allocate", allocate(claims, out_off, n_out).tobytes() == ref.tobytes(), detail)
 half = len(claims) // 2
 ctx.deallocate(claims[:half], ref, out_off[:half])
 state = O.deallocate(state, claims[:half], ref, out_off[:half], n_node=w.n_node)
@@ -79,12 +57,6 @@ ctx.set_shard_map(bounds, stray_rank=0)
 c2 = w.claims.copy(); c2["node"] = (c2["node"] + 3) % w.n_node
 o2, n2 = R.out_offsets(c2, w.n_node)
 ref2, state = O.allocate(state, w.node_off, w.table, c2, o2, int(n2))
-report("sharded Allocate after the re-map", allocate(c2, o2, int(n2)).tobytes() == ref2.tobytes())
+report("sharded Allocate after the re-map", allocate(c2, o2, int(n2)).tobytes() == ref2.tobytes(), detail)
 sync_and_check("sync after the re-map", state)
-dist.barrier()
-ctx.close()
-t = torch.tensor([fails], device=dev); dist.all_reduce(t)
-if rank == 0:
-    print("ALL OK" if int(t.item()) == 0 else f"{int(t.item())} FAILURES")
-dist.destroy_process_group()
-sys.exit(1 if int(t.item()) else 0)
+finish([ctx])

@@ -7,24 +7,14 @@ candidate-list forms, first-fit and exhaustive, claims of every kind with counts
 
   python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 tests/multi_gpu_shard_unsuitable_check.py
 """
-import importlib, os, sys
 import numpy as np
 import torch
-import torch.distributed as dist
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-pkg = importlib.import_module("k8s-dra-driver_b200")
+from multi_gpu_rank import dv, finish, join, pkg, report, start
 from oracle import oracle as O
 R = pkg.records
 
-rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-os.environ.setdefault("NCCL_DEBUG", "WARN")
-torch.cuda.set_device(local)
-dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", local))
-dev = torch.device("cuda", local)
-stream = torch.cuda.Stream(device=dev); torch.cuda.set_stream(stream)
-fails = 0
-
+rank, world, dev, stream = start()
 w = pkg.synth.mixed(9000, 97, 41)
 ranges = pkg.shard.plan(w.claims["node"], w.n_node, world)
 n_pod = 800
@@ -34,21 +24,9 @@ rng = np.random.default_rng(7)
 per = rng.integers(0, 12, n_pod)
 cand_off = np.zeros(n_pod + 1, dtype=np.uint32); cand_off[1:] = np.cumsum(per)
 cand_nodes = rng.integers(0, w.n_node + 3, int(cand_off[-1])).astype(np.uint32)      # some name no node
-ctx = pkg.api.Context(device=local, stream=stream.cuda_stream)
+ctx = pkg.api.Context(device=dev.index, stream=stream.cuda_stream)
 ctx.set_table(w.table); ctx.set_inventory(w.gpus, w.node_off)
-uid = [pkg.api.Context.comm_unique_id() if rank == 0 else None]
-dist.broadcast_object_list(uid, src=0)
-ctx.comm_init(uid[0], rank, world)
-ctx.set_shard_map([r[0] for r in ranges] + [ranges[-1][1]], stray_rank=0)
-ctx.set_shard_pairs(n_pod * w.n_node)
-hs = [None] * world
-dist.all_gather_object(hs, ctx.shard_export(w.n_out))
-ctx.peer_import(hs)
-
-
-def dv(a):
-    return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).copy()).to(dev)
-
+join(ctx, [r[0] for r in ranges] + [ranges[-1][1]], 0, w.n_out, pairs=(n_pod * w.n_node,))
 
 d_claims, d_off = dv(w.claims), dv(w.out_off)
 ctx.allocate_global_device(d_claims.data_ptr(), w.n_claim, d_off.data_ptr(), w.n_out, 0)
@@ -66,14 +44,6 @@ for rep in range(2):                                   # repeated calls: both st
                                          None if dco is None else dco.data_ptr(), n_pair, bits.data_ptr(), flags)
             ctx.sync()
             ref = O.unsuitable(real, w.node_off, w.table, pods, pod_off, cn, co, flags=oflags)
-            ok = bits.cpu().numpy().tobytes() == ref.tobytes()
-            fails += not ok
-            if rank == 0:
-                print(f"sharded UnsuitableNodes rep {rep}, {form}, flags {flags}: {'OK' if ok else 'MISMATCH'} ({n_pair} pairs, {world} ranks)")
-dist.barrier()
-ctx.close()
-t = torch.tensor([fails], device=dev); dist.all_reduce(t)
-if rank == 0:
-    print("ALL OK" if int(t.item()) == 0 else f"{int(t.item())} FAILURES")
-dist.destroy_process_group()
-sys.exit(1 if int(t.item()) else 0)
+            report(f"sharded UnsuitableNodes rep {rep}, {form}, flags {flags}", bits.cpu().numpy().tobytes() == ref.tobytes(),
+                   f"{n_pair} pairs, {world} ranks")
+finish([ctx])

@@ -21,7 +21,7 @@ import numpy as np
 import limit_problems as LP
 from preempt_problems import _Rng
 from test_gpu_limits import FIXTURES, SEEDS, _fixture, _tile
-from test_gpu_shard_unsuitable import _bounds
+from shard_world import bounds as _bounds
 from test_oracle_selector_properties import selector_programs
 
 PKG = importlib.import_module("k8s-dra-driver_b200")

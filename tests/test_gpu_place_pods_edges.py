@@ -25,8 +25,8 @@ import preempt_oracle as PR
 import preempt_place_oracle as PP
 import test_place_pods_edges as E
 from test_gpu_pod_call_checks import PLACE, PODS, PRE, PREPL, SENTINEL, _base, _raw
-from test_gpu_shard_place import PlaceWorld
-from test_gpu_shard_unsuitable import _bounds
+import shard_world as S
+from test_gpu_shard_place import _check as _check_sharded
 from test_preempt import mig_running, occupied
 
 pytestmark = pytest.mark.gpu
@@ -310,11 +310,12 @@ def test_fresh_inventory_on_a_changed_live_state(pkg, pctx):
 # ---- f. the same problems on a sharded world ------------------------------------------------------------------------
 def _sharded(pkg, pb, world, kind, flags, what):
     w = SimpleNamespace(gpus=pb.gpus, node_off=pb.node_off, table=pb.table, n_node=pb.n_node)
-    W = PlaceWorld(pkg, w, world, _bounds(pb.n_node, world, kind), world - 1, max_pods=max(len(pb.pod_off) - 1, 1))
+    W = S.World(pkg, pb.table, pb.node_off, pb.gpus, world, S.bounds(pb.n_node, world, kind), world - 1, n_out_max=1 << 16,
+                place=max(len(pb.pod_off) - 1, 1))
     try:
         for cn, co in (E.cand_arrays(pb), (None, None)):
-            W.check_place(pb.claims, pb.pod_off, cn, co, pb.out_off, pb.n_out, flags,
-                          f"{what} world {world} {kind} {'dense' if cn is None else 'cands'}")
+            _check_sharded(W, w, pb.claims, pb.pod_off, cn, co, pb.out_off, pb.n_out, flags,
+                           f"{what} world {world} {kind} {'dense' if cn is None else 'cands'}")
     finally:
         W.close()
 

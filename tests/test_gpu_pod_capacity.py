@@ -208,18 +208,17 @@ def test_sharded_world_sync_then_capacity_on_any_rank(pkg, oracle):
     """Two ranks on one device: after sharded pods Allocate calls each rank's copy is right for its own range only;
     dra_shard_sync_inventory_device makes every copy the world's state, and the capacity call on either rank then answers
     as the oracle does on that state."""
-    from test_gpu_shard_pods import _malformed_mixed
-    from test_gpu_shard_sync import SyncWorld
+    import shard_world as S
     w = pkg.synth.mixed(2400, 31, 72, invalid=True)
     bounds = [0, 11, w.n_node]
     rng = np.random.default_rng(2)
-    W = SyncWorld(pkg, w, 2, bounds)
+    W = S.World(pkg, w.table, w.node_off, w.gpus, 2, bounds, n_out_max=1 << 16)
     try:
         state = w.gpus
         for flags, oflags in ((0, 0), (pkg.api.F_EXHAUSTIVE, oracle.F_EXHAUSTIVE)):
-            pc, po, poo, pn = _malformed_mixed(pkg, w, bounds, rng, True)
+            pc, po, poo, pn = S.malformed_mixed(pkg, w, bounds, rng, True)
             _, state = oracle.allocate_pods(state, w.node_off, w.table, pc, po, poo, pn, oflags)
-            W.call(pc, po, poo, pn, flags)
+            S.pods(W, pc, po, poo, pn, flags)
         assert any(inv.tobytes() != state.tobytes() for inv in W.inventories())
         W.sync_inventory()
         pods_w, pod_off = pkg.synth.pods(n_pod=50, n_node=w.n_node, seed=1)

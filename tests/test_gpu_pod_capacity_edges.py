@@ -288,22 +288,22 @@ def test_sums_past_two_to_the_32(pkg, cctx):
 
 @pytest.mark.parametrize("world", [1, 2])
 def test_sharded_sums_past_two_to_the_32(pkg, world):
-    from test_gpu_shard_pod_capacity import World, _same4
+    import shard_world as S
     t = R.default_table()
     n_node = 65538
     g, off = R.make_inventory([1] * n_node, mig=True)
-    W = World(pkg, g, off, t, world, [0, 40000, n_node][:: (1 if world == 2 else 2)], max_pairs=2_200_000)
+    W = S.World(pkg, t, off, g, world, [0, 40000, n_node][:: (1 if world == 2 else 2)], capacity=2_200_000)
     try:
         for n_list in SUM_LISTS:
             c, po, cn, co = sum_problem(n_list, n_node)
             ref = K.capacity(g, off, t, c, po, cn, co, 65535)
             assert int(ref[2][0]) > 1 << 32
-            for r, got in enumerate(W.call(c, po, (cn, co), 65535)):
-                _same4(got, ref, f"world {world} rank {r} {n_list}")
+            for r, got in enumerate(S.capacity(W, c, po, (cn, co), 65535)):
+                S.same(got, ref, S.CAPACITY_NAMES, f"world {world} rank {r} {n_list}")
         c, po = _pods([EMPTY, ONEGPU])
         ref = K.capacity(g, off, t, c, po, None, None, 65535)
-        for r, got in enumerate(W.call(c, po, None, 65535)):
-            _same4(got, ref, f"world {world} rank {r} dense")
+        for r, got in enumerate(S.capacity(W, c, po, None, 65535)):
+            S.same(got, ref, S.CAPACITY_NAMES, f"world {world} rank {r} dense")
         assert all(ctx.get_inventory().tobytes() == g.tobytes() for ctx in W.ctxs)
     finally:
         W.close()
@@ -424,13 +424,13 @@ def _rows_against_oracle(got_row, g, off, t, pod, mc, fl, what):
 def test_sharded_capacity_dense_at_the_pair_cap(pkg):
     """dra_pod_capacity_batch_global_device at world 1 over 0xFFFFFFF0 dense pairs, outputs kept on the device"""
     import torch
-    from test_gpu_shard_pod_capacity import World
+    import shard_world as S
     n_node, n_pod, mc = 6960, 617093, 3
     n_pair = n_node * n_pod
     _need(28 << 30, 1 << 30)
     g, off, c, po, real = limit_problem(n_node, n_pod, 8)
     t = R.default_table()
-    W = World(pkg, g, off, t, 1, [0, n_node])
+    W = S.World(pkg, t, off, g, 1, [0, n_node])
     try:
         ctx = W.ctxs[0]
         outs = [torch.full((s + SLACK,), SENT, dtype=torch.uint8, device="cuda:0")

@@ -7,7 +7,6 @@ Every case compares OutRecs and inventory byte for byte with the C oracle, with 
 exhaustive UnsuitableNodes bitmap with the oracle's in the dense form and with candidate lists; then it asserts the
 property it exists for.  The literal fixtures and their descent counts are checked without a GPU in
 tests/test_pod_search_fixtures.py."""
-import types
 
 import numpy as np
 import pytest
@@ -342,13 +341,12 @@ def test_pod_sequences_and_fresh_inventory(pkg, ctx, oracle):
 # ---- 7. the same fixtures through the sharded call ---------------------------------------------------------------------
 @pytest.mark.parametrize("world", [1, 2])
 def test_sharded_call_matches_single_context(pkg, oracle, world):
-    from test_gpu_shard_pods import PodWorld
+    import shard_world as S
     api = pkg.api
     inv = Inv(F.deep_fixtures() + F.budget_fixtures() + F.colocation_fixtures() + _selector_fixtures())
     attrs, sels = _selectors(inv)
-    w = types.SimpleNamespace(gpus=inv.gpus, node_off=inv.node_off, table=inv.table)
     bounds = [0, inv.n_node] if world == 1 else [0, inv.n_node // 2, inv.n_node]
-    W = PodWorld(pkg, w, world, bounds, stray_rank=0, attrs=attrs, sels=sels)
+    W = S.World(pkg, inv.table, inv.node_off, inv.gpus, world, bounds, attrs=attrs, sels=sels, n_out_max=1 << 16)
     oracle.set_selectors(attrs, sels)
     try:
         with api.Context(device=0) as single:
@@ -357,7 +355,7 @@ def test_sharded_call_matches_single_context(pkg, oracle, world):
             for flags in (api.F_EXHAUSTIVE, api.F_FRESH_INVENTORY, api.F_EXHAUSTIVE | api.F_FRESH_INVENTORY):
                 single.set_inventory(inv.gpus, inv.node_off)
                 want = single.allocate_pods(inv.claims, inv.pod_off, flags=flags & ~api.F_FRESH_INVENTORY)
-                tables = W.call(inv.claims, inv.pod_off, None, len(inv.claims), flags)
+                tables = S.pods(W, inv.claims, inv.pod_off, None, len(inv.claims), flags)
                 for r, t in enumerate(tables):
                     assert t.tobytes() == want.tobytes(), f"world {world} rank {r} flags {flags}: table differs"
                 for r in range(world):

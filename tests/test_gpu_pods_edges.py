@@ -20,8 +20,7 @@ import numpy as np
 import pytest
 
 import test_pods_edges as E
-from test_gpu_shard_pods import PodWorld
-from test_gpu_shard_unsuitable import _bounds
+import shard_world as S
 
 pytestmark = pytest.mark.gpu
 SENT, SLACK = 0xA5, 16
@@ -321,8 +320,8 @@ WORLDS = [(1, "even"), (2, "uneven"), (3, "even"), (3, "empty")]
 
 
 def _world(pkg, pb, world, kind):
-    w = SimpleNamespace(gpus=pb.gpus, node_off=pb.node_off, table=pb.table, n_node=pb.n_node)
-    return PodWorld(pkg, w, world, _bounds(pb.n_node, world, kind), world - 1)
+    return S.World(pkg, pb.table, pb.node_off, pb.gpus, world, S.bounds(pb.n_node, world, kind), world - 1,
+                   n_out_max=1 << 16)
 
 
 def _sharded_same(pkg, W, single, pb, flags, what):
@@ -331,7 +330,7 @@ def _sharded_same(pkg, W, single, pb, flags, what):
     A = pkg.api
     rc, ref = raw_pods(pkg, single, pb, flags=flags)
     assert rc == A.OK, f"{what}: single rc {rc}"
-    tables = W.call(pb.claims, pb.pod_off, pb.out_off, pb.n_out, flags)
+    tables = S.pods(W, pb.claims, pb.pod_off, pb.out_off, pb.n_out, flags)
     mine = E.owned(pb)
     inv = single.get_inventory()
     for r, t in enumerate(tables):
@@ -375,16 +374,7 @@ def test_sharded_slot_fault(pkg, pctx, world, kind):
             for claims, oo, what in faults(R, pb, where):
                 for flags in (0, A.F_FRESH_INVENTORY, A.F_EXHAUSTIVE):
                     before = W.inventories()
-                    keep = W.enqueue(claims, pb.pod_off, oo, pb.n_out, flags)
-                    codes = []
-                    for c in W.ctxs:
-                        try:
-                            c.sync()
-                            codes.append(A.OK)
-                        except A.DraError as e:
-                            codes.append(e.code)
-                    del keep
-                    assert codes == [A.E_INVAL] * world, f"{what} f{flags}: {codes}"
+                    S.pods(W, claims, pb.pod_off, oo, pb.n_out, flags, expect=A.E_INVAL)
                     for r, (b, a) in enumerate(zip(before, W.inventories())):
                         assert a.tobytes() == b.tobytes(), f"{what} f{flags}: rank {r} inventory changed"
                 _sharded_same(pkg, W, pctx, pb, A.F_EXHAUSTIVE, f"after {what}")

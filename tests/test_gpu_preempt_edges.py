@@ -11,7 +11,6 @@ import dataclasses
 import functools
 import inspect
 import os
-from types import SimpleNamespace
 
 import numpy as np
 import pytest
@@ -22,8 +21,8 @@ import preempt_oracle as P
 import test_preempt as T
 from preempt_problems import I32_MAX, I32_MIN, NONE, Problem, problems, random_problem
 from test_gpu_preempt import _raw
-from test_gpu_shard_preempt import Running, World, _same
-from test_gpu_shard_unsuitable import _bounds
+import shard_world as S
+from shard_world import Running
 from test_pod_mode import _mig
 from test_preempt import mig_running, occupied
 
@@ -364,8 +363,8 @@ def _sharded(pkg, pb, world, kind, bounds=None, what=""):
     """pb on a world of `world` contexts, every rank against the oracle; returns rank 0's outputs (None: a call-level
     error, which must fail every rank with nothing written)"""
     A = pkg.api
-    w = SimpleNamespace(gpus=pb.gpus, node_off=pb.node_off, table=pb.table, run_claims=pb.run_claims)
-    W = World(pkg, w, world, bounds or _bounds(pb.n_node, world, kind), sizes=(64, 4096, 64), n_out=len(pb.run_out))
+    W = S.World(pkg, pb.table, pb.node_off, pb.gpus, world, bounds or S.bounds(pb.n_node, world, kind),
+                n_out_max=max(1, len(pb.run_out)), preempt=(64, 4096, 64), pairs=4096)
     what = f"{what} world {world} {kind}"
     try:
         run = Running(pkg, pb.run_claims, pb.run_pod_off, pb.run_prio, pb.run_out, out_off=pb.run_out_off)
@@ -375,20 +374,16 @@ def _sharded(pkg, pb, world, kind, bounds=None, what=""):
         except ValueError:
             ref = None
         if ref is None:
-            outs, _ = W.enqueue(pb.claims, pb.pod_off, pb.prio, run, pb.cand_arrays() if pb.cands is not None else None,
-                                pb.max_victims, fl)
-            for r, c in enumerate(W.ctxs):
-                with pytest.raises(A.DraError) as e:
-                    c.sync()
-                assert e.value.code == A.E_INVAL, (what, r)
+            outs = S.preempt(W, pb.claims, pb.pod_off, pb.prio, run, pb.cand_arrays() if pb.cands is not None else None,
+                             pb.max_victims, fl, expect=A.E_INVAL)
             for r, o in enumerate(outs):
-                assert all((t.cpu().numpy() == 0x5C).all() for t in o), f"{what}: rank {r} wrote an output"
+                assert all((h == 0x5C).all() for h in o), f"{what}: rank {r} wrote an output"
             got = None
         else:
-            res = W.call(pb.claims, pb.pod_off, pb.prio, run, pb.cand_arrays() if pb.cands is not None else None,
-                         pb.max_victims, fl)
+            res = S.preempt(W, pb.claims, pb.pod_off, pb.prio, run, pb.cand_arrays() if pb.cands is not None else None,
+                            pb.max_victims, fl)
             for r, x in enumerate(res):
-                _same(x, ref, f"{what} rank {r}")
+                S.same(x, ref, S.PREEMPT_NAMES, f"{what} rank {r}")
                 assert "preempt_shard" in W.ctxs[r].last_chain(), (what, r)
             got = res[0]
         for r, c in enumerate(W.ctxs):

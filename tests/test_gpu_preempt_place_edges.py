@@ -18,7 +18,6 @@ import dataclasses
 import functools
 import inspect
 import os
-from types import SimpleNamespace
 
 import numpy as np
 import pytest
@@ -31,9 +30,9 @@ import test_preempt_place as TP
 from preempt_problems import NONE, PlaceProblem, Problem, _Rng, as_place, place_problems, random_place_problem
 from test_gpu_preempt_edges import _call as _call14, _fixture_problems, _load, _n_sm, _sum_world, _warp_world
 from test_gpu_preempt_place import _raw
-from test_gpu_shard_preempt import Running
-from test_gpu_shard_preempt_place import World
-from test_gpu_shard_unsuitable import _bounds
+import shard_world as S
+from shard_world import Running
+from test_gpu_shard_preempt_place import _check as _check_sharded
 from test_pod_mode import _mig
 from test_preempt import mig_running, occupied
 from test_preempt_place import check_matched
@@ -430,8 +429,8 @@ def _sharded(pkg, pb, world, kind, what=""):
     """pb on a world of `world` contexts, every rank against the oracle on the world's state; a call-level error must
     fail every rank with nothing written"""
     A = pkg.api
-    w = SimpleNamespace(gpus=pb.gpus, node_off=pb.node_off, table=pb.table, run_claims=pb.run_claims)
-    W = World(pkg, w, world, _bounds(pb.n_node, world, kind), sizes=(64, 4096, 512))
+    W = S.World(pkg, pb.table, pb.node_off, pb.gpus, world, S.bounds(pb.n_node, world, kind), n_out_max=65536,
+                preempt_place=(64, 4096, 512))
     what = f"{what} world {world} {kind}"
     fl = A.F_EXHAUSTIVE if pb.flags else 0
     cands = pb.cand_arrays() if pb.cands is not None else None
@@ -440,19 +439,17 @@ def _sharded(pkg, pb, world, kind, what=""):
         run = Running(pkg, *ra, out_off=pb.run_out_off)
         if pb.error:
             try:
-                outs, _ = W.enqueue(pb.claims, pb.pod_off, pb.prio, run, cands, fl, (pb.out_off, pb.n_out))
+                outs = S.preempt_place(W, pb.claims, pb.pod_off, pb.prio, run, cands, pb.out_off, pb.n_out, fl,
+                                       expect=A.E_INVAL)
             except A.DraError as e:                      # refused on the host: nothing was enqueued on any rank
                 assert e.code == A.E_INVAL, what
                 outs = None
             if outs is not None:
-                for r, c in enumerate(W.ctxs):
-                    with pytest.raises(A.DraError) as e:
-                        c.sync()
-                    assert e.value.code == A.E_INVAL, (what, r)
                 for r, o in enumerate(outs):
-                    assert all((t.cpu().numpy() == 0x5C).all() for t in o), f"{what}: rank {r} wrote an output"
+                    assert all((h == 0x5C).all() for h in o), f"{what}: rank {r} wrote an output"
         else:
-            W.check(pb.claims, pb.pod_off, pb.prio, ra, run, cands, fl, what, (pb.out_off, pb.n_out), pb.run_out_off)
+            _check_sharded(W, pb, pb.claims, pb.pod_off, pb.prio, ra, run, cands, fl, what, (pb.out_off, pb.n_out),
+                           pb.run_out_off)
         for r, c in enumerate(W.ctxs):
             if pb.error:
                 assert c.get_inventory().tobytes() == pb.gpus.tobytes(), f"{what}: rank {r}'s live inventory changed"

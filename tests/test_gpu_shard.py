@@ -6,12 +6,9 @@ the sort path, bit-exact with the oracle on the global batch."""
 import numpy as np
 import pytest
 
+import shard_world as S
+
 pytestmark = pytest.mark.gpu
-
-
-def _dev(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).copy()).to("cuda:0")
 
 
 def _make_world(pkg, world, flags=0):
@@ -41,8 +38,8 @@ def test_sharded_global_batch(pkg, oracle, world, cfg_flags, seed, monkeypatch):
             c.shard_export(w.n_out, 0, want_handle=False)
         for c in ctxs:
             c.peer_import_local(ctxs)
-        d_claims = _dev(w.claims)
-        d_off = None if out_off is None else _dev(out_off)
+        d_claims = S.dev(w.claims)
+        d_off = None if out_off is None else S.dev(out_off)
         ref, ref_inv = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, out_off, w.n_out)
         for rep in range(4):                                             # repeated calls: parity double-buffering, plan from the hint
             l0 = ctxs[0].launch_count()
@@ -69,7 +66,7 @@ def test_sharded_global_batch_world1_and_empty_shards(pkg, oracle):
     ref, _ = oracle.allocate(w.gpus, w.node_off, w.table, w.claims)
     with pkg.api.Context(device=0) as c:
         c.set_table(w.table); c.set_inventory(w.gpus, w.node_off); c.set_shard(0, w.n_node, True)
-        d = _dev(w.claims)
+        d = S.dev(w.claims)
         c.allocate_global_device(d.data_ptr(), w.n_claim, None, w.n_out, pkg.api.F_FRESH_INVENTORY)
         assert c.gather_read(np.zeros(w.n_out, dtype=R.OUT_DTYPE)).tobytes() == ref.tobytes()
     ctxs = _make_world(pkg, 3)
@@ -80,7 +77,7 @@ def test_sharded_global_batch_world1_and_empty_shards(pkg, oracle):
             c.shard_export(w.n_out, 0, want_handle=False)
         for c in ctxs:
             c.peer_import_local(ctxs)
-        d = _dev(w.claims)
+        d = S.dev(w.claims)
         for _ in range(3):
             for c in ctxs:
                 c.allocate_global_device(d.data_ptr(), w.n_claim, None, w.n_out, pkg.api.F_FRESH_INVENTORY)
@@ -90,7 +87,7 @@ def test_sharded_global_batch_world1_and_empty_shards(pkg, oracle):
         # fails WITHOUT touching anything ("call again"), the peers are told at once (no time-out), the retry succeeds.
         w2 = pkg.synth.cfg2(3000, 12); w2.claims["node"] = 5 + w2.claims["node"] % 7
         ref2, _ = oracle.allocate(w2.gpus, w2.node_off, w2.table, w2.claims)
-        d2 = _dev(w2.claims)
+        d2 = S.dev(w2.claims)
         for c in ctxs:
             c.allocate_global_device(d2.data_ptr(), w2.n_claim, None, w2.n_out, pkg.api.F_FRESH_INVENTORY)
         errs = []
@@ -124,8 +121,8 @@ def test_per_rank_slices_gather(pkg, oracle, world, nofused):
             c._check(c._lib.dra_peer_export(c._h, n_per, (__import__("ctypes").c_uint8 * 64)()))
         for c in ctxs:
             c.peer_import_local(ctxs)
-        dc = [_dev(lb.claims) for lb in lbs]
-        do = [_dev(lb.out_off) for lb in lbs]
+        dc = [S.dev(lb.claims) for lb in lbs]
+        do = [S.dev(lb.out_off) for lb in lbs]
         ref, _ = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out)
         for rep in range(3):
             for c, lb, a, b in zip(ctxs, lbs, dc, do):
@@ -174,40 +171,6 @@ def test_device_rendezvous_of_world_contexts(pkg):
 # it matters: the kept claims' positions among dropped ones.  The shard writes the OutRecs of its kept claims only; those
 # slots, and the shard's slice of the inventory, must be the oracle's answer to the whole batch (nodes are independent).
 
-def _kept(w, lo, hi, stray):
-    node = w.claims["node"].astype(np.int64)
-    return np.where(node >= w.n_node, bool(stray), (node >= lo) & (node < hi))
-
-
-def _slots_of(pkg, w, keep):
-    """OutRec slots of the claims in `keep` (bool mask over the claims)."""
-    sl = pkg.records.claim_slots(w.claims, w.n_node).astype(np.int64)
-    start = (np.arange(w.n_claim) if w.out_off is None else w.out_off.astype(np.int64))[keep]
-    n = sl[keep]
-    first = np.repeat(np.cumsum(n) - n, n)
-    m = np.zeros(w.n_out, dtype=bool)
-    m[np.repeat(start, n) + np.arange(int(n.sum())) - first] = True
-    return m
-
-
-def _shard_call(pkg, c, w, d_claims, d_off, lo, hi, stray, ref, ref_inv, what):
-    """One sharded call on [lo, hi): kept slots and the shard's inventory slice against the oracle, the rest untouched."""
-    R = pkg.records
-    c.allocate_global_device(d_claims.data_ptr(), w.n_claim, None if d_off is None else d_off.data_ptr(), w.n_out,
-                             pkg.api.F_FRESH_INVENTORY)
-    got = c.gather_read(np.zeros(w.n_out, dtype=R.OUT_DTYPE))
-    keep = _kept(w, lo, hi, stray)
-    assert 0 < keep.sum() < w.n_claim, f"{what}: the shard must keep some claims and drop others"
-    m = _slots_of(pkg, w, keep)
-    if got[m].tobytes() != ref[m].tobytes():
-        bad = np.nonzero(got.view(np.uint64)[m] != ref.view(np.uint64)[m])[0]
-        raise AssertionError(f"{what}: {len(bad)} kept OutRecs differ, first at slot {np.nonzero(m)[0][bad[0]]}")
-    inv = c.get_inventory()
-    g0, g1 = int(w.node_off[lo]), int(w.node_off[hi])
-    assert inv[g0:g1].tobytes() == ref_inv[g0:g1].tobytes(), f"{what}: shard inventory differs"
-    return got, m, c.last_chain()
-
-
 @pytest.mark.parametrize("n_claim,compaction", [(262_144, "compact_flat1"), (262_145, "compact_flat8"),
                                                 (2_097_152, "compact_flat8"), (2_097_153, "compact_lookback")])
 def test_shard_compaction_forms_drop_claims(pkg, oracle, n_claim, compaction):
@@ -216,8 +179,8 @@ def test_shard_compaction_forms_drop_claims(pkg, oracle, n_claim, compaction):
     ref, ref_inv = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out, threads=8)
     with pkg.api.Context(device=0) as c:
         c.set_table(w.table); c.set_inventory(w.gpus, w.node_off); c.set_shard(500, 1_300, take_stray=True)
-        d, o = _dev(w.claims), _dev(w.out_off)
-        _, _, chain = _shard_call(pkg, c, w, d, o, 500, 1_300, True, ref, ref_inv, f"{n_claim} claims")
+        d, o = S.dev(w.claims), S.dev(w.out_off)
+        _, _, chain = S.shard_call(pkg, c, w, d, o, 500, 1_300, True, ref, ref_inv, f"{n_claim} claims")
         assert compaction in chain, chain
         outside = np.ones(w.n_gpu, dtype=bool); outside[int(w.node_off[500]):int(w.node_off[1_300])] = False
         assert c.get_inventory()[outside].tobytes() == w.gpus[outside].tobytes(), "a GPU outside the shard changed"
@@ -232,10 +195,10 @@ def test_three_shards_cover_the_inventory(pkg, oracle):
     covered = np.zeros(w.n_out, dtype=bool)
     with pkg.api.Context(device=0) as c:
         c.set_table(w.table); c.set_inventory(w.gpus, w.node_off)
-        d, o = _dev(w.claims), _dev(w.out_off)
+        d, o = S.dev(w.claims), S.dev(w.out_off)
         for lo, hi, stray in ((0, 400, False), (400, 1_111, True), (1_111, 1_500, False)):
             c.set_shard(lo, hi, take_stray=stray)
-            got, m, chain = _shard_call(pkg, c, w, d, o, lo, hi, stray, ref, ref_inv, f"shard [{lo}, {hi})")
+            got, m, chain = S.shard_call(pkg, c, w, d, o, lo, hi, stray, ref, ref_inv, f"shard [{lo}, {hi})")
             assert "compact_flat8" in chain, chain
             assert not (covered & m).any()
             merged[m] = got[m]; covered |= m
@@ -250,11 +213,11 @@ def test_plan_hint_takes_the_staged_kernel_on_a_narrow_shard(pkg, oracle):
     ref, ref_inv = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out, threads=8)
     with pkg.api.Context(device=0) as c:
         c.set_table(w.table); c.set_inventory(w.gpus, w.node_off); c.set_shard(960, 1_000, take_stray=False)
-        d, o = _dev(w.claims), _dev(w.out_off)
-        _, _, first = _shard_call(pkg, c, w, d, o, 960, 1_000, False, ref, ref_inv, "first call")
+        d, o = S.dev(w.claims), S.dev(w.out_off)
+        _, _, first = S.shard_call(pkg, c, w, d, o, 960, 1_000, False, ref, ref_inv, "first call")
         assert "compact_flat8" in first and not first & {"fused_staged", "fused_stream"}, first
         for rep in range(2):
-            _, _, chain = _shard_call(pkg, c, w, d, o, 960, 1_000, False, ref, ref_inv, f"planned call {rep}")
+            _, _, chain = S.shard_call(pkg, c, w, d, o, 960, 1_000, False, ref, ref_inv, f"planned call {rep}")
             assert chain == {"compact_flat8", "fused_staged"}, chain
 
 
@@ -265,13 +228,13 @@ def test_shard_beyond_the_cta_wide_histogram_is_an_error(pkg, oracle):
     ref, ref_inv = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out)
     with pkg.api.Context(device=0) as c:
         c.set_table(w.table); c.set_inventory(w.gpus, w.node_off); c.set_shard(0, 12_799, take_stray=True)
-        d, o = _dev(w.claims), _dev(w.out_off)
+        d, o = S.dev(w.claims), S.dev(w.out_off)
         with pytest.raises(pkg.api.DraError) as e:
             c.allocate_global_device(d.data_ptr(), w.n_claim, o.data_ptr(), w.n_out, pkg.api.F_FRESH_INVENTORY)
         assert e.value.code == pkg.api.E_INVAL
         assert c.get_inventory().tobytes() == w.gpus.tobytes()
         c.set_shard(0, 12_798, take_stray=True)
-        _, _, chain = _shard_call(pkg, c, w, d, o, 0, 12_798, True, ref, ref_inv, "12,798 local nodes")
+        _, _, chain = S.shard_call(pkg, c, w, d, o, 0, 12_798, True, ref, ref_inv, "12,798 local nodes")
         assert {"compact_flat1", "hist8", "scan8"} <= chain, chain
 
 
@@ -291,15 +254,15 @@ def test_shard_status_words_do_not_alias_after_1024_calls(pkg, oracle):
     with pkg.api.Context(device=0) as c:
         c.set_table(x.table); c.set_inventory(x.gpus, x.node_off); c.set_shard(0, 200, take_stray=True)
         rx, rx_inv = oracle.allocate(x.gpus, x.node_off, x.table, x.claims, x.out_off, x.n_out, threads=8)
-        dx, ox = _dev(x.claims), _dev(x.out_off)
-        _shard_call(pkg, c, x, dx, ox, 0, 200, True, rx, rx_inv, "first large call")
-        ds, os_ = _dev(small.claims), _dev(small.out_off)
+        dx, ox = S.dev(x.claims), S.dev(x.out_off)
+        S.shard_call(pkg, c, x, dx, ox, 0, 200, True, rx, rx_inv, "first large call")
+        ds, os_ = S.dev(small.claims), S.dev(small.out_off)
         for _ in range(1_023):
             c.allocate_global_device(ds.data_ptr(), small.n_claim, os_.data_ptr(), small.n_out, pkg.api.F_FRESH_INVENTORY)
         c.sync()
         ry, ry_inv = oracle.allocate(y.gpus, y.node_off, y.table, y.claims, y.out_off, y.n_out, threads=8)
-        dy, oy = _dev(y.claims), _dev(y.out_off)
-        _, _, chain = _shard_call(pkg, c, y, dy, oy, 0, 200, True, ry, ry_inv, "large call 1,024 epochs later")
+        dy, oy = S.dev(y.claims), S.dev(y.out_off)
+        _, _, chain = S.shard_call(pkg, c, y, dy, oy, 0, 200, True, ry, ry_inv, "large call 1,024 epochs later")
         assert "compact_flat1" in chain
 
 

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 from test_gpu_pod_call_checks import _world
-from test_gpu_shard_preempt import _dev
+import shard_world as S
 
 pytestmark = pytest.mark.gpu
 SENTINEL = 0xA7
@@ -22,33 +22,24 @@ OUT_BYTES = 256                                            # each output buffer,
 
 def _setup(pkg, w, world, shard="map", export=True, sizes=True, inv=True, n_out_max=64):
     """world contexts serving the two-node inventory of w, rank r node r.  shard: "map", "bare" (dra_set_shard) or None;
-    sizes: the five setters called before the export (False: none); inv: the inventory loaded before the export."""
-    ctxs = [pkg.api.Context(device=0) for _ in range(world)]
+    sizes: the five setters called before the export (False: none); inv False: a world of 2 whose inventory and map are
+    loaded after the export, so no staging was reserved for it."""
     bounds = [0, 1, 2] if world == 2 else [0, 2]
+    if inv:
+        sz = dict(pairs=64, place=8, preempt=(8, 64, 8), capacity=64, preempt_place=(8, 64, 8)) if sizes else {}
+        return S.World(pkg, w.t, w.off, w.g, world, None if shard is None else bounds, bare=shard == "bare", export=export,
+                       n_out_max=n_out_max, **sz).ctxs
+    ctxs = [pkg.api.Context(device=0) for _ in range(world)]
     for r, c in enumerate(ctxs):
         c.comm_init_local(r, world)
         c.set_table(w.t)
-        if inv:
-            c.set_inventory(w.g, w.off)
-        if shard == "map" and inv:
-            c.set_shard_map(bounds, stray_rank=0)
-        elif shard == "bare" and inv:
-            c.set_shard(bounds[r], bounds[r + 1], r == 0)
-        if sizes:
-            c.set_shard_pairs(64)
-            c.set_shard_place(8)
-            c.set_shard_preempt(8, 64, 8)
-            c.set_shard_capacity(64)
-            c.set_shard_preempt_place(8, 64, 8)
-        if world > 1 and export:
-            c.shard_export(n_out_max, 0, want_handle=False)
-        if not inv:                                        # loaded after the export: no staging was reserved for it
-            c.set_inventory(w.g, w.off)
-            if shard == "map":
-                c.set_shard_map(bounds, stray_rank=0)
-    if world > 1 and export:
-        for c in ctxs:
-            c.peer_import_local(ctxs)
+        c.set_shard_pairs(64); c.set_shard_place(8); c.set_shard_preempt(8, 64, 8); c.set_shard_capacity(64)
+        c.set_shard_preempt_place(8, 64, 8)
+        c.shard_export(n_out_max, 0, want_handle=False)
+        c.set_inventory(w.g, w.off)
+        c.set_shard_map(bounds, stray_rank=0)
+    for c in ctxs:
+        c.peer_import_local(ctxs)
     return ctxs
 
 
@@ -64,9 +55,9 @@ class Call:
         import torch
         c = w.c.copy()
         c["node"] = [0, 1]                                 # pods Allocate: each pod names its node
-        self.keep = {"c": _dev(w.c), "ca": _dev(c), "po": _dev(w.po), "prio": _dev(w.prio), "cn": _dev(np.array([0, 1, 1], np.uint32)),
-                     "co": _dev(np.array([0, 2, 3], np.uint32))}
-        self.run_keep = [_dev(w.rc), _dev(w.rpo), _dev(w.rpr), _dev(w.ro)]
+        self.keep = {"c": S.dev(w.c), "ca": S.dev(c), "po": S.dev(w.po), "prio": S.dev(w.prio), "cn": S.dev(np.array([0, 1, 1], np.uint32)),
+                     "co": S.dev(np.array([0, 2, 3], np.uint32))}
+        self.run_keep = [S.dev(w.rc), S.dev(w.rpo), S.dev(w.rpr), S.dev(w.ro)]
         self.run = pkg.api.RunningPods(self.run_keep[0].data_ptr(), len(w.rc), self.run_keep[1].data_ptr(), len(w.rpo) - 1,
                                        self.run_keep[2].data_ptr(), None, self.run_keep[3].data_ptr(), len(w.ro))
         self.outs = [torch.full((OUT_BYTES,), SENTINEL, dtype=torch.uint8, device="cuda:0") for _ in range(6)]

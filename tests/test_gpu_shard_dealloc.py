@@ -3,83 +3,24 @@ device, wired like test_gpu_shard_sync.py.  The CPU oracle runs spec §9 on ONE 
 Deallocate (a) every rank's own GPU range equals the oracle's state byte for byte, (b) every GPU outside a rank's range is
 byte for byte what that rank held before the call, and (c) after an inventory sync every rank's whole inventory equals the
 oracle's."""
-import ctypes as C
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-from test_gpu_shard_pods import PodWorld, _malformed_mixed
-from test_gpu_shard_sync import SyncWorld, _check_tables, _shared_mixed
-from test_gpu_shard_unsuitable import _bounds, _candidates, _dense, _dev
+import shard_world as S
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _devp(a):
-    """_dev, with room for at least one record even when `a` is empty (a non-null pointer)."""
-    import torch
-    return _dev(a) if len(a) else torch.zeros(16, dtype=torch.uint8, device="cuda:0")
-
-
-def _table_ptr(c):
-    """Device pointer of the context's last gathered table (dra_gather_table)."""
-    p, n = C.c_void_p(), C.c_uint32()
-    rc = c._lib.dra_gather_table(c._h, C.byref(p), C.byref(n))
-    assert rc == 0, rc
-    return p.value
-
-
-class DeallocWorld(SyncWorld):
-    """SyncWorld plus the sharded Deallocate, checked against the oracle after every call."""
-
-    def enqueue_release(self, claims, out_off, n_out, out=None, ptrs=None):
-        """The call on every rank: `out` is one OutRec array uploaded for all ranks, or `ptrs` one device pointer per rank
-        (each rank's gathered table).  Returns the buffers to keep alive until the ranks are synced."""
-        import torch
-        keep = [_devp(claims), _devp(out_off) if out_off is not None else None]
-        if ptrs is None:
-            keep.append(_devp(out))
-            ptrs = [keep[2].data_ptr()] * len(self.ctxs)
-        torch.cuda.synchronize()                         # (the contexts' streams do not wait for torch's)
-        for c, p in zip(self.ctxs, ptrs):
-            c.deallocate_global_device(keep[0].data_ptr(), len(claims), keep[1].data_ptr() if keep[1] is not None else None,
-                                       p, n_out)
-        return keep
-
-    def release(self, claims, out_off, n_out, state, what, out=None, ptrs=None):
-        """One sharded Deallocate on every rank; `state` is the oracle's state after it.  Checks (a) and (b) and that the
-        call enqueued exactly two kernels on every rank."""
-        before, l0 = self.inventories(), [c.launch_count() for c in self.ctxs]
-        keep = self.enqueue_release(claims, out_off, n_out, out, ptrs)
-        for c in self.ctxs:
-            c.sync()
-        del keep
-        assert [c.launch_count() - l for c, l in zip(self.ctxs, l0)] == [2] * len(self.ctxs), f"{what}: launches"
-        self.assert_release(before, state, what)
-
-    def assert_release(self, before, state, what):
-        for r, (b, a) in enumerate(zip(before, self.inventories())):
-            g0, g1 = self.gpu_range(r)
-            assert a[g0:g1].tobytes() == state[g0:g1].tobytes(), f"{what}: rank {r} own range differs from the oracle"
-            assert a[:g0].tobytes() == b[:g0].tobytes() and a[g1:].tobytes() == b[g1:].tobytes(), \
-                f"{what}: rank {r} wrote GPUs outside its range"
-
-    def assert_synced(self, state, what):
-        """(c): after an inventory sync every rank holds the oracle's whole inventory (world 1: no sync is needed)."""
-        if len(self.ctxs) > 1:
-            self.sync_inventory()
-        for r, inv in enumerate(self.inventories()):
-            assert inv.tobytes() == state.tobytes(), f"{what}: rank {r} inventory after the sync differs from the oracle"
+def _world(pkg, w, world, bounds, stray_rank, max_pairs=None):
+    return S.World(pkg, w.table, w.node_off, w.gpus, world, bounds, stray_rank, n_out_max=1 << 16, pairs=max_pairs)
 
 
 def _pods_allocate(pkg, oracle, W, w, rng, state, flags, oflags):
-    pc, po, poo, pn = _malformed_mixed(pkg, w, W.bounds, rng, True)
+    pc, po, poo, pn = S.malformed_mixed(pkg, w, W.bounds, rng, True)
     ref, state = oracle.allocate_pods(state, w.node_off, w.table, pc, po, poo, pn, oflags)
-    _check_tables(W.call(pc, po, poo, pn, flags), ref, f"sharded pods Allocate flags {flags}")
+    S.same_tables(S.pods(W, pc, po, poo, pn, flags), ref, f"sharded pods Allocate flags {flags}")
     return pc, poo, pn, ref, state
 
 
@@ -92,22 +33,22 @@ def test_mixed_sequence_released_from_gathered_tables(pkg, oracle, world):
     rng = np.random.default_rng(300 + world)
     w = pkg.synth.mixed(2400, 31, 170 + world, invalid=True)
     kind = {1: "even", 2: "uneven", 3: "empty", 4: "uneven"}[world]
-    W = DeallocWorld(pkg, w, world, _bounds(w.n_node, world, kind), world - 1)
+    W = _world(pkg, w, world, S.bounds(w.n_node, world, kind), world - 1)
     try:
         state = w.gpus.copy()
-        claims = _shared_mixed(pkg, w, rng)
+        claims = S.shared_mixed(pkg, w, rng)
         out_off, n_out = R.out_offsets(claims, w.n_node)
         ref, state = oracle.allocate(state, w.node_off, w.table, claims, out_off, int(n_out))
-        _check_tables(W.allocate(claims, out_off, int(n_out)), ref, "sharded Allocate")
+        S.same_tables(S.allocate(W, claims, out_off, int(n_out)), ref, "sharded Allocate")
         shared_ok = (ref["status"] == R.ST_OK) & (ref["profile"] == R.PROFILE_SHARED)
         assert shared_ok.any() and (ref["size"][ref["status"] == R.ST_OK] > 0).any()
         state = oracle.deallocate(state, claims, ref, out_off, n_node=w.n_node)
-        W.release(claims, out_off, int(n_out), state, "release of the Allocate", ptrs=[_table_ptr(c) for c in W.ctxs])
+        S.deallocate(W, claims, out_off, int(n_out), state, "release of the Allocate", ptrs=[S.table_ptr(c) for c in W.ctxs])
         for flags, oflags in ((0, 0), (api.F_EXHAUSTIVE, oracle.F_EXHAUSTIVE)):
             pc, poo, pn, ref, state = _pods_allocate(pkg, oracle, W, w, rng, state, flags, oflags)
             assert (ref["status"] == R.ST_OK).any()
             state = oracle.deallocate(state, pc, ref, poo, n_node=w.n_node)
-            W.release(pc, poo, pn, state, f"release of the pods flags {flags}", ptrs=[_table_ptr(c) for c in W.ctxs])
+            S.deallocate(W, pc, poo, pn, state, f"release of the pods flags {flags}", ptrs=[S.table_ptr(c) for c in W.ctxs])
         for r, inv in enumerate(W.inventories()):
             assert (inv["share_cnt"] < 0x8000).all(), f"rank {r}: a share count wrapped"
         assert state.tobytes() == w.gpus.tobytes(), "releasing every table must give back the loaded inventory"
@@ -125,37 +66,37 @@ def test_release_a_subset_then_allocate_and_unsuitable(pkg, oracle, world):
     rng = np.random.default_rng(40 + world)
     w = pkg.synth.mixed(3000, 29, 60 + world, invalid=True)
     n_pod_uns = 200
-    W = DeallocWorld(pkg, w, world, _bounds(w.n_node, world, "uneven" if world == 3 else "even"), world - 1,
+    W = _world(pkg, w, world, S.bounds(w.n_node, world, "uneven" if world == 3 else "even"), world - 1,
                      max_pairs=n_pod_uns * w.n_node)
     try:
-        claims = _shared_mixed(pkg, w, rng)
+        claims = S.shared_mixed(pkg, w, rng)
         out_off, n_out = R.out_offsets(claims, w.n_node)
         ref, full = oracle.allocate(w.gpus, w.node_off, w.table, claims, out_off, int(n_out))
-        _check_tables(W.allocate(claims, out_off, int(n_out)), ref, "sharded Allocate")
+        S.same_tables(S.allocate(W, claims, out_off, int(n_out)), ref, "sharded Allocate")
         sel = np.sort(rng.choice(len(claims), len(claims) // 3, replace=False))
         sub, sub_off = claims[sel].copy(), out_off[sel].copy()
         state = oracle.deallocate(full, sub, ref, sub_off, n_node=w.n_node)
         assert state.tobytes() != full.tobytes()
-        W.release(sub, sub_off, int(n_out), state, "subset release", ptrs=[_table_ptr(c) for c in W.ctxs])
+        S.deallocate(W, sub, sub_off, int(n_out), state, "subset release", ptrs=[S.table_ptr(c) for c in W.ctxs])
         slots = R.claim_slots(sub, w.n_node)
         freed = {int(ref["gpu"][int(o) + k]) for o, s in zip(sub_off, slots) for k in range(int(s))
                  if ref["status"][int(o) + k] == R.ST_OK}
-        c2 = _shared_mixed(pkg, w, rng)
+        c2 = S.shared_mixed(pkg, w, rng)
         o2, n2 = R.out_offsets(c2, w.n_node)
         ref2, state2 = oracle.allocate(state, w.node_off, w.table, c2, o2, int(n2))
         assert ref2.tobytes() != oracle.allocate(full, w.node_off, w.table, c2, o2, int(n2))[0].tobytes()
-        _check_tables(W.allocate(c2, o2, int(n2)), ref2, "sharded Allocate after the release")
+        S.same_tables(S.allocate(W, c2, o2, int(n2)), ref2, "sharded Allocate after the release")
         assert freed & set(ref2["gpu"][ref2["status"] == R.ST_OK].tolist()), "the freed capacity was not reused"
         uc = c2[:900]
         upo = np.unique(np.concatenate([[0, 900], rng.integers(0, 900, n_pod_uns - 20)])).astype(np.uint32)
         n_pod = len(upo) - 1
-        cn, co = _candidates(rng, n_pod, w.n_node)
+        cn, co = S.candidates(rng, n_pod, w.n_node)
         for flags, oflags in ((0, 0), (api.F_EXHAUSTIVE, oracle.F_EXHAUSTIVE)):
-            for name, dn, do, on, oo in (("dense", None, None) + _dense(n_pod, w.n_node), ("candidates", cn, co, cn, co)):
+            for name, dn, do, on, oo in (("dense", None, None) + S.dense(n_pod, w.n_node), ("candidates", cn, co, cn, co)):
                 want = oracle.unsuitable(state2, w.node_off, w.table, uc, upo, on, oo, flags=oflags)
-                for r, b in enumerate(W.unsuitable(uc, upo, dn, do, flags)):
+                for r, b in enumerate(S.unsuitable(W, uc, upo, None if dn is None else (dn, do), flags)):
                     assert b.tobytes() == want.tobytes(), f"UnsuitableNodes {name} flags {flags}: rank {r} differs"
-        W.assert_own_ranges(state2, "after the further Allocate")
+        W.assert_ranges(None, state2, "after the further Allocate")
         W.assert_synced(state2, "after the release and the further calls")
     finally:
         W.close()
@@ -175,7 +116,7 @@ def test_no_peer_is_waited_for(pkg, oracle):
             c.comm_init_local(r, 3)
             c.set_table(w.table); c.set_inventory(loaded, w.node_off)
             c.set_shard(bounds[r], bounds[r + 1], take_stray=r == 0)
-        d = [_devp(w.claims), _devp(w.out_off), _devp(ref)]
+        d = [S.dev(w.claims), S.dev(w.out_off), S.dev(ref)]
         import torch
         torch.cuda.synchronize()
         for r, c in enumerate(ctxs):
@@ -210,11 +151,11 @@ def test_slots_counted_on_the_whole_inventory(pkg, oracle, bounds):
     out["start"], out["size"], out["profile"], out["status"] = [0, 0, 0, 0, 2], [0, 0, 0, 0, 2], [0xFF] * 4 + [1], R.ST_OK
     w = type("W", (), {})()
     w.gpus, w.node_off, w.table, w.n_node = gpus, node_off, R.default_table(), 4
-    W = DeallocWorld(pkg, w, len(bounds) - 1, bounds, len(bounds) - 2)
+    W = _world(pkg, w, len(bounds) - 1, bounds, len(bounds) - 2)
     try:
         want = oracle.deallocate(gpus, claims, out, out_off, n_node=4)
         assert not (want["flags"][[0, 1, 2, 13]] & R.GPU_FULL_ALLOCATED).any() and want["busy"][3] == 0xF3
-        W.release(claims, out_off, 5, want, f"bounds {bounds}", out=out)
+        S.deallocate(W, claims, out_off, 5, want, f"bounds {bounds}", out=out)
         W.assert_synced(want, f"bounds {bounds}")
     finally:
         W.close()
@@ -252,10 +193,10 @@ def test_many_ctas_with_contended_atomics(pkg, oracle):
     gpus, node_off, claims, out_off, n_out, out = _contended(pkg, rng, 128, 8, 240_000)
     w = type("W", (), {})()
     w.gpus, w.node_off, w.table, w.n_node = gpus, node_off, pkg.records.default_table(), len(node_off) - 1
-    W = DeallocWorld(pkg, w, 3, [0, 30, 31, 128], 1)
+    W = _world(pkg, w, 3, [0, 30, 31, 128], 1)
     try:
         state = oracle.deallocate(gpus, claims, out, out_off, n_node=w.n_node)
-        W.release(claims, out_off, n_out, state, "contended release", out=out)
+        S.deallocate(W, claims, out_off, n_out, state, "contended release", out=out)
         W.assert_synced(state, "contended release")
     finally:
         W.close()
@@ -301,12 +242,12 @@ def test_world1_equals_deallocate_batch(pkg, oracle, with_off):
     assert (out["status"] == R.ST_OK).sum() > n_out // 2
     w1 = type("W", (), {})()
     w1.gpus, w1.node_off, w1.table, w1.n_node = loaded, w.node_off, w.table, w.n_node
-    W = DeallocWorld(pkg, w1, 1, [0, w.n_node], 0)
+    W = _world(pkg, w1, 1, [0, w.n_node], 0)
     with pkg.api.Context(device=0) as single:
         single.set_table(w.table); single.set_inventory(loaded, w.node_off)
         try:
             want = oracle.deallocate(loaded, claims, out, out_off, n_node=w.n_node)
-            W.release(claims, out_off, n_out, want, "world 1", out=out)
+            S.deallocate(W, claims, out_off, n_out, want, "world 1", out=out)
             single.deallocate(claims, out, out_off)
             assert W.ctxs[0].get_inventory().tobytes() == single.get_inventory().tobytes()
             assert want.tobytes() != loaded.tobytes()
@@ -356,15 +297,16 @@ def test_problems_replayed_sharded(pkg, oracle, world):
                 assert moved["size"][k] <= 16
             w = type("W", (), {})()
             w.gpus, w.node_off, w.table, w.n_node = loaded, off, t, n_node
-            W = DeallocWorld.__new__(DeallocWorld)
-            W.pkg, W.w, W.world, W.bounds, W.ctxs = pkg, w, world, bounds, ctxs
+            W = S.World.__new__(S.World)                 # the contexts above, on this problem's inventory and ranges
+            W.pkg, W.table, W.node_off, W.n_node, W.world, W.bounds, W.ctxs, W.loaded = \
+                pkg, t, off, n_node, world, bounds, ctxs, [loaded] * world
             for recs, what in ((ref, "the Allocate's records"), (moved, "moved records")):
                 for x in ctxs:
                     x.set_table(t); x.set_inventory(loaded, off); x.set_shard_map(bounds, stray_rank=stray)
                 if len(c) == 0:
                     continue
                 want = oracle.deallocate(loaded, c, recs, out_off, n_node=n_node)
-                W.release(c, out_off, n_out, want, f"{what}, bounds {bounds}", out=recs[:n_out])
+                S.deallocate(W, c, out_off, n_out, want, f"{what}, bounds {bounds}", out=recs[:n_out])
                 W.assert_synced(want, f"{what}, bounds {bounds}")
 
         run()
@@ -386,7 +328,7 @@ def test_pinned_host_buffers(pkg, oracle):
     want = oracle.deallocate(loaded, claims, ref, out_off, n_node=w.n_node)
     got = []
     for pinned in (True, False):
-        W = DeallocWorld(pkg, w1, 3, [0, 4, 17, 31], 2)
+        W = _world(pkg, w1, 3, [0, 4, 17, 31], 2)
         try:
             if pinned:
                 bufs = [api.PinnedBuffer(len(claims), R.CLAIM_DTYPE), api.PinnedBuffer(len(out_off), np.uint32),
@@ -394,16 +336,13 @@ def test_pinned_host_buffers(pkg, oracle):
                 for b, a in zip(bufs, (claims, out_off, ref[:n_out])):
                     b.array[:] = a
                 before, l0 = W.inventories(), [c.launch_count() for c in W.ctxs]
-                for c in W.ctxs:
-                    c.deallocate_global_device(bufs[0].ptr, len(claims), bufs[1].ptr, bufs[2].ptr, n_out)
-                for c in W.ctxs:
-                    c.sync()
+                W.each(lambda r, c: c.deallocate_global_device(bufs[0].ptr, len(claims), bufs[1].ptr, bufs[2].ptr, n_out))
                 assert all(c.launch_count() == l + 2 for c, l in zip(W.ctxs, l0))
-                W.assert_release(before, want, "pinned buffers")
+                W.assert_ranges(before, want, "pinned buffers")
                 for b in bufs:
                     b.free()
             else:
-                W.release(claims, out_off, n_out, want, "device pointers", out=ref[:n_out])
+                S.deallocate(W, claims, out_off, n_out, want, "device pointers", out=ref[:n_out])
             got.append(W.inventories())
             W.assert_synced(want, "pinned" if pinned else "device")
         finally:
@@ -420,37 +359,29 @@ def test_bad_slot_range_changes_nothing(pkg, oracle, world):
     R, api = pkg.records, pkg.api
     rng = np.random.default_rng(8 + world)
     w = pkg.synth.mixed(2400, 31, 44, invalid=True)
-    W = DeallocWorld(pkg, w, world, _bounds(w.n_node, world, "uneven"), 0)
+    W = _world(pkg, w, world, S.bounds(w.n_node, world, "uneven"), 0)
     try:
-        claims = _shared_mixed(pkg, w, rng)
+        claims = S.shared_mixed(pkg, w, rng)
         claims["kind"][-1], claims["count"][-1], claims["node"][-1] = R.KIND_GPU, 2, 3
         out_off, n_out = R.out_offsets(claims, w.n_node)
         n_out = int(n_out)
         ref, state = oracle.allocate(w.gpus, w.node_off, w.table, claims, out_off, n_out)
-        _check_tables(W.allocate(claims, out_off, n_out), ref, "sharded Allocate")
+        S.same_tables(S.allocate(W, claims, out_off, n_out), ref, "sharded Allocate")
         first, last = out_off.copy(), out_off.copy()
         first[0] = n_out                                       # one slot at n_out
         last[-1] = n_out - 1                                   # two slots from n_out - 1
         for bad, what in ((first, "first"), (last, "last")):
             before = W.inventories()
-            keep = W.enqueue_release(claims, bad, n_out, out=ref)
-            codes = []
-            for c in W.ctxs:
-                try:
-                    c.sync(); codes.append(0)
-                except api.DraError as e:
-                    codes.append(e.code)
-            del keep
-            assert codes == [api.E_INVAL] * world, (what, codes)
+            S.deallocate(W, claims, bad, n_out, out=ref, expect=api.E_INVAL)
             for r, (b, a) in enumerate(zip(before, W.inventories())):
                 assert a.tobytes() == b.tobytes(), f"bad slot range {what}: rank {r} inventory changed"
         state = oracle.deallocate(state, claims, ref, out_off, n_node=w.n_node)
-        W.release(claims, out_off, n_out, state, "after the refused calls", out=ref)
-        c2 = _shared_mixed(pkg, w, rng)
+        S.deallocate(W, claims, out_off, n_out, state, "after the refused calls", out=ref)
+        c2 = S.shared_mixed(pkg, w, rng)
         o2, n2 = R.out_offsets(c2, w.n_node)
         ref2, state2 = oracle.allocate(w.gpus, w.node_off, w.table, c2, o2, int(n2))
-        _check_tables(W.allocate(c2, o2, int(n2), api.F_FRESH_INVENTORY), ref2, "fresh Allocate")
-        W.assert_own_ranges(state2, "fresh Allocate")
+        S.same_tables(S.allocate(W, c2, o2, int(n2), api.F_FRESH_INVENTORY), ref2, "fresh Allocate")
+        W.assert_ranges(None, state2, "fresh Allocate")
     finally:
         W.close()
 
@@ -461,7 +392,7 @@ def test_refusals_and_empty_calls(pkg):
     R, api = pkg.records, pkg.api
     w = pkg.synth.mixed(600, 11, 3, invalid=True)
     small = pkg.synth.mixed(200, 5, 4, invalid=True)
-    d_c, d_o, d_r = _devp(w.claims), _devp(w.out_off), _devp(np.zeros(int(w.n_out), dtype=R.OUT_DTYPE))
+    d_c, d_o, d_r = S.dev(w.claims), S.dev(w.out_off), S.dev(np.zeros(int(w.n_out), dtype=R.OUT_DTYPE))
     torch.cuda.synchronize()
 
     def raw(c, **k):
@@ -494,17 +425,3 @@ def test_refusals_and_empty_calls(pkg):
         n = c.launch_count()
         assert raw(c, n_claim=0) == api.OK and c.launch_count() == n
         c.sync()
-
-
-def test_multi_process_dealloc():
-    """tests/multi_gpu_shard_dealloc_check.py under torchrun: one process per GPU, peers mapped with IPC handles."""
-    import torch
-    n = torch.cuda.device_count()
-    if n < 2:
-        pytest.skip("needs >= 2 GPUs")
-    world = min(n, 4)
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}",
-                        "--master-addr", "127.0.0.1", "--master-port", "29641",
-                        os.path.join(ROOT, "tests", "multi_gpu_shard_dealloc_check.py")],
-                       capture_output=True, text=True, timeout=600, cwd=ROOT)
-    assert r.returncode == 0 and "ALL OK" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]

@@ -11,16 +11,13 @@ shard can take, byte for byte against the oracle on the whole batch.  The proble
            each compaction and chain limit; the kept slots and the shard's inventory are the oracle's, no other GPU changes.
 (Worlds above 1 run only problems the default plan sends through the single-launch kernel with its gather tail: the end
 of test_gpu_shard.py says why two world contexts on one device cannot run the stand-alone gather after a large kernel.)"""
-from types import SimpleNamespace
-
 import numpy as np
 import pytest
 
 import shard_limit_problems as SP
 from test_gpu_limits import ONE_WAVE_FUSED_MAX, _sms
 from test_gpu_paths import SORT8, STAGED_CAP, assert_same
-from test_gpu_shard import _shard_call
-from test_gpu_shard_dealloc import DeallocWorld, _devp, _table_ptr
+import shard_world as S
 
 pytestmark = pytest.mark.gpu
 
@@ -29,16 +26,16 @@ N_OUT_MAX = 1 << 16                      # the exported table: far above every n
 TAIL = {"compact_flat1", "fused_staged"}
 
 
-class ShardWorld(DeallocWorld):
-    """DeallocWorld exported once for an inventory of 256 GPUs; load() puts any smaller problem on it."""
+class ShardWorld(S.World):
+    """A world exported once for an inventory of 256 GPUs; load() puts any smaller problem on it."""
 
     def __init__(self, pkg, world):
         g, off = R.make_inventory([32] * 8, mig=True)
-        big = SimpleNamespace(gpus=g, node_off=off, table=R.default_table())
-        super().__init__(pkg, big, world, [8 * r // world for r in range(world)] + [8])
+        super().__init__(pkg, R.default_table(), off, g, world, [8 * r // world for r in range(world)] + [8],
+                         n_out_max=N_OUT_MAX)
 
     def load(self, w, bounds, stray_rank, mapped):
-        self.w, self.bounds = w, list(bounds)
+        self.node_off, self.n_node, self.loaded, self.bounds = w.node_off, len(w.node_off) - 1, [w.gpus] * self.world, list(bounds)
         attrs = getattr(w, "attrs", None)
         for r, c in enumerate(self.ctxs):
             c.set_table(w.table); c.set_inventory(w.gpus, w.node_off)
@@ -85,21 +82,21 @@ def run_form_a(pkg, oracle, W, w, bounds, stray, mapped, slot, what):
     out_off, n_out = SP.slot_form(w, slot)
     world = len(W.ctxs)
     W.load(w, bounds, stray, mapped)
-    d_c, d_o = _devp(w.claims), None if out_off is None else _devp(out_off)
+    d_c, d_o = S.dev(w.claims), None if out_off is None else S.dev(out_off)
     ref1, s1 = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, out_off, n_out)
     t1 = W.sharded(d_c, d_o, w.n_claim, n_out, pkg.api.F_FRESH_INVENTORY, ref1, s1, what)
     # the first call's gathered tables, kept for the release (world 1 has one table, which the next call overwrites)
-    keep = [_devp(t) for t in t1] if world == 1 else None
-    p1 = [k.data_ptr() for k in keep] if world == 1 else [_table_ptr(c) for c in W.ctxs]
+    keep = [S.dev(t) for t in t1] if world == 1 else None
+    p1 = [k.data_ptr() for k in keep] if world == 1 else [S.table_ptr(c) for c in W.ctxs]
     ref2, s2 = oracle.allocate(s1, w.node_off, w.table, w.claims, out_off, n_out)
     W.sharded(d_c, d_o, w.n_claim, n_out, 0, ref2, s2, f"{what}, second call")
-    p2 = [_table_ptr(c) for c in W.ctxs]
+    p2 = [S.table_ptr(c) for c in W.ctxs]
     assert world == 1 or not set(p1) & set(p2), "the two calls' tables share a buffer"
     st = oracle.deallocate(s2, w.claims, ref2, out_off, n_node=w.n_node)
-    W.release(w.claims, out_off, n_out, st, f"{what}: release of the second call", ptrs=p2)
+    S.deallocate(W, w.claims, out_off, n_out, st, f"{what}: release of the second call", ptrs=p2)
     st = oracle.deallocate(st, w.claims, ref1, out_off, n_node=w.n_node)
     assert st.tobytes() == w.gpus.tobytes(), f"{what}: the oracle does not release to pristine"
-    W.release(w.claims, out_off, n_out, st, f"{what}: release of the first call", ptrs=p1)
+    S.deallocate(W, w.claims, out_off, n_out, st, f"{what}: release of the first call", ptrs=p1)
     del keep
     if world > 1:
         if not mapped:
@@ -177,12 +174,12 @@ def test_gathered_table_padding_is_left_alone(pkg, oracle, worlds, world):
     w = SP.packet_fixture("statuses")
     assert N_OUT_MAX >= w.n_out + 64
     W.load(w, [0] * world + [1], 0, True)
-    d_c, d_o = _devp(w.claims), _devp(w.out_off)
+    d_c, d_o = S.dev(w.claims), S.dev(w.out_off)
     ref, st = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out)
     ptrs = []
     for k in range(2):
         W.sharded(d_c, d_o, w.n_claim, w.n_out, pkg.api.F_FRESH_INVENTORY, ref, st, f"call {k}")
-        ptrs.append([_table_ptr(c) for c in W.ctxs])
+        ptrs.append([S.table_ptr(c) for c in W.ctxs])
     pads = [torch.as_tensor(_Raw(p + 8 * w.n_out, 8 * (N_OUT_MAX - w.n_out)), device="cuda:0") for ps in ptrs for p in ps]
     assert len({p for ps in ptrs for p in ps}) == 2 * world
     for t in pads:
@@ -206,11 +203,11 @@ def _form_b(pkg, oracle, v, first, hinted, what, flags=0):
         if attrs is not None:
             c.set_gpu_attrs(attrs); c.set_selectors(v.sels.reshape(-1, R.SEL_MAX_INS))
         c.set_shard(v.lo, v.hi, take_stray=True)
-        d, o = _devp(v.claims), _devp(v.out_off)
+        d, o = S.dev(v.claims), S.dev(v.out_off)
         for k, want in enumerate((first, hinted)):
             if want is None:
                 continue
-            _, _, chain = _shard_call(pkg, c, v, d, o, v.lo, v.hi, True, ref, ref_inv, f"{what}, call {k}")
+            _, _, chain = S.shard_call(pkg, c, v, d, o, v.lo, v.hi, True, ref, ref_inv, f"{what}, call {k}")
             assert want(chain) if callable(want) else chain == want, f"{what}, call {k}: took {sorted(chain)}"
             g0, g1 = int(v.node_off[v.lo]), int(v.node_off[v.hi])
             inv = c.get_inventory()

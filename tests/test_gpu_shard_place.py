@@ -2,90 +2,52 @@
 device, wired like test_gpu_shard_pods.py.  Every rank's whole table and pod_node must be byte for byte the §13 oracle's
 answer on the world's real state (the inventory each rank holds for its own node range), each rank's own GPU range the
 oracle's inventory afterwards, and no rank may write GPUs outside its range."""
-import os
-import subprocess
-import sys
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
-from test_gpu_shard_pods import N_OUT_MAX, PodWorld, _flags, _malformed_mixed
-from test_gpu_shard_unsuitable import _bounds, _dense, _dev
 from test_place_pods import NONE, _flat, placed_offsets
 
 import place_oracle as P
+import shard_world as S
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MAX_PODS = 4096
+N_OUT_MAX = 1 << 16
 
 
-class PlaceWorld(PodWorld):
-    """PodWorld with room for the replicated pod states reserved before the export."""
+def _flags(api):
+    return [0, api.F_EXHAUSTIVE, api.F_FRESH_INVENTORY, api.F_EXHAUSTIVE | api.F_FRESH_INVENTORY]
 
-    def __init__(self, pkg, w, world, bounds, stray_rank=0, max_pods=MAX_PODS, attrs=None, sels=None, cap_per_rank=0,
-                 max_pairs=0):
-        R = pkg.records
-        self.pkg, self.w, self.world, self.bounds = pkg, w, world, list(bounds)
-        self.ctxs = [pkg.api.Context(device=0) for _ in range(world)]
-        for r, c in enumerate(self.ctxs):
-            c.comm_init_local(r, world)
-            c.set_table(w.table); c.set_inventory(w.gpus, w.node_off)
-            if sels is not None:
-                c.set_gpu_attrs(attrs); c.set_selectors(sels.reshape(-1, R.SEL_MAX_INS))
-            c.set_shard_map(bounds, stray_rank=stray_rank)
-            if world > 1:
-                c.set_shard_place(max_pods)
-                if max_pairs:
-                    c.set_shard_pairs(max_pairs)
-                c.shard_export(N_OUT_MAX, cap_per_rank, want_handle=False)
-        if world > 1:
-            for c in self.ctxs:
-                c.peer_import_local(self.ctxs)
 
-    def place_enqueue(self, claims, pod_off, cn, co, out_off, n_out, flags=0, n_pair=None):
-        import torch
-        n_pod = len(pod_off) - 1
-        z = torch.zeros(16, dtype=torch.uint8, device="cuda:0")
-        keep = [_dev(claims) if len(claims) else z, _dev(pod_off), _dev(out_off) if out_off is not None else None,
-                _dev(cn) if co is not None and len(cn) else (z if co is not None else None),
-                _dev(co) if co is not None else None,
-                [torch.zeros(max(n_pod, 1) * 4, dtype=torch.uint8, device="cuda:0") for _ in self.ctxs]]
-        if n_pair is None:
-            n_pair = int(co[-1]) if co is not None else 0
-        torch.cuda.synchronize()
-        ptr = lambda t: t.data_ptr() if t is not None else None
-        for c, pn in zip(self.ctxs, keep[5]):
-            c.place_pods_global_device(ptr(keep[0]), len(claims), ptr(keep[1]), n_pod, ptr(keep[3]), ptr(keep[4]), n_pair,
-                                       ptr(keep[2]), n_out, pn.data_ptr(), flags)
-        return keep
+def _world(pkg, w, world, bounds, stray_rank=0, max_pods=MAX_PODS, attrs=None, sels=None, cap_per_rank=0, max_pairs=None):
+    """every rank holding the whole inventory, with room for the replicated pod states reserved before the export"""
+    return S.World(pkg, w.table, w.node_off, w.gpus, world, bounds, stray_rank, attrs, sels, n_out_max=N_OUT_MAX,
+                   cap_per_rank=cap_per_rank, pairs=max_pairs, place=max_pods)
 
-    def place(self, claims, pod_off, cn, co, out_off, n_out, flags=0):
-        """The call on every rank (all enqueued, then waited for): every rank's whole table and pod_node."""
-        keep = self.place_enqueue(claims, pod_off, cn, co, out_off, n_out, flags)
-        for c in self.ctxs:
-            c.sync()
-        n_pod = len(pod_off) - 1
-        nodes = [pn.cpu().numpy().view(np.uint32)[:n_pod].copy() for pn in keep[5]]
-        return [c.gather_read(np.zeros(n_out, dtype=self.pkg.records.OUT_DTYPE)) for c in self.ctxs], nodes
 
-    def check_place(self, claims, pod_off, cn, co, out_off, n_out, flags, what):
-        api = self.pkg.api
-        before = self.inventories()
-        src = self.w.gpus if flags & api.F_FRESH_INVENTORY else self.real_state()
-        ref, ref_node, ref_inv = P.place_pods(src, self.w.node_off, self.w.table, claims, pod_off, cn, co, out_off, n_out,
-                                              P.F_EXHAUSTIVE if flags & api.F_EXHAUSTIVE else 0)
-        tables, nodes = self.place(claims, pod_off, cn, co, out_off, n_out, flags)
-        after = self.inventories()
-        for r in range(self.world):
-            assert tables[r].tobytes() == ref.tobytes(), f"{what}: rank {r} table differs"
-            assert nodes[r].tobytes() == ref_node.tobytes(), f"{what}: rank {r} pod_node differs"
-            g0, g1 = self.gpu_range(r)
-            assert after[r][g0:g1].tobytes() == ref_inv[g0:g1].tobytes(), f"{what}: rank {r} inventory of its range differs"
-            assert after[r][:g0].tobytes() == before[r][:g0].tobytes() and \
-                after[r][g1:].tobytes() == before[r][g1:].tobytes(), f"{what}: rank {r} wrote GPUs outside its range"
-        assert "place_shard" in self.ctxs[0].last_chain()
-        return ref, ref_node
+def _place(W, claims, pod_off, cn, co, out_off, n_out, flags=0):
+    """every rank's whole table and pod_node"""
+    res = S.place(W, claims, pod_off, None if co is None else (cn, co), out_off, n_out, flags)
+    return [t for t, _ in res], [n for _, n in res]
+
+
+def _check(W, w, claims, pod_off, cn, co, out_off, n_out, flags, what):
+    """One call against the §13 oracle on the world's state: every rank's table and pod_node, its own range the oracle's,
+    nothing written outside it, the chain taken."""
+    api = W.pkg.api
+    before = W.inventories()
+    src = w.gpus if flags & api.F_FRESH_INVENTORY else W.state()
+    ref, ref_node, ref_inv = P.place_pods(src, w.node_off, w.table, claims, pod_off, cn, co, out_off, n_out,
+                                          P.F_EXHAUSTIVE if flags & api.F_EXHAUSTIVE else 0)
+    tables, nodes = _place(W, claims, pod_off, cn, co, out_off, n_out, flags)
+    S.same_tables(tables, ref, what)
+    for r in range(W.world):
+        assert nodes[r].tobytes() == ref_node.tobytes(), f"{what}: rank {r} pod_node differs"
+    W.assert_ranges(before, ref_inv, what)
+    assert "place_shard" in W.ctxs[0].last_chain()
+    return ref, ref_node
 
 
 def _forms(rng, n_pod, n_node, bounds):
@@ -112,12 +74,12 @@ def test_matches_oracle(pkg, world):
     kind = ["even", "uneven", "empty", "uneven"][world - 1]
     w, pod_off = pkg.synth.pods(500, 23, 100 + world)
     n_pod = len(pod_off) - 1
-    bounds = _bounds(w.n_node, world, kind)
-    W = PlaceWorld(pkg, w, world, bounds, world - 1)
+    bounds = S.bounds(w.n_node, world, kind)
+    W = _world(pkg, w, world, bounds, world - 1)
     try:
         for i, (name, (cn, co)) in enumerate(_forms(rng, n_pod, w.n_node, bounds).items()):
             flags = _flags(pkg.api)[i % 4]
-            ref, ref_node = W.check_place(w.claims, pod_off, cn, co, None, len(w.claims), flags, f"{name} flags {flags}")
+            ref, ref_node = _check(W, w, w.claims, pod_off, cn, co, None, len(w.claims), flags, f"{name} flags {flags}")
             if name != "duplicates":
                 assert (ref_node != NONE).any() and (ref_node == NONE).any(), name
     finally:
@@ -131,14 +93,14 @@ def test_flags_in_sequence(pkg, world):
     rng = np.random.default_rng(7 + world)
     w, pod_off = pkg.synth.pods(400, 17, 60 + world)
     n_pod = len(pod_off) - 1
-    bounds = _bounds(w.n_node, world, "uneven")
-    W = PlaceWorld(pkg, w, world, bounds, 0)
+    bounds = S.bounds(w.n_node, world, "uneven")
+    W = _world(pkg, w, world, bounds, 0)
     try:
         for rep in range(2):
             for flags in _flags(pkg.api):
                 cn = rng.integers(0, w.n_node, n_pod * 6).astype(np.uint32)
                 co = (np.arange(n_pod + 1) * 6).astype(np.uint32)
-                W.check_place(w.claims, pod_off, cn, co, None, len(w.claims), flags, f"rep {rep} flags {flags}")
+                _check(W, w, w.claims, pod_off, cn, co, None, len(w.claims), flags, f"rep {rep} flags {flags}")
     finally:
         W.close()
 
@@ -151,18 +113,18 @@ def test_mixed_pods(pkg, world):
     rng = np.random.default_rng(30 + world)
     w = pkg.synth.mixed(2400, 31, 70 + world, invalid=True)
     attrs, sels = pkg.synth.with_selectors(w, world)
-    bounds = _bounds(w.n_node, world, "even")
-    claims, pod_off, _, _ = _malformed_mixed(pkg, w, bounds, rng, False)
+    bounds = S.bounds(w.n_node, world, "even")
+    claims, pod_off, _, _ = S.malformed_mixed(pkg, w, bounds, rng, False)
     out_off, n_out = placed_offsets(pkg.records, claims, w.n_node)
     n_pod = len(pod_off) - 1
     cn = rng.integers(0, w.n_node + 2, n_pod * 5).astype(np.uint32)
     co = (np.arange(n_pod + 1) * 5).astype(np.uint32)
-    W = PlaceWorld(pkg, w, world, bounds, 0, attrs=attrs, sels=sels)
+    W = _world(pkg, w, world, bounds, 0, attrs=attrs, sels=sels)
     P.set_selectors(attrs, sels)
     try:
         for flags in (0, api.F_EXHAUSTIVE | api.F_FRESH_INVENTORY):
             for c_, o_ in ((cn, co), (None, None)):
-                ref, _ = W.check_place(claims, pod_off, c_, o_, out_off, int(n_out), flags, f"mixed flags {flags}")
+                ref, _ = _check(W, w, claims, pod_off, c_, o_, out_off, int(n_out), flags, f"mixed flags {flags}")
                 assert (ref["status"] == pkg.records.ST_INVALID).any()
     finally:
         P.set_selectors()
@@ -176,18 +138,17 @@ def test_search_limit_survives_a_hand_off(pkg):
     from test_pod_mode import _mig
     g, off = R.make_inventory([1, 1, 1], mig=True)
     g["busy"][1] = 0xFF
-    w = type("W", (), {})()
-    w.gpus, w.node_off, w.table, w.n_node = g, off, R.default_table(), 3
+    w = SimpleNamespace(gpus=g, node_off=off, table=R.default_table(), n_node=3)
     c = _mig(R, [R.GI_1_SLICE] * 7 + [R.GI_7_SLICE])
     pod_off = np.array([0, 8], np.uint32)
-    W = PlaceWorld(pkg, w, 3, [0, 1, 2, 3], 2)
+    W = _world(pkg, w, 3, [0, 1, 2, 3], 2)
     try:
         for cands in ([0, 1], [1, 0], [0, 1, 2], [2, 1, 0]):
             cn, co = _flat([cands])
-            ref, node = W.check_place(c, pod_off, cn, co, None, 8, api.F_EXHAUSTIVE | api.F_FRESH_INVENTORY, f"cands {cands}")
+            ref, node = _check(W, w, c, pod_off, cn, co, None, 8, api.F_EXHAUSTIVE | api.F_FRESH_INVENTORY, f"cands {cands}")
             assert set(ref["status"]) == {R.ST_SEARCH_LIMIT} and list(node) == [NONE]
         cn, co = _flat([[0, 1]])
-        ref, _ = W.check_place(c, pod_off, cn, co, None, 8, api.F_FRESH_INVENTORY, "first-fit")
+        ref, _ = _check(W, w, c, pod_off, cn, co, None, 8, api.F_FRESH_INVENTORY, "first-fit")
         assert set(ref["status"]) == {R.ST_POD}
     finally:
         W.close()
@@ -201,10 +162,10 @@ def test_windows_wider_than_the_resident_warps(pkg):
     n_pod = len(pod_off) - 1
     cn = rng.integers(0, w.n_node + 2, n_pod * 8).astype(np.uint32)
     co = (np.arange(n_pod + 1) * 8).astype(np.uint32)
-    W = PlaceWorld(pkg, w, 2, [0, 5000, 10_000], 0, max_pods=n_pod)
+    W = _world(pkg, w, 2, [0, 5000, 10_000], 0, max_pods=n_pod)
     try:
         for flags in (0, pkg.api.F_EXHAUSTIVE):
-            W.check_place(w.claims, pod_off, cn, co, None, len(w.claims), flags, f"10k nodes flags {flags}")
+            _check(W, w, w.claims, pod_off, cn, co, None, len(w.claims), flags, f"10k nodes flags {flags}")
     finally:
         W.close()
 
@@ -215,12 +176,12 @@ def test_single_candidate_equals_sharded_pods_allocate(pkg):
     w, pod_off = pkg.synth.pods(600, 20, 9)
     first = w.claims["node"][pod_off[:-1]].astype(np.uint32)
     co = np.arange(len(pod_off), dtype=np.uint32)
-    W = PlaceWorld(pkg, w, 3, _bounds(w.n_node, 3, "uneven"), 1)
+    W = _world(pkg, w, 3, S.bounds(w.n_node, 3, "uneven"), 1)
     try:
         for flags in (api.F_FRESH_INVENTORY, api.F_FRESH_INVENTORY | api.F_EXHAUSTIVE):
-            ref = W.call(w.claims, pod_off, None, len(w.claims), flags)
+            ref = S.pods(W, w.claims, pod_off, None, len(w.claims), flags)
             inv = W.inventories()
-            tables, nodes = W.place(w.claims, pod_off, first, co, None, len(w.claims), flags)
+            tables, nodes = _place(W, w.claims, pod_off, first, co, None, len(w.claims), flags)
             for r in range(3):
                 assert tables[r].tobytes() == ref[r].tobytes(), f"flags {flags} rank {r}"
                 assert W.inventories()[r].tobytes() == inv[r].tobytes()
@@ -236,29 +197,19 @@ def test_world1_equals_single_inventory_call(pkg):
     n_pod = len(pod_off) - 1
     cn = rng.integers(0, w.n_node + 2, n_pod * 8).astype(np.uint32)
     co = (np.arange(n_pod + 1) * 8).astype(np.uint32)
-    W = PlaceWorld(pkg, w, 1, [0, w.n_node], 0)
+    W = _world(pkg, w, 1, [0, w.n_node], 0)
     with api.Context(device=0) as single:
         single.set_table(w.table); single.set_inventory(w.gpus, w.node_off)
         try:
             for flags in _flags(api):
                 for c_, o_ in ((cn, co), (None, None)):
-                    tables, nodes = W.place(w.claims, pod_off, c_, o_, None, len(w.claims), flags)
+                    tables, nodes = _place(W, w.claims, pod_off, c_, o_, None, len(w.claims), flags)
                     out, pod_node = single.place_pods(w.claims, pod_off, c_, o_, None, len(w.claims), flags)
                     assert tables[0].tobytes() == out.tobytes() and nodes[0].tobytes() == pod_node.tobytes()
                     assert W.ctxs[0].get_inventory().tobytes() == single.get_inventory().tobytes(), f"flags {flags}"
             assert "place_shard" in W.ctxs[0].last_chain() and "pod_gather" not in W.ctxs[0].last_chain()
         finally:
             W.close()
-
-
-def _codes(W):
-    codes = []
-    for c in W.ctxs:
-        try:
-            c.sync(); codes.append(0)
-        except W.pkg.api.DraError as e:
-            codes.append(e.code)
-    return codes
 
 
 def test_errors(pkg):
@@ -272,7 +223,7 @@ def test_errors(pkg):
     rng = np.random.default_rng(1)
     cn = rng.integers(0, w.n_node, n_pod * 4).astype(np.uint32)
     co = (np.arange(n_pod + 1) * 4).astype(np.uint32)
-    d_c, d_p, d_n, d_o, d_pn = _dev(w.claims), _dev(pod_off), _dev(cn), _dev(co), _dev(np.zeros(n_pod, np.uint32))
+    d_c, d_p, d_n, d_o, d_pn = S.dev(w.claims), S.dev(pod_off), S.dev(cn), S.dev(co), S.dev(np.zeros(n_pod, np.uint32))
     torch.cuda.synchronize()
 
     def raw(c, **k):
@@ -290,7 +241,7 @@ def test_errors(pkg):
         assert raw(c) == api.E_STATE                                         # world 2 after a bare set_shard
         c.set_shard_map(bounds, 0)
         assert raw(c) == api.E_STATE                                         # world 2 without export + import
-    W = PlaceWorld(pkg, w, 2, bounds, 1, max_pods=n_pod)
+    W = _world(pkg, w, 2, bounds, 1, max_pods=n_pod)
     try:
         c0 = W.ctxs[0]
         with pytest.raises(api.DraError) as e:
@@ -305,7 +256,7 @@ def test_errors(pkg):
         assert raw(c0, cn=None, co=None) == api.E_INVAL                      # dense form with n_pair != 0
         assert raw(c0, n_pod=n_pod + 1) == api.E_STATE                       # beyond max_pods of the export
         assert raw(c0, pod_node=None) == api.E_INVAL
-        W.check_place(w.claims, pod_off, cn, co, None, len(w.claims), 0, "after host-side refusals")
+        _check(W, w, w.claims, pod_off, cn, co, None, len(w.claims), 0, "after host-side refusals")
         bad_po = pod_off.copy(); bad_po[5] = bad_po[7] + 1
         short_po = pod_off.copy(); short_po[-1] -= 1
         bad_co = co.copy(); bad_co[3] = bad_co[5] + 1
@@ -317,27 +268,23 @@ def test_errors(pkg):
                                          ("cand_off not spanning", pod_off, long_co, None, api.F_FRESH_INVENTORY),
                                          ("slot past n_out", pod_off, co, past, 0)):
             before = W.inventories()
-            keep = W.place_enqueue(w.claims, po, cn, co_, oo, len(w.claims), flags, n_pair=len(cn))
-            assert _codes(W) == [api.E_INVAL] * 2, what
-            del keep
+            S.place(W, w.claims, po, (cn, co_), oo, len(w.claims), flags, n_pair=len(cn), expect=api.E_INVAL)
             for b, a in zip(before, W.inventories()):
                 assert a.tobytes() == b.tobytes(), f"{what}: a failed call changed an inventory"
-            W.check_place(w.claims, pod_off, cn, co, None, len(w.claims), api.F_EXHAUSTIVE, f"after {what}")
+            _check(W, w, w.claims, pod_off, cn, co, None, len(w.claims), api.F_EXHAUSTIVE, f"after {what}")
         # the pristine copies are untouched: a fresh call answers from the inventory as loaded
-        W.check_place(w.claims, pod_off, cn, co, None, len(w.claims), api.F_FRESH_INVENTORY, "fresh after the faults")
+        _check(W, w, w.claims, pod_off, cn, co, None, len(w.claims), api.F_FRESH_INVENTORY, "fresh after the faults")
     finally:
         W.close()
     # a rank that could finalise more slots than the packet room its export reserved: every rank fails, nothing changes
-    W = PlaceWorld(pkg, w, 2, bounds, 1, cap_per_rank=8)
+    W = _world(pkg, w, 2, bounds, 1, cap_per_rank=8)
     try:
         before = W.inventories()
-        keep = W.place_enqueue(w.claims, pod_off, cn, co, None, len(w.claims), 0)
-        assert _codes(W) == [api.E_INVAL] * 2
-        del keep
+        S.place(W, w.claims, pod_off, (cn, co), None, len(w.claims), 0, expect=api.E_INVAL)
         for b, a in zip(before, W.inventories()):
             assert a.tobytes() == b.tobytes()
         one = np.array([0, int(pod_off[1])], np.uint32)                      # one pod: within the room
-        W.check_place(w.claims[: one[1]], one, cn[:4], co[:2], None, int(one[1]), 0, "within the packet room")
+        _check(W, w, w.claims[: one[1]], one, cn[:4], co[:2], None, int(one[1]), 0, "within the packet room")
     finally:
         W.close()
 
@@ -369,53 +316,25 @@ def test_classic_flow_without_a_sync(pkg, oracle, world):
     R, api = pkg.records, pkg.api
     w, pod_off = pkg.synth.pods(300, 24, 40 + world)
     n_pod = len(pod_off) - 1
-    bounds = _bounds(w.n_node, world, "even")
+    bounds = S.bounds(w.n_node, world, "even")
     n_pair = n_pod * w.n_node
-    W = PlaceWorld(pkg, w, world, bounds, 0, max_pairs=n_pair)
+    W = _world(pkg, w, world, bounds, 0, max_pairs=n_pair)
     try:
-        d_c, d_p = _dev(w.claims), _dev(pod_off)
-        bits = [torch.zeros((n_pair + 7) // 8 + 8, dtype=torch.uint8, device="cuda:0") for _ in W.ctxs]
-        torch.cuda.synchronize()
-        for c, b in zip(W.ctxs, bits):
-            c.unsuitable_global_device(d_c.data_ptr(), len(w.claims), d_p.data_ptr(), n_pod, None, None, n_pair, b.data_ptr(),
-                                       api.F_EXHAUSTIVE)
-        verdict = None
-        for c in W.ctxs:
-            c.sync()
-        verdict = np.unpackbits(bits[0].cpu().numpy()[: (n_pair + 7) // 8], bitorder="little")[:n_pair].reshape(n_pod, w.n_node)
-        dn, do = _dense(n_pod, w.n_node)
+        bits = S.unsuitable(W, w.claims, pod_off, flags=api.F_EXHAUSTIVE)
+        verdict = np.unpackbits(bits[0], bitorder="little")[:n_pair].reshape(n_pod, w.n_node)
+        dn, do = S.dense(n_pod, w.n_node)
         ref_bits = oracle.unsuitable(w.gpus, w.node_off, w.table, w.claims, pod_off, dn, do, flags=oracle.F_EXHAUSTIVE)
         assert np.packbits(verdict.ravel(), bitorder="little").tobytes() == ref_bits.tobytes()
         cn, co = _flat([list(np.flatnonzero(verdict[p])) for p in range(n_pod)])
-        ref, ref_node = W.check_place(w.claims, pod_off, cn, co, None, len(w.claims), api.F_EXHAUSTIVE, "place on the verdict")
+        ref, ref_node = _check(W, w, w.claims, pod_off, cn, co, None, len(w.claims), api.F_EXHAUSTIVE, "place on the verdict")
         assert (ref_node != NONE).sum() > n_pod // 4
         claims = w.claims.copy()
         for p in range(n_pod):
             claims["node"][pod_off[p]: pod_off[p + 1]] = ref_node[p] if ref_node[p] != NONE else 0
-        table = _dev(ref)
-        d_c2 = _dev(claims)
+        table, d_c2 = S.dev(ref), S.dev(claims)
         torch.cuda.synchronize()
-        for c in W.ctxs:
+        for c in W.ctxs:                                 # the release and the sync enqueued with no wait in between
             c.deallocate_global_device(d_c2.data_ptr(), len(claims), None, table.data_ptr(), len(claims))
-        for c in W.ctxs:
-            c.shard_sync_inventory_device()
-        for c in W.ctxs:
-            c.sync()
-        for r, inv in enumerate(W.inventories()):
-            assert inv.tobytes() == w.gpus.tobytes(), f"rank {r} does not hold the starting inventory"
+        W.assert_synced(w.gpus, "the release of the placed table")
     finally:
         W.close()
-
-
-def test_multi_process_place():
-    """tests/multi_gpu_shard_place_check.py under torchrun: one process per GPU, peers mapped with IPC handles."""
-    import torch
-    n = torch.cuda.device_count()
-    if n < 2:
-        pytest.skip("needs >= 2 GPUs")
-    world = min(n, 4)
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}",
-                        "--master-addr", "127.0.0.1", "--master-port", "29641",
-                        os.path.join(ROOT, "tests", "multi_gpu_shard_place_check.py")],
-                       capture_output=True, text=True, timeout=600, cwd=ROOT)
-    assert r.returncode == 0 and "ALL OK" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]

@@ -2,104 +2,43 @@
 device, wired with dra_comm_init_local / dra_peer_import_local like test_gpu_shard_pods.py.  The CPU oracle runs every call
 on ONE whole inventory; after a sync every rank's live inventory must be byte for byte that inventory, every rank's own
 range must be what it held before, and calls under a new shard map must answer as the oracle does on that state."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
-from test_gpu_shard_pods import PodWorld, _malformed_mixed
-from test_gpu_shard_unsuitable import _bounds, _candidates, _dense, _dev, _pod_cuts
+import shard_world as S
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 N_POD_UNS = 300
 
 
-class SyncWorld(PodWorld):
-    """PodWorld plus the sharded claim Allocate, UnsuitableNodes, per-rank Deallocate, the sync and a re-map."""
-
-    def sync_inventory(self):
-        for c in self.ctxs:                              # enqueued on every rank before any waits
-            c.shard_sync_inventory_device()
-        for c in self.ctxs:
-            c.sync()
-
-    def remap(self, bounds, stray_rank):
-        for c in self.ctxs:
-            c.set_shard_map(bounds, stray_rank=stray_rank)
-        self.bounds = list(bounds)
-
-    def allocate(self, claims, out_off, n_out, flags=0):
-        import torch
-        keep = [_dev(claims), _dev(out_off)]
-        torch.cuda.synchronize()
-        for c in self.ctxs:
-            c.allocate_global_device(keep[0].data_ptr(), len(claims), keep[1].data_ptr(), n_out, flags)
-        for c in self.ctxs:
-            c.sync()
-        return [c.gather_read(np.zeros(n_out, dtype=self.pkg.records.OUT_DTYPE)) for c in self.ctxs]
-
-    def unsuitable(self, claims, pod_off, cand_nodes, cand_off, flags):
-        import torch
-        n_pod = len(pod_off) - 1
-        n_pair = n_pod * self.w.n_node if cand_nodes is None else int(cand_off[-1])
-        keep = [_dev(claims), _dev(pod_off)] + ([_dev(cand_nodes), _dev(cand_off)] if cand_nodes is not None else [])
-        bits = [torch.zeros((n_pair + 7) // 8 + 8, dtype=torch.uint8, device="cuda:0") for _ in self.ctxs]
-        torch.cuda.synchronize()
-        for c, b in zip(self.ctxs, bits):
-            c.unsuitable_global_device(keep[0].data_ptr(), len(claims), keep[1].data_ptr(), n_pod,
-                                       keep[2].data_ptr() if cand_nodes is not None else None,
-                                       keep[3].data_ptr() if cand_nodes is not None else None, n_pair, b.data_ptr(), flags)
-        for c in self.ctxs:
-            c.sync()
-        return [b.cpu().numpy()[: (n_pair + 7) // 8] for b in bits]
-
-    def deallocate(self, claims, out, out_off):
-        for c in self.ctxs:                              # every rank applies every gathered record
-            c.deallocate(claims, out, out_off)
-
-    def assert_own_ranges(self, state, what):
-        for r, inv in enumerate(self.inventories()):
-            g0, g1 = self.gpu_range(r)
-            assert inv[g0:g1].tobytes() == state[g0:g1].tobytes(), f"{what}: rank {r} own range differs from the oracle"
+def _world(pkg, w, world, bounds, stray_rank, max_pairs=None):
+    return S.World(pkg, w.table, w.node_off, w.gpus, world, bounds, stray_rank, n_out_max=1 << 16, pairs=max_pairs)
 
 
-def _shared_mixed(pkg, w, rng):
-    """synth.mixed's claims with a fifth of them turned into cfg4-style SHARED claims (MPS limits of 1-10 GiB)."""
-    R = pkg.records
-    c = w.claims.copy()
-    sh = rng.random(len(c)) < 0.2
-    c["kind"][sh], c["count"][sh], c["group"][sh] = R.KIND_SHARED, 1, 0
-    c["mem_limit_mib"][sh] = rng.choice(np.array([1024, 2048, 4096, 8192, 10240], dtype=np.uint32), int(sh.sum()))
-    return c
-
-
-def _check_tables(tables, ref, what):
-    for r, t in enumerate(tables):
-        assert t.tobytes() == ref.tobytes(), f"{what}: rank {r} table differs from the oracle"
+def _deallocate(W, claims, out, out_off):
+    for c in W.ctxs:                                     # every rank applies every gathered record
+        c.deallocate(claims, out, out_off)
 
 
 def _mixed_sequence(pkg, oracle, W, w, rng, state):
     """Sharded Allocate, sharded pods Allocate first-fit and exhaustive, then every rank deallocates the Allocate's and the
     first-fit pods' gathered records.  Returns the oracle's state of the one whole inventory after the same calls."""
     R, api = pkg.records, pkg.api
-    claims = _shared_mixed(pkg, w, rng)
+    claims = S.shared_mixed(pkg, w, rng)
     out_off, n_out = R.out_offsets(claims, w.n_node)
     ref, state = oracle.allocate(state, w.node_off, w.table, claims, out_off, int(n_out))
-    _check_tables(W.allocate(claims, out_off, int(n_out)), ref, "sharded Allocate")
+    S.same_tables(S.allocate(W, claims, out_off, int(n_out)), ref, "sharded Allocate")
     assert (ref["status"] == 0).any() and (ref["profile"][ref["status"] == 0] == R.PROFILE_SHARED).any()
     done = [(claims, ref, out_off)]
     for flags, oflags in ((0, 0), (api.F_EXHAUSTIVE, oracle.F_EXHAUSTIVE)):
-        pc, po, poo, pn = _malformed_mixed(pkg, w, W.bounds, rng, True)
+        pc, po, poo, pn = S.malformed_mixed(pkg, w, W.bounds, rng, True)
         ref, state = oracle.allocate_pods(state, w.node_off, w.table, pc, po, poo, pn, oflags)
-        _check_tables(W.call(pc, po, poo, pn, flags), ref, f"sharded pods Allocate flags {flags}")
+        S.same_tables(S.pods(W, pc, po, poo, pn, flags), ref, f"sharded pods Allocate flags {flags}")
         done.append((pc, ref, poo))
     for c, out, off in done[:2]:
         state = oracle.deallocate(state, c, out, off, n_node=w.n_node)
-        W.deallocate(c, out, off)
-    W.assert_own_ranges(state, "after the mixed sequence")
+        _deallocate(W, c, out, off)
+    W.assert_ranges(None, state, "after the mixed sequence")
     return state
 
 
@@ -120,7 +59,7 @@ def test_sync_after_mixed_sequence(pkg, oracle, world):
     rng = np.random.default_rng(100 + world)
     w = pkg.synth.mixed(2400, 31, 70 + world, invalid=True)
     kind = {1: "even", 2: "uneven", 3: "empty", 4: "uneven"}[world]
-    W = SyncWorld(pkg, w, world, _bounds(w.n_node, world, kind), world - 1)
+    W = _world(pkg, w, world, S.bounds(w.n_node, world, kind), world - 1)
     try:
         state = _mixed_sequence(pkg, oracle, W, w, rng, w.gpus.copy())
         if world > 1:
@@ -135,11 +74,11 @@ def test_sync_after_mixed_sequence(pkg, oracle, world):
             assert all(c.launch_count() == l + 2 for c, l in zip(W.ctxs, l0))
         _sync_and_check(W, state, "second sync")
         # the pristine copy: a fresh-inventory sharded Allocate answers from the loaded inventory
-        claims = _shared_mixed(pkg, w, rng)
+        claims = S.shared_mixed(pkg, w, rng)
         out_off, n_out = R.out_offsets(claims, w.n_node)
         ref, ref_inv = oracle.allocate(w.gpus, w.node_off, w.table, claims, out_off, int(n_out))
-        _check_tables(W.allocate(claims, out_off, int(n_out), api.F_FRESH_INVENTORY), ref, "fresh Allocate after a sync")
-        W.assert_own_ranges(ref_inv, "fresh Allocate after a sync")
+        S.same_tables(S.allocate(W, claims, out_off, int(n_out), api.F_FRESH_INVENTORY), ref, "fresh Allocate after a sync")
+        W.assert_ranges(None, ref_inv, "fresh Allocate after a sync")
     finally:
         W.close()
 
@@ -152,19 +91,19 @@ def test_sync_across_several_copy_ctas(pkg, oracle):
     rng = np.random.default_rng(17)
     w = pkg.synth.mixed(3000, 300, 17, invalid=True)
     assert w.n_gpu > 4 * 256, "the inventory must span at least five copy CTAs"
-    W = SyncWorld(pkg, w, 4, [0, 40, 40, 170, 300], 2)
+    W = _world(pkg, w, 4, [0, 40, 40, 170, 300], 2)
     try:
         state = _mixed_sequence(pkg, oracle, W, w, rng, w.gpus.copy())
         _sync_and_check(W, state, "first sync")
-        claims = _shared_mixed(pkg, w, rng)
+        claims = S.shared_mixed(pkg, w, rng)
         out_off, n_out = R.out_offsets(claims, w.n_node)
         ref, state = oracle.allocate(state, w.node_off, w.table, claims, out_off, int(n_out))
-        _check_tables(W.allocate(claims, out_off, int(n_out)), ref, "sharded Allocate between syncs")
+        S.same_tables(S.allocate(W, claims, out_off, int(n_out)), ref, "sharded Allocate between syncs")
         _sync_and_check(W, state, "second sync")
-        pc, po, poo, pn = _malformed_mixed(pkg, w, W.bounds, rng, True)
+        pc, po, poo, pn = S.malformed_mixed(pkg, w, W.bounds, rng, True)
         ref, state = oracle.allocate_pods(state, w.node_off, w.table, pc, po, poo, pn, oracle.F_EXHAUSTIVE)
-        _check_tables(W.call(pc, po, poo, pn, api.F_EXHAUSTIVE), ref, "pods Allocate between syncs")
-        W.deallocate(pc, ref, poo)
+        S.same_tables(S.pods(W, pc, po, poo, pn, api.F_EXHAUSTIVE), ref, "pods Allocate between syncs")
+        _deallocate(W, pc, ref, poo)
         state = oracle.deallocate(state, pc, ref, poo, n_node=w.n_node)
         _sync_and_check(W, state, "third sync")
     finally:
@@ -219,7 +158,7 @@ def test_ipc_import_requires_alike_exports(pkg, sizes):
 
 def _pods_for_unsuitable(pkg, w, rng):
     claims = w.claims.copy()
-    pod_off = _pod_cuts(rng, 900, N_POD_UNS - 60)
+    pod_off = S.pod_cuts(rng, 900, N_POD_UNS - 60)
     return claims[: pod_off[-1]], pod_off
 
 
@@ -233,33 +172,33 @@ def test_reshard_keeps_allocations(pkg, oracle):
     world = 3
     w = pkg.synth.mixed(2400, 31, 91, invalid=True)
     bounds_a, bounds_b = [0, 3, 9, 31], [0, 20, 20, 31]
-    W = SyncWorld(pkg, w, world, bounds_a, 2, max_pairs=N_POD_UNS * w.n_node)
+    W = _world(pkg, w, world, bounds_a, 2, max_pairs=N_POD_UNS * w.n_node)
     try:
         state = _mixed_sequence(pkg, oracle, W, w, rng, w.gpus.copy())
         _sync_and_check(W, state, "sync under map A")
         W.remap(bounds_b, 0)
-        W.assert_own_ranges(state, "after the re-map")
-        claims = _shared_mixed(pkg, w, rng)
+        W.assert_ranges(None, state, "after the re-map")
+        claims = S.shared_mixed(pkg, w, rng)
         out_off, n_out = R.out_offsets(claims, w.n_node)
         ref, state = oracle.allocate(state, w.node_off, w.table, claims, out_off, int(n_out))
-        _check_tables(W.allocate(claims, out_off, int(n_out)), ref, "sharded Allocate under map B")
+        S.same_tables(S.allocate(W, claims, out_off, int(n_out)), ref, "sharded Allocate under map B")
         uc, upo = _pods_for_unsuitable(pkg, w, rng)
         n_pod = len(upo) - 1
-        cn, co = _candidates(rng, n_pod, w.n_node)
-        forms = [("dense", None, None) + _dense(n_pod, w.n_node), ("candidates", cn, co, cn, co)]
+        cn, co = S.candidates(rng, n_pod, w.n_node)
+        forms = [("dense", None, None) + S.dense(n_pod, w.n_node), ("candidates", cn, co, cn, co)]
         for flags, oflags in ((0, 0), (api.F_EXHAUSTIVE, oracle.F_EXHAUSTIVE)):
             for name, dn, do, on, oo in forms:
                 ref_bits = oracle.unsuitable(state, w.node_off, w.table, uc, upo, on, oo, flags=oflags)
-                for r, b in enumerate(W.unsuitable(uc, upo, dn, do, flags)):
+                for r, b in enumerate(S.unsuitable(W, uc, upo, None if dn is None else (dn, do), flags)):
                     assert b.tobytes() == ref_bits.tobytes(), f"UnsuitableNodes {name} flags {flags}: rank {r} differs"
         for flags, oflags in ((0, 0), (api.F_EXHAUSTIVE, oracle.F_EXHAUSTIVE)):
-            pc, po, poo, pn = _malformed_mixed(pkg, w, W.bounds, rng, True)
+            pc, po, poo, pn = S.malformed_mixed(pkg, w, W.bounds, rng, True)
             ref, state = oracle.allocate_pods(state, w.node_off, w.table, pc, po, poo, pn, oflags)
-            _check_tables(W.call(pc, po, poo, pn, flags), ref, f"pods Allocate under map B flags {flags}")
-        W.assert_own_ranges(state, "after the calls under map B")
+            S.same_tables(S.pods(W, pc, po, poo, pn, flags), ref, f"pods Allocate under map B flags {flags}")
+        W.assert_ranges(None, state, "after the calls under map B")
         _sync_and_check(W, state, "sync under map B")
         for flags, oflags in ((0, 0), (api.F_EXHAUSTIVE, oracle.F_EXHAUSTIVE)):
-            sharded = W.unsuitable(uc, upo, cn, co, flags)[0]
+            sharded = S.unsuitable(W, uc, upo, (cn, co), flags)[0]
             assert sharded.tobytes() == oracle.unsuitable(state, w.node_off, w.table, uc, upo, cn, co, flags=oflags).tobytes()
             single = W.ctxs[1].unsuitable(uc, upo, cn, co, flags)
             assert single.tobytes() == sharded.tobytes(), f"flags {flags}: one rank's dra_unsuitable_batch differs"
@@ -302,7 +241,7 @@ def test_errors_change_nothing(pkg, oracle):
     finally:
         for c in ctxs:
             c.close()
-    W = SyncWorld(pkg, w, 2, [0, 5, 11], 1)
+    W = _world(pkg, w, 2, [0, 5, 11], 1)
     try:
         for c in W.ctxs:                                                 # the inventory grows after the export
             c.set_inventory(big.gpus, big.node_off); c.set_shard_map([0, 9, 23], 1)
@@ -314,17 +253,3 @@ def test_errors_change_nothing(pkg, oracle):
         _sync_and_check(W, state, "after refused calls")
     finally:
         W.close()
-
-
-def test_multi_process_sync():
-    """tests/multi_gpu_shard_sync_check.py under torchrun: one process per GPU, peers mapped with IPC handles."""
-    import torch
-    n = torch.cuda.device_count()
-    if n < 2:
-        pytest.skip("needs >= 2 GPUs")
-    world = min(n, 4)
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}",
-                        "--master-addr", "127.0.0.1", "--master-port", "29637",
-                        os.path.join(ROOT, "tests", "multi_gpu_shard_sync_check.py")],
-                       capture_output=True, text=True, timeout=600, cwd=ROOT)
-    assert r.returncode == 0 and "ALL OK" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]

@@ -4,108 +4,21 @@ byte for byte the oracle's answer on the world's real state: the inventory each 
 import numpy as np
 import pytest
 
+import shard_world as S
+
 pytestmark = pytest.mark.gpu
 
 SENTINEL = 0xA5
 
 
-def _dev(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).copy()).to("cuda:0")
+def _world(pkg, w, world, bounds, max_pairs, inv=None, attrs=None, sels=None):
+    """every rank holding the whole inventory, the table exported for w's records"""
+    return S.World(pkg, w.table, w.node_off, w.gpus if inv is None else inv, world, bounds, attrs=attrs, sels=sels,
+                   n_out_max=max(1, w.n_out), pairs=max_pairs)
 
 
-def _dense(n_pod, n_node):
-    return (np.tile(np.arange(n_node, dtype=np.uint32), n_pod),
-            (np.arange(n_pod + 1, dtype=np.uint64) * n_node).astype(np.uint32))
-
-
-class World:
-    """world contexts on device 0, every one holding the whole inventory, rank r serving [bounds[r], bounds[r+1])."""
-
-    def __init__(self, pkg, w, world, bounds, max_pairs, inv=None, attrs=None, sels=None):
-        R = pkg.records
-        self.pkg, self.w = pkg, w
-        self.ctxs = [pkg.api.Context(device=0) for _ in range(world)]
-        for r, c in enumerate(self.ctxs):
-            c.comm_init_local(r, world)
-            c.set_table(w.table); c.set_inventory(w.gpus if inv is None else inv, w.node_off)
-            if sels is not None:
-                c.set_gpu_attrs(attrs); c.set_selectors(sels.reshape(-1, R.SEL_MAX_INS))
-            c.set_shard_map(bounds, stray_rank=0)
-            if world > 1:
-                c.set_shard_pairs(max_pairs)
-                c.shard_export(max(1, w.n_out), 0, want_handle=False)
-        if world > 1:
-            for c in self.ctxs:
-                c.peer_import_local(self.ctxs)
-
-    def close(self):
-        for c in self.ctxs:
-            c.close()
-
-    def enqueue(self, claims, pod_off, cand_nodes=None, cand_off=None, flags=0, n_pair=None):
-        """The call on every rank (enqueued on all of them first, then waited for); returns one buffer per rank."""
-        import torch
-        n_pod = len(pod_off) - 1
-        if n_pair is None:
-            n_pair = n_pod * self.w.n_node if cand_nodes is None else int(cand_off[-1])
-        keep = [_dev(claims) if len(claims) else torch.zeros(16, dtype=torch.uint8, device="cuda:0"), _dev(pod_off)]
-        if cand_nodes is not None:
-            keep += [_dev(cand_nodes) if len(cand_nodes) else torch.zeros(4, dtype=torch.uint8, device="cuda:0"), _dev(cand_off)]
-        outs = [torch.full(((n_pair + 7) // 8 + 16,), SENTINEL, dtype=torch.uint8, device="cuda:0") for _ in self.ctxs]
-        torch.cuda.synchronize()                         # (the contexts' streams do not wait for torch's)
-        for c, o in zip(self.ctxs, outs):
-            c.unsuitable_global_device(keep[0].data_ptr(), len(claims), keep[1].data_ptr(), n_pod,
-                                       keep[2].data_ptr() if cand_nodes is not None else None,
-                                       keep[3].data_ptr() if cand_nodes is not None else None, n_pair, o.data_ptr(), flags)
-        return outs, keep, n_pair
-
-    def call(self, *a, **k):
-        outs, _, n_pair = self.enqueue(*a, **k)
-        for c in self.ctxs:
-            c.sync()
-        res = []
-        nb = (n_pair + 7) // 8
-        for r, o in enumerate(outs):
-            h = o.cpu().numpy()
-            assert (h[nb:] == SENTINEL).all(), f"rank {r} wrote past ceil(n_pair/8) bytes"
-            if n_pair % 8:
-                assert h[nb - 1] >> (n_pair % 8) == 0, f"rank {r}: bits past n_pair are set"
-            res.append(h[:nb])
-        return res
-
-
-def _bounds(n_node, world, kind):
-    if kind == "even":
-        return [n_node * r // world for r in range(world)] + [n_node]
-    if kind == "uneven":                                  # rank 0 a sliver, the last rank most of it
-        b = [0] + [min(n_node, 1 + 2 * r * r) for r in range(1, world)] + [n_node]
-        return sorted(b)
-    # "empty": an empty range in the middle and one at the end
-    b = [0] + [n_node // 2] * (world - 1) + [n_node]
-    if world > 2:
-        b[-2] = n_node
-    return b
-
-
-def _pod_cuts(rng, n_claim, n_cut, big=False):
-    cuts = np.unique(np.concatenate([[0, n_claim], rng.integers(0, n_claim, n_cut)])).astype(np.uint32)
-    cuts = np.insert(cuts, 3, cuts[3])                   # an empty pod
-    if big and n_claim > 100:
-        cuts = np.unique(np.concatenate([cuts[cuts < 40], cuts[cuts > 80]])).astype(np.uint32)   # one pod of > 32 claims
-        cuts = np.insert(cuts, 1, cuts[1])
-    return cuts
-
-
-def _candidates(rng, n_pod, n_node):
-    per = rng.integers(0, 9, n_pod)
-    per[::7] = 0                                          # pods with no candidate
-    cand_off = np.zeros(n_pod + 1, dtype=np.uint32); cand_off[1:] = np.cumsum(per)
-    cand_nodes = rng.integers(0, n_node + 4, int(cand_off[-1])).astype(np.uint32)   # some name no node
-    if len(cand_nodes) > 3:
-        cand_nodes[1] = cand_nodes[0]                     # a repeated candidate
-        cand_nodes[2] = 0xFFFFFFFF
-    return cand_nodes, cand_off
+def _call(W, claims, pod_off, cn=None, co=None, flags=0):
+    return S.unsuitable(W, claims, pod_off, None if cn is None else (cn, co), flags, sentinel=SENTINEL)
 
 
 @pytest.mark.parametrize("world", [1, 2, 3, 4])
@@ -124,23 +37,23 @@ def test_matches_oracle(pkg, oracle, world, workload):
         attrs, sels = pkg.synth.with_selectors(w, world)
         inv = oracle.allocate(w.gpus, w.node_off, w.table, w.claims[:800])[1]        # partly filled
         claims = w.claims.copy()
-        pod_off = _pod_cuts(rng, w.n_claim, 700, big=True)
+        pod_off = S.pod_cuts(rng, w.n_claim, 700, big=True)
         for p in range(len(pod_off) - 1):                 # most pods on one node, as a scheduler would ask
             if rng.integers(0, 10):
                 claims["node"][pod_off[p]: pod_off[p + 1]] = claims["node"][pod_off[p]]
     n_pod, n_node = len(pod_off) - 1, w.n_node
-    cn, co = _candidates(rng, n_pod, n_node)
-    dn, do = _dense(n_pod, n_node)
-    bounds = _bounds(n_node, world, "uneven" if world == 3 else "even")
-    W = World(pkg, w, world, bounds, max(n_pod * n_node, int(co[-1])), inv, attrs, sels)
+    cn, co = S.candidates(rng, n_pod, n_node)
+    dn, do = S.dense(n_pod, n_node)
+    bounds = S.bounds(n_node, world, "uneven" if world == 3 else "even")
+    W = _world(pkg, w, world, bounds, max(n_pod * n_node, int(co[-1])), inv, attrs, sels)
     oracle.set_selectors(attrs, sels)
     try:
         for flags, oflags in ((0, 0), (pkg.api.F_EXHAUSTIVE, oracle.F_EXHAUSTIVE)):
             ref_dense = oracle.unsuitable(inv, w.node_off, w.table, claims, pod_off, dn, do, flags=oflags)
             ref_cand = oracle.unsuitable(inv, w.node_off, w.table, claims, pod_off, cn, co, flags=oflags)
-            for r, got in enumerate(W.call(claims, pod_off, flags=flags)):
+            for r, got in enumerate(_call(W, claims, pod_off, flags=flags)):
                 assert got.tobytes() == ref_dense.tobytes(), f"dense, flags {flags}, rank {r}"
-            for r, got in enumerate(W.call(claims, pod_off, cn, co, flags=flags)):
+            for r, got in enumerate(_call(W, claims, pod_off, cn, co, flags=flags)):
                 assert got.tobytes() == ref_cand.tobytes(), f"candidates, flags {flags}, rank {r}"
             assert ref_dense.any() and not np.all(ref_dense == 0xFF)
     finally:
@@ -159,18 +72,14 @@ def test_sharded_allocate_then_unsuitable(pkg, oracle, world):
     n_pod = 600
     pods = w.claims[:n_pod].copy()
     pod_off = np.arange(n_pod + 1, dtype=np.uint32)
-    W = World(pkg, w, world, bounds, n_pod * w.n_node)
+    W = _world(pkg, w, world, bounds, n_pod * w.n_node)
     try:
-        d = _dev(w.claims)
-        for c in W.ctxs:
-            c.allocate_global_device(d.data_ptr(), w.n_claim, None, w.n_out, 0)
-        for c in W.ctxs:
-            c.gather_read(np.zeros(w.n_out, dtype=R.OUT_DTYPE))
+        S.allocate(W, w.claims, None, w.n_out)
         _, real = oracle.allocate(w.gpus, w.node_off, w.table, w.claims)
-        dn, do = _dense(n_pod, w.n_node)
+        dn, do = S.dense(n_pod, w.n_node)
         for flags, oflags in ((0, 0), (pkg.api.F_EXHAUSTIVE, oracle.F_EXHAUSTIVE)):
             ref = oracle.unsuitable(real, w.node_off, w.table, pods, pod_off, dn, do, flags=oflags)
-            for r, got in enumerate(W.call(pods, pod_off, flags=flags)):
+            for r, got in enumerate(_call(W, pods, pod_off, flags=flags)):
                 assert got.tobytes() == ref.tobytes(), f"rank {r}, flags {flags}"
         stale = W.ctxs[0].unsuitable(pods, pod_off)
         ref = oracle.unsuitable(real, w.node_off, w.table, pods, pod_off, dn, do)
@@ -184,14 +93,14 @@ def test_edge_shapes(pkg, oracle):
     w = pkg.synth.mixed(1200, 23, 71, invalid=True)
     rng = np.random.default_rng(5)
     world = 4
-    W = World(pkg, w, world, _bounds(w.n_node, world, "empty"), 4096)
+    W = _world(pkg, w, world, S.bounds(w.n_node, world, "empty"), 4096)
     try:
         for n_pod in (1, 3, 5, 7):                        # dense n_pair = n_pod * 23: odd, never a multiple of 8
             pod_off = np.linspace(0, 40 * n_pod, n_pod + 1).astype(np.uint32)
             c = w.claims[: pod_off[-1]]
-            dn, do = _dense(n_pod, w.n_node)
+            dn, do = S.dense(n_pod, w.n_node)
             ref = oracle.unsuitable(w.gpus, w.node_off, w.table, c, pod_off, dn, do)
-            for got in W.call(c, pod_off):
+            for got in _call(W, c, pod_off):
                 assert got.tobytes() == ref.tobytes()
         for n_pair in (1, 31, 33, 63, 65, 4096):
             pod_off = np.array([0, 2, 2, 5], dtype=np.uint32)
@@ -200,18 +109,15 @@ def test_edge_shapes(pkg, oracle):
             c = w.claims[:5]
             for flags, oflags in ((0, 0), (pkg.api.F_EXHAUSTIVE, oracle.F_EXHAUSTIVE)):
                 ref = oracle.unsuitable(w.gpus, w.node_off, w.table, c, pod_off, cand_nodes, cand_off, flags=oflags)
-                for got in W.call(c, pod_off, cand_nodes, cand_off, flags=flags):
+                for got in _call(W, c, pod_off, cand_nodes, cand_off, flags=flags):
                     assert got.tobytes() == ref.tobytes(), f"n_pair {n_pair}"
         # n_pair == 0 (two pods without candidates): nothing to decide, no output buffer needed, the next call still works
-        z = _dev(np.zeros(3, dtype=np.uint32))
-        for c in W.ctxs:
-            c.unsuitable_global_device(0, 0, z.data_ptr(), 2, z.data_ptr(), z.data_ptr(), 0, 0, 0)
-        for c in W.ctxs:
-            c.sync()
+        z = S.dev(np.zeros(3, dtype=np.uint32))
+        W.each(lambda r, c: c.unsuitable_global_device(0, 0, z.data_ptr(), 2, z.data_ptr(), z.data_ptr(), 0, 0, 0))
         pod_off = np.array([0, 3], dtype=np.uint32)
-        dn, do = _dense(1, w.n_node)
+        dn, do = S.dense(1, w.n_node)
         ref = oracle.unsuitable(w.gpus, w.node_off, w.table, w.claims[:3], pod_off, dn, do)
-        for got in W.call(w.claims[:3], pod_off):
+        for got in _call(W, w.claims[:3], pod_off):
             assert got.tobytes() == ref.tobytes()
     finally:
         W.close()
@@ -220,14 +126,14 @@ def test_edge_shapes(pkg, oracle):
 def test_world1_equals_single_inventory_call(pkg, oracle):
     w = pkg.synth.mixed(2000, 29, 88)
     rng = np.random.default_rng(1)
-    pod_off = _pod_cuts(rng, w.n_claim, 500, big=True)
-    cn, co = _candidates(rng, len(pod_off) - 1, w.n_node)
-    W = World(pkg, w, 1, [0, w.n_node], 0)
+    pod_off = S.pod_cuts(rng, w.n_claim, 500, big=True)
+    cn, co = S.candidates(rng, len(pod_off) - 1, w.n_node)
+    W = _world(pkg, w, 1, [0, w.n_node], 0)
     try:
         c = W.ctxs[0]
         for flags in (0, pkg.api.F_EXHAUSTIVE):
-            assert W.call(w.claims, pod_off, flags=flags)[0].tobytes() == c.unsuitable(w.claims, pod_off, flags=flags).tobytes()
-            assert W.call(w.claims, pod_off, cn, co, flags=flags)[0].tobytes() == \
+            assert _call(W, w.claims, pod_off, flags=flags)[0].tobytes() == c.unsuitable(w.claims, pod_off, flags=flags).tobytes()
+            assert _call(W, w.claims, pod_off, cn, co, flags=flags)[0].tobytes() == \
                 c.unsuitable(w.claims, pod_off, cn, co, flags=flags).tobytes()
     finally:
         W.close()
@@ -242,32 +148,27 @@ def test_consecutive_calls_interleaved_with_sharded_allocates(pkg, oracle):
     w = pkg.synth.cfg2(4000, 30)
     ranges = pkg.shard.plan(w.claims["node"], w.n_node, world)
     bounds = [x[0] for x in ranges] + [ranges[-1][1]]
-    W = World(pkg, w, world, bounds, 500 * w.n_node)
+    W = _world(pkg, w, world, bounds, 500 * w.n_node)
     rng = np.random.default_rng(3)
     try:
-        d = _dev(w.claims)
         state = w.gpus
         for step, (n_pod, flags) in enumerate([(500, 0), (37, pkg.api.F_EXHAUSTIVE), (211, 0), (1, 0), (333, pkg.api.F_EXHAUSTIVE), (64, 0)]):
             if step % 2 == 0:                             # a sharded allocate on the live inventory (part of the claims)
                 lo = step * 300
                 part = w.claims[lo: lo + 600]
-                dp = _dev(part)
-                for c in W.ctxs:
-                    c.allocate_global_device(dp.data_ptr(), len(part), None, len(part), 0)
-                for c in W.ctxs:
-                    c.gather_read(np.zeros(len(part), dtype=R.OUT_DTYPE))
+                S.allocate(W, part, None, len(part))
                 _, state = oracle.allocate(state, w.node_off, w.table, part)
             pods = w.claims[rng.integers(0, w.n_claim, n_pod)]
             pod_off = np.arange(n_pod + 1, dtype=np.uint32)
             oflags = oracle.F_EXHAUSTIVE if flags else 0
             if step % 3 == 1:
-                cn, co = _candidates(rng, n_pod, w.n_node)
+                cn, co = S.candidates(rng, n_pod, w.n_node)
                 ref = oracle.unsuitable(state, w.node_off, w.table, pods, pod_off, cn, co, flags=oflags)
-                got = W.call(pods, pod_off, cn, co, flags=flags)
+                got = _call(W, pods, pod_off, cn, co, flags=flags)
             else:
-                dn, do = _dense(n_pod, w.n_node)
+                dn, do = S.dense(n_pod, w.n_node)
                 ref = oracle.unsuitable(state, w.node_off, w.table, pods, pod_off, dn, do, flags=oflags)
-                got = W.call(pods, pod_off, flags=flags)
+                got = _call(W, pods, pod_off, flags=flags)
             for r, g in enumerate(got):
                 assert g.tobytes() == ref.tobytes(), f"step {step} rank {r}"
     finally:
@@ -285,9 +186,9 @@ def test_errors(pkg, oracle):
     n_pod = 20
     pod_off = np.arange(0, 3 * n_pod + 1, 3, dtype=np.uint32)
     claims = w.claims[: pod_off[-1]]
-    dn, do = _dense(n_pod, w.n_node)
+    dn, do = S.dense(n_pod, w.n_node)
     ref = oracle.unsuitable(w.gpus, w.node_off, w.table, claims, pod_off, dn, do)
-    d_c, d_p = _dev(claims), _dev(pod_off)
+    d_c, d_p = S.dev(claims), S.dev(pod_off)
     bits = torch.zeros(64, dtype=torch.uint8, device="cuda:0")
     torch.cuda.synchronize()
 
@@ -307,33 +208,28 @@ def test_errors(pkg, oracle):
         c.set_shard_pairs(10)
         c.shard_export(16, 0, want_handle=False)
         assert c._lib.dra_set_shard_pairs(c._h, 100) == E.E_STATE   # after the export
-    W = World(pkg, w, world, bounds, n_pod * w.n_node)
+    W = _world(pkg, w, world, bounds, n_pod * w.n_node)
     try:
         c0 = W.ctxs[0]
         assert raw(c0, n_pair=n_pod * w.n_node + 1) == E.E_INVAL                 # dense n_pair != n_pod * n_node
         assert raw(c0, flags=0x80) == E.E_INVAL                                  # unknown flag
         assert raw(c0, n_pod=n_pod + 1, n_pair=(n_pod + 1) * w.n_node) == E.E_INVAL   # above max_pairs
         assert raw(c0, cn=d_p.data_ptr()) == E.E_INVAL                           # cand_nodes without cand_off
-        for r, got in enumerate(W.call(claims, pod_off)):
+        for r, got in enumerate(_call(W, claims, pod_off)):
             assert got.tobytes() == ref.tobytes(), f"after host-side errors, rank {r}"
         # device-side: pod_off not monotone / not spanning the claims, cand_off not spanning the pairs
         bad_po = pod_off.copy(); bad_po[5] = bad_po[7] + 1
         short_po = pod_off.copy(); short_po[-1] -= 1
-        cn, co = _candidates(np.random.default_rng(0), n_pod, w.n_node)
+        cn, co = S.candidates(np.random.default_rng(0), n_pod, w.n_node)
         bad_co = co.copy(); bad_co[-1] -= 1
         for po, c_nodes, c_off, n_pair in ((bad_po, None, None, None), (short_po, None, None, None),
                                            (pod_off, cn, bad_co, int(co[-1]))):
-            outs, keep, n_pair = W.enqueue(claims, po, c_nodes, c_off, n_pair=n_pair)
-            codes = []
-            for c in W.ctxs:
-                try:
-                    c.sync(); codes.append(0)
-                except E.DraError as e:
-                    codes.append(e.code)
-            assert codes == [E.E_INVAL] * world, codes
+            n_pair = n_pod * w.n_node if n_pair is None else n_pair
+            outs = S.unsuitable(W, claims, po, None if c_nodes is None else (c_nodes, c_off), n_pair=n_pair,
+                                sentinel=SENTINEL, expect=E.E_INVAL)
             for o in outs:                                # nothing was evaluated: every bit zero
-                assert not o.cpu().numpy()[: (n_pair + 7) // 8].any()
-            for r, got in enumerate(W.call(claims, pod_off)):
+                assert not o[0][: (n_pair + 7) // 8].any()
+            for r, got in enumerate(_call(W, claims, pod_off)):
                 assert got.tobytes() == ref.tobytes(), f"after a device-side error, rank {r}"
     finally:
         W.close()

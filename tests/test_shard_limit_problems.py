@@ -13,7 +13,7 @@ import limit_problems as LP
 import shard_limit_problems as SP
 from test_gpu_limits import N_EX, ONE_WAVE_FUSED_MAX
 from test_gpu_paths import STAGED_CAP
-from test_gpu_shard import _kept
+from shard_world import kept as _kept
 
 R = SP.R
 
