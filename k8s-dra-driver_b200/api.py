@@ -407,13 +407,16 @@ class Context:
                     run_out_off=None, cand_nodes=None, cand_off=None, max_victims: int = 8, flags: int = 0):
         """preempt() with disruption budgets (spec §14, "Disruption budgets"): run_pdb[r] the budget running pod r counts
         against (PDB_NONE for none; None: no array), pdb_allowed[b] each budget's disruptionsAllowed (None: no budgets).
-        Returns preempt()'s six outputs, then pair_violations and pod_violations (uint32)."""
+        Returns preempt()'s six outputs, then pair_violations and pod_violations (uint32).  Raises ValueError when run_pdb
+        is given and does not hold one entry per running pod (the library reads one per running pod)."""
         c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
         po = np.ascontiguousarray(pod_off, dtype=np.uint32)
         pr = np.ascontiguousarray(prio, dtype=np.int32)
         n_pod = len(po) - 1
         run = _running(run_claims, run_pod_off, run_prio, run_out, run_out_off)
         rp = None if run_pdb is None else np.ascontiguousarray(run_pdb, dtype=np.uint32)
+        if rp is not None and len(rp) != run.n_pod:
+            raise ValueError(f"run_pdb holds {len(rp)} entries for {run.n_pod} running pods")
         al = None if pdb_allowed is None else np.ascontiguousarray(pdb_allowed, dtype=np.int32)
         bud = DisruptionBudgets(None if rp is None or not len(rp) else rp.ctypes.data,
                                 None if al is None or not len(al) else al.ctypes.data, 0 if al is None else len(al))

@@ -348,16 +348,19 @@ PREEMPT_NAMES = ("pair_status", "pair_victims", "pod_node", "pod_status", "n_vic
 
 
 def preempt(W, claims, pod_off, prio, run, cands=None, max_victims=16, flags=0, pairs=True, pdb=False, bud=None,
-            sentinel=0x5C, expect=0):
+            sentinel=0x5C, expect=0, asked=None):
     """dra_preempt_batch_global_device, or with pdb=True dra_preempt_pdb_batch_global_device with the budgets `bud` (None:
     a null struct): every rank's six or eight outputs, the per-pair ones None unless `pairs`.  `run`: the running pods of
-    every rank, or a list of one per rank."""
+    every rank, or a list of one per rank.  asked: one flag per output in PREEMPT_NAMES order, False for an output passed
+    as NULL (read back as None), instead of what `pairs` says."""
     n_pod = len(pod_off) - 1
     cn, co = (None, None) if cands is None else cands
     n_pair = n_pod * W.n_node if co is None else int(co[-1])
     keep = [dev(claims), dev(pod_off), dev(prio)] + ([None, None] if cn is None else [dev(cn), dev(co)])
     sizes = [n_pair, n_pair * 4, n_pod * 4, n_pod, n_pod * 4, n_pod * max_victims * 4] + ([n_pair * 4, n_pod * 4] if pdb else [])
-    asked = [pairs, pairs, True, True, True, True] + ([pairs, True] if pdb else [])
+    if asked is None:
+        asked = [pairs, pairs, True, True, True, True] + ([pairs, True] if pdb else [])
+    assert len(asked) == len(sizes)
     outs = W.outputs(sizes, sentinel)
 
     def call(r, c):

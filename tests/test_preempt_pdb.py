@@ -111,6 +111,126 @@ def test_a_budget_spanning_two_nodes_starts_full_on_each_pair(allowed):
     assert list(got[6]) == [1 - allowed] * 2 and list(got[7]) == [1 - allowed] and list(got[2]) == [1]
 
 
+@pytest.mark.parametrize("allowed", [0, 1])
+def test_members_at_or_above_the_pending_priority_do_not_count(allowed):
+    """One GPU: 1g pods of priority 20 (slice 1) and 10 (slice 0), a 3g pod of priority 5 (slices 4-7) and a 1g pod of
+    priority 3 (slice 2), all of one budget.  A 3g pod of priority 10 can only start at 4, so the priority-5 pod goes.  V
+    is (priority 5, priority 3): the two members before it on the node are not in V and do not count, so with one
+    eviction allowed the victim is clean; with none it is violating."""
+    g, off = R.make_inventory([1], mig=True)
+    rc, rpo, rpr, ro = mig_running([(0, 0, 1, R.GI_1_SLICE, 10), (0, 1, 1, R.GI_1_SLICE, 20), (0, 4, 4, R.GI_3_SLICE, 5),
+                                    (0, 2, 1, R.GI_1_SLICE, 3)], off)
+    g, t = occupied(g, rc, ro), R.default_table()
+    got = run_both(g, off, t, _mig(R, [R.GI_3_SLICE]), np.array([0, 1], np.uint32), [10], rc, rpo, rpr, ro, [0] * 4,
+                   [allowed])
+    assert list(got[4]) == [1] and list(got[5][0][:2]) == [2, NONE]
+    assert list(got[6]) == [1 - allowed] and list(got[7]) == [1 - allowed]
+
+
+def _seven_slivers():
+    """One GPU, 1g pods at slices 0..6 with priorities 7..1 (V order is index order); budget 0 holds pods 0, 3 and 5,
+    budget 1 pods 2 and 6, pods 1 and 4 none: budget 0's chain passes a NONE member and a member of budget 1 each step"""
+    g, off = R.make_inventory([1], mig=True)
+    rc, rpo, rpr, ro = mig_running([(0, s, 1, R.GI_1_SLICE, 7 - s) for s in range(7)], off)
+    return occupied(g, rc, ro), off, R.default_table(), rc, rpo, rpr, ro, [0, NONE, 1, 0, NONE, 0, 1]
+
+
+@pytest.mark.parametrize("allowed0", [0, 1, 2, 3])
+def test_a_budget_chain_through_none_and_other_budgets(allowed0):
+    """Budget 1 allows nothing, budget 0 allowed0.  A 7g pod evicts all seven: budget 1's two and budget 0's members past
+    the first allowed0 are violating.  A 3g pod (slices 0-3 or 4-7): the violating members are tried first; pod 2
+    (slice 2) stays, so the pod goes to 4-7 and pods 4, 5, 6 go — two of them violating until budget 0 allows three."""
+    g, off, t, rc, rpo, rpr, ro, pdb = _seven_slivers()
+    po = np.array([0, 1], np.uint32)
+    got = run_both(g, off, t, _mig(R, [R.GI_7_SLICE]), po, [10], rc, rpo, rpr, ro, pdb, [allowed0, 0])
+    assert list(got[4]) == [7] and list(got[5][0][:7]) == list(range(7))
+    assert list(got[7]) == [max(0, 3 - allowed0) + 2]
+    got = run_both(g, off, t, _mig(R, [R.GI_3_SLICE]), po, [10], rc, rpo, rpr, ro, pdb, [allowed0, 0])
+    assert list(got[4]) == [3] and list(got[5][0][:4]) == [4, 5, 6, NONE]
+    assert list(got[7]) == [2 if allowed0 < 3 else 1]
+
+
+@pytest.mark.parametrize("cands", [None, [[0, 1]], [[1, 0]]])
+def test_the_highest_victim_index_is_the_lowest_when_the_violating_phase_goes_first(cands):
+    """Two one-GPU nodes, each held by two 3g pods of priority 5: pods 0 and 3 on node 0, pods 1 and 2 on node 1.  Pods 3
+    and 2 allow nothing, so each node's violating phase evicts its higher-index pod first.  A 7g pod evicts both on either
+    node: one violation, the same priorities and count, so the latest start decides on the LOWEST index at the highest
+    priority (node 0: 0, node 1: 1), and node 1 wins; on the first victim's index (3 against 2) node 0 would."""
+    g, off = R.make_inventory([1, 1], mig=True)
+    rc, rpo, rpr, ro = mig_running([(0, 0, 4, R.GI_3_SLICE, 5), (1, 0, 4, R.GI_3_SLICE, 5), (1, 4, 4, R.GI_3_SLICE, 5),
+                                    (0, 4, 4, R.GI_3_SLICE, 5)], off)
+    g, t = occupied(g, rc, ro), R.default_table()
+    got = run_both(g, off, t, _mig(R, [R.GI_7_SLICE]), np.array([0, 1], np.uint32), [10], rc, rpo, rpr, ro,
+                   [NONE, NONE, 1, 0], [0, 0], cands=cands)
+    assert list(got[0]) == [P.EVICT, P.EVICT] and list(got[6]) == [1, 1]
+    assert list(got[2]) == [1] and list(got[4]) == [2] and list(got[5][0][:3]) == [1, 2, NONE] and list(got[7]) == [1]
+
+
+def sum_world(a_first):
+    """Spec §14's 64-bit-sum shape: two one-GPU nodes, each held by two 3g pods; A's priorities {10, -9}, B's {10, -11}
+    (running pods 0, 1 on A and 2, 3 on B).  A 7g pod of priority 11 evicts both on either node.  Returns the problem's
+    arrays and B's node."""
+    g, off = R.make_inventory([1, 1], mig=True)
+    na, nb = (0, 1) if a_first else (1, 0)
+    rc, rpo, rpr, ro = mig_running([(na, 0, 4, R.GI_3_SLICE, 10), (na, 4, 4, R.GI_3_SLICE, -9),
+                                    (nb, 0, 4, R.GI_3_SLICE, 10), (nb, 4, 4, R.GI_3_SLICE, -11)], off)
+    return occupied(g, rc, ro), off, R.default_table(), rc, rpo, rpr, ro, nb
+
+
+@pytest.mark.parametrize("a_first", [True, False])
+def test_the_sum_decides_on_tied_violations_and_violations_beat_the_sum(a_first):
+    g, off, t, rc, rpo, rpr, ro, nb = sum_world(a_first)
+    c, po = _mig(R, [R.GI_7_SLICE]), np.array([0, 1], np.uint32)
+    for cands in (None, [[0, 1]], [[1, 0]]):
+        tie = run_both(g, off, t, c, po, [11], rc, rpo, rpr, ro, [0, NONE, 0, NONE], [0], cands=cands)
+        assert list(tie[2]) == [nb] and list(tie[6]) == [1, 1] and list(tie[5][0][:3]) == [2, 3, NONE]
+        over = run_both(g, off, t, c, po, [11], rc, rpo, rpr, ro, [NONE, NONE, 0, 0], [1], cands=cands)
+        assert list(over[2]) == [1 - nb] and list(over[7]) == [0] and list(over[5][0][:3]) == [0, 1, NONE]
+
+
+def warp_world():
+    """Spec §14's choice-past-one-warp shape: three one-GPU nodes, each held by one 7g pod: running pod 0 on node 2
+    (priority 5), 1 on node 1 (priority 6), 2 on node 0 (priority 5).  Without budgets a 7g pod picks node 0."""
+    g, off = R.make_inventory([1, 1, 1], mig=True)
+    rc, rpo, rpr, ro = mig_running([(2, 0, 8, R.GI_7_SLICE, 5), (1, 0, 8, R.GI_7_SLICE, 6), (0, 0, 8, R.GI_7_SLICE, 5)],
+                                   off)
+    return occupied(g, rc, ro), off, R.default_table(), rc, rpo, rpr, ro
+
+
+WARP_TIE, WARP_OVER = ([0, 0, 0], [0]), ([0, NONE, 0], [0])    # every pair one violation; node 1's pair none
+
+
+def warp_cands():
+    """Two pods' 70 candidates: pod 0's only violation-free pair (node 1) at position 33 (lane 1's second slot), pod 1's
+    at 63 and 64 (lane 31's second slot, lane 0's third); nodes 0 and 2 and strays everywhere else"""
+    other = [0, 2, 3, NONE]
+    a = [other[k % 4] for k in range(70)]
+    a[33] = 1
+    b = [other[(k // 2) % 4] for k in range(70)]
+    b[63] = b[64] = 1
+    return [a, b]
+
+
+def test_violations_beat_a_lower_highest_priority_and_ties_keep_the_later_keys():
+    g, off, t, rc, rpo, rpr, ro = warp_world()
+    c, po = _mig(R, [R.GI_7_SLICE]), np.array([0, 1], np.uint32)
+    tie = run_both(g, off, t, c, po, [100], rc, rpo, rpr, ro, *WARP_TIE)
+    assert list(tie[6]) == [1, 1, 1] and list(tie[2]) == [0] and list(tie[5][0][:2]) == [2, NONE]
+    over = run_both(g, off, t, c, po, [100], rc, rpo, rpr, ro, *WARP_OVER)
+    assert list(over[6]) == [1, 0, 1] and list(over[2]) == [1] and list(over[5][0][:2]) == [1, NONE]
+    assert list(over[7]) == [0]
+
+
+def test_the_fewest_violations_past_one_warp():
+    g, off, t, rc, rpo, rpr, ro = warp_world()
+    c, po = _mig(R, [R.GI_7_SLICE] * 2), np.array([0, 1, 2], np.uint32)
+    cands = warp_cands()
+    over = run_both(g, off, t, c, po, [100, 100], rc, rpo, rpr, ro, *WARP_OVER, cands=cands, max_victims=2)
+    assert list(over[2]) == [1, 1] and list(over[7]) == [0, 0] and over[5].tolist() == [[1, NONE], [1, NONE]]
+    tie = run_both(g, off, t, c, po, [100, 100], rc, rpo, rpr, ro, *WARP_TIE, cands=cands, max_victims=2)
+    assert list(tie[2]) == [0, 0] and list(tie[7]) == [1, 1] and tie[5].tolist() == [[2, NONE], [2, NONE]]
+
+
 @pytest.mark.parametrize("seed", range(12))
 def test_no_budgets_is_preempt_byte_for_byte(seed):
     w, c, po, prio, cands = _small_world(seed)
