@@ -207,10 +207,7 @@ struct dra_ctx {
     volatile uint32_t* h_sc_counts = nullptr;   // mapped host copy of the last call's counts
     uint32_t* h_sc_counts_dev = nullptr;
     uint2* d_gtable = nullptr; size_t cap_gtable = 0;   // result table when no peers are set up (world 1)
-    // 16 words, zeroed when allocated: [4] the shard compaction's tile ticket, [8] k_bucket_scan8's, [10, 11]
-    // k_bucket_scan_rows' ticket and epoch; and the 64-bit counters of the counter walks (walk_counter), each zeroed
-    // before its launch: [6, 7] preemption, [12, 13] UnsuitableNodes, [14, 15] pod capacity
-    uint32_t* d_ticket = nullptr;
+    uint32_t* d_ticket = nullptr;               // 16 words, zeroed when allocated (dra_ctx_create): see Ticket
     ShardSizes shard_req{};                     // the sizes the setters asked for, reserved by the next peer_setup
     ShardSizes shard_rsv{};                     // the sizes the last peer_setup reserved
     // sharded UnsuitableNodes: bit exchange in the peer buffer ([staging x2: world slices of uns_stride words][flags])
@@ -265,6 +262,19 @@ int fail(dra_ctx* c, int code, const char* fmt, ...) {
 #define CU(call)                                                                                       \
     do { cudaError_t e_ = (call);                                                                     \
          if (e_ != cudaSuccess) return fail(ctx, DRA_E_CUDA, "%s: %s", #call, cudaGetErrorString(e_)); } while (0)
+
+// The words of d_ticket: the shard compaction's tile ticket, k_bucket_scan8's ticket, k_bucket_scan_rows' ticket and epoch
+// (two words), and the 64-bit counters of the counter walks (walk_counter, two words each)
+enum Ticket : int { TK_COMPACT = 4, TK_WALK_PREEMPT = 6, TK_SCAN8 = 8, TK_SCAN_ROWS = 10, TK_WALK_UNSUITABLE = 12, TK_WALK_CAPACITY = 14 };
+
+// The 64-bit walk counter at d_ticket word `word` (even: 8-aligned), zeroed on the stream for the walk about to be
+// enqueued.  64 bits because a walk may cover up to 2^32 - 1 pairs and every warp takes one more value past its end: a
+// 32-bit counter would wrap and walk the pairs again.
+int walk_counter(dra_ctx* ctx, Ticket word, unsigned long long*& work) {
+    work = reinterpret_cast<unsigned long long*>(ctx->d_ticket + word);
+    CU(cudaMemsetAsync(work, 0, 8, ctx->stream));
+    return DRA_OK;
+}
 
 template <class T>
 int grow(dra_ctx* ctx, T*& p, size_t& cap, size_t need, size_t slack = 16) {
@@ -472,7 +482,6 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
                     CU(cudaFuncSetAttribute(k_bucket_hist8<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                     ctx->hist8_smem_set = (int)smem;
                 }
-                if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, ctx->stream)); }
                 if (t.T == H8_TILE) k_bucket_hist8<false><<<t.n_tiles, 256, smem, ctx->stream>>>(d_claims, n_claim, n_node, ctx->d_hist, ctx->d_rank, n_dev, t.T);
                 else k_bucket_hist8<true><<<t.n_tiles, 256, smem, ctx->stream>>>(d_claims, n_claim, n_node, ctx->d_hist, ctx->d_rank, n_dev, t.T);
                 ctx->chain |= t.T == H8_TILE ? DRA_K_HIST8 : DRA_K_HIST8_MULTI;
@@ -482,10 +491,10 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
                 if (!no_rows && (size_t)t.n_tiles * (n_node + 1) > (size_t)512 * 1024) {
                     const uint32_t n_cta = (n_node + 1 + 31) / 32;
                     if (ctx->cap_scan_status < n_cta) return fail(ctx, DRA_E_STATE, "scan status words not allocated (ensure_batch)");
-                    CU(launch_k(k_bucket_scan_rows, dim3(n_cta), dim3(256), 0, ctx->stream, pdl, ctx->d_hist, t.n_tiles, n_node, ctx->d_claim_off, ctx->d_ticket + 10, ctx->d_scan_status, err));
+                    CU(launch_k(k_bucket_scan_rows, dim3(n_cta), dim3(256), 0, ctx->stream, pdl, ctx->d_hist, t.n_tiles, n_node, ctx->d_claim_off, ctx->d_ticket + TK_SCAN_ROWS, ctx->d_scan_status, err));
                     ctx->chain |= DRA_K_SCAN_ROWS;
                 } else {
-                    CU(launch_k(k_bucket_scan8, dim3((n_node + 1 + 7) / 8), dim3(256), 0, ctx->stream, pdl, ctx->d_hist, t.n_tiles, n_node, ctx->d_claim_off, ctx->d_ticket + 8));
+                    CU(launch_k(k_bucket_scan8, dim3((n_node + 1 + 7) / 8), dim3(256), 0, ctx->stream, pdl, ctx->d_hist, t.n_tiles, n_node, ctx->d_claim_off, ctx->d_ticket + TK_SCAN8));
                     ctx->chain |= DRA_K_SCAN8;
                 }
                 prof.mark();
@@ -676,39 +685,34 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
     return DRA_OK;
 }
 
-// Lanes per (pod, node) pair for k_unsuitable and the preemption pair kernels: one per GPU of the widest node
+// Lanes per (pod, node) pair for the pair kernels (k_unsuitable, preemption's, pod capacity's): one per GPU of the widest node
 uint32_t pair_width(const dra_ctx* ctx) { return ctx->max_width <= 8 ? 8u : (ctx->max_width <= 16 ? 16u : 32u); }
 
-template <bool WIN>
-void launch_unsuitable_w(dra_ctx* ctx, const UnsArgs& a, uint32_t W, uint32_t grid) {
-    if (a.exhaustive) {
-        if (W == 8) k_unsuitable<8, 8, true, WIN><<<grid, 256, 0, ctx->stream>>>(a);
-        else if (W == 16) k_unsuitable<8, 16, true, WIN><<<grid, 256, 0, ctx->stream>>>(a);
-        else k_unsuitable<8, 32, true, WIN><<<grid, 256, 0, ctx->stream>>>(a);
-    } else {
-        if (W == 8) k_unsuitable<8, 8, false, WIN><<<grid, 256, 0, ctx->stream>>>(a);
-        else if (W == 16) k_unsuitable<8, 16, false, WIN><<<grid, 256, 0, ctx->stream>>>(a);
-        else k_unsuitable<8, 32, false, WIN><<<grid, 256, 0, ctx->stream>>>(a);
-    }
+// f(std::integral_constant<int, W>{}) for W = pair_width: f launches the pair kernel instantiated for W
+template <class F>
+void at_pair_width(const dra_ctx* ctx, F&& f) {
+    const uint32_t W = pair_width(ctx);
+    if (W == 8) f(std::integral_constant<int, 8>{});
+    else if (W == 16) f(std::integral_constant<int, 16>{});
+    else f(std::integral_constant<int, 32>{});
 }
 
-// The 64-bit walk counter at d_ticket word `word` (even: 8-aligned).  64 bits because a walk may cover up to 2^32 - 1
-// pairs and every warp takes one more value past its end: a 32-bit counter would wrap and walk the pairs again.
-unsigned long long* walk_counter(dra_ctx* ctx, int word) { return reinterpret_cast<unsigned long long*>(ctx->d_ticket + word); }
+// A pair kernel's grid for n pairs (or pods): 8 warps of 32 / W pairs per CTA, at most 8 CTAs per SM
+uint32_t pair_grid(const dra_ctx* ctx, uint32_t n) {
+    const uint32_t per_cta = 8 * (32 / pair_width(ctx));
+    return std::max(1u, std::min((n + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
+}
 
-// k_unsuitable over n_walk pairs (win: the sharded call's node window, n_walk = a.n_walk; else n_walk = a.n_pair); lanes per
-// pair from the widest node: 8 lanes = 4 pairs per warp.  Enqueues only.
+// k_unsuitable over a.n_walk pairs (win: the sharded call's node window and gate; else the whole inventory).  Enqueues only.
 int launch_unsuitable(dra_ctx* ctx, UnsArgs& a, bool win) {
-    const uint32_t W = pair_width(ctx);
-    const uint32_t per_cta = 8 * (32 / W);
-    const uint32_t n_walk = win ? a.n_walk : a.n_pair;
-    const uint32_t grid = std::max(1u, std::min((n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
-    if (a.exhaustive) {
-        a.work = walk_counter(ctx, 12);
-        CU(cudaMemsetAsync(a.work, 0, 8, ctx->stream));
-    }
-    if (win) launch_unsuitable_w<true>(ctx, a, W, grid);
-    else launch_unsuitable_w<false>(ctx, a, W, grid);
+    const uint32_t grid = pair_grid(ctx, a.n_walk);
+    if (a.exhaustive) { if (int rc = walk_counter(ctx, TK_WALK_UNSUITABLE, a.work)) return rc; }
+    at_pair_width(ctx, [&](auto w) {
+        constexpr int W = decltype(w)::value;
+        const auto k = win ? (a.exhaustive ? k_unsuitable<8, W, true, true> : k_unsuitable<8, W, false, true>)
+                           : (a.exhaustive ? k_unsuitable<8, W, true, false> : k_unsuitable<8, W, false, false>);
+        k<<<grid, 256, 0, ctx->stream>>>(a);
+    });
     ctx->launches += 1;
     return DRA_OK;
 }
@@ -1041,50 +1045,36 @@ int launch_running_lists(dra_ctx* ctx, PreArgs& a, Prof& prof, bool walk) {
     return DRA_OK;
 }
 
-// k_pods_preempt over s's pairs (none: no launch), pair_width lanes per pair, 8 warps per CTA.  Enqueues only.
+// k_pods_preempt over s's pairs (none: no launch).  Enqueues only.
 int launch_preempt_pairs(dra_ctx* ctx, PreArgs a, const PreShard& s) {
     if (!s.n_walk) return DRA_OK;
-    cudaStream_t st = ctx->stream;
-    if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, st)); }
-    a.work = walk_counter(ctx, 6);
-    CU(cudaMemsetAsync(a.work, 0, 8, st));
-    const uint32_t W = pair_width(ctx), per_cta = 8 * (32 / W);
-    const uint32_t grid = std::max(1u, std::min((s.n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
-    if (W == 8) k_pods_preempt<8, 8><<<grid, 256, 0, st>>>(a, s);
-    else if (W == 16) k_pods_preempt<8, 16><<<grid, 256, 0, st>>>(a, s);
-    else k_pods_preempt<8, 32><<<grid, 256, 0, st>>>(a, s);
+    if (int rc = walk_counter(ctx, TK_WALK_PREEMPT, a.work)) return rc;
+    const uint32_t grid = pair_grid(ctx, s.n_walk);
+    at_pair_width(ctx, [&](auto w) { k_pods_preempt<8, decltype(w)::value><<<grid, 256, 0, ctx->stream>>>(a, s); });
     ctx->launches += 1;
     return DRA_OK;
 }
 
 // k_pods_preempt_victims for a's pods: pod p's chosen pair at choice[p * cstride], its row at rows + p * rstride.  Enqueues only.
 void launch_preempt_victims(dra_ctx* ctx, const PreArgs& a, const uint32_t* choice, uint32_t cstride, uint32_t* rows, uint32_t rstride) {
-    const uint32_t W = pair_width(ctx), per_cta = 8 * (32 / W);
-    const uint32_t grid = std::max(1u, std::min((a.n_pod + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
-    cudaStream_t st = ctx->stream;
-    if (W == 8) k_pods_preempt_victims<8, 8><<<grid, 256, 0, st>>>(a, choice, cstride, rows, rstride);
-    else if (W == 16) k_pods_preempt_victims<8, 16><<<grid, 256, 0, st>>>(a, choice, cstride, rows, rstride);
-    else k_pods_preempt_victims<8, 32><<<grid, 256, 0, st>>>(a, choice, cstride, rows, rstride);
+    const uint32_t grid = pair_grid(ctx, a.n_pod);
+    at_pair_width(ctx, [&](auto w) {
+        k_pods_preempt_victims<8, decltype(w)::value><<<grid, 256, 0, ctx->stream>>>(a, choice, cstride, rows, rstride);
+    });
     ctx->launches += 1;
 }
 
-// k_pods_capacity over a's walk (none: no launch), pair_width lanes per pair, 8 warps per CTA, then k_pods_capacity_sum
-// over its pods when a per-pod output is asked for.  Enqueues only.
+// k_pods_capacity over a's walk (none: no launch), then k_pods_capacity_sum over its pods when a per-pod output is asked
+// for.  Enqueues only.
 int launch_capacity(dra_ctx* ctx, CapArgs a) {
-    cudaStream_t st = ctx->stream;
     if (a.n_walk) {
-        if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, st)); }
-        a.work = walk_counter(ctx, 14);
-        CU(cudaMemsetAsync(a.work, 0, 8, st));
-        const uint32_t W = pair_width(ctx), per_cta = 8 * (32 / W);
-        const uint32_t grid = std::max(1u, std::min((a.n_walk + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
-        if (W == 8) k_pods_capacity<8, 8><<<grid, 256, 0, st>>>(a);
-        else if (W == 16) k_pods_capacity<8, 16><<<grid, 256, 0, st>>>(a);
-        else k_pods_capacity<8, 32><<<grid, 256, 0, st>>>(a);
+        if (int rc = walk_counter(ctx, TK_WALK_CAPACITY, a.work)) return rc;
+        const uint32_t grid = pair_grid(ctx, a.n_walk);
+        at_pair_width(ctx, [&](auto w) { k_pods_capacity<8, decltype(w)::value><<<grid, 256, 0, ctx->stream>>>(a); });
         ctx->launches += 1;
     }
     if (a.pod_total || a.pod_nodes) {
-        k_pods_capacity_sum<<<(a.n_pod + 7) / 8, 256, 0, st>>>(a);
+        k_pods_capacity_sum<<<(a.n_pod + 7) / 8, 256, 0, ctx->stream>>>(a);
         ctx->launches += 1;
     }
     return DRA_OK;
@@ -1687,11 +1677,12 @@ int dra_unsuitable_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
         CU(cudaMemsetAsync(ctx->d_bits, 0, words * 4, ctx->stream));
         UnsArgs a; memset(&a, 0, sizeof a);
         a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.n_pod = n_pod;
-        a.cand_nodes = ctx->d_cand_nodes; a.cand_off = ctx->d_cand_off; a.pair_pod = ctx->d_pair_pod; a.n_pair = n_pair;
+        a.cand_nodes = ctx->d_cand_nodes; a.pair_pod = ctx->d_pair_pod;
+        a.cand_off = dense ? nullptr : ctx->d_cand_off;   // (not staged: k_unsuitable reads only whether it is nullptr)
         a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.tbl = ctx->d_tbl; a.bits = ctx->d_bits;
         a.sel = sel_of(ctx);
-        a.dense = dense ? 1u : 0u;
         a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
+        a.n_walk = n_pair;                                 // (the window is the whole inventory)
         Prof prof(ctx);
         if ((rc = launch_unsuitable(ctx, a, false))) return rc;
         prof.mark();
@@ -1893,7 +1884,7 @@ int dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
     a.pair_viol = pair_violations ? ctx->d_pre_pairviol : nullptr; a.pod_viol = pod_violations ? ctx->d_pre_podviol : nullptr;
     Prof prof(ctx);
     if ((rc = launch_running_lists(ctx, a, prof, false))) return rc;
-    const PreShard whole{0u, ctx->n_node, n_pair, 0u, nullptr, nullptr};
+    const PreShard whole{0u, ctx->n_node, n_pair, 0u, nullptr, nullptr};   // every node: the walk index is the pair index
     if ((rc = launch_preempt_pairs(ctx, a, whole))) return rc;
     cudaStream_t st = ctx->stream;
     k_pre_choose<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a);
@@ -2224,6 +2215,12 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
     ctx->uns_stride = (uint32_t)(((size_t)z.uns_pairs + 127) / 128 * 4);     // words, whole 16-byte units
     if (ctx->uns_stride) {
         reserve(ctx->uns_x, (size_t)ctx->world * ctx->uns_stride * 4, (size_t)ctx->uns_stride * 4, (size_t)PEER_MAX * 4);
+        if (int rc = preload(ctx, {(const void*)k_uns_prep, (const void*)k_unsuitable<8, 8, false, true>,
+                                   (const void*)k_unsuitable<8, 16, false, true>, (const void*)k_unsuitable<8, 32, false, true>,
+                                   (const void*)k_unsuitable<8, 8, true, true>, (const void*)k_unsuitable<8, 16, true, true>,
+                                   (const void*)k_unsuitable<8, 32, true, true>, (const void*)k_peer_push},
+                             {(const void*)k_uns_merge}, false))
+            return rc;
         // the call's own buffers at full size now: growing one inside the call would cudaFree the old one, which waits for
         // the whole device — where a peer's merge may already be spinning for this rank's push (ranks sharing a device)
         int rc;
@@ -2322,6 +2319,31 @@ PeerExchange bind_exchange(dra_ctx* ctx, PeerRegion& rg) {
     x.my_stage = (const uint4*)(ctx->peer_local + stage);
     x.my_flags = (const uint32_t*)(ctx->peer_local + rg.flags);
     return x;
+}
+
+// The next call of the exchange whose region is rg, with this rank's n4 units at src pushed to every peer (k_peer_push).
+// World 1 (no gather): no peers, nothing pushed.
+PeerExchange push_slice(dra_ctx* ctx, PeerRegion& rg, bool gather, const uint4* src, uint32_t n4) {
+    if (!gather) return PeerExchange{};
+    const PeerExchange x = bind_exchange(ctx, rg);
+    k_peer_push<<<push_grid(ctx, n4), 256, 0, ctx->stream>>>(x, src, 0u, n4);
+    ctx->launches += 1;
+    return x;
+}
+
+// The first kernel of the sharded pair calls (k_uns_prep): pod_off and cand_off (nullptr: dense form) checked, and in the
+// candidate form pair -> pod into d_upair_pod.  Its fault gates the pair kernel.
+void launch_uns_prep(dra_ctx* ctx, const uint32_t* d_pod_off, const uint32_t* d_cand_off, uint32_t n_pod, uint32_t n_claim,
+                     uint32_t n_pair) {
+    k_uns_prep<<<std::max(1u, (n_pod + 7) / 8), 256, 0, ctx->stream>>>(d_pod_off, d_cand_off, n_pod, n_claim, n_pair,
+                                                                       ctx->d_upair_pod, err_of(ctx));
+    ctx->launches += 1;
+}
+
+// A merge's shard bounds: rank r owns nodes [bounds[r], bounds[r + 1]); world 1 (no gather): every node
+void merge_bounds(const dra_ctx* ctx, bool gather, uint32_t (&bounds)[PEER_MAX + 1]) {
+    bounds[0] = 0; bounds[1] = ctx->n_node;
+    if (gather) for (int r = 0; r <= ctx->world; ++r) bounds[r] = ctx->shard_bounds[r];
 }
 
 // The result table of a global Allocate call: at world > 1 the table of g, a gather of a new epoch, else this context's own
@@ -2575,7 +2597,6 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
         ctx->h_sc_counts = (volatile uint32_t*)hp;
         CU(cudaHostGetDevicePointer((void**)&ctx->h_sc_counts_dev, hp, 0));
     }
-    if (!ctx->d_ticket) { CU(cudaMalloc((void**)&ctx->d_ticket, 64)); CU(cudaMemsetAsync(ctx->d_ticket, 0, 64, ctx->stream)); }
     if (!ctx->d_rank_slots) { CU(cudaMalloc((void**)&ctx->d_rank_slots, 2 * PEER_MAX * 4)); CU(cudaMemsetAsync(ctx->d_rank_slots, 0, 2 * PEER_MAX * 4, ctx->stream)); }
     const bool counted = gather && ctx->shard_map_on;          // every rank counts every rank's slots: the gather needs no header
     uint2* table = nullptr; PktGather g; memset(&g, 0, sizeof g);
@@ -2596,7 +2617,7 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
     sa.node_lo = ctx->shard_lo; sa.node_hi = ctx->shard_hi; sa.n_node_global = ctx->n_node; sa.take_stray = ctx->shard_stray;
     sa.have_off = d_out_off != nullptr;
     sa.cclaims = ctx->d_cclaims; sa.coff = ctx->d_coff; sa.cap = (uint32_t)std::min<size_t>(ctx->cap_cclaims, 0xFFFFFFFFu);
-    sa.status = ctx->d_sc_status; sa.ticket = ctx->d_ticket + 4; sa.n_tiles = n_tiles; sa.epoch = ctx->shard_epoch;
+    sa.status = ctx->d_sc_status; sa.ticket = ctx->d_ticket + TK_COMPACT; sa.n_tiles = n_tiles; sa.epoch = ctx->shard_epoch;
     sa.counts = ctx->d_sc_counts; sa.h_counts = ctx->h_sc_counts_dev; sa.err = err_of(ctx);
     if (getenv("DRA_TIMELINE")) {                              // instrumentation: two words, read back with dra_debug_shard_times
         if (!ctx->d_sc_times) CU(cudaMalloc((void**)&ctx->d_sc_times, 16));
@@ -2653,17 +2674,13 @@ int dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     // world > 1: peer_setup sized both for max_pairs, so these never reallocate there (no cudaFree while peers wait)
     if ((rc = grow(ctx, ctx->d_ubits, ctx->cap_ubits, n_words4))) return rc;
     if (!dense && (rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, n_pair))) return rc;
-    const Err err = err_of(ctx);
     CU(cudaMemsetAsync(ctx->d_ubits, 0, n_words4 * 4, ctx->stream));
-    k_uns_prep<<<std::max(1u, (n_pod + 7) / 8), 256, 0, ctx->stream>>>(d_pod_off, dense ? nullptr : d_cand_off, n_pod, n_claim, n_pair,
-                                                                       ctx->d_upair_pod, err);
-    ctx->launches += 1;
+    launch_uns_prep(ctx, d_pod_off, d_cand_off, n_pod, n_claim, n_pair);
     UnsArgs a; memset(&a, 0, sizeof a);
     a.claims = (const uint4*)d_claims; a.pod_off = d_pod_off; a.n_pod = n_pod;
-    a.cand_nodes = d_cand_nodes; a.cand_off = d_cand_off; a.pair_pod = ctx->d_upair_pod; a.n_pair = n_pair;
+    a.cand_nodes = d_cand_nodes; a.cand_off = d_cand_off; a.pair_pod = ctx->d_upair_pod;
     a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.tbl = ctx->d_tbl; a.bits = ctx->d_ubits;
     a.sel = sel_of(ctx);
-    a.dense = dense ? 1u : 0u;
     a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
     a.node_lo = ctx->shard_lo; a.n_win = ctx->shard_hi - ctx->shard_lo;
     a.n_walk = dense ? n_pod * a.n_win : n_pair;           // (n_pod * n_win <= n_pod * n_node = n_pair)
@@ -2674,12 +2691,7 @@ int dra_unsuitable_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     UnsMerge m; memset(&m, 0, sizeof m);
     m.bits = ctx->d_ubits; m.out = d_suitable_bits;
     m.n_words = (uint32_t)n_words; m.n_bytes = (uint32_t)(((size_t)n_pair + 7) / 8); m.stride = ctx->uns_stride;
-    const PeerExchange x = gather ? bind_exchange(ctx, ctx->uns_x) : PeerExchange{};   // world 1: no peers
-    if (gather) {
-        const uint32_t n4 = (uint32_t)(n_words4 / 4);
-        k_peer_push<<<push_grid(ctx, n4), 256, 0, ctx->stream>>>(x, (const uint4*)ctx->d_ubits, 0u, n4);
-        ctx->launches += 1;
-    }
+    const PeerExchange x = push_slice(ctx, ctx->uns_x, gather, (const uint4*)ctx->d_ubits, (uint32_t)(n_words4 / 4));
     k_uns_merge<<<wait_grid(ctx, (n_words + 1023) / 1024), 256, 0, ctx->stream>>>(x, m);
     ctx->launches += 1;
     cudaError_t e = cudaGetLastError();
@@ -2946,7 +2958,7 @@ int dra_preempt_pdb_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cla
     const uint32_t lo = gather ? ctx->shard_lo : 0u, hi = gather ? ctx->shard_hi : ctx->n_node;   // world 1: every node
     const bool want_pairs = d_pair_status || d_pair_victims || d_pair_violations;
     PreShard s; memset(&s, 0, sizeof s);
-    s.node_lo = lo; s.node_hi = hi; s.n_walk = dense ? n_pod * (hi - lo) : n_pair;
+    s.node_lo = lo; s.n_win = hi - lo; s.n_walk = dense ? n_pod * s.n_win : n_pair;
     s.stride = 2 + (max_victims + 3) / 4; s.part = ctx->d_spre_part;
     s.pairs = want_pairs ? reinterpret_cast<uint2*>(ctx->d_spre_part + 1 + (size_t)n_pod * s.stride) : nullptr;
 
@@ -2955,9 +2967,7 @@ int dra_preempt_pdb_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cla
     a.pair_pod = dense ? nullptr : ctx->d_upair_pod; a.max_victims = max_victims;
     pre_budgets(ctx, a, budgets);
     Prof prof(ctx);
-    k_uns_prep<<<std::max(1u, (n_pod + 7) / 8), 256, 0, st>>>(d_pod_off, dense ? nullptr : d_cand_off, n_pod, n_claim, n_pair,
-                                                              ctx->d_upair_pod, a.err);
-    ctx->launches += 1;
+    launch_uns_prep(ctx, d_pod_off, d_cand_off, n_pod, n_claim, n_pair);
     if ((rc = launch_running_lists(ctx, a, prof, false))) return rc;
     if ((rc = launch_preempt_pairs(ctx, a, s))) return rc;
     k_spre_reduce<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, s);
@@ -2973,18 +2983,13 @@ int dra_preempt_pdb_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cla
     m.claims = a.claims; m.pod_off = d_pod_off; m.n_pod = n_pod;
     m.cand_nodes = a.cand_nodes; m.cand_off = a.cand_off; m.n_pair = n_pair; m.n_node = ctx->n_node;
     m.sel = a.sel; m.max_victims = max_victims; m.gate = a.gate;
-    m.bounds[0] = 0; m.bounds[1] = ctx->n_node;
-    if (gather) for (int r = 0; r <= ctx->world; ++r) m.bounds[r] = ctx->shard_bounds[r];
+    merge_bounds(ctx, gather, m.bounds);
     m.pair_status = d_pair_status; m.pair_victims = d_pair_victims;
     m.pod_node = d_pod_node; m.pod_status = d_pod_status; m.n_victims = d_n_victims; m.victims = max_victims ? d_victims : nullptr;
     m.pair_viol = d_pair_violations; m.pod_viol = d_pod_violations;
-    const PeerExchange x = gather ? bind_exchange(ctx, ctx->pre_x) : PeerExchange{};   // world 1: no peers
-    if (gather) {
-        m.slice4 = (uint32_t)(ctx->pre_x.slice / 16);
-        const uint32_t n4 = (uint32_t)(1 + (size_t)n_pod * s.stride + (want_pairs ? ((size_t)n_pair + 1) / 2 : 0));
-        k_peer_push<<<push_grid(ctx, n4), 256, 0, st>>>(x, s.part, 0u, n4);
-        ctx->launches += 1;
-    }
+    const uint32_t n4 = (uint32_t)(1 + (size_t)n_pod * s.stride + (want_pairs ? ((size_t)n_pair + 1) / 2 : 0));
+    const PeerExchange x = push_slice(ctx, ctx->pre_x, gather, s.part, n4);
+    if (gather) m.slice4 = (uint32_t)(ctx->pre_x.slice / 16);
     const size_t work = std::max(((size_t)n_pod + 7) / 8, want_pairs ? ((size_t)n_pair + 255) / 256 : 0);
     k_spre_merge<<<wait_grid(ctx, work), 256, 0, st>>>(x, m);
     ctx->launches += 1;
@@ -3069,26 +3074,20 @@ int dra_pod_capacity_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cl
     a.pair_stop = d_pair_stop ? reinterpret_cast<uint8_t*>(part + 1 + copies4) : nullptr;
     a.gate = gate;
     Prof prof(ctx);
-    k_uns_prep<<<std::max(1u, (n_pod + 7) / 8), 256, 0, st>>>(d_pod_off, dense ? nullptr : d_cand_off, n_pod, n_claim, n_pair,
-                                                              ctx->d_upair_pod, err_of(ctx));
-    ctx->launches += 1;
+    launch_uns_prep(ctx, d_pod_off, d_cand_off, n_pod, n_claim, n_pair);
     if ((rc = launch_capacity(ctx, a))) return rc;
     prof.mark();
     CapMerge m; memset(&m, 0, sizeof m);
     m.part = part; m.cand_nodes = a.cand_nodes; m.cand_off = a.cand_off;
     m.n_pod = n_pod; m.n_pair = n_pair; m.n_node = ctx->n_node;
-    m.bounds[0] = 0; m.bounds[1] = ctx->n_node;
-    if (gather) for (int r = 0; r <= ctx->world; ++r) m.bounds[r] = ctx->shard_bounds[r];
+    merge_bounds(ctx, gather, m.bounds);
     m.gate = gate;
     m.pair_copies = d_pair_copies; m.pair_stop = d_pair_stop; m.pod_total = (unsigned long long*)d_pod_total; m.pod_nodes = d_pod_nodes;
-    const PeerExchange x = gather ? bind_exchange(ctx, ctx->scap_x) : PeerExchange{};   // world 1: no peers
     if (gather) {
         m.slice4 = (uint32_t)(ctx->scap_x.slice / 16);
         CU(cudaMemcpyAsync(part, gate, 4, cudaMemcpyDeviceToDevice, st));   // the header: this rank's fault word
-        const uint32_t n4 = (uint32_t)(1 + copies4 + stops4);
-        k_peer_push<<<push_grid(ctx, n4), 256, 0, st>>>(x, part, 0u, n4);
-        ctx->launches += 1;
     }
+    const PeerExchange x = push_slice(ctx, ctx->scap_x, gather, part, (uint32_t)(1 + copies4 + stops4));
     k_scap_merge<<<wait_grid(ctx, (n_pod + 7) / 8), 256, 0, st>>>(x, m);
     ctx->launches += 1;
     cudaError_t e = cudaGetLastError();

@@ -2641,14 +2641,20 @@ struct PodArgs {
     uint32_t n_node, exhaustive; SelCtx sel; Err err;
 };
 
+// The placement table into the CTA's shared tbl_s, by its NT threads; every thread returns once it is in place
+template <int NT>
+__device__ __forceinline__ void stage_table(uint32_t* tbl_s, const uint32_t* tbl) {
+    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += NT) tbl_s[i] = __ldg(&tbl[i]);
+    __syncthreads();
+}
+
 // one warp per node, one lane per GPU; the node's pods in input order
 template <int WPC>
 __global__ void __launch_bounds__(WPC * 32)
 k_pods(const PodArgs a) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
     pdl_wait();
-    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
-    __syncthreads();
+    stage_table<WPC * 32>(tbl_s, a.tbl);
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     for (uint32_t node = blockIdx.x * WPC + wid; node < a.n_node; node += gridDim.x * WPC) {
         const uint32_t g0 = __ldg(&a.node_off[node]), ng = __ldg(&a.node_off[node + 1]) - g0;
@@ -2798,8 +2804,7 @@ __global__ void __launch_bounds__(WPC * 32)
 k_pods_place(const PlaceArgs a, const PlaceShard sh) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
     if constexpr (SHARD) { if (__ldcg(sh.gated)) return; }
-    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
-    __syncthreads();
+    stage_table<WPC * 32>(tbl_s, a.tbl);
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t w0 = blockIdx.x * WPC + (threadIdx.x >> 5), n_warp = gridDim.x * WPC;
     const bool dense = a.cand_off == nullptr, have_off = a.out_off != nullptr;
@@ -2933,19 +2938,15 @@ k_pods_place(const PlaceArgs a, const PlaceShard sh) {
 
 struct UnsArgs {
     const uint4* claims; const uint32_t* pod_off; uint32_t n_pod;
-    const uint32_t* cand_nodes; const uint32_t* cand_off; const uint32_t* pair_pod;   // pair -> pod
-    uint32_t n_pair;
+    const uint32_t* cand_nodes; const uint32_t* cand_off; const uint32_t* pair_pod;   // cand_off == nullptr: dense form
     const uint4* inv; const uint32_t* node_off; uint32_t n_node; const uint32_t* tbl;
     uint32_t* bits;     // n_pair bits, zeroed by the caller, set with atomicOr
     SelCtx sel;
-    uint32_t dense;     // 1: every pod x every node, pair = pod * n_node + node (cand arrays unused)
     uint32_t exhaustive; // spec §12: pod evaluation with the backtracking search
     unsigned long long* work;   // EXH: next unclaimed pair (zeroed by the caller) — searches differ by orders of magnitude
                                 //      in length, so the warps take their pairs from a counter instead of a fixed stride
-    // sharded call only (k_unsuitable<..., WIN = true>):
-    uint32_t node_lo, n_win;   // node window: only pairs whose node lies in [node_lo, node_lo + n_win) are evaluated
-    uint32_t n_walk;           // pairs the kernel walks: dense n_pod * n_win (mapped back to pod * n_node + node), else n_pair
-    const uint32_t* gate;      // *gate != 0: the inputs failed their device-side check, evaluate nothing
+    uint32_t node_lo, n_win, n_walk;   // the node window (pair_decode; WIN = false: [0, n_node)), the pairs walked
+    const uint32_t* gate;      // sharded call only: *gate != 0: the inputs failed their device-side check, evaluate nothing
 };
 
 struct GlobalGet {
@@ -2964,37 +2965,59 @@ __device__ __forceinline__ uint32_t walk_fetch(unsigned long long* work, uint32_
     return __shfl_sync(FULLMASK, nxt, 0);
 }
 
+// Walk index `walk` of a pair walk over the node window [node_lo, node_lo + n_win) as pod, node and pair.  Dense form (cand_off
+// nullptr): walk w is pod w / n_win at node node_lo + w % n_win.  Candidate form: the walk index is the pair index.  False
+// only for a candidate on another rank's node (of the inventory, outside the window); one naming no node is the caller's.
+__device__ __forceinline__ bool pair_decode(uint32_t walk, uint32_t node_lo, uint32_t n_win, uint32_t n_node, const uint32_t* cand_off,
+                                            const uint32_t* cand_nodes, const uint32_t* pair_pod, uint32_t& pod, uint32_t& node, uint32_t& pair) {
+    if (!cand_off) { pod = walk / n_win; node = node_lo + (walk - pod * n_win); pair = pod * n_node + node; return true; }
+    pair = walk; node = __ldg(&cand_nodes[pair]); pod = __ldg(&pair_pod[pair]);
+    return !(node < n_node && node - node_lo >= n_win);
+}
+
+// Pod p's pairs [k0, k1): its candidates, or dense the columns [lo, lo + n_win) of its row.  T: the caller's index width.
+template <class T>
+__device__ __forceinline__ void pod_pairs(const uint32_t* cand_off, uint32_t p, uint32_t n_node, uint32_t lo, uint32_t n_win, T& k0, T& k1) {
+    if (cand_off) { k0 = __ldg(&cand_off[p]); k1 = __ldg(&cand_off[p + 1]); } else { k0 = (T)p * n_node + lo; k1 = k0 + n_win; }
+}
+
+// The node of pod p's pair k: its candidate's node, or dense (cand_off nullptr) the pair's column
+template <class T>
+__device__ __forceinline__ uint32_t pair_node(const uint32_t* cand_off, const uint32_t* cand_nodes, T k, uint32_t p, uint32_t n_node) {
+    return cand_off ? __ldg(&cand_nodes[k]) : (uint32_t)(k - (T)p * n_node);
+}
+
+// A lane of a pair kernel with W lanes per pair: lane gl of group grp, whose lanes are gbase .. gbase + W - 1 (gmask)
+struct LaneGroup { uint32_t lane, grp, gl, gbase, gmask; };
+template <int W>
+__device__ __forceinline__ LaneGroup lane_group() {
+    const uint32_t lane = threadIdx.x & 31, grp = lane / W, gbase = grp * W;
+    return {lane, grp, lane - gbase, gbase, W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase)};
+}
+
 // W lanes per (pod, candidate) pair: 32/W pairs share a warp (W = 8 for the usual <= 8 GPUs per node), each
-// group running its own claim loop with group-wide ballots.  dense = every pod against every node
-// (pair = pod * n_node + node): no candidate arrays at all.
-// WIN: the node window and the gate of the sharded call (own instantiations: with the window the exhaustive kernel needs
-// 81 registers instead of 80, which costs dra_unsuitable_batch a third of its CTAs per SM).
+// group running its own claim loop with group-wide ballots.  Dense form: every pod against every node, no candidate arrays.
+// WIN: the node window and the gate of the sharded call, else the window [0, n_node) (own instantiations: with the window
+// the exhaustive kernel needs 81 registers instead of 78, which costs dra_unsuitable_batch a third of its CTAs per SM).
 template <int WPC, int W, bool EXH, bool WIN>          // EXH: spec §12 (own instantiation: the default kernel stays as lean as it was)
 __global__ void __launch_bounds__(WPC * 32, 2)
 k_unsuitable(const UnsArgs a) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
     if (WIN && a.gate && __ldcg(a.gate)) return;
-    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
-    __syncthreads();
+    stage_table<WPC * 32>(tbl_s, a.tbl);
     constexpr uint32_t G = 32 / W;
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const uint32_t grp = lane / W, gl = lane % W, gbase = grp * W;
-    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
-    const uint32_t stride = gridDim.x * WPC * G;
-    const uint32_t n_walk = WIN ? a.n_walk : a.n_pair;
+    const auto [lane, grp, gl, gbase, gmask] = lane_group<W>();
+    const uint32_t wid = threadIdx.x >> 5, stride = gridDim.x * WPC * G, n_walk = a.n_walk;
+    const uint32_t node_lo = WIN ? a.node_lo : 0u, n_win = WIN ? a.n_win : a.n_node;
     // the stride steps at most to n_walk: a plain pw += stride wraps past 2^32 near the top of the range and walks again
     for (uint32_t pw = (blockIdx.x * WPC + wid) * G; ; pw += min(stride, n_walk - pw)) {
         if (EXH) pw = walk_fetch<G>(a.work, lane);
         if (pw >= n_walk) break;
         const uint32_t walk = pw + grp;
         if (walk >= n_walk) continue;                                    // whole group skips together
-        uint32_t pod, node, pair = walk;
-        if (a.dense) {
-            if (WIN) { pod = walk / a.n_win; node = a.node_lo + (walk - pod * a.n_win); pair = pod * a.n_node + node; }
-            else { pod = pair / a.n_node; node = pair - pod * a.n_node; }
-        }
-        else { pod = __ldg(&a.pair_pod[pair]); node = __ldg(&a.cand_nodes[pair]); }
-        if ((WIN ? node - a.node_lo >= a.n_win : node >= a.n_node) || pod >= a.n_pod) continue;   // unknown node (or another rank's): unsuitable here
+        uint32_t pod, node, pair;
+        if (!pair_decode(walk, node_lo, n_win, a.n_node, a.cand_off, a.cand_nodes, a.pair_pod, pod, node, pair) ||
+            node - node_lo >= n_win || pod >= a.n_pod) continue;         // another rank's node, or none: unsuitable here
         const uint32_t c0 = __ldg(&a.pod_off[pod]);
         const uint32_t cnt = __ldg(&a.pod_off[pod + 1]) - c0;
         const uint32_t g0 = __ldg(&a.node_off[node]);
@@ -3566,8 +3589,8 @@ constexpr uint32_t PRE_VSHIFT = 3, PRE_ST_MASK = (1u << PRE_VSHIFT) - 1u;
 // The pair kernel's node window and the sharded call's partials (layout at k_spre_reduce).  The single-inventory call:
 // the window [0, n_node), n_walk = n_pair, no partials.
 struct PreShard {
-    uint32_t node_lo, node_hi;    // the pairs to judge are those of the nodes in [node_lo, node_hi), or of no node
-    uint32_t n_walk;              // pairs the evaluation walks: dense n_pod * (node_hi - node_lo), else n_pair
+    uint32_t node_lo, n_win;      // the pairs to judge are those of the nodes in [node_lo, node_lo + n_win), or of no node
+    uint32_t n_walk;              // pairs the evaluation walks: dense n_pod * n_win, else n_pair
     uint32_t stride;              // uint4 units per pod partial: 2 + ceil(max_victims / 4)
     uint4* part;                  // the partials (header, pods)
     uint2* pairs;                 // the window's pair results (nullptr: the caller asked for none)
@@ -3809,33 +3832,23 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
 }
 
 // W lanes per (pod, candidate) pair, 32/W pairs per warp, in k_unsuitable's layout; pairs are taken from a counter, since
-// a pair costs from one evaluation to |V| + 2 of them.  The pairs of s's node window: dense, the window's columns; with
-// candidates, every pair but those naming another rank's node (a pair naming no node is judged NO, as k_pre_choose
-// reads every pair).
+// a pair costs from one evaluation to |V| + 2 of them.  The pairs of s's node window (pair_decode); a pair naming no node
+// is judged NO, as k_pre_choose reads every pair.
 template <int WPC, int W>
 __global__ void __launch_bounds__(WPC * 32, 2)
 k_pods_preempt(const PreArgs a, const PreShard s) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
     if (__ldcg(a.gate)) return;
-    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
-    __syncthreads();
+    stage_table<WPC * 32>(tbl_s, a.tbl);
     constexpr uint32_t G = 32 / W;
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t grp = lane / W, gbase = grp * W;
-    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
-    const uint32_t n_win = s.node_hi - s.node_lo;
+    const auto [lane, grp, gl, gbase, gmask] = lane_group<W>();
     while (true) {
         const uint32_t pw = walk_fetch<G>(a.work, lane);
         if (pw >= s.n_walk) break;
         const uint32_t walk = pw + grp;
         if (walk >= s.n_walk) continue;                                  // whole group skips together
         uint32_t pod, node, pair;
-        if (!a.cand_off) { pod = walk / n_win; node = s.node_lo + (walk - pod * n_win); pair = pod * a.n_node + node; }
-        else {
-            pair = walk; node = __ldg(&a.cand_nodes[pair]);
-            if (node < a.n_node && node - s.node_lo >= n_win) continue;   // another rank's node
-            pod = __ldg(&a.pair_pod[pair]);
-        }
+        if (!pair_decode(walk, s.node_lo, s.n_win, a.n_node, a.cand_off, a.cand_nodes, a.pair_pod, pod, node, pair)) continue;
         const PreSum r = pre_pair<W>(a, tbl_s, pod, node, lane, gmask, gbase, false, nullptr);
         if (lane == gbase) {
             const uint32_t nv = r.st == DRA_PRE_EVICT ? r.count : 0u;   // (r.viol is 0 unless EVICT)
@@ -3923,13 +3936,13 @@ k_pre_choose(const PreArgs a) {
     if (__ldcg(a.gate)) return;
     const uint32_t lane = threadIdx.x & 31, p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (p >= a.n_pod) return;
-    const bool dense = a.cand_off == nullptr;
-    const uint32_t k0 = dense ? p * a.n_node : __ldg(&a.cand_off[p]), k1 = dense ? k0 + a.n_node : __ldg(&a.cand_off[p + 1]);
+    uint32_t k0, k1;
+    pod_pairs(a.cand_off, p, a.n_node, 0u, a.n_node, k0, k1);
     uint32_t k; uint4 bs;
     const uint32_t st = pre_reduce(a, p, k0, k1, lane, k, bs);
     if (lane != 0) return;
     a.pod_status[p] = (uint8_t)st;
-    a.pod_node[p] = k == DRA_GPU_NONE ? DRA_GPU_NONE : dense ? k - k0 : __ldg(&a.cand_nodes[k]);
+    a.pod_node[p] = k == DRA_GPU_NONE ? DRA_GPU_NONE : pair_node(a.cand_off, a.cand_nodes, k, p, a.n_node);
     a.n_victims[p] = st == DRA_PRE_EVICT ? bs.y : 0u;
     if (a.pod_viol) a.pod_viol[p] = st == DRA_PRE_EVICT ? bs.x >> PRE_VSHIFT : 0u;
     a.choice[p] = st == DRA_PRE_EVICT ? k : DRA_GPU_NONE;
@@ -3943,18 +3956,16 @@ __global__ void __launch_bounds__(WPC * 32, 2)
 k_pods_preempt_victims(const PreArgs a, const uint32_t* choice, const uint32_t cstride, uint32_t* rows, const uint32_t rstride) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
     if (__ldcg(a.gate)) return;
-    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
-    __syncthreads();
+    stage_table<WPC * 32>(tbl_s, a.tbl);
     constexpr uint32_t G = 32 / W;
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const uint32_t grp = lane / W, gbase = grp * W;
-    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
+    const uint32_t wid = threadIdx.x >> 5;
+    const auto [lane, grp, gl, gbase, gmask] = lane_group<W>();
     for (uint32_t pw = (blockIdx.x * WPC + wid) * G; pw < a.n_pod; pw += gridDim.x * WPC * G) {
         const uint32_t p = pw + grp;
         if (p >= a.n_pod) continue;
         const uint32_t k = __ldcg(&choice[(size_t)p * cstride]);
         if (k == DRA_GPU_NONE) continue;
-        const uint32_t node = a.cand_off ? __ldg(&a.cand_nodes[k]) : k - p * a.n_node;
+        const uint32_t node = pair_node(a.cand_off, a.cand_nodes, k, p, a.n_node);
         (void)pre_pair<W>(a, tbl_s, p, node, lane, gmask, gbase, true, rows + (size_t)p * rstride);
     }
 }
@@ -4041,8 +4052,7 @@ __global__ void __launch_bounds__(WPC * 32, 1)
 k_pods_preempt_place(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
     if (__ldcg(a.gate)) return;
-    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&pl.tbl[i]);
-    __syncthreads();
+    stage_table<WPC * 32>(tbl_s, pl.tbl);
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t w0 = blockIdx.x * WPC + (threadIdx.x >> 5), n_warp = gridDim.x * WPC;
     const bool dense = pl.cand_off == nullptr, have_off = pl.out_off != nullptr;
@@ -4276,11 +4286,9 @@ k_spre_reduce(const PreArgs a, const PreShard s) {
     if (gate) return;
     const uint32_t lane = threadIdx.x & 31, p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (p >= a.n_pod) return;
-    const bool dense = a.cand_off == nullptr;
-    const uint32_t n_win = s.node_hi - s.node_lo;
-    const uint32_t k0 = dense ? p * a.n_node + s.node_lo : __ldg(&a.cand_off[p]);
-    const uint32_t k1 = dense ? k0 + n_win : __ldg(&a.cand_off[p + 1]);
-    PreScan r = pre_scan(a, k0, k1, lane, dense ? nullptr : a.cand_nodes, s.node_lo, n_win);
+    uint32_t k0, k1;
+    pod_pairs(a.cand_off, p, a.n_node, s.node_lo, s.n_win, k0, k1);
+    PreScan r = pre_scan(a, k0, k1, lane, a.cand_off ? a.cand_nodes : nullptr, s.node_lo, s.n_win);
     if (lane != 0) return;
     if (r.fit != DRA_GPU_NONE) r.best = DRA_GPU_NONE;                    // a FITS pair anywhere beats every EVICT pair
     uint4* q = s.part + 1 + (size_t)p * s.stride;
@@ -4341,7 +4349,6 @@ k_spre_merge(const PeerExchange x, const PreMerge m) {
     if (!merge_start(x, m.gate, m.slice4, world, rank, tid)) return;
     const uint32_t lane = tid & 31;
     const uint32_t warp = (blockIdx.x * blockDim.x + tid) >> 5, n_warp = (gridDim.x * blockDim.x) >> 5;
-    const bool dense = m.cand_off == nullptr;
     for (uint32_t p = warp; p < m.n_pod; p += n_warp) {
         const uint4* src = nullptr;
         uint4 A = make_uint4(DRA_GPU_NONE, DRA_GPU_NONE, 0u, 0u), B = make_uint4(0u, 0u, 0u, 0u);
@@ -4360,7 +4367,7 @@ k_spre_merge(const PeerExchange x, const PreMerge m) {
         uint32_t k;
         const uint32_t st = pre_decide(fit, best, lim, inv, k);
         const uint32_t nv = st == DRA_PRE_EVICT ? bs.y : 0u;
-        const uint32_t node = k == DRA_GPU_NONE ? DRA_GPU_NONE : dense ? k - p * m.n_node : __ldg(&m.cand_nodes[k]);
+        const uint32_t node = k == DRA_GPU_NONE ? DRA_GPU_NONE : pair_node(m.cand_off, m.cand_nodes, k, p, m.n_node);
         if (lane == 0) {
             m.pod_status[p] = (uint8_t)st;
             m.pod_node[p] = node;
@@ -4380,7 +4387,7 @@ k_spre_merge(const PeerExchange x, const PreMerge m) {
     if (!m.pair_status && !m.pair_victims && !m.pair_viol) return;
     const size_t pair4 = 1 + (size_t)m.n_pod * m.stride;                 // a slice's pair results follow its partials
     for (uint32_t k = blockIdx.x * blockDim.x + tid; k < m.n_pair; k += gridDim.x * blockDim.x) {
-        const uint32_t node = dense ? k % m.n_node : __ldg(&m.cand_nodes[k]);
+        const uint32_t node = m.cand_off ? __ldg(&m.cand_nodes[k]) : k % m.n_node;
         uint2 v = make_uint2(DRA_PRE_NO, 0u);                             // a candidate naming no node
         if (node < m.n_node) {
             const uint32_t r = node_owner(m.bounds, world, node);
@@ -4406,9 +4413,7 @@ struct CapArgs {
     uint32_t n_pair;
     const uint4* inv; const uint32_t* node_off; uint32_t n_node; const uint32_t* tbl; SelCtx sel;
     uint32_t exhaustive, max_copies;
-    // the node window: the pairs of the nodes in [node_lo, node_lo + n_win), or of no node.  n_walk: the pairs walked,
-    // dense n_pod * n_win, else n_pair.  The single-inventory call: [0, n_node), n_walk = n_pair.
-    uint32_t node_lo, n_win, n_walk;
+    uint32_t node_lo, n_win, n_walk;   // the node window and the pairs walked, as in UnsArgs (one inventory: [0, n_node))
     uint16_t* pair_copies; uint8_t* pair_stop;            // at the walk index; pair_stop: nullptr unless asked for
     unsigned long long* pod_total; uint32_t* pod_nodes;   // each nullptr unless asked for
     unsigned long long* work;                             // next unclaimed pair (zeroed by the host)
@@ -4418,31 +4423,27 @@ struct CapArgs {
 // k_pods_preempt's layout: W lanes per pair, 32/W pairs per warp, pairs taken from a counter, since a pair costs from one
 // evaluation to max_copies of them.  One writer per pair, so the results are plain stores and nothing is zeroed first.
 // A candidate naming no node, an empty pod and a pod of more than DRA_MAX_POD claims are answered without loading a node.
-// The results go to the walk index: dense walk w is pod w / n_win at node node_lo + w % n_win; in the candidate form the
-// walk index is the pair index, and a pair on a node outside the window is skipped.  With the window [0, n_node) the walk
-// index is the pair index in both forms.
+// The results go to the walk index (pair_decode's), which with the window [0, n_node) is the pair index in both forms.
 template <int WPC, int W>
 __global__ void __launch_bounds__(WPC * 32, 2)
 k_pods_capacity(const CapArgs a) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
     if (a.gate && __ldcg(a.gate)) return;
-    for (uint32_t i = threadIdx.x; i < DRA_MAX_MODELS * DRA_MAX_PROFILES; i += WPC * 32) tbl_s[i] = __ldg(&a.tbl[i]);
-    __syncthreads();
+    stage_table<WPC * 32>(tbl_s, a.tbl);
     constexpr uint32_t G = 32 / W;
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t grp = lane / W, gbase = grp * W, gl = lane - gbase;
-    const uint32_t gmask = W == 32 ? FULLMASK : (((1u << (W & 31)) - 1u) << gbase);
+    const auto [lane, grp, gl, gbase, gmask] = lane_group<W>();
     while (true) {
         const uint32_t pw = walk_fetch<G>(a.work, lane);
         if (pw >= a.n_walk) break;
-        const uint32_t pair = pw + grp;                                  // the walk index
-        if (pair >= a.n_walk) continue;                                  // whole group skips together
+        const uint32_t walk = pw + grp;                                  // (results go to the walk index)
+        if (walk >= a.n_walk) continue;                                  // whole group skips together
+        // pair_decode's rule written out: through it, 76 registers instead of 74 and 11% slower at two ranks per device
         uint32_t pod, node;
-        if (!a.cand_off) { pod = pair / a.n_win; node = a.node_lo + (pair - pod * a.n_win); }
+        if (!a.cand_off) { pod = walk / a.n_win; node = a.node_lo + (walk - pod * a.n_win); }
         else {
-            node = __ldg(&a.cand_nodes[pair]);
+            node = __ldg(&a.cand_nodes[walk]);
             if (node < a.n_node && node - a.node_lo >= a.n_win) continue;   // another rank's node
-            pod = __ldg(&a.pair_pod[pair]);
+            pod = __ldg(&a.pair_pod[walk]);
         }
         const uint32_t c0 = __ldg(&a.pod_off[pod]), cnt = __ldg(&a.pod_off[pod + 1]) - c0;
         uint32_t copies = 0, stop = DRA_ST_POD;                           // a candidate naming no node: unsuitable (§8)
@@ -4468,8 +4469,8 @@ k_pods_capacity(const CapArgs a) {
             }
         }
         if (lane == gbase) {
-            a.pair_copies[pair] = (uint16_t)copies;
-            if (a.pair_stop) a.pair_stop[pair] = (uint8_t)stop;
+            a.pair_copies[walk] = (uint16_t)copies;
+            if (a.pair_stop) a.pair_stop[walk] = (uint8_t)stop;
         }
     }
 }
@@ -4500,8 +4501,8 @@ __global__ void __launch_bounds__(256)
 k_pods_capacity_sum(const CapArgs a) {
     const uint32_t lane = threadIdx.x & 31, p = blockIdx.x * 8 + (threadIdx.x >> 5);
     if (p >= a.n_pod) return;
-    const unsigned long long k0 = a.cand_off ? __ldg(&a.cand_off[p]) : (unsigned long long)p * a.n_node;
-    const unsigned long long k1 = a.cand_off ? __ldg(&a.cand_off[p + 1]) : k0 + a.n_node;
+    unsigned long long k0, k1;
+    pod_pairs(a.cand_off, p, a.n_node, 0u, a.n_node, k0, k1);
     cap_pod_sums(p, lane, k0, k1, [&](unsigned long long k) { return (uint32_t)a.pair_copies[k]; }, a.pod_total, a.pod_nodes);
 }
 
@@ -4537,10 +4538,10 @@ k_scap_merge(const PeerExchange x, const CapMerge m) {
     const uint32_t warp = (blockIdx.x * blockDim.x + tid) >> 5, n_warp = (gridDim.x * blockDim.x) >> 5;
     const bool dense = m.cand_off == nullptr;
     for (uint32_t p = warp; p < m.n_pod; p += n_warp) {
-        const unsigned long long k0 = dense ? (unsigned long long)p * m.n_node : __ldg(&m.cand_off[p]);
-        const unsigned long long k1 = dense ? k0 + m.n_node : __ldg(&m.cand_off[p + 1]);
+        unsigned long long k0, k1;
+        pod_pairs(m.cand_off, p, m.n_node, 0u, m.n_node, k0, k1);
         cap_pod_sums(p, lane, k0, k1, [&](unsigned long long k) {
-            const uint32_t node = dense ? (uint32_t)(k - k0) : __ldg(&m.cand_nodes[k]);
+            const uint32_t node = pair_node(m.cand_off, m.cand_nodes, k, p, m.n_node);
             uint32_t copies = 0, stop = DRA_ST_POD;                        // a candidate naming no node
             if (node < m.n_node) {
                 const uint32_t r = node_owner(m.bounds, world, node);
