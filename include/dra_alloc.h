@@ -421,7 +421,10 @@ int  dra_pod_capacity_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
                             uint64_t* pod_total, uint32_t* pod_nodes, uint32_t flags);
 
 /* Deallocate(): stands in for controller.Driver.Deallocate(ctx, claim).  Inverse update from the
- * claims and the OutRecs dra_allocate_batch produced for them (same out_off convention). */
+ * claims and the OutRecs dra_allocate_batch produced for them (same out_off convention), or any other records: a MIG
+ * record frees ((1 << size) - 1) << start cut to 16 bits, nothing when start >= 16 (spec §9).  Every claim's slot range
+ * is checked before anything is enqueued: one that leaves [0, n_out), or n_out < n_claim without out_off, returns
+ * DRA_E_INVAL with nothing launched and the inventory unchanged. */
 int  dra_deallocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
                           const uint32_t* out_off, const dra_out_rec* out, uint32_t n_out);
 

@@ -485,6 +485,8 @@ class Context:
                 None if nodes is None else nodes[:n_pod])
 
     def deallocate(self, claims, out, out_off=None):
+        """Spec §9: release the OK records `out` of `claims` (slots counted as Allocate counts them).  A claim whose slot
+        range leaves [0, len(out)) raises DraError(DRA_E_INVAL) before anything is launched: the inventory is unchanged."""
         c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
         o = np.ascontiguousarray(out, dtype=R.OUT_DTYPE)
         oo = None if out_off is None else np.ascontiguousarray(out_off, dtype=np.uint32)

@@ -925,10 +925,10 @@ int check_cands(dra_ctx* ctx, uint32_t n_pod, const uint32_t* cand_nodes, const 
     return DRA_OK;
 }
 
-// The pod calls' slots: n_out >= n_claim without out_off, and each claim's OutRec slots within n_out.  A GPU claim of
-// count 1 .. DRA_MAX_COUNT (more than 1 only with out_off) has count slots, every other claim one.  any_node (spec §13):
-// counted as if the claim named a node of the inventory; otherwise (spec §12, as k_pod_records counts them) only a GPU
-// claim naming a node < n_node has count slots.
+// The slots of the pod calls and dra_deallocate_batch: n_out >= n_claim without out_off, and each claim's OutRec slots
+// within n_out.  A GPU claim of count 1 .. DRA_MAX_COUNT (more than 1 only with out_off) has count slots, every other
+// claim one.  any_node (spec §13): counted as if the claim named a node of the inventory; otherwise (spec §12, as
+// k_pod_records and k_dealloc count them) only a GPU claim naming a node < n_node has count slots.
 int check_slots(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* out_off, uint32_t n_out,
                 bool any_node) {
     if (!out_off) {                                       // one slot per claim: claim i owns slot i
@@ -2039,11 +2039,15 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     return read_back(ctx, "preempt-and-place kernels", 1, outs);
 }
 
+// Deallocate on one inventory (spec §9).  Every claim's slot range is checked here, with the slots k_dealloc counts, before
+// anything is staged: k_dealloc applies each claim in its own thread, so a bad range found only on the device would leave
+// the other claims' records applied.
 int dra_deallocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* out_off,
                          const dra_out_rec* out, uint32_t n_out) {
     if (!ctx || (n_claim && (!claims || !out))) return DRA_E_INVAL;
     QUIESCE();
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    if (int rc = check_slots(ctx, claims, n_claim, out_off, n_out, false)) return rc;
     if (!n_claim) return DRA_OK;
     CU(cudaSetDevice(ctx->device));
     int rc = ensure_batch(ctx, n_claim, n_out, true);

@@ -3155,6 +3155,12 @@ __device__ __forceinline__ uint32_t dealloc_slots(const uint4 c, uint32_t n_node
     return (kind == DRA_KIND_GPU && c.y < n_node && count >= 1 && count <= DRA_MAX_COUNT && (have_off || count == 1)) ? count : 1u;
 }
 
+// The slices an OutRec's u8 start and size name (spec §9): ((1 << size) - 1) << start cut to 16 bits, empty when start >= 16.
+// Written without a shift of 32 or more, so the answer does not rest on how the hardware treats such counts.
+__device__ __forceinline__ uint32_t slice_mask(const uint32_t start, const uint32_t size) {
+    return start >= 16u ? 0u : (((size >= 16u ? 0xFFFFu : (1u << size) - 1u) << start) & 0xFFFFu);
+}
+
 // The sharded Deallocate's all-or-nothing check (dra_deallocate_batch_global_device), grid-stride over every claim: a slot
 // range [base, base + slots) outside [0, n_out) sets ERR_BAD_DEALLOC, which gates k_dealloc.  Every rank reads the same
 // arrays, so every rank finds the same fault.
@@ -3173,7 +3179,8 @@ k_dealloc_check(const uint4* __restrict__ claims, uint32_t n_claim, const uint32
 
 // GPUs outside [gpu_lo, gpu_hi) are not written (dra_deallocate_batch: [0, n_gpu)).  gate: when set (the sharded call,
 // launched as a programmatic dependent of k_dealloc_check), a non-zero word means the check found a bad slot range and
-// nothing is applied; without it a bad range stops the thread with ERR_OUT_RANGE after others may have applied theirs.
+// nothing is applied.  dra_deallocate_batch checks every slot range on the host before it launches, so the ERR_OUT_RANGE
+// test below only guards a launch that skipped that check.
 __global__ void __launch_bounds__(256)
 k_dealloc(const uint4* __restrict__ claims, uint32_t n_claim, const uint32_t* __restrict__ out_off,
           const uint2* __restrict__ out, uint32_t n_out, uint32_t* __restrict__ inv, uint32_t gpu_lo, uint32_t gpu_hi,
@@ -3195,10 +3202,8 @@ k_dealloc(const uint4* __restrict__ claims, uint32_t n_claim, const uint32_t* __
         if ((o.y >> 24) != DRA_ST_OK || o.x < gpu_lo || o.x >= gpu_hi) continue;
         uint32_t* w = inv + (size_t)o.x * 4;
         if (kind == DRA_KIND_GPU) atomicAnd(&w[0], ~((uint32_t)DRA_GPU_FULL_ALLOCATED << 16));
-        else if (kind == DRA_KIND_MIG) {
-            const uint32_t st = o.y & 0xFFu, sz = (o.y >> 8) & 0xFFu;
-            atomicAnd(&w[0], ~(((((1u << sz) - 1u) << st)) & 0xFFFFu));
-        } else if (kind == DRA_KIND_SHARED) {
+        else if (kind == DRA_KIND_MIG) atomicAnd(&w[0], ~slice_mask(o.y & 0xFFu, (o.y >> 8) & 0xFFu));
+        else if (kind == DRA_KIND_SHARED) {
             atomicAdd(&w[1], c.z);
             uint32_t old = w[3], assumed;
             do { assumed = old; old = atomicCAS(&w[3], assumed, (assumed & 0xFFFF0000u) | ((assumed - 1u) & 0xFFFFu)); }
@@ -3674,8 +3679,7 @@ __device__ __forceinline__ void pre_apply(Lane& L, const PreArgs& a, const uint4
             if (kind == DRA_KIND_GPU) {
                 L.flags = add ? (L.flags | DRA_GPU_FULL_ALLOCATED) : (L.flags & ~(uint32_t)DRA_GPU_FULL_ALLOCATED);
             } else if (kind == DRA_KIND_MIG) {
-                const uint32_t start = o.y & 0xFFu, size = (o.y >> 8) & 0xFFu;
-                const uint32_t m = start >= 16u ? 0u : (((size >= 16u ? 0xFFFFu : (1u << size) - 1u) << start) & 0xFFFFu);
+                const uint32_t m = slice_mask(o.y & 0xFFu, (o.y >> 8) & 0xFFu);
                 L.busy = add ? (L.busy | m) : (L.busy & ~m);
             } else if (kind == DRA_KIND_SHARED) {
                 L.mem = add ? L.mem - c.z : L.mem + c.z;

@@ -735,26 +735,39 @@ int dra_oracle_unsuitable_ex(const dra_gpu_rec* gpus, uint32_t n_gpu, const uint
     return 0;
 }
 
-/* spec §9 */
+/* slots(c) of spec §1/§3, the same as Allocate used: an INVALID claim (here: naming no node) has one */
+static uint32_t dealloc_slots(const dra_claim_rec* c, uint32_t n_node, int have_off)
+{
+    return (c->kind == DRA_KIND_GPU && c->node < n_node && c->count >= 1 && c->count <= DRA_MAX_COUNT &&
+            (have_off || c->count == 1)) ? c->count : 1;
+}
+
+/* spec §9: the slices ((1 << size) - 1) << start cut to 16 bits, empty when start >= 16, for any u8 start and size */
+static uint16_t dealloc_mask(uint8_t start, uint8_t size)
+{
+    uint32_t m = size >= 16 ? 0xFFFFu : (1u << size) - 1u;
+    return start >= 16 ? 0 : (uint16_t)(m << start);
+}
+
+/* spec §9: every claim's slot range is checked before any record is applied, so a failed call changes nothing */
 int dra_oracle_deallocate(dra_gpu_rec* gpus, uint32_t n_gpu, uint32_t n_node,
                           const dra_claim_rec* claims, uint32_t n_claim,
                           const uint32_t* out_off, const dra_out_rec* out, uint32_t n_out)
 {
     int have_off = out_off != NULL;
     for (uint32_t i = 0; i < n_claim; i++) {
-        const dra_claim_rec* c = &claims[i];
-        uint32_t base = have_off ? out_off[i] : i;
-        /* slots(c) of spec §1/§3, the same as Allocate used: an INVALID claim (here: naming no node) has one */
-        uint32_t sl = (c->kind == DRA_KIND_GPU && c->node < n_node && c->count >= 1 && c->count <= DRA_MAX_COUNT &&
-                       (have_off || c->count == 1)) ? c->count : 1;
+        uint32_t base = have_off ? out_off[i] : i, sl = dealloc_slots(&claims[i], n_node, have_off);
         if (base > n_out || sl > n_out - base) return -1;
+    }
+    for (uint32_t i = 0; i < n_claim; i++) {
+        const dra_claim_rec* c = &claims[i];
+        uint32_t base = have_off ? out_off[i] : i, sl = dealloc_slots(c, n_node, have_off);
         for (uint32_t k = 0; k < sl; k++) {
             const dra_out_rec* o = &out[base + k];
             if (o->status != DRA_ST_OK || o->gpu >= n_gpu) continue;
             dra_gpu_rec* r = &gpus[o->gpu];
             if (c->kind == DRA_KIND_GPU) r->flags &= (uint8_t)~DRA_GPU_FULL_ALLOCATED;
-            else if (c->kind == DRA_KIND_MIG)
-                r->busy &= (uint16_t)~(((1u << o->size) - 1u) << o->start);
+            else if (c->kind == DRA_KIND_MIG) r->busy &= (uint16_t)~dealloc_mask(o->start, o->size);
             else if (c->kind == DRA_KIND_SHARED) { r->mem_free_mib += c->mem_limit_mib; r->share_cnt--; }
         }
     }

@@ -57,7 +57,7 @@ int dra_oracle_unsuitable_ex(const dra_gpu_rec* gpus, uint32_t n_gpu, const uint
                              const uint32_t* cand_nodes, const uint32_t* cand_off, uint8_t* suitable_bits,
                              uint32_t flags);
 
-/* Deallocate (spec §9). */
+/* Deallocate (spec §9).  -1, with gpus untouched, when a claim's slot range leaves [0, n_out). */
 int dra_oracle_deallocate(dra_gpu_rec* gpus, uint32_t n_gpu, uint32_t n_node,
                           const dra_claim_rec* claims, uint32_t n_claim,
                           const uint32_t* out_off, const dra_out_rec* out, uint32_t n_out);

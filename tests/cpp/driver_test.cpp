@@ -147,6 +147,36 @@ int main() {
         EXPECT(m1.Error.empty() && gg.Error.empty() && m2.Error.empty());
         EXPECT(m1.Allocation[0].GpuIndex == m2.Allocation[0].GpuIndex);
     }
+    // --- a shared claim of Count copies that fails part way gives back the copies it took -----------------------------
+    // Two 40 GiB GPUs and a 30 GiB MPS limit: each GPU holds one copy.  Count = 3 takes gpu-0 and gpu-1, the third copy
+    // finds no memory, and the claim fails as a whole.  Driver exposes no memory or share counts, so the rollback shows in
+    // what can be allocated next: two Count = 1 claims land on gpu-0 and gpu-1, as on a fresh node.
+    for (const bool exhaustive : {false, true}) {
+        d.SetExhaustive(exhaustive);
+        d.SetNodes({node("mps", 0, 2)});
+        auto three = gpu("mps-3", 3, SharingStrategy::MPS, 30ll << 30);
+        d.Allocate({&three}, "mps");
+        // exhaustive: the pod fails as a whole on the device and nothing is taken, so the rollback releases nothing
+        EXPECT_EQ_S(three.Error, exhaustive ? "the pod's claims do not fit on the selected node together"
+                                            : "no shareable GPU with enough free memory");
+        EXPECT(three.Allocation.empty() && three.AllocatedNode.empty());
+        d.Deallocate(three);                              // never held: a no-op
+        auto a = gpu("mps-a", 1, SharingStrategy::MPS, 30ll << 30), b = gpu("mps-b", 1, SharingStrategy::MPS, 30ll << 30),
+             c = gpu("mps-c", 1, SharingStrategy::MPS, 30ll << 30);
+        d.Allocate({&a}, "mps"); d.Allocate({&b}, "mps"); d.Allocate({&c}, "mps");
+        EXPECT(a.Error.empty() && b.Error.empty() && a.Allocation.size() == 1 && b.Allocation.size() == 1);
+        if (a.Allocation.size() == 1 && b.Allocation.size() == 1) {
+            EXPECT_EQ_S(a.Allocation[0].Device, "gpu-0");
+            EXPECT_EQ_S(b.Allocation[0].Device, "gpu-1");
+        }
+        EXPECT(!c.Error.empty() && c.Allocation.empty());  // and the node is full again, with no copy left over
+        // released and taken again: the copies a Deallocate gives back are the copies a later claim gets
+        d.Deallocate(b);
+        auto e = gpu("mps-e", 1, SharingStrategy::MPS, 30ll << 30);
+        d.Allocate({&e}, "mps");
+        EXPECT(e.Allocation.size() == 1 && e.Allocation[0].Device == "gpu-1");
+    }
+    d.SetExhaustive(false);
     if (failures) { printf("%d FAILED\n", failures); return 1; }
     printf("driver_test: all checks passed\n");
     return 0;
