@@ -763,7 +763,6 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_COMPACT_FLAT1     0x08000u  /* sharded call: compaction in 256-claim tiles */
 #define DRA_K_COMPACT_FLAT8     0x10000u  /* sharded call: compaction in 2048-claim tiles */
 #define DRA_K_COMPACT_LOOKBACK  0x20000u  /* sharded call: compaction with a decoupled look-back (beyond 2M claims) */
-#define DRA_K_COMPACT_IN_KERNEL 0x40000u  /* sharded call: compaction inside the single-launch kernel */
 #define DRA_K_POD_SHARD         0x80000u  /* sharded pods Allocate: pod records + ownership, gate, k_pods on the node window */
 #define DRA_K_POD_GATHER        0x100000u /* sharded pods Allocate: all-gather of the owned pods' records (world > 1) */
 #define DRA_K_PLACE             0x200000u /* place pods: pod states + pair records, persistent walk of the nodes' visit lists */

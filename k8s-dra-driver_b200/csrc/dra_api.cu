@@ -148,9 +148,6 @@ struct dra_ctx {
     bool ev_ok = false;
     float timings[5] = {0, 0, 0, 0, 0};
     uint32_t ev_mask = 0;
-    // dynamic shared-memory limits are raised ONCE per device to the opt-in maximum (raise_smem_limits): the attribute is
-    // per function, not per context — a lazily "grown" per-context value would LOWER it under another context's feet
-    int hist8_smem_set = 1 << 30, hist_smem_set = 1 << 30, small_smem_set = 1 << 30, fused_smem_set = 1 << 30, fused_smem_set_stage = 1 << 30;
     uint64_t fused_max_work = 3000000ull;   // n_node * n_claim up to which the single-launch kernel is used
     uint32_t fused_max_one_wave = 14000u, fused_max_multi = 7500u;   // claims up to which it beats the sort path (profiles/path_crossover.py,
                                                                      // fused_plan); dra_calibrate re-measures them on the device at hand
@@ -158,10 +155,9 @@ struct dra_ctx {
     DirectIO dio_pending{};                 // set by dra_allocate_batch for the next launch_allocate, then cleared
     uint32_t* d_gbar = nullptr;             // grid barrier words
     int n_sm = 0, coop_ok = 0;
-    int dio_cap_smem = -1, dio_cap_cta = 0; // co-resident CTA capacity of k_fused at dio_cap_smem bytes of shared memory
+    int fused_occ_stage = -1, fused_occ_smem = -1, fused_occ_cta = 0;   // fused_resident_ctas: the last query's answer
     unsigned long long* d_scan_status = nullptr; uint32_t cap_scan_status = 0;   // k_bucket_scan_rows: one word per CTA
     int pack4_occ = -1;              // resident CTAs of k_pack<4> per SM (occupancy query, once)
-    int tail_cap_smem = -1, tail_cap_stage = -1, tail_cap_cta = 0;   // the same for the gather tail
     const void* dio_seen[3] = {nullptr, nullptr, nullptr};   // host pointers already checked to be device-visible as-is
 
     ncclComm_t comm = nullptr;
@@ -329,11 +325,8 @@ Tiling tiling(uint32_t n_claim, uint32_t n_node, int n_sm) {
     // CTA-wide tiles (k_bucket_hist8) whenever 8 x (n_node+1) u16 counters fit in shared memory: 2048 claims, or — once
     // such tiles would outnumber the SMs — the multiple of 2048 that fills the SMs once (<= 32768: ranks are u16)
     if ((size_t)8 * ((size_t)n_node + 2) * 2 <= 200 * 1024) {
-        static const bool fixed = getenv("DRA_HIST_TILE_2048") != nullptr;           // experiment switch: the round-1 tiling
         uint32_t T = H8_TILE;
-        static const char* force = getenv("DRA_HIST_TILE");                          // experiment switch: a given multiple of 2048
-        if (force && n_claim > (uint32_t)n_sm * H8_TILE) T = std::min<uint32_t>(32768u, std::max<uint32_t>(H8_TILE, (uint32_t)atoi(force) / H8_TILE * H8_TILE));
-        else if (!fixed && n_claim > (uint32_t)n_sm * H8_TILE)
+        if (n_claim > (uint32_t)n_sm * H8_TILE)
             T = std::min<uint32_t>(32768u, ((n_claim + (uint32_t)n_sm - 1) / (uint32_t)n_sm + H8_TILE - 1) / H8_TILE * H8_TILE);
         uint32_t n_tiles = n_claim ? (n_claim + T - 1) / T : 1;
         return {T, n_tiles, true};
@@ -394,17 +387,24 @@ int upload_table(dra_ctx* ctx) {
     return DRA_OK;
 }
 
-// Kernel launch with (optionally) the programmatic-dependent-launch attribute: the kernel's CTAs may be scheduled
-// while its predecessor in the stream drains; it blocks in griddepcontrol.wait until that grid has completed.
+// Kernel launch with at most one launch attribute.  LA_PDL (programmatic dependent launch): the kernel's CTAs may be
+// scheduled while its predecessor in the stream drains; it blocks in griddepcontrol.wait until that grid has completed.
+// LA_COOP (cooperative launch): every CTA of the grid is resident at once, or the launch fails.
+enum LaunchAttr { LA_NONE, LA_PDL, LA_COOP };
 template <typename... KA, typename... A>
-static cudaError_t launch_k(void (*k)(KA...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, A&&... args) {
+static cudaError_t launch_k(void (*k)(KA...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, LaunchAttr la, A&&... args) {
     cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
     lc.gridDim = grid; lc.blockDim = block; lc.dynamicSmemBytes = smem; lc.stream = st;
     cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
-    lc.attrs = at; lc.numAttrs = pdl ? 1u : 0u;
+    if (la == LA_PDL) { at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1; }
+    else { at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1; }
+    lc.attrs = at; lc.numAttrs = la == LA_NONE ? 0u : 1u;
     return cudaLaunchKernelEx(&lc, k, static_cast<KA>(args)...);
 }
+
+// A kernel that follows another in the stream is its programmatic dependent (its launch latency and prologue overlap the
+// predecessor's tail), except while per-kernel events are being recorded
+LaunchAttr pdl_attr(const dra_ctx* ctx) { return ctx->profiling ? LA_NONE : LA_PDL; }
 
 struct Prof {          // event i brackets stage i: [hist, scan, scatter, pack/fused, all-gather]
     dra_ctx* c; int i = 0;
@@ -420,9 +420,8 @@ constexpr int FUSED_NW = 8;
 // stream for itself (n_node * n_claim key tests spread over n_node SMs, data from L2) and packs; no sort, no copy.
 struct FusedPlan { bool fused, stage; size_t smem; };
 FusedPlan fused_plan(const dra_ctx* ctx, uint32_t n_claim, uint32_t flags, uint32_t n_node) {
-    static const bool no_stage = getenv("DRA_NO_STAGE") != nullptr;          // experiment switch
     FusedPlan p;
-    p.stage = !no_stage && n_claim <= FUSED_NW * FU_PIECE * FU_MAXPIECE && fused_smem_bytes(n_claim, FUSED_NW, true) <= 225 * 1024;
+    p.stage = n_claim <= FUSED_NW * FU_PIECE * FU_MAXPIECE && fused_smem_bytes(n_claim, FUSED_NW, true) <= 225 * 1024;
     p.smem = fused_smem_bytes(n_claim, FUSED_NW, p.stage);
     // Measured crossover against the sort path (profiles/path_crossover.py, H100 SXM at 700 W): with 125 nodes (one wave
     // of CTAs) the single launch takes 15-19 us up to 12,000 claims against 21-23 us for the sort path; with 250 nodes
@@ -431,6 +430,19 @@ FusedPlan fused_plan(const dra_ctx* ctx, uint32_t n_claim, uint32_t flags, uint3
     p.fused = !(flags & DRA_F_NODE_SORTED) && !(ctx->cfg_flags & DRA_CFG_NO_FUSED) && n_claim <= fused_max_claims &&
               (uint64_t)n_node * n_claim <= ctx->fused_max_work && p.smem <= 225 * 1024 && n_node <= 16384;
     return p;
+}
+
+// CTAs of k_fused<FUSED_NW, stage> that can be resident at once with smem bytes of dynamic shared memory (the last
+// answer is cached)
+int fused_resident_ctas(dra_ctx* ctx, bool stage, size_t smem, int& ctas) {
+    if (ctx->fused_occ_stage != (int)stage || ctx->fused_occ_smem != (int)smem) {
+        int nb = 0;
+        if (stage) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, true>, FUSED_NW * 32, smem));
+        else CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, false>, FUSED_NW * 32, smem));
+        ctx->fused_occ_stage = (int)stage; ctx->fused_occ_smem = (int)smem; ctx->fused_occ_cta = nb * ctx->n_sm;
+    }
+    ctas = ctx->fused_occ_cta;
+    return DRA_OK;
 }
 
 // The counting sort's widest node range: its one-warp histogram (the form for ranges too wide for the CTA-wide one)
@@ -442,11 +454,10 @@ size_t sort_warp_hist_smem(uint32_t n_node) { return ((size_t)n_node + 1) * size
 // front half of the sort path.  Records naming no node get an INVALID OutRec (d_out != nullptr) or are dropped
 // (d_out == nullptr: pod records).  Enqueues only.
 int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uint32_t* d_out_off, uint2* d_out,
-                uint32_t n_out, uint32_t flags, Prof& prof, const void* inv_src, bool pdl,
+                uint32_t n_out, uint32_t flags, Prof& prof, const void* inv_src, LaunchAttr pdl,
                 uint32_t n_node, const uint32_t* d_node_off, const uint32_t* n_dev = nullptr) {
     Err err = err_of(ctx);
-    // sort path: the kernels after the first are programmatic dependents of their predecessor (launch latency and
-    // prologue overlap the predecessor's tail); not while per-kernel events are being recorded
+    // sort path: the kernels after the first are launched with pdl (pdl_attr, or LA_NONE)
     if (flags & DRA_F_NODE_SORTED) {
         if (n_dev) return fail(ctx, DRA_E_INVAL, "DRA_F_NODE_SORTED is not supported by the sharded call");
         uint32_t blocks = std::max(1u, (n_claim + 255) / 256);
@@ -459,10 +470,6 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
         const size_t small_smem = nbp * 4 + 32 * nbp * 2 + (size_t)n_claim * 2 + 16;
         if (n_claim <= 8192 && small_smem <= 200 * 1024) {
             // one launch: the whole stable counting sort in a single CTA
-            if (small_smem > 48 * 1024 && ctx->small_smem_set < (int)small_smem) {
-                CU(cudaFuncSetAttribute(k_bucket_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)small_smem));
-                ctx->small_smem_set = (int)small_smem;
-            }
             Prefetch pf;
             pf.p[0] = inv_src;
             pf.bytes[0] = std::min<uint32_t>(ctx->n_gpu * 16u, 1u << 20) & ~15u;
@@ -477,18 +484,12 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
             Tiling t = tiling(n_claim, n_node, ctx->n_sm);
             if (t.cta_wide) {
                 const size_t smem = (size_t)8 * (((size_t)n_node + 2) & ~(size_t)1) * 2;
-                if (smem > 48 * 1024 && ctx->hist8_smem_set < (int)smem) {
-                    CU(cudaFuncSetAttribute(k_bucket_hist8<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                    CU(cudaFuncSetAttribute(k_bucket_hist8<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                    ctx->hist8_smem_set = (int)smem;
-                }
                 if (t.T == H8_TILE) k_bucket_hist8<false><<<t.n_tiles, 256, smem, ctx->stream>>>(d_claims, n_claim, n_node, ctx->d_hist, ctx->d_rank, n_dev, t.T);
                 else k_bucket_hist8<true><<<t.n_tiles, 256, smem, ctx->stream>>>(d_claims, n_claim, n_node, ctx->d_hist, ctx->d_rank, n_dev, t.T);
                 ctx->chain |= t.T == H8_TILE ? DRA_K_HIST8 : DRA_K_HIST8_MULTI;
                 prof.mark();
                 // the scan: a warp per node with every load in flight at once (latency), or — big matrices — coalesced rows
-                static const bool no_rows = getenv("DRA_SCAN_BY_NODE") != nullptr;
-                if (!no_rows && (size_t)t.n_tiles * (n_node + 1) > (size_t)512 * 1024) {
+                if ((size_t)t.n_tiles * (n_node + 1) > (size_t)512 * 1024) {
                     const uint32_t n_cta = (n_node + 1 + 31) / 32;
                     if (ctx->cap_scan_status < n_cta) return fail(ctx, DRA_E_STATE, "scan status words not allocated (ensure_batch)");
                     CU(launch_k(k_bucket_scan_rows, dim3(n_cta), dim3(256), 0, ctx->stream, pdl, ctx->d_hist, t.n_tiles, n_node, ctx->d_claim_off, ctx->d_ticket + TK_SCAN_ROWS, ctx->d_scan_status, err));
@@ -502,10 +503,6 @@ int launch_sort(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const uin
                 if (n_dev) return fail(ctx, DRA_E_INVAL, "sharded call: node range too wide for the CTA-wide histogram");
                 size_t smem = sort_warp_hist_smem(n_node);
                 if (smem > SORT_SMEM_MAX) return fail(ctx, DRA_E_INVAL, "n_node=%u exceeds the bucketing limit", n_node);
-                if (smem > 48 * 1024 && ctx->hist_smem_set < (int)smem) {
-                    CU(cudaFuncSetAttribute(k_bucket_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                    ctx->hist_smem_set = (int)smem;
-                }
                 k_bucket_hist<<<t.n_tiles, 32, smem, ctx->stream>>>(d_claims, n_claim, n_node, t.T, ctx->d_hist, ctx->d_rank);
                 prof.mark();
                 CU(launch_k(k_bucket_scan, dim3(1), dim3(1024), 0, ctx->stream, pdl, ctx->d_hist, t.n_tiles, n_node, ctx->d_claim_off));
@@ -529,9 +526,8 @@ struct AllocView {
     uint32_t node_lo = 0, n_node = 0;
     const uint32_t* n_dev = nullptr;      // device-side claim count (the claim list was compacted on the device)
     int have_off = -1;                    // -1: from d_out_off; else the CALLER's out_off convention (spec §1/§3)
-    bool no_pdl_first = false;
-    const ShardArgs* sa = nullptr;        // the compaction that produces the claim list: launched by launch_allocate — as its
-    uint32_t sc_rows = 1; bool sc_flat = true;   // own kernel, or run inside k_fused when the shard takes the single-launch kernel
+    const ShardArgs* sa = nullptr;        // the compaction that produces the claim list, launched by launch_allocate
+    uint32_t sc_rows = 1; bool sc_flat = true;
 };
 
 int launch_compaction(dra_ctx* ctx, const ShardArgs& sa, uint32_t sc_rows, bool sc_flat) {
@@ -556,6 +552,7 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
     const uint32_t* n_dev = view ? view->n_dev : nullptr;
     Err err = err_of(ctx);
     Prof prof(ctx);
+    if (view && view->sa && (rc = launch_compaction(ctx, *view->sa, view->sc_rows, view->sc_flat))) return rc;
 
     PackArgs a;
     memset(&a, 0, sizeof a);
@@ -578,38 +575,15 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
     if (fused) {
         // the gather tail has every CTA wait for its peers' packets: all CTAs of the grid must be resident at once.
         // Shared memory left over goes to the send queue (records leave for the peers while the pack still runs).
-        bool tail_ok = tail != nullptr;
-        const bool want_in = view && view->sa;             // a compaction comes with this launch
         size_t launch_smem = fused_smem;
-        uint32_t q_cap = 0;
-        if (tail_ok || want_in) {
-            static const bool no_q = getenv("DRA_NO_SENDQ") != nullptr;
+        if (tail) {
             const size_t room = fused_smem + 32 <= 225 * 1024 ? (225 * 1024 - fused_smem - 32) / 16 : 0;
-            q_cap = no_q ? 0u : (uint32_t)std::min<size_t>(room, 2048);
-            launch_smem = fused_smem + 32 + (size_t)q_cap * 16;
-            if (ctx->tail_cap_smem != (int)launch_smem || ctx->tail_cap_stage != (int)stage) {
-                int nb = 0;
-                if (stage) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, true>, FUSED_NW * 32, launch_smem));
-                else CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, false>, FUSED_NW * 32, launch_smem));
-                ctx->tail_cap_smem = (int)launch_smem; ctx->tail_cap_stage = (int)stage; ctx->tail_cap_cta = nb * ctx->n_sm;
-            }
-            const bool resident = (int)(n_node + 1) <= ctx->tail_cap_cta;
-            tail_ok = tail_ok && resident;
-            // the compaction inside the kernel: one 1024-claim tile per CTA, then a grid barrier (needs every CTA resident).
-            // An experiment, off by default (DRA_SHARD_IN_KERNEL=1 turns it on): it saves the second launch but pays a
-            // cooperative launch and a grid barrier, and loses the overlap of this kernel's prologue with the compaction
-            const bool want_inside = getenv("DRA_SHARD_IN_KERNEL") != nullptr;
-            if (want_in && resident && stage && want_inside && ctx->coop_ok && !ctx->profiling && view->sc_flat &&
-                (view->sa->n_claim + 256u * SC_IN_ROWS - 1) / (256u * SC_IN_ROWS) <= n_node + 1) {
-                a.sh = *view->sa; a.sh_on = 1;
-                a.sh.n_tiles = std::max(1u, (view->sa->n_claim + 256u * SC_IN_ROWS - 1) / (256u * SC_IN_ROWS));
-                if (!ctx->d_gbar) { CU(cudaMalloc((void**)&ctx->d_gbar, 64)); CU(cudaMemsetAsync(ctx->d_gbar, 0, 64, ctx->stream)); }
-                a.dio.gbar = ctx->d_gbar;
-            }
+            const uint32_t q_cap = (uint32_t)std::min<size_t>(room, 2048);
+            const size_t tail_smem = fused_smem + 32 + (size_t)q_cap * 16;
+            int ctas = 0;
+            if ((rc = fused_resident_ctas(ctx, stage, tail_smem, ctas))) return rc;
+            if ((int)(n_node + 1) <= ctas) { a.peer = *tail; a.q_cap = q_cap; launch_smem = tail_smem; if (tail_done) *tail_done = true; }
         }
-        if (want_in && !a.sh_on && (rc = launch_compaction(ctx, *view->sa, view->sc_rows, view->sc_flat))) return rc;
-        if (tail_ok) { a.peer = *tail; a.q_cap = q_cap; if (tail_done) *tail_done = true; }
-        else if (!a.sh_on) launch_smem = fused_smem;
         a.claims = d_claims; a.out_off = d_out_off; a.n_claim = n_claim;
         if (getenv("DRA_TIMELINE")) {           // instrumentation only: per-CTA clock stamps of the last fused launch
             if (ctx->tl_cap < (size_t)(2 * n_node + 24) * 8) {
@@ -622,43 +596,25 @@ int launch_allocate(dra_ctx* ctx, const uint4* d_claims, uint32_t n_claim, const
         }
         prof.skip_to(3);
         // grid = one CTA per node + one CTA for the claims that name no node
+        const dim3 grid(n_node + 1), block(FUSED_NW * 32);
         if (stage && dio.h_claims) {
             // direct host I/O: two grid barriers inside, so every CTA must be resident — cooperative launch
             a.dio = dio;
-            cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
-            lc.gridDim = dim3(n_node + 1); lc.blockDim = dim3(FUSED_NW * 32); lc.dynamicSmemBytes = fused_smem; lc.stream = ctx->stream;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
-            lc.attrs = at; lc.numAttrs = 1;
-            CU(cudaLaunchKernelEx(&lc, k_fused<FUSED_NW, true>, a));
-        }
-        else {
-            static const bool no_pdl_fused = getenv("DRA_NO_PDL") != nullptr;
-            const bool dep = n_dev != nullptr && !ctx->profiling && !no_pdl_fused && !a.sh_on;      // programmatic dependent of the compaction
-            if (a.sh_on) {                                  // compaction inside: a grid barrier, so a cooperative launch
-                cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
-                lc.gridDim = dim3(n_node + 1); lc.blockDim = dim3(FUSED_NW * 32); lc.dynamicSmemBytes = launch_smem; lc.stream = ctx->stream;
-                cudaLaunchAttribute at[1];
-                at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
-                lc.attrs = at; lc.numAttrs = 1;
-                if (stage) CU(cudaLaunchKernelEx(&lc, k_fused<FUSED_NW, true>, a));
-                else CU(cudaLaunchKernelEx(&lc, k_fused<FUSED_NW, false>, a));
-            }
-            else if (stage) CU(launch_k(k_fused<FUSED_NW, true>, dim3(n_node + 1), dim3(FUSED_NW * 32), launch_smem, ctx->stream, dep, a));
-            else CU(launch_k(k_fused<FUSED_NW, false>, dim3(n_node + 1), dim3(FUSED_NW * 32), launch_smem, ctx->stream, dep, a));
+            CU(launch_k(k_fused<FUSED_NW, true>, grid, block, fused_smem, ctx->stream, LA_COOP, a));
+        } else {
+            const LaunchAttr dep = n_dev ? pdl_attr(ctx) : LA_NONE;      // programmatic dependent of the compaction
+            if (stage) CU(launch_k(k_fused<FUSED_NW, true>, grid, block, launch_smem, ctx->stream, dep, a));
+            else CU(launch_k(k_fused<FUSED_NW, false>, grid, block, launch_smem, ctx->stream, dep, a));
         }
         ctx->launches += 1;
         ctx->chain |= (stage && dio.h_claims) ? DRA_K_FUSED_DIRECT : stage ? DRA_K_FUSED_STAGED : DRA_K_FUSED_STREAM;
-        if (a.sh_on) ctx->chain |= DRA_K_COMPACT_IN_KERNEL;
         prof.mark();
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "kernel launch: %s", cudaGetErrorString(e));
         return DRA_OK;
     }
 
-    if (view && view->sa && (rc = launch_compaction(ctx, *view->sa, view->sc_rows, view->sc_flat))) return rc;
-    static const bool no_pdl = getenv("DRA_NO_PDL") != nullptr;
-    const bool pdl = !no_pdl && !ctx->profiling;
+    const LaunchAttr pdl = pdl_attr(ctx);
     if ((rc = launch_sort(ctx, d_claims, n_claim, d_out_off, d_out, n_out, flags, prof, a.inv_src, pdl, n_node, d_node_off, n_dev))) return rc;
 
     a.sorted = ctx->d_sorted;
@@ -965,12 +921,7 @@ int launch_walk(dra_ctx* ctx, int& occ, const char* name, void (*k)(KA...), A&&.
     }
     if (occ < 1) return fail(ctx, DRA_E_CUDA, "%s: no CTA can be resident", name);
     const uint32_t grid = std::max(1u, std::min((ctx->n_node + 3) / 4, (uint32_t)(occ * ctx->n_sm)));
-    cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
-    lc.gridDim = dim3(grid); lc.blockDim = dim3(128); lc.dynamicSmemBytes = 0; lc.stream = ctx->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
-    lc.attrs = at; lc.numAttrs = 1;
-    CU(cudaLaunchKernelEx(&lc, k, static_cast<KA>(args)...));
+    CU(launch_k(k, dim3(grid), dim3(128), 0, ctx->stream, LA_COOP, std::forward<A>(args)...));
     ctx->launches += 1;
     return DRA_OK;
 }
@@ -1032,7 +983,7 @@ int launch_running_lists(dra_ctx* ctx, PreArgs& a, Prof& prof, bool walk) {
     k_pre_running<<<std::max(1u, (a.rn_pod + 255) / 256), 256, 0, st>>>(a);
     ctx->launches += 1;
     if (!a.rn_pod) CU(cudaMemsetAsync(walk ? ctx->d_pp_runoff : ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, st));
-    else if (int rc = launch_sort(ctx, a.rrec, a.rn_pod, nullptr, nullptr, 0, 0, prof, a.inv, false, ctx->n_node, ctx->d_node_off))
+    else if (int rc = launch_sort(ctx, a.rrec, a.rn_pod, nullptr, nullptr, 0, 0, prof, a.inv, LA_NONE, ctx->n_node, ctx->d_node_off))
         return rc;
     if (ctx->n_node && (a.rn_pod || !walk)) {
         k_pre_vsort<<<std::min(ctx->n_node, (uint32_t)ctx->n_sm * 8u), 256, 0, st>>>(a);
@@ -1157,6 +1108,8 @@ struct CallScope {
 }  // namespace
 
 namespace {
+// Dynamic shared-memory limits are raised ONCE per device to the opt-in maximum, when a context is created: the attribute
+// is per function, not per context — a lazily "grown" per-context value would LOWER it under another context's feet
 template <class K>
 int raise_one(dra_ctx* ctx, K k, int optin) {
     cudaFuncAttributes fa;
@@ -1241,12 +1194,7 @@ int serve_start(dra_ctx* ctx) {
     sa.idle_cycles = std::max(1ll, idle_ms) * 1900000ll;
     ctx->h_stat[1] = 0; ctx->h_stat[2] = 0;
     CU(cudaMemsetAsync(ctx->d_go, 0, 256, ctx->serve_stream));
-    cudaLaunchConfig_t lc; memset(&lc, 0, sizeof lc);
-    lc.gridDim = dim3(ctx->n_node + 1); lc.blockDim = dim3(FUSED_NW * 32); lc.dynamicSmemBytes = ctx->serve_smem; lc.stream = ctx->serve_stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;
-    lc.attrs = at; lc.numAttrs = 1;
-    CU(cudaLaunchKernelEx(&lc, k_serve<FUSED_NW>, sa));
+    CU(launch_k(k_serve<FUSED_NW>, dim3(ctx->n_node + 1), dim3(FUSED_NW * 32), ctx->serve_smem, ctx->serve_stream, LA_COOP, sa));
     ctx->launches += 1;
     ctx->serve_on = true; ctx->serve_epoch = ctx->state_epoch;
     return DRA_OK;
@@ -1280,6 +1228,21 @@ int serve_call(dra_ctx* ctx, const void* src_c, uint32_t n_claim, const void* sr
         ctx->serve_on = false;
     }
     return fail(ctx, DRA_E_CUDA, "resident kernel keeps leaving before it takes the batch");
+}
+
+// Whether a kernel can read the caller's claims (src_c) and offsets (src_o, or NULL) and write its OutRecs (dst_o) in these
+// host buffers as they are: 16-byte aligned records, 4-byte aligned offsets, and pointers the device can use unchanged
+// (UVA identity mapping; checked once each)
+bool host_io_ok(dra_ctx* ctx, const void* src_c, const void* src_o, void* dst_o) {
+    if (((uintptr_t)src_c & 15) || ((uintptr_t)dst_o & 15) || ((uintptr_t)src_o & 3)) return false;
+    const void* hp[3] = {src_c, src_o, dst_o};
+    for (int k = 0; k < 3; ++k) {
+        if (!hp[k] || ctx->dio_seen[k] == hp[k]) continue;
+        void* dp = nullptr;
+        if (cudaHostGetDevicePointer(&dp, const_cast<void*>(hp[k]), 0) != cudaSuccess || dp != hp[k]) { (void)cudaGetLastError(); return false; }
+        ctx->dio_seen[k] = hp[k];
+    }
+    return true;
 }
 
 #define QUIESCE() do { int q_ = serve_stop(ctx); if (q_) return q_; } while (0)
@@ -1531,20 +1494,10 @@ int dra_allocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
     // completion word.  Same eligibility as direct host I/O below; anything else stops the resident kernel first.
     {
         bool ok = (ctx->cfg_flags & DRA_CFG_RESIDENT) && ctx->coop_ok && n_claim && rb && !ctx->profiling && !getenv("DRA_TIMELINE") &&
-                  !(flags & ~DRA_F_FRESH_INVENTORY) && (int)(ctx->n_node + 1) <= ctx->n_sm && ctx->d_inv_live &&
-                  ((uintptr_t)src_c & 15) == 0 && ((uintptr_t)dst_o & 15) == 0 && (!src_o || ((uintptr_t)src_o & 3) == 0);
+                  !(flags & ~DRA_F_FRESH_INVENTORY) && (int)(ctx->n_node + 1) <= ctx->n_sm && ctx->d_inv_live;
         if (ok) {
             if (!ctx->serve_cap) ctx->serve_cap = serve_capacity();
-            ok = n_claim <= ctx->serve_cap && n_out <= 2 * ctx->serve_cap;
-        }
-        if (ok) {
-            const void* hp[3] = {src_c, src_o, dst_o};
-            for (int k = 0; k < 3 && ok; ++k) {
-                if (!hp[k] || ctx->dio_seen[k] == hp[k]) continue;
-                void* dp = nullptr;
-                if (cudaHostGetDevicePointer(&dp, const_cast<void*>(hp[k]), 0) != cudaSuccess || dp != hp[k]) { (void)cudaGetLastError(); ok = false; }
-                else ctx->dio_seen[k] = hp[k];
-            }
+            ok = n_claim <= ctx->serve_cap && n_out <= 2 * ctx->serve_cap && host_io_ok(ctx, src_c, src_o, dst_o);
         }
         if (ok) {
             rc = serve_call(ctx, src_c, n_claim, src_o, dst_o, n_out, flags);
@@ -1559,32 +1512,11 @@ int dra_allocate_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_cla
     // and all its CTAs can be resident at once, the kernel itself reads the claims from the (pinned, device-mapped)
     // host buffer and writes the OutRecs back there — no copy-engine transfers, no graph, one cooperative launch.
     {
-        static const bool no_direct = getenv("DRA_NO_DIRECT") != nullptr;
         const FusedPlan plan = fused_plan(ctx, n_claim, flags, ctx->n_node);
-        bool ok = !no_direct && !(ctx->cfg_flags & DRA_CFG_NO_DIRECT) && ctx->coop_ok && plan.fused && plan.stage && n_claim && rb &&
-                  !ctx->profiling && ((uintptr_t)src_c & 15) == 0 && ((uintptr_t)dst_o & 15) == 0 &&
-                  (!src_o || ((uintptr_t)src_o & 3) == 0);
-        if (ok && ctx->dio_cap_smem != (int)plan.smem) {
-            // co-resident capacity at this shared-memory size (the attribute must be raised before the query)
-            if (plan.smem > 48 * 1024 && ctx->fused_smem_set_stage < (int)plan.smem) {
-                CU(cudaFuncSetAttribute(k_fused<FUSED_NW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
-                ctx->fused_smem_set_stage = (int)plan.smem;
-            }
-            int nb = 0;
-            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_fused<FUSED_NW, true>, FUSED_NW * 32, plan.smem));
-            ctx->dio_cap_smem = (int)plan.smem; ctx->dio_cap_cta = nb * ctx->n_sm;
-        }
-        ok = ok && (int)(ctx->n_node + 1) <= ctx->dio_cap_cta;
-        if (ok) {
-            // the host pointers must be usable by the device as they are (UVA identity mapping); checked once each
-            const void* hp[3] = {src_c, src_o, dst_o};
-            for (int k = 0; k < 3 && ok; ++k) {
-                if (!hp[k] || ctx->dio_seen[k] == hp[k]) continue;
-                void* dp = nullptr;
-                if (cudaHostGetDevicePointer(&dp, const_cast<void*>(hp[k]), 0) != cudaSuccess || dp != hp[k]) { (void)cudaGetLastError(); ok = false; }
-                else ctx->dio_seen[k] = hp[k];
-            }
-        }
+        bool ok = !(ctx->cfg_flags & DRA_CFG_NO_DIRECT) && ctx->coop_ok && plan.fused && plan.stage && n_claim && rb && !ctx->profiling;
+        int ctas = 0;
+        if (ok && (rc = fused_resident_ctas(ctx, true, plan.smem, ctas))) return rc;
+        ok = ok && (int)(ctx->n_node + 1) <= ctas && host_io_ok(ctx, src_c, src_o, dst_o);
         if (ok && !ctx->d_gbar) { CU(cudaMalloc((void**)&ctx->d_gbar, 64)); CU(cudaMemsetAsync(ctx->d_gbar, 0, 64, ctx->stream)); }
         if (ok) {
             DirectIO d;
@@ -1734,10 +1666,8 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     const uint32_t* d_oo = out_off ? ctx->d_out_off : nullptr;
     k_pod_records<<<(n_pod + 255) / 256, 256, 0, ctx->stream>>>(ctx->d_claims, ctx->d_pod_off, n_pod, ctx->n_node, d_oo, d_out, n_out, ctx->d_podrec, err);
     ctx->launches += 1;
-    static const bool no_pdl = getenv("DRA_NO_PDL") != nullptr;
-    const bool pdl = !no_pdl && !ctx->profiling;
     const uint4* inv_src = (flags & DRA_F_FRESH_INVENTORY) ? ctx->d_inv_pristine : ctx->d_inv_live;
-    if ((rc = launch_sort(ctx, ctx->d_podrec, n_pod, nullptr, nullptr, 0, 0, prof, inv_src, false, ctx->n_node, ctx->d_node_off))) return rc;
+    if ((rc = launch_sort(ctx, ctx->d_podrec, n_pod, nullptr, nullptr, 0, 0, prof, inv_src, LA_NONE, ctx->n_node, ctx->d_node_off))) return rc;
     PodArgs a; memset(&a, 0, sizeof a);
     a.claims = ctx->d_claims; a.out_off = d_oo; a.out = d_out;
     a.sorted = ctx->d_sorted; a.claim_off = ctx->d_claim_off;
@@ -1745,7 +1675,7 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     a.n_node = ctx->n_node; a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.sel = sel_of(ctx); a.err = err;
     if (ctx->n_node) {
         const uint32_t grid = std::max(1u, std::min((ctx->n_node + 3) / 4, (uint32_t)ctx->n_sm * 8u));
-        CU(launch_k(k_pods<4>, dim3(grid), dim3(128), 0, ctx->stream, pdl, a));
+        CU(launch_k(k_pods<4>, dim3(grid), dim3(128), 0, ctx->stream, pdl_attr(ctx), a));
         ctx->launches += 1;
     }
     prof.mark();                                          // the walk: the pack stage of the timings
@@ -1807,7 +1737,7 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     k_pods_place_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, ctx->stream>>>(a);
     ctx->launches += 1;
     if (!dense && n_pair &&
-        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, a.inv_src, false, ctx->n_node, ctx->d_node_off)))
+        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, a.inv_src, LA_NONE, ctx->n_node, ctx->d_node_off)))
         return rc;
     if ((rc = launch_walk(ctx, ctx->place_occ, "k_pods_place", k_pods_place<4>, a, PlaceShard{}))) return rc;
     ctx->chain |= DRA_K_PLACE;
@@ -2031,7 +1961,7 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     k_pp_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, pl, pp);
     ctx->launches += 1;
     if (!dense && n_pair &&
-        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, ctx->n_node, ctx->d_node_off)))
+        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, LA_NONE, ctx->n_node, ctx->d_node_off)))
         return rc;
     if ((rc = launch_walk(ctx, ctx->pp_occ, "k_pods_preempt_place", k_pods_preempt_place<4>, a, pl, pp))) return rc;
     ctx->chain |= DRA_K_PREEMPT_PLACE;
@@ -2629,7 +2559,7 @@ int dra_allocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims
         CU(cudaMemcpyAsync(ctx->d_sc_times, init, 16, cudaMemcpyHostToDevice, ctx->stream));
         sa.timeline = ctx->d_sc_times;
     }
-    // (launched by launch_allocate: as its own kernel, or inside k_fused)
+    // (launched by launch_allocate, right before the kernel that reads the list)
     // 2. the usual chain on the shard's view of the inventory, results at the claims' GLOBAL slots
     AllocView view; view.node_lo = ctx->shard_lo; view.n_node = n_local_node; view.n_dev = ctx->d_sc_counts; view.have_off = d_out_off != nullptr;
     view.sa = &sa; view.sc_rows = sc_rows; view.sc_flat = sc_flat;
@@ -2751,7 +2681,7 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
                                                     ctx->d_inv_live, ctx->d_node_off);
     ctx->launches += 2; ctx->chain |= DRA_K_POD_SHARD;
     const uint32_t* d_node_off = ctx->d_node_off + ctx->shard_lo;
-    if ((rc = launch_sort(ctx, ctx->d_podrec, n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, n_win, d_node_off,
+    if ((rc = launch_sort(ctx, ctx->d_podrec, n_pod, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, LA_NONE, n_win, d_node_off,
                           ctx->d_spod + SP_NDEV))) return rc;
     if (n_win) {
         PodArgs a; memset(&a, 0, sizeof a);
@@ -2759,9 +2689,8 @@ int dra_allocate_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
         a.sorted = ctx->d_sorted; a.claim_off = ctx->d_claim_off;
         a.inv_src = ctx->d_inv_live; a.inv_dst = ctx->d_inv_live; a.node_off = d_node_off; a.tbl = ctx->d_tbl;
         a.n_node = n_win; a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.sel = sel_of(ctx); a.err = err;
-        static const bool no_pdl = getenv("DRA_NO_PDL") != nullptr;
         const uint32_t grid = std::max(1u, std::min((n_win + 3) / 4, (uint32_t)ctx->n_sm * 8u));
-        CU(launch_k(k_pods<4>, dim3(grid), dim3(128), 0, ctx->stream, !no_pdl && !ctx->profiling, a));
+        CU(launch_k(k_pods<4>, dim3(grid), dim3(128), 0, ctx->stream, pdl_attr(ctx), a));
         ctx->launches += 1;
     }
     prof.mark();
@@ -2874,7 +2803,7 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
                                                     ctx->d_inv_live, ctx->d_node_off);
     ctx->launches += 2;
     if (!dense && n_pair && n_win &&
-        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, false, n_win, d_node_off,
+        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, LA_NONE, n_win, d_node_off,
                           ctx->d_spod + SP_NDEV)))
         return rc;
     // The gate has read the bounds: k_splace_final counts the slots each rank really finalises in the same words.  (Zeroed
@@ -3207,7 +3136,7 @@ int dra_preempt_place_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     k_spp_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, pl, pp, s);
     ctx->launches += 1;
     if (!dense && n_pair &&
-        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_spp_inv, false, ctx->n_node, ctx->d_node_off)))
+        (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_spp_inv, LA_NONE, ctx->n_node, ctx->d_node_off)))
         return rc;
     if (ctx->n_node) {                 // every CTA resident (shard_walk_grid); the walk itself waits for no peer
         PreArgs aw = a;
@@ -3264,8 +3193,7 @@ int dra_deallocate_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     const uint32_t gpu_lo = ctx->h_node_off[ctx->shard_lo], gpu_hi = ctx->h_node_off[ctx->shard_hi];
     k_dealloc_check<<<std::max(1u, std::min((n_claim + 255) / 256, (uint32_t)ctx->n_sm * 4u)), 256, 0, ctx->stream>>>(
         (const uint4*)d_claims, n_claim, d_out_off, n_out, ctx->n_node, err);
-    static const bool no_pdl = getenv("DRA_NO_PDL") != nullptr;
-    CU(launch_k(k_dealloc, dim3((n_claim + 255) / 256), dim3(256), 0, ctx->stream, !no_pdl && !ctx->profiling,
+    CU(launch_k(k_dealloc, dim3((n_claim + 255) / 256), dim3(256), 0, ctx->stream, pdl_attr(ctx),
                 (const uint4*)d_claims, n_claim, d_out_off, (const uint2*)d_out, n_out, (uint32_t*)ctx->d_inv_live, gpu_lo, gpu_hi,
                 ctx->n_node, (const uint32_t*)(ctx->d_err + ERR_BAD_DEALLOC), err));
     ctx->launches += 2;

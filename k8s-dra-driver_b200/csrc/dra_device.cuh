@@ -975,7 +975,6 @@ k_sorted_prep(const uint4* __restrict__ claims, uint32_t n_claim, uint32_t n_nod
 // take_stray set (they come back INVALID, spec §3).  coff[j] = first GLOBAL OutRec slot of kept claim j.
 __device__ __forceinline__ unsigned long long globaltimer_ns();
 constexpr uint32_t SC_TILE = 2048;
-constexpr int SC_IN_ROWS = 4;             // in-kernel form: tiles of 1024 claims, one per CTA of k_fused
 struct ShardArgs {
     const uint4* claims; uint32_t n_claim; const uint32_t* out_off;
     uint32_t node_lo, node_hi, n_node_global, take_stray, have_off;
@@ -1108,8 +1107,7 @@ k_shard_compact(const ShardArgs a) {
 // claims, all CTAs resident), and no chain at all: a tile publishes its aggregate and then reads the aggregates of
 // ALL its predecessors at once (8 loads per lane in flight: 256 predecessors per L2 round trip), spinning only until the last of
 // them has published.
-// One tile (ROWS x 256 claims) by one CTA of 256 threads; used by the kernel below and, for shards that take the single-launch
-// kernel, INSIDE k_fused (one tile per CTA, then a grid barrier: no second launch at all).
+// One tile (ROWS x 256 claims) by one CTA of 256 threads, for the kernel below.
 template <int ROWS>
 __device__ __forceinline__ void shard_tile_flat(const ShardArgs& a, const uint32_t tile) {
     __shared__ uint32_t rowc[8 * ROWS], rows[8 * ROWS], pre_c, rs_s[PEER_MAX];
@@ -1463,7 +1461,6 @@ struct PackArgs {
     const uint4* claims;          // claims in input order                             (k_fused)
     const uint32_t* out_off;      // first out slot per claim or NULL                  (k_fused)
     uint32_t n_claim;             //                                                   (k_fused)
-    ShardArgs sh; uint32_t sh_on; // sharded call, shard small enough: the compaction runs INSIDE this kernel (one tile per CTA)  (k_fused)
     uint32_t q_cap;               // multi-GPU: entries of the shared-memory send queue behind the staged claims (0: none) (k_fused)
     const uint32_t* n_dev;        // if set: the real number of claims (<= n_claim, which then only sizes the layout) (k_fused)
     const uint4* inv_src;         // inventory read from here ...
@@ -2049,13 +2046,7 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
     const uint32_t ng = g1 - g0;
     if (threadIdx.x == 32 && ng) tma_load_a(sbase + FU_INV, b.inv_src + g0, ng * 16u, ibar);
     // sharded call: the claim list was compacted on the device by the kernel before this one; b.n_claim is its capacity
-    if (a.sh_on) {
-        // ... or right here: one 1024-claim tile per CTA (cooperative launch), a grid barrier, and the list is there —
-        // no second launch; the table and inventory copies above are already in flight behind it
-        if (blockIdx.x < a.sh.n_tiles) shard_tile_flat<SC_IN_ROWS>(a.sh, blockIdx.x);
-        grid_barrier(a.dio.gbar, gridDim.x, a.err);
-    }
-    else if (a.n_dev) pdl_wait();                            // (launched as a programmatic dependent of the compaction)
+    if (a.n_dev) pdl_wait();                                 // (launched as a programmatic dependent of the compaction)
     const uint32_t n_claim = a.n_dev ? min(b.n_claim, __ldcg(a.n_dev)) : b.n_claim;
     if (a.n_dev && __ldcg(a.n_dev) > b.n_claim) {            // laid out for fewer claims: touch nothing, tell everybody
         if (blockIdx.x == 0) {
@@ -2085,8 +2076,8 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
     // STAGE: each lane loads whole claims into registers, tests the key there and stores the claim into the stage, from
     // which the pack, the stray CTA and the tail read it after the filter's __syncthreads.  (Filling the stage with
     // 4 KiB bulk copies instead left the filter waiting for them to be issued and land: profiles/timeline.py.)
-    // L2-coherent loads only: the array may have been written inside this launch by other CTAs (direct-I/O ingest,
-    // in-kernel compaction) or, in k_serve, rewritten for this batch while the kernel stayed up.
+    // L2-coherent loads only: the array may have been written inside this launch by other CTAs (direct-I/O ingest) or,
+    // in k_serve, rewritten for this batch while the kernel stayed up.
     // The first 8 claims of every lane go out now, so warp 0's are in flight while it waits for the table and GpuRecs.
     constexpr int U = 8;
     const uint4 none = make_uint4(0u, 0xFFFFFFFFu, 0u, 0u);

@@ -17,7 +17,6 @@ def timeit(w, n_claim, do_flush, reps=50):
         if it>=5: ts.append(a.elapsed_time(b)*1e3)
     return np.median(ts)
 w = pkg.synth.cfg2()
-print("stage=%s" % ("off" if os.environ.get("DRA_NO_STAGE") else "on"))
 print("cfg2 full batch, flush:    %.2f us" % timeit(w, w.n_claim, True))
 print("cfg2 full batch, no flush: %.2f us" % timeit(w, w.n_claim, False))
 print("empty batch (0 claims, 126 CTAs), flush:    %.2f us" % timeit(w, 0, True))

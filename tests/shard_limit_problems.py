@@ -129,19 +129,16 @@ def place(n, n_total, tile):
     return pos
 
 
-IN_KERNEL_PAD = 2048                                   # two 1,024-claim tiles: within n_node + 1 CTAs for every problem
-
-
 def SORT_CHAIN_PAD(w):
     """The batch of the one-CTA counting sort's test: at most 8,192 claims, chunks of at most a quarter tile"""
     return 4 * w.n_claim + 600
 
 
-def padded(w, n_total, tile=None):
+def padded(w, n_total):
     """behind_empty_node(w) padded to n_total claims that the shard drops (_pad), its own
     claims placed by `place` at the compaction's tile (256 up to 262,144 claims, else 2,048).  `pos`: where they went."""
     v = behind_empty_node(w)
-    tile = tile or (SMALL_TILE if n_total <= 256 * 1024 else LARGE_TILE)
+    tile = SMALL_TILE if n_total <= 256 * 1024 else LARGE_TILE
     pos = place(v.n_claim, n_total, tile)
     c = _pad(n_total)
     c["node"] = np.where(np.arange(n_total) % 2, v.n_node - 1, 0)

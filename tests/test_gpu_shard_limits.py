@@ -249,15 +249,6 @@ def test_limit_problems_tiled_on_a_shard_pack4(pkg, oracle):
                 f"{w.name} over {v.hi - v.lo} nodes")
 
 
-def test_limit_problems_compacted_in_kernel(pkg, oracle, monkeypatch):
-    """DRA_SHARD_IN_KERNEL=1: the compaction inside the single-launch kernel (1,024-claim tiles, one per CTA)."""
-    monkeypatch.setenv("DRA_SHARD_IN_KERNEL", "1")
-    for w in SP.problems():
-        v = SP.padded(w, SP.IN_KERNEL_PAD, SP.SMALL_TILE)
-        _form_b(pkg, oracle, v, lambda ch: "fused_staged" in ch, {"compact_in_kernel", "fused_staged"},
-                f"{w.name}, compaction in the kernel")
-
-
 @pytest.mark.parametrize("form", ["stream", "flat8", "lookback"])
 def test_selectors_padded_on_a_shard(pkg, oracle, form):
     n_total, first, hinted = PADDED[form]

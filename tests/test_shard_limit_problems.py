@@ -117,17 +117,15 @@ def test_paddings_straddle_tile_boundaries(n_total):
 
 
 def test_every_padding_keeps_the_problem_in_order():
-    """The paddings of the chain tests (the one-CTA sort, the compaction inside the kernel) and of the selector problems."""
-    cases = [(w, SP.SORT_CHAIN_PAD(w)) for w in SP.problems()] + [(w, SP.IN_KERNEL_PAD) for w in SP.problems()] + \
+    """The paddings of the chain test of the one-CTA sort and of the selector problems."""
+    cases = [(w, SP.SORT_CHAIN_PAD(w)) for w in SP.problems()] + \
             [(SP.selector_problem(s), n) for s in SP.SEL_SEEDS for n in (STAGED_CAP + 1, 262_145, 2_097_153)]
     for w, n_total in cases:
-        v = SP.padded(w, n_total, SP.SMALL_TILE if n_total <= 8192 else None)
+        v = SP.padded(w, n_total)
         assert v.n_claim == n_total and (v.n_claim <= 8192) == (n_total <= 8192)
         keep = _kept(v, v.lo, v.hi, True)
         assert np.nonzero(keep)[0].tolist() == v.pos.tolist(), w.name
         assert v.claims[keep].tobytes() == SP.behind_empty_node(w).claims.tobytes(), w.name
-        if n_total == SP.IN_KERNEL_PAD:
-            assert -(-n_total // 1024) <= v.hi - v.lo + 1
 
 
 def test_selector_problems_reach_the_claim_beyond_the_table(oracle):
