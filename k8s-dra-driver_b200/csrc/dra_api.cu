@@ -1736,6 +1736,9 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     a.n_node = ctx->n_node; a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.sel = sel_of(ctx); a.err = err_of(ctx);
     k_pods_place_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, ctx->stream>>>(a);
     ctx->launches += 1;
+    // A candidate form with no pair sorts nothing, so the visit lists are zeroed instead: the walk must not read the
+    // offsets an earlier call's sort left in d_claim_off (an Allocate's claims by node), as lists of this call's pairs
+    if (!dense && !n_pair) CU(cudaMemsetAsync(ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, ctx->stream));
     if (!dense && n_pair &&
         (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, a.inv_src, LA_NONE, ctx->n_node, ctx->d_node_off)))
         return rc;
@@ -1960,6 +1963,9 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     PpArgs pp{ctx->d_pp_pending, ctx->d_pp_evicted, ctx->d_pp_judged};
     k_pp_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, pl, pp);
     ctx->launches += 1;
+    // A candidate form with no pair sorts nothing, so the visit lists are zeroed instead: the walk must not read the
+    // offsets an earlier call's sort left in d_claim_off (an Allocate's claims by node), as lists of this call's pairs
+    if (!dense && !n_pair) CU(cudaMemsetAsync(ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, st));
     if (!dense && n_pair &&
         (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, LA_NONE, ctx->n_node, ctx->d_node_off)))
         return rc;
@@ -2802,6 +2808,9 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     k_spod_gate<<<gate_grid, 256, 0, ctx->stream>>>(sa_sort, gather ? ctx->peer_cap : 0u, fresh ? ctx->d_inv_pristine : nullptr,
                                                     ctx->d_inv_live, ctx->d_node_off);
     ctx->launches += 2;
+    // A candidate form with no pair sorts nothing, so the visit lists are zeroed instead: the walk must not read the
+    // offsets an earlier call's sort left in d_claim_off (an Allocate's claims by node), as lists of this call's pairs
+    if (!dense && !n_pair) CU(cudaMemsetAsync(ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, ctx->stream));
     if (!dense && n_pair && n_win &&
         (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, LA_NONE, n_win, d_node_off,
                           ctx->d_spod + SP_NDEV)))
@@ -3135,6 +3144,9 @@ int dra_preempt_place_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
     s.inv_src = ctx->d_spp_inv; s.inv_dst = ctx->d_inv_live; s.gpu_lo = gpu_lo; s.gpu_hi = gpu_hi;
     k_spp_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, pl, pp, s);
     ctx->launches += 1;
+    // A candidate form with no pair sorts nothing, so the visit lists are zeroed instead: the walk must not read the
+    // offsets an earlier call's sort left in d_claim_off (an Allocate's claims by node), as lists of this call's pairs
+    if (!dense && !n_pair) CU(cudaMemsetAsync(ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, st));
     if (!dense && n_pair &&
         (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_spp_inv, LA_NONE, ctx->n_node, ctx->d_node_off)))
         return rc;

@@ -78,11 +78,11 @@ def preempt_place(gpus, node_off, table, claims, pod_off, prio, run_claims, run_
 
 
 def preempt_place_naive(gpus, node_off, table, claims, pod_off, prio, cands, exhaustive, run_claims, run_pod_off,
-                        run_prio, run_out, out_off=None):
-    """spec §15 as the host loop, on the naive restatements (small cases, no selectors, running pods without out_off).
-    gpus / claims / run_claims: lists of dicts as naive.py takes them; run_out: list of (gpu, start, size, profile,
-    status); cands: one list of node indices per pod, or None for every node ascending.  Returns (out list, pod_node,
-    pod_status, evicted_by, gpus_after)."""
+                        run_prio, run_out, out_off=None, run_out_off=None):
+    """spec §15 as the host loop, on the naive restatements (small cases, no selectors).  gpus / claims / run_claims:
+    lists of dicts as naive.py takes them; run_out: list of (gpu, start, size, profile, status), run_out_off: the
+    running claims' slot offsets into it, or None for one slot each; cands: one list of node indices per pod, or None
+    for every node ascending.  Returns (out list, pod_node, pod_status, evicted_by, gpus_after)."""
     from oracle import naive as N
     from preempt_oracle import preempt_naive
     n_node = len(node_off) - 1
@@ -98,17 +98,19 @@ def preempt_place_naive(gpus, node_off, table, claims, pod_off, prio, cands, exh
 
     def release(r):                                   # §9 on the state dicts
         for i in range(run_pod_off[r], run_pod_off[r + 1]):
-            c, (gpu, start, size, _, st) = run_claims[i], run_out[i]
-            if st != 0:
-                continue
-            g = G[gpu]
-            if c["kind"] == 0:
-                g["full"] = False
-            elif c["kind"] == 1:
-                g["used"] -= set(range(start, min(start + size, 16))) if start < 16 else set()
-            elif c["kind"] == 2:
-                g["mem"] = (g["mem"] + c["mem_limit_mib"]) % (1 << 32)
-                g["share"] = (g["share"] - 1) % (1 << 16)
+            c = run_claims[i]
+            base = i if run_out_off is None else run_out_off[i]
+            for gpu, start, size, _, st in run_out[base: base + N._slots(c, n_node, run_out_off is not None)]:
+                if st != 0:
+                    continue
+                g = G[gpu]
+                if c["kind"] == 0:
+                    g["full"] = False
+                elif c["kind"] == 1:
+                    g["used"] -= set(range(start, min(start + size, 16))) if start < 16 else set()
+                elif c["kind"] == 2:
+                    g["mem"] = (g["mem"] + c["mem_limit_mib"]) % (1 << 32)
+                    g["share"] = (g["share"] - 1) % (1 << 16)
 
     for p in range(len(pod_off) - 1):
         c0, c1 = pod_off[p], pod_off[p + 1]
@@ -124,8 +126,9 @@ def preempt_place_naive(gpus, node_off, table, claims, pod_off, prio, cands, exh
                 rpo.append(rpo[-1] + run_pod_off[r + 1] - run_pod_off[r])
             _, _, node, st, nv, rows = preempt_naive(
                 N._dump(gpus, G), node_off, table, pod, [0, len(pod)], [prio[p]], None if cands is None else [cands[p]],
-                exhaustive, [run_claims[i] for i in idx], rpo, [run_prio[r] for r in alive], [run_out[i] for i in idx],
-                None, max(len(alive), 1))
+                exhaustive, [run_claims[i] for i in idx], rpo, [run_prio[r] for r in alive],
+                [run_out[i] for i in idx] if run_out_off is None else run_out,
+                None if run_out_off is None else [run_out_off[i] for i in idx], max(len(alive), 1))
             node, st = node[0], st[0]
             for v in rows[0][: nv[0]]:
                 evicted_by[alive[v]] = p

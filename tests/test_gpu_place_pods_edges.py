@@ -307,6 +307,31 @@ def test_fresh_inventory_on_a_changed_live_state(pkg, pctx):
         check(pkg, pctx, few, flags, f"fresh dense f{flags}", dense=True, start=g)
 
 
+def test_no_candidates_after_a_sorted_allocate(pkg, oracle):
+    """The candidate form with no candidate at all sorts no pair, so the walk must find every visit list empty, not the
+    node offsets the previous call's counting sort left (here an Allocate on the sorting chain): every pod is placed
+    nowhere and the inventory keeps what the Allocate took."""
+    A, R = pkg.api, pkg.records
+    w = pkg.synth.mixed(600, 8, 5)
+    with A.Context(device=0, flags=A.CFG_NO_FUSED) as ctx:
+        ctx.set_table(w.table)
+        ctx.set_inventory(w.gpus, w.node_off)
+        out = ctx.allocate(w.claims, w.out_off, w.n_out)
+        assert not {"fused_staged", "fused_stream", "fused_direct"} & ctx.last_chain()
+        ref, live = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out)
+        assert out.tobytes() == ref.tobytes() and ctx.get_inventory().tobytes() == live.tobytes()
+        c, po = w.claims[:6].copy(), np.array([0, 2, 4, 6], np.uint32)
+        placed = c.copy()
+        placed["node"] = 0
+        oo, n_out = R.out_offsets(placed, 1)
+        cn, co = np.zeros(0, np.uint32), np.zeros(4, np.uint32)
+        for flags in (0, A.F_EXHAUSTIVE):
+            got, node = ctx.place_pods(c, po, cn, co, oo, n_out, flags)
+            want, want_node, after = P.place_pods(live, w.node_off, w.table, c, po, cn, co, oo, n_out, flags)
+            assert got.tobytes() == want.tobytes() and node.tobytes() == want_node.tobytes(), flags
+            assert (node == NONE).all() and ctx.get_inventory().tobytes() == live.tobytes(), flags
+
+
 # ---- f. the same problems on a sharded world ------------------------------------------------------------------------
 def _sharded(pkg, pb, world, kind, flags, what):
     w = SimpleNamespace(gpus=pb.gpus, node_off=pb.node_off, table=pb.table, n_node=pb.n_node)

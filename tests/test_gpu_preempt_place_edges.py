@@ -473,3 +473,33 @@ def test_sharded_fixtures(pkg, monkeypatch):
     for i, pb in enumerate(pbs):
         for world, kind in CONFIGS:
             _sharded(pkg, pb, world, kind, what=f"fixture {i}")
+
+
+# ---- 8. no candidate at all after a sorting call --------------------------------------------------------------------
+def test_no_candidates_after_a_sorted_allocate(pkg, oracle):
+    """The candidate form with no candidate at all sorts no pair, so the walk must find every visit list empty.  It once
+    read instead the node offsets the previous call's counting sort had left (here an Allocate on the sorting chain), as
+    lists of pairs this call never had, and failed.  Every pod is placed nowhere, and the inventory keeps what the Allocate
+    took."""
+    A, R = pkg.api, pkg.records
+    w = pkg.synth.mixed(600, 8, 5)
+    with A.Context(device=0, flags=A.CFG_NO_FUSED) as ctx:
+        ctx.set_table(w.table)
+        ctx.set_inventory(w.gpus, w.node_off)
+        out = ctx.allocate(w.claims, w.out_off, w.n_out)
+        assert not {"fused_staged", "fused_stream", "fused_direct"} & ctx.last_chain()
+        ref, live = oracle.allocate(w.gpus, w.node_off, w.table, w.claims, w.out_off, w.n_out)
+        assert out.tobytes() == ref.tobytes() and ctx.get_inventory().tobytes() == live.tobytes()
+        c, po = w.claims[:6].copy(), np.array([0, 2, 4, 6], np.uint32)
+        placed = c.copy()
+        placed["node"] = 0
+        oo, n_out = R.out_offsets(placed, 1)
+        cn, co = np.zeros(0, np.uint32), np.zeros(4, np.uint32)
+        run = (c[:0], np.zeros(1, np.uint32), np.zeros(0, np.int32), np.zeros(0, R.OUT_DTYPE))
+        prio = np.array([5, 5, 5], np.int32)
+        for flags in (0, P.F_EXHAUSTIVE):
+            got = ctx.preempt_place(c, po, prio, *run, None, cn, co, oo, n_out, flags)
+            want = PP.preempt_place(live, w.node_off, w.table, c, po, prio, *run, None, cn, co, oo, n_out, flags)
+            for name, x, y in zip(NAMES, got, want):
+                assert x.tobytes() == y.tobytes(), (flags, name)
+            assert (got[1] == NONE).all() and ctx.get_inventory().tobytes() == live.tobytes(), flags
