@@ -1569,7 +1569,64 @@ struct NodeCtx {
         small8 = homog && __all_sync(FULLMASK, lane >= DRA_MAX_PROFILES ||
                                      (lds32(tbl_addr + ((m0 * DRA_MAX_PROFILES + (lane & (DRA_MAX_PROFILES - 1))) << 2)) & 0xFFu) <= 8u);
     }
+    // k_fused's node-wide pack: lane p writes, at addr + 32p, the prepared MIG record of profile p on this node's table
+    // row (meaningful on a homogeneous node), as segment_run builds it, with the static failure word where the record
+    // keeps its out slot: {s1, s2, s3, s4}, {start mask | p<<16 | 1<<24, failure word, 0, size bits}
+    __device__ __forceinline__ void shape_table(uint32_t addr) const {
+        if (lane < DRA_MAX_PROFILES) {
+            const uint32_t e = lds32(tbl_addr + ((m0 * DRA_MAX_PROFILES + lane) << 2));
+            const uint32_t size = e & 0xFFu, sh = shifts_of(size);
+            const uint32_t fail = 0xFFu | (((offer_any && (e >> 16) != 0) ? DRA_ST_NO_CAPACITY : DRA_ST_BAD_PROFILE) << 24);
+            sts128(addr + (lane << 5), make_uint4(sh & 15u, (sh >> 4) & 15u, (sh >> 8) & 15u, sh >> 12));
+            sts128(addr + (lane << 5) + 16, make_uint4((e >> 16) | (lane << 16) | (1u << 24), fail, 0u, (1u << size) - 1u));
+        }
+    }
 };
+
+// The lean MIG loop (segment_run's common case, and k_fused's node-wide pack): n prepared records at rec_addr, one
+// result word each at res_addr.  A single warp is bound by max(loop-carried chain at ~6 cycles per dependent ALU op,
+// 2 cycles per ALU instruction) — profiles/chain_bench.cu measures it against the earlier forms — so:
+//  - the state is the FREE mask (no NOT on the chain), 0 on lanes that cannot take MIG devices;
+//  - the start mask is static: a shape that died earlier simply finds no candidate (occupancy only grows), so
+//    no dead-shape memo is read here;
+//  - no failure handling at all: every result word was initialised to the shape's (static) failure;
+//  - winner test = one LOP3 with a predicate output, update = select between two precomputed masks.
+// STOP (node-wide pack): r1.z of a record holds the shapes of that record and of every record after it (low 16 bits)
+// and its own shape (high 16 bits).  A vote of 0 kills the record's shape for the rest of the node (a predicated
+// AND, off the chain); the loop leaves at the top of a pair of records once no shape of the records left is alive —
+// their failure words stand.  Returns the number of records stepped.
+template <int NR, bool STOP>
+__device__ __forceinline__ uint32_t lean_loop(uint32_t& fre, const uint32_t gate, const uint32_t lane,
+                                              const uint32_t rec_addr, const uint32_t res_addr, const uint32_t n) {
+    const uint32_t lanebit = 1u << lane, lemask = lanebit | (lanebit - 1u);
+    uint32_t alive = 0xFFFFu;
+    auto fstep = [&](const uint4 r0, const uint4 r1, const uint32_t q) {
+        uint32_t t = fre;
+        t &= t >> r0.x; t &= t >> r0.y; t &= t >> r0.z;
+        if (NR == 4) t &= t >> r0.w;                                   // shapes of 9..16 slices
+        const uint32_t cand = t & r1.x & gate;                         // gate has 16 bits: drops prof/class of r1.x
+        const uint32_t b = __ballot_sync(FULLMASK, cand != 0);
+        const uint32_t low = cand & (0u - cand);                       // lowest start, one-hot
+        const uint32_t freW = fre & ~(r1.w * low);                     // off the chain: overlaps the vote
+        const bool lose = ((b & lemask) ^ lanebit) != 0;               // win: lowest GPU with a candidate
+        fre = lose ? fre : freW;
+        sts32_if(!lose, res_addr + (q << 2), lane + (cand << 8));      // start = lowest set bit, decoded in the epilogue
+        if (STOP) alive = b ? alive : (alive & ~(r1.z >> 16));
+    };
+    // ping-pong: the next record is in flight while the current one is stepped
+    uint4 a0 = lds128(rec_addr), a1 = lds128(rec_addr + 16), b0, b1;
+    uint32_t q = 0;
+    for (; q < n; q += 2) {
+        if (STOP && (alive & a1.z) == 0) break;
+        const uint32_t nb_ = rec_addr + ((q + 1) << 5);
+        if (q + 1 < n) { b0 = lds128(nb_); b1 = lds128(nb_ + 16); }
+        fstep(a0, a1, q);
+        if (q + 1 >= n) { ++q; break; }
+        if (q + 2 < n) { a0 = lds128(nb_ + 32); a1 = lds128(nb_ + 48); }
+        fstep(b0, b1, q + 1);
+    }
+    return q;
+}
 
 // One segment of <= 32 consecutive claims of the node; lane j holds claim j (c.y = first out slot).
 //   1. lane-parallel: malformed claims and request shapes already known to fail on this node (Dead memo)
@@ -1737,40 +1794,11 @@ __device__ __forceinline__ void segment_run(NodeCtx& x, const uint4 c, const boo
             sstep(b0, q + 1);
         }
     } else if (fast) {
-        // Lean step (profiles/chain_bench.cu measures it against the earlier forms).  A single warp is
-        // bound by max(loop-carried chain at ~6 cycles per dependent ALU op, 2 cycles per ALU instruction), so:
-        //  - the state is the FREE mask (no NOT on the chain), 0 on lanes that cannot take MIG devices;
-        //  - the start mask is static: a shape that died earlier simply finds no candidate (occupancy only grows), so
-        //    the dead-shape memo is not read here; it is brought up to date once, in the epilogue;
-        //  - no failure handling at all: the pre-pass initialised every result word to the shape's (static) failure;
-        //  - winner test = one LOP3 with a predicate output, update = select between two precomputed masks.
+        // the lean loop; the dead-shape memo is brought up to date once, in the epilogue
         uint32_t fre = ~L.busy & x.gate;
-        const uint32_t lemask = lanebit | (lanebit - 1u), gate = x.gate;
-        auto fstep = [&](auto NRtag, const uint4 r0, const uint4 r1, const uint32_t q) {
-            uint32_t t = fre;
-            t &= t >> r0.x; t &= t >> r0.y; t &= t >> r0.z;
-            if (decltype(NRtag)::value == 4) t &= t >> r0.w;               // shapes of 9..16 slices
-            const uint32_t cand = t & r1.x & gate;                         // gate has 16 bits: drops prof/class of r1.x
-            const uint32_t b = __ballot_sync(FULLMASK, cand != 0);
-            const uint32_t low = cand & (0u - cand);                       // lowest start, one-hot
-            const uint32_t freW = fre & ~(r1.w * low);                     // off the chain: overlaps the vote
-            const bool lose = ((b & lemask) ^ lanebit) != 0;               // win: lowest GPU with a candidate
-            fre = lose ? fre : freW;
-            sts32_if(!lose, res_addr + (q << 2), lane + (cand << 8));      // start = lowest set bit, decoded in the epilogue
-        };
-        auto floop = [&](auto NRtag) {
-            uint4 a0 = lds128(x.live_addr), a1 = lds128(x.live_addr + 16), b0, b1;
-            for (uint32_t q = 0; q < nlive; q += 2) {
-                const uint32_t nb_ = x.live_addr + ((q + 1) << 5);
-                if (q + 1 < nlive) { b0 = lds128(nb_); b1 = lds128(nb_ + 16); }
-                fstep(NRtag, a0, a1, q);
-                if (q + 1 >= nlive) break;
-                if (q + 2 < nlive) { a0 = lds128(nb_ + 32); a1 = lds128(nb_ + 48); }
-                fstep(NRtag, b0, b1, q + 1);
-            }
-        };
-        if (x.small8) floop(std::integral_constant<int, 3>{}); else floop(std::integral_constant<int, 4>{});
-        L.busy = gate ? (~fre & 0xFFFFu) : L.busy;
+        if (x.small8) lean_loop<3, false>(fre, x.gate, lane, x.live_addr, res_addr, nlive);
+        else lean_loop<4, false>(fre, x.gate, lane, x.live_addr, res_addr, nlive);
+        L.busy = x.gate ? (~fre & 0xFFFFu) : L.busy;
     } else {
     // ping-pong: the next record is in flight while the current one is stepped, no register shuffling
     uint4 a0 = lds128(x.live_addr), a1 = lds128(x.live_addr + 16), b0, b1;
@@ -1927,6 +1955,7 @@ k_pack(const PackArgs a) {
 // n_node SMs and every byte after the first CTA's touch comes from L2.
 // dynamic smem: [tbl 1024][bars 16][inv 512][live 1024+128][counts 64][index lists: n_claim u32, warp w at w*chunk]
 constexpr uint32_t FU_TBL = 0, FU_TBAR = 1024, FU_IBAR = 1032, FU_INV = 1040, FU_LIVE = 1552, FU_CNT = 2704, FU_LIST = 2832;   // counts: up to 32 warps
+constexpr uint32_t FU_LEAN = FU_CNT + 112;  // u32 in the counts area (behind the 8 warp counts, 8 slot counts and 4 words): 1 = try the node-wide pack
 constexpr uint32_t FU_PIECE = 256;          // claims per staged piece: one warp's 8 loads of 32 claims
 constexpr uint32_t FU_MAXPIECE = 8;         // pieces per warp part => staging needs n_claim <= NW * 2048
 // per-warp part of the claim array: a multiple of 32 claims, of a whole piece when the array is staged
@@ -2009,6 +2038,7 @@ struct Batch {
 
 template <int NW, bool STAGE>
 __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uint8_t* dyn_smem, const bool again) {
+    static_assert(NW <= 8, "the counts area holds 8 warp counts, 8 slot counts, 4 words of the tail and FU_LEAN");
     DRA_STAMP(0); DRA_STAMP(1); DRA_TSTAMP(0);
     const uint32_t sbase = smem_base(dyn_smem);
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -2102,6 +2132,12 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
         mbar_wait_a(tbar, 0);
         if (ng) { mbar_wait_a(ibar, 0); if (lane < ng) rec = lds128(sbase + FU_INV + lane * 16); }
         x.begin(rec, lane < ng);
+        // the node-wide pack below: only a homogeneous node that offers MIG devices tries it.  The flag lives in a spare
+        // word of the counts area, which nothing else writes: warp 0 may already pack segment by segment (and write
+        // the live area) while another warp still reads it.
+        const bool try_lean = x.homog && x.offer_any;
+        if (try_lean) x.shape_table(sbase + FU_LIVE);    // read by every warp after the filter
+        if (lane == 0) sts32(sbase + FU_LEAN, try_lean ? 1u : 0u);
     }
 
     // ---- filter: which claims select this node (all warps) ------------------------------------------
@@ -2201,20 +2237,63 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
             else a.err.set(ERR_OUT_RANGE);
         }
     }
+    // ---- node-wide pack (all warps): a homogeneous node whose claims are all plain MIG claims --------------------
+    // Thread m prepares claim m's record once for the whole node, warp 0 runs ONE lean loop over all of them, and thread
+    // q stores OutRec q — instead of a pre-pass, a loop and an epilogue per 32-claim segment on warp 0 alone.  The
+    // records overwrite the index lists (read into registers first); the multi-GPU tail without a send queue still
+    // needs those lists, so it keeps the per-segment pack.
+    long long pre_t0 = 0;
+    const uint32_t rec_addr = list_addr, res_addr = list_addr + (cnt << 5);
+    // (a node that offers no MIG device, or whose GPUs differ, never takes it: such nodes skip the preparation and its vote)
+    bool lean = has_node && cnt != 0 && cnt <= (uint32_t)NW * 32u && (!gather || use_q) &&
+                cnt * 36u <= (uint32_t)fused_list_bytes(b.n_claim, NW, STAGE) && lds32(sbase + FU_LEAN) != 0;
+    uint4 c_m = make_uint4(0xFFu, 0, 0, 0);                   // claim m = threadIdx.x of the node (warp 0: segment 0)
+    const bool tried = lean;
+    if (lean) {                                               // CTA-uniform
+        DRA_STAMP(5);
+        if (a.timeline && threadIdx.x == 0) pre_t0 = clock64();
+        const uint32_t m = threadIdx.x;
+        const bool have = m < cnt;
+        if (have) c_m = get(m);
+        const uint32_t kind = c_m.x & 0xFFu, prof = (c_m.x >> 8) & 0xFFu;
+        // plain MIG claim: valid profile, no selector (c.z), no co-location group (c.w).  The vote does not wait for the
+        // out slot (c.y, an out_off load): a claim whose slot is out of range gets a record that never wins and never
+        // kills its shape, and raises the range error in the epilogue.
+        const bool plain = !have || (kind == DRA_KIND_MIG && prof < DRA_MAX_PROFILES && c_m.z == 0 && c_m.w == 0);
+        // shapes of this claim and of every later claim of the warp's part (suffix OR); warp totals for the others
+        uint32_t suf = have ? 1u << (prof & 31u) : 0u;
+        #pragma unroll
+        for (int d = 1; d < 32; d <<= 1) suf |= __shfl_down_sync(FULLMASK, suf, d);   // (the top lanes get their own: harmless)
+        if (lane == 0) sts32(sbase + FU_LIVE + 1024 + (wid << 2), suf);
+        lean = __syncthreads_and(plain && (wid != 0 || x.homog)) != 0;
+        if (lean) {
+            if (have) {
+                #pragma unroll
+                for (int w = 1; w < NW; ++w) if ((uint32_t)w > wid) suf |= lds32(sbase + FU_LIVE + 1024 + (w << 2));
+                const uint32_t t_ = sbase + FU_LIVE + (prof << 5);
+                const uint4 t0 = lds128(t_), t1 = lds128(t_ + 16);
+                const bool oor = c_m.y >= b.n_out;           // (its shape stays in the suffixes: they only end the loop early)
+                sts128(rec_addr + (m << 5), t0);
+                sts128(rec_addr + (m << 5) + 16, make_uint4(oor ? t1.x & 0xFFFF0000u : t1.x, c_m.y,
+                                                            suf | (oor ? 0u : 1u << (prof + 16)), t1.w));
+                sts32(res_addr + (m << 2), t1.y);
+            }
+        }
+    }
     // ---- pack: warp 0 ----------------------------------------------------------------------------------
-    if (wid == 0 && has_node) {
+    if (wid == 0 && has_node && !lean) {
         if (cnt == 0) {
             if (b.inv_src != a.inv_dst && lane < ng) a.inv_dst[g0 + lane] = __ldg(&b.inv_src[g0 + lane]);
         } else {
-            // the first segment's claims are requested before waiting for the table / inventory
+            // the first segment's claims are requested before waiting for the table / inventory (or were fetched above)
             auto fetch = [&](uint32_t seg, uint4& c, bool& present) {
                 const uint32_t m = seg * SEG + lane;
                 present = m < cnt;
                 c = make_uint4(0xFFu, 0, 0, 0);
                 if (present) c = get(m);
             };
-            uint4 c_cur; bool p_cur;
-            fetch(0, c_cur, p_cur);
+            uint4 c_cur = c_m; bool p_cur = lane < cnt;
+            if (!tried) fetch(0, c_cur, p_cur);
 
             x.prof_on = a.timeline != nullptr;
             if (use_q) { x.sink.q_addr = q_base; x.sink.q_cap = a.q_cap; x.sink.q_cnt = q_cnt_addr; x.sink.q_tag = q_tag; }
@@ -2240,6 +2319,48 @@ __device__ __forceinline__ void fused_body(const PackArgs& a, const Batch b, uin
                     ((unsigned long long)(x.t_fetch & 0xFFFF) << 32) | ((unsigned long long)(x.t_pre_a & 0xFFFF) << 48);
                 a.timeline[blockIdx.x * 8 + 0] = (unsigned long long)x.t_pre | ((unsigned long long)x.t_loop << 20) | ((unsigned long long)x.t_epi << 40);
             }
+        }
+    }
+    // the node-wide pack's loop and epilogue, placed after the per-segment pack so that a node taking that one runs its
+    // code straight through
+    if (lean) {                                               // CTA-uniform
+        const uint32_t m = threadIdx.x, prof = (c_m.x >> 8) & 0xFFu;
+        const bool have = m < cnt;
+        __syncthreads();
+        long long tl0 = 0, tl1 = 0; uint32_t stepped = 0;
+        if (wid == 0) {
+            if (a.timeline) tl0 = clock64();
+            uint32_t fre = ~x.L.busy & x.gate;
+            stepped = x.small8 ? lean_loop<3, true>(fre, x.gate, lane, rec_addr, res_addr, cnt)
+                               : lean_loop<4, true>(fre, x.gate, lane, rec_addr, res_addr, cnt);
+            x.L.busy = x.gate ? (~fre & 0xFFFFu) : x.L.busy;
+            if (a.timeline) tl1 = clock64();
+        }
+        __syncthreads();
+        // epilogue: thread q composes and stores the OutRec of record q
+        if (have) {
+            OutSink sk{a.out, b.n_out, a.err, lane};
+            if (use_q) { sk.q_addr = q_base; sk.q_cap = a.q_cap; sk.q_cnt = q_cnt_addr; sk.q_tag = q_tag; }
+            const uint4 r1 = lds128(rec_addr + (m << 5) + 16);
+            const uint32_t res = lds32(res_addr + (m << 2)), w = res & 0xFFu;
+            const bool failed = w == 0xFFu;
+            const uint32_t m_ok = ((uint32_t)__popc(r1.w) << 8) | (prof << 16) | ((uint32_t)__ffs((res >> 8) & 0xFFFFu) - 1u);
+            if (r1.y >= b.n_out) a.err.set(ERR_OUT_RANGE);
+            else sk.put(r1.y, failed ? (uint32_t)DRA_GPU_NONE : g0 + w, failed ? meta(0, 0, prof, res >> 24) : m_ok);
+        }
+        if (wid == 0 && lane < ng) a.inv_dst[g0 + lane] = x.L.store(rec);
+        if (use_q) {                                      // the senders may leave after this many
+            __syncthreads();                              // every warp's records are in the queue
+            if (threadIdx.x == 0) { const uint32_t put_ = lds32(q_cnt_addr); sts32(q_done_addr, put_); if (put_ > a.q_cap) a.err.set(ERR_PEER_TIMEOUT); }
+        }
+        DRA_STAMP(6);
+        // pre-pass = preparation, live records = records stepped; the fetch and part-a fields (bits 32..63 of word 7)
+        // stay 0, which is how a reader tells this form from the per-segment one (whose part a is never 0 cycles)
+        if (a.timeline && threadIdx.x == 0) {
+            const long long te = clock64();
+            a.timeline[blockIdx.x * 8 + 7] = (cnt & 0xFFFFu) | ((unsigned long long)(stepped & 0xFFFFu) << 16);
+            a.timeline[blockIdx.x * 8 + 0] = (unsigned long long)(tl0 - pre_t0) | ((unsigned long long)(tl1 - tl0) << 20) |
+                                             ((unsigned long long)(te - tl1) << 40);
         }
     }
     if (use_q && wid != 0) {
