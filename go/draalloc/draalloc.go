@@ -554,6 +554,53 @@ func (c *Context) PodCapacityBatch(claims []ClaimRec, podOff []uint32, cands, ca
 	return r, nil
 }
 
+// UnsuitableWhy is UnsuitableWhyBatch's answer (spec §17): per (pod, candidate) pair the reason (DRA_ST_*, or
+// DRA_WHY_NO_NODE = 8) and the blocking claim (an index into the claims passed, or DRA_WHY_CLAIM_NONE); per pod the
+// pairs of each reason (PodWhy[p*9+r]); per claim the pairs it blocks.
+type UnsuitableWhy struct {
+	PairWhy     []uint8
+	PairClaim   []uint32
+	PodWhy      []uint32
+	ClaimBlocks []uint32
+}
+
+// UnsuitableWhyBatch answers UnsuitableBatch's pairs with the reason each node is unsuitable and the claim that blocks
+// it (dra_unsuitable_why_batch, spec §17).  Pure.  Candidates as PlaceBatch (cands == candOff == nil: every node,
+// ascending, nNode of them).  The claim indices refer to the lowered claims, in lowering order.  Unbuilt, like the rest
+// of this file.
+func (c *Context) UnsuitableWhyBatch(claims []ClaimRec, podOff []uint32, cands, candOff []uint32, nNode int,
+	flags uint32) (*UnsuitableWhy, error) {
+	nPod := len(podOff) - 1
+	if nPod <= 0 {
+		return &UnsuitableWhy{}, nil
+	}
+	nPair := nPod * nNode
+	var cp *C.dra_claim_rec
+	var cn, co *C.uint32_t
+	if len(claims) > 0 {
+		cp = (*C.dra_claim_rec)(unsafe.Pointer(&claims[0]))
+	}
+	if candOff != nil {
+		nPair = int(candOff[nPod])
+		co = (*C.uint32_t)(unsafe.Pointer(&candOff[0]))
+		if len(cands) == 0 {
+			cands = []uint32{0} // an empty list still needs an address (nil means the dense form)
+		}
+		cn = (*C.uint32_t)(unsafe.Pointer(&cands[0]))
+	}
+	r := &UnsuitableWhy{make([]uint8, nPair+1), make([]uint32, nPair+1), make([]uint32, nPod*9), make([]uint32, len(claims)+1)}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_unsuitable_why_batch(c.h, cp, C.uint32_t(len(claims)), (*C.uint32_t)(unsafe.Pointer(&podOff[0])),
+		C.uint32_t(nPod), cn, co, (*C.uint8_t)(unsafe.Pointer(&r.PairWhy[0])), (*C.uint32_t)(unsafe.Pointer(&r.PairClaim[0])),
+		(*C.uint32_t)(unsafe.Pointer(&r.PodWhy[0])), (*C.uint32_t)(unsafe.Pointer(&r.ClaimBlocks[0])), C.uint32_t(flags))
+	if rc != 0 {
+		return nil, lastError(c.h)
+	}
+	r.PairWhy, r.PairClaim, r.ClaimBlocks = r.PairWhy[:nPair], r.PairClaim[:nPair], r.ClaimBlocks[:len(claims)]
+	return r, nil
+}
+
 func (c *Context) DeallocateBatch(claims []ClaimRec, outOff []uint32, out []OutRec) error {
 	if len(claims) == 0 {
 		return nil

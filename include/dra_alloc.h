@@ -95,6 +95,9 @@ typedef struct dra_out_rec {
 #define DRA_ST_INVALID     5u
 #define DRA_ST_POD         6u     /* pod mode (spec §12): the pod does not fit on the node; nothing of it was taken */
 #define DRA_ST_SEARCH_LIMIT 7u    /* pod mode: the exhaustive search ran out of budget (DRA_EXH_BUDGET descents) */
+#define DRA_WHY_NO_NODE    8u     /* dra_unsuitable_why_batch (spec §17): the candidate names no node of the inventory */
+#define DRA_WHY_N          9u     /* reasons of spec §17: DRA_ST_OK .. DRA_ST_SEARCH_LIMIT, DRA_WHY_NO_NODE */
+#define DRA_WHY_CLAIM_NONE 0xFFFFFFFFu   /* spec §17: no blocking claim */
 
 /* One (model, profile) cell of the placement table: what getGpuInfo() collects from
  * GetGpuInstanceProfileInfo + GetGpuInstancePossiblePlacements (nvlib.go:244-295). */
@@ -249,6 +252,32 @@ int  dra_unsuitable_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
                           const uint32_t* pod_off, uint32_t n_pod,
                           const uint32_t* cand_nodes, const uint32_t* cand_off,
                           uint8_t* suitable_bits, uint32_t flags /* 0 or DRA_F_EXHAUSTIVE (spec §12) */);
+
+/* Why each node is unsuitable (spec §17): dra_unsuitable_batch's pairs, each answered with a reason and the claim that
+ * blocks it, and the per-pod and per-claim tallies of those answers — what a scheduler needs for "0/125 nodes are
+ * available: 100 ..., 25 ...".  Pure: nothing is written to the inventory.  Same inputs and flags as dra_unsuitable_batch
+ * (each claim's node field is ignored).  For pair k:
+ *   pair_why[k]       DRA_ST_OK exactly when dra_unsuitable_batch sets bit k with the same flags; else NO_CAPACITY,
+ *                     BAD_PROFILE, GROUP, MEM_LIMIT, INVALID, POD, SEARCH_LIMIT, or DRA_WHY_NO_NODE for a candidate
+ *                     that names no node of the inventory
+ *   pair_claim[k]     (may be NULL) the blocking claim, a global index into claims, or DRA_WHY_CLAIM_NONE (OK, NO_NODE,
+ *                     and with DRA_F_EXHAUSTIVE a pod of more than DRA_MAX_POD claims)
+ *   pod_why[p * DRA_WHY_N + r]  (may be NULL) how many of pod p's pairs have reason r
+ *   claim_blocks[c]   (may be NULL, n_claim entries) how many pairs name claim c as their blocking claim
+ * Without DRA_F_EXHAUSTIVE the blocking claim is the first claim whose slot an Allocate of the pod on the node's snapshot
+ * leaves not OK (a co-location run: its first member), the reason that slot's status.  With it: INVALID at the lowest
+ * invalid claim; the first GPU / SHARED claim that fails (NO_CAPACITY / MEM_LIMIT); the first MIG claim with no
+ * placement at all (BAD_PROFILE when no GPU of the node offers its profile to it, else NO_CAPACITY); else POD or
+ * SEARCH_LIMIT at the MIG claim of level d, d the most MIG levels the search held placed at once.
+ * DRA_E_INVAL with nothing written: unknown flags, pod_off / cand_off not monotone or not spanning, dense
+ * n_pod * n_node >= 2^32, pair_why NULL with pairs to answer.  n_pod == 0 returns DRA_OK after those checks.  On a
+ * sharded world the call is exact on any rank after dra_shard_sync_inventory_device, which makes that rank's live copy the
+ * world's state. */
+int  dra_unsuitable_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
+                              const uint32_t* pod_off, uint32_t n_pod,
+                              const uint32_t* cand_nodes, const uint32_t* cand_off,
+                              uint8_t* pair_why, uint32_t* pair_claim, uint32_t* pod_why, uint32_t* claim_blocks,
+                              uint32_t flags);
 
 /* Allocate() with pod boundaries (spec §12): what the classic driver's Allocate did after UnsuitableNodes had found
  * an assignment for ALL of a pod's claims on the selected node (SURVEY App. A) — each pod (claims
@@ -773,6 +802,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_PREEMPT_PLACE_SHARD 0x4000000u /* sharded preempt and place: state exchange, the §15 chain on it, own range back */
 #define DRA_K_POD_CAPACITY     0x8000000u /* pod capacity: the pairs' copy counts, the per-pod sums */
 #define DRA_K_POD_CAPACITY_SHARD 0x10000000u /* sharded pod capacity: prep, the window's pairs, exchange, merge with the sums */
+#define DRA_K_UNSUITABLE_WHY   0x20000000u /* reasons of UnsuitableNodes: the pair records, the tallies */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

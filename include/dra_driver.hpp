@@ -121,6 +121,12 @@ public:
     // node name -> copies for pod q; a node the inventory does not know counts 0, and a pod whose claims cannot be
     // lowered gets an empty map (each claim's Error says why).  SelectedNode is not read.
     std::vector<std::map<std::string, uint32_t>> PodCapacityBatch(const std::vector<PodRequest>& pods, uint32_t maxCopies);
+    // why each pod fits none, some or all of its PotentialNodes (spec §17, dra_unsuitable_why_batch), as kube-scheduler's
+    // FitError says it: one message per pod, e.g. `0/3 nodes are available: 2 nodes: claim "c1" (MIG 3g.20gb) no
+    // capacity; 1 node: not in the inventory.`  Nodes are grouped by (reason, blocking claim), largest group first, ties
+    // in the order of PotentialNodes; claims are named by ClaimUID.  Judged as UnsuitableNodesBatch judges them under
+    // SetExhaustive; pure.  A pod whose claims cannot be lowered names its first such claim and its Error.
+    std::vector<std::string> UnsuitableReasonsBatch(const std::vector<PodRequest>& pods);
 
     // live occupancy of one GPU (memory-slice mask), for inspection
     uint16_t BusyMask(const std::string& node, uint32_t gpuIndex);

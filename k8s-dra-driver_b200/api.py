@@ -27,7 +27,9 @@ KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x0
            "compact_lookback": 0x20000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000,
            "place_shard": 0x400000, "preempt": 0x800000, "preempt_shard": 0x1000000,
            "preempt_place": 0x2000000, "preempt_place_shard": 0x4000000, "pod_capacity": 0x8000000,
-           "pod_capacity_shard": 0x10000000}
+           "pod_capacity_shard": 0x10000000, "unsuitable_why": 0x20000000}
+# spec §17: the reasons of dra_unsuitable_why_batch are DRA_ST_OK .. DRA_ST_SEARCH_LIMIT (0 .. 7) and WHY_NO_NODE
+WHY_NO_NODE, WHY_N, WHY_CLAIM_NONE = 8, 9, 0xFFFFFFFF
 
 
 class DraError(RuntimeError):
@@ -69,6 +71,7 @@ SYMBOLS = {
     "dra_allocate_batch_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _u32]),
     "dra_ctx_sync": (_i32, [_vp]),
     "dra_unsuitable_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _u32]),
+    "dra_unsuitable_why_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _u32]),
     "dra_allocate_pods_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _u32]),
     "dra_place_pods_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u32]),
     "dra_deallocate_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
@@ -483,6 +486,29 @@ class Context:
                                                      F_EXHAUSTIVE if exhaustive else 0))
         return (copies[:n_pair], None if stop is None else stop[:n_pair], None if total is None else total[:n_pod],
                 None if nodes is None else nodes[:n_pod])
+
+    def unsuitable_why(self, claims, pod_off, cand_nodes=None, cand_off=None, exhaustive: bool = False,
+                       want_claims: bool = True, want_tallies: bool = True):
+        """Why each node is unsuitable (spec §17): unsuitable()'s pairs, each with a reason and its blocking claim.
+        cand_nodes/cand_off None = every node, pair k = pod * n_node + node.  Pure.  Returns (pair_why u8, pair_claim u32
+        or None, pod_why u32 [n_pod, WHY_N] or None, claim_blocks u32 [n_claim] or None): reason ST_OK exactly where
+        unsuitable() with the same flag sets the bit, WHY_NO_NODE for a candidate naming no node; the blocking claim is a
+        global claim index or WHY_CLAIM_NONE; pod_why counts each pod's pairs by reason, claim_blocks the pairs each claim
+        blocks."""
+        c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
+        po = np.ascontiguousarray(pod_off, dtype=np.uint32)
+        n_pod = len(po) - 1
+        cn, co = _cands(cand_nodes, cand_off)
+        n_pair = n_pod * self.n_node if co is None else int(co[-1])
+        why = np.zeros(max(n_pair, 1), dtype=np.uint8)
+        blk = np.zeros(max(n_pair, 1), dtype=np.uint32) if want_claims else None
+        pod_why = np.zeros((max(n_pod, 1), WHY_N), dtype=np.uint32) if want_tallies else None
+        blocks = np.zeros(max(len(c), 1), dtype=np.uint32) if want_tallies else None
+        self._check(self._lib.dra_unsuitable_why_batch(self._h, _ptr(c), len(c), _ptr(po), n_pod, _ptr(cn), _ptr(co),
+                                                       _ptr(why), _ptr(blk), _ptr(pod_why), _ptr(blocks),
+                                                       F_EXHAUSTIVE if exhaustive else 0))
+        return (why[:n_pair], None if blk is None else blk[:n_pair], None if pod_why is None else pod_why[:n_pod],
+                None if blocks is None else blocks[:len(c)])
 
     def deallocate(self, claims, out, out_off=None):
         """Spec §9: release the OK records `out` of `claims` (slots counted as Allocate counts them).  A claim whose slot

@@ -131,6 +131,8 @@ struct dra_ctx {
     // pod capacity (spec §16): per pair, per pod
     uint16_t* d_cap_copies = nullptr; uint8_t* d_cap_stop = nullptr; size_t cap_cap_pairs = 0;
     unsigned long long* d_cap_total = nullptr; uint32_t* d_cap_nodes = nullptr; size_t cap_cap_pods = 0;
+    uint8_t* d_why = nullptr; uint32_t* d_why_claim = nullptr; size_t cap_why_pairs = 0;      // dra_unsuitable_why_batch
+    uint32_t* d_why_pod = nullptr; size_t cap_why_pods = 0; uint32_t* d_why_blocks = nullptr; size_t cap_why_claims = 0;
 
     // error flags
     uint32_t* d_err = nullptr;            // device memory
@@ -659,13 +661,15 @@ uint32_t pair_grid(const dra_ctx* ctx, uint32_t n) {
     return std::max(1u, std::min((n + per_cta - 1) / per_cta, (uint32_t)ctx->n_sm * 8u));
 }
 
-// k_unsuitable over a.n_walk pairs (win: the sharded call's node window and gate; else the whole inventory).  Enqueues only.
-int launch_unsuitable(dra_ctx* ctx, UnsArgs& a, bool win) {
+// k_unsuitable over a.n_walk pairs (win: the sharded call's node window and gate; else the whole inventory; why: the
+// reasons of spec §17 into a.why / a.why_claim instead of the bits, on the whole inventory).  Enqueues only.
+int launch_unsuitable(dra_ctx* ctx, UnsArgs& a, bool win, bool why = false) {
     const uint32_t grid = pair_grid(ctx, a.n_walk);
     if (a.exhaustive) { if (int rc = walk_counter(ctx, TK_WALK_UNSUITABLE, a.work)) return rc; }
     at_pair_width(ctx, [&](auto w) {
         constexpr int W = decltype(w)::value;
-        const auto k = win ? (a.exhaustive ? k_unsuitable<8, W, true, true> : k_unsuitable<8, W, false, true>)
+        const auto k = why ? (a.exhaustive ? k_unsuitable<8, W, true, false, true> : k_unsuitable<8, W, false, false, true>)
+                     : win ? (a.exhaustive ? k_unsuitable<8, W, true, true> : k_unsuitable<8, W, false, true>)
                            : (a.exhaustive ? k_unsuitable<8, W, true, false> : k_unsuitable<8, W, false, false>);
         k<<<grid, 256, 0, ctx->stream>>>(a);
     });
@@ -1323,7 +1327,8 @@ void dra_ctx_destroy(dra_ctx* c) {
                    c->d_pre_rrec, c->d_pre_vlist, c->d_pre_rout, c->d_pre_vic, c->d_spre_part, c->d_pre_podviol,
                    c->d_pre_pairviol, c->d_pre_rpdb, c->d_pre_vprev, c->d_pre_allowed,
                    c->d_pp_pending, c->d_pp_evicted, c->d_pp_runoff, c->d_pp_judged, c->d_spp_inv, c->d_spp_gate,
-                   c->d_cap_copies, c->d_cap_stop, c->d_cap_total, c->d_cap_nodes, c->d_scap_part};
+                   c->d_cap_copies, c->d_cap_stop, c->d_cap_total, c->d_cap_nodes, c->d_scap_part,
+                   c->d_why, c->d_why_claim, c->d_why_pod, c->d_why_blocks};
     for (void* p : dev) if (p) cudaFree(p);
     for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
@@ -1628,6 +1633,69 @@ int dra_unsuitable_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     collect_timings(ctx, 1);
     if (n_pair) memcpy(suitable_bits, ctx->h_out, ((size_t)n_pair + 7) / 8);
     return DRA_OK;
+}
+
+// Why each node is unsuitable (spec §17): every argument is checked here, before anything is staged or launched, so a
+// rejected call writes nothing.  k_unsuitable's reasons instantiation writes a record per pair, k_why_tally the sums; the
+// outputs reach the caller after one synchronise.
+int dra_unsuitable_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, uint32_t n_pod,
+                             const uint32_t* cand_nodes, const uint32_t* cand_off, uint8_t* pair_why, uint32_t* pair_claim,
+                             uint32_t* pod_why, uint32_t* claim_blocks, uint32_t flags) {
+    if (!ctx || !pod_off || (n_claim && !claims)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_unsuitable_why_batch: unknown flags 0x%x", flags);
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    bool dense; uint32_t n_pair;
+    int rc;
+    if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
+        (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, 0xFFFFFFFFu, ctx->n_node, 0xFFFFFFFFull, dense, n_pair))) return rc;
+    if (n_pair && !pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+    ctx->chain = DRA_K_UNSUITABLE_WHY; ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;
+    CU(cudaSetDevice(ctx->device));
+    if ((rc = ensure_batch(ctx, n_claim, 1, true))) return rc;
+    if ((rc = upload_table(ctx))) return rc;
+    if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
+        (!dense && (rc = grow_set(ctx, ctx->cap_pairs, (size_t)n_pair + 64, ctx->d_cand_nodes, ctx->d_pair_pod))) ||
+        (rc = grow_set(ctx, ctx->cap_why_pairs, (size_t)n_pair + 8, ctx->d_why, ctx->d_why_claim)) ||
+        (rc = grow_set(ctx, ctx->cap_why_pods, (size_t)n_pod * DRA_WHY_N + 8, ctx->d_why_pod)) ||
+        (rc = grow_set(ctx, ctx->cap_why_claims, (size_t)n_claim + 8, ctx->d_why_blocks))) return rc;
+    const Outputs outs = {{pair_why, ctx->d_why, (size_t)n_pair},
+                          {pair_claim, ctx->d_why_claim, pair_claim ? (size_t)n_pair * 4 : 0},
+                          {pod_why, ctx->d_why_pod, pod_why ? (size_t)n_pod * DRA_WHY_N * 4 : 0},
+                          {claim_blocks, ctx->d_why_blocks, claim_blocks ? (size_t)n_claim * 4 : 0}};
+    if ((rc = reserve_out(ctx, outs))) return rc;
+    Staging s;
+    s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
+    s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
+    if (!dense) {
+        s.add(ctx->d_cand_off, cand_off, ((size_t)n_pod + 1) * 4);
+        s.add(ctx->d_cand_nodes, cand_nodes, (size_t)n_pair * 4);
+        s.add(ctx->d_pair_pod, nullptr, (size_t)n_pair * 4);
+    }
+    if ((rc = stage_in(ctx, s, [&](uint8_t* h) { expand_pairs((uint32_t*)h, cand_off, n_pod); }))) return rc;
+    if (claim_blocks && n_claim) CU(cudaMemsetAsync(ctx->d_why_blocks, 0, (size_t)n_claim * 4, ctx->stream));
+    Prof prof(ctx);
+    if (n_pair) {
+        UnsArgs a; memset(&a, 0, sizeof a);
+        a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.n_pod = n_pod;
+        a.cand_nodes = ctx->d_cand_nodes; a.pair_pod = ctx->d_pair_pod;
+        a.cand_off = dense ? nullptr : ctx->d_cand_off;
+        a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.tbl = ctx->d_tbl;
+        a.sel = sel_of(ctx);
+        a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
+        a.n_walk = n_pair;                                 // (the window is the whole inventory)
+        a.why = ctx->d_why; a.why_claim = ctx->d_why_claim;
+        if ((rc = launch_unsuitable(ctx, a, false, true))) return rc;
+    }
+    if (pod_why || claim_blocks) {
+        const WhyTally t{ctx->d_why, ctx->d_why_claim, dense ? nullptr : ctx->d_cand_off, n_pod, ctx->n_node,
+                         pod_why ? ctx->d_why_pod : nullptr, claim_blocks ? ctx->d_why_blocks : nullptr};
+        k_why_tally<<<n_pod / 8 + 1, 256, 0, ctx->stream>>>(t);
+        ctx->launches += 1;
+    }
+    prof.mark();
+    return read_back(ctx, "unsuitable reasons kernels", 1, outs);
 }
 
 // Allocate with pod boundaries (spec §12): pod records -> stable counting sort of the PODS by node (the claim path's

@@ -194,6 +194,18 @@ struct FlagSink {
     __device__ __forceinline__ bool stop() const { return failed; }
 };
 
+// Sink for the reasons of UnsuitableNodes (spec §17): FlagSink that also keeps the status of the first failure
+// (a co-location run that fails reports GROUP through mark_failed).
+struct WhySink {
+    bool failed = false; uint32_t st = DRA_ST_OK;
+    __device__ __forceinline__ bool range(uint32_t, uint32_t) const { return true; }
+    __device__ __forceinline__ void put(uint32_t, uint32_t, uint32_t) const {}
+    __device__ __forceinline__ bool in_range(uint32_t) const { return true; }
+    __device__ __forceinline__ void fail(uint32_t, uint32_t, uint32_t, uint32_t s) { if (!failed) st = s; failed = true; }
+    __device__ __forceinline__ void mark_failed() { if (!failed) st = DRA_ST_GROUP; failed = true; }
+    __device__ __forceinline__ bool stop() const { return failed; }
+};
+
 // ---- selectors (spec §10) ----------------------------------------------------------------------------
 // GpuAttr as uint4: x memTotalMiB, y cc, z index, w product | driverMajor<<16.  Selector = 4 x uint4 (8 SelIns).
 struct SelCtx { const uint4* attrs; const uint4* sels; uint32_t n_sel; };
@@ -2572,7 +2584,10 @@ struct PodGet {            // claim m of the pod, .y = its first OutRec slot
 // Evaluates the pod pc[0..cnt) (cnt <= 32) on the node whose GPUs sit on the W lanes gbase.. of this warp.
 // Returns 0 when the pod was placed (L updated, OutRecs written when out != nullptr), else the failure status
 // (L untouched, every slot of the pod rewritten with it / INVALID).  All lanes of the group must call it together.
-template <int W>
+// WHY (spec §17): a failure returns instead its reason | blocking position << 8 — INVALID at the lowest invalid claim;
+// NO_CAPACITY / MEM_LIMIT at the first GPU / SHARED claim that fails; BAD_PROFILE / NO_CAPACITY at the first MIG claim
+// the pre-check rejects; POD / SEARCH_LIMIT at the MIG claim of level d, the most levels the search held at once.
+template <int W, bool WHY = false>
 __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const uint32_t gmask, const uint32_t gbase,
                                           const uint32_t g0, const uint32_t* __restrict__ tbl_s, const PodGet get,
                                           const uint32_t cnt, const SelCtx sc, const bool exhaustive, const bool have_off,
@@ -2597,6 +2612,8 @@ __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const ui
         grpmask |= ((__ballot_sync(gmask, mig && c.w != 0) & gmask) >> gbase) << (q * W);
     }
     uint32_t status = invmask ? (uint32_t)DRA_ST_POD : 0u;
+    uint32_t why = 0;                          // WHY: the reason | blocking position << 8
+    if constexpr (WHY) if (invmask) why = DRA_ST_INVALID | ((uint32_t)(__ffs(invmask) - 1) << 8);
     // ---- 2. the GPU / SHARED claims, in order, by the default rules (spec §4, §7) ----
     if (!status) {
         PodSink ps{out};
@@ -2605,6 +2622,8 @@ __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const ui
         while (nm && !ps.failed) {
             const uint32_t pos = (uint32_t)__ffs(nm) - 1u; nm &= nm - 1u;
             (void)node_step(L, D, lane, g0, tbl_s, get, pos, cnt, ps, have_off, sc, gmask, gbase);
+            if constexpr (WHY)
+                if (ps.failed) why = ((get(pos).x & 0xFFu) == DRA_KIND_GPU ? DRA_ST_NO_CAPACITY : DRA_ST_MEM_LIMIT) | (pos << 8);
         }
         if (ps.failed) status = DRA_ST_POD;
     }
@@ -2618,7 +2637,14 @@ __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const ui
             bool ok = L.valid && (L.flags & BLOCKED) == DRA_GPU_MIG_ENABLED && (e >> 16) != 0;
             if (c.z != 0) ok = sel_pass(sc, c.z, g0 + gl, L.valid) && ok;
             const bool fits = ok && (fit_map(~L.busy & 0xFFFFu, e & 0xFFu) & (e >> 16)) != 0;
-            if (!(__ballot_sync(gmask, fits) & gmask)) status = DRA_ST_POD;
+            if (!(__ballot_sync(gmask, fits) & gmask)) {
+                status = DRA_ST_POD;
+                if constexpr (WHY) {                                              // spec §5's "offers", the claim's selector
+                    const bool offers = L.valid && (L.flags & (DRA_GPU_MIG_ENABLED | DRA_GPU_UNAVAILABLE)) == DRA_GPU_MIG_ENABLED &&
+                                        (e >> 16) != 0 && (c.z == 0 || sel_pass(sc, c.z, g0 + gl, L.valid));
+                    why = ((__ballot_sync(gmask, offers) & gmask) ? DRA_ST_NO_CAPACITY : DRA_ST_BAD_PROFILE) | (pos << 8);
+                }
+            }
         }
     }
     // ---- the MIG claims: depth-first search in canonical order (GPUs ascending, starts ascending) ----
@@ -2626,6 +2652,7 @@ __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const ui
     unsigned long long st_lo = 0, st_hi = 0;   // its start there, one nibble per position
     if (!status && migmask) {
         uint32_t descents = 0, pos = (uint32_t)__ffs(migmask) - 1u;
+        uint32_t depth = 0, dmax = 0;          // WHY: the levels placed now, the most placed at once (d)
         uint32_t rl = 0xFFFFFFFFu, rs = 0;     // resume point after a backtrack: candidates after (lane rl, start rs)
         while (true) {
             const uint4 c = get(pos);
@@ -2647,6 +2674,7 @@ __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const ui
             if (b) {
                 if (descents == DRA_EXH_BUDGET) { status = DRA_ST_SEARCH_LIMIT; break; }
                 ++descents;
+                if constexpr (WHY) { ++depth; dmax = max(dmax, depth); }
                 if (lane == (uint32_t)__ffs(b) - 1u) {
                     const uint32_t s_ = (uint32_t)__ffs(cand) - 1u;
                     L.busy |= ((1u << size) - 1u) << s_;
@@ -2670,6 +2698,14 @@ __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const ui
                 if (mine) { L.busy &= ~(((1u << size2) - 1u) << s2); chosen &= ~(1u << pos); }
                 rs = __shfl_sync(gmask, s2, wabs);
                 rl = wabs - gbase;
+                if constexpr (WHY) --depth;
+            }
+        }
+        if constexpr (WHY) {
+            if (status) {                                                         // the MIG claim of level dmax (< the levels)
+                uint32_t m = migmask;
+                for (uint32_t i = 0; i < dmax; ++i) m &= m - 1u;
+                why = status | ((uint32_t)(__ffs(m) - 1) << 8);
             }
         }
     }
@@ -2689,6 +2725,7 @@ __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const ui
                 for (uint32_t k = 0; k < slots; ++k) out[c.y + k] = make_uint2(DRA_GPU_NONE, meta(0, 0, op, st));
             }
         }
+        if constexpr (WHY) return why;
         return status;
     }
     if (out) {
@@ -3059,7 +3096,14 @@ struct UnsArgs {
                                 //      in length, so the warps take their pairs from a counter instead of a fixed stride
     uint32_t node_lo, n_win, n_walk;   // the node window (pair_decode; WIN = false: [0, n_node)), the pairs walked
     const uint32_t* gate;      // sharded call only: *gate != 0: the inputs failed their device-side check, evaluate nothing
+    uint8_t* why; uint32_t* why_claim;   // WHY (spec §17): each walked pair's reason and blocking claim, instead of bits
 };
+
+// One pair's record of the reasons kernel (k_unsuitable<..., WHY = true>), by the group's lane 0
+__device__ __forceinline__ void why_put(const UnsArgs& a, uint32_t pair, uint32_t reason, uint32_t claim) {
+    a.why[pair] = (uint8_t)reason;
+    a.why_claim[pair] = reason == DRA_ST_OK ? DRA_WHY_CLAIM_NONE : claim;
+}
 
 struct GlobalGet {
     const uint4* base;
@@ -3111,7 +3155,9 @@ __device__ __forceinline__ LaneGroup lane_group() {
 // group running its own claim loop with group-wide ballots.  Dense form: every pod against every node, no candidate arrays.
 // WIN: the node window and the gate of the sharded call, else the window [0, n_node) (own instantiations: with the window
 // the exhaustive kernel needs 81 registers instead of 78, which costs dra_unsuitable_batch a third of its CTAs per SM).
-template <int WPC, int W, bool EXH, bool WIN>          // EXH: spec §12 (own instantiation: the default kernel stays as lean as it was)
+// WHY (spec §17): the same walk writes every pair's reason and blocking claim (UnsArgs::why) instead of the bits; own
+// instantiations, so the bit kernels stay as they were.
+template <int WPC, int W, bool EXH, bool WIN, bool WHY = false>   // EXH: spec §12 (own instantiation: the default kernel stays as lean as it was)
 __global__ void __launch_bounds__(WPC * 32, 2)
 k_unsuitable(const UnsArgs a) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
@@ -3129,7 +3175,10 @@ k_unsuitable(const UnsArgs a) {
         if (walk >= n_walk) continue;                                    // whole group skips together
         uint32_t pod, node, pair;
         if (!pair_decode(walk, node_lo, n_win, a.n_node, a.cand_off, a.cand_nodes, a.pair_pod, pod, node, pair) ||
-            node - node_lo >= n_win || pod >= a.n_pod) continue;         // another rank's node, or none: unsuitable here
+            node - node_lo >= n_win || pod >= a.n_pod) {                 // another rank's node, or none: unsuitable here
+            if constexpr (WHY) if (gl == 0 && node >= a.n_node) why_put(a, pair, DRA_WHY_NO_NODE, DRA_WHY_CLAIM_NONE);
+            continue;
+        }
         const uint32_t c0 = __ldg(&a.pod_off[pod]);
         const uint32_t cnt = __ldg(&a.pod_off[pod + 1]) - c0;
         const uint32_t g0 = __ldg(&a.node_off[node]);
@@ -3138,18 +3187,70 @@ k_unsuitable(const UnsArgs a) {
         if (gl < ng) rec = __ldg(&a.inv[g0 + gl]);
         Lane L; L.load(rec, gl < ng);
         if (EXH) {                                                        // spec §12
-            if (cnt > DRA_MAX_POD || ng > W) continue;
+            if (cnt > DRA_MAX_POD || ng > W) {
+                if constexpr (WHY) if (gl == 0) why_put(a, pair, DRA_ST_INVALID, DRA_WHY_CLAIM_NONE);
+                continue;
+            }
             const PodGet pget{a.claims + c0, nullptr, 0};
             Lane Lt = L;                                                    // by copy: a reference would pin L in local memory
-            const uint32_t st = pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, pget, cnt, a.sel, true, true, nullptr);
-            if (st == 0 && gl == 0) atomicOr(&a.bits[pair >> 5], 1u << (pair & 31));
+            const uint32_t st = pod_eval<W, WHY>(Lt, lane, gmask, gbase, g0, tbl_s, pget, cnt, a.sel, true, true, nullptr);
+            if constexpr (WHY) { if (gl == 0) why_put(a, pair, st & 0xFFu, c0 + (st >> 8)); }
+            else if (st == 0 && gl == 0) atomicOr(&a.bits[pair >> 5], 1u << (pair & 31));
             continue;
         }
-        Dead D; FlagSink sink; GlobalGet get{a.claims + c0};
-        if (ng > W) sink.failed = true;                                   // cannot happen: W is chosen from the inventory
-        uint32_t k = 0;
-        while (k < cnt && !sink.stop()) k += node_step(L, D, lane, g0, tbl_s, get, k, cnt, sink, true, a.sel, gmask, gbase);
-        if (!sink.failed && gl == 0) atomicOr(&a.bits[pair >> 5], 1u << (pair & 31));
+        Dead D; GlobalGet get{a.claims + c0};
+        if constexpr (WHY) {
+            WhySink sink;
+            if (ng > W) sink.fail(0, 0, 0, DRA_ST_INVALID);                // cannot happen: W is chosen from the inventory
+            uint32_t k = 0, kf = 0;                                         // kf: the step that failed (a run: its first member)
+            while (k < cnt && !sink.stop()) { kf = k; k += node_step(L, D, lane, g0, tbl_s, get, k, cnt, sink, true, a.sel, gmask, gbase); }
+            if (gl == 0) why_put(a, pair, sink.st, c0 + kf);
+        } else {
+            FlagSink sink;
+            if (ng > W) sink.failed = true;                               // cannot happen: W is chosen from the inventory
+            uint32_t k = 0;
+            while (k < cnt && !sink.stop()) k += node_step(L, D, lane, g0, tbl_s, get, k, cnt, sink, true, a.sel, gmask, gbase);
+            if (!sink.failed && gl == 0) atomicOr(&a.bits[pair >> 5], 1u << (pair & 31));
+        }
+    }
+}
+
+// The tallies of spec §17 from the pair records of k_unsuitable<..., WHY = true>: warp per pod over its pairs (pod_pairs);
+// pod_why[p * DRA_WHY_N + r] the pod's pairs of reason r, claim_blocks[c] (zeroed by the caller) the pairs blocked by claim c.
+// Integer sums: the schedule does not change them.  Either output may be nullptr.
+struct WhyTally {
+    const uint8_t* why; const uint32_t* why_claim; const uint32_t* cand_off;   // cand_off nullptr: dense form
+    uint32_t n_pod, n_node;
+    uint32_t* pod_why; uint32_t* claim_blocks;
+};
+
+__global__ void __launch_bounds__(256)
+k_why_tally(const WhyTally t) {
+    const uint32_t lane = threadIdx.x & 31, p = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (p >= t.n_pod) return;
+    unsigned long long k0, k1;
+    pod_pairs(t.cand_off, p, t.n_node, 0u, t.n_node, k0, k1);
+    uint32_t cnt[DRA_WHY_N];
+    #pragma unroll
+    for (uint32_t r = 0; r < DRA_WHY_N; ++r) cnt[r] = 0;
+    for (unsigned long long k0w = k0; k0w < k1; k0w += 32) {             // the whole warp steps together
+        const unsigned long long k = k0w + lane;
+        const bool in = k < k1;
+        const uint32_t r = in ? __ldg(&t.why[k]) : DRA_WHY_N;
+        #pragma unroll
+        for (uint32_t q = 0; q < DRA_WHY_N; ++q) cnt[q] += r == q;
+        if (t.claim_blocks) {
+            // a pod's pairs mostly name the same few claims: one atomic per distinct claim of the warp's 32 pairs
+            const uint32_t c = in ? __ldg(&t.why_claim[k]) : DRA_WHY_CLAIM_NONE;
+            const uint32_t same = __match_any_sync(FULLMASK, c);
+            if (c != DRA_WHY_CLAIM_NONE && lane == (uint32_t)__ffs(same) - 1u) atomicAdd(&t.claim_blocks[c], (uint32_t)__popc(same));
+        }
+    }
+    if (!t.pod_why) return;
+    #pragma unroll
+    for (uint32_t r = 0; r < DRA_WHY_N; ++r) {
+        const uint32_t v = __reduce_add_sync(FULLMASK, cnt[r]);
+        if (lane == 0) t.pod_why[(size_t)p * DRA_WHY_N + r] = v;
     }
 }
 

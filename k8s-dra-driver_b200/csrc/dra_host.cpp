@@ -355,6 +355,97 @@ std::vector<std::map<std::string, uint32_t>> Driver::PodCapacityBatch(const std:
     return res;
 }
 
+// "1 node" / "2 nodes"
+static std::string nodes_text(size_t n) { return std::to_string(n) + (n == 1 ? " node" : " nodes"); }
+
+static const char* why_text(uint8_t r) {
+    switch (r) {
+        case DRA_ST_NO_CAPACITY: return "no capacity";
+        case DRA_ST_BAD_PROFILE: return "no GPU offers the MIG profile";
+        case DRA_ST_GROUP: return "co-located MIG devices do not fit on one parent GPU";
+        case DRA_ST_MEM_LIMIT: return "no shareable GPU with enough free memory";
+        case DRA_ST_INVALID: return "invalid claim";
+        case DRA_ST_POD: return "does not fit together with the pod's other claims";
+        case DRA_ST_SEARCH_LIMIT: return "placement search budget exhausted";
+        default: return "";
+    }
+}
+
+// `claim "uid" (MIG 3g.20gb)`, `claim "uid" (2 GPUs)`, `claim "uid" (shared GPU)`
+static std::string claim_text(const ClaimAllocation& ca) {
+    std::string what;
+    if (ca.IsMig) what = "MIG " + ca.Mig.Profile;
+    else if (ca.Gpu.Sharing.Strategy == SharingStrategy::None) what = std::to_string(ca.Gpu.Count) + (ca.Gpu.Count == 1 ? " GPU" : " GPUs");
+    else what = "shared GPU";
+    return "claim \"" + ca.ClaimUID + "\" (" + what + ")";
+}
+
+std::vector<std::string> Driver::UnsuitableReasonsBatch(const std::vector<PodRequest>& pods) {
+    std::vector<std::string> res(pods.size());
+    Lowered lo;
+    std::vector<uint32_t> podOff(1, 0), candOff(1, 0), cand;
+    std::vector<size_t> podOf;                                  // lowered pod -> index in pods
+    for (size_t pi = 0; pi < pods.size(); ++pi) {
+        const auto& pod = pods[pi];
+        uint32_t model = 0;                                     // profile names: as in UnsuitableNodesBatch
+        for (const auto& nn : pod.PotentialNodes) { const uint32_t n = nodeIndex(nn); if (n != 0xFFFFFFFFu) { model = nodeModel_[n]; break; } }
+        std::map<std::string, uint32_t> groups;
+        bool ok = true;
+        const size_t mark = lo.recs.size();
+        const uint32_t markOut = lo.nOut;
+        for (ClaimAllocation* ca : groupAdjacent(pod.Claims)) {
+            uint32_t g = 0;
+            if (ca->IsMig && !ca->Mig.GpuClaimName.empty()) {
+                auto it = groups.find(ca->Mig.GpuClaimName);
+                g = it == groups.end() ? (groups[ca->Mig.GpuClaimName] = nextGroup_++) : it->second;
+                if (nextGroup_ == 0) nextGroup_ = 1;
+            }
+            ok = lower(*ca, 0, g, lo, model) && ok;
+        }
+        if (!ok) {
+            lo.recs.resize(mark); lo.outOff.resize(mark); lo.owner.resize(mark); lo.nOut = markOut;
+            const size_t n = pod.PotentialNodes.size();
+            for (ClaimAllocation* ca : pod.Claims)
+                if (!ca->Error.empty()) {
+                    res[pi] = "0/" + std::to_string(n) + " nodes are available" + (n ? ": " + nodes_text(n) + ": " + claim_text(*ca) + " " + ca->Error : "") + ".";
+                    break;
+                }
+            continue;
+        }
+        podOff.push_back((uint32_t)lo.recs.size());
+        for (const auto& nn : pod.PotentialNodes) cand.push_back(nodeIndex(nn));
+        candOff.push_back((uint32_t)cand.size());
+        podOf.push_back(pi);
+    }
+    if (podOf.empty()) return res;
+    std::vector<uint8_t> why(cand.size() + 1, 0);
+    std::vector<uint32_t> blk(cand.size() + 1, 0);
+    check(dra_unsuitable_why_batch(ctx_, lo.recs.data(), (uint32_t)lo.recs.size(), podOff.data(), (uint32_t)podOf.size(),
+                                   cand.data(), candOff.data(), why.data(), blk.data(), nullptr, nullptr,
+                                   exhaustive_ ? DRA_F_EXHAUSTIVE : 0u), "dra_unsuitable_why_batch");
+    for (size_t q = 0; q < podOf.size(); ++q) {
+        // the blocking claim is an index into the LOWERED records: lo.owner maps it back (group members were made
+        // adjacent, so it is not the position in pod.Claims)
+        std::vector<std::pair<std::string, size_t>> parts;      // text, nodes; in order of first appearance
+        std::map<std::string, size_t> at;
+        size_t ok = 0;
+        for (uint32_t k = candOff[q]; k < candOff[q + 1]; ++k) {
+            if (why[k] == DRA_ST_OK) { ++ok; continue; }
+            std::string t;
+            if (why[k] == DRA_WHY_NO_NODE) t = "not in the inventory";
+            else if (blk[k] == DRA_WHY_CLAIM_NONE) t = std::string("more than ") + std::to_string(DRA_MAX_POD) + " claims";
+            else t = claim_text(*lo.owner[blk[k]]) + " " + why_text(why[k]);
+            auto it = at.find(t);
+            if (it == at.end()) { at[t] = parts.size(); parts.push_back({t, 1}); } else ++parts[it->second].second;
+        }
+        std::stable_sort(parts.begin(), parts.end(), [](const auto& a, const auto& b) { return a.second > b.second; });
+        std::string m = std::to_string(ok) + "/" + std::to_string(candOff[q + 1] - candOff[q]) + " nodes are available";
+        for (size_t i = 0; i < parts.size(); ++i) m += (i ? "; " : ": ") + nodes_text(parts[i].second) + ": " + parts[i].first;
+        res[podOf[q]] = m + ".";
+    }
+    return res;
+}
+
 void Driver::UnsuitableNodes(const std::vector<ClaimAllocation*>& claims, const std::vector<std::string>& potentialNodes) {
     PodRequest p; p.Claims = claims; p.PotentialNodes = potentialNodes;
     UnsuitableNodesBatch({p});
