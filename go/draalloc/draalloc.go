@@ -864,6 +864,35 @@ func (c *Context) PodCapacityBatchGlobalDevice(pinnedClaims unsafe.Pointer, nCla
 	return nil
 }
 
+// SetShardWhy reserves room for the sharded reasons call's pair records: before ShardExport, the same on every context.
+// Unbuilt, like the rest of this file.
+func (c *Context) SetShardWhy(maxPairs uint32) error {
+	if rc := C.dra_set_shard_why(c.h, C.uint32_t(maxPairs)); rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
+// UnsuitableWhyBatchGlobalDevice: why each node is unsuitable (spec §17) on a sharded world
+// (dra_unsuitable_why_batch_global_device).  The same pods, candidates (pinnedCandNodes == pinnedCandOff == nil: dense
+// form, nPair = nPod * nNode) and flags on every context, every array in dra_host_alloc'ed (pinned) memory; each context
+// judges the pairs of its own nodes, and every context ends with the whole outputs (all but pinnedPairWhy may be nil).
+// Returns at once; Sync reports completion and errors found on the device.  Unbuilt, like the rest of this file.
+func (c *Context) UnsuitableWhyBatchGlobalDevice(pinnedClaims unsafe.Pointer, nClaim int, pinnedPodOff unsafe.Pointer, nPod int,
+	pinnedCandNodes, pinnedCandOff unsafe.Pointer, nPair int,
+	pinnedPairWhy, pinnedPairClaim, pinnedPodWhy, pinnedClaimBlocks unsafe.Pointer, flags uint32) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_unsuitable_why_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
+		(*C.uint32_t)(pinnedPodOff), C.uint32_t(nPod), (*C.uint32_t)(pinnedCandNodes), (*C.uint32_t)(pinnedCandOff),
+		C.uint32_t(nPair), (*C.uint8_t)(pinnedPairWhy), (*C.uint32_t)(pinnedPairClaim), (*C.uint32_t)(pinnedPodWhy),
+		(*C.uint32_t)(pinnedClaimBlocks), C.uint32_t(flags))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
 // SetShardPreemptPlace reserves room for the sharded preempt-and-place call (pending pods, judged pairs, running pods):
 // after SetInventory, before ShardExport, the same on every context.  Unbuilt, like the rest of this file.
 func (c *Context) SetShardPreemptPlace(maxPods, maxPairs, maxRun uint32) error {

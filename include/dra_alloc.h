@@ -272,7 +272,8 @@ int  dra_unsuitable_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
  * DRA_E_INVAL with nothing written: unknown flags, pod_off / cand_off not monotone or not spanning, dense
  * n_pod * n_node >= 2^32, pair_why NULL with pairs to answer.  n_pod == 0 returns DRA_OK after those checks.  On a
  * sharded world the call is exact on any rank after dra_shard_sync_inventory_device, which makes that rank's live copy the
- * world's state. */
+ * world's state; dra_unsuitable_why_batch_global_device answers across the ranks without the sync, each rank judging the
+ * pairs of its own nodes. */
 int  dra_unsuitable_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
                               const uint32_t* pod_off, uint32_t n_pod,
                               const uint32_t* cand_nodes, const uint32_t* cand_off,
@@ -480,7 +481,7 @@ int  dra_gather_read(dra_ctx* ctx, dra_out_rec* out_all, uint32_t n_rec);
  *                                              cudaIpcMemHandle_t;  the host runtime all-gathers the handles;
  *   dra_peer_import(ctx, handles)              world * 64 bytes, in rank order.
  * Requires all ranks on one node with P2P access; on failure the NCCL path stays in use.  Every rank must export alike (the
- * same sizes, dra_set_shard_pairs, dra_set_shard_place, dra_set_shard_preempt, dra_set_shard_capacity, dra_set_shard_preempt_place and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
+ * same sizes, dra_set_shard_pairs, dra_set_shard_place, dra_set_shard_preempt, dra_set_shard_capacity, dra_set_shard_preempt_place, dra_set_shard_why and, for dra_shard_export, inventory size): each rank addresses its peers' buffers by its
  * own layout, so dra_peer_import / dra_peer_import_local refuse a peer set up differently with DRA_E_INVAL.
  * dra_peer_export(ctx, 0, NULL) switches the peer path off again. */
 int  dra_peer_export(dra_ctx* ctx, uint32_t n_per_rank, void* handle64);
@@ -667,6 +668,39 @@ int  dra_pod_capacity_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_c
                                           uint16_t* d_pair_copies, uint8_t* d_pair_stop,
                                           uint64_t* d_pod_total, uint32_t* d_pod_nodes, uint32_t flags);
 
+/* Room for the sharded reasons call in the buffer dra_shard_export maps: each rank's slice holds a 16-byte header, then
+ * a u8 reason per pair padded to 16 bytes, then a u32 blocking claim per pair, so 16 * (1 + ceil(max_pairs / 16) +
+ * ceil(max_pairs / 4)) bytes, one slice per rank and call parity: world * 2 slices per rank (about 102 MB for 1.28 M pairs
+ * at world 8).  World > 1: call before dra_shard_export (afterwards: DRA_E_STATE), every rank with the same max_pairs; the
+ * peer import refuses a peer set up differently.  A max_pairs whose slice would exceed 4 GiB: DRA_E_INVAL.  The export also
+ * sizes the call's scratch for max_pairs (one slice and 4 bytes a pair), so that no call frees a buffer while a peer
+ * waits for it.  World 1 needs no call. */
+int  dra_set_shard_why(dra_ctx* ctx, uint32_t max_pairs);
+/* Why each node is unsuitable over a sharded world (spec §17, "Sharded form"): dra_unsuitable_why_batch answered on the
+ * world's state.  The SAME claims, pod_off, candidates (cand_nodes == cand_off == NULL: the dense form, n_pair = n_pod *
+ * n_node) and flags on every rank (device pointers, or dra_host_alloc'ed buffers).  A pair is judged by the rank whose node
+ * range holds its candidate node, against that rank's live inventory; a candidate naming no node of the inventory is
+ * DRA_WHY_NO_NODE with DRA_WHY_CLAIM_NONE.  Every rank ends with the WHOLE outputs, laid out as dra_unsuitable_why_batch's,
+ * byte for byte what that call answers on ONE inventory made of every rank's own nodes: pod_why and claim_blocks are taken
+ * over the merged pairs.  d_pair_claim, d_pod_why and d_claim_blocks may be NULL.  So d_pair_why[k] == DRA_ST_OK exactly
+ * where dra_unsuitable_batch_global_device sets bit k with the same flags, and with DRA_F_EXHAUSTIVE exactly where
+ * dra_pod_capacity_batch_global_device counts at least one copy.  Nothing is written to any inventory, live or pristine.
+ * Needs dra_set_shard (else DRA_E_STATE); world > 1 needs dra_set_shard_map spanning the inventory (a bare dra_set_shard:
+ * DRA_E_STATE), dra_shard_export after dra_set_shard_why with max_pairs > 0 (even for a call with no pairs), and
+ * dra_peer_import / dra_peer_import_local (else DRA_E_STATE).  World 1 needs no export, judges every node, and answers
+ * byte for byte as dra_unsuitable_why_batch.  Host-side argument errors (DRA_E_INVAL) return before anything is enqueued:
+ * unknown flags, one candidate array without the other, a dense n_pair other than n_pod * n_node, n_pair above 2^32 - 16
+ * or (world > 1) above max_pairs, n_pod above 2^26, NULL d_pair_why with pairs to answer.  Enqueues on ctx's stream and
+ * returns; n_pod == 0 enqueues nothing.  Completion and device-detected errors surface at dra_ctx_sync: pod_off / cand_off
+ * not monotone or not spanning their arrays give DRA_E_INVAL on EVERY rank with none of the outputs written, d_claim_blocks
+ * included; a peer that does not arrive within DRA_PEER_TIMEOUT_MS gives DRA_E_NCCL, and d_claim_blocks is not written.
+ * flags: 0 or DRA_F_EXHAUSTIVE. */
+int  dra_unsuitable_why_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                           const uint32_t* d_pod_off, uint32_t n_pod,
+                                           const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                           uint8_t* d_pair_why, uint32_t* d_pair_claim,
+                                           uint32_t* d_pod_why, uint32_t* d_claim_blocks, uint32_t flags);
+
 /* Every rank's live inventory becomes the world's state: for each GPU, the record its owning rank holds (the rank whose
  * node range contains the GPU's node, per the current dra_set_shard_map).  Own range untouched, pristine copy untouched.
  * Afterwards dra_get_inventory on any rank returns the whole world, and dra_set_shard_map may move node ranges between
@@ -803,6 +837,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_POD_CAPACITY     0x8000000u /* pod capacity: the pairs' copy counts, the per-pod sums */
 #define DRA_K_POD_CAPACITY_SHARD 0x10000000u /* sharded pod capacity: prep, the window's pairs, exchange, merge with the sums */
 #define DRA_K_UNSUITABLE_WHY   0x20000000u /* reasons of UnsuitableNodes: the pair records, the tallies */
+#define DRA_K_UNSUITABLE_WHY_SHARD 0x40000000u /* sharded reasons: prep, the window's pair records, exchange, merge with the tallies */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

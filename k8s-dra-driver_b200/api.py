@@ -27,7 +27,7 @@ KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x0
            "compact_lookback": 0x20000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000,
            "place_shard": 0x400000, "preempt": 0x800000, "preempt_shard": 0x1000000,
            "preempt_place": 0x2000000, "preempt_place_shard": 0x4000000, "pod_capacity": 0x8000000,
-           "pod_capacity_shard": 0x10000000, "unsuitable_why": 0x20000000}
+           "pod_capacity_shard": 0x10000000, "unsuitable_why": 0x20000000, "unsuitable_why_shard": 0x40000000}
 # spec §17: the reasons of dra_unsuitable_why_batch are DRA_ST_OK .. DRA_ST_SEARCH_LIMIT (0 .. 7) and WHY_NO_NODE
 WHY_NO_NODE, WHY_N, WHY_CLAIM_NONE = 8, 9, 0xFFFFFFFF
 
@@ -110,6 +110,8 @@ SYMBOLS = {
     "dra_set_shard_capacity": (_i32, [_vp, _u32]),
     "dra_pod_capacity_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp,
                                                     _u32]),
+    "dra_set_shard_why": (_i32, [_vp, _u32]),
+    "dra_unsuitable_why_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _u32]),
     "dra_shard_sync_inventory_device": (_i32, [_vp]),
     "dra_deallocate_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_mps_limits_batch": (_i32, [_vp, _vp, _u32, _vp, _vp]),
@@ -674,6 +676,23 @@ class Context:
         self._check(self._lib.dra_pod_capacity_batch_global_device(
             self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod, _ptr(d_cand_nodes), _ptr(d_cand_off), n_pair,
             max_copies, _ptr(d_pair_copies), _ptr(d_pair_stop), _ptr(d_pod_total), _ptr(d_pod_nodes), flags))
+
+    def set_shard_why(self, max_pairs: int) -> None:
+        """Room for the sharded reasons call's pair records; world > 1: before shard_export, the same on every rank."""
+        self._check(self._lib.dra_set_shard_why(self._h, max_pairs))
+
+    def unsuitable_why_global_device(self, d_claims: int, n_claim: int, d_pod_off: int, n_pod: int, d_cand_nodes: int | None,
+                                     d_cand_off: int | None, n_pair: int, d_pair_why: int | None,
+                                     d_pair_claim: int | None = None, d_pod_why: int | None = None,
+                                     d_claim_blocks: int | None = None, flags: int = 0) -> None:
+        """Sharded reasons of UnsuitableNodes (spec §17): the SAME pods and candidates on every rank (device pointers);
+        d_cand_nodes / d_cand_off None = dense form (n_pair = n_pod * n_node).  Each rank judges the pairs of its own nodes;
+        every rank receives the whole outputs, laid out as unsuitable_why()'s (u8 reasons, u32 blocking claims, u32
+        [n_pod, WHY_N] per-pod counts, u32 per-claim counts); all but d_pair_why may be None.  Enqueues, no
+        synchronisation; errors found on the device surface at sync()."""
+        self._check(self._lib.dra_unsuitable_why_batch_global_device(
+            self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod, _ptr(d_cand_nodes), _ptr(d_cand_off), n_pair,
+            _ptr(d_pair_why), _ptr(d_pair_claim), _ptr(d_pod_why), _ptr(d_claim_blocks), flags))
 
     def set_shard_preempt_place(self, max_pods: int, max_pairs: int, max_run: int) -> None:
         """Room for the sharded preempt-and-place call (pending pods, judged pairs, running pods); world > 1: before

@@ -78,6 +78,7 @@ struct ShardSizes {
     uint32_t pre_pods, pre_pairs, pre_victims;      // dra_set_shard_preempt
     uint32_t scap_pairs;                            // dra_set_shard_capacity
     uint32_t spp_pods, spp_pairs, spp_run;          // dra_set_shard_preempt_place
+    uint32_t swhy_pairs;                            // dra_set_shard_why
 };
 
 struct dra_ctx {
@@ -230,6 +231,10 @@ struct dra_ctx {
     // sharded pod capacity: a region [slices x2: world slices][flags] (dra_device.cuh CapMerge) in the peer buffer
     PeerRegion scap_x;
     uint4* d_scap_part = nullptr; size_t cap_scap_part = 0;           // this rank's slice (uint4 units)
+    // sharded reasons of UnsuitableNodes: a region [slices x2: world slices][flags] (dra_device.cuh WhyMerge) in the peer buffer
+    PeerRegion swhy_x;
+    uint4* d_swhy_part = nullptr; size_t cap_swhy_part = 0;           // this rank's slice (uint4 units)
+    uint32_t* d_swhy_blocks = nullptr; size_t cap_swhy_blocks = 0;    // the merge's per-claim counts and blocks-done counter
     int splace_occ = -1;                        // resident CTAs of k_pods_place<4, true> per SM (occupancy query, once)
     int peers_on_device = 1;                    // ranks whose contexts share this device (dra_peer_import_local)
     // inventory sync: records in the peer buffer ([staging x2: peer_inv_gpus records][flags[PEER_MAX], elect[2]])
@@ -662,13 +667,14 @@ uint32_t pair_grid(const dra_ctx* ctx, uint32_t n) {
 }
 
 // k_unsuitable over a.n_walk pairs (win: the sharded call's node window and gate; else the whole inventory; why: the
-// reasons of spec §17 into a.why / a.why_claim instead of the bits, on the whole inventory).  Enqueues only.
+// reasons of spec §17 into a.why / a.why_claim instead of the bits, at the walk index).  Enqueues only.
 int launch_unsuitable(dra_ctx* ctx, UnsArgs& a, bool win, bool why = false) {
     const uint32_t grid = pair_grid(ctx, a.n_walk);
     if (a.exhaustive) { if (int rc = walk_counter(ctx, TK_WALK_UNSUITABLE, a.work)) return rc; }
     at_pair_width(ctx, [&](auto w) {
         constexpr int W = decltype(w)::value;
-        const auto k = why ? (a.exhaustive ? k_unsuitable<8, W, true, false, true> : k_unsuitable<8, W, false, false, true>)
+        const auto k = why ? (win ? (a.exhaustive ? k_unsuitable<8, W, true, true, true> : k_unsuitable<8, W, false, true, true>)
+                                  : (a.exhaustive ? k_unsuitable<8, W, true, false, true> : k_unsuitable<8, W, false, false, true>))
                      : win ? (a.exhaustive ? k_unsuitable<8, W, true, true> : k_unsuitable<8, W, false, true>)
                            : (a.exhaustive ? k_unsuitable<8, W, true, false> : k_unsuitable<8, W, false, false>);
         k<<<grid, 256, 0, ctx->stream>>>(a);
@@ -719,6 +725,9 @@ int check_err(dra_ctx* ctx) {
                                       "candidates for a pod, a pending slot outside n_out, or running pods: pod_off not monotone or not "
                                       "spanning the claims, a slot range outside n_out, or OK slots naming a GPU index >= n_gpu or GPUs of "
                                       "two nodes; nothing was written", PL_POS);
+    if (bo && (ctx->chain & DRA_K_UNSUITABLE_WHY_SHARD))
+        return fail(ctx, DRA_E_INVAL, "sharded unsuitable reasons: pod_off / cand_off not monotone or not spanning their arrays (on this "
+                                      "rank or a peer); nothing was written");
     if (bo) return fail(ctx, DRA_E_INVAL, "sharded UnsuitableNodes: pod_off / cand_off not monotone or not spanning their arrays; nothing was evaluated");
     if (bp && (ctx->chain & DRA_K_PLACE_SHARD))
         return fail(ctx, DRA_E_INVAL, "sharded place pods: pod_off / cand_off not monotone or not spanning their arrays, more than %u candidates for a pod, "
@@ -1328,7 +1337,7 @@ void dra_ctx_destroy(dra_ctx* c) {
                    c->d_pre_pairviol, c->d_pre_rpdb, c->d_pre_vprev, c->d_pre_allowed,
                    c->d_pp_pending, c->d_pp_evicted, c->d_pp_runoff, c->d_pp_judged, c->d_spp_inv, c->d_spp_gate,
                    c->d_cap_copies, c->d_cap_stop, c->d_cap_total, c->d_cap_nodes, c->d_scap_part,
-                   c->d_why, c->d_why_claim, c->d_why_pod, c->d_why_blocks};
+                   c->d_why, c->d_why_claim, c->d_why_pod, c->d_why_blocks, c->d_swhy_part, c->d_swhy_blocks};
     for (void* p : dev) if (p) cudaFree(p);
     for (void* p : c->retired) cudaFree(p);
     if (c->h_err) cudaFreeHost((void*)c->h_err);
@@ -2148,6 +2157,10 @@ int preload(dra_ctx* ctx, Kernels ks, Kernels waiting, bool sorts) {
 // n u8 stops, each padded to 16 bytes
 size_t scap_units(uint32_t n) { return 1 + ((size_t)n + 7) / 8 + ((size_t)n + 15) / 16; }
 
+// uint4 units of one rank's slice of the sharded reasons for n walked pairs (dra_device.cuh WhyMerge): the header, n u8
+// reasons padded to 16 bytes, then (claims) n u32 blocking claims
+size_t swhy_units(uint32_t n, bool claims = true) { return 1 + ((size_t)n + 15) / 16 + (claims ? ((size_t)n + 3) / 4 : 0); }
+
 // The sharded preempt-and-place chain's kernels (preload), and the walk's occupancy query (which loads it too).  Its one
 // wait is the inventory exchange (k_isync_copy), before the walk, and it keeps its split.
 int preload_preempt_place_shard(dra_ctx* ctx) {
@@ -2197,6 +2210,7 @@ int spre_buffers(dra_ctx* ctx, uint32_t n_pod, uint32_t n_pair, uint32_t max_vic
 // and, after dra_set_shard_place(max_pods > 0), [place pods: progress counter, 64 bytes][max_pods state words of 8 bytes]
 // and, after dra_set_shard_preempt(max_pods > 0), [preemption partials x2: world slices of spre_units][their flags]
 // and, after dra_set_shard_capacity(max_pairs > 0), [pod-capacity slices x2: world slices of scap_units][their flags]
+// and, after dra_set_shard_why(max_pairs > 0), [reasons slices x2: world slices of swhy_units][their flags]
 int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, uint32_t cap) {
     if (ctx->world > (int)PEER_MAX) return fail(ctx, DRA_E_INVAL, "world %d > %u", ctx->world, PEER_MAX);
     CU(cudaSetDevice(ctx->device));
@@ -2274,6 +2288,21 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
             return rc;
         if (int rc = grow(ctx, ctx->d_scap_part, ctx->cap_scap_part, scap_units(z.scap_pairs))) return rc;
         if (int rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, z.scap_pairs)) return rc;
+    }
+    // sharded reasons, after dra_set_shard_why: the slices' exchange (room for the claims: whether a call sends them is its
+    // own choice), and the call's slice and pair -> pod at full size now (no cudaFree inside a call while a peer's merge
+    // waits for this rank)
+    if (z.swhy_pairs) {
+        const size_t slice = swhy_units(z.swhy_pairs) * 16;
+        reserve(ctx->swhy_x, (size_t)ctx->world * slice, slice, (size_t)PEER_MAX * 4);
+        if (int rc = preload(ctx, {(const void*)k_uns_prep, (const void*)k_unsuitable<8, 8, false, true, true>,
+                                   (const void*)k_unsuitable<8, 16, false, true, true>, (const void*)k_unsuitable<8, 32, false, true, true>,
+                                   (const void*)k_unsuitable<8, 8, true, true, true>, (const void*)k_unsuitable<8, 16, true, true, true>,
+                                   (const void*)k_unsuitable<8, 32, true, true, true>, (const void*)k_peer_push},
+                             {(const void*)k_swhy_merge}, false))
+            return rc;
+        if (int rc = grow(ctx, ctx->d_swhy_part, ctx->cap_swhy_part, swhy_units(z.swhy_pairs))) return rc;
+        if (int rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, z.swhy_pairs)) return rc;
     }
     // sharded preempt and place, after dra_set_shard_preempt_place: its kernels loaded and its buffers at full size now (no
     // module load and no cudaFree inside a call while a peer's exchange waits for this rank)
@@ -3102,6 +3131,94 @@ int dra_pod_capacity_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_cl
     ctx->launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded pod capacity launch: %s", cudaGetErrorString(e));
+    return DRA_OK;
+}
+
+int dra_set_shard_why(dra_ctx* ctx, uint32_t max_pairs) {
+    if (!ctx) return DRA_E_INVAL;
+    if (int rc = check_before_export(ctx, "dra_set_shard_why")) return rc;
+    if (max_pairs > 0xFFFFFFF0u) return fail(ctx, DRA_E_INVAL, "dra_set_shard_why: max_pairs %u above 2^32 - 16", max_pairs);
+    if (swhy_units(max_pairs) > ((size_t)1 << 32) / 16)
+        return fail(ctx, DRA_E_INVAL, "dra_set_shard_why: one rank's slice would exceed 4 GiB");
+    ctx->shard_req.swhy_pairs = max_pairs;
+    return DRA_OK;
+}
+
+// Sharded reasons of UnsuitableNodes: offset checks and pair -> pod (k_uns_prep) -> the window's reasons into this rank's
+// slice (k_unsuitable<..., WIN, WHY>) -> push to every peer -> wait + merge into the caller's buffers, with the tallies
+// (k_swhy_merge).  Enqueues only.
+int dra_unsuitable_why_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                           const uint32_t* d_pod_off, uint32_t n_pod,
+                                           const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                           uint8_t* d_pair_why, uint32_t* d_pair_claim,
+                                           uint32_t* d_pod_why, uint32_t* d_claim_blocks, uint32_t flags) {
+    if (!ctx || !d_pod_off || (n_claim && !d_claims)) return DRA_E_INVAL;
+    QUIESCE();
+    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_unsuitable_why_batch_global_device: unknown flags 0x%x", flags);
+    if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
+    if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
+    bool dense;
+    if (int rc = check_dev_cands(ctx, d_cand_nodes, d_cand_off, n_pod, n_pair, true, dense)) return rc;
+    if (n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "n_pod %u too large for the sharded call (2^26)", n_pod);
+    const bool gather = ctx->world > 1;
+    const uint32_t max_pairs = ctx->shard_rsv.swhy_pairs;
+    // no exchange reserved: even a call with no pairs pushes a header and raises flags, which would land in the peers'
+    // buffers at offset 0
+    if (int rc = check_world(ctx, "the merge needs", true, [&] {
+            if (max_pairs) return (int)DRA_OK;
+            return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_why(max_pairs > 0) was not called before dra_shard_export");
+        }, -1, [&] {
+            if (n_pair <= max_pairs) return (int)DRA_OK;
+            return fail(ctx, DRA_E_INVAL, "n_pair %u exceeds the max_pairs (%u) of dra_set_shard_why before dra_shard_export", n_pair, max_pairs);
+        }))
+        return rc;
+    if (n_pair && !d_pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+    ctx->chain = DRA_K_UNSUITABLE_WHY_SHARD; ctx->chain_tile = 0;
+    if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
+    CallScope scope{ctx};
+    int rc = scope.open(gather);
+    if (rc) return rc;
+    // world > 1: peer_setup sized both for max_pairs, so these never reallocate there.  The per-claim counts depend on
+    // n_claim, which no setter bounds: a larger batch grows them here, the old buffer retired until the next dra_ctx_sync.
+    if ((rc = grow(ctx, ctx->d_swhy_part, ctx->cap_swhy_part, swhy_units(n_pair)))) return rc;
+    if (!dense && (rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, n_pair))) return rc;
+    if (d_claim_blocks && (rc = grow(ctx, ctx->d_swhy_blocks, ctx->cap_swhy_blocks, (size_t)n_claim + 1))) return rc;
+    cudaStream_t st = ctx->stream;
+    const uint32_t lo = gather ? ctx->shard_lo : 0u, hi = gather ? ctx->shard_hi : ctx->n_node;   // world 1: every node
+    const uint32_t* gate = ctx->d_err + ERR_BAD_OFFSETS;
+    if (d_claim_blocks) CU(cudaMemsetAsync(ctx->d_swhy_blocks, 0, ((size_t)n_claim + 1) * 4, st));
+    UnsArgs a; memset(&a, 0, sizeof a);
+    a.claims = (const uint4*)d_claims; a.pod_off = d_pod_off; a.n_pod = n_pod;
+    a.cand_nodes = dense ? nullptr : d_cand_nodes; a.cand_off = dense ? nullptr : d_cand_off;
+    a.pair_pod = dense ? nullptr : ctx->d_upair_pod;
+    a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.tbl = ctx->d_tbl; a.sel = sel_of(ctx);
+    a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
+    a.node_lo = lo; a.n_win = hi - lo; a.n_walk = dense ? n_pod * a.n_win : n_pair;   // (n_pod * n_win <= n_pair)
+    a.gate = gate;
+    uint4* part = ctx->d_swhy_part;
+    const bool claims = d_pair_claim || d_claim_blocks;
+    a.why = reinterpret_cast<uint8_t*>(part + 1);
+    a.why_claim = reinterpret_cast<uint32_t*>(part + 1 + ((size_t)a.n_walk + 15) / 16);   // (written whether sent or not)
+    Prof prof(ctx);
+    launch_uns_prep(ctx, d_pod_off, d_cand_off, n_pod, n_claim, n_pair);
+    if (a.n_walk && (rc = launch_unsuitable(ctx, a, true, true))) return rc;
+    prof.mark();
+    WhyMerge m; memset(&m, 0, sizeof m);
+    m.part = part; m.cand_nodes = a.cand_nodes; m.cand_off = a.cand_off;
+    m.n_pod = n_pod; m.n_pair = n_pair; m.n_node = ctx->n_node; m.n_claim = n_claim;
+    merge_bounds(ctx, gather, m.bounds);
+    m.gate = gate;
+    m.pair_why = d_pair_why; m.pair_claim = d_pair_claim; m.pod_why = d_pod_why; m.claim_blocks = d_claim_blocks;
+    m.blocks = ctx->d_swhy_blocks;
+    if (gather) {
+        m.slice4 = (uint32_t)(ctx->swhy_x.slice / 16);
+        CU(cudaMemcpyAsync(part, gate, 4, cudaMemcpyDeviceToDevice, st));   // the header: this rank's fault word
+    }
+    const PeerExchange x = push_slice(ctx, ctx->swhy_x, gather, part, (uint32_t)swhy_units(a.n_walk, claims));
+    k_swhy_merge<<<wait_grid(ctx, (n_pod + 7) / 8), 256, 0, st>>>(x, m);
+    ctx->launches += 1;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded unsuitable reasons launch: %s", cudaGetErrorString(e));
     return DRA_OK;
 }
 

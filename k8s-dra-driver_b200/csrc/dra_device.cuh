@@ -2587,7 +2587,9 @@ struct PodGet {            // claim m of the pod, .y = its first OutRec slot
 // WHY (spec §17): a failure returns instead its reason | blocking position << 8 — INVALID at the lowest invalid claim;
 // NO_CAPACITY / MEM_LIMIT at the first GPU / SHARED claim that fails; BAD_PROFILE / NO_CAPACITY at the first MIG claim
 // the pre-check rejects; POD / SEARCH_LIMIT at the MIG claim of level d, the most levels the search held at once.
-template <int W, bool WHY = false>
+// OWN: a copy of its own for a caller (the sharded reasons walk), so that the callers of the shared copy keep their code:
+// ptxas allocates a __noinline__ function's registers over all of its callers.
+template <int W, bool WHY = false, bool OWN = false>
 __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const uint32_t gmask, const uint32_t gbase,
                                           const uint32_t g0, const uint32_t* __restrict__ tbl_s, const PodGet get,
                                           const uint32_t cnt, const SelCtx sc, const bool exhaustive, const bool have_off,
@@ -3156,7 +3158,9 @@ __device__ __forceinline__ LaneGroup lane_group() {
 // WIN: the node window and the gate of the sharded call, else the window [0, n_node) (own instantiations: with the window
 // the exhaustive kernel needs 81 registers instead of 78, which costs dra_unsuitable_batch a third of its CTAs per SM).
 // WHY (spec §17): the same walk writes every pair's reason and blocking claim (UnsArgs::why) instead of the bits; own
-// instantiations, so the bit kernels stay as they were.
+// instantiations, so the bit kernels stay as they were.  WIN and WHY (the sharded reasons): the records go to the walk
+// index (with the window [0, n_node) that is the pair index), and a pair off the window, a stray included, writes
+// nothing: the merge answers it.
 template <int WPC, int W, bool EXH, bool WIN, bool WHY = false>   // EXH: spec §12 (own instantiation: the default kernel stays as lean as it was)
 __global__ void __launch_bounds__(WPC * 32, 2)
 k_unsuitable(const UnsArgs a) {
@@ -3176,9 +3180,10 @@ k_unsuitable(const UnsArgs a) {
         uint32_t pod, node, pair;
         if (!pair_decode(walk, node_lo, n_win, a.n_node, a.cand_off, a.cand_nodes, a.pair_pod, pod, node, pair) ||
             node - node_lo >= n_win || pod >= a.n_pod) {                 // another rank's node, or none: unsuitable here
-            if constexpr (WHY) if (gl == 0 && node >= a.n_node) why_put(a, pair, DRA_WHY_NO_NODE, DRA_WHY_CLAIM_NONE);
+            if constexpr (WHY && !WIN) if (gl == 0 && node >= a.n_node) why_put(a, pair, DRA_WHY_NO_NODE, DRA_WHY_CLAIM_NONE);
             continue;
         }
+        if constexpr (WIN && WHY) pair = walk;                          // the record's index in this rank's slice
         const uint32_t c0 = __ldg(&a.pod_off[pod]);
         const uint32_t cnt = __ldg(&a.pod_off[pod + 1]) - c0;
         const uint32_t g0 = __ldg(&a.node_off[node]);
@@ -3193,7 +3198,7 @@ k_unsuitable(const UnsArgs a) {
             }
             const PodGet pget{a.claims + c0, nullptr, 0};
             Lane Lt = L;                                                    // by copy: a reference would pin L in local memory
-            const uint32_t st = pod_eval<W, WHY>(Lt, lane, gmask, gbase, g0, tbl_s, pget, cnt, a.sel, true, true, nullptr);
+            const uint32_t st = pod_eval<W, WHY, WIN && WHY>(Lt, lane, gmask, gbase, g0, tbl_s, pget, cnt, a.sel, true, true, nullptr);
             if constexpr (WHY) { if (gl == 0) why_put(a, pair, st & 0xFFu, c0 + (st >> 8)); }
             else if (st == 0 && gl == 0) atomicOr(&a.bits[pair >> 5], 1u << (pair & 31));
             continue;
@@ -3224,34 +3229,44 @@ struct WhyTally {
     uint32_t* pod_why; uint32_t* claim_blocks;
 };
 
-__global__ void __launch_bounds__(256)
-k_why_tally(const WhyTally t) {
-    const uint32_t lane = threadIdx.x & 31, p = blockIdx.x * 8 + (threadIdx.x >> 5);
-    if (p >= t.n_pod) return;
-    unsigned long long k0, k1;
-    pod_pairs(t.cand_off, p, t.n_node, 0u, t.n_node, k0, k1);
+// A warp's tallies over pod p's pairs [k0, k1), the lanes striding them: reason(k) gives pair k's reason, claim(k) its
+// blocking claim (called only when claim_blocks is non-null).  pod_why gets the pod's row (plain stores), claim_blocks
+// one atomic per distinct claim of the warp's 32 pairs; either may be nullptr.  Shared by k_why_tally and k_swhy_merge.
+template <class FR, class FC>
+__device__ __forceinline__ void why_pod_sums(uint32_t p, uint32_t lane, unsigned long long k0, unsigned long long k1, FR reason,
+                                             FC claim, uint32_t* pod_why, uint32_t* claim_blocks) {
     uint32_t cnt[DRA_WHY_N];
     #pragma unroll
     for (uint32_t r = 0; r < DRA_WHY_N; ++r) cnt[r] = 0;
     for (unsigned long long k0w = k0; k0w < k1; k0w += 32) {             // the whole warp steps together
         const unsigned long long k = k0w + lane;
         const bool in = k < k1;
-        const uint32_t r = in ? __ldg(&t.why[k]) : DRA_WHY_N;
+        const uint32_t r = in ? reason(k) : DRA_WHY_N;
         #pragma unroll
         for (uint32_t q = 0; q < DRA_WHY_N; ++q) cnt[q] += r == q;
-        if (t.claim_blocks) {
+        if (claim_blocks) {
             // a pod's pairs mostly name the same few claims: one atomic per distinct claim of the warp's 32 pairs
-            const uint32_t c = in ? __ldg(&t.why_claim[k]) : DRA_WHY_CLAIM_NONE;
+            const uint32_t c = in ? claim(k) : DRA_WHY_CLAIM_NONE;
             const uint32_t same = __match_any_sync(FULLMASK, c);
-            if (c != DRA_WHY_CLAIM_NONE && lane == (uint32_t)__ffs(same) - 1u) atomicAdd(&t.claim_blocks[c], (uint32_t)__popc(same));
+            if (c != DRA_WHY_CLAIM_NONE && lane == (uint32_t)__ffs(same) - 1u) atomicAdd(&claim_blocks[c], (uint32_t)__popc(same));
         }
     }
-    if (!t.pod_why) return;
+    if (!pod_why) return;
     #pragma unroll
     for (uint32_t r = 0; r < DRA_WHY_N; ++r) {
         const uint32_t v = __reduce_add_sync(FULLMASK, cnt[r]);
-        if (lane == 0) t.pod_why[(size_t)p * DRA_WHY_N + r] = v;
+        if (lane == 0) pod_why[(size_t)p * DRA_WHY_N + r] = v;
     }
+}
+
+__global__ void __launch_bounds__(256)
+k_why_tally(const WhyTally t) {
+    const uint32_t lane = threadIdx.x & 31, p = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (p >= t.n_pod) return;
+    unsigned long long k0, k1;
+    pod_pairs(t.cand_off, p, t.n_node, 0u, t.n_node, k0, k1);
+    why_pod_sums(p, lane, k0, k1, [&](unsigned long long k) { return (uint32_t)__ldg(&t.why[k]); },
+                 [&](unsigned long long k) { return __ldg(&t.why_claim[k]); }, t.pod_why, t.claim_blocks);
 }
 
 // ---- sharded UnsuitableNodes (dra_unsuitable_batch_global_device) ----------------------------------------------------
@@ -4774,6 +4789,73 @@ k_scap_merge(const PeerExchange x, const CapMerge m) {
             return copies;
         }, m.pod_total, m.pod_nodes);
     }
+}
+
+// ---- sharded reasons of UnsuitableNodes (dra_unsuitable_why_batch_global_device) ------------------------------------
+// Every rank gets the same pods and candidates.  k_uns_prep checks pod_off / cand_off and writes pair -> pod; its fault
+// word gates k_unsuitable<..., WIN, WHY>, which answers this rank's window into its slice; k_peer_push sends the slice to
+// every peer; k_swhy_merge waits and writes the caller's buffers.  A rank's slice, in uint4 units, for its nw walked pairs
+// (dense n_pod * its window's width, else n_pair): [0] header {fault word}, then nw u8 reasons padded to 16 bytes, then nw
+// u32 blocking claims (always written; pushed only when the caller asked for pair_claim or claim_blocks).  A pair's answer
+// depends on its own node's state alone, so taking each pair from the rank that owns its node gives the single-inventory
+// answer on the world's state for any partition, and the tallies over the merged pairs are the single-inventory sums.
+struct WhyMerge {
+    const uint4* part;            // this rank's slice; a peer's is at my_stage + sender * slice4
+    uint32_t slice4;              // uint4 units of one sender's slice in the exchange
+    const uint32_t* cand_nodes; const uint32_t* cand_off;   // cand_off == nullptr: dense form
+    uint32_t n_pod, n_pair, n_node, n_claim;
+    uint32_t bounds[PEER_MAX + 1];   // rank r owns nodes [bounds[r], bounds[r + 1])
+    const uint32_t* gate;            // this rank's fault word
+    uint8_t* pair_why; uint32_t* pair_claim; uint32_t* pod_why; uint32_t* claim_blocks;   // the caller's (all but pair_why
+                                                                                           // nullptr unless asked)
+    uint32_t* blocks;             // claim_blocks: the counts (n_claim words), then the blocks-done counter, zeroed first
+};
+
+// At most SMs / 4 CTAs, launched after the evaluation: ranks sharing one device must not find their evaluation's SMs
+// held by a peer's waiting CTAs.  Block 0 raises this rank's flags, every block waits and checks every rank's fault word;
+// then a warp per pod: each lane takes a pair from the slice of the rank owning its node (a candidate naming no node:
+// NO_NODE, no claim), writes the pair's outputs and feeds the pod's tallies (why_pod_sums).  The per-claim counts take
+// atomics, so they go to scratch; the last block to finish copies them to the caller's claim_blocks, and only when every
+// block got past merge_start.  Nothing is written after a fault or a timeout.  With world 1 (an all-zero PeerExchange)
+// nothing is waited for.
+__global__ void __launch_bounds__(256)
+k_swhy_merge(const PeerExchange x, const WhyMerge m) {
+    const uint32_t tid = threadIdx.x, world = x.world ? x.world : 1u, rank = x.rank;
+    if (!merge_start(x, m.gate, m.slice4, world, rank, tid)) return;
+    const uint32_t lane = tid & 31;
+    const uint32_t warp = (blockIdx.x * blockDim.x + tid) >> 5, n_warp = (gridDim.x * blockDim.x) >> 5;
+    const bool dense = m.cand_off == nullptr, claims = m.pair_claim || m.claim_blocks;
+    for (uint32_t p = warp; p < m.n_pod; p += n_warp) {
+        unsigned long long k0, k1;
+        pod_pairs(m.cand_off, p, m.n_node, 0u, m.n_node, k0, k1);
+        uint32_t c = DRA_WHY_CLAIM_NONE;
+        why_pod_sums(p, lane, k0, k1, [&](unsigned long long k) {
+            const uint32_t node = pair_node(m.cand_off, m.cand_nodes, k, p, m.n_node);
+            uint32_t r = DRA_WHY_NO_NODE;                                  // a candidate naming no node
+            c = DRA_WHY_CLAIM_NONE;
+            if (node < m.n_node) {
+                const uint32_t o = node_owner(m.bounds, world, node);
+                const uint32_t lo = m.bounds[o], n_win = m.bounds[o + 1] - lo;
+                const uint32_t w = dense ? p * n_win + (node - lo) : (uint32_t)k;
+                const uint32_t nw = dense ? m.n_pod * n_win : m.n_pair;
+                const uint4* src = o == rank ? m.part : x.my_stage + (size_t)o * m.slice4;
+                r = __ldcg(reinterpret_cast<const unsigned char*>(src + 1) + w);
+                if (claims) c = __ldcg(reinterpret_cast<const unsigned int*>(src + 1 + ((size_t)nw + 15) / 16) + w);
+            }
+            m.pair_why[k] = (uint8_t)r;
+            if (m.pair_claim) m.pair_claim[k] = c;
+            return r;
+        }, [&](unsigned long long) { return c; }, m.pod_why, m.claim_blocks ? m.blocks : nullptr);
+    }
+    if (!m.claim_blocks) return;
+    __shared__ uint32_t s_last;
+    __threadfence();                                                      // this thread's counts, before the block's tick
+    __syncthreads();
+    if (tid == 0) s_last = atomicAdd(&m.blocks[m.n_claim], 1u) == gridDim.x - 1u;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    for (uint32_t i = tid; i < m.n_claim; i += blockDim.x) m.claim_blocks[i] = __ldcg(&m.blocks[i]);
 }
 
 }  // namespace dra
