@@ -873,6 +873,54 @@ func (c *Context) SetShardWhy(maxPairs uint32) error {
 	return nil
 }
 
+// PlacePodsWhyBatch places exactly as PlacePodsBatch and also says why each pod went where it did, or nowhere
+// (dra_place_pods_why_batch, spec §18): every (pod, candidate) pair answered with a reason and a blocking claim on the
+// state the pods before it left, laid out as UnsuitableWhyBatch's (cands == candOff == nil: every node, ascending,
+// nNode of them).  Returns the OutRecs, per pod the node it was placed on (0xFFFFFFFF: none), and the reasons.  Unbuilt,
+// like the rest of this file.
+func (c *Context) PlacePodsWhyBatch(claims []ClaimRec, podOff []uint32, cands, candOff []uint32, nNode int, outOff []uint32,
+	nOut int, flags uint32) ([]OutRec, []uint32, *UnsuitableWhy, error) {
+	out := make([]OutRec, nOut)
+	nPod := len(podOff) - 1
+	if nPod <= 0 {
+		return out, []uint32{}, &UnsuitableWhy{}, nil
+	}
+	podNode := make([]uint32, nPod)
+	nPair := nPod * nNode
+	var cp *C.dra_claim_rec
+	var oo, cn, co *C.uint32_t
+	if len(claims) > 0 {
+		cp = (*C.dra_claim_rec)(unsafe.Pointer(&claims[0]))
+	}
+	if outOff != nil {
+		oo = (*C.uint32_t)(unsafe.Pointer(&outOff[0]))
+	}
+	if candOff != nil {
+		nPair = int(candOff[nPod])
+		co = (*C.uint32_t)(unsafe.Pointer(&candOff[0]))
+		if len(cands) == 0 {
+			cands = []uint32{0} // an empty list still needs an address (nil means the dense form)
+		}
+		cn = (*C.uint32_t)(unsafe.Pointer(&cands[0]))
+	}
+	var op *C.dra_out_rec
+	if nOut > 0 {
+		op = (*C.dra_out_rec)(unsafe.Pointer(&out[0]))
+	}
+	r := &UnsuitableWhy{make([]uint8, nPair+1), make([]uint32, nPair+1), make([]uint32, nPod*9), make([]uint32, len(claims)+1)}
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_place_pods_why_batch(c.h, cp, C.uint32_t(len(claims)), (*C.uint32_t)(unsafe.Pointer(&podOff[0])),
+		C.uint32_t(nPod), cn, co, oo, op, C.uint32_t(nOut), (*C.uint32_t)(unsafe.Pointer(&podNode[0])),
+		(*C.uint8_t)(unsafe.Pointer(&r.PairWhy[0])), (*C.uint32_t)(unsafe.Pointer(&r.PairClaim[0])),
+		(*C.uint32_t)(unsafe.Pointer(&r.PodWhy[0])), (*C.uint32_t)(unsafe.Pointer(&r.ClaimBlocks[0])), C.uint32_t(flags))
+	if rc != 0 {
+		return nil, nil, nil, lastError(c.h)
+	}
+	r.PairWhy, r.PairClaim, r.ClaimBlocks = r.PairWhy[:nPair], r.PairClaim[:nPair], r.ClaimBlocks[:len(claims)]
+	return out, podNode, r, nil
+}
+
 // UnsuitableWhyBatchGlobalDevice: why each node is unsuitable (spec §17) on a sharded world
 // (dra_unsuitable_why_batch_global_device).  The same pods, candidates (pinnedCandNodes == pinnedCandOff == nil: dense
 // form, nPair = nPod * nNode) and flags on every context, every array in dra_host_alloc'ed (pinned) memory; each context

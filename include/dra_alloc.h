@@ -317,6 +317,35 @@ int  dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
                           const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
                           uint32_t* pod_node, uint32_t flags);
 
+/* Why place pods put each pod where it did, or nowhere (spec §18): dra_place_pods_batch's call, which also answers each
+ * of its (pod, candidate) pairs with a reason and a blocking claim in the state that pod met — the inventory as the pods
+ * before it left it — and sums the per-pod and per-claim tallies.  A batch scheduler writes a pending pod's
+ * "0/125 nodes are available: ..." from these, as kube-scheduler writes it from the state the pod met in its own cycle.
+ * Same inputs and flags as dra_place_pods_batch; out, pod_node and the inventory are byte for byte what that call
+ * leaves: asking for reasons changes no placement.  Pairs are laid out as dra_unsuitable_why_batch's (dense form: pair
+ * k = pod * n_node + node), and every pair is answered, including those after the candidate that took the pod (a dry run
+ * on the same state; a later pair naming the chosen node is OK).  Reasons follow §12's steps (dra_unsuitable_why_batch
+ * with DRA_F_EXHAUSTIVE) with the call's own evaluation:
+ *   pair_why[k]       NO_NODE for a candidate naming no node of the inventory; a pod of more than DRA_MAX_POD claims is
+ *                     INVALID, an empty pod OK; else INVALID at the lowest invalid claim (judged in the call's slot mode:
+ *                     without out_off a GPU claim of count != 1 is invalid), the first GPU / SHARED claim that fails, the
+ *                     first MIG claim with no placement at all (BAD_PROFILE / NO_CAPACITY), else POD or SEARCH_LIMIT at the
+ *                     MIG claim of level d.  Without DRA_F_EXHAUSTIVE the search does not backtrack: POD at the first MIG
+ *                     level with no admissible choice, and never SEARCH_LIMIT.  GROUP does not occur.
+ *   pair_claim[k]     (may be NULL) the blocking claim, a global index into claims, or DRA_WHY_CLAIM_NONE
+ *   pod_why[p * DRA_WHY_N + r]  (may be NULL) how many of pod p's pairs have reason r
+ *   claim_blocks[c]   (may be NULL, n_claim entries) how many pairs name claim c as their blocking claim
+ * For a non-empty pod of at most DRA_MAX_POD claims, pod_node[p] is the node of its first OK pair, and none exactly when
+ * it has none.  DRA_E_INVAL with nothing written (no output, no inventory word): dra_place_pods_batch's refusals, pair_why
+ * NULL with pairs to answer, dense n_pod * n_node >= 2^32.  n_pod == 0 returns DRA_OK after those checks.  Host buffers;
+ * flags: DRA_F_EXHAUSTIVE, DRA_F_FRESH_INVENTORY. */
+int  dra_place_pods_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
+                              const uint32_t* pod_off, uint32_t n_pod,
+                              const uint32_t* cand_nodes, const uint32_t* cand_off,
+                              const uint32_t* out_off, dra_out_rec* out, uint32_t n_out, uint32_t* pod_node,
+                              uint8_t* pair_why, uint32_t* pair_claim, uint32_t* pod_why, uint32_t* claim_blocks,
+                              uint32_t flags);
+
 /* Preemption (spec §14): for pods that fit nowhere, which lower-priority running pods to evict on each candidate node,
  * and which node to evict them on — kube-scheduler's DefaultPreemption (SelectVictimsOnNode, pickOneNodeForPreemption)
  * without start times; PodDisruptionBudgets through dra_preempt_pdb_batch.  Pure: nothing is written to the inventory. */
@@ -838,6 +867,7 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_POD_CAPACITY_SHARD 0x10000000u /* sharded pod capacity: prep, the window's pairs, exchange, merge with the sums */
 #define DRA_K_UNSUITABLE_WHY   0x20000000u /* reasons of UnsuitableNodes: the pair records, the tallies */
 #define DRA_K_UNSUITABLE_WHY_SHARD 0x40000000u /* sharded reasons: prep, the window's pair records, exchange, merge with the tallies */
+#define DRA_K_PLACE_WHY        0x80000000u /* place pods' reasons (with DRA_K_PLACE): the reasons walk, the tallies */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

@@ -127,6 +127,10 @@ public:
     // in the order of PotentialNodes; claims are named by ClaimUID.  Judged as UnsuitableNodesBatch judges them under
     // SetExhaustive; pure.  A pod whose claims cannot be lowered names its first such claim and its Error.
     std::vector<std::string> UnsuitableReasonsBatch(const std::vector<PodRequest>& pods);
+    // PlaceBatch that also says why each pod went where it did, or nowhere (spec §18, dra_place_pods_why_batch): places
+    // exactly as PlaceBatch, setting the same AllocatedNode, Allocation and Error on the claims, and returns one message
+    // per pod in UnsuitableReasonsBatch's format, each node judged as the pod met it, after the pods before it.
+    std::vector<std::string> PlaceBatchWithReasons(const std::vector<PodRequest>& pods);
 
     // live occupancy of one GPU (memory-slice mask), for inspection
     uint16_t BusyMask(const std::string& node, uint32_t gpuIndex);

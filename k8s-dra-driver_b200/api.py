@@ -27,7 +27,8 @@ KERNELS = {"fused_staged": 0x00001, "fused_stream": 0x00002, "fused_direct": 0x0
            "compact_lookback": 0x20000, "pod_shard": 0x80000, "pod_gather": 0x100000, "place": 0x200000,
            "place_shard": 0x400000, "preempt": 0x800000, "preempt_shard": 0x1000000,
            "preempt_place": 0x2000000, "preempt_place_shard": 0x4000000, "pod_capacity": 0x8000000,
-           "pod_capacity_shard": 0x10000000, "unsuitable_why": 0x20000000, "unsuitable_why_shard": 0x40000000}
+           "pod_capacity_shard": 0x10000000, "unsuitable_why": 0x20000000, "unsuitable_why_shard": 0x40000000,
+           "place_why": 0x80000000}
 # spec §17: the reasons of dra_unsuitable_why_batch are DRA_ST_OK .. DRA_ST_SEARCH_LIMIT (0 .. 7) and WHY_NO_NODE
 WHY_NO_NODE, WHY_N, WHY_CLAIM_NONE = 8, 9, 0xFFFFFFFF
 
@@ -74,6 +75,8 @@ SYMBOLS = {
     "dra_unsuitable_why_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _u32]),
     "dra_allocate_pods_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _u32]),
     "dra_place_pods_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _u32]),
+    "dra_place_pods_why_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp,
+                                        _u32]),
     "dra_deallocate_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_preempt_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32]),
     "dra_preempt_pdb_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
@@ -362,6 +365,33 @@ class Context:
         self._check(self._lib.dra_place_pods_batch(self._h, _ptr(c), len(c), _ptr(po), n_pod, _ptr(cn), _ptr(co), _ptr(oo),
                                                    _ptr(out), n_out, _ptr(pod_node), flags))
         return out, pod_node[:n_pod]
+
+    def place_pods_why(self, claims, pod_off, cand_nodes=None, cand_off=None, out_off=None, n_out=None, flags: int = 0,
+                       want_claims: bool = True, want_tallies: bool = True):
+        """place_pods() that also says why each pod went where it did, or nowhere (spec §18): each (pod, candidate) pair
+        answered with a reason and a blocking claim on the state that pod met, laid out as unsuitable_why()'s.  out,
+        pod_node and the inventory are exactly place_pods()'s.  Returns (out, pod_node, pair_why u8, pair_claim u32 or
+        None, pod_why u32 [n_pod, WHY_N] or None, claim_blocks u32 [n_claim] or None).  flags: F_EXHAUSTIVE,
+        F_FRESH_INVENTORY."""
+        c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
+        po = np.ascontiguousarray(pod_off, dtype=np.uint32)
+        oo = None if out_off is None else np.ascontiguousarray(out_off, dtype=np.uint32)
+        if n_out is None:
+            n_out = _placed_n_out(c, oo)
+        cn, co = _cands(cand_nodes, cand_off)
+        n_pod = len(po) - 1
+        n_pair = n_pod * self.n_node if co is None else int(co[-1])
+        out = np.zeros(n_out, dtype=R.OUT_DTYPE)
+        pod_node = np.zeros(max(n_pod, 1), dtype=np.uint32)
+        why = np.zeros(max(n_pair, 1), dtype=np.uint8)
+        blk = np.zeros(max(n_pair, 1), dtype=np.uint32) if want_claims else None
+        pod_why = np.zeros((max(n_pod, 1), WHY_N), dtype=np.uint32) if want_tallies else None
+        blocks = np.zeros(max(len(c), 1), dtype=np.uint32) if want_tallies else None
+        self._check(self._lib.dra_place_pods_why_batch(self._h, _ptr(c), len(c), _ptr(po), n_pod, _ptr(cn), _ptr(co),
+                                                       _ptr(oo), _ptr(out), n_out, _ptr(pod_node), _ptr(why), _ptr(blk),
+                                                       _ptr(pod_why), _ptr(blocks), flags))
+        return (out, pod_node[:n_pod], why[:n_pair], None if blk is None else blk[:n_pair],
+                None if pod_why is None else pod_why[:n_pod], None if blocks is None else blocks[:len(c)])
 
     def unsuitable(self, claims, pod_off, cand_nodes=None, cand_off=None, flags: int = 0) -> np.ndarray:
         """cand_nodes/cand_off None = dense form: every pod against every node (bit k = pod * n_node + node).

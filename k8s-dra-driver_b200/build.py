@@ -129,5 +129,24 @@ def build_cpp_why_test(force: bool = False) -> str:
     return exe
 
 
+def build_cpp_place_why_test(force: bool = False) -> str:
+    """tests/cpp/place_why_test: the C++ host layer's test of Driver::PlaceBatchWithReasons, linked like driver_test (in
+    the tree when it is writable, else into a temporary directory removed at exit)."""
+    build()
+    src, exe = os.path.join(ROOT, "tests", "cpp", "place_why_test.cpp"), os.path.join(ROOT, "tests", "cpp", "place_why_test")
+    if not force and os.path.exists(exe) and os.path.getmtime(exe) >= max(os.path.getmtime(src), os.path.getmtime(SO)):
+        return exe
+    if not os.access(os.path.dirname(exe), os.W_OK):
+        tmp = tempfile.mkdtemp(prefix="dra_place_why_test_")
+        atexit.register(shutil.rmtree, tmp, True)
+        exe = os.path.join(tmp, "place_why_test")
+    cmd = ["g++", "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include"), src, "-o", exe,
+           "-L", HERE, "-ldra_alloc", "-Wl,-rpath," + HERE]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        raise RuntimeError("g++ failed:\n" + r.stdout + r.stderr)
+    return exe
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose=True))

@@ -112,6 +112,7 @@ struct dra_ctx {
     uint32_t *d_place_state = nullptr, *d_place_node = nullptr; size_t cap_place_pods = 0;   // place pods: per pod
     uint32_t* d_place_cursor = nullptr; size_t cap_place_cursor = 0;                          // place pods: per node (+ 1)
     int place_occ = -1;                   // resident CTAs of k_pods_place<4> per SM (occupancy query, once)
+    int place_why_occ = -1;               // resident CTAs of k_pods_place<4, false, true> per SM (dra_place_pods_why_batch)
     // preemption (spec §14): per pending pod, per pair, the running pods and the victim rows
     uint32_t *d_pre_prio = nullptr, *d_pre_node = nullptr, *d_pre_nvic = nullptr, *d_pre_choice = nullptr; uint8_t* d_pre_pst = nullptr;
     uint32_t* d_pre_podviol = nullptr; size_t cap_pre_pods = 0;
@@ -1761,13 +1762,17 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
 
 // Place pods (spec §13): pod records -> (candidate form) the pair records stably sorted by node with the claim path's
 // bucketing kernels -> one persistent cooperative launch in which each warp walks its nodes' visit lists.  Everything is
-// validated here, before anything is enqueued: a rejected call changes nothing.
-int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, uint32_t n_pod,
-                         const uint32_t* cand_nodes, const uint32_t* cand_off, const uint32_t* out_off, dra_out_rec* out,
-                         uint32_t n_out, uint32_t* pod_node, uint32_t flags) {
+// validated here, before anything is enqueued: a rejected call changes nothing.  With why (spec §18) the walk is the
+// reasons instantiation, which also answers every pair (the prep the pairs no walk reaches), k_why_tally sums them, and
+// every output comes back after the same one synchronise.
+namespace {
+int place_pods_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off,
+                    uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, const uint32_t* out_off,
+                    dra_out_rec* out, uint32_t n_out, uint32_t* pod_node, bool why, uint8_t* pair_why, uint32_t* pair_claim,
+                    uint32_t* pod_why, uint32_t* claim_blocks, uint32_t flags) {
     if (!ctx || !pod_off || (n_claim && (!claims || !out)) || (n_pod && !pod_node)) return DRA_E_INVAL;
     QUIESCE();
-    if (flags & ~(DRA_F_EXHAUSTIVE | DRA_F_FRESH_INVENTORY)) return fail(ctx, DRA_E_INVAL, "dra_place_pods_batch: unknown flags 0x%x", flags);
+    if (flags & ~(DRA_F_EXHAUSTIVE | DRA_F_FRESH_INVENTORY)) return fail(ctx, DRA_E_INVAL, "%s: unknown flags 0x%x", name, flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     bool dense; uint32_t n_pair;                          // the dense form walks every node, ascending: no pair records
     int rc;
@@ -1776,9 +1781,16 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
     if ((rc = check_slots(ctx, claims, n_claim, out_off, n_out, true)) ||
         (rc = check_sortable(ctx, dense ? 0 : n_pair))) return rc;
+    uint32_t n_why = 0;                                   // the pairs answered (spec §18): dense, every pod at every node
+    if (why) {
+        const uint64_t n = dense ? (uint64_t)n_pod * ctx->n_node : n_pair;
+        if (n > 0xFFFFFFFFull) return fail(ctx, DRA_E_INVAL, "%llu (pod, node) pairs: more than %llu", (unsigned long long)n, 0xFFFFFFFFull);
+        n_why = (uint32_t)n;
+        if (n_why && !pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+    }
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
-    if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "dra_place_pods_batch needs cooperative launches, which this device does not offer");
+    if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "%s needs cooperative launches, which this device does not offer", name);
     CU(cudaSetDevice(ctx->device));
     if ((rc = ensure_batch(ctx, std::max(std::max(n_claim, n_pod), n_pair), n_out, true))) return rc;
     if ((rc = upload_table(ctx))) return rc;
@@ -1787,8 +1799,15 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
         (rc = grow_set(ctx, ctx->cap_podrec, (size_t)n_pair + 8, ctx->d_podrec)) ||
         (rc = grow_set(ctx, ctx->cap_place_pods, (size_t)n_pod + 8, ctx->d_place_state, ctx->d_place_node)) ||
         (rc = grow_set(ctx, ctx->cap_place_cursor, (size_t)ctx->n_node + 8, ctx->d_place_cursor))) return rc;
+    if (why && ((rc = grow_set(ctx, ctx->cap_why_pairs, (size_t)n_why + 8, ctx->d_why, ctx->d_why_claim)) ||
+                (rc = grow_set(ctx, ctx->cap_why_pods, (size_t)n_pod * DRA_WHY_N + 8, ctx->d_why_pod)) ||
+                (rc = grow_set(ctx, ctx->cap_why_claims, (size_t)n_claim + 8, ctx->d_why_blocks)))) return rc;
     const size_t rb = (size_t)n_out * 8;
-    const Outputs outs = {{out, ctx->d_out, rb}, {pod_node, ctx->d_place_node, (size_t)n_pod * 4}};
+    const Outputs outs = {{out, ctx->d_out, rb}, {pod_node, ctx->d_place_node, (size_t)n_pod * 4},
+                          {pair_why, ctx->d_why, why ? (size_t)n_why : 0},
+                          {pair_claim, ctx->d_why_claim, why && pair_claim ? (size_t)n_why * 4 : 0},
+                          {pod_why, ctx->d_why_pod, why && pod_why ? (size_t)n_pod * DRA_WHY_N * 4 : 0},
+                          {claim_blocks, ctx->d_why_blocks, why && claim_blocks ? (size_t)n_claim * 4 : 0}};
     if ((rc = reserve_out(ctx, outs))) return rc;
     Staging s;
     s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
@@ -1801,6 +1820,7 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     if ((rc = stage_in(ctx, s))) return rc;
     if (rb) CU(cudaMemsetAsync(ctx->d_out, 0, rb, ctx->stream));
     CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)ctx->n_node + 1) * 4, ctx->stream));
+    if (why && claim_blocks && n_claim) CU(cudaMemsetAsync(ctx->d_why_blocks, 0, (size_t)n_claim * 4, ctx->stream));
     Prof prof(ctx);
     PlaceArgs a; memset(&a, 0, sizeof a);
     a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.n_pod = n_pod;
@@ -1811,6 +1831,7 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     a.inv_src = (flags & DRA_F_FRESH_INVENTORY) ? ctx->d_inv_pristine : ctx->d_inv_live; a.inv_dst = ctx->d_inv_live;
     a.node_off = ctx->d_node_off; a.tbl = ctx->d_tbl;
     a.n_node = ctx->n_node; a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.sel = sel_of(ctx); a.err = err_of(ctx);
+    if (why) { a.why = ctx->d_why; a.why_claim = ctx->d_why_claim; }
     k_pods_place_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, ctx->stream>>>(a);
     ctx->launches += 1;
     // A candidate form with no pair sorts nothing, so the visit lists are zeroed instead: the walk must not read the
@@ -1819,10 +1840,41 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
     if (!dense && n_pair &&
         (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, a.inv_src, LA_NONE, ctx->n_node, ctx->d_node_off)))
         return rc;
-    if ((rc = launch_walk(ctx, ctx->place_occ, "k_pods_place", k_pods_place<4>, a, PlaceShard{}))) return rc;
-    ctx->chain |= DRA_K_PLACE;
+    if (!why) {
+        if ((rc = launch_walk(ctx, ctx->place_occ, "k_pods_place", k_pods_place<4>, a, PlaceShard{}))) return rc;
+        ctx->chain |= DRA_K_PLACE;
+    } else {
+        // (sized by its own occupancy: its registers are not k_pods_place<4>'s)
+        if ((rc = launch_walk(ctx, ctx->place_why_occ, "k_pods_place<4, false, true>", k_pods_place<4, false, true>, a, PlaceShard{})))
+            return rc;
+        if (pod_why || claim_blocks) {
+            const WhyTally t{ctx->d_why, ctx->d_why_claim, dense ? nullptr : ctx->d_cand_off, n_pod, ctx->n_node,
+                             pod_why ? ctx->d_why_pod : nullptr, claim_blocks ? ctx->d_why_blocks : nullptr};
+            k_why_tally<<<n_pod / 8 + 1, 256, 0, ctx->stream>>>(t);
+            ctx->launches += 1;
+        }
+        ctx->chain |= DRA_K_PLACE | DRA_K_PLACE_WHY;
+    }
     prof.mark();
-    return read_back(ctx, "place kernels", 4, outs);
+    return read_back(ctx, why ? "place reasons kernels" : "place kernels", 4, outs);
+}
+}  // namespace
+
+int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, uint32_t n_pod,
+                         const uint32_t* cand_nodes, const uint32_t* cand_off, const uint32_t* out_off, dra_out_rec* out,
+                         uint32_t n_out, uint32_t* pod_node, uint32_t flags) {
+    return place_pods_call(ctx, "dra_place_pods_batch", claims, n_claim, pod_off, n_pod, cand_nodes, cand_off, out_off, out, n_out,
+                           pod_node, false, nullptr, nullptr, nullptr, nullptr, flags);
+}
+
+// Why place pods put each pod where it did (spec §18): dra_place_pods_batch's call, every pair answered on the state its
+// pod met
+int dra_place_pods_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, uint32_t n_pod,
+                             const uint32_t* cand_nodes, const uint32_t* cand_off, const uint32_t* out_off, dra_out_rec* out,
+                             uint32_t n_out, uint32_t* pod_node, uint8_t* pair_why, uint32_t* pair_claim, uint32_t* pod_why,
+                             uint32_t* claim_blocks, uint32_t flags) {
+    return place_pods_call(ctx, "dra_place_pods_why_batch", claims, n_claim, pod_off, n_pod, cand_nodes, cand_off, out_off, out,
+                           n_out, pod_node, true, pair_why, pair_claim, pod_why, claim_blocks, flags);
 }
 
 // Preemption (spec §14): the pending-pod arrays are checked here; the running pods on the device (k_pre_running), whose

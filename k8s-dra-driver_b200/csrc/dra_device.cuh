@@ -2587,9 +2587,9 @@ struct PodGet {            // claim m of the pod, .y = its first OutRec slot
 // WHY (spec §17): a failure returns instead its reason | blocking position << 8 — INVALID at the lowest invalid claim;
 // NO_CAPACITY / MEM_LIMIT at the first GPU / SHARED claim that fails; BAD_PROFILE / NO_CAPACITY at the first MIG claim
 // the pre-check rejects; POD / SEARCH_LIMIT at the MIG claim of level d, the most levels the search held at once.
-// OWN: a copy of its own for a caller (the sharded reasons walk), so that the callers of the shared copy keep their code:
-// ptxas allocates a __noinline__ function's registers over all of its callers.
-template <int W, bool WHY = false, bool OWN = false>
+// OWN: a copy of its own for a caller (1: the sharded reasons walk, 2: place pods' reasons walk), so that the callers of the
+// shared copy keep their code: ptxas allocates a __noinline__ function's registers over all of its callers.
+template <int W, bool WHY = false, int OWN = 0>
 __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const uint32_t gmask, const uint32_t gbase,
                                           const uint32_t g0, const uint32_t* __restrict__ tbl_s, const PodGet get,
                                           const uint32_t cnt, const SelCtx sc, const bool exhaustive, const bool have_off,
@@ -2838,6 +2838,9 @@ k_pods(const PodArgs a) {
 // has passed its cursor.  Progress: the lowest unfinished pod heads its current node's list (everything before it there
 // belongs to finished pods or to its own earlier positions), so with every CTA resident the loop always advances.
 constexpr uint32_t PL_DONE = 0x80000000u, PL_LIMIT = 0x40000000u, PL_POS = 0x3FFFFFFFu;
+// The reasons walk (spec §18, k_pods_place<..., WHY = true>) answers every pair: a placed pod's word is DONE | PL_PLACED |
+// the position it was placed at, and the visits after that position are dry runs on the node as the pod met it.
+constexpr uint32_t PL_PLACED = 0x40000000u;   // (in a DONE word only)
 
 struct PlaceArgs {
     const uint4* claims; const uint32_t* pod_off; uint32_t n_pod;
@@ -2850,6 +2853,7 @@ struct PlaceArgs {
     uint32_t* cursor;             // [n_node] per node: entries of its list already passed; [n_node]: evaluations so far
     const uint4* inv_src; uint4* inv_dst; const uint32_t* node_off; const uint32_t* tbl;
     uint32_t n_node, exhaustive; SelCtx sel; Err err;
+    uint8_t* why; uint32_t* why_claim;   // spec §18 (nullptr: place pods alone): each pair's reason and blocking claim
 };
 
 // Sharded form (dra_place_pods_batch_global_device): each rank walks the visit lists of its own node window, and every
@@ -2913,9 +2917,31 @@ __device__ __forceinline__ void place_fail(const PlaceArgs& a, uint32_t c0, uint
     }
 }
 
+// The reasons of pod p's pairs that no walk reaches (spec §18; warp-wide): a candidate naming no node is NO_NODE; at the
+// others a pod of more than 32 claims is INVALID and an empty pod OK, neither with a claim.  Dense form: n_node per pod.
+__device__ __forceinline__ void place_why_prep(const PlaceArgs& a, uint32_t p, uint32_t cnt, uint32_t lane) {
+    const bool live = cnt != 0 && cnt <= DRA_MAX_POD;
+    const uint8_t r = cnt ? (uint8_t)DRA_ST_INVALID : (uint8_t)DRA_ST_OK;
+    if (!a.cand_off) {
+        if (live) return;
+        for (uint32_t n = lane; n < a.n_node; n += 32) {
+            const uint32_t k = p * a.n_node + n;                    // (n_pod * n_node < 2^32: checked by the host)
+            a.why[k] = r; a.why_claim[k] = DRA_WHY_CLAIM_NONE;
+        }
+        return;
+    }
+    const uint32_t k0 = __ldg(&a.cand_off[p]), k1 = __ldg(&a.cand_off[p + 1]);
+    for (uint32_t k = k0 + lane; k < k1; k += 32) {
+        const bool named = __ldg(&a.cand_nodes[k]) < a.n_node;
+        if (named && live) continue;
+        a.why[k] = named ? r : (uint8_t)DRA_WHY_NO_NODE; a.why_claim[k] = DRA_WHY_CLAIM_NONE;
+    }
+}
+
 // Warp per pod: the pod's state word (first usable position, or done), pod_node = NONE, the records of the pods that
 // will never be evaluated (more than 32 claims, or no candidate naming a node of the inventory) and, candidate form, the
 // pair records.  Pairs of pods that are never evaluated, and pairs naming no node, carry node NONE: the sort drops them.
+// With a.why, the reasons of the pairs no walk reaches (place_why_prep).
 __global__ void __launch_bounds__(256)
 k_pods_place_prep(const PlaceArgs a) {
     const uint32_t lane = threadIdx.x & 31;
@@ -2942,6 +2968,7 @@ k_pods_place_prep(const PlaceArgs a) {
         a.state[p] = live ? first : PL_DONE;
     }
     if (cnt != 0 && (!live || first == PL_DONE)) place_fail(a, c0, cnt, live ? (uint32_t)DRA_ST_POD : (uint32_t)DRA_ST_INVALID, lane);
+    if (a.why) place_why_prep(a, p, cnt, lane);
 }
 
 // Persistent: every CTA resident (cooperative launch); warp w owns nodes w, w + warps, ... and cycles over them.
@@ -2950,7 +2977,11 @@ k_pods_place_prep(const PlaceArgs a) {
 // stays until every pod's word here is DONE: a rank's own lists can end while pods still move on other ranks.  Launched
 // without the cooperative attribute (cooperative grids do not run beside each other), sized to the rank's share of the
 // residency.
-template <int WPC, bool SHARD = false>
+// WHY (spec §18, not with SHARD): every visit also writes its pair's reason and blocking claim (a.why, a.why_claim), and
+// a placed pod's word keeps its position (PL_PLACED), so a visit past it is no longer skipped: on the chosen node it is
+// OK, elsewhere a dry run of pod_eval on the node's state, which changes neither the node nor the pod.  Own
+// instantiation, so that the place pods walk keeps its registers.
+template <int WPC, bool SHARD = false, bool WHY = false>
 __global__ void __launch_bounds__(WPC * 32)
 k_pods_place(const PlaceArgs a, const PlaceShard sh) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
@@ -2988,13 +3019,16 @@ k_pods_place(const PlaceArgs a, const PlaceShard sh) {
                     if constexpr (SHARD) s = (uint32_t)ld_acquire_sys_u64(&sh.rep[sh.rank][q]);
                     else s = ld_acquire_u32(&a.state[q]);
                 }
-                const bool skip = (s & PL_DONE) || (s & PL_POS) > k;
+                bool skip;
+                if constexpr (WHY) skip = (s & PL_DONE) ? !((s & PL_PLACED) && (s & PL_POS) < k) : (s & PL_POS) > k;
+                else skip = (s & PL_DONE) || (s & PL_POS) > k;
                 const uint32_t act = __ballot_sync(FULLMASK, !skip);
                 if (!act) { cur = min(cur + 32u, l1); continue; }
                 const uint32_t f = (uint32_t)__ffs(act) - 1u;
                 cur += f;
                 const uint32_t qf = __shfl_sync(FULLMASK, q, f), kf = __shfl_sync(FULLMASK, k, f), sf = __shfl_sync(FULLMASK, s, f);
-                if ((sf & PL_POS) < kf) break;                   // q may still come here: this node waits
+                const bool dry = WHY && (sf & PL_DONE);           // WHY: q was placed at an earlier position
+                if (!dry && (sf & PL_POS) < kf) break;           // q may still come here: this node waits
                 if constexpr (SHARD) (void)ld_acquire_sys_u64(&sh.rep[sh.rank][qf]);
                 else (void)ld_acquire_u32(&a.state[qf]);         // every lane: ordered after the previous owner's records
                 if (!loaded) {
@@ -3002,7 +3036,24 @@ k_pods_place(const PlaceArgs a, const PlaceShard sh) {
                     loaded = true;
                 }
                 uint32_t st;
-                {
+                if constexpr (WHY) {
+                    // reason | blocking position << 8; a dry run writes no OutRec, and on the chosen node it is OK unevaluated
+                    // (the state the pod was placed on, not the one after its own placement)
+                    const uint32_t c0 = __ldg(&a.pod_off[qf]), cnt = __ldg(&a.pod_off[qf + 1]) - c0;
+                    const PodGet get{a.claims + c0, have_off ? a.out_off + c0 : nullptr, c0};
+                    Lane Lt = L;
+                    st = 0;
+                    if (!dry || __ldcg(&a.pod_node[qf]) != node)
+                        st = pod_eval<32, true, 2>(Lt, lane, FULLMASK, 0, g0, tbl_s, get, cnt, a.sel, a.exhaustive != 0, have_off,
+                                                   dry ? nullptr : a.out);
+                    if (st == 0 && !dry) L = Lt;
+                    if (lane == 0) {
+                        const uint32_t pair = dense ? qf * a.n_node + node : __ldg(&a.cand_off[qf]) + kf;
+                        a.why[pair] = (uint8_t)(st & 0xFFu);
+                        a.why_claim[pair] = st == 0 ? DRA_WHY_CLAIM_NONE : c0 + (st >> 8);
+                    }
+                    if (dry) { ++cur; continue; }
+                } else {
                     const uint32_t c0 = __ldg(&a.pod_off[qf]), cnt = __ldg(&a.pod_off[qf + 1]) - c0;
                     const PodGet get{a.claims + c0, have_off ? a.out_off + c0 : nullptr, c0};
                     Lane Lt = L;
@@ -3010,10 +3061,11 @@ k_pods_place(const PlaceArgs a, const PlaceShard sh) {
                     if (st == 0) L = Lt;
                 }
                 uint32_t next = PL_DONE;
-                const uint32_t lim = (sf & PL_LIMIT) | (st == DRA_ST_SEARCH_LIMIT ? PL_LIMIT : 0u);
+                const uint32_t lim = (sf & PL_LIMIT) | ((WHY ? st & 0xFFu : st) == DRA_ST_SEARCH_LIMIT ? PL_LIMIT : 0u);
                 if (st == 0) {
                     dirty = true;
                     if (!SHARD && lane == 0) a.pod_node[qf] = node;
+                    if constexpr (WHY) next = PL_DONE | PL_PLACED | kf;
                 } else {
                     // the pod's next candidate that names a node of the inventory
                     if (dense) { if (kf + 1u < a.n_node) next = (kf + 1u) | lim; }

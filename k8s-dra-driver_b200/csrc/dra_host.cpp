@@ -380,6 +380,39 @@ static std::string claim_text(const ClaimAllocation& ca) {
     return "claim \"" + ca.ClaimUID + "\" (" + what + ")";
 }
 
+// One pod's message from its pairs [k0, k1): "2/5 nodes are available: 2 nodes: claim ... no capacity; 1 node: ...",
+// nodes grouped by (reason, blocking claim), largest group first, ties in pair order.  The blocking claim is an index
+// into the LOWERED records: owner maps it back (group members were made adjacent, so it is not the position in
+// pod.Claims).
+static std::string why_message(const std::vector<ClaimAllocation*>& owner, const uint8_t* why, const uint32_t* blk,
+                               uint32_t k0, uint32_t k1) {
+    std::vector<std::pair<std::string, size_t>> parts;          // text, nodes; in order of first appearance
+    std::map<std::string, size_t> at;
+    size_t ok = 0;
+    for (uint32_t k = k0; k < k1; ++k) {
+        if (why[k] == DRA_ST_OK) { ++ok; continue; }
+        std::string t;
+        if (why[k] == DRA_WHY_NO_NODE) t = "not in the inventory";
+        else if (blk[k] == DRA_WHY_CLAIM_NONE) t = std::string("more than ") + std::to_string(DRA_MAX_POD) + " claims";
+        else t = claim_text(*owner[blk[k]]) + " " + why_text(why[k]);
+        auto it = at.find(t);
+        if (it == at.end()) { at[t] = parts.size(); parts.push_back({t, 1}); } else ++parts[it->second].second;
+    }
+    std::stable_sort(parts.begin(), parts.end(), [](const auto& a, const auto& b) { return a.second > b.second; });
+    std::string m = std::to_string(ok) + "/" + std::to_string(k1 - k0) + " nodes are available";
+    for (size_t i = 0; i < parts.size(); ++i) m += (i ? "; " : ": ") + nodes_text(parts[i].second) + ": " + parts[i].first;
+    return m + ".";
+}
+
+// The message of a pod whose claims cannot be lowered: its first such claim and that claim's Error
+static std::string unlowered_message(const Driver::PodRequest& pod) {
+    const size_t n = pod.PotentialNodes.size();
+    for (ClaimAllocation* ca : pod.Claims)
+        if (!ca->Error.empty())
+            return "0/" + std::to_string(n) + " nodes are available" + (n ? ": " + nodes_text(n) + ": " + claim_text(*ca) + " " + ca->Error : "") + ".";
+    return "";
+}
+
 std::vector<std::string> Driver::UnsuitableReasonsBatch(const std::vector<PodRequest>& pods) {
     std::vector<std::string> res(pods.size());
     Lowered lo;
@@ -404,12 +437,7 @@ std::vector<std::string> Driver::UnsuitableReasonsBatch(const std::vector<PodReq
         }
         if (!ok) {
             lo.recs.resize(mark); lo.outOff.resize(mark); lo.owner.resize(mark); lo.nOut = markOut;
-            const size_t n = pod.PotentialNodes.size();
-            for (ClaimAllocation* ca : pod.Claims)
-                if (!ca->Error.empty()) {
-                    res[pi] = "0/" + std::to_string(n) + " nodes are available" + (n ? ": " + nodes_text(n) + ": " + claim_text(*ca) + " " + ca->Error : "") + ".";
-                    break;
-                }
+            res[pi] = unlowered_message(pod);
             continue;
         }
         podOff.push_back((uint32_t)lo.recs.size());
@@ -423,26 +451,60 @@ std::vector<std::string> Driver::UnsuitableReasonsBatch(const std::vector<PodReq
     check(dra_unsuitable_why_batch(ctx_, lo.recs.data(), (uint32_t)lo.recs.size(), podOff.data(), (uint32_t)podOf.size(),
                                    cand.data(), candOff.data(), why.data(), blk.data(), nullptr, nullptr,
                                    exhaustive_ ? DRA_F_EXHAUSTIVE : 0u), "dra_unsuitable_why_batch");
-    for (size_t q = 0; q < podOf.size(); ++q) {
-        // the blocking claim is an index into the LOWERED records: lo.owner maps it back (group members were made
-        // adjacent, so it is not the position in pod.Claims)
-        std::vector<std::pair<std::string, size_t>> parts;      // text, nodes; in order of first appearance
-        std::map<std::string, size_t> at;
-        size_t ok = 0;
-        for (uint32_t k = candOff[q]; k < candOff[q + 1]; ++k) {
-            if (why[k] == DRA_ST_OK) { ++ok; continue; }
-            std::string t;
-            if (why[k] == DRA_WHY_NO_NODE) t = "not in the inventory";
-            else if (blk[k] == DRA_WHY_CLAIM_NONE) t = std::string("more than ") + std::to_string(DRA_MAX_POD) + " claims";
-            else t = claim_text(*lo.owner[blk[k]]) + " " + why_text(why[k]);
-            auto it = at.find(t);
-            if (it == at.end()) { at[t] = parts.size(); parts.push_back({t, 1}); } else ++parts[it->second].second;
+    for (size_t q = 0; q < podOf.size(); ++q) res[podOf[q]] = why_message(lo.owner, why.data(), blk.data(), candOff[q], candOff[q + 1]);
+    return res;
+}
+
+std::vector<std::string> Driver::PlaceBatchWithReasons(const std::vector<PodRequest>& pods) {
+    std::vector<std::string> res(pods.size());
+    Lowered lo;
+    std::vector<uint32_t> podOff(1, 0), candOff(1, 0), cand;
+    std::vector<size_t> podOf;                                  // lowered pod -> index in pods
+    for (size_t pi = 0; pi < pods.size(); ++pi) {
+        const auto& pod = pods[pi];
+        uint32_t model = 0;                                     // profile names: as in PlaceBatch
+        for (const auto& nn : pod.PotentialNodes) { const uint32_t n = nodeIndex(nn); if (n != 0xFFFFFFFFu) { model = nodeModel_[n]; break; } }
+        std::map<std::string, uint32_t> groups;
+        bool ok = true;
+        const size_t mark = lo.recs.size();
+        const uint32_t markOut = lo.nOut;
+        for (ClaimAllocation* ca : groupAdjacent(pod.Claims)) {
+            uint32_t g = 0;
+            if (ca->IsMig && !ca->Mig.GpuClaimName.empty()) {
+                auto it = groups.find(ca->Mig.GpuClaimName);
+                g = it == groups.end() ? (groups[ca->Mig.GpuClaimName] = nextGroup_++) : it->second;
+                if (nextGroup_ == 0) nextGroup_ = 1;
+            }
+            ca->AllocatedNode.clear();
+            ok = lower(*ca, 0, g, lo, model) && ok;
         }
-        std::stable_sort(parts.begin(), parts.end(), [](const auto& a, const auto& b) { return a.second > b.second; });
-        std::string m = std::to_string(ok) + "/" + std::to_string(candOff[q + 1] - candOff[q]) + " nodes are available";
-        for (size_t i = 0; i < parts.size(); ++i) m += (i ? "; " : ": ") + nodes_text(parts[i].second) + ": " + parts[i].first;
-        res[podOf[q]] = m + ".";
+        if (!ok) {
+            lo.recs.resize(mark); lo.outOff.resize(mark); lo.owner.resize(mark); lo.nOut = markOut;
+            res[pi] = unlowered_message(pod);
+            continue;
+        }
+        podOff.push_back((uint32_t)lo.recs.size());
+        for (const auto& nn : pod.PotentialNodes) cand.push_back(nodeIndex(nn));
+        candOff.push_back((uint32_t)cand.size());
+        podOf.push_back(pi);
     }
+    if (podOf.empty()) return res;
+    std::vector<dra_out_rec> out(lo.nOut);
+    std::vector<uint32_t> podNode(podOf.size());
+    std::vector<uint8_t> why(cand.size() + 1, 0);
+    std::vector<uint32_t> blk(cand.size() + 1, 0);
+    check(dra_place_pods_why_batch(ctx_, lo.recs.data(), (uint32_t)lo.recs.size(), podOff.data(), (uint32_t)podOf.size(),
+                                   cand.data(), candOff.data(), lo.outOff.data(), out.data(), lo.nOut, podNode.data(),
+                                   why.data(), blk.data(), nullptr, nullptr, exhaustive_ ? DRA_F_EXHAUSTIVE : 0u),
+          "dra_place_pods_why_batch");
+    for (size_t q = 0; q < podOf.size(); ++q) res[podOf[q]] = why_message(lo.owner, why.data(), blk.data(), candOff[q], candOff[q + 1]);
+    for (size_t q = 0; q < podOf.size(); ++q)                   // from here on as PlaceBatch
+        for (uint32_t i = podOff[q]; i < podOff[q + 1]; ++i) lo.recs[i].node = podNode[q] == DRA_GPU_NONE ? 0u : podNode[q];
+    lift(lo, out, true);
+    for (size_t q = 0; q < podOf.size(); ++q)
+        if (podNode[q] == DRA_GPU_NONE)
+            for (ClaimAllocation* ca : pods[podOf[q]].Claims)
+                if (ca->Error == status_text(DRA_ST_POD)) ca->Error = "the pod's claims fit together on none of its potential nodes";
     return res;
 }
 
