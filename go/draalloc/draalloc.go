@@ -941,6 +941,29 @@ func (c *Context) UnsuitableWhyBatchGlobalDevice(pinnedClaims unsafe.Pointer, nC
 	return nil
 }
 
+// PlacePodsWhyBatchGlobalDevice: place pods with reasons (spec §18) on a sharded world
+// (dra_place_pods_why_batch_global_device).  The same pods, candidates (pinnedCandNodes == pinnedCandOff == nil and
+// nPair == 0: dense form, nPod * nNode pairs answered), outOff, nOut and flags on every context, every array in
+// dra_host_alloc'ed (pinned) memory; each context walks the visits to its own nodes, and every context ends with the
+// whole table (GatherRead), the whole pod_node and the whole reason outputs (all but pinnedPairWhy may be nil).  Needs
+// SetShardPlace and SetShardWhy before ShardExport at world > 1.  Returns at once; Sync reports completion and errors
+// found on the device.  Unbuilt, like the rest of this file.
+func (c *Context) PlacePodsWhyBatchGlobalDevice(pinnedClaims unsafe.Pointer, nClaim int, pinnedPodOff unsafe.Pointer, nPod int,
+	pinnedCandNodes, pinnedCandOff unsafe.Pointer, nPair int, pinnedOutOff unsafe.Pointer, nOut int, pinnedPodNode unsafe.Pointer,
+	pinnedPairWhy, pinnedPairClaim, pinnedPodWhy, pinnedClaimBlocks unsafe.Pointer, flags uint32) error {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_place_pods_why_batch_global_device(c.h, (*C.dra_claim_rec)(pinnedClaims), C.uint32_t(nClaim),
+		(*C.uint32_t)(pinnedPodOff), C.uint32_t(nPod), (*C.uint32_t)(pinnedCandNodes), (*C.uint32_t)(pinnedCandOff),
+		C.uint32_t(nPair), (*C.uint32_t)(pinnedOutOff), C.uint32_t(nOut), (*C.uint32_t)(pinnedPodNode),
+		(*C.uint8_t)(pinnedPairWhy), (*C.uint32_t)(pinnedPairClaim), (*C.uint32_t)(pinnedPodWhy),
+		(*C.uint32_t)(pinnedClaimBlocks), C.uint32_t(flags))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
 // SetShardPreemptPlace reserves room for the sharded preempt-and-place call (pending pods, judged pairs, running pods):
 // after SetInventory, before ShardExport, the same on every context.  Unbuilt, like the rest of this file.
 func (c *Context) SetShardPreemptPlace(maxPods, maxPairs, maxRun uint32) error {

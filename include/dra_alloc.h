@@ -729,6 +729,29 @@ int  dra_unsuitable_why_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d
                                            const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
                                            uint8_t* d_pair_why, uint32_t* d_pair_claim,
                                            uint32_t* d_pod_why, uint32_t* d_claim_blocks, uint32_t flags);
+/* Why place pods put each pod where it did, or nowhere, over a sharded world (spec §18, "Sharded form"):
+ * dra_place_pods_why_batch applied to the world's state.  The arguments of dra_place_pods_batch_global_device (dense form:
+ * cand_nodes == cand_off == NULL and n_pair == 0), plus the four reason outputs laid out as dra_place_pods_why_batch's
+ * (dense form: pair k = pod * n_node + node); d_pair_claim, d_pod_why and d_claim_blocks may be NULL.  Each rank walks the
+ * visits to its own nodes as dra_place_pods_batch_global_device does and also answers them, a visit after the one that
+ * took its pod being a dry run on the node as the pod met it; the ranks then exchange their pairs' records as
+ * dra_unsuitable_why_batch_global_device does.  The table (dra_gather_table / dra_gather_read), d_pod_node and each rank's
+ * own GPU range are byte for byte what dra_place_pods_batch_global_device leaves on the same world — asking for reasons
+ * changes no placement — and every rank ends with the WHOLE reason outputs, byte for byte what dra_place_pods_why_batch
+ * answers on ONE inventory made of every rank's own nodes.  Prerequisites as for dra_place_pods_batch_global_device; world
+ * > 1 also needs dra_set_shard_why with max_pairs > 0 before dra_shard_export (else DRA_E_STATE, even for a call with no
+ * pairs).  World 1 needs no export and answers exactly as dra_place_pods_why_batch, inventory included.  Host-side errors
+ * (DRA_E_INVAL) return before anything is enqueued: dra_place_pods_batch_global_device's, a dense n_pod * n_node >= 2^32,
+ * more pairs than (world > 1) max_pairs, NULL d_pair_why with pairs to answer.  Enqueues on ctx's stream and returns;
+ * n_pod == 0 enqueues nothing.  The device-detected faults of dra_place_pods_batch_global_device give DRA_E_INVAL on EVERY
+ * rank at dra_ctx_sync with no inventory word and none of the reason outputs written, d_claim_blocks included; a peer that
+ * stops making progress gives DRA_E_NCCL, with no reason output written.  flags: DRA_F_EXHAUSTIVE, DRA_F_FRESH_INVENTORY. */
+int  dra_place_pods_why_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                            const uint32_t* d_pod_off, uint32_t n_pod,
+                                            const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                            const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node,
+                                            uint8_t* d_pair_why, uint32_t* d_pair_claim, uint32_t* d_pod_why,
+                                            uint32_t* d_claim_blocks, uint32_t flags);
 
 /* Every rank's live inventory becomes the world's state: for each GPU, the record its owning rank holds (the rank whose
  * node range contains the GPU's node, per the current dra_set_shard_map).  Own range untouched, pristine copy untouched.
@@ -867,7 +890,8 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_POD_CAPACITY_SHARD 0x10000000u /* sharded pod capacity: prep, the window's pairs, exchange, merge with the sums */
 #define DRA_K_UNSUITABLE_WHY   0x20000000u /* reasons of UnsuitableNodes: the pair records, the tallies */
 #define DRA_K_UNSUITABLE_WHY_SHARD 0x40000000u /* sharded reasons: prep, the window's pair records, exchange, merge with the tallies */
-#define DRA_K_PLACE_WHY        0x80000000u /* place pods' reasons (with DRA_K_PLACE): the reasons walk, the tallies */
+#define DRA_K_PLACE_WHY        0x80000000u /* place pods' reasons (with DRA_K_PLACE: the reasons walk, the tallies; with
+                                                   DRA_K_PLACE_SHARD: the sharded reasons walk, exchange, merge with the tallies) */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

@@ -115,6 +115,8 @@ SYMBOLS = {
                                                     _u32]),
     "dra_set_shard_why": (_i32, [_vp, _u32]),
     "dra_unsuitable_why_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _u32]),
+    "dra_place_pods_why_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _u32, _vp, _vp, _vp,
+                                                      _vp, _vp, _u32]),
     "dra_shard_sync_inventory_device": (_i32, [_vp]),
     "dra_deallocate_batch_global_device": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32]),
     "dra_mps_limits_batch": (_i32, [_vp, _vp, _u32, _vp, _vp]),
@@ -723,6 +725,22 @@ class Context:
         self._check(self._lib.dra_unsuitable_why_batch_global_device(
             self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod, _ptr(d_cand_nodes), _ptr(d_cand_off), n_pair,
             _ptr(d_pair_why), _ptr(d_pair_claim), _ptr(d_pod_why), _ptr(d_claim_blocks), flags))
+
+    def place_pods_why_global_device(self, d_claims: int, n_claim: int, d_pod_off: int, n_pod: int,
+                                     d_cand_nodes: int | None, d_cand_off: int | None, n_pair: int, d_out_off: int | None,
+                                     n_out: int, d_pod_node: int, d_pair_why: int | None, d_pair_claim: int | None = None,
+                                     d_pod_why: int | None = None, d_claim_blocks: int | None = None,
+                                     flags: int = 0) -> None:
+        """Sharded place pods with reasons (spec §18 "Sharded form"): place_pods_global_device()'s arguments (d_cand_nodes /
+        d_cand_off None and n_pair 0 = dense form) and placement, plus every (pod, candidate) pair's reason on the state its
+        pod met, laid out as place_pods_why()'s (u8 reasons, u32 blocking claims, u32 [n_pod, WHY_N] per-pod counts, u32
+        per-claim counts; dense: n_pod * n_node pairs).  Every rank receives the whole outputs; all but d_pair_why may be
+        None.  Needs set_shard_place() and set_shard_why() before shard_export at world > 1.  flags: F_EXHAUSTIVE,
+        F_FRESH_INVENTORY.  Enqueues, no synchronisation; errors found on the device surface at sync()."""
+        self._check(self._lib.dra_place_pods_why_batch_global_device(
+            self._h, _ptr(d_claims), n_claim, _ptr(d_pod_off), n_pod, _ptr(d_cand_nodes), _ptr(d_cand_off), n_pair,
+            _ptr(d_out_off), n_out, _ptr(d_pod_node), _ptr(d_pair_why), _ptr(d_pair_claim), _ptr(d_pod_why),
+            _ptr(d_claim_blocks), flags))
 
     def set_shard_preempt_place(self, max_pods: int, max_pairs: int, max_run: int) -> None:
         """Room for the sharded preempt-and-place call (pending pods, judged pairs, running pods); world > 1: before

@@ -237,6 +237,7 @@ struct dra_ctx {
     uint4* d_swhy_part = nullptr; size_t cap_swhy_part = 0;           // this rank's slice (uint4 units)
     uint32_t* d_swhy_blocks = nullptr; size_t cap_swhy_blocks = 0;    // the merge's per-claim counts and blocks-done counter
     int splace_occ = -1;                        // resident CTAs of k_pods_place<4, true> per SM (occupancy query, once)
+    int splace_why_occ = -1;                    // resident CTAs of k_pods_place<4, true, true> per SM (sharded §18)
     int peers_on_device = 1;                    // ranks whose contexts share this device (dra_peer_import_local)
     // inventory sync: records in the peer buffer ([staging x2: peer_inv_gpus records][flags[PEER_MAX], elect[2]])
     uint32_t peer_inv_gpus = 0;                 // n_gpu when the export ran (0: no inventory then)
@@ -2356,6 +2357,11 @@ int peer_setup(dra_ctx* ctx, uint32_t form, uint32_t n_per, uint32_t tab_len, ui
         if (int rc = grow(ctx, ctx->d_swhy_part, ctx->cap_swhy_part, swhy_units(z.swhy_pairs))) return rc;
         if (int rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, z.swhy_pairs)) return rc;
     }
+    // sharded place pods' reasons, after both reservations: the reasons walk and its prep loaded now (no module load
+    // inside a call once a peer's walk may wait for this rank)
+    if (z.place_pods && z.swhy_pairs) {
+        if (int rc = preload(ctx, {(const void*)k_splace_why_prep}, {(const void*)k_pods_place<4, true, true>}, false)) return rc;
+    }
     // sharded preempt and place, after dra_set_shard_preempt_place: its kernels loaded and its buffers at full size now (no
     // module load and no cudaFree inside a call while a peer's exchange waits for this rank)
     if (z.spp_pods) {
@@ -2871,14 +2877,20 @@ int dra_set_shard_place(dra_ctx* ctx, uint32_t max_pods) {
 // copy (k_spod_gate) -> stable counting sort of the pairs by window node -> the persistent walk of the window's visit lists,
 // every state word published to every rank (k_pods_place<4, true>) -> pod_node and the finalisers' slots (k_splace_final) ->
 // expected counts (k_spod_gate) -> all-gather of the finalised pods' records (k_spod_gather<true>).  Enqueues only.
-int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
-                                       const uint32_t* d_pod_off, uint32_t n_pod,
-                                       const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
-                                       const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node, uint32_t flags) {
+// With why (spec §18, dra_place_pods_why_batch_global_device): the reasons walk k_pods_place<4, true, true> writes this
+// rank's slice of §17's sharded exchange at the walk index, k_splace_why_prep (after the gate) the window's pairs no walk
+// reaches, and after the gather the slice goes to every peer behind its header — the walk's fault word, set when the call
+// is gated or the walk timed out — and k_swhy_merge writes the four reason outputs on every rank.
+namespace {
+int place_pods_shard_call(dra_ctx* ctx, const char* name, const dra_claim_rec* d_claims, uint32_t n_claim,
+                          const uint32_t* d_pod_off, uint32_t n_pod, const uint32_t* d_cand_nodes, const uint32_t* d_cand_off,
+                          uint32_t n_pair, const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node, bool why,
+                          uint8_t* d_pair_why, uint32_t* d_pair_claim, uint32_t* d_pod_why, uint32_t* d_claim_blocks,
+                          uint32_t flags) {
     if (!ctx || !d_pod_off || (n_claim && !d_claims) || (n_pod && !d_pod_node)) return DRA_E_INVAL;
     QUIESCE();
     if (flags & ~(DRA_F_EXHAUSTIVE | DRA_F_FRESH_INVENTORY))
-        return fail(ctx, DRA_E_INVAL, "dra_place_pods_batch_global_device: unknown flags 0x%x", flags);
+        return fail(ctx, DRA_E_INVAL, "%s: unknown flags 0x%x", name, flags);
     if (!ctx->shard_on) return fail(ctx, DRA_E_STATE, "dra_set_shard has not been called");
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     if (n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "batch too large for the sharded call (2^26)");
@@ -2887,19 +2899,41 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     bool dense;
     if (int rc = check_dev_cands(ctx, d_cand_nodes, d_cand_off, n_pod, n_pair, false, dense)) return rc;
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
+    uint32_t n_why = 0;                                   // the pairs answered (spec §18): dense, every pod at every node
+    if (why) {
+        const uint64_t n = dense ? (uint64_t)n_pod * ctx->n_node : n_pair;
+        if (n > 0xFFFFFFFFull) return fail(ctx, DRA_E_INVAL, "%llu (pod, node) pairs: more than %llu", (unsigned long long)n, 0xFFFFFFFFull);
+        n_why = (uint32_t)n;
+    }
     const bool gather = ctx->world > 1;
-    const uint32_t max_pods = ctx->shard_rsv.place_pods;
-    if (int rc = check_world(ctx, "the walk and the gather need", false, no_check, n_out, [&] {
-            if (n_pod <= max_pods) return (int)DRA_OK;
-            return fail(ctx, DRA_E_STATE, "n_pod %u exceeds the max_pods (%u) of dra_set_shard_place before dra_shard_export", n_pod, max_pods);
+    const uint32_t max_pods = ctx->shard_rsv.place_pods, max_pairs = ctx->shard_rsv.swhy_pairs;
+    // the reasons without their exchange reserved: even a call with no pairs pushes a header and raises flags, which would
+    // land in the peers' buffers at offset 0
+    if (int rc = check_world(ctx, "the walk and the gather need", false, [&] {
+            if (!why || max_pairs) return (int)DRA_OK;
+            return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_why(max_pairs > 0) was not called before dra_shard_export");
+        }, n_out, [&] {
+            if (n_pod > max_pods)
+                return fail(ctx, DRA_E_STATE, "n_pod %u exceeds the max_pods (%u) of dra_set_shard_place before dra_shard_export", n_pod, max_pods);
+            if (n_why > max_pairs)
+                return fail(ctx, DRA_E_INVAL, "%u pairs exceed the max_pairs (%u) of dra_set_shard_why before dra_shard_export", n_why, max_pairs);
+            return (int)DRA_OK;
         }))
         return rc;
+    if (n_why && !d_pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
     CallScope scope{ctx};
     int rc = scope.open(gather);
     if (rc) return rc;
     const uint32_t n_win = ctx->shard_hi - ctx->shard_lo;
+    // the reasons' slice (world > 1: peer_setup sized it for max_pairs, which bounds n_walk) and, with claim_blocks, the
+    // merge's per-claim counts, which depend on n_claim: a larger batch grows them here, the old buffer retired until the
+    // next dra_ctx_sync.  Both before anything is enqueued.
+    const uint32_t n_walk = dense ? n_pod * n_win : n_pair;           // (n_pod * n_win <= n_pod * n_node < 2^32)
+    if (why && ((rc = grow(ctx, ctx->d_swhy_part, ctx->cap_swhy_part, swhy_units(n_walk))) ||
+                (d_claim_blocks && (rc = grow(ctx, ctx->d_swhy_blocks, ctx->cap_swhy_blocks, (size_t)n_claim + 1)))))
+        return rc;
     if ((rc = ensure_batch(ctx, std::max(n_pod, n_pair), 1, false))) return rc;
     const Tiling t = tiling(n_pair, n_win, ctx->n_sm);                // the sort's tiles are laid out on the window
     if ((rc = grow(ctx, ctx->d_hist, ctx->cap_hist, (size_t)t.n_tiles * (n_win + 1), 64))) return rc;
@@ -2940,6 +2974,11 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     a.sorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.cursor = ctx->d_place_cursor;
     a.inv_src = ctx->d_inv_live; a.inv_dst = ctx->d_inv_live; a.node_off = d_node_off; a.tbl = ctx->d_tbl;
     a.n_node = ctx->n_node; a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.sel = sel_of(ctx); a.err = err;
+    uint4* part = ctx->d_swhy_part;                   // why: [header][n_walk u8 reasons, padded][n_walk u32 claims]
+    if (why) {
+        a.why = reinterpret_cast<uint8_t*>(part + 1);
+        a.why_claim = reinterpret_cast<uint32_t*>(part + 1 + ((size_t)n_walk + 15) / 16);   // (written whether sent or not)
+    }
     // the gate's SPodArgs: its record count is the sort's (the pairs), its world the one the bounds were counted for
     SPodArgs sa; memset(&sa, 0, sizeof sa);
     sa.claims = (const uint4*)d_claims; sa.pod_off = d_pod_off; sa.out_off = d_out_off;
@@ -2952,11 +2991,19 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     CU(cudaMemsetAsync(ctx->d_spod, 0, (SP_BAD + 1) * 4, ctx->stream));
     if (n_out) CU(cudaMemsetAsync(table, 0, (size_t)n_out * 8, ctx->stream));
     CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)n_win + 1) * 4, ctx->stream));
+    if (why) {
+        CU(cudaMemsetAsync(ctx->d_spod + SP_WHY_FAULT, 0, 4, ctx->stream));
+        if (d_claim_blocks) CU(cudaMemsetAsync(ctx->d_swhy_blocks, 0, ((size_t)n_claim + 1) * 4, ctx->stream));
+    }
     k_splace_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, ctx->stream>>>(a, sh);
     const uint32_t gate_grid = fresh ? std::max(1u, std::min((uint32_t)ctx->n_sm, (ctx->n_gpu + 255) / 256)) : 1u;
     k_spod_gate<<<gate_grid, 256, 0, ctx->stream>>>(sa_sort, gather ? ctx->peer_cap : 0u, fresh ? ctx->d_inv_pristine : nullptr,
                                                     ctx->d_inv_live, ctx->d_node_off);
     ctx->launches += 2;
+    if (why) {
+        k_splace_why_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, ctx->stream>>>(a, sh);
+        ctx->launches += 1;
+    }
     // A candidate form with no pair sorts nothing, so the visit lists are zeroed instead: the walk must not read the
     // offsets an earlier call's sort left in d_claim_off (an Allocate's claims by node), as lists of this call's pairs
     if (!dense && !n_pair) CU(cudaMemsetAsync(ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, ctx->stream));
@@ -2970,13 +3017,24 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
     CU(cudaMemsetAsync(ctx->d_spod, 0, PEER_MAX * 4, ctx->stream));
     // Every CTA resident, not a cooperative launch: cooperative grids do not run beside each other, and a rank's walk waits
     // for its peers' walks
-    if (ctx->splace_occ < 0) {
-        int occ = 0;
-        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_place<4, true>, 128, 0));
-        ctx->splace_occ = occ;
+    if (!why) {
+        if (ctx->splace_occ < 0) {
+            int occ = 0;
+            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_place<4, true>, 128, 0));
+            ctx->splace_occ = occ;
+        }
+        if (ctx->splace_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_place<4, true>: no CTA can be resident");
+        k_pods_place<4, true><<<shard_walk_grid(ctx, ctx->splace_occ, gather, n_win), 128, 0, ctx->stream>>>(a, sh);
+    } else {
+        // (sized by its own occupancy: its registers are not k_pods_place<4, true>'s)
+        if (ctx->splace_why_occ < 0) {
+            int occ = 0;
+            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_place<4, true, true>, 128, 0));
+            ctx->splace_why_occ = occ;
+        }
+        if (ctx->splace_why_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_place<4, true, true>: no CTA can be resident");
+        k_pods_place<4, true, true><<<shard_walk_grid(ctx, ctx->splace_why_occ, gather, n_win), 128, 0, ctx->stream>>>(a, sh);
     }
-    if (ctx->splace_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_place<4, true>: no CTA can be resident");
-    k_pods_place<4, true><<<shard_walk_grid(ctx, ctx->splace_occ, gather, n_win), 128, 0, ctx->stream>>>(a, sh);
     ctx->launches += 1;
     k_splace_final<<<(n_pod + 255) / 256, 256, 0, ctx->stream>>>(a, sh);
     ctx->launches += 1; ctx->chain |= DRA_K_PLACE_SHARD;
@@ -2986,10 +3044,50 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
         k_spod_gather<true><<<wait_grid(ctx, (std::max(n_pod, g.world * g.cap / 4u) + 255u) / 256u), 256, 0, ctx->stream>>>(g, sa, ctx->peer_tab_len);
         ctx->launches += 2;
     }
+    if (why) {
+        // every rank's slice to every rank behind its header (push_slice advances the region's call parity, as every
+        // §17 call does), then the owner-indexed merge with the tallies
+        const uint32_t* gate = ctx->d_spod + SP_WHY_FAULT;
+        WhyMerge m; memset(&m, 0, sizeof m);
+        m.part = part; m.cand_nodes = a.cand_nodes; m.cand_off = a.cand_off;
+        m.n_pod = n_pod; m.n_pair = n_pair; m.n_node = ctx->n_node; m.n_claim = n_claim;
+        merge_bounds(ctx, gather, m.bounds);
+        m.gate = gate;
+        m.pair_why = d_pair_why; m.pair_claim = d_pair_claim; m.pod_why = d_pod_why; m.claim_blocks = d_claim_blocks;
+        m.blocks = ctx->d_swhy_blocks;
+        if (gather) {
+            m.slice4 = (uint32_t)(ctx->swhy_x.slice / 16);
+            CU(cudaMemcpyAsync(part, gate, 4, cudaMemcpyDeviceToDevice, ctx->stream));   // the header: the walk's fault word
+        }
+        const PeerExchange x = push_slice(ctx, ctx->swhy_x, gather, part, (uint32_t)swhy_units(n_walk, d_pair_claim || d_claim_blocks));
+        k_swhy_merge<<<wait_grid(ctx, (n_pod + 7) / 8), 256, 0, ctx->stream>>>(x, m);
+        ctx->launches += 1; ctx->chain |= DRA_K_PLACE_WHY;
+    }
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded place pods launch: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "%s launch: %s", why ? "sharded place reasons" : "sharded place pods", cudaGetErrorString(e));
     ctx->gather_table = (const dra_out_rec*)table; ctx->gather_n_per = n_out; ctx->gather_len = n_out;
     return DRA_OK;
+}
+}  // namespace
+
+int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                       const uint32_t* d_pod_off, uint32_t n_pod,
+                                       const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                       const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node, uint32_t flags) {
+    return place_pods_shard_call(ctx, "dra_place_pods_batch_global_device", d_claims, n_claim, d_pod_off, n_pod, d_cand_nodes,
+                                 d_cand_off, n_pair, d_out_off, n_out, d_pod_node, false, nullptr, nullptr, nullptr, nullptr, flags);
+}
+
+// Why place pods put each pod where it did, across a sharded world (spec §18 "Sharded form")
+int dra_place_pods_why_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_claims, uint32_t n_claim,
+                                           const uint32_t* d_pod_off, uint32_t n_pod,
+                                           const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
+                                           const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node,
+                                           uint8_t* d_pair_why, uint32_t* d_pair_claim, uint32_t* d_pod_why,
+                                           uint32_t* d_claim_blocks, uint32_t flags) {
+    return place_pods_shard_call(ctx, "dra_place_pods_why_batch_global_device", d_claims, n_claim, d_pod_off, n_pod,
+                                 d_cand_nodes, d_cand_off, n_pair, d_out_off, n_out, d_pod_node, true, d_pair_why, d_pair_claim,
+                                 d_pod_why, d_claim_blocks, flags);
 }
 
 int dra_set_shard_preempt(dra_ctx* ctx, uint32_t max_pods, uint32_t max_pairs, uint32_t max_victims) {

@@ -2587,8 +2587,9 @@ struct PodGet {            // claim m of the pod, .y = its first OutRec slot
 // WHY (spec §17): a failure returns instead its reason | blocking position << 8 — INVALID at the lowest invalid claim;
 // NO_CAPACITY / MEM_LIMIT at the first GPU / SHARED claim that fails; BAD_PROFILE / NO_CAPACITY at the first MIG claim
 // the pre-check rejects; POD / SEARCH_LIMIT at the MIG claim of level d, the most levels the search held at once.
-// OWN: a copy of its own for a caller (1: the sharded reasons walk, 2: place pods' reasons walk), so that the callers of the
-// shared copy keep their code: ptxas allocates a __noinline__ function's registers over all of its callers.
+// OWN: a copy of its own for a caller (1: the sharded reasons walk, 2: place pods' reasons walk, 3: its sharded form), so
+// that the callers of the shared copy keep their code: ptxas allocates a __noinline__ function's registers over all of
+// its callers.
 template <int W, bool WHY = false, int OWN = 0>
 __device__ __noinline__ uint32_t pod_eval(Lane& L, const uint32_t lane, const uint32_t gmask, const uint32_t gbase,
                                           const uint32_t g0, const uint32_t* __restrict__ tbl_s, const PodGet get,
@@ -2875,6 +2876,10 @@ struct PlaceShard {
     uint32_t rank_hi[PEER_MAX];          // rank r serves nodes [rank_hi[r-1], rank_hi[r])
     long long spin_limit;                // cycles without a publication anywhere before ERR_PEER_TIMEOUT
 };
+// The call word (of PlaceShard::w, beside the SP_* words below) that the sharded reasons walk (k_pods_place<4, true,
+// true>) sets when it evaluates nothing (the call is gated) or times out: the header of this rank's reasons slice, zeroed
+// by the host before the call
+constexpr uint32_t SP_WHY_FAULT = 3 * PEER_MAX + 2;
 
 __device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) {
     uint32_t v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
@@ -2977,15 +2982,24 @@ k_pods_place_prep(const PlaceArgs a) {
 // stays until every pod's word here is DONE: a rank's own lists can end while pods still move on other ranks.  Launched
 // without the cooperative attribute (cooperative grids do not run beside each other), sized to the rank's share of the
 // residency.
-// WHY (spec §18, not with SHARD): every visit also writes its pair's reason and blocking claim (a.why, a.why_claim), and
-// a placed pod's word keeps its position (PL_PLACED), so a visit past it is no longer skipped: on the chosen node it is
-// OK, elsewhere a dry run of pod_eval on the node's state, which changes neither the node nor the pod.  Own
-// instantiation, so that the place pods walk keeps its registers.
+// WHY (spec §18): every visit also writes its pair's reason and blocking claim (a.why, a.why_claim), and a visit past a
+// placed pod's position is no longer skipped: on the chosen node it is OK, elsewhere a dry run of pod_eval on the node's
+// state, which changes neither the node nor the pod.  Single inventory: the placed word keeps its position (PL_PLACED).
+// SHARD: the word stays DONE | global node — a visit can only find its pod DONE-and-placed once it lies past the chosen
+// position (the word passes every usable position in order, and only that position's own visit moves it on), so every
+// such visit is a dry run; a PL_NOWHERE pod was evaluated at every pair and is skipped.  Records go to this rank's slice
+// at the walk index (dense: pod * n_win + window node), each dry run counts as progress for the peers' watchdogs, and a
+// gated or timed-out walk sets w[SP_WHY_FAULT].  Own instantiations, so that the place pods walks keep their registers.
 template <int WPC, bool SHARD = false, bool WHY = false>
 __global__ void __launch_bounds__(WPC * 32)
 k_pods_place(const PlaceArgs a, const PlaceShard sh) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
-    if constexpr (SHARD) { if (__ldcg(sh.gated)) return; }
+    if constexpr (SHARD) {
+        if (__ldcg(sh.gated)) {
+            if (WHY && blockIdx.x == 0 && threadIdx.x == 0) sh.w[SP_WHY_FAULT] = 1u;
+            return;
+        }
+    }
     stage_table<WPC * 32>(tbl_s, a.tbl);
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t w0 = blockIdx.x * WPC + (threadIdx.x >> 5), n_warp = gridDim.x * WPC;
@@ -3020,7 +3034,8 @@ k_pods_place(const PlaceArgs a, const PlaceShard sh) {
                     else s = ld_acquire_u32(&a.state[q]);
                 }
                 bool skip;
-                if constexpr (WHY) skip = (s & PL_DONE) ? !((s & PL_PLACED) && (s & PL_POS) < k) : (s & PL_POS) > k;
+                if constexpr (WHY && SHARD) skip = (s & PL_DONE) ? s == PL_NOWHERE : (s & PL_POS) > k;
+                else if constexpr (WHY) skip = (s & PL_DONE) ? !((s & PL_PLACED) && (s & PL_POS) < k) : (s & PL_POS) > k;
                 else skip = (s & PL_DONE) || (s & PL_POS) > k;
                 const uint32_t act = __ballot_sync(FULLMASK, !skip);
                 if (!act) { cur = min(cur + 32u, l1); continue; }
@@ -3043,14 +3058,18 @@ k_pods_place(const PlaceArgs a, const PlaceShard sh) {
                     const PodGet get{a.claims + c0, have_off ? a.out_off + c0 : nullptr, c0};
                     Lane Lt = L;
                     st = 0;
-                    if (!dry || __ldcg(&a.pod_node[qf]) != node)
-                        st = pod_eval<32, true, 2>(Lt, lane, FULLMASK, 0, g0, tbl_s, get, cnt, a.sel, a.exhaustive != 0, have_off,
-                                                   dry ? nullptr : a.out);
+                    // (a dry run on the node the pod was placed on is OK unevaluated)
+                    const bool eval = SHARD ? !dry || (sf & ~PL_DONE) != node + node_base : !dry || __ldcg(&a.pod_node[qf]) != node;
+                    if (eval)
+                        st = pod_eval<32, true, SHARD ? 3 : 2>(Lt, lane, FULLMASK, 0, g0, tbl_s, get, cnt, a.sel, a.exhaustive != 0,
+                                                               have_off, dry ? nullptr : a.out);
                     if (st == 0 && !dry) L = Lt;
                     if (lane == 0) {
-                        const uint32_t pair = dense ? qf * a.n_node + node : __ldg(&a.cand_off[qf]) + kf;
+                        const uint32_t pair = dense ? qf * (SHARD ? sh.n_win : a.n_node) + node : __ldg(&a.cand_off[qf]) + kf;
                         a.why[pair] = (uint8_t)(st & 0xFFu);
                         a.why_claim[pair] = st == 0 ? DRA_WHY_CLAIM_NONE : c0 + (st >> 8);
+                        if constexpr (SHARD)
+                            if (dry) for (uint32_t r = 0; r < sh.world; ++r) red_add_sys_u32(sh.prog[r], 1u);
                     }
                     if (dry) { ++cur; continue; }
                 } else {
@@ -3112,6 +3131,7 @@ k_pods_place(const PlaceArgs a, const PlaceShard sh) {
         if (pr != seen) { seen = pr; t0 = clock64(); }
         else if (clock64() - t0 > (SHARD ? sh.spin_limit : 4000000000ll)) {
             if (lane == 0) a.err.set(SHARD ? ERR_PEER_TIMEOUT : ERR_DEVICE_WAIT);
+            if (SHARD && WHY && lane == 0) sh.w[SP_WHY_FAULT] = 1u;
             dead = true;
             break;
         }
@@ -3130,7 +3150,11 @@ k_pods_place(const PlaceArgs a, const PlaceShard sh) {
             __nanosleep(256);
             const uint32_t pr = __shfl_sync(FULLMASK, ld_acquire_sys_u32(sh.prog[sh.rank]), 0);
             if (pr != seen) { seen = pr; t0 = clock64(); }
-            else if (clock64() - t0 > sh.spin_limit) { if (lane == 0) a.err.set(ERR_PEER_TIMEOUT); break; }
+            else if (clock64() - t0 > sh.spin_limit) {
+                if (lane == 0) a.err.set(ERR_PEER_TIMEOUT);
+                if (WHY && lane == 0) sh.w[SP_WHY_FAULT] = 1u;
+                break;
+            }
         }
     }
 }
@@ -3750,6 +3774,31 @@ k_splace_prep(const PlaceArgs a, const PlaceShard sh) {
     if (lane == 0) atomicMax(&sh.rep[sh.rank][p], ((unsigned long long)sh.seq << 32) | (walks ? first : PL_NOWHERE));
     if (cnt != 0 && !walks) place_fail(a, c0, cnt, live ? (uint32_t)DRA_ST_POD : (uint32_t)DRA_ST_INVALID, lane);
     if (walks && sh.world > 1 && lane < sh.world && ((owners >> lane) & 1u)) atomicAdd(&sh.w[lane], total);
+}
+
+// Warp per pod, after k_spod_gate, for the sharded reasons (dra_place_pods_why_batch_global_device): the records of this
+// rank's pairs that no walk reaches, into its slice at the walk index — a pod of more than 32 claims is INVALID, an empty
+// pod OK, neither with a claim (place_why_prep's rule on the window).  A candidate naming no node is the merge's.  Nothing
+// when the call is gated: the offsets are only known to be sound after the gate.  (A kernel of its own, so that
+// k_splace_prep keeps its registers.)
+__global__ void __launch_bounds__(256)
+k_splace_why_prep(const PlaceArgs a, const PlaceShard sh) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (p >= a.n_pod || __ldcg(sh.gated)) return;
+    const uint32_t cnt = __ldg(&a.pod_off[p + 1]) - __ldg(&a.pod_off[p]);
+    if (cnt != 0 && cnt <= DRA_MAX_POD) return;
+    const uint8_t r = cnt ? (uint8_t)DRA_ST_INVALID : (uint8_t)DRA_ST_OK;
+    if (!a.cand_off) {
+        for (uint32_t n = lane; n < sh.n_win; n += 32) {
+            const uint32_t k = p * sh.n_win + n;                    // (n_pod * n_node < 2^32: checked by the host)
+            a.why[k] = r; a.why_claim[k] = DRA_WHY_CLAIM_NONE;
+        }
+        return;
+    }
+    const uint32_t k0 = __ldg(&a.cand_off[p]), k1 = __ldg(&a.cand_off[p + 1]);
+    for (uint32_t k = k0 + lane; k < k1; k += 32)
+        if (__ldg(&a.cand_nodes[k]) - sh.node_lo < sh.n_win) { a.why[k] = r; a.why_claim[k] = DRA_WHY_CLAIM_NONE; }
 }
 
 // Thread per pod, after the walk (every word here is DONE): pod_node from the final word, and the pod's FINALISER — the
