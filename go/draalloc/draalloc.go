@@ -506,6 +506,132 @@ func (c *Context) PreemptPlaceBatch(claims []ClaimRec, podOff []uint32, prio []i
 	return r, nil
 }
 
+// cRunning: run as dra_running_pods.  The struct holds Go pointers, which cgo accepts only for pinned memory: pin keeps
+// them pinned until the caller unpins it.
+func cRunning(run RunningPods, pin *runtime.Pinner) C.dra_running_pods {
+	var rcp *C.dra_claim_rec
+	var rp *C.int32_t
+	var roo *C.uint32_t
+	var rop *C.dra_out_rec
+	if len(run.Claims) > 0 {
+		rcp = (*C.dra_claim_rec)(unsafe.Pointer(&run.Claims[0]))
+	}
+	if len(run.Prio) > 0 {
+		rp = (*C.int32_t)(unsafe.Pointer(&run.Prio[0]))
+	}
+	if run.OutOff != nil {
+		roo = (*C.uint32_t)(unsafe.Pointer(&run.OutOff[0]))
+	}
+	if len(run.Out) > 0 {
+		rop = (*C.dra_out_rec)(unsafe.Pointer(&run.Out[0]))
+	}
+	for _, q := range []unsafe.Pointer{unsafe.Pointer(rcp), unsafe.Pointer(&run.PodOff[0]), unsafe.Pointer(rp),
+		unsafe.Pointer(roo), unsafe.Pointer(rop)} {
+		if q != nil {
+			pin.Pin(q)
+		}
+	}
+	return C.dra_running_pods{claims: rcp, n_claim: C.uint32_t(len(run.Claims)),
+		pod_off: (*C.uint32_t)(unsafe.Pointer(&run.PodOff[0])), n_pod: C.uint32_t(len(run.PodOff) - 1), prio: rp,
+		out_off: roo, out: rop, n_out: C.uint32_t(len(run.Out))}
+}
+
+// PreemptWhyBatch says why preemption judged each candidate node as it did (dra_preempt_why_batch, spec §19): per pair the
+// status PreemptBatch gives it (pairStatus, may be nil), a reason and a blocking claim, and the per-pod and per-claim
+// tallies (podWhy, claimBlocks, may be nil), laid out as UnsuitableWhyBatch's.  Every slice is the caller's, sized as
+// the C call documents (pairWhy and pairClaim: one entry per pair).  Pure.  Unbuilt, like the rest of this file.
+func (c *Context) PreemptWhyBatch(claims []ClaimRec, podOff []uint32, prio []int32, cands, candOff []uint32, run RunningPods,
+	pairStatus, pairWhy []uint8, pairClaim, podWhy, claimBlocks []uint32, flags uint32) error {
+	nPod := len(podOff) - 1
+	if nPod <= 0 || len(run.PodOff) == 0 {
+		return nil
+	}
+	var cp *C.dra_claim_rec
+	var cn, co *C.uint32_t
+	if len(claims) > 0 {
+		cp = (*C.dra_claim_rec)(unsafe.Pointer(&claims[0]))
+	}
+	if candOff != nil {
+		co = (*C.uint32_t)(unsafe.Pointer(&candOff[0]))
+		if len(cands) == 0 {
+			cands = []uint32{0} // an empty list still needs an address (nil means the dense form)
+		}
+		cn = (*C.uint32_t)(unsafe.Pointer(&cands[0]))
+	}
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	cr := cRunning(run, &pin)
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_preempt_why_batch(c.h, cp, C.uint32_t(len(claims)), (*C.uint32_t)(unsafe.Pointer(&podOff[0])),
+		(*C.int32_t)(unsafe.Pointer(&prio[0])), C.uint32_t(nPod), cn, co, &cr, (*C.uint8_t)(sliceAddr8(pairStatus)),
+		(*C.uint8_t)(sliceAddr8(pairWhy)), (*C.uint32_t)(sliceAddr32(pairClaim)), (*C.uint32_t)(sliceAddr32(podWhy)),
+		(*C.uint32_t)(sliceAddr32(claimBlocks)), C.uint32_t(flags))
+	if rc != 0 {
+		return lastError(c.h)
+	}
+	return nil
+}
+
+// PreemptPlaceWhyBatch is PreemptPlaceBatch that also says why each pod was judged as it was on each candidate
+// (dra_preempt_place_why_batch, spec §19): the reason outputs of PreemptWhyBatch, each pair judged on the state its pod
+// met.  Placement, eviction and the inventory are PreemptPlaceBatch's.  Unbuilt, like the rest of this file.
+func (c *Context) PreemptPlaceWhyBatch(claims []ClaimRec, podOff []uint32, prio []int32, cands, candOff []uint32,
+	run RunningPods, outOff []uint32, nOut int, pairStatus, pairWhy []uint8, pairClaim, podWhy, claimBlocks []uint32,
+	flags uint32) (*PreemptPlacement, error) {
+	nPod := len(podOff) - 1
+	if nPod <= 0 || len(run.PodOff) == 0 {
+		return &PreemptPlacement{Out: make([]OutRec, nOut)}, nil
+	}
+	r := &PreemptPlacement{make([]OutRec, nOut+1), make([]uint32, nPod), make([]uint8, nPod), make([]uint32, len(run.PodOff))}
+	var cp *C.dra_claim_rec
+	var oo, cn, co *C.uint32_t
+	if len(claims) > 0 {
+		cp = (*C.dra_claim_rec)(unsafe.Pointer(&claims[0]))
+	}
+	if outOff != nil {
+		oo = (*C.uint32_t)(unsafe.Pointer(&outOff[0]))
+	}
+	if candOff != nil {
+		co = (*C.uint32_t)(unsafe.Pointer(&candOff[0]))
+		if len(cands) == 0 {
+			cands = []uint32{0} // an empty list still needs an address (nil means the dense form)
+		}
+		cn = (*C.uint32_t)(unsafe.Pointer(&cands[0]))
+	}
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	cr := cRunning(run, &pin)
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	rc := C.dra_preempt_place_why_batch(c.h, cp, C.uint32_t(len(claims)), (*C.uint32_t)(unsafe.Pointer(&podOff[0])),
+		(*C.int32_t)(unsafe.Pointer(&prio[0])), C.uint32_t(nPod), cn, co, &cr, oo,
+		(*C.dra_out_rec)(unsafe.Pointer(&r.Out[0])), C.uint32_t(nOut), (*C.uint32_t)(unsafe.Pointer(&r.PodNode[0])),
+		(*C.uint8_t)(unsafe.Pointer(&r.PodStatus[0])), (*C.uint32_t)(unsafe.Pointer(&r.EvictedBy[0])),
+		(*C.uint8_t)(sliceAddr8(pairStatus)), (*C.uint8_t)(sliceAddr8(pairWhy)), (*C.uint32_t)(sliceAddr32(pairClaim)),
+		(*C.uint32_t)(sliceAddr32(podWhy)), (*C.uint32_t)(sliceAddr32(claimBlocks)), C.uint32_t(flags))
+	if rc != 0 {
+		return nil, lastError(c.h)
+	}
+	r.Out, r.EvictedBy = r.Out[:nOut], r.EvictedBy[:len(run.PodOff)-1]
+	return r, nil
+}
+
+// sliceAddr8 / sliceAddr32: the first element's address, nil for an empty or nil slice (an optional output)
+func sliceAddr8(b []uint8) unsafe.Pointer {
+	if len(b) == 0 {
+		return nil
+	}
+	return unsafe.Pointer(&b[0])
+}
+
+func sliceAddr32(b []uint32) unsafe.Pointer {
+	if len(b) == 0 {
+		return nil
+	}
+	return unsafe.Pointer(&b[0])
+}
+
 // Pod-capacity answer (spec §16).  Per pair (candOff order; dense: pod*nNode + node): the copies of the pod the node
 // still takes and why counting stopped (DRA_ST_OK: maxCopies reached, DRA_ST_POD, DRA_ST_SEARCH_LIMIT, DRA_ST_INVALID).
 // Per pod: the sum over its pairs and how many of them take at least one copy.

@@ -415,6 +415,33 @@ int  dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n
                            uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims, uint32_t* pod_violations,
                            uint32_t* victims, uint32_t max_victims, uint32_t flags);
 
+/* Why preemption judged each node as it did (spec §19): dra_preempt_batch's pairs, each answered with its status, a
+ * reason and the claim that blocks it, and the per-pod and per-claim tallies of those answers — what a scheduler needs to
+ * say why a pod it could not preempt for stays pending.  Pure: nothing is written to the inventory.  Same pending pods,
+ * candidates, running pods and flags as dra_preempt_batch; pairs laid out as its pair_status (dense form: pair k =
+ * pod * n_node + node).  For pair k:
+ *   pair_status[k]    (may be NULL) DRA_PRE_*, byte for byte dra_preempt_batch's
+ *   pair_why[k]       DRA_WHY_NO_NODE for a candidate naming no node (status NO); INVALID for a pod of more than
+ *                     DRA_MAX_POD claims; DRA_ST_OK exactly when the pair FITS; for INVALID, INVALID at the lowest invalid
+ *                     claim; for EVICT, the reason the pod does not fit on the node as it is; for NO / SEARCH_LIMIT, the
+ *                     reason it does not fit even with every lower-priority pod on the node gone.  A reason is §12's, as
+ *                     dra_unsuitable_why_batch with DRA_F_EXHAUSTIVE gives it, with the call's own evaluation: without
+ *                     DRA_F_EXHAUSTIVE the search does not backtrack (POD at the first MIG level with no admissible
+ *                     choice, never SEARCH_LIMIT).  GROUP does not occur.
+ *   pair_claim[k]     (may be NULL) the blocking claim, a global index into claims, or DRA_WHY_CLAIM_NONE
+ *   pod_why[p * DRA_WHY_N + r]  (may be NULL) how many of pod p's pairs have reason r
+ *   claim_blocks[c]   (may be NULL, n_claim entries) how many pairs name claim c as their blocking claim
+ * Disruption budgets change no pair's status and no reason, so the answers hold for dra_preempt_pdb_batch as well.
+ * DRA_E_INVAL with nothing written: dra_preempt_batch's refusals, and pair_why NULL with pairs to answer.  n_pod == 0
+ * returns DRA_OK after the checks of the pending arrays, without examining the running pods.  Host buffers; flags: 0 or
+ * DRA_F_EXHAUSTIVE. */
+int  dra_preempt_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
+                           const uint32_t* pod_off, const int32_t* prio, uint32_t n_pod,
+                           const uint32_t* cand_nodes, const uint32_t* cand_off,
+                           const dra_running_pods* running,
+                           uint8_t* pair_status, uint8_t* pair_why, uint32_t* pair_claim,
+                           uint32_t* pod_why, uint32_t* claim_blocks, uint32_t flags);
+
 /* Preempt and place (spec §15): dra_preempt_batch's question for a batch that sees itself, answered and applied.  Pods
  * are taken in input order; pod p is judged as dra_preempt_batch judges it, but on the inventory as the pods before it
  * left it (their placements held, their victims gone), with only the running pods no earlier pod evicted as possible
@@ -447,6 +474,28 @@ int  dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t
                              const dra_running_pods* running,
                              const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
                              uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, uint32_t flags);
+
+/* Why preempt and place judged each node as it did (spec §19): dra_preempt_place_batch's call, which also answers each of
+ * its (pod, candidate) pairs with a status, a reason and a blocking claim, judged as dra_preempt_why_batch judges them but
+ * on the state that pod met: the inventory as the pods before it left it, with only the running pods no earlier pod
+ * evicted as possible victims.  out, pod_node, pod_status, evicted_by and the inventory are byte for byte what
+ * dra_preempt_place_batch leaves: asking for reasons changes no placement and no eviction.  Pairs and the four reason
+ * outputs are laid out as dra_preempt_why_batch's, pair_status may be NULL.  A pod that is never judged gets its pairs
+ * filled in directly: a pod invalid in the call's slot mode (without out_off a GPU claim of count != 1 is invalid) is
+ * INVALID at every pair naming a node, at its lowest invalid claim (DRA_WHY_CLAIM_NONE for more than DRA_MAX_POD claims);
+ * an empty pod is FITS / OK; a candidate naming no node is NO / DRA_WHY_NO_NODE.  When no running pod has a lower priority
+ * than any pending pod, the reason outputs are byte for byte dra_place_pods_why_batch's with the same flags.
+ * DRA_E_INVAL with nothing written (no output and no inventory word): dra_preempt_place_batch's refusals, and pair_why NULL
+ * with pairs to answer.  n_pod == 0 returns DRA_OK after the checks of the pending arrays, without examining the running
+ * pods.  Host buffers; flags: 0 or DRA_F_EXHAUSTIVE. */
+int  dra_preempt_place_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim,
+                                 const uint32_t* pod_off, const int32_t* prio, uint32_t n_pod,
+                                 const uint32_t* cand_nodes, const uint32_t* cand_off,
+                                 const dra_running_pods* running,
+                                 const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
+                                 uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by,
+                                 uint8_t* pair_status, uint8_t* pair_why, uint32_t* pair_claim,
+                                 uint32_t* pod_why, uint32_t* claim_blocks, uint32_t flags);
 
 /* Pod capacity (spec §16): how many copies of each pod every candidate node still takes — the question asked about a
  * workload rather than a pod (replicas of a Deployment that fit and where, an autoscaler's simulation, "free 3g.40gb
@@ -882,16 +931,20 @@ int  dra_debug_last_chain(const dra_ctx* ctx, uint32_t* kernels, uint32_t* hist_
 #define DRA_K_POD_GATHER        0x100000u /* sharded pods Allocate: all-gather of the owned pods' records (world > 1) */
 #define DRA_K_PLACE             0x200000u /* place pods: pod states + pair records, persistent walk of the nodes' visit lists */
 #define DRA_K_PLACE_SHARD       0x400000u /* sharded place pods: prep, gate, walk of the node window, finalisers (+ all-gather) */
-#define DRA_K_PREEMPT           0x800000u /* preemption: running-pod prep, victim lists, pairs, choice, victim rows */
+#define DRA_K_PREEMPT           0x800000u /* preemption: running-pod prep, victim lists, pairs, choice, victim rows (with
+                                                   DRA_K_UNSUITABLE_WHY: its reasons, the pairs' records and the tallies) */
 #define DRA_K_PREEMPT_SHARD    0x1000000u /* sharded preemption: prep, victim lists, the window's pairs, partials, merge */
-#define DRA_K_PREEMPT_PLACE    0x2000000u /* preempt and place: running-pod prep, victim lists, visit lists, persistent walk */
+#define DRA_K_PREEMPT_PLACE    0x2000000u /* preempt and place: running-pod prep, victim lists, visit lists, persistent walk (with
+                                                   DRA_K_PLACE_WHY: the reasons walk, the unreached pairs' records, the tallies) */
 #define DRA_K_PREEMPT_PLACE_SHARD 0x4000000u /* sharded preempt and place: state exchange, the §15 chain on it, own range back */
 #define DRA_K_POD_CAPACITY     0x8000000u /* pod capacity: the pairs' copy counts, the per-pod sums */
 #define DRA_K_POD_CAPACITY_SHARD 0x10000000u /* sharded pod capacity: prep, the window's pairs, exchange, merge with the sums */
-#define DRA_K_UNSUITABLE_WHY   0x20000000u /* reasons of UnsuitableNodes: the pair records, the tallies */
+#define DRA_K_UNSUITABLE_WHY   0x20000000u /* reasons of UnsuitableNodes: the pair records, the tallies (with
+                                                   DRA_K_PREEMPT: the reasons of preemption) */
 #define DRA_K_UNSUITABLE_WHY_SHARD 0x40000000u /* sharded reasons: prep, the window's pair records, exchange, merge with the tallies */
 #define DRA_K_PLACE_WHY        0x80000000u /* place pods' reasons (with DRA_K_PLACE: the reasons walk, the tallies; with
-                                                   DRA_K_PLACE_SHARD: the sharded reasons walk, exchange, merge with the tallies) */
+                                                   DRA_K_PLACE_SHARD: the sharded reasons walk, exchange, merge with the tallies;
+                                                   with DRA_K_PREEMPT_PLACE: the reasons of preempt and place) */
 /* Instrumentation (env DRA_TIMELINE=1): globaltimer of the last shard compaction's first CTA in / last CTA out. */
 int  dra_debug_shard_times(dra_ctx* ctx, unsigned long long* two);
 /* Instrumentation: globaltimer stamps of the resident kernel's last batch — doorbell seen, CTA 0's egress issued, every CTA

@@ -82,6 +82,9 @@ SYMBOLS = {
     "dra_preempt_pdb_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                      _u32, _u32]),
     "dra_preempt_place_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _u32]),
+    "dra_preempt_why_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32]),
+    "dra_preempt_place_why_batch": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp,
+                                           _vp, _vp, _vp, _vp, _u32]),
     "dra_pod_capacity_batch": (_i32, [_vp, _vp, _u32, _vp, _u32, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _u32]),
     "dra_comm_unique_id": (_i32, [_vp]),
     "dra_comm_init": (_i32, [_vp, _vp, _i32, _i32]),
@@ -498,6 +501,65 @@ class Context:
                                                       C.byref(run), _ptr(oo), _ptr(out), n_out, _ptr(pod_node),
                                                       _ptr(pod_status), _ptr(evicted_by), flags))
         return out[:n_out], pod_node[:n_pod], pod_status[:n_pod], evicted_by[:run.n_pod]
+
+    def preempt_why(self, claims, pod_off, prio, run_claims, run_pod_off, run_prio, run_out, run_out_off=None,
+                    cand_nodes=None, cand_off=None, flags: int = 0, want_claims: bool = True, want_tallies: bool = True):
+        """Why preemption judged each node as it did (spec §19): preempt()'s pairs, each with its status, a reason and a
+        blocking claim, laid out as unsuitable_why()'s.  Pure.  Budgets change no status and no reason, so the answers
+        hold for preempt_pdb() too.  Returns (pair_status u8, pair_why u8, pair_claim u32 or None, pod_why u32
+        [n_pod, WHY_N] or None, claim_blocks u32 [n_claim] or None).  flags: 0 or F_EXHAUSTIVE."""
+        c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
+        po = np.ascontiguousarray(pod_off, dtype=np.uint32)
+        pr = np.ascontiguousarray(prio, dtype=np.int32)
+        n_pod = len(po) - 1
+        run = _running(run_claims, run_pod_off, run_prio, run_out, run_out_off)
+        cn, co = _cands(cand_nodes, cand_off)
+        n_pair = n_pod * self.n_node if co is None else int(co[-1])
+        pair_status = np.zeros(max(n_pair, 1), dtype=np.uint8)
+        why = np.zeros(max(n_pair, 1), dtype=np.uint8)
+        blk = np.zeros(max(n_pair, 1), dtype=np.uint32) if want_claims else None
+        pod_why = np.zeros((max(n_pod, 1), WHY_N), dtype=np.uint32) if want_tallies else None
+        blocks = np.zeros(max(len(c), 1), dtype=np.uint32) if want_tallies else None
+        self._check(self._lib.dra_preempt_why_batch(self._h, _ptr(c), len(c), _ptr(po), _ptr(pr), n_pod, _ptr(cn), _ptr(co),
+                                                    C.byref(run), _ptr(pair_status), _ptr(why), _ptr(blk), _ptr(pod_why),
+                                                    _ptr(blocks), flags))
+        return (pair_status[:n_pair], why[:n_pair], None if blk is None else blk[:n_pair],
+                None if pod_why is None else pod_why[:n_pod], None if blocks is None else blocks[:len(c)])
+
+    def preempt_place_why(self, claims, pod_off, prio, run_claims, run_pod_off, run_prio, run_out, run_out_off=None,
+                          cand_nodes=None, cand_off=None, out_off=None, n_out=None, flags: int = 0,
+                          want_claims: bool = True, want_tallies: bool = True):
+        """preempt_place() that also says why each pod was judged as it was on each candidate (spec §19): every pair's
+        status, reason and blocking claim on the state its pod met, laid out as preempt_why()'s.  out, pod_node,
+        pod_status, evicted_by and the inventory are exactly preempt_place()'s.  Returns (out, pod_node, pod_status,
+        evicted_by, pair_status u8, pair_why u8, pair_claim u32 or None, pod_why u32 [n_pod, WHY_N] or None,
+        claim_blocks u32 [n_claim] or None).  flags: 0 or F_EXHAUSTIVE."""
+        c = np.ascontiguousarray(claims, dtype=R.CLAIM_DTYPE)
+        po = np.ascontiguousarray(pod_off, dtype=np.uint32)
+        pr = np.ascontiguousarray(prio, dtype=np.int32)
+        n_pod = len(po) - 1
+        oo = None if out_off is None else np.ascontiguousarray(out_off, dtype=np.uint32)
+        if n_out is None:
+            n_out = _placed_n_out(c, oo)
+        run = _running(run_claims, run_pod_off, run_prio, run_out, run_out_off)
+        cn, co = _cands(cand_nodes, cand_off)
+        n_pair = n_pod * self.n_node if co is None else int(co[-1])
+        out = np.zeros(max(n_out, 1), dtype=R.OUT_DTYPE)
+        pod_node = np.zeros(max(n_pod, 1), dtype=np.uint32)
+        pod_status = np.zeros(max(n_pod, 1), dtype=np.uint8)
+        evicted_by = np.zeros(max(run.n_pod, 1), dtype=np.uint32)
+        pair_status = np.zeros(max(n_pair, 1), dtype=np.uint8)
+        why = np.zeros(max(n_pair, 1), dtype=np.uint8)
+        blk = np.zeros(max(n_pair, 1), dtype=np.uint32) if want_claims else None
+        pod_why = np.zeros((max(n_pod, 1), WHY_N), dtype=np.uint32) if want_tallies else None
+        blocks = np.zeros(max(len(c), 1), dtype=np.uint32) if want_tallies else None
+        self._check(self._lib.dra_preempt_place_why_batch(
+            self._h, _ptr(c), len(c), _ptr(po), _ptr(pr), n_pod, _ptr(cn), _ptr(co), C.byref(run), _ptr(oo), _ptr(out), n_out,
+            _ptr(pod_node), _ptr(pod_status), _ptr(evicted_by), _ptr(pair_status), _ptr(why), _ptr(blk), _ptr(pod_why),
+            _ptr(blocks), flags))
+        return (out[:n_out], pod_node[:n_pod], pod_status[:n_pod], evicted_by[:run.n_pod], pair_status[:n_pair],
+                why[:n_pair], None if blk is None else blk[:n_pair], None if pod_why is None else pod_why[:n_pod],
+                None if blocks is None else blocks[:len(c)])
 
     def pod_capacity(self, claims, pod_off, cand_nodes=None, cand_off=None, max_copies: int = 64, exhaustive: bool = False,
                      want_stop: bool = True, want_totals: bool = True):

@@ -130,6 +130,7 @@ struct dra_ctx {
     uint32_t* d_pp_evicted = nullptr; size_t cap_pp_rpods = 0;
     uint32_t *d_pp_runoff = nullptr, *d_pp_judged = nullptr; size_t cap_pp_nodes = 0;
     int pp_occ = -1;                      // resident CTAs of k_pods_preempt_place<4> per SM (occupancy query, once)
+    int pp_why_occ = -1;                  // resident CTAs of k_pods_preempt_place<4, true> per SM (dra_preempt_place_why_batch)
     // pod capacity (spec §16): per pair, per pod
     uint16_t* d_cap_copies = nullptr; uint8_t* d_cap_stop = nullptr; size_t cap_cap_pairs = 0;
     unsigned long long* d_cap_total = nullptr; uint32_t* d_cap_nodes = nullptr; size_t cap_cap_pods = 0;
@@ -1012,11 +1013,12 @@ int launch_running_lists(dra_ctx* ctx, PreArgs& a, Prof& prof, bool walk) {
 }
 
 // k_pods_preempt over s's pairs (none: no launch).  Enqueues only.
-int launch_preempt_pairs(dra_ctx* ctx, PreArgs a, const PreShard& s) {
+int launch_preempt_pairs(dra_ctx* ctx, PreArgs a, const PreShard& s, bool why = false) {
     if (!s.n_walk) return DRA_OK;
     if (int rc = walk_counter(ctx, TK_WALK_PREEMPT, a.work)) return rc;
     const uint32_t grid = pair_grid(ctx, s.n_walk);
-    at_pair_width(ctx, [&](auto w) { k_pods_preempt<8, decltype(w)::value><<<grid, 256, 0, ctx->stream>>>(a, s); });
+    if (why) at_pair_width(ctx, [&](auto w) { k_pods_preempt<8, decltype(w)::value, true><<<grid, 256, 0, ctx->stream>>>(a, s); });
+    else at_pair_width(ctx, [&](auto w) { k_pods_preempt<8, decltype(w)::value><<<grid, 256, 0, ctx->stream>>>(a, s); });
     ctx->launches += 1;
     return DRA_OK;
 }
@@ -1880,18 +1882,23 @@ int dra_place_pods_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t
 
 // Preemption (spec §14): the pending-pod arrays are checked here; the running pods on the device (k_pre_running), whose
 // fault gates every later kernel.  Inputs are staged in, the kernels launched, the outputs copied back after ONE
-// synchronise, and the caller's buffers are written only when no fault was found.
-int dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, const int32_t* prio,
-                          uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, const dra_running_pods* running,
-                          const dra_disruption_budgets* budgets, uint8_t* pair_status, uint32_t* pair_victims,
-                          uint32_t* pair_violations, uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
-                          uint32_t* pod_violations, uint32_t* victims, uint32_t max_victims, uint32_t flags) {
-    if (!ctx || !pod_off || !running || !running->pod_off || (n_claim && !claims) || (n_pod && (!prio || !pod_node || !pod_status || !n_victims)))
+// synchronise, and the caller's buffers are written only when no fault was found.  With why (spec §19,
+// dra_preempt_why_batch) the pairs are the reasons instantiation of k_pods_preempt, which stops at each pair's status;
+// nothing is chosen and no victim row is built, and k_why_tally sums the records.
+namespace {
+int preempt_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off,
+                 const int32_t* prio, uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off,
+                 const dra_running_pods* running, const dra_disruption_budgets* budgets, uint8_t* pair_status,
+                 uint32_t* pair_victims, uint32_t* pair_violations, uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
+                 uint32_t* pod_violations, uint32_t* victims, uint32_t max_victims, bool why, uint8_t* pair_why,
+                 uint32_t* pair_claim, uint32_t* pod_why, uint32_t* claim_blocks, uint32_t flags) {
+    if (!ctx || !pod_off || !running || !running->pod_off || (n_claim && !claims) ||
+        (n_pod && (!prio || (!why && (!pod_node || !pod_status || !n_victims)))))
         return DRA_E_INVAL;
     const dra_running_pods& R = *running;
     if ((R.n_claim && !R.claims) || (R.n_pod && !R.prio) || (R.n_out && !R.out)) return DRA_E_INVAL;
     QUIESCE();
-    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_preempt_batch: unknown flags 0x%x", flags);
+    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "%s: unknown flags 0x%x", why ? name : "dra_preempt_batch", flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     if (max_victims && !victims) return fail(ctx, DRA_E_INVAL, "max_victims %u without a victims buffer", max_victims);
     if (budgets && budgets->n_pdb && !budgets->allowed)
@@ -1901,7 +1908,8 @@ int dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
     if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
         (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, 0xFFFFFFFFu, ctx->n_node, 0xFFFFFFFFull, dense, n_pair)) ||
         (rc = check_sortable(ctx, n_pod ? R.n_pod : 0))) return rc;
-    ctx->chain = DRA_K_PREEMPT; ctx->chain_tile = 0;
+    if (why && n_pair && !pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+    ctx->chain = why ? DRA_K_PREEMPT | DRA_K_UNSUITABLE_WHY : DRA_K_PREEMPT; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     if ((rc = check_budgets(ctx, "dra_preempt_pdb_batch", budgets, R.n_pod))) return rc;
     CU(cudaSetDevice(ctx->device));
@@ -1915,14 +1923,22 @@ int dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
         (rc = grow_set(ctx, ctx->cap_pre_pairs, (size_t)n_pair + 8, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic,
                        ctx->d_pre_pairviol)) ||
         (rc = grow_set(ctx, ctx->cap_pre_vic, vb / 4 + 8, ctx->d_pre_vic))) return rc;
+    if (why && ((rc = grow_set(ctx, ctx->cap_why_pairs, (size_t)n_pair + 8, ctx->d_why, ctx->d_why_claim)) ||
+                (rc = grow_set(ctx, ctx->cap_why_pods, (size_t)n_pod * DRA_WHY_N + 8, ctx->d_why_pod)) ||
+                (rc = grow_set(ctx, ctx->cap_why_claims, (size_t)n_claim + 8, ctx->d_why_blocks)))) return rc;
+    const size_t np = why ? 0 : n_pod;                   // (the reasons call chooses nothing: no per-pod output)
     const Outputs outs = {{pair_status, ctx->d_pre_pairst, pair_status ? (size_t)n_pair : 0},
                           {pair_victims, ctx->d_pre_pairvic, pair_victims ? (size_t)n_pair * 4 : 0},
-                          {pod_node, ctx->d_pre_node, (size_t)n_pod * 4},
-                          {pod_status, ctx->d_pre_pst, n_pod},
-                          {n_victims, ctx->d_pre_nvic, (size_t)n_pod * 4},
+                          {pod_node, ctx->d_pre_node, np * 4},
+                          {pod_status, ctx->d_pre_pst, np},
+                          {n_victims, ctx->d_pre_nvic, np * 4},
                           {victims, ctx->d_pre_vic, vb},
                           {pair_violations, ctx->d_pre_pairviol, pair_violations ? (size_t)n_pair * 4 : 0},
-                          {pod_violations, ctx->d_pre_podviol, pod_violations ? (size_t)n_pod * 4 : 0}};
+                          {pod_violations, ctx->d_pre_podviol, pod_violations ? (size_t)n_pod * 4 : 0},
+                          {pair_why, ctx->d_why, why ? (size_t)n_pair : 0},
+                          {pair_claim, ctx->d_why_claim, why && pair_claim ? (size_t)n_pair * 4 : 0},
+                          {pod_why, ctx->d_why_pod, why && pod_why ? (size_t)n_pod * DRA_WHY_N * 4 : 0},
+                          {claim_blocks, ctx->d_why_blocks, why && claim_blocks ? (size_t)n_claim * 4 : 0}};
     if ((rc = reserve_out(ctx, outs))) return rc;
     Staging s;
     s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
@@ -1948,6 +1964,19 @@ int dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
     Prof prof(ctx);
     if ((rc = launch_running_lists(ctx, a, prof, false))) return rc;
     const PreShard whole{0u, ctx->n_node, n_pair, 0u, nullptr, nullptr};   // every node: the walk index is the pair index
+    if (why) {
+        if (claim_blocks && n_claim) CU(cudaMemsetAsync(ctx->d_why_blocks, 0, (size_t)n_claim * 4, ctx->stream));
+        a.why = ctx->d_why; a.why_claim = ctx->d_why_claim;
+        if ((rc = launch_preempt_pairs(ctx, a, whole, true))) return rc;
+        if (pod_why || claim_blocks) {
+            const WhyTally t{ctx->d_why, ctx->d_why_claim, dense ? nullptr : ctx->d_cand_off, n_pod, ctx->n_node,
+                             pod_why ? ctx->d_why_pod : nullptr, claim_blocks ? ctx->d_why_blocks : nullptr};
+            k_why_tally<<<n_pod / 8 + 1, 256, 0, ctx->stream>>>(t);
+            ctx->launches += 1;
+        }
+        prof.mark();
+        return read_back(ctx, "preemption reasons kernels", 1, outs);
+    }
     if ((rc = launch_preempt_pairs(ctx, a, whole))) return rc;
     cudaStream_t st = ctx->stream;
     k_pre_choose<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a);
@@ -1958,6 +1987,28 @@ int dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
     }
     prof.mark();
     return read_back(ctx, "preemption kernels", 1, outs);
+}
+}  // namespace
+
+int dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, const int32_t* prio,
+                          uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, const dra_running_pods* running,
+                          const dra_disruption_budgets* budgets, uint8_t* pair_status, uint32_t* pair_victims,
+                          uint32_t* pair_violations, uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
+                          uint32_t* pod_violations, uint32_t* victims, uint32_t max_victims, uint32_t flags) {
+    return preempt_call(ctx, "dra_preempt_pdb_batch", claims, n_claim, pod_off, prio, n_pod, cand_nodes, cand_off, running, budgets,
+                        pair_status, pair_victims, pair_violations, pod_node, pod_status, n_victims, pod_violations, victims,
+                        max_victims, false, nullptr, nullptr, nullptr, nullptr, flags);
+}
+
+// Why preemption judged each node as it did (spec §19): dra_preempt_batch's pairs, each with its status, reason and
+// blocking claim.  Budgets change no status and no reason, so the call takes none.
+int dra_preempt_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, const int32_t* prio,
+                          uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, const dra_running_pods* running,
+                          uint8_t* pair_status, uint8_t* pair_why, uint32_t* pair_claim, uint32_t* pod_why, uint32_t* claim_blocks,
+                          uint32_t flags) {
+    return preempt_call(ctx, "dra_preempt_why_batch", claims, n_claim, pod_off, prio, n_pod, cand_nodes, cand_off, running, nullptr,
+                        pair_status, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, true, pair_why, pair_claim,
+                        pod_why, claim_blocks, flags);
 }
 
 int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, const int32_t* prio,
@@ -2025,18 +2076,21 @@ int dra_pod_capacity_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n
 // whose fault gates the walk, so a rejected call writes no inventory word.  Running lists as in dra_preempt_batch (their
 // offsets kept aside, since the visit lists reuse the sort's buffers), visit lists as in dra_place_pods_batch, then one
 // persistent cooperative launch; the outputs are copied back after ONE synchronise and reach the caller only without a
-// fault.
-int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off,
-                            const int32_t* prio, uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off,
-                            const dra_running_pods* running, const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
-                            uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, uint32_t flags) {
+// fault.  With why (spec §19, dra_preempt_place_why_batch) the walk is the reasons instantiation, k_pp_why_prep writes the
+// pairs no walk reaches, and k_why_tally sums the records.
+namespace {
+int preempt_place_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off,
+                       const int32_t* prio, uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off,
+                       const dra_running_pods* running, const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
+                       uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, bool why, uint8_t* pair_status,
+                       uint8_t* pair_why, uint32_t* pair_claim, uint32_t* pod_why, uint32_t* claim_blocks, uint32_t flags) {
     if (!ctx || !pod_off || !running || !running->pod_off || (n_claim && (!claims || !out)) ||
         (n_pod && (!prio || !pod_node || !pod_status)))
         return DRA_E_INVAL;
     const dra_running_pods& R = *running;
     if ((R.n_claim && !R.claims) || (R.n_pod && (!R.prio || !evicted_by)) || (R.n_out && !R.out)) return DRA_E_INVAL;
     QUIESCE();
-    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "dra_preempt_place_batch: unknown flags 0x%x", flags);
+    if (flags & ~DRA_F_EXHAUSTIVE) return fail(ctx, DRA_E_INVAL, "%s: unknown flags 0x%x", name, flags);
     if (!ctx->d_inv_live) return fail(ctx, DRA_E_STATE, "dra_set_inventory has not been called");
     bool dense; uint32_t n_pair;
     int rc;
@@ -2047,18 +2101,27 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     if ((rc = check_slots(ctx, claims, n_claim, out_off, n_out, true)) ||
         (rc = check_sortable(ctx, n_pod ? R.n_pod : 0)) ||
         (rc = check_sortable(ctx, n_pod && !dense ? n_pair : 0))) return rc;
-    ctx->chain = DRA_K_PREEMPT_PLACE; ctx->chain_tile = 0;
+    if (why && n_pair && !pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+    ctx->chain = why ? DRA_K_PREEMPT_PLACE | DRA_K_PLACE_WHY : DRA_K_PREEMPT_PLACE; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
-    if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "dra_preempt_place_batch needs cooperative launches, which this device does not offer");
+    if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "%s needs cooperative launches, which this device does not offer", name);
     CU(cudaSetDevice(ctx->device));
     if ((rc = ensure_batch(ctx, std::max(std::max(n_claim, R.n_pod), n_pair), n_out, true))) return rc;
     if ((rc = upload_table(ctx))) return rc;
     if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
         (!dense && (rc = grow_set(ctx, ctx->cap_pairs, (size_t)n_pair + 64, ctx->d_cand_nodes, ctx->d_pair_pod))) ||
         (rc = pp_buffers(ctx, n_pod, n_pair, R.n_pod))) return rc;
+    if (why && ((rc = grow_set(ctx, ctx->cap_why_pairs, (size_t)n_pair + 8, ctx->d_why, ctx->d_why_claim)) ||
+                (rc = grow_set(ctx, ctx->cap_why_pods, (size_t)n_pod * DRA_WHY_N + 8, ctx->d_why_pod)) ||
+                (rc = grow_set(ctx, ctx->cap_why_claims, (size_t)n_claim + 8, ctx->d_why_blocks)))) return rc;
     const size_t rb = (size_t)n_out * 8;
     const Outputs outs = {{out, ctx->d_out, rb}, {pod_node, ctx->d_pre_node, (size_t)n_pod * 4}, {pod_status, ctx->d_pre_pst, n_pod},
-                          {evicted_by, ctx->d_pp_evicted, (size_t)R.n_pod * 4}};
+                          {evicted_by, ctx->d_pp_evicted, (size_t)R.n_pod * 4},
+                          {pair_status, ctx->d_pre_pairst, why && pair_status ? (size_t)n_pair : 0},
+                          {pair_why, ctx->d_why, why ? (size_t)n_pair : 0},
+                          {pair_claim, ctx->d_why_claim, why && pair_claim ? (size_t)n_pair * 4 : 0},
+                          {pod_why, ctx->d_why_pod, why && pod_why ? (size_t)n_pod * DRA_WHY_N * 4 : 0},
+                          {claim_blocks, ctx->d_why_blocks, why && claim_blocks ? (size_t)n_claim * 4 : 0}};
     if ((rc = reserve_out(ctx, outs))) return rc;
     Staging s;
     s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
@@ -2076,9 +2139,11 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)ctx->n_node + 1) * 4, st));
     CU(cudaMemsetAsync(ctx->d_pp_judged, 0, ((size_t)ctx->n_node + 1) * 4, st));
     if (R.n_pod) CU(cudaMemsetAsync(ctx->d_pp_evicted, 0xFF, (size_t)R.n_pod * 4, st));
+    if (why && claim_blocks && n_claim) CU(cudaMemsetAsync(ctx->d_why_blocks, 0, (size_t)n_claim * 4, st));
 
     PreArgs a = pre_args(ctx, ctx->d_claims, ctx->d_pod_off, (const int32_t*)ctx->d_pre_prio, n_pod, dense ? nullptr : ctx->d_cand_nodes,
                          dense ? nullptr : ctx->d_cand_off, n_pair, Rd, ctx->d_inv_live, flags);
+    if (why) { a.pair_status = pair_status ? ctx->d_pre_pairst : nullptr; a.why = ctx->d_why; a.why_claim = ctx->d_why_claim; }
     Prof prof(ctx);
     if ((rc = launch_running_lists(ctx, a, prof, true))) return rc;
     // the visit lists (§13)
@@ -2093,16 +2158,54 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
     PpArgs pp{ctx->d_pp_pending, ctx->d_pp_evicted, ctx->d_pp_judged};
     k_pp_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, pl, pp);
     ctx->launches += 1;
+    if (why) {
+        k_pp_why_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, st>>>(a, pl);
+        ctx->launches += 1;
+    }
     // A candidate form with no pair sorts nothing, so the visit lists are zeroed instead: the walk must not read the
     // offsets an earlier call's sort left in d_claim_off (an Allocate's claims by node), as lists of this call's pairs
     if (!dense && !n_pair) CU(cudaMemsetAsync(ctx->d_claim_off, 0, ((size_t)ctx->n_node + 2) * 4, st));
     if (!dense && n_pair &&
         (rc = launch_sort(ctx, ctx->d_podrec, n_pair, nullptr, nullptr, 0, 0, prof, ctx->d_inv_live, LA_NONE, ctx->n_node, ctx->d_node_off)))
         return rc;
-    if ((rc = launch_walk(ctx, ctx->pp_occ, "k_pods_preempt_place", k_pods_preempt_place<4>, a, pl, pp))) return rc;
-    ctx->chain |= DRA_K_PREEMPT_PLACE;
+    if (!why) {
+        if ((rc = launch_walk(ctx, ctx->pp_occ, "k_pods_preempt_place", k_pods_preempt_place<4>, a, pl, pp))) return rc;
+    } else {
+        // (sized by its own occupancy: its registers are not k_pods_preempt_place<4>'s)
+        if ((rc = launch_walk(ctx, ctx->pp_why_occ, "k_pods_preempt_place<4, true>", k_pods_preempt_place<4, true>, a, pl, pp)))
+            return rc;
+        if (pod_why || claim_blocks) {
+            const WhyTally t{ctx->d_why, ctx->d_why_claim, dense ? nullptr : ctx->d_cand_off, n_pod, ctx->n_node,
+                             pod_why ? ctx->d_why_pod : nullptr, claim_blocks ? ctx->d_why_blocks : nullptr};
+            k_why_tally<<<n_pod / 8 + 1, 256, 0, st>>>(t);
+            ctx->launches += 1;
+        }
+    }
     prof.mark();
-    return read_back(ctx, "preempt-and-place kernels", 1, outs);
+    return read_back(ctx, why ? "preempt-and-place reasons kernels" : "preempt-and-place kernels", 1, outs);
+}
+}  // namespace
+
+int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off,
+                            const int32_t* prio, uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off,
+                            const dra_running_pods* running, const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
+                            uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, uint32_t flags) {
+    return preempt_place_call(ctx, "dra_preempt_place_batch", claims, n_claim, pod_off, prio, n_pod, cand_nodes, cand_off, running,
+                              out_off, out, n_out, pod_node, pod_status, evicted_by, false, nullptr, nullptr, nullptr, nullptr,
+                              nullptr, flags);
+}
+
+// Why preemption judged each node as it did, in preempt and place (spec §19): dra_preempt_place_batch's call, every pair
+// answered on the state its pod met
+int dra_preempt_place_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off,
+                                const int32_t* prio, uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off,
+                                const dra_running_pods* running, const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
+                                uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, uint8_t* pair_status,
+                                uint8_t* pair_why, uint32_t* pair_claim, uint32_t* pod_why, uint32_t* claim_blocks,
+                                uint32_t flags) {
+    return preempt_place_call(ctx, "dra_preempt_place_why_batch", claims, n_claim, pod_off, prio, n_pod, cand_nodes, cand_off,
+                              running, out_off, out, n_out, pod_node, pod_status, evicted_by, true, pair_status, pair_why,
+                              pair_claim, pod_why, claim_blocks, flags);
 }
 
 // Deallocate on one inventory (spec §9).  Every claim's slot range is checked here, with the slots k_dealloc counts, before

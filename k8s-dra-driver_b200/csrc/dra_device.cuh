@@ -3914,6 +3914,8 @@ struct PreArgs {
     uint32_t pdb;                 // non-zero: budgets in force (n_pdb > 0, running pods): vprev is built and read
     uint32_t* vprev;              // [rn_pod] per vlist position, the previous position of its node's list with the same budget
     uint32_t* pair_viol; uint32_t* pod_viol;                        // caller's violation outputs (may be nullptr)
+    // reasons (spec §19; dra_preempt_why_batch, dra_preempt_place_why_batch), nullptr without them
+    uint8_t* why; uint32_t* why_claim;                              // per pair: reason, blocking claim
 };
 
 // psum[k].x and the sharded call's pair records hold status | violations << PRE_VSHIFT (a status takes 3 bits; the
@@ -4056,10 +4058,17 @@ __device__ __forceinline__ bool pod_invalid(const uint4* claims, const uint32_t 
 // LIVE (spec §15, k_pods_preempt_place): the node as it stands is *live, the walk's working state, instead of a.inv; `row` is
 // then the call's evicted-by word per running pod: running pods whose word is set are gone and left out of V, and with
 // skip_first each victim's word is set to `pod`.  Lane gbase writes the words and its reading decides for the group.
-template <int W, bool LIVE = false>
+// WHY (spec §19): *why gets the pair's reason | blocking position << 8 (pod_eval's WHY form; 0 for FITS): for EVICT the
+// failing evaluation on S, for NO / SEARCH_LIMIT the one on S'.  NO_NODE and more than 32 claims leave it to the caller.
+// Every evaluation runs on the reasons' own pod_eval copy (OWN 4: the §14 reasons kernel, 5: the §15 reasons walk), so
+// the existing callers of the shared copies keep their registers.  Without LIVE (the §14 reasons call, which returns no
+// victims) the pair stops once EVICT is known: no reprieve.
+template <int W, bool LIVE = false, bool WHY = false>
 __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __restrict__ tbl_s, const uint32_t pod,
                                            const uint32_t node, const uint32_t lane, const uint32_t gmask, const uint32_t gbase,
-                                           const bool skip_first, uint32_t* row, const Lane* live = nullptr) {
+                                           const bool skip_first, uint32_t* row, const Lane* live = nullptr,
+                                           uint32_t* why = nullptr) {
+    constexpr int OWN = WHY ? (LIVE ? 5 : 4) : 0;
     PreSum s{DRA_PRE_NO, 0u, 0x80000000u, 0xFFFFFFFFu, 0ull, 0u};
     if (node >= a.n_node) return s;
     const uint32_t c0 = __ldg(&a.pod_off[pod]), cnt = __ldg(&a.pod_off[pod + 1]) - c0;
@@ -4077,10 +4086,13 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
     Lane Lt;                                                          // ONE copy handed to every pod_eval: one stack slot
     if (!skip_first) {
         Lt = L;
-        st1 = pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr);
+        st1 = pod_eval<W, WHY, OWN>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr);
+        if constexpr (WHY) *why = st1;
         if (st1 == 0) { s.st = DRA_PRE_FITS; return s; }
         if (pod_invalid<W>(a.claims + c0, cnt, a.sel.n_sel, true, gl, gmask)) { s.st = DRA_PRE_INVALID; return s; }
     }
+    // (WHY: a failed evaluation's reason is SEARCH_LIMIT exactly when its status is)
+    const auto limited = [](const uint32_t st) { return (WHY ? st & 0xFFu : st) == DRA_ST_SEARCH_LIMIT; };
     // V: the tail of the node's list below the pod's priority (the list is by priority descending)
     const int32_t P = __ldg(&a.prio[pod]);
     uint32_t v0 = __ldcg(&a.list_off[node]), hi = __ldcg(&a.list_off[node + 1]);
@@ -4089,20 +4101,25 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
         const uint32_t mid = (v0 + hi) >> 1;
         if ((int32_t)__ldcg(&a.vlist[mid]).w >= P) v0 = mid + 1; else hi = mid;
     }
-    if (v0 == v1) { s.st = st1 == DRA_ST_SEARCH_LIMIT ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO; return s; }   // S' = S
+    if (v0 == v1) { s.st = limited(st1) ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO; return s; }   // S' = S
     bool any = !LIVE;
     for (uint32_t v = v0; v < v1; ++v) {
         const uint4 r = __ldcg(&a.vlist[v]);
         if constexpr (LIVE) { if (__shfl_sync(gmask, __ldcg(&row[r.y]), gbase) != DRA_GPU_NONE) continue; any = true; }
         pre_apply(L, a, r, gidx, false);
     }
-    if (!any) { s.st = st1 == DRA_ST_SEARCH_LIMIT ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO; return s; }   // every member gone: S' = S
+    if (!any) { s.st = limited(st1) ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO; return s; }   // every member gone: S' = S
     {
         Lt = L;
-        const uint32_t st = pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr);
-        if (st != 0) { s.st = st == DRA_ST_SEARCH_LIMIT ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO; return s; }
+        const uint32_t st = pod_eval<W, WHY, OWN>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr);
+        if (st != 0) {
+            if constexpr (WHY) *why = st;
+            s.st = limited(st) ? DRA_PRE_SEARCH_LIMIT : DRA_PRE_NO;
+            return s;
+        }
     }
     s.st = DRA_PRE_EVICT;
+    if constexpr (WHY && !LIVE) return s;
     if constexpr (!LIVE) {
         if (a.pdb) {
             // Budgets: the reprieve over V's violating members first, then over the others, each phase in V order.
@@ -4111,7 +4128,7 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
                 Lane Lk = S;
                 pre_apply(Lk, a, r, gidx, true);
                 Lt = Lk;
-                if (pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr) != 0) return false;
+                if (pod_eval<W, WHY, OWN>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr) != 0) return false;
                 S = Lk;
                 return true;
             };
@@ -4154,7 +4171,7 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
         Lane Lk = L;
         pre_apply(Lk, a, r, gidx, true);
         Lt = Lk;
-        if (pod_eval<W>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr) == 0) { L = Lk; continue; }
+        if (pod_eval<W, WHY, OWN>(Lt, lane, gmask, gbase, g0, tbl_s, get, cnt, a.sel, exh, true, nullptr) == 0) { L = Lk; continue; }
         if (s.count == 0) { s.hi = r.w; s.hi_idx = r.y; }            // V order: the first victim has the highest priority
         s.sum += (unsigned long long)((long long)(int32_t)r.w + 2147483648ll);
         if constexpr (LIVE) { if (skip_first && lane == gbase) row[r.y] = pod; }
@@ -4167,7 +4184,9 @@ __device__ __forceinline__ PreSum pre_pair(const PreArgs& a, const uint32_t* __r
 // W lanes per (pod, candidate) pair, 32/W pairs per warp, in k_unsuitable's layout; pairs are taken from a counter, since
 // a pair costs from one evaluation to |V| + 2 of them.  The pairs of s's node window (pair_decode); a pair naming no node
 // is judged NO, as k_pre_choose reads every pair.
-template <int WPC, int W>
+// WHY (spec §19, dra_preempt_why_batch; single inventory): each pair's status, reason and blocking claim, and nothing else:
+// no summary, since nothing is chosen, and no reprieve (pre_pair stops at EVICT).
+template <int WPC, int W, bool WHY = false>
 __global__ void __launch_bounds__(WPC * 32, 2)
 k_pods_preempt(const PreArgs a, const PreShard s) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
@@ -4182,6 +4201,19 @@ k_pods_preempt(const PreArgs a, const PreShard s) {
         if (walk >= s.n_walk) continue;                                  // whole group skips together
         uint32_t pod, node, pair;
         if (!pair_decode(walk, s.node_lo, s.n_win, a.n_node, a.cand_off, a.cand_nodes, a.pair_pod, pod, node, pair)) continue;
+        if constexpr (WHY) {
+            uint32_t why = 0;
+            const PreSum r = pre_pair<W, false, true>(a, tbl_s, pod, node, lane, gmask, gbase, false, nullptr, nullptr, &why);
+            if (lane == gbase) {
+                const uint32_t c0 = __ldg(&a.pod_off[pod]);
+                const bool unjudged = node >= a.n_node || __ldg(&a.pod_off[pod + 1]) - c0 > DRA_MAX_POD;
+                const uint32_t rs = node >= a.n_node ? DRA_WHY_NO_NODE : unjudged ? DRA_ST_INVALID : why & 0xFFu;
+                if (a.pair_status) a.pair_status[pair] = (uint8_t)r.st;
+                a.why[pair] = (uint8_t)rs;
+                a.why_claim[pair] = unjudged || why == 0 ? DRA_WHY_CLAIM_NONE : c0 + (why >> 8);
+            }
+            continue;
+        }
         const PreSum r = pre_pair<W>(a, tbl_s, pod, node, lane, gmask, gbase, false, nullptr);
         if (lane == gbase) {
             const uint32_t nv = r.st == DRA_PRE_EVICT ? r.count : 0u;   // (r.viol is 0 unless EVICT)
@@ -4377,10 +4409,48 @@ k_pp_prep(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
     pp_prep_pod(a, pl, pp, p, lane);
 }
 
+// Warp per pod, after k_pp_prep (spec §19, dra_preempt_place_why_batch): the status, reason and blocking claim of pod p's pairs
+// that no walk judges.  A candidate naming no node is NO / NO_NODE.  At the others: a pod invalid in the call's slot mode
+// is INVALID, at its lowest invalid claim (none for more than 32 claims), and an empty pod FITS / OK.  Dense form: n_node
+// pairs per pod, every one naming a node.
+__global__ void __launch_bounds__(256)
+k_pp_why_prep(const PreArgs a, const PlaceArgs pl) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (p >= pl.n_pod) return;
+    const uint32_t c0 = __ldg(&pl.pod_off[p]), cnt = __ldg(&pl.pod_off[p + 1]) - c0;
+    uint32_t bad = DRA_WHY_CLAIM_NONE;                                   // the lowest invalid claim
+    if (cnt <= DRA_MAX_POD) {
+        const bool have_off = pl.out_off != nullptr;
+        bool inv = false;
+        if (lane < cnt) {
+            const uint4 c = __ldg(&pl.claims[c0 + lane]);
+            const uint32_t kind = c.x & 0xFFu, prof = (c.x >> 8) & 0xFFu, count = c.x >> 16;
+            inv = claim_invalid(kind, prof, count, have_off) || claim_sel(kind, c.z, c.w) > a.sel.n_sel;
+        }
+        const uint32_t b = __ballot_sync(FULLMASK, inv);
+        if (b) bad = c0 + (uint32_t)__ffs(b) - 1u;
+    }
+    const bool judged = cnt != 0 && cnt <= DRA_MAX_POD && bad == DRA_WHY_CLAIM_NONE;
+    const uint8_t st = (uint8_t)(cnt ? DRA_PRE_INVALID : DRA_PRE_FITS), r = (uint8_t)(cnt ? DRA_ST_INVALID : DRA_ST_OK);
+    const uint32_t k0 = pl.cand_off ? __ldg(&pl.cand_off[p]) : p * pl.n_node;   // (n_pod * n_node < 2^32: checked by the host)
+    const uint32_t k1 = pl.cand_off ? __ldg(&pl.cand_off[p + 1]) : k0 + pl.n_node;
+    for (uint32_t k = k0 + lane; k < k1; k += 32) {
+        const bool named = !pl.cand_off || __ldg(&pl.cand_nodes[k]) < pl.n_node;
+        if (named && judged) continue;
+        if (a.pair_status) a.pair_status[k] = named ? st : (uint8_t)DRA_PRE_NO;
+        a.why[k] = named ? r : (uint8_t)DRA_WHY_NO_NODE;
+        a.why_claim[k] = named ? bad : DRA_WHY_CLAIM_NONE;
+    }
+}
+
 // Persistent: every CTA resident (cooperative launch); warp w owns nodes w, w + warps, ... and cycles over them.  Minimum
 // one CTA per SM in the bounds: the walk's state beside pre_pair's then fits in registers without spilling (the stack
 // holds only the two Lane copies handed to pod_eval).
-template <int WPC>
+// WHY (spec §19, dra_preempt_place_why_batch): a judgement also writes its pair's status, reason and blocking claim at every
+// list position it covers; k_pp_why_prep writes the pairs no walk reaches.  Every evaluation, the apply's included, runs on
+// the reasons' own pod_eval copy, so that k_pods_preempt_place<4> keeps its registers.  Placement and eviction are §15's.
+template <int WPC, bool WHY = false>
 __global__ void __launch_bounds__(WPC * 32, 1)
 k_pods_preempt_place(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
     __shared__ uint32_t tbl_s[DRA_MAX_MODELS * DRA_MAX_PROFILES];
@@ -4423,7 +4493,9 @@ k_pods_preempt_place(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
                 if (sf == PP_OPEN) {
                     if (__shfl_sync(FULLMASK, __ldcg(&pp.judged[node]), 0) == qf + 1u) break;   // judged, undecided: wait
                     // judge q here once, for each of its consecutive entries
-                    const PreSum r = pre_pair<32, true>(a, tbl_s, qf, node, lane, FULLMASK, 0u, false, pp.evicted_by, &L);
+                    uint32_t why = 0;
+                    const PreSum r = pre_pair<32, true, WHY>(a, tbl_s, qf, node, lane, FULLMASK, 0u, false, pp.evicted_by, &L,
+                                                             WHY ? &why : nullptr);
                     const uint32_t kb = dense ? qf * pl.n_node : __ldg(&pl.cand_off[qf]);
                     uint32_t n_here = 0;
                     for (uint32_t e2 = cur; e2 < l1; ++e2) {
@@ -4431,6 +4503,13 @@ k_pods_preempt_place(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
                         if (!dense) { const uint4 r2 = __ldcg(&pl.sorted[e2]); if (r2.x != qf) break; pos = r2.z; }
                         else if (e2 != cur) break;
                         if (lane == 0) { a.psum[kb + pos] = make_uint4(r.st, r.count, r.hi, r.hi_idx); a.psum64[kb + pos] = r.sum; }
+                        if constexpr (WHY) {
+                            if (lane == 0) {
+                                if (a.pair_status) a.pair_status[kb + pos] = (uint8_t)r.st;
+                                a.why[kb + pos] = (uint8_t)(why & 0xFFu);
+                                a.why_claim[kb + pos] = why == 0 ? DRA_WHY_CLAIM_NONE : __ldg(&pl.pod_off[qf]) + (why >> 8);
+                            }
+                        }
                         ++n_here;
                     }
                     __threadfence();
@@ -4467,7 +4546,7 @@ k_pods_preempt_place(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
                 // q is decided, for this entry of this node: apply it
                 const uint32_t c0 = __ldg(&pl.pod_off[qf]), cnt = __ldg(&pl.pod_off[qf + 1]) - c0;
                 if (sf & PP_EVICT) {
-                    (void)pre_pair<32, true>(a, tbl_s, qf, node, lane, FULLMASK, 0u, true, pp.evicted_by, &L);   // marks the victims
+                    (void)pre_pair<32, true, WHY>(a, tbl_s, qf, node, lane, FULLMASK, 0u, true, pp.evicted_by, &L);   // marks the victims
                     __syncwarp();
                     const uint32_t gidx = lane < ng ? g0 + lane : DRA_GPU_NONE;
                     const uint32_t v0 = __ldcg(&a.list_off[node]), v1 = __ldcg(&a.list_off[node + 1]);
@@ -4479,7 +4558,8 @@ k_pods_preempt_place(const PreArgs a, const PlaceArgs pl, const PpArgs pp) {
                 {
                     const PodGet get{pl.claims + c0, have_off ? pl.out_off + c0 : nullptr, c0};
                     Lane Lt = L;
-                    if (pod_eval<32>(Lt, lane, FULLMASK, 0, g0, tbl_s, get, cnt, pl.sel, pl.exhaustive != 0, have_off, pl.out) == 0) L = Lt;
+                    if (pod_eval<32, WHY, WHY ? 5 : 0>(Lt, lane, FULLMASK, 0, g0, tbl_s, get, cnt, pl.sel, pl.exhaustive != 0, have_off,
+                                                       pl.out) == 0) L = Lt;
                 }
                 dirty = true;
                 __threadfence();
