@@ -199,6 +199,20 @@ def _placed_n_out(claims, out_off) -> int:
     return int(R.claim_slots(placed, 1).sum())
 
 
+def _why_arrays(n_pair: int, n_pod: int, n_claim: int, want_claims: bool, want_tallies: bool) -> tuple:
+    """The four reason outputs of a reasons call (spec §17–§19), each at least one entry long: (pair_why, pair_claim,
+    pod_why, claim_blocks), pair_claim only with want_claims and the two tallies only with want_tallies (else None)."""
+    return (np.zeros(max(n_pair, 1), dtype=np.uint8),
+            np.zeros(max(n_pair, 1), dtype=np.uint32) if want_claims else None,
+            np.zeros((max(n_pod, 1), WHY_N), dtype=np.uint32) if want_tallies else None,
+            np.zeros(max(n_claim, 1), dtype=np.uint32) if want_tallies else None)
+
+
+def _why_results(why: tuple, n_pair: int, n_pod: int, n_claim: int) -> tuple:
+    """_why_arrays' outputs cut to the call's pairs, pods and claims (None stays None)."""
+    return tuple(None if a is None else a[:n] for a, n in zip(why, (n_pair, n_pair, n_pod, n_claim)))
+
+
 def _ptr(a):
     if a is None:
         return None
@@ -388,15 +402,10 @@ class Context:
         n_pair = n_pod * self.n_node if co is None else int(co[-1])
         out = np.zeros(n_out, dtype=R.OUT_DTYPE)
         pod_node = np.zeros(max(n_pod, 1), dtype=np.uint32)
-        why = np.zeros(max(n_pair, 1), dtype=np.uint8)
-        blk = np.zeros(max(n_pair, 1), dtype=np.uint32) if want_claims else None
-        pod_why = np.zeros((max(n_pod, 1), WHY_N), dtype=np.uint32) if want_tallies else None
-        blocks = np.zeros(max(len(c), 1), dtype=np.uint32) if want_tallies else None
+        why = _why_arrays(n_pair, n_pod, len(c), want_claims, want_tallies)
         self._check(self._lib.dra_place_pods_why_batch(self._h, _ptr(c), len(c), _ptr(po), n_pod, _ptr(cn), _ptr(co),
-                                                       _ptr(oo), _ptr(out), n_out, _ptr(pod_node), _ptr(why), _ptr(blk),
-                                                       _ptr(pod_why), _ptr(blocks), flags))
-        return (out, pod_node[:n_pod], why[:n_pair], None if blk is None else blk[:n_pair],
-                None if pod_why is None else pod_why[:n_pod], None if blocks is None else blocks[:len(c)])
+                                                       _ptr(oo), _ptr(out), n_out, _ptr(pod_node), *map(_ptr, why), flags))
+        return (out, pod_node[:n_pod]) + _why_results(why, n_pair, n_pod, len(c))
 
     def unsuitable(self, claims, pod_off, cand_nodes=None, cand_off=None, flags: int = 0) -> np.ndarray:
         """cand_nodes/cand_off None = dense form: every pod against every node (bit k = pod * n_node + node).
@@ -516,15 +525,10 @@ class Context:
         cn, co = _cands(cand_nodes, cand_off)
         n_pair = n_pod * self.n_node if co is None else int(co[-1])
         pair_status = np.zeros(max(n_pair, 1), dtype=np.uint8)
-        why = np.zeros(max(n_pair, 1), dtype=np.uint8)
-        blk = np.zeros(max(n_pair, 1), dtype=np.uint32) if want_claims else None
-        pod_why = np.zeros((max(n_pod, 1), WHY_N), dtype=np.uint32) if want_tallies else None
-        blocks = np.zeros(max(len(c), 1), dtype=np.uint32) if want_tallies else None
+        why = _why_arrays(n_pair, n_pod, len(c), want_claims, want_tallies)
         self._check(self._lib.dra_preempt_why_batch(self._h, _ptr(c), len(c), _ptr(po), _ptr(pr), n_pod, _ptr(cn), _ptr(co),
-                                                    C.byref(run), _ptr(pair_status), _ptr(why), _ptr(blk), _ptr(pod_why),
-                                                    _ptr(blocks), flags))
-        return (pair_status[:n_pair], why[:n_pair], None if blk is None else blk[:n_pair],
-                None if pod_why is None else pod_why[:n_pod], None if blocks is None else blocks[:len(c)])
+                                                    C.byref(run), _ptr(pair_status), *map(_ptr, why), flags))
+        return (pair_status[:n_pair],) + _why_results(why, n_pair, n_pod, len(c))
 
     def preempt_place_why(self, claims, pod_off, prio, run_claims, run_pod_off, run_prio, run_out, run_out_off=None,
                           cand_nodes=None, cand_off=None, out_off=None, n_out=None, flags: int = 0,
@@ -549,17 +553,12 @@ class Context:
         pod_status = np.zeros(max(n_pod, 1), dtype=np.uint8)
         evicted_by = np.zeros(max(run.n_pod, 1), dtype=np.uint32)
         pair_status = np.zeros(max(n_pair, 1), dtype=np.uint8)
-        why = np.zeros(max(n_pair, 1), dtype=np.uint8)
-        blk = np.zeros(max(n_pair, 1), dtype=np.uint32) if want_claims else None
-        pod_why = np.zeros((max(n_pod, 1), WHY_N), dtype=np.uint32) if want_tallies else None
-        blocks = np.zeros(max(len(c), 1), dtype=np.uint32) if want_tallies else None
+        why = _why_arrays(n_pair, n_pod, len(c), want_claims, want_tallies)
         self._check(self._lib.dra_preempt_place_why_batch(
             self._h, _ptr(c), len(c), _ptr(po), _ptr(pr), n_pod, _ptr(cn), _ptr(co), C.byref(run), _ptr(oo), _ptr(out), n_out,
-            _ptr(pod_node), _ptr(pod_status), _ptr(evicted_by), _ptr(pair_status), _ptr(why), _ptr(blk), _ptr(pod_why),
-            _ptr(blocks), flags))
-        return (out[:n_out], pod_node[:n_pod], pod_status[:n_pod], evicted_by[:run.n_pod], pair_status[:n_pair],
-                why[:n_pair], None if blk is None else blk[:n_pair], None if pod_why is None else pod_why[:n_pod],
-                None if blocks is None else blocks[:len(c)])
+            _ptr(pod_node), _ptr(pod_status), _ptr(evicted_by), _ptr(pair_status), *map(_ptr, why), flags))
+        return ((out[:n_out], pod_node[:n_pod], pod_status[:n_pod], evicted_by[:run.n_pod], pair_status[:n_pair])
+                + _why_results(why, n_pair, n_pod, len(c)))
 
     def pod_capacity(self, claims, pod_off, cand_nodes=None, cand_off=None, max_copies: int = 64, exhaustive: bool = False,
                      want_stop: bool = True, want_totals: bool = True):
@@ -596,15 +595,10 @@ class Context:
         n_pod = len(po) - 1
         cn, co = _cands(cand_nodes, cand_off)
         n_pair = n_pod * self.n_node if co is None else int(co[-1])
-        why = np.zeros(max(n_pair, 1), dtype=np.uint8)
-        blk = np.zeros(max(n_pair, 1), dtype=np.uint32) if want_claims else None
-        pod_why = np.zeros((max(n_pod, 1), WHY_N), dtype=np.uint32) if want_tallies else None
-        blocks = np.zeros(max(len(c), 1), dtype=np.uint32) if want_tallies else None
+        why = _why_arrays(n_pair, n_pod, len(c), want_claims, want_tallies)
         self._check(self._lib.dra_unsuitable_why_batch(self._h, _ptr(c), len(c), _ptr(po), n_pod, _ptr(cn), _ptr(co),
-                                                       _ptr(why), _ptr(blk), _ptr(pod_why), _ptr(blocks),
-                                                       F_EXHAUSTIVE if exhaustive else 0))
-        return (why[:n_pair], None if blk is None else blk[:n_pair], None if pod_why is None else pod_why[:n_pod],
-                None if blocks is None else blocks[:len(c)])
+                                                       *map(_ptr, why), F_EXHAUSTIVE if exhaustive else 0))
+        return _why_results(why, n_pair, n_pod, len(c))
 
     def deallocate(self, claims, out, out_off=None):
         """Spec §9: release the OK records `out` of `claims` (slots counted as Allocate counts them).  A claim whose slot

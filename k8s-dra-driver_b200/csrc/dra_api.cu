@@ -837,21 +837,34 @@ void expand_pairs(uint32_t* pair_pod, const uint32_t* cand_off, uint32_t n_pod) 
 
 // One output of a synchronous call: bytes from the device at src to the caller's dst
 struct ReadBack { void* dst; const void* src; size_t bytes; };
-using Outputs = std::initializer_list<ReadBack>;
 
-size_t out_bytes(Outputs outs) {
-    size_t total = 0;
-    for (const ReadBack& o : outs) total += al16(o.bytes);
-    return total;
-}
+// The outputs of a synchronous call.  A fixed array like Staging: an output beyond CAP is not kept, and reserve_out
+// refuses the call.
+struct Outputs {
+    static constexpr int CAP = 12;
+    ReadBack out[CAP];
+    int n = 0;
+    bool overflow = false;
+    Outputs(std::initializer_list<ReadBack> l = {}) { for (const ReadBack& o : l) add(o.dst, o.src, o.bytes); }
+    void add(void* dst, const void* src, size_t bytes) {
+        if (n < CAP) out[n++] = ReadBack{dst, src, bytes};
+        else overflow = true;
+    }
+    const ReadBack* begin() const { return out; }
+    const ReadBack* end() const { return out + n; }
+    size_t bytes() const { size_t t = 0; for (const ReadBack& o : *this) t += al16(o.bytes); return t; }
+};
 
 // The pinned h_out for outs, grown before the call enqueues anything: a failed allocation leaves the inventory as it was
-int reserve_out(dra_ctx* ctx, Outputs outs) { return grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, out_bytes(outs)); }
+int reserve_out(dra_ctx* ctx, const Outputs& outs) {
+    if (outs.overflow) return fail(ctx, DRA_E_STATE, "more than %d outputs in one call", Outputs::CAP);
+    return grow_pinned(ctx, ctx->h_out, ctx->h_out_cap, outs.bytes());
+}
 
 // The tail of a synchronous call: the outputs into h_out (reserve_out), one synchronise, the launch error as DRA_E_CUDA
 // "<name>: ...", the times of n_marks stages, the device's fault words; the caller's buffers are written only when all passed
-int read_back(dra_ctx* ctx, const char* name, int n_marks, Outputs outs) {
-    if (out_bytes(outs) > ctx->h_out_cap) return fail(ctx, DRA_E_STATE, "%s: outputs not reserved before the launch", name);
+int read_back(dra_ctx* ctx, const char* name, int n_marks, const Outputs& outs) {
+    if (outs.bytes() > ctx->h_out_cap) return fail(ctx, DRA_E_STATE, "%s: outputs not reserved before the launch", name);
     uint8_t* h = ctx->h_out;
     for (const ReadBack& o : outs) {
         if (o.bytes) CU(cudaMemcpyAsync(h, o.src, o.bytes, cudaMemcpyDeviceToHost, ctx->stream));
@@ -925,17 +938,24 @@ int check_sortable(dra_ctx* ctx, uint32_t n_rec) {
     return DRA_OK;
 }
 
-// A persistent walk k over the inventory's nodes (none: no launch): CTAs of 4 warps, one per 4 nodes up to all that can be
-// resident at once (occ per SM, queried once), launched cooperatively so that every one of them is.  Enqueues only.
-template <typename... KA, typename... A>
-int launch_walk(dra_ctx* ctx, int& occ, const char* name, void (*k)(KA...), A&&... args) {
-    if (!ctx->n_node) return DRA_OK;
+// occ: how many CTAs of 4 warps of the walk k can be resident per SM, queried once; none fails
+template <class K>
+int walk_occupancy(dra_ctx* ctx, int& occ, const char* name, K k) {
     if (occ < 0) {
         int nb = 0;
         CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k, 128, 0));
         occ = nb;
     }
     if (occ < 1) return fail(ctx, DRA_E_CUDA, "%s: no CTA can be resident", name);
+    return DRA_OK;
+}
+
+// A persistent walk k over the inventory's nodes (none: no launch): CTAs of 4 warps, one per 4 nodes up to all that can be
+// resident at once (walk_occupancy), launched cooperatively so that every one of them is.  Enqueues only.
+template <typename... KA, typename... A>
+int launch_walk(dra_ctx* ctx, int& occ, const char* name, void (*k)(KA...), A&&... args) {
+    if (!ctx->n_node) return DRA_OK;
+    if (int rc = walk_occupancy(ctx, occ, name, k)) return rc;
     const uint32_t grid = std::max(1u, std::min((ctx->n_node + 3) / 4, (uint32_t)(occ * ctx->n_sm)));
     CU(launch_k(k, dim3(grid), dim3(128), 0, ctx->stream, LA_COOP, std::forward<A>(args)...));
     ctx->launches += 1;
@@ -1045,6 +1065,52 @@ int launch_capacity(dra_ctx* ctx, CapArgs a) {
         k_pods_capacity_sum<<<(a.n_pod + 7) / 8, 256, 0, ctx->stream>>>(a);
         ctx->launches += 1;
     }
+    return DRA_OK;
+}
+
+// The caller's reason outputs of a reasons call (spec §17–§19): pair_why whenever there are pairs, the others when asked
+// for (NULL: not).  Host pointers in the synchronous calls, device pointers in the sharded ones.
+struct WhyOut { uint8_t* pair_why; uint32_t* pair_claim; uint32_t* pod_why; uint32_t* claim_blocks; };
+
+// A reasons call (w; nullptr: the plain call, which answers no pair) with n_why pairs to answer needs pair_why
+int why_check(dra_ctx* ctx, const WhyOut* w, uint32_t n_why) {
+    if (w && n_why && !w->pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+    return DRA_OK;
+}
+
+// n_why: the pairs a place-pods call answers (spec §18; none without w): every pod at every node in the dense form
+int place_why_pairs(dra_ctx* ctx, const WhyOut* w, bool dense, uint32_t n_pod, uint32_t n_pair, uint32_t& n_why) {
+    const uint64_t n = !w ? 0 : dense ? (uint64_t)n_pod * ctx->n_node : n_pair;
+    if (n > 0xFFFFFFFFull) return fail(ctx, DRA_E_INVAL, "%llu (pod, node) pairs: more than %llu", (unsigned long long)n, 0xFFFFFFFFull);
+    n_why = (uint32_t)n;
+    return DRA_OK;
+}
+
+// The device buffers of w's outputs (none without w) for n_why pairs, n_pod pods and n_claim claims, and their
+// read-backs appended to outs: pair_why for every pair, each other output only when asked for
+int why_buffers(dra_ctx* ctx, const WhyOut* w, Outputs& outs, uint32_t n_why, uint32_t n_pod, uint32_t n_claim) {
+    if (!w) return DRA_OK;
+    int rc;
+    if ((rc = grow_set(ctx, ctx->cap_why_pairs, (size_t)n_why + 8, ctx->d_why, ctx->d_why_claim)) ||
+        (rc = grow_set(ctx, ctx->cap_why_pods, (size_t)n_pod * DRA_WHY_N + 8, ctx->d_why_pod)) ||
+        (rc = grow_set(ctx, ctx->cap_why_claims, (size_t)n_claim + 8, ctx->d_why_blocks))) return rc;
+    outs.add(w->pair_why, ctx->d_why, n_why);
+    outs.add(w->pair_claim, ctx->d_why_claim, w->pair_claim ? (size_t)n_why * 4 : 0);
+    outs.add(w->pod_why, ctx->d_why_pod, w->pod_why ? (size_t)n_pod * DRA_WHY_N * 4 : 0);
+    outs.add(w->claim_blocks, ctx->d_why_blocks, w->claim_blocks ? (size_t)n_claim * 4 : 0);
+    return DRA_OK;
+}
+
+// The tallies of w, when pod_why or claim_blocks is asked for: d_why_blocks zeroed (in these calls only k_why_tally writes
+// it, so just before it is soon enough), then k_why_tally over the records the walk wrote.  cand_off: the staged
+// candidates' offsets, nullptr in the dense form.  Enqueues only.
+int launch_why_tally(dra_ctx* ctx, const WhyOut& w, const uint32_t* cand_off, uint32_t n_pod, uint32_t n_claim) {
+    if (!w.pod_why && !w.claim_blocks) return DRA_OK;
+    if (w.claim_blocks && n_claim) CU(cudaMemsetAsync(ctx->d_why_blocks, 0, (size_t)n_claim * 4, ctx->stream));
+    const WhyTally t{ctx->d_why, ctx->d_why_claim, cand_off, n_pod, ctx->n_node, w.pod_why ? ctx->d_why_pod : nullptr,
+                     w.claim_blocks ? ctx->d_why_blocks : nullptr};
+    k_why_tally<<<n_pod / 8 + 1, 256, 0, ctx->stream>>>(t);
+    ctx->launches += 1;
     return DRA_OK;
 }
 
@@ -1662,22 +1728,18 @@ int dra_unsuitable_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t
     int rc;
     if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
         (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, 0xFFFFFFFFu, ctx->n_node, 0xFFFFFFFFull, dense, n_pair))) return rc;
-    if (n_pair && !pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+    const WhyOut w{pair_why, pair_claim, pod_why, claim_blocks};
+    if ((rc = why_check(ctx, &w, n_pair))) return rc;
     ctx->chain = DRA_K_UNSUITABLE_WHY; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     CU(cudaSetDevice(ctx->device));
     if ((rc = ensure_batch(ctx, n_claim, 1, true))) return rc;
     if ((rc = upload_table(ctx))) return rc;
+    Outputs outs;
     if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
         (!dense && (rc = grow_set(ctx, ctx->cap_pairs, (size_t)n_pair + 64, ctx->d_cand_nodes, ctx->d_pair_pod))) ||
-        (rc = grow_set(ctx, ctx->cap_why_pairs, (size_t)n_pair + 8, ctx->d_why, ctx->d_why_claim)) ||
-        (rc = grow_set(ctx, ctx->cap_why_pods, (size_t)n_pod * DRA_WHY_N + 8, ctx->d_why_pod)) ||
-        (rc = grow_set(ctx, ctx->cap_why_claims, (size_t)n_claim + 8, ctx->d_why_blocks))) return rc;
-    const Outputs outs = {{pair_why, ctx->d_why, (size_t)n_pair},
-                          {pair_claim, ctx->d_why_claim, pair_claim ? (size_t)n_pair * 4 : 0},
-                          {pod_why, ctx->d_why_pod, pod_why ? (size_t)n_pod * DRA_WHY_N * 4 : 0},
-                          {claim_blocks, ctx->d_why_blocks, claim_blocks ? (size_t)n_claim * 4 : 0}};
-    if ((rc = reserve_out(ctx, outs))) return rc;
+        (rc = why_buffers(ctx, &w, outs, n_pair, n_pod, n_claim)) ||
+        (rc = reserve_out(ctx, outs))) return rc;
     Staging s;
     s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
     s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
@@ -1687,7 +1749,6 @@ int dra_unsuitable_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t
         s.add(ctx->d_pair_pod, nullptr, (size_t)n_pair * 4);
     }
     if ((rc = stage_in(ctx, s, [&](uint8_t* h) { expand_pairs((uint32_t*)h, cand_off, n_pod); }))) return rc;
-    if (claim_blocks && n_claim) CU(cudaMemsetAsync(ctx->d_why_blocks, 0, (size_t)n_claim * 4, ctx->stream));
     Prof prof(ctx);
     if (n_pair) {
         UnsArgs a; memset(&a, 0, sizeof a);
@@ -1701,12 +1762,7 @@ int dra_unsuitable_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t
         a.why = ctx->d_why; a.why_claim = ctx->d_why_claim;
         if ((rc = launch_unsuitable(ctx, a, false, true))) return rc;
     }
-    if (pod_why || claim_blocks) {
-        const WhyTally t{ctx->d_why, ctx->d_why_claim, dense ? nullptr : ctx->d_cand_off, n_pod, ctx->n_node,
-                         pod_why ? ctx->d_why_pod : nullptr, claim_blocks ? ctx->d_why_blocks : nullptr};
-        k_why_tally<<<n_pod / 8 + 1, 256, 0, ctx->stream>>>(t);
-        ctx->launches += 1;
-    }
+    if ((rc = launch_why_tally(ctx, w, dense ? nullptr : ctx->d_cand_off, n_pod, n_claim))) return rc;
     prof.mark();
     return read_back(ctx, "unsuitable reasons kernels", 1, outs);
 }
@@ -1771,8 +1827,7 @@ int dra_allocate_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
 namespace {
 int place_pods_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off,
                     uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, const uint32_t* out_off,
-                    dra_out_rec* out, uint32_t n_out, uint32_t* pod_node, bool why, uint8_t* pair_why, uint32_t* pair_claim,
-                    uint32_t* pod_why, uint32_t* claim_blocks, uint32_t flags) {
+                    dra_out_rec* out, uint32_t n_out, uint32_t* pod_node, const WhyOut* why, uint32_t flags) {
     if (!ctx || !pod_off || (n_claim && (!claims || !out)) || (n_pod && !pod_node)) return DRA_E_INVAL;
     QUIESCE();
     if (flags & ~(DRA_F_EXHAUSTIVE | DRA_F_FRESH_INVENTORY)) return fail(ctx, DRA_E_INVAL, "%s: unknown flags 0x%x", name, flags);
@@ -1784,13 +1839,8 @@ int place_pods_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims,
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
     if ((rc = check_slots(ctx, claims, n_claim, out_off, n_out, true)) ||
         (rc = check_sortable(ctx, dense ? 0 : n_pair))) return rc;
-    uint32_t n_why = 0;                                   // the pairs answered (spec §18): dense, every pod at every node
-    if (why) {
-        const uint64_t n = dense ? (uint64_t)n_pod * ctx->n_node : n_pair;
-        if (n > 0xFFFFFFFFull) return fail(ctx, DRA_E_INVAL, "%llu (pod, node) pairs: more than %llu", (unsigned long long)n, 0xFFFFFFFFull);
-        n_why = (uint32_t)n;
-        if (n_why && !pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
-    }
+    uint32_t n_why;
+    if ((rc = place_why_pairs(ctx, why, dense, n_pod, n_pair, n_why)) || (rc = why_check(ctx, why, n_why))) return rc;
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "%s needs cooperative launches, which this device does not offer", name);
@@ -1802,16 +1852,9 @@ int place_pods_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims,
         (rc = grow_set(ctx, ctx->cap_podrec, (size_t)n_pair + 8, ctx->d_podrec)) ||
         (rc = grow_set(ctx, ctx->cap_place_pods, (size_t)n_pod + 8, ctx->d_place_state, ctx->d_place_node)) ||
         (rc = grow_set(ctx, ctx->cap_place_cursor, (size_t)ctx->n_node + 8, ctx->d_place_cursor))) return rc;
-    if (why && ((rc = grow_set(ctx, ctx->cap_why_pairs, (size_t)n_why + 8, ctx->d_why, ctx->d_why_claim)) ||
-                (rc = grow_set(ctx, ctx->cap_why_pods, (size_t)n_pod * DRA_WHY_N + 8, ctx->d_why_pod)) ||
-                (rc = grow_set(ctx, ctx->cap_why_claims, (size_t)n_claim + 8, ctx->d_why_blocks)))) return rc;
     const size_t rb = (size_t)n_out * 8;
-    const Outputs outs = {{out, ctx->d_out, rb}, {pod_node, ctx->d_place_node, (size_t)n_pod * 4},
-                          {pair_why, ctx->d_why, why ? (size_t)n_why : 0},
-                          {pair_claim, ctx->d_why_claim, why && pair_claim ? (size_t)n_why * 4 : 0},
-                          {pod_why, ctx->d_why_pod, why && pod_why ? (size_t)n_pod * DRA_WHY_N * 4 : 0},
-                          {claim_blocks, ctx->d_why_blocks, why && claim_blocks ? (size_t)n_claim * 4 : 0}};
-    if ((rc = reserve_out(ctx, outs))) return rc;
+    Outputs outs = {{out, ctx->d_out, rb}, {pod_node, ctx->d_place_node, (size_t)n_pod * 4}};
+    if ((rc = why_buffers(ctx, why, outs, n_why, n_pod, n_claim)) || (rc = reserve_out(ctx, outs))) return rc;
     Staging s;
     s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
     s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
@@ -1823,7 +1866,6 @@ int place_pods_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims,
     if ((rc = stage_in(ctx, s))) return rc;
     if (rb) CU(cudaMemsetAsync(ctx->d_out, 0, rb, ctx->stream));
     CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)ctx->n_node + 1) * 4, ctx->stream));
-    if (why && claim_blocks && n_claim) CU(cudaMemsetAsync(ctx->d_why_blocks, 0, (size_t)n_claim * 4, ctx->stream));
     Prof prof(ctx);
     PlaceArgs a; memset(&a, 0, sizeof a);
     a.claims = ctx->d_claims; a.pod_off = ctx->d_pod_off; a.n_pod = n_pod;
@@ -1848,14 +1890,9 @@ int place_pods_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims,
         ctx->chain |= DRA_K_PLACE;
     } else {
         // (sized by its own occupancy: its registers are not k_pods_place<4>'s)
-        if ((rc = launch_walk(ctx, ctx->place_why_occ, "k_pods_place<4, false, true>", k_pods_place<4, false, true>, a, PlaceShard{})))
+        if ((rc = launch_walk(ctx, ctx->place_why_occ, "k_pods_place<4, false, true>", k_pods_place<4, false, true>, a, PlaceShard{})) ||
+            (rc = launch_why_tally(ctx, *why, dense ? nullptr : ctx->d_cand_off, n_pod, n_claim)))
             return rc;
-        if (pod_why || claim_blocks) {
-            const WhyTally t{ctx->d_why, ctx->d_why_claim, dense ? nullptr : ctx->d_cand_off, n_pod, ctx->n_node,
-                             pod_why ? ctx->d_why_pod : nullptr, claim_blocks ? ctx->d_why_blocks : nullptr};
-            k_why_tally<<<n_pod / 8 + 1, 256, 0, ctx->stream>>>(t);
-            ctx->launches += 1;
-        }
         ctx->chain |= DRA_K_PLACE | DRA_K_PLACE_WHY;
     }
     prof.mark();
@@ -1867,7 +1904,7 @@ int dra_place_pods_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_c
                          const uint32_t* cand_nodes, const uint32_t* cand_off, const uint32_t* out_off, dra_out_rec* out,
                          uint32_t n_out, uint32_t* pod_node, uint32_t flags) {
     return place_pods_call(ctx, "dra_place_pods_batch", claims, n_claim, pod_off, n_pod, cand_nodes, cand_off, out_off, out, n_out,
-                           pod_node, false, nullptr, nullptr, nullptr, nullptr, flags);
+                           pod_node, nullptr, flags);
 }
 
 // Why place pods put each pod where it did (spec §18): dra_place_pods_batch's call, every pair answered on the state its
@@ -1876,8 +1913,9 @@ int dra_place_pods_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t
                              const uint32_t* cand_nodes, const uint32_t* cand_off, const uint32_t* out_off, dra_out_rec* out,
                              uint32_t n_out, uint32_t* pod_node, uint8_t* pair_why, uint32_t* pair_claim, uint32_t* pod_why,
                              uint32_t* claim_blocks, uint32_t flags) {
+    const WhyOut w{pair_why, pair_claim, pod_why, claim_blocks};
     return place_pods_call(ctx, "dra_place_pods_why_batch", claims, n_claim, pod_off, n_pod, cand_nodes, cand_off, out_off, out,
-                           n_out, pod_node, true, pair_why, pair_claim, pod_why, claim_blocks, flags);
+                           n_out, pod_node, &w, flags);
 }
 
 // Preemption (spec §14): the pending-pod arrays are checked here; the running pods on the device (k_pre_running), whose
@@ -1890,8 +1928,7 @@ int preempt_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims, ui
                  const int32_t* prio, uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off,
                  const dra_running_pods* running, const dra_disruption_budgets* budgets, uint8_t* pair_status,
                  uint32_t* pair_victims, uint32_t* pair_violations, uint32_t* pod_node, uint8_t* pod_status, uint32_t* n_victims,
-                 uint32_t* pod_violations, uint32_t* victims, uint32_t max_victims, bool why, uint8_t* pair_why,
-                 uint32_t* pair_claim, uint32_t* pod_why, uint32_t* claim_blocks, uint32_t flags) {
+                 uint32_t* pod_violations, uint32_t* victims, uint32_t max_victims, const WhyOut* why, uint32_t flags) {
     if (!ctx || !pod_off || !running || !running->pod_off || (n_claim && !claims) ||
         (n_pod && (!prio || (!why && (!pod_node || !pod_status || !n_victims)))))
         return DRA_E_INVAL;
@@ -1907,8 +1944,8 @@ int preempt_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims, ui
     int rc;
     if ((rc = check_pod_off(ctx, pod_off, n_pod, n_claim)) ||
         (rc = check_cands(ctx, n_pod, cand_nodes, cand_off, 0xFFFFFFFFu, ctx->n_node, 0xFFFFFFFFull, dense, n_pair)) ||
-        (rc = check_sortable(ctx, n_pod ? R.n_pod : 0))) return rc;
-    if (why && n_pair && !pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+        (rc = check_sortable(ctx, n_pod ? R.n_pod : 0)) ||
+        (rc = why_check(ctx, why, n_pair))) return rc;
     ctx->chain = why ? DRA_K_PREEMPT | DRA_K_UNSUITABLE_WHY : DRA_K_PREEMPT; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     if ((rc = check_budgets(ctx, "dra_preempt_pdb_batch", budgets, R.n_pod))) return rc;
@@ -1923,23 +1960,16 @@ int preempt_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims, ui
         (rc = grow_set(ctx, ctx->cap_pre_pairs, (size_t)n_pair + 8, ctx->d_pre_psum, ctx->d_pre_psum64, ctx->d_pre_pairst, ctx->d_pre_pairvic,
                        ctx->d_pre_pairviol)) ||
         (rc = grow_set(ctx, ctx->cap_pre_vic, vb / 4 + 8, ctx->d_pre_vic))) return rc;
-    if (why && ((rc = grow_set(ctx, ctx->cap_why_pairs, (size_t)n_pair + 8, ctx->d_why, ctx->d_why_claim)) ||
-                (rc = grow_set(ctx, ctx->cap_why_pods, (size_t)n_pod * DRA_WHY_N + 8, ctx->d_why_pod)) ||
-                (rc = grow_set(ctx, ctx->cap_why_claims, (size_t)n_claim + 8, ctx->d_why_blocks)))) return rc;
     const size_t np = why ? 0 : n_pod;                   // (the reasons call chooses nothing: no per-pod output)
-    const Outputs outs = {{pair_status, ctx->d_pre_pairst, pair_status ? (size_t)n_pair : 0},
-                          {pair_victims, ctx->d_pre_pairvic, pair_victims ? (size_t)n_pair * 4 : 0},
-                          {pod_node, ctx->d_pre_node, np * 4},
-                          {pod_status, ctx->d_pre_pst, np},
-                          {n_victims, ctx->d_pre_nvic, np * 4},
-                          {victims, ctx->d_pre_vic, vb},
-                          {pair_violations, ctx->d_pre_pairviol, pair_violations ? (size_t)n_pair * 4 : 0},
-                          {pod_violations, ctx->d_pre_podviol, pod_violations ? (size_t)n_pod * 4 : 0},
-                          {pair_why, ctx->d_why, why ? (size_t)n_pair : 0},
-                          {pair_claim, ctx->d_why_claim, why && pair_claim ? (size_t)n_pair * 4 : 0},
-                          {pod_why, ctx->d_why_pod, why && pod_why ? (size_t)n_pod * DRA_WHY_N * 4 : 0},
-                          {claim_blocks, ctx->d_why_blocks, why && claim_blocks ? (size_t)n_claim * 4 : 0}};
-    if ((rc = reserve_out(ctx, outs))) return rc;
+    Outputs outs = {{pair_status, ctx->d_pre_pairst, pair_status ? (size_t)n_pair : 0},
+                    {pair_victims, ctx->d_pre_pairvic, pair_victims ? (size_t)n_pair * 4 : 0},
+                    {pod_node, ctx->d_pre_node, np * 4},
+                    {pod_status, ctx->d_pre_pst, np},
+                    {n_victims, ctx->d_pre_nvic, np * 4},
+                    {victims, ctx->d_pre_vic, vb},
+                    {pair_violations, ctx->d_pre_pairviol, pair_violations ? (size_t)n_pair * 4 : 0},
+                    {pod_violations, ctx->d_pre_podviol, pod_violations ? (size_t)n_pod * 4 : 0}};
+    if ((rc = why_buffers(ctx, why, outs, n_pair, n_pod, n_claim)) || (rc = reserve_out(ctx, outs))) return rc;
     Staging s;
     s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
     s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
@@ -1965,15 +1995,9 @@ int preempt_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims, ui
     if ((rc = launch_running_lists(ctx, a, prof, false))) return rc;
     const PreShard whole{0u, ctx->n_node, n_pair, 0u, nullptr, nullptr};   // every node: the walk index is the pair index
     if (why) {
-        if (claim_blocks && n_claim) CU(cudaMemsetAsync(ctx->d_why_blocks, 0, (size_t)n_claim * 4, ctx->stream));
         a.why = ctx->d_why; a.why_claim = ctx->d_why_claim;
-        if ((rc = launch_preempt_pairs(ctx, a, whole, true))) return rc;
-        if (pod_why || claim_blocks) {
-            const WhyTally t{ctx->d_why, ctx->d_why_claim, dense ? nullptr : ctx->d_cand_off, n_pod, ctx->n_node,
-                             pod_why ? ctx->d_why_pod : nullptr, claim_blocks ? ctx->d_why_blocks : nullptr};
-            k_why_tally<<<n_pod / 8 + 1, 256, 0, ctx->stream>>>(t);
-            ctx->launches += 1;
-        }
+        if ((rc = launch_preempt_pairs(ctx, a, whole, true)) ||
+            (rc = launch_why_tally(ctx, *why, dense ? nullptr : ctx->d_cand_off, n_pod, n_claim))) return rc;
         prof.mark();
         return read_back(ctx, "preemption reasons kernels", 1, outs);
     }
@@ -1997,7 +2021,7 @@ int dra_preempt_pdb_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
                           uint32_t* pod_violations, uint32_t* victims, uint32_t max_victims, uint32_t flags) {
     return preempt_call(ctx, "dra_preempt_pdb_batch", claims, n_claim, pod_off, prio, n_pod, cand_nodes, cand_off, running, budgets,
                         pair_status, pair_victims, pair_violations, pod_node, pod_status, n_victims, pod_violations, victims,
-                        max_victims, false, nullptr, nullptr, nullptr, nullptr, flags);
+                        max_victims, nullptr, flags);
 }
 
 // Why preemption judged each node as it did (spec §19): dra_preempt_batch's pairs, each with its status, reason and
@@ -2006,9 +2030,9 @@ int dra_preempt_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_
                           uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off, const dra_running_pods* running,
                           uint8_t* pair_status, uint8_t* pair_why, uint32_t* pair_claim, uint32_t* pod_why, uint32_t* claim_blocks,
                           uint32_t flags) {
+    const WhyOut w{pair_why, pair_claim, pod_why, claim_blocks};
     return preempt_call(ctx, "dra_preempt_why_batch", claims, n_claim, pod_off, prio, n_pod, cand_nodes, cand_off, running, nullptr,
-                        pair_status, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, true, pair_why, pair_claim,
-                        pod_why, claim_blocks, flags);
+                        pair_status, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, &w, flags);
 }
 
 int dra_preempt_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off, const int32_t* prio,
@@ -2082,8 +2106,8 @@ namespace {
 int preempt_place_call(dra_ctx* ctx, const char* name, const dra_claim_rec* claims, uint32_t n_claim, const uint32_t* pod_off,
                        const int32_t* prio, uint32_t n_pod, const uint32_t* cand_nodes, const uint32_t* cand_off,
                        const dra_running_pods* running, const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
-                       uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, bool why, uint8_t* pair_status,
-                       uint8_t* pair_why, uint32_t* pair_claim, uint32_t* pod_why, uint32_t* claim_blocks, uint32_t flags) {
+                       uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, const WhyOut* why, uint8_t* pair_status,
+                       uint32_t flags) {
     if (!ctx || !pod_off || !running || !running->pod_off || (n_claim && (!claims || !out)) ||
         (n_pod && (!prio || !pod_node || !pod_status)))
         return DRA_E_INVAL;
@@ -2100,8 +2124,8 @@ int preempt_place_call(dra_ctx* ctx, const char* name, const dra_claim_rec* clai
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
     if ((rc = check_slots(ctx, claims, n_claim, out_off, n_out, true)) ||
         (rc = check_sortable(ctx, n_pod ? R.n_pod : 0)) ||
-        (rc = check_sortable(ctx, n_pod && !dense ? n_pair : 0))) return rc;
-    if (why && n_pair && !pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+        (rc = check_sortable(ctx, n_pod && !dense ? n_pair : 0)) ||
+        (rc = why_check(ctx, why, n_pair))) return rc;
     ctx->chain = why ? DRA_K_PREEMPT_PLACE | DRA_K_PLACE_WHY : DRA_K_PREEMPT_PLACE; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;
     if (!ctx->coop_ok) return fail(ctx, DRA_E_STATE, "%s needs cooperative launches, which this device does not offer", name);
@@ -2111,18 +2135,11 @@ int preempt_place_call(dra_ctx* ctx, const char* name, const dra_claim_rec* clai
     if ((rc = grow_set(ctx, ctx->cap_pods, (size_t)n_pod + 8, ctx->d_pod_off, ctx->d_cand_off)) ||
         (!dense && (rc = grow_set(ctx, ctx->cap_pairs, (size_t)n_pair + 64, ctx->d_cand_nodes, ctx->d_pair_pod))) ||
         (rc = pp_buffers(ctx, n_pod, n_pair, R.n_pod))) return rc;
-    if (why && ((rc = grow_set(ctx, ctx->cap_why_pairs, (size_t)n_pair + 8, ctx->d_why, ctx->d_why_claim)) ||
-                (rc = grow_set(ctx, ctx->cap_why_pods, (size_t)n_pod * DRA_WHY_N + 8, ctx->d_why_pod)) ||
-                (rc = grow_set(ctx, ctx->cap_why_claims, (size_t)n_claim + 8, ctx->d_why_blocks)))) return rc;
     const size_t rb = (size_t)n_out * 8;
-    const Outputs outs = {{out, ctx->d_out, rb}, {pod_node, ctx->d_pre_node, (size_t)n_pod * 4}, {pod_status, ctx->d_pre_pst, n_pod},
-                          {evicted_by, ctx->d_pp_evicted, (size_t)R.n_pod * 4},
-                          {pair_status, ctx->d_pre_pairst, why && pair_status ? (size_t)n_pair : 0},
-                          {pair_why, ctx->d_why, why ? (size_t)n_pair : 0},
-                          {pair_claim, ctx->d_why_claim, why && pair_claim ? (size_t)n_pair * 4 : 0},
-                          {pod_why, ctx->d_why_pod, why && pod_why ? (size_t)n_pod * DRA_WHY_N * 4 : 0},
-                          {claim_blocks, ctx->d_why_blocks, why && claim_blocks ? (size_t)n_claim * 4 : 0}};
-    if ((rc = reserve_out(ctx, outs))) return rc;
+    Outputs outs = {{out, ctx->d_out, rb}, {pod_node, ctx->d_pre_node, (size_t)n_pod * 4}, {pod_status, ctx->d_pre_pst, n_pod},
+                    {evicted_by, ctx->d_pp_evicted, (size_t)R.n_pod * 4},
+                    {pair_status, ctx->d_pre_pairst, pair_status ? (size_t)n_pair : 0}};
+    if ((rc = why_buffers(ctx, why, outs, n_pair, n_pod, n_claim)) || (rc = reserve_out(ctx, outs))) return rc;
     Staging s;
     s.add(ctx->d_claims, claims, (size_t)n_claim * 16);
     s.add(ctx->d_pod_off, pod_off, ((size_t)n_pod + 1) * 4);
@@ -2139,7 +2156,6 @@ int preempt_place_call(dra_ctx* ctx, const char* name, const dra_claim_rec* clai
     CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)ctx->n_node + 1) * 4, st));
     CU(cudaMemsetAsync(ctx->d_pp_judged, 0, ((size_t)ctx->n_node + 1) * 4, st));
     if (R.n_pod) CU(cudaMemsetAsync(ctx->d_pp_evicted, 0xFF, (size_t)R.n_pod * 4, st));
-    if (why && claim_blocks && n_claim) CU(cudaMemsetAsync(ctx->d_why_blocks, 0, (size_t)n_claim * 4, st));
 
     PreArgs a = pre_args(ctx, ctx->d_claims, ctx->d_pod_off, (const int32_t*)ctx->d_pre_prio, n_pod, dense ? nullptr : ctx->d_cand_nodes,
                          dense ? nullptr : ctx->d_cand_off, n_pair, Rd, ctx->d_inv_live, flags);
@@ -2172,14 +2188,9 @@ int preempt_place_call(dra_ctx* ctx, const char* name, const dra_claim_rec* clai
         if ((rc = launch_walk(ctx, ctx->pp_occ, "k_pods_preempt_place", k_pods_preempt_place<4>, a, pl, pp))) return rc;
     } else {
         // (sized by its own occupancy: its registers are not k_pods_preempt_place<4>'s)
-        if ((rc = launch_walk(ctx, ctx->pp_why_occ, "k_pods_preempt_place<4, true>", k_pods_preempt_place<4, true>, a, pl, pp)))
+        if ((rc = launch_walk(ctx, ctx->pp_why_occ, "k_pods_preempt_place<4, true>", k_pods_preempt_place<4, true>, a, pl, pp)) ||
+            (rc = launch_why_tally(ctx, *why, dense ? nullptr : ctx->d_cand_off, n_pod, n_claim)))
             return rc;
-        if (pod_why || claim_blocks) {
-            const WhyTally t{ctx->d_why, ctx->d_why_claim, dense ? nullptr : ctx->d_cand_off, n_pod, ctx->n_node,
-                             pod_why ? ctx->d_why_pod : nullptr, claim_blocks ? ctx->d_why_blocks : nullptr};
-            k_why_tally<<<n_pod / 8 + 1, 256, 0, st>>>(t);
-            ctx->launches += 1;
-        }
     }
     prof.mark();
     return read_back(ctx, why ? "preempt-and-place reasons kernels" : "preempt-and-place kernels", 1, outs);
@@ -2191,8 +2202,7 @@ int dra_preempt_place_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint32_t 
                             const dra_running_pods* running, const uint32_t* out_off, dra_out_rec* out, uint32_t n_out,
                             uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, uint32_t flags) {
     return preempt_place_call(ctx, "dra_preempt_place_batch", claims, n_claim, pod_off, prio, n_pod, cand_nodes, cand_off, running,
-                              out_off, out, n_out, pod_node, pod_status, evicted_by, false, nullptr, nullptr, nullptr, nullptr,
-                              nullptr, flags);
+                              out_off, out, n_out, pod_node, pod_status, evicted_by, nullptr, nullptr, flags);
 }
 
 // Why preemption judged each node as it did, in preempt and place (spec §19): dra_preempt_place_batch's call, every pair
@@ -2203,9 +2213,9 @@ int dra_preempt_place_why_batch(dra_ctx* ctx, const dra_claim_rec* claims, uint3
                                 uint32_t* pod_node, uint8_t* pod_status, uint32_t* evicted_by, uint8_t* pair_status,
                                 uint8_t* pair_why, uint32_t* pair_claim, uint32_t* pod_why, uint32_t* claim_blocks,
                                 uint32_t flags) {
+    const WhyOut w{pair_why, pair_claim, pod_why, claim_blocks};
     return preempt_place_call(ctx, "dra_preempt_place_why_batch", claims, n_claim, pod_off, prio, n_pod, cand_nodes, cand_off,
-                              running, out_off, out, n_out, pod_node, pod_status, evicted_by, true, pair_status, pair_why,
-                              pair_claim, pod_why, claim_blocks, flags);
+                              running, out_off, out, n_out, pod_node, pod_status, evicted_by, &w, pair_status, flags);
 }
 
 // Deallocate on one inventory (spec §9).  Every claim's slot range is checked here, with the slots k_dealloc counts, before
@@ -2542,6 +2552,63 @@ void launch_uns_prep(dra_ctx* ctx, const uint32_t* d_pod_off, const uint32_t* d_
 void merge_bounds(const dra_ctx* ctx, bool gather, uint32_t (&bounds)[PEER_MAX + 1]) {
     bounds[0] = 0; bounds[1] = ctx->n_node;
     if (gather) for (int r = 0; r <= ctx->world; ++r) bounds[r] = ctx->shard_bounds[r];
+}
+
+// The sharded reasons' exchange at world > 1 (check_world's reserved()): dra_set_shard_why before the export, since even a
+// call with no pairs pushes a header and raises flags, which would land in the peers' buffers at offset 0
+int swhy_reserved(dra_ctx* ctx) {
+    if (ctx->shard_rsv.swhy_pairs) return DRA_OK;
+    return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_why(max_pairs > 0) was not called before dra_shard_export");
+}
+
+// n_why answered pairs within the sharded reasons' exchange (check_world's fits())
+int swhy_fits(dra_ctx* ctx, uint32_t n_why) {
+    if (n_why <= ctx->shard_rsv.swhy_pairs) return DRA_OK;
+    return fail(ctx, DRA_E_INVAL, "%u pairs exceed the max_pairs (%u) of dra_set_shard_why before dra_shard_export", n_why,
+                ctx->shard_rsv.swhy_pairs);
+}
+
+// The sharded reasons' buffers, grown before the call enqueues anything else: this rank's slice for n_walk walked pairs
+// (world > 1: peer_setup sized it for max_pairs, which bounds n_walk, so it never reallocates there) and, with
+// claim_blocks, the merge's per-claim counts, zeroed.  Those depend on n_claim, which no setter bounds: a larger batch grows
+// them here, the old buffer retired until the next dra_ctx_sync.
+int swhy_buffers(dra_ctx* ctx, const WhyOut& w, uint32_t n_walk, uint32_t n_claim) {
+    if (int rc = grow(ctx, ctx->d_swhy_part, ctx->cap_swhy_part, swhy_units(n_walk))) return rc;
+    if (!w.claim_blocks) return DRA_OK;
+    if (int rc = grow(ctx, ctx->d_swhy_blocks, ctx->cap_swhy_blocks, (size_t)n_claim + 1)) return rc;
+    CU(cudaMemsetAsync(ctx->d_swhy_blocks, 0, ((size_t)n_claim + 1) * 4, ctx->stream));
+    return DRA_OK;
+}
+
+// Where the walk writes its reasons in this rank's slice: [header][n_walk u8 reasons, padded][n_walk u32 claims].  The
+// claims are written whether they are sent or not.
+void swhy_slice(const dra_ctx* ctx, uint32_t n_walk, uint8_t*& why, uint32_t*& why_claim) {
+    why = reinterpret_cast<uint8_t*>(ctx->d_swhy_part + 1);
+    why_claim = reinterpret_cast<uint32_t*>(ctx->d_swhy_part + 1 + ((size_t)n_walk + 15) / 16);
+}
+
+// After the walk: this rank's slice to every rank behind its header, the fault word at gate (push_slice advances the
+// region's call parity, as every §17 call does), then the owner-indexed merge writes w's outputs and the tallies on every
+// rank (k_swhy_merge).  cand_nodes and cand_off: nullptr in the dense form.  Enqueues only.
+int launch_swhy_merge(dra_ctx* ctx, const WhyOut& w, const uint32_t* gate, uint32_t n_walk, const uint32_t* cand_nodes,
+                      const uint32_t* cand_off, uint32_t n_pod, uint32_t n_pair, uint32_t n_claim) {
+    const bool gather = ctx->world > 1;
+    uint4* part = ctx->d_swhy_part;
+    WhyMerge m; memset(&m, 0, sizeof m);
+    m.part = part; m.cand_nodes = cand_nodes; m.cand_off = cand_off;
+    m.n_pod = n_pod; m.n_pair = n_pair; m.n_node = ctx->n_node; m.n_claim = n_claim;
+    merge_bounds(ctx, gather, m.bounds);
+    m.gate = gate;
+    m.pair_why = w.pair_why; m.pair_claim = w.pair_claim; m.pod_why = w.pod_why; m.claim_blocks = w.claim_blocks;
+    m.blocks = ctx->d_swhy_blocks;
+    if (gather) {
+        m.slice4 = (uint32_t)(ctx->swhy_x.slice / 16);
+        CU(cudaMemcpyAsync(part, gate, 4, cudaMemcpyDeviceToDevice, ctx->stream));   // the header: this rank's fault word
+    }
+    const PeerExchange x = push_slice(ctx, ctx->swhy_x, gather, part, (uint32_t)swhy_units(n_walk, w.pair_claim || w.claim_blocks));
+    k_swhy_merge<<<wait_grid(ctx, (n_pod + 7) / 8), 256, 0, ctx->stream>>>(x, m);
+    ctx->launches += 1;
+    return DRA_OK;
 }
 
 // The result table of a global Allocate call: at world > 1 the table of g, a gather of a new epoch, else this context's own
@@ -2987,8 +3054,7 @@ int dra_set_shard_place(dra_ctx* ctx, uint32_t max_pods) {
 namespace {
 int place_pods_shard_call(dra_ctx* ctx, const char* name, const dra_claim_rec* d_claims, uint32_t n_claim,
                           const uint32_t* d_pod_off, uint32_t n_pod, const uint32_t* d_cand_nodes, const uint32_t* d_cand_off,
-                          uint32_t n_pair, const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node, bool why,
-                          uint8_t* d_pair_why, uint32_t* d_pair_claim, uint32_t* d_pod_why, uint32_t* d_claim_blocks,
+                          uint32_t n_pair, const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node, const WhyOut* why,
                           uint32_t flags) {
     if (!ctx || !d_pod_off || (n_claim && !d_claims) || (n_pod && !d_pod_node)) return DRA_E_INVAL;
     QUIESCE();
@@ -3002,41 +3068,27 @@ int place_pods_shard_call(dra_ctx* ctx, const char* name, const dra_claim_rec* d
     bool dense;
     if (int rc = check_dev_cands(ctx, d_cand_nodes, d_cand_off, n_pod, n_pair, false, dense)) return rc;
     if (ctx->n_node > PL_POS) return fail(ctx, DRA_E_INVAL, "more than %u nodes", PL_POS);
-    uint32_t n_why = 0;                                   // the pairs answered (spec §18): dense, every pod at every node
-    if (why) {
-        const uint64_t n = dense ? (uint64_t)n_pod * ctx->n_node : n_pair;
-        if (n > 0xFFFFFFFFull) return fail(ctx, DRA_E_INVAL, "%llu (pod, node) pairs: more than %llu", (unsigned long long)n, 0xFFFFFFFFull);
-        n_why = (uint32_t)n;
-    }
+    uint32_t n_why;
+    if (int rc = place_why_pairs(ctx, why, dense, n_pod, n_pair, n_why)) return rc;
     const bool gather = ctx->world > 1;
-    const uint32_t max_pods = ctx->shard_rsv.place_pods, max_pairs = ctx->shard_rsv.swhy_pairs;
-    // the reasons without their exchange reserved: even a call with no pairs pushes a header and raises flags, which would
-    // land in the peers' buffers at offset 0
-    if (int rc = check_world(ctx, "the walk and the gather need", false, [&] {
-            if (!why || max_pairs) return (int)DRA_OK;
-            return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_why(max_pairs > 0) was not called before dra_shard_export");
-        }, n_out, [&] {
+    const uint32_t max_pods = ctx->shard_rsv.place_pods;
+    if (int rc = check_world(ctx, "the walk and the gather need", false, [&] { return why ? swhy_reserved(ctx) : (int)DRA_OK; },
+                             n_out, [&] {
             if (n_pod > max_pods)
                 return fail(ctx, DRA_E_STATE, "n_pod %u exceeds the max_pods (%u) of dra_set_shard_place before dra_shard_export", n_pod, max_pods);
-            if (n_why > max_pairs)
-                return fail(ctx, DRA_E_INVAL, "%u pairs exceed the max_pairs (%u) of dra_set_shard_why before dra_shard_export", n_why, max_pairs);
-            return (int)DRA_OK;
+            return swhy_fits(ctx, n_why);
         }))
         return rc;
-    if (n_why && !d_pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+    if (int rc = why_check(ctx, why, n_why)) return rc;
     ctx->chain = ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
     CallScope scope{ctx};
     int rc = scope.open(gather);
     if (rc) return rc;
     const uint32_t n_win = ctx->shard_hi - ctx->shard_lo;
-    // the reasons' slice (world > 1: peer_setup sized it for max_pairs, which bounds n_walk) and, with claim_blocks, the
-    // merge's per-claim counts, which depend on n_claim: a larger batch grows them here, the old buffer retired until the
-    // next dra_ctx_sync.  Both before anything is enqueued.
     const uint32_t n_walk = dense ? n_pod * n_win : n_pair;           // (n_pod * n_win <= n_pod * n_node < 2^32)
-    if (why && ((rc = grow(ctx, ctx->d_swhy_part, ctx->cap_swhy_part, swhy_units(n_walk))) ||
-                (d_claim_blocks && (rc = grow(ctx, ctx->d_swhy_blocks, ctx->cap_swhy_blocks, (size_t)n_claim + 1)))))
-        return rc;
+    // (the blocks are zeroed here, before the walk: after it, this thread launches only kernels peer_setup preloaded)
+    if (why && (rc = swhy_buffers(ctx, *why, n_walk, n_claim))) return rc;
     if ((rc = ensure_batch(ctx, std::max(n_pod, n_pair), 1, false))) return rc;
     const Tiling t = tiling(n_pair, n_win, ctx->n_sm);                // the sort's tiles are laid out on the window
     if ((rc = grow(ctx, ctx->d_hist, ctx->cap_hist, (size_t)t.n_tiles * (n_win + 1), 64))) return rc;
@@ -3077,11 +3129,7 @@ int place_pods_shard_call(dra_ctx* ctx, const char* name, const dra_claim_rec* d
     a.sorted = ctx->d_sorted; a.list_off = ctx->d_claim_off; a.cursor = ctx->d_place_cursor;
     a.inv_src = ctx->d_inv_live; a.inv_dst = ctx->d_inv_live; a.node_off = d_node_off; a.tbl = ctx->d_tbl;
     a.n_node = ctx->n_node; a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u; a.sel = sel_of(ctx); a.err = err;
-    uint4* part = ctx->d_swhy_part;                   // why: [header][n_walk u8 reasons, padded][n_walk u32 claims]
-    if (why) {
-        a.why = reinterpret_cast<uint8_t*>(part + 1);
-        a.why_claim = reinterpret_cast<uint32_t*>(part + 1 + ((size_t)n_walk + 15) / 16);   // (written whether sent or not)
-    }
+    if (why) swhy_slice(ctx, n_walk, a.why, a.why_claim);
     // the gate's SPodArgs: its record count is the sort's (the pairs), its world the one the bounds were counted for
     SPodArgs sa; memset(&sa, 0, sizeof sa);
     sa.claims = (const uint4*)d_claims; sa.pod_off = d_pod_off; sa.out_off = d_out_off;
@@ -3094,10 +3142,7 @@ int place_pods_shard_call(dra_ctx* ctx, const char* name, const dra_claim_rec* d
     CU(cudaMemsetAsync(ctx->d_spod, 0, (SP_BAD + 1) * 4, ctx->stream));
     if (n_out) CU(cudaMemsetAsync(table, 0, (size_t)n_out * 8, ctx->stream));
     CU(cudaMemsetAsync(ctx->d_place_cursor, 0, ((size_t)n_win + 1) * 4, ctx->stream));
-    if (why) {
-        CU(cudaMemsetAsync(ctx->d_spod + SP_WHY_FAULT, 0, 4, ctx->stream));
-        if (d_claim_blocks) CU(cudaMemsetAsync(ctx->d_swhy_blocks, 0, ((size_t)n_claim + 1) * 4, ctx->stream));
-    }
+    if (why) CU(cudaMemsetAsync(ctx->d_spod + SP_WHY_FAULT, 0, 4, ctx->stream));
     k_splace_prep<<<(unsigned)(((size_t)n_pod * 32 + 255) / 256), 256, 0, ctx->stream>>>(a, sh);
     const uint32_t gate_grid = fresh ? std::max(1u, std::min((uint32_t)ctx->n_sm, (ctx->n_gpu + 255) / 256)) : 1u;
     k_spod_gate<<<gate_grid, 256, 0, ctx->stream>>>(sa_sort, gather ? ctx->peer_cap : 0u, fresh ? ctx->d_inv_pristine : nullptr,
@@ -3115,27 +3160,17 @@ int place_pods_shard_call(dra_ctx* ctx, const char* name, const dra_claim_rec* d
                           ctx->d_spod + SP_NDEV)))
         return rc;
     // The gate has read the bounds: k_splace_final counts the slots each rank really finalises in the same words.  (Zeroed
-    // before the walk: after it, this thread launches only kernels preload_place_shard loaded, since anything it waits for
-    // there would hold back the peers' calls that the walk waits for.)
+    // before the walk: after it, this thread launches only kernels peer_setup preloaded, since anything it waits for there
+    // would hold back the peers' calls that the walk waits for.)
     CU(cudaMemsetAsync(ctx->d_spod, 0, PEER_MAX * 4, ctx->stream));
     // Every CTA resident, not a cooperative launch: cooperative grids do not run beside each other, and a rank's walk waits
     // for its peers' walks
     if (!why) {
-        if (ctx->splace_occ < 0) {
-            int occ = 0;
-            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_place<4, true>, 128, 0));
-            ctx->splace_occ = occ;
-        }
-        if (ctx->splace_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_place<4, true>: no CTA can be resident");
+        if ((rc = walk_occupancy(ctx, ctx->splace_occ, "k_pods_place<4, true>", k_pods_place<4, true>))) return rc;
         k_pods_place<4, true><<<shard_walk_grid(ctx, ctx->splace_occ, gather, n_win), 128, 0, ctx->stream>>>(a, sh);
     } else {
         // (sized by its own occupancy: its registers are not k_pods_place<4, true>'s)
-        if (ctx->splace_why_occ < 0) {
-            int occ = 0;
-            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pods_place<4, true, true>, 128, 0));
-            ctx->splace_why_occ = occ;
-        }
-        if (ctx->splace_why_occ < 1) return fail(ctx, DRA_E_CUDA, "k_pods_place<4, true, true>: no CTA can be resident");
+        if ((rc = walk_occupancy(ctx, ctx->splace_why_occ, "k_pods_place<4, true, true>", k_pods_place<4, true, true>))) return rc;
         k_pods_place<4, true, true><<<shard_walk_grid(ctx, ctx->splace_why_occ, gather, n_win), 128, 0, ctx->stream>>>(a, sh);
     }
     ctx->launches += 1;
@@ -3148,23 +3183,10 @@ int place_pods_shard_call(dra_ctx* ctx, const char* name, const dra_claim_rec* d
         ctx->launches += 2;
     }
     if (why) {
-        // every rank's slice to every rank behind its header (push_slice advances the region's call parity, as every
-        // §17 call does), then the owner-indexed merge with the tallies
-        const uint32_t* gate = ctx->d_spod + SP_WHY_FAULT;
-        WhyMerge m; memset(&m, 0, sizeof m);
-        m.part = part; m.cand_nodes = a.cand_nodes; m.cand_off = a.cand_off;
-        m.n_pod = n_pod; m.n_pair = n_pair; m.n_node = ctx->n_node; m.n_claim = n_claim;
-        merge_bounds(ctx, gather, m.bounds);
-        m.gate = gate;
-        m.pair_why = d_pair_why; m.pair_claim = d_pair_claim; m.pod_why = d_pod_why; m.claim_blocks = d_claim_blocks;
-        m.blocks = ctx->d_swhy_blocks;
-        if (gather) {
-            m.slice4 = (uint32_t)(ctx->swhy_x.slice / 16);
-            CU(cudaMemcpyAsync(part, gate, 4, cudaMemcpyDeviceToDevice, ctx->stream));   // the header: the walk's fault word
-        }
-        const PeerExchange x = push_slice(ctx, ctx->swhy_x, gather, part, (uint32_t)swhy_units(n_walk, d_pair_claim || d_claim_blocks));
-        k_swhy_merge<<<wait_grid(ctx, (n_pod + 7) / 8), 256, 0, ctx->stream>>>(x, m);
-        ctx->launches += 1; ctx->chain |= DRA_K_PLACE_WHY;
+        // the gate: the walk's fault word
+        if ((rc = launch_swhy_merge(ctx, *why, ctx->d_spod + SP_WHY_FAULT, n_walk, a.cand_nodes, a.cand_off, n_pod, n_pair, n_claim)))
+            return rc;
+        ctx->chain |= DRA_K_PLACE_WHY;
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "%s launch: %s", why ? "sharded place reasons" : "sharded place pods", cudaGetErrorString(e));
@@ -3178,7 +3200,7 @@ int dra_place_pods_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_clai
                                        const uint32_t* d_cand_nodes, const uint32_t* d_cand_off, uint32_t n_pair,
                                        const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node, uint32_t flags) {
     return place_pods_shard_call(ctx, "dra_place_pods_batch_global_device", d_claims, n_claim, d_pod_off, n_pod, d_cand_nodes,
-                                 d_cand_off, n_pair, d_out_off, n_out, d_pod_node, false, nullptr, nullptr, nullptr, nullptr, flags);
+                                 d_cand_off, n_pair, d_out_off, n_out, d_pod_node, nullptr, flags);
 }
 
 // Why place pods put each pod where it did, across a sharded world (spec §18 "Sharded form")
@@ -3188,9 +3210,9 @@ int dra_place_pods_why_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_
                                            const uint32_t* d_out_off, uint32_t n_out, uint32_t* d_pod_node,
                                            uint8_t* d_pair_why, uint32_t* d_pair_claim, uint32_t* d_pod_why,
                                            uint32_t* d_claim_blocks, uint32_t flags) {
+    const WhyOut w{d_pair_why, d_pair_claim, d_pod_why, d_claim_blocks};
     return place_pods_shard_call(ctx, "dra_place_pods_why_batch_global_device", d_claims, n_claim, d_pod_off, n_pod,
-                                 d_cand_nodes, d_cand_off, n_pair, d_out_off, n_out, d_pod_node, true, d_pair_why, d_pair_claim,
-                                 d_pod_why, d_claim_blocks, flags);
+                                 d_cand_nodes, d_cand_off, n_pair, d_out_off, n_out, d_pod_node, &w, flags);
 }
 
 int dra_set_shard_preempt(dra_ctx* ctx, uint32_t max_pods, uint32_t max_pairs, uint32_t max_victims) {
@@ -3414,62 +3436,36 @@ int dra_unsuitable_why_batch_global_device(dra_ctx* ctx, const dra_claim_rec* d_
     if (int rc = check_dev_cands(ctx, d_cand_nodes, d_cand_off, n_pod, n_pair, true, dense)) return rc;
     if (n_pod > (1u << 26)) return fail(ctx, DRA_E_INVAL, "n_pod %u too large for the sharded call (2^26)", n_pod);
     const bool gather = ctx->world > 1;
-    const uint32_t max_pairs = ctx->shard_rsv.swhy_pairs;
-    // no exchange reserved: even a call with no pairs pushes a header and raises flags, which would land in the peers'
-    // buffers at offset 0
-    if (int rc = check_world(ctx, "the merge needs", true, [&] {
-            if (max_pairs) return (int)DRA_OK;
-            return fail(ctx, DRA_E_STATE, "world > 1: dra_set_shard_why(max_pairs > 0) was not called before dra_shard_export");
-        }, -1, [&] {
-            if (n_pair <= max_pairs) return (int)DRA_OK;
-            return fail(ctx, DRA_E_INVAL, "n_pair %u exceeds the max_pairs (%u) of dra_set_shard_why before dra_shard_export", n_pair, max_pairs);
-        }))
+    if (int rc = check_world(ctx, "the merge needs", true, [ctx] { return swhy_reserved(ctx); }, -1,
+                             [&] { return swhy_fits(ctx, n_pair); }))
         return rc;
-    if (n_pair && !d_pair_why) return fail(ctx, DRA_E_INVAL, "pair_why is NULL");
+    const WhyOut w{d_pair_why, d_pair_claim, d_pod_why, d_claim_blocks};
+    if (int rc = why_check(ctx, &w, n_pair)) return rc;
     ctx->chain = DRA_K_UNSUITABLE_WHY_SHARD; ctx->chain_tile = 0;
     if (!n_pod) return DRA_OK;                         // every rank sees the same n_pod: none of them exchanges anything
     CallScope scope{ctx};
     int rc = scope.open(gather);
     if (rc) return rc;
-    // world > 1: peer_setup sized both for max_pairs, so these never reallocate there.  The per-claim counts depend on
-    // n_claim, which no setter bounds: a larger batch grows them here, the old buffer retired until the next dra_ctx_sync.
-    if ((rc = grow(ctx, ctx->d_swhy_part, ctx->cap_swhy_part, swhy_units(n_pair)))) return rc;
-    if (!dense && (rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, n_pair))) return rc;
-    if (d_claim_blocks && (rc = grow(ctx, ctx->d_swhy_blocks, ctx->cap_swhy_blocks, (size_t)n_claim + 1))) return rc;
-    cudaStream_t st = ctx->stream;
     const uint32_t lo = gather ? ctx->shard_lo : 0u, hi = gather ? ctx->shard_hi : ctx->n_node;   // world 1: every node
+    const uint32_t n_walk = dense ? n_pod * (hi - lo) : n_pair;                                 // (n_pod * n_win <= n_pair)
+    // (world > 1: peer_setup sized d_upair_pod for max_pairs too, so it never reallocates there)
+    if ((rc = swhy_buffers(ctx, w, n_walk, n_claim)) ||
+        (!dense && (rc = grow(ctx, ctx->d_upair_pod, ctx->cap_upair_pod, n_pair)))) return rc;
     const uint32_t* gate = ctx->d_err + ERR_BAD_OFFSETS;
-    if (d_claim_blocks) CU(cudaMemsetAsync(ctx->d_swhy_blocks, 0, ((size_t)n_claim + 1) * 4, st));
     UnsArgs a; memset(&a, 0, sizeof a);
     a.claims = (const uint4*)d_claims; a.pod_off = d_pod_off; a.n_pod = n_pod;
     a.cand_nodes = dense ? nullptr : d_cand_nodes; a.cand_off = dense ? nullptr : d_cand_off;
     a.pair_pod = dense ? nullptr : ctx->d_upair_pod;
     a.inv = ctx->d_inv_live; a.node_off = ctx->d_node_off; a.n_node = ctx->n_node; a.tbl = ctx->d_tbl; a.sel = sel_of(ctx);
     a.exhaustive = (flags & DRA_F_EXHAUSTIVE) ? 1u : 0u;
-    a.node_lo = lo; a.n_win = hi - lo; a.n_walk = dense ? n_pod * a.n_win : n_pair;   // (n_pod * n_win <= n_pair)
+    a.node_lo = lo; a.n_win = hi - lo; a.n_walk = n_walk;
     a.gate = gate;
-    uint4* part = ctx->d_swhy_part;
-    const bool claims = d_pair_claim || d_claim_blocks;
-    a.why = reinterpret_cast<uint8_t*>(part + 1);
-    a.why_claim = reinterpret_cast<uint32_t*>(part + 1 + ((size_t)a.n_walk + 15) / 16);   // (written whether sent or not)
+    swhy_slice(ctx, n_walk, a.why, a.why_claim);
     Prof prof(ctx);
     launch_uns_prep(ctx, d_pod_off, d_cand_off, n_pod, n_claim, n_pair);
-    if (a.n_walk && (rc = launch_unsuitable(ctx, a, true, true))) return rc;
+    if (n_walk && (rc = launch_unsuitable(ctx, a, true, true))) return rc;
     prof.mark();
-    WhyMerge m; memset(&m, 0, sizeof m);
-    m.part = part; m.cand_nodes = a.cand_nodes; m.cand_off = a.cand_off;
-    m.n_pod = n_pod; m.n_pair = n_pair; m.n_node = ctx->n_node; m.n_claim = n_claim;
-    merge_bounds(ctx, gather, m.bounds);
-    m.gate = gate;
-    m.pair_why = d_pair_why; m.pair_claim = d_pair_claim; m.pod_why = d_pod_why; m.claim_blocks = d_claim_blocks;
-    m.blocks = ctx->d_swhy_blocks;
-    if (gather) {
-        m.slice4 = (uint32_t)(ctx->swhy_x.slice / 16);
-        CU(cudaMemcpyAsync(part, gate, 4, cudaMemcpyDeviceToDevice, st));   // the header: this rank's fault word
-    }
-    const PeerExchange x = push_slice(ctx, ctx->swhy_x, gather, part, (uint32_t)swhy_units(a.n_walk, claims));
-    k_swhy_merge<<<wait_grid(ctx, (n_pod + 7) / 8), 256, 0, st>>>(x, m);
-    ctx->launches += 1;
+    if ((rc = launch_swhy_merge(ctx, w, gate, n_walk, a.cand_nodes, a.cand_off, n_pod, n_pair, n_claim))) return rc;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(ctx, DRA_E_CUDA, "sharded unsuitable reasons launch: %s", cudaGetErrorString(e));
     return DRA_OK;
